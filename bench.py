@@ -2,19 +2,21 @@
 bench.py -- anomaly windows/sec of the fused predict+score hot path on BASELINE.json configs[1]:
 1 000 machines x 64-tag feedforward_hourglass autoencoder, 10 000 rows per machine, per GPU.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--machines M] [--rows R] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--machines M] [--rows R] [--impl ours|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 A step = one pass of the hot path (gb_ffae_infer_score) over every machine of the rank: 10^7 windows per GPU, inputs
-resident in HBM.  `value` is whole-job windows/s (all ranks' windows / max-over-ranks device time).  `e2e` repeats the
+resident in HBM.  `value` is whole-job windows/s (all ranks' windows / max-over-ranks device time).  `--dump-outputs DIR` writes,
+after the timed steps, what the last timed step returned (every output array, float32, rows of a fixed seeded sample of
+DUMP_ROWS windows) as DIR/<output name>.npy, so that two builds can be compared output for output on identical inputs.  `e2e` repeats the
 measurement through the fleet API with HOST buffers: pinned H2D of x and y and D2H of every output inside the timed
 region.  `roofline` is the algorithmic HBM bytes (1 548 B/window, SURVEY 8d) over the CUDA-event time, against the
-measured copy bandwidth in MEASURED_PEAKS.json.  `cpu_baseline` times the CPU oracle (a restatement of the reference's
-Keras predict loop + diff.py arithmetic -- NOT TensorFlow, which is not installable here, and not the reference's own diff.py,
-which lives under /root/reference and does not exist on the GPU box) on a bounded sample, imports warmed, arithmetic only.
+copy bandwidth in MEASURED_PEAKS.json when present, else the H100 SXM data sheet's 3.35 TB/s.  `cpu_baseline` times the CPU oracle (a restatement of the reference's
+Keras predict loop + diff.py arithmetic -- NOT TensorFlow and not the reference's own diff.py, neither of which this package
+depends on) on a bounded sample, imports warmed, arithmetic only.
 Machines shard across ranks with no data-path collective (weak scaling: the per-GPU workload is fixed); NCCL only
 broadcasts the machine assignment and gathers one score summary per machine after the timed region.  Beside the weak-scaling
-`value` the line carries `strong` (the SAME 1 000 machines split over the N ranks, BASELINE's "1k machines at 1/2/4/8 B200") and
+`value` the line carries `strong` (the SAME 1 000 machines split over the N ranks, BASELINE's "1k machines at 1/2/4/8 GPUs") and
 `secondary` (one GPU's share of BASELINE configs[2], [3] and the configs[4] request shape, benchmarks/secondary.py, ~20 s).
 """
 from __future__ import annotations
@@ -36,9 +38,7 @@ if ROOT not in sys.path:
 
 T = 64
 BYTES_PER_WINDOW = 4 * T + 4 * T + 4 * 4 * T + 12  # read x, y; write model-output, 2 tag-anomaly blocks, confidence; 3 row scalars
-# dram__bytes_read.sum + dram__bytes_write.sum per window from the committed `ncu --set full` captures (profiles/, file names below)
-NCU_DRAM_BYTES_PER_WINDOW = {"tcgen05": (1.569383e9 + 3.048933e9) / 3.0e6, "fma": (1.037003e9 + 2.019607e9) / 2.0e6}
-NCU_SOURCE = {"tcgen05": "profiles/r02_ffae_tc_ncu.txt (300-machine capture)", "fma": "profiles/r01_ffae_infer_fma_ncu.txt (200-machine capture)"}
+DUMP_ROWS = 16384  # windows of the --dump-outputs sample: 4 MB per per-tag output
 METRIC = "anomaly windows/sec (64-tag feedforward_hourglass AE, 1k machines x 10k rows per GPU, fused predict+score)"
 
 
@@ -47,7 +47,7 @@ def measured_peaks():
     if os.path.exists(p):
         with open(p) as f:
             return json.load(f), "measured"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0}, "fallback"
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "H100 SXM data sheet (700 W), not measured"
 
 
 def host_info():
@@ -96,7 +96,7 @@ def bind_to_gpu_numa_node(local_rank: int):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled during the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi clocks / throttle reasons sampled during the timed region (read-only queries)."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -180,7 +180,7 @@ def cpu_pool(workers: int):
     """
     Persistent worker pool (created and warmed outside any timed region).  Workers are SPAWNED with single-threaded BLAS: forked
     children of a parent that already initialised a 128-thread OpenBLAS each bring up their own 128 threads, and the arm then
-    measures oversubscription (round 1: 1.7 M vs 8.0 M windows/s on two boxes with the same core count).
+    measures oversubscription.
     """
     global _POOL
     if _POOL is None and workers > 1:
@@ -230,7 +230,7 @@ def run_reference_arm(args, rank, world):
         "dtype": "f32", "data": "synthetic",
         "config": workload_config(args.machines, args.rows, args.gpus),
         "note": ("reference-restated CPU oracle (NumPy batch-32 predict loop + diff.py arithmetic), not TensorFlow and not the reference's diff.py: "
-                 "neither is installable / present on the GPU box; each step is a bounded sample of the configured workload"),
+                 "neither is a dependency of this package; each step is a bounded sample of the configured workload"),
         "cpu_baseline": {"value": value, "unit": "windows/s", "cores": cores, "kind": "port", "sample": sample, "host": host},
         "e2e": {"value": value, "unit": "windows/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
         "gpu_launches": 0,
@@ -244,7 +244,7 @@ def workload_config(machines, rows, world, variant=None):
     """The `config` object: identical for both arms (the reference arm runs bounded samples of the same workload)."""
     cfg = {"workload": "configs[1]: 1000 machines x 64-tag feedforward_hourglass AE, batched predict+anomaly score",
            "machines_per_gpu": machines, "rows_per_machine": rows, "tags": T, "parallelism": f"machines sharded over {world} GPU(s), no data-path collective",
-           "l2": "inputs+outputs per step = 15.5 GB >> 126 MB L2 (no flush needed)"}
+           "l2": "inputs+outputs per step = 15.5 GB >> 50 MB L2 (no flush needed)"}
     if variant is not None:
         cfg["kernel_variant"] = variant
     return cfg
@@ -277,7 +277,8 @@ def main():
     ap.add_argument("--machines", type=int, default=1000, help="machines per GPU")
     ap.add_argument("--rows", type=int, default=10000, help="rows per machine")
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
-    ap.add_argument("--variant", type=int, default=0, help="0 auto, 1 fp32 CUDA cores, 2 tcgen05")
+    ap.add_argument("--variant", type=int, default=0, help="0 auto, 1 fp32 CUDA cores, 2 tensor cores (wgmma)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write the last timed step's outputs (a fixed seeded row sample) as DIR/<name>.npy")
     ap.add_argument("--e2e-steps", type=int, default=3)
     ap.add_argument("--cpu-machines", type=int, default=150, help="machines in the one-core cpu_baseline sample (~10 s of CPU work)")
     ap.add_argument("--secondary", type=int, default=1, help="0: skip the configs[2]/[3]/[4] block")
@@ -347,6 +348,8 @@ def main():
     if dist is not None:
         dist.barrier()
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, out, M * R)
     elapsed_ms = ev[0].elapsed_time(ev[-1])
     per_launch_ms = [ev[i].elapsed_time(ev[i + 1]) for i in range(args.steps)]
     t = torch.tensor([elapsed_ms], device=dev, dtype=torch.float64)
@@ -356,7 +359,7 @@ def main():
     windows_per_step = M * R * world
     value = windows_per_step * args.steps / (elapsed_ms_max * 1e-3)
 
-    # ---- strong scaling: the SAME M machines split over the ranks (BASELINE: "1k machines at 1/2/4/8 B200") ----------
+    # ---- strong scaling: the SAME M machines split over the ranks (BASELINE: "1k machines at 1/2/4/8 GPUs") ----------
     Ms = len(fleet.partition(M, world)[rank])
     jobs_s = engine.jobs_to_device(engine.uniform_jobs(Ms, R), dev)
     step_s = lambda: eng.infer_score(params, jobs_s, Ms, R, x, y, scale, feat, agg, out=out, variant=args.variant)  # noqa: E731
@@ -441,12 +444,10 @@ def main():
         line = {
             "metric": METRIC, "value": value, "unit": "windows/s", "n_gpus": world, "steps": args.steps, "warmup": max(args.warmup, 3),
             "ms_per_step": elapsed_ms_max / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-            "dtype": "f32" if vname == "fma" else "tf32x3", "data": "synthetic",
+            "dtype": "f32" if vname == "fma" else "split tf32/bf16/fp16", "data": "synthetic",
             "config": workload_config(M, R, world, vname),
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peaks["hbm_gbs"], "unit": "GB/s", "frac": achieved / peaks["hbm_gbs"],
-                         # dram__bytes_read+write per window from the committed ncu --set full capture of this kernel, times the windows of one launch
-                         "traffic": int(M * R * NCU_DRAM_BYTES_PER_WINDOW[vname]),
-                         "traffic_source": NCU_SOURCE[vname] + ", scaled per window to this launch", "peak_source": f"MEASURED_PEAKS.json ({peak_kind})", "algorithmic_bytes_per_window": BYTES_PER_WINDOW,
+                         "peak_source": peak_kind if peak_kind != "measured" else "MEASURED_PEAKS.json", "algorithmic_bytes_per_window": BYTES_PER_WINDOW,
                          "kernel_ms_mean": float(np.mean(per_launch_ms)), "kernel_ms_min": float(np.min(per_launch_ms))},
             "cpu_baseline": {"value": cpu_v1, "unit": "windows/s", "cores": 1, "kind": "port", "host": host_info(),
                              "sample": (f"{args.cpu_machines} machines x {R} rows, NumPy oracle (batch-32 predict loop + diff.py arithmetic), warm, arithmetic only: {cpu_dt1:.1f} s"
@@ -472,11 +473,22 @@ def eng_variant_name(variant, eng):
     if variant == 1:
         return "fma"
     if variant == 2:
-        return "tcgen05"
+        return "wgmma"
     from gordo_components_b200 import _cabi
     import ctypes as C
 
-    return "tcgen05" if _cabi.load_library().gb_ffae_tc_supported(C.byref(eng.net)) == 0 else "fma"
+    return "wgmma" if _cabi.load_library().gb_ffae_tc_supported(C.byref(eng.net)) == 0 else "fma"
+
+
+def dump_outputs(directory, out, n_rows):
+    """Every output array of the last timed step, restricted to a fixed seeded sample of rows, as float32 .npy files."""
+    os.makedirs(directory, exist_ok=True)
+    rows = np.sort(np.random.default_rng(12345).choice(n_rows, size=min(DUMP_ROWS, n_rows), replace=False))
+    import torch
+
+    idx = torch.from_numpy(rows).to(next(iter(out.values())).device)
+    for name, arr in out.items():
+        np.save(os.path.join(directory, f"{name}.npy"), arr.index_select(0, idx).float().cpu().numpy())
 
 
 if __name__ == "__main__":

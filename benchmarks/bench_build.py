@@ -2,7 +2,7 @@
 The batched form of `gordo build` for one bucket of machines: 3-fold TimeSeriesSplit cross-validation + final fit + thresholds +
 scalers (what ModelBuilder._build does per machine, gordo/builder/build_model.py:192-339) for ALL machines in four launches.
 
-    python benchmarks/bench_build.py [--machines 148] [--rows 10000] [--epochs 5] [--batch 32]
+    python benchmarks/bench_build.py [--machines 132] [--rows 10000] [--epochs 5] [--batch 32]
 """
 import argparse, json, os, sys
 sys.path.insert(0, os.path.abspath(os.path.join(os.path.dirname(__file__), "..")))
@@ -10,7 +10,7 @@ sys.path.insert(0, os.path.abspath(os.path.join(os.path.dirname(__file__), "..")
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--machines", type=int, default=148)
+    ap.add_argument("--machines", type=int, default=132)
     ap.add_argument("--rows", type=int, default=10000)
     ap.add_argument("--epochs", type=int, default=5)
     ap.add_argument("--batch", type=int, default=32)

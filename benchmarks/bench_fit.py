@@ -42,7 +42,7 @@ def main():
     torch.cuda.synchronize()
     ms = ev0.elapsed_time(ev1)
     steps = E * ((N + B - 1) // B)
-    sms = 148
+    sms = 132
     waves = (M + sms - 1) // sms
     out = {
         "workload": f"{M} machines x {a.tags}-tag hourglass, {N} rows, {E} epochs, batch {B}",

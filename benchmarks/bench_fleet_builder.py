@@ -7,8 +7,7 @@ number a `gordo build` user sees.
 
     python benchmarks/bench_fleet_builder.py [--machines 125] [--rows 10000] [--tags 64] [--epochs 10] [--scaled] [--single 3]
 
-NOT YET RUN on a B200: written after round 1's GPU budget was spent; the code paths it times are covered by
-tests/test_gpu_builder.py.
+Not measured on the H100; the code paths it times are covered by tests/test_gpu_builder.py.
 """
 import argparse, json, os, sys, tempfile, time
 sys.path.insert(0, os.path.abspath(os.path.join(os.path.dirname(__file__), "..")))

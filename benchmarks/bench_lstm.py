@@ -15,7 +15,7 @@ def main():
     ap.add_argument("--rows", type=int, default=1400)
     ap.add_argument("--lookback", type=int, default=144)
     ap.add_argument("--cpu", type=int, default=1)
-    ap.add_argument("--variant", type=int, default=0, help="0 auto (tcgen05 when supported), 1 fp32 CUDA cores, 2 tcgen05")
+    ap.add_argument("--variant", type=int, default=0, help="0 auto (tensor cores when supported), 1 fp32 CUDA cores, 2 tensor cores (wgmma)")
     a = ap.parse_args()
     import torch
     import __graft_entry__ as ge
@@ -42,7 +42,7 @@ def main():
     torch.cuda.synchronize()
     ms = ev0.elapsed_time(ev1)
     out = {"workload": f"{M} machines x 128-tag lstm_symmetric(256,128,64), lookback {a.lookback}, {nwin} windows each",
-           "kernel": "tcgen05" if (a.variant == 2 or (a.variant == 0 and eng.tc_supported)) else "fp32 CUDA cores",
+           "kernel": "wgmma" if (a.variant == 2 or (a.variant == 0 and eng.tc_supported)) else "fp32 CUDA cores",
            "ms": ms, "windows_per_s": M * nwin / (ms * 1e-3), "tflops": M * nwin * spec.flop_per_window / (ms * 1e-3) / 1e12}
     if a.cpu:
         Xc = np.random.default_rng(0).random((a.lookback + 31, 128)).astype(np.float32)

@@ -5,7 +5,7 @@ through server.anomaly_prediction, for models built by builder.FleetModelBuilder
 
     python benchmarks/bench_requests.py [--machines 20] [--tags 8] [--rows 100] [--requests 500] [--threads 8]
 
-NOT YET RUN on a B200 (written after round 1's GPU budget was spent); host-side cost with the score mocked: 3.4 ms per 4-row request.
+Not measured on the H100.
 """
 import argparse, json, os, sys, tempfile, time
 from concurrent.futures import ThreadPoolExecutor

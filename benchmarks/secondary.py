@@ -44,7 +44,7 @@ def lstm_share(torch, engine, machines: int = 32, rows: int = 10_000, lookback: 
     wps = machines * nwin / (ms * 1e-3)
     tflops = wps * LSTM_FLOP_PER_WINDOW / 1e12
     out = {"workload": f"configs[3] share: {machines} machines x 128-tag lstm_symmetric(256,128,64), lookback {lookback}, {nwin} windows each",
-           "kernel": "tcgen05" if eng.tc_supported else "fp32", "ms": ms, "windows_per_s": wps, "algorithmic_tflops": tflops}
+           "kernel": "wgmma" if eng.tc_supported else "fp32", "ms": ms, "windows_per_s": wps, "algorithmic_tflops": tflops}
     if peaks:
         sustained = peaks.get("bf16_tflops_sustained", peaks.get("bf16_tflops"))
         out["frac_of_bf16_sustained_peak"] = tflops / sustained

@@ -1,5 +1,5 @@
 """
-gordo_components_b200 -- B200-native (sm_100a) implementation of gordo's per-machine
+gordo_components_b200 -- H100-native (sm_90a) implementation of gordo's per-machine
 autoencoder train-and-score hot path, behind gordo's own sklearn-style model API.
 
 Drop-in: replace the ``gordo.`` prefix of the model classes in a gordo model definition

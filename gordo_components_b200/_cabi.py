@@ -1,7 +1,7 @@
 """
 ctypes binding of the C-ABI library (include/gordo_b200.h, built by csrc/build.py).
 
-There is no CPU fallback: if the shared library is missing, or no sm_100 device is
+There is no CPU fallback: if the shared library is missing, or no sm_90 (H100) device is
 visible, every compute entry point raises.  PyTorch is used only as the owner of device
 memory and streams; the pointers handed to the library are raw device addresses.
 """
@@ -147,7 +147,7 @@ _device_ok = {}
 
 
 def require_device(device_index: int = 0) -> int:
-    """Fail loudly unless `device_index` is an sm_100 GPU.  Returns its SM count."""
+    """Fail loudly unless `device_index` is an sm_90 (H100) GPU.  Returns its SM count."""
     if device_index in _device_ok:
         return _device_ok[device_index]
     lib = load_library()
@@ -169,7 +169,7 @@ def make_ffnet(dims, acts, l1=None) -> GbFFNet:
         net.dims[i] = int(d)
     for i, a in enumerate(acts):
         if a not in ACT_CODES:
-            raise ValueError(f"activation {a!r} is not supported by the B200 kernels (supported: tanh, relu, sigmoid, linear)")
+            raise ValueError(f"activation {a!r} is not supported by the CUDA kernels (supported: tanh, relu, sigmoid, linear)")
         net.act[i] = ACT_CODES[a]
         net.l1[i] = float(l1[i]) if l1 is not None else 0.0
     return net
@@ -183,10 +183,10 @@ def make_lstmnet(n_features, units, acts, n_features_out, out_act, lookback) -> 
     net.n_features, net.n_features_out = int(n_features), int(n_features_out)
     for i, (u, a) in enumerate(zip(units, acts)):
         if a not in ACT_CODES:
-            raise ValueError(f"activation {a!r} is not supported by the B200 kernels")
+            raise ValueError(f"activation {a!r} is not supported by the CUDA kernels")
         net.units[i], net.act[i] = int(u), ACT_CODES[a]
     if out_act not in ACT_CODES:
-        raise ValueError(f"activation {out_act!r} is not supported by the B200 kernels")
+        raise ValueError(f"activation {out_act!r} is not supported by the CUDA kernels")
     net.out_act = ACT_CODES[out_act]
     net.lookback = int(lookback)
     return net

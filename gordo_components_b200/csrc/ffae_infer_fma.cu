@@ -1,7 +1,7 @@
 // K1+K4, variant 1: fused Dense-stack forward + anomaly score on the fp32 CUDA cores.
 //
 // Generic in the architecture (any widths <= GB_MAX_WIDTH, any supported activation); this is the
-// path for the architectures the tcgen05 kernel (ffae_infer_tc.cu) does not cover, and the exact-fp32
+// path for the architectures the tensor-core kernel (ffae_infer_tc.cu) does not cover, and the exact-fp32
 // cross-check for it.  One CTA owns one job chunk: the slot's weights are copied once into a padded
 // shared-memory image, then 128-row tiles stream through: X tile -> smem, every layer is a register-tiled
 // [128 x K] x [K x N] product out of shared memory (4 rows x 4 cols per thread, rows interleaved by 32 so
@@ -270,7 +270,7 @@ extern "C" int gb_ffae_infer_score_fma(const gb_ffnet* net, const float* params,
   a.o_model = out_model; a.o_ts = out_tag_scaled; a.o_tu = out_tag_unscaled; a.o_tots = out_total_scaled;
   a.o_totu = out_total_unscaled; a.o_conf = out_conf; a.o_totconf = out_total_conf;
 
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   GB_CUDA_CHECK(cudaGetDevice(&dev));
   GB_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   const int tiles_per_job = (max_rows + ROWS - 1) / ROWS;

@@ -1,494 +1,205 @@
-// K1+K4, variant 2: fused Dense-stack forward + anomaly score on the 5th-gen tensor cores (tcgen05 / TMEM / TMA).
+// K1+K4, variant 2: fused Dense-stack forward + anomaly score on the Hopper tensor cores (warpgroup MMA, wgmma).
 //
-// Covers autoencoders of 24..64 tags (multiples of 4; narrower rows ride in zero-padded columns that TMA fills) with hidden
-// widths <= 64 (feedforward_hourglass(64) = 64-53-43-32-32-43-53-64 is the BASELINE workload).  The path is HBM-bound (1 548 algorithmic bytes and 30 236 FLOP per window => 128 TFLOP/s at
-// the measured 6.58 TB/s): fp32 CUDA cores (74 TFLOP/s peak) cannot keep up, the tensor cores can.
+// Covers autoencoders of 24..64 tags (multiples of 4; narrower rows ride in zero-padded columns) with hidden widths <= 64
+// (feedforward_hourglass(64) = 64-53-43-32-32-43-53-64 is the BASELINE workload).  The path is bound by HBM traffic
+// (1 548 algorithmic bytes and 30 236 FLOP per window): fp32 CUDA cores would be the limit, the tensor cores are not.
 //
 // Numerics: 1e-4 parity with the float32 reference forbids plain TF32/FP16 (2^-11 per operand), so operands are split.
 // Layer 0 (x is raw data of any magnitude):
-//        D  =  A_lo*W_hi  +  A_hi*W_hi            (kind::tf32, A = A_hi + A_lo exactly, W_hi = W rounded to TF32)
-//           +  bf16(A)*bf16(W - W_hi)             (kind::f16, the 2^-11-sized correction needs only 8 bits)
+//        D  =  A_hi*W_hi                              (tf32, A_hi = A truncated to TF32, W_hi = W rounded to TF32)
+//           +  bf16(A - A_hi)*bf16(W_hi)  +  bf16(A)*bf16(W - W_hi)   (bf16: the 2^-11-sized corrections need only 8 bits)
 // Layers >= 1 (A = tanh(.) in [-1, 1], so FP16 cannot overflow): A = a1 + a2, W = w1 + w2 with a1 = fp16(A),
 // a2 = fp16(A - a1) and likewise for W (22 significant bits each):
-//        D  =  a2*w1  +  a1*w2  +  a1*w1          (kind::f16, products exact in the fp32 accumulator, dropped a2*w2 ~ 2^-22)
-// i.e. 3 MMAs per 16 values of K instead of 5 per 16 with the TF32 scheme, and 1 TMEM word per activation instead of 2.5.
-// Accumulation is fp32 in TMEM; measured error against the float64 oracle ~2e-6 absolute.
+//        D  =  a2*w1  +  a1*w2  +  a1*w1          (f16, products exact in the fp32 accumulator, dropped a2*w2 ~ 2^-22)
+// Accumulation is fp32; error against the float64 oracle ~2e-6 absolute.
 //
-// One persistent CTA per SM: 8 epilogue warps + 1 control warp, TWO 128-row tiles in flight (TMEM slots 0/1).  Per work
-// item (job chunk) the slot's weights are split and laid out once in shared memory as UMMA K-major operands
-// ([K/4][N][4] TF32, [K/8][N][8] BF16).  Per tile: TMA (SWIZZLE_128B boxes) brings x into shared memory; the epilogue
-// warps (one thread per row: warp%4 = TMEM lane quadrant, warp/4 = column half) split x into the A operand held in TMEM;
-// for every layer the control thread issues tcgen05.mma (A from TMEM, B from the resident weight image, D in TMEM) and
-// commits to an mbarrier; the epilogue warps tcgen05.ld the accumulator, add bias, apply tanh, split and tcgen05.st the
-// next layer's A operand -- and while one tile's MMAs run they do the same for the other tile, so tensor-core latency and
-// epilogue math overlap.  The last layer's epilogue forms every anomaly column against the y rows (requested while
-// the last MMA runs) and writes each output array as full 128-byte lines: rows are transposed between "one thread = one
-// row" and "8 lanes = one line" through a per-warp swizzled 4 KB staging box (warp-level sync only).  Activations never
-// touch HBM.
+// One persistent CTA per SM, NWG warpgroups.  Per work item (a range of one job's rows) the slot's weights are split and
+// laid out once in shared memory as K-major wgmma B operands.  A warpgroup owns a 64-row tile at a time, one thread per
+// (row pair, column pair) as the wgmma fragments lay it out: x is loaded from global memory straight into the A fragment of
+// layer 0, and every layer's accumulator becomes the next layer's A fragment in registers (bias, tanh, FP16 split), so
+// activations never leave the register file.  The output layer's accumulator is scored against y in the same fragment
+// layout and every output array is stored from there (each access of a warp fills whole 32-byte sectors).  The warpgroups
+// of an SM overlap one another's tensor-core waits, and each prefetches its next tile's x while the hidden layers run.
 //
 // Reference arithmetic replaced: keras Dense under Model.predict (gordo/machine/model/models.py:289-300) and
 // DiffBasedAnomalyDetector.anomaly (gordo/machine/model/anomaly/diff.py:350-385, 420-444).
-#include <cuda.h>
 #include <atomic>
-#include <cstdlib>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include "gb_common.cuh"
+#include "gb_sm90.cuh"
 
 namespace {
 
-constexpr int TILE = 128;
-#ifndef GB_TC_NSLOT
-#define GB_TC_NSLOT 2  // measured (profiles/r02_*): three slots convoy behind the in-order layer warps and run 40 % slower than two
-#endif
-#ifndef GB_TC_YPREF
-#define GB_TC_YPREF 2  // y rows of a tile into L2 ahead of the output warps' loads: 0 never (0.702 of the HBM peak), 1 with the tile's x boxes
-                       // (0.655: ~60 % of the lines are evicted again before use and read twice, ncu dram__bytes_read +30 %), 2 when layer
-                       // GB_TC_YPREF_LAYER is issued (0.720; same box, back to back)
-#endif
-#ifndef GB_TC_YPREF_LAYER
-#define GB_TC_YPREF_LAYER 4
-#endif
-#ifndef GB_TC_STATIC
-#define GB_TC_STATIC 1  // 0: always the generic instantiation (A/B measurements)
-#endif
-constexpr int NSLOT = GB_TC_NSLOT;  // tiles in flight (2 or 3)
-static_assert(NSLOT == 2 || NSLOT == 3, "two or three tile slots");
-#ifndef GB_TC_DEDICATED
-#define GB_TC_DEDICATED 0  // 1: every tile slot has its own eight layer warps, which also prepare the slot's layer-0 operands one tile ahead
-                           // (26 warps, 72 registers, no spills; parity-green).  Measured: the slot's tile-to-tile chain shortens to
-                           // ~16 k cycles, but the eight output warps -- 8.2 k cycles per tile, taking the tiles strictly in turn --
-                           // become the bottleneck: 0.715-0.757 of the HBM peak against 0.78 for 0 (one shared group), same box.
-#endif
-// Warp roles.  Layer warps (SFU-bound hidden-layer epilogues): MAIN_WARPS per group, one group per tile slot (DEDICATED) or one
-// group for all slots; then OUT_WARPS output warps (LSU-bound: x split, accumulator parking, anomaly columns); then one control warp
-// per slot.  In every group warp%4 = TMEM lane quadrant and (warp/4)%2 = column half.  With one shared group the slots' epilogues
-// serialise (the timeline showed each MMA commit waiting 1.2-2.1k cycles for the group to finish the other slot, with the SFU only
-// ~40 % busy); dedicated groups let both slots' epilogues run at once.
-constexpr int MAIN_WARPS = 8, LAYER_GROUPS = GB_TC_DEDICATED ? NSLOT : 1, OUT0 = MAIN_WARPS * LAYER_GROUPS, OUT_WARPS = 8, EPI_WARPS = OUT0 + OUT_WARPS;
-constexpr int NTHREADS = 32 * (EPI_WARPS + NSLOT);
-constexpr int MAXL = 8;
-constexpr int BOX_BYTES = TILE * 128;  // x box: 128 rows x 32 fp32 (SWIZZLE_128B)
-constexpr int OBOX_BYTES = 32 * 128;   // staging box of one output warp: 32 rows x 32 fp32
-constexpr int W = 64;                  // widest feature / hidden width; narrower tag counts T (multiples of 4) ride in zero-padded columns
+using namespace gb::sm90;
 
-// TMEM column map of one tile slot (fp32 columns); slot s starts at s * SLOT_COLS
-// Shared layer group: accumulator 64 | operand images 64 (layer 0's BF16 pair and the later layers' FP16 pair share the columns).
-// DEDICATED: layer 0's images get their own 64 columns, so the slot's layer warps can prepare the NEXT tile's layer-0 operands
-// while the current tile is still in its hidden layers.
-constexpr uint32_t COL_D = 0, COL_A1 = 64, COL_A2 = 96, COL_ALB = GB_TC_DEDICATED ? 128 : 64, COL_ABF = GB_TC_DEDICATED ? 160 : 96,
-                   SLOT_COLS = GB_TC_DEDICATED ? 192 : 128, COL_DX = NSLOT * SLOT_COLS, TMEM_COLS = 512;
-static_assert(COL_DX + (GB_TC_DEDICATED ? NSLOT : NSLOT - 1) * 64 <= TMEM_COLS, "tile slots + spare accumulators exceed the 512 TMEM columns");
-// layers >= 1 keep their two packed-FP16 operand images (32 columns each) where layer 0's TF32-hi image was
-// COL_DX: spare accumulator (absolute column) that receives the OUTPUT layer of slot-1 tiles, so slot 1 can start its next
-// tile while the output warps are still busy with the previous pair (they drain slot 0's accumulator first)
+constexpr int TILE = 64;  // rows per warpgroup tile (wgmma M)
+constexpr int NWG = 3;    // warpgroups per CTA (168 registers per thread)
+constexpr int NTHREADS = 128 * NWG;
+constexpr int MAXL = 8;
+constexpr int W = 64;  // widest feature / hidden width
 
 struct TcArgs {
-  int T;                     // tags per row of x / y / every per-tag output (row pitch); <= W, multiple of 4
-  int n_layers, last_layer;  // layers actually evaluated: 0..last_layer (debug aid; == n_layers-1 in production)
-  int K[MAXL], N[MAXL], Np[MAXL], n8[MAXL], k8[MAXL], k16[MAXL], act[MAXL];  // Np = N rounded up to 16 (MMA N), n8 = to 8 (columns evaluated)
-  int whi_ofs[MAXL], wlo_ofs[MAXL], bias_ofs[MAXL];  // byte offsets into dynamic smem
-  int whb_ofs;                                       // layer 0: BF16 image of W_hi [K/8][Np][8]
-  int pofs[MAXL];                                    // float offsets of W_l in the canonical parameter vector
-  int w_bytes;                                       // bytes of the weight+bias region (zero-filled before staging)
-  int param_bytes, bulk_params;                      // parameter vector of one slot: bytes (multiple of 16) / 1 = fetch with one bulk copy
-  int vec_ofs, xbox_ofs, stage_ofs, pair_ofs, bar_ofs;
-  int n_jobs, tiles_per_job, flags;
+  int T;  // tags per row of x / y / every per-tag output (row pitch); <= W, multiple of 4
+  int L;  // layers
+  int N[MAXL], Np[MAXL], k16[MAXL];                  // Np = N rounded up to 16 (wgmma N), k16 = K steps of 16
+  int img0_ofs[MAXL], img1_ofs[MAXL], img2_ofs[MAXL];  // byte offsets into dynamic smem of the weight images
+  int bias_ofs[MAXL];
+  int pofs[MAXL];  // float offsets of W_l in the canonical parameter vector
+  int K[MAXL];
+  int w_bytes;  // bytes of the weight+bias region (zero-filled before staging)
+  int vec_ofs;
+  int n_jobs, tiles_per_job;
   long pstride;
   const float* params;
   const gb_job* jobs;
-  const float *y, *scale, *feat_thr, *agg_thr;
+  const float *x, *y, *scale, *feat_thr, *agg_thr;
   float *o_model, *o_ts, *o_tu, *o_conf, *o_tots, *o_totu, *o_totconf;
   unsigned int* work_ctr;  // global tile counter of this launch (zeroed by the launcher, stream-ordered)
-  long long* trace;  // debug: (event, clock) pairs of CTA 0 (gb_debug_set_trace); NULL in production
-  int trace_cap, trace_from, trace_head;  // record events of tiles >= trace_from or < trace_head only
 };
-
-enum { FLAG_NO_STORES = 2 };  // debug aid (variant bit 9): skip the global stores of the output warps
-constexpr int DEFAULT_NE = 0;
-
-// debug timeline (gb_debug_set_trace): three recorder threads of CTA 0 (epilogue tid 0, the two control leaders) stamp
-// events into shared memory (one clock read + one store each) and flush them to global memory when the kernel ends
-constexpr int TRACE_SLOTS = NSLOT == 2 ? 256 : 32;  // events per recorder (gb_debug_trace_slots() tells the reader: the buffer layout depends on it)
-__device__ __forceinline__ void trace_ev(const TcArgs& a, unsigned long long* ring, int& cnt, int code, int tile, int layer, int slot) {
-  if (a.trace == nullptr || blockIdx.x != 0 || cnt >= TRACE_SLOTS || (tile < a.trace_from && tile >= a.trace_head)) return;
-  ring[cnt++] = ((unsigned long long)clock64() << 24) | ((unsigned long long)(tile & 0xfff) << 12) | ((layer & 0xf) << 8) | ((slot & 0xf) << 4) | (code & 0xf);  // code < 16
-}
-
-// ------------------------------------------------------------------------------------------------ PTX helpers
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "WAIT_%=:\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1, %2;\n\t"  // suspend-time hint: sleep in hardware, do not spin
-      "@p bra DONE_%=;\n\t"
-      "bra WAIT_%=;\n\t"
-      "DONE_%=:\n\t"
-      "}" ::"r"(bar), "r"(parity), "r"(0x989680u)
-      : "memory");
-}
-__device__ __forceinline__ void named_bar_sync(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, int c0, int c1, uint32_t bar) {
-  asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(dst),
-               "l"(map), "r"(c0), "r"(c1), "r"(bar)
-               : "memory");
-}
-
-// D[tmem] (+)= A[tmem] * B[smem desc]
-__device__ __forceinline__ void mma_bf16_ts(uint32_t d, uint32_t a, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t"
-      "}" ::"r"(d), "r"(a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// A and B from shared memory (layer 0's A_hi is the TMA'd x box itself: the tensor core ignores the low 13 mantissa bits of fp32 data)
-__device__ __forceinline__ void mma_tf32_ss(uint32_t d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// K-major SWIZZLE_128B operand (a TMA box of 128-byte rows): 8-row groups 1024 bytes apart; K steps advance the start address
-__device__ __forceinline__ uint64_t make_adesc_sw128(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-__device__ __forceinline__ void mma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-
-// K-major, no-swizzle UMMA shared-memory descriptor: core matrix = 8 rows x 16 B contiguous;
-// SBO = byte distance between 8-row groups (along N), LBO = byte distance between 16-byte K chunks.
-__device__ __forceinline__ uint64_t make_bdesc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;  // descriptor version (Blackwell)
-  return d;                // layout_type (bits 61-63) = 0: SWIZZLE_NONE
-}
-// instruction descriptor: D fp32, A/B format fmt (2 = TF32, 1 = BF16), both K-major, M = 128, N = n
-__host__ __device__ __forceinline__ uint32_t make_idesc(int fmt, int n) {
-  return (1u << 4) | ((uint32_t)fmt << 7) | ((uint32_t)fmt << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(TILE >> 4) << 24);
-}
-
-// TMEM -> registers without waiting; tmem_wait_ld() below ties the wait to the registers it guards
-__device__ __forceinline__ void tmem_ld8_nowait(uint32_t taddr, float* v) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=f"(v[0]), "=f"(v[1]), "=f"(v[2]), "=f"(v[3]), "=f"(v[4]), "=f"(v[5]), "=f"(v[6]), "=f"(v[7])
-               : "r"(taddr)
-               : "memory");
-}
-// wait for all outstanding tcgen05.ld of this thread; the "+f" operands keep every consumer of v[0..7] behind the wait
-__device__ __forceinline__ void tmem_wait_ld8(float* v) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+f"(v[0]), "+f"(v[1]), "+f"(v[2]), "+f"(v[3]), "+f"(v[4]), "+f"(v[5]), "+f"(v[6]), "+f"(v[7])
-               :
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld4_nowait(uint32_t taddr, float* v) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0,%1,%2,%3}, [%4];" : "=f"(v[0]), "=f"(v[1]), "=f"(v[2]), "=f"(v[3]) : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tmem_wait_ld4(float* v) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" : "+f"(v[0]), "+f"(v[1]), "+f"(v[2]), "+f"(v[3]) : : "memory");
-}
-__device__ __forceinline__ void tmem_st2(uint32_t taddr, const uint32_t* r) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x2.b32 [%0], {%1,%2};" ::"r"(taddr), "r"(r[0]), "r"(r[1]) : "memory");
-}
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const uint32_t* r) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]),
-               "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st4(uint32_t taddr, const uint32_t* r) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x4.b32 [%0], {%1,%2,%3,%4};" ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3])
-               : "memory");
-}
 
 // tanh(x) = 1 - 2/(1 + 2^(2x*log2 e)); absolute error ~2e-7 (ex2.approx / rcp.approx are ~1-2 ulp), exact limits at +-inf.
 // The argument arrives pre-scaled: t = (z + b) * 2*log2(e) is formed as fma(z, TANH_ARG_SCALE, b*TANH_ARG_SCALE).
 constexpr float TANH_ARG_SCALE = 2.8853900817779268f;
-__device__ __forceinline__ float tanh_from_scaled(float t) {  // 2 MUFU (ex2, rcp) + 3 FMA-pipe
+__device__ __forceinline__ float tanh_from_scaled(float t) {
   float e, r;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(t));
   asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(e + 1.0f));
   return fmaf(-2.0f, r, 1.0f);
 }
-// Same function with the reciprocal done by three Newton steps on the FMA pipe (1 MUFU + 10 FMA/ALU): the SFU can
-// retire one warp-wide op per 8 cycles per SM sub-partition, so alternating the two variants element by element
-// balances the SFU against the FMA pipe (measured: the 2-MUFU form alone is SFU-bound).
-__device__ __forceinline__ float tanh_from_scaled_fma(float t) {
-  float e;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(fminf(t, 126.0f)));  // keep 1 + e finite
-  const float d = e + 1.0f;                                              // d in [1, 2^126]
-  float r = __int_as_float(0x7EF311C7 - __float_as_int(d));              // 1/d to ~12 %
-  r = fmaf(r, fmaf(-d, r, 1.0f), r);
-  r = fmaf(r, fmaf(-d, r, 1.0f), r);
-  r = fmaf(r, fmaf(-d, r, 1.0f), r);                                     // ~6e-8 relative
-  return fmaf(-2.0f, r, 1.0f);
+
+__device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
+  const __nv_bfloat162 p = __floats2bfloat162_rn(lo, hi);  // low half = even k (the order the MMA expects)
+  return *reinterpret_cast<const uint32_t*>(&p);
+}
+__device__ __forceinline__ float trunc_tf32(float v) { return __uint_as_float(__float_as_uint(v) & 0xffffe000u); }
+// FP16 pair of two activations: w1 = fp16(a), w2 = fp16(a - w1)
+__device__ __forceinline__ void split_f16(float a0, float a1, uint32_t& w1, uint32_t& w2) {
+  const __half2 h = __floats2half2_rn(a0, a1);
+  const float2 f = __half22float2(h);
+  const __half2 r = __floats2half2_rn(a0 - f.x, a1 - f.y);
+  w1 = *reinterpret_cast<const uint32_t*>(&h);
+  w2 = *reinterpret_cast<const uint32_t*>(&r);
 }
 
-// NE: every NE-th element takes the 1-MUFU tanh (0: never) -- the knob that trades SFU against FMA-pipe load
+// Position of weight row k inside layer 0's TF32 image.  A thread's x registers hold, per 16 columns, the pairs 2t, 2t+1 and
+// 2t+8, 2t+9 (the 16-bit A fragment); the TF32 MMA (K = 8) expects columns t and t+4 of each 8.  The sum over K does not
+// care about the order, so the TF32 steps take the registers as they are and the weight rows are permuted to match:
+// column 8s + 2t + e of the data is row 8s + t + 4e of the image.
+__host__ __device__ __forceinline__ int tf32_row(int k) { return (k & ~7) | (((k & 7) >> 1) + 4 * (k & 1)); }
 
-// layer 0: NC (16) inputs -> packed BF16 images of A_lo = A - trunc_tf32(A) and of A itself, at column `col`
-// (A_hi is not stored: the tensor core reads it straight from the x box)
-template <int NC>
-__device__ __forceinline__ void store_a_operands(uint32_t slot_lane, int col, const float* a) {
-  uint32_t lb[NC / 2], bf[NC / 2];
+// ---- one layer's MMAs for wgmma width N (the accumulator is d[0 .. N/2))
+template <int N>
+__device__ __forceinline__ void mma_layer0(float* d, const uint32_t (&xhi)[4][8], const uint32_t (&alo)[4][4], const uint32_t (&abf)[4][4],
+                                           uint32_t img0, uint32_t img1, uint32_t img2, int k16) {
+  const uint32_t lbo = N * 16, step = 2 * N * 16;
 #pragma unroll
-  for (int i = 0; i < NC / 2; ++i) {
-    const float l0 = a[2 * i] - __uint_as_float(__float_as_uint(a[2 * i]) & 0xffffe000u);
-    const float l1 = a[2 * i + 1] - __uint_as_float(__float_as_uint(a[2 * i + 1]) & 0xffffe000u);
-    const __nv_bfloat162 pl = __floats2bfloat162_rn(l0, l1);  // low half = even k (the order the MMA expects)
-    const __nv_bfloat162 pa = __floats2bfloat162_rn(a[2 * i], a[2 * i + 1]);
-    lb[i] = *reinterpret_cast<const uint32_t*>(&pl);
-    bf[i] = *reinterpret_cast<const uint32_t*>(&pa);
-  }
-  constexpr int C8 = NC / 8, R4 = (NC % 8) / 4;  // NC = 8*C8 + 4*R4
+  for (int ks = 0; ks < 8; ++ks)  // A_hi * W_hi, first MMA overwrites
+    if (ks < 2 * k16) {
+      const uint32_t a[4] = {xhi[ks >> 1][4 * (ks & 1) + 0], xhi[ks >> 1][4 * (ks & 1) + 1], xhi[ks >> 1][4 * (ks & 1) + 2], xhi[ks >> 1][4 * (ks & 1) + 3]};
+      if (N == 16) wgmma_rs_tf32_n16(d, a, desc_noswizzle(img0 + ks * step, lbo, 128), ks > 0);
+      if (N == 32) wgmma_rs_tf32_n32(d, a, desc_noswizzle(img0 + ks * step, lbo, 128), ks > 0);
+      if (N == 48) wgmma_rs_tf32_n48(d, a, desc_noswizzle(img0 + ks * step, lbo, 128), ks > 0);
+      if (N == 64) wgmma_rs_tf32_n64(d, a, desc_noswizzle(img0 + ks * step, lbo, 128), ks > 0);
+    }
 #pragma unroll
-  for (int c = 0; c < C8; ++c) {
-    tmem_st4(slot_lane + COL_ALB + ((col + 8 * c) >> 1), lb + 4 * c);
-    tmem_st4(slot_lane + COL_ABF + ((col + 8 * c) >> 1), bf + 4 * c);
-  }
-  if (R4) {
-    tmem_st2(slot_lane + COL_ALB + ((col + 8 * C8) >> 1), lb + 4 * C8);
-    tmem_st2(slot_lane + COL_ABF + ((col + 8 * C8) >> 1), bf + 4 * C8);
-  }
+  for (int ks = 0; ks < 4; ++ks)  // bf16(A_lo) * bf16(W_hi)
+    if (ks < k16) {
+      if (N == 16) wgmma_rs_bf16_n16(d, alo[ks], desc_noswizzle(img1 + ks * step, lbo, 128), 1);
+      if (N == 32) wgmma_rs_bf16_n32(d, alo[ks], desc_noswizzle(img1 + ks * step, lbo, 128), 1);
+      if (N == 48) wgmma_rs_bf16_n48(d, alo[ks], desc_noswizzle(img1 + ks * step, lbo, 128), 1);
+      if (N == 64) wgmma_rs_bf16_n64(d, alo[ks], desc_noswizzle(img1 + ks * step, lbo, 128), 1);
+    }
+#pragma unroll
+  for (int ks = 0; ks < 4; ++ks)  // bf16(A) * bf16(W_lo)
+    if (ks < k16) {
+      if (N == 16) wgmma_rs_bf16_n16(d, abf[ks], desc_noswizzle(img2 + ks * step, lbo, 128), 1);
+      if (N == 32) wgmma_rs_bf16_n32(d, abf[ks], desc_noswizzle(img2 + ks * step, lbo, 128), 1);
+      if (N == 48) wgmma_rs_bf16_n48(d, abf[ks], desc_noswizzle(img2 + ks * step, lbo, 128), 1);
+      if (N == 64) wgmma_rs_bf16_n64(d, abf[ks], desc_noswizzle(img2 + ks * step, lbo, 128), 1);
+    }
+}
+template <int N>
+__device__ __forceinline__ void mma_f16(float* d, const uint32_t* a, uint64_t desc, uint32_t acc) {
+  if (N == 16) wgmma_rs_f16_n16(d, a, desc, acc);
+  if (N == 32) wgmma_rs_f16_n32(d, a, desc, acc);
+  if (N == 48) wgmma_rs_f16_n48(d, a, desc, acc);
+  if (N == 64) wgmma_rs_f16_n64(d, a, desc, acc);
+}
+template <int N>
+__device__ __forceinline__ void mma_hidden(float* d, const uint32_t (&a1)[4][4], const uint32_t (&a2)[4][4], uint32_t img0, uint32_t img1, int k16) {
+  const uint32_t lbo = N * 16, step = 2 * N * 16;
+#pragma unroll
+  for (int ks = 0; ks < 4; ++ks)  // a2 * w1 (first MMA overwrites the accumulator)
+    if (ks < k16) mma_f16<N>(d, a2[ks], desc_noswizzle(img0 + ks * step, lbo, 128), ks > 0);
+#pragma unroll
+  for (int ks = 0; ks < 4; ++ks)  // a1 * w2
+    if (ks < k16) mma_f16<N>(d, a1[ks], desc_noswizzle(img1 + ks * step, lbo, 128), 1);
+#pragma unroll
+  for (int ks = 0; ks < 4; ++ks)  // a1 * w1
+    if (ks < k16) mma_f16<N>(d, a1[ks], desc_noswizzle(img0 + ks * step, lbo, 128), 1);
 }
 
-// layers >= 1: split NC activations (|a| <= 1) into two packed-FP16 images a1 = fp16(a), a2 = fp16(a - a1)
-template <int NW>
-__device__ __forceinline__ void tmem_st_words(uint32_t taddr, const uint32_t* r) {  // NW in {2, 4, 6, 8}
-  if (NW == 8) tmem_st8(taddr, r);
-  if (NW == 6) { tmem_st4(taddr, r); tmem_st2(taddr + 4, r + 4); }
-  if (NW == 4) tmem_st4(taddr, r);
-  if (NW == 2) tmem_st2(taddr, r);
-}
-template <int NC>
-__device__ __forceinline__ void store_a_fp16(uint32_t slot_lane, int col, const float* a) {
-  uint32_t w1[NC / 2], w2[NC / 2];
+__device__ __forceinline__ void fence_acc(float (&d)[32]) {
 #pragma unroll
-  for (int i = 0; i < NC / 2; ++i) {
-    const __half2 h = __floats2half2_rn(a[2 * i], a[2 * i + 1]);  // low half = even k
-    const float2 f = __half22float2(h);
-    const __half2 r = __floats2half2_rn(a[2 * i] - f.x, a[2 * i + 1] - f.y);
-    w1[i] = *reinterpret_cast<const uint32_t*>(&h);
-    w2[i] = *reinterpret_cast<const uint32_t*>(&r);
-  }
-  tmem_st_words<NC / 2>(slot_lane + COL_A1 + (col >> 1), w1);
-  tmem_st_words<NC / 2>(slot_lane + COL_A2 + (col >> 1), w2);
+  for (int i = 0; i < 32; ++i) fence_reg(d[i]);
 }
-
-template <int NC>
-__device__ __forceinline__ void tmem_load_cols(uint32_t taddr, float* v) {
-  constexpr int C8 = NC / 8, R4 = (NC % 8) / 4;
+// the tensor cores read register A operands asynchronously: they stay allocated until the wait that follows the MMAs
+template <int R, int C>
+__device__ __forceinline__ void fence_frag(uint32_t (&f)[R][C]) {
 #pragma unroll
-  for (int c = 0; c < C8; ++c) tmem_ld8_nowait(taddr + 8 * c, v + 8 * c);
-  if (R4) tmem_ld4_nowait(taddr + 8 * C8, v + 8 * C8);
+  for (int i = 0; i < R; ++i)
 #pragma unroll
-  for (int c = 0; c < C8; ++c) tmem_wait_ld8(v + 8 * c);
-  if (R4) tmem_wait_ld4(v + 8 * C8);
-}
-
-// hidden layer epilogue of one warp: NC accumulator columns -> bias, activation -> next layer's A operand
-// (activation is tanh by construction: gb_ffae_tc_supported admits only tanh hidden layers + linear output, so the
-// compiler sees straight-line code and interleaves the NC independent ex2/rcp chains)
-template <int NC, int NE>
-__device__ __forceinline__ void hidden_epilogue(uint32_t slot_lane, int col0, const float* bias) {
-  float v[NC];
-  tmem_load_cols<NC>(slot_lane + COL_D + col0, v);
-#pragma unroll
-  for (int i = 0; i < NC; i += 4) {
-    const float4 b = *reinterpret_cast<const float4*>(bias + i);
-    const float t[4] = {fmaf(v[i], TANH_ARG_SCALE, b.x), fmaf(v[i + 1], TANH_ARG_SCALE, b.y), fmaf(v[i + 2], TANH_ARG_SCALE, b.z),
-                        fmaf(v[i + 3], TANH_ARG_SCALE, b.w)};
-#pragma unroll
-    for (int j = 0; j < 4; ++j)
-      v[i + j] = (NE > 0 && ((i + j) % (NE > 0 ? NE : 1)) == 0) ? tanh_from_scaled_fma(t[j]) : tanh_from_scaled(t[j]);
-  }
-  store_a_fp16<NC>(slot_lane, col0, v);
-}
-// the columns [c0, c0 + C1 + C2) of one warp, as two independent chunks (C2 may be 0)
-template <int C1, int C2, int NE>
-__device__ __forceinline__ void hidden_epilogue_pair(uint32_t slot_lane, int c0, const float* bias_all) {
-  hidden_epilogue<C1, NE>(slot_lane, c0, bias_all + c0);
-  if (C2 > 0) hidden_epilogue<(C2 > 0 ? C2 : 4), NE>(slot_lane, c0 + C1, bias_all + c0 + C1);
-}
-
-// One lane of a converged warp.  Code under `if (elect_one())` lets ptxas prove that a single thread executes it: the
-// tcgen05.mma / TMA instructions inside become straight-line uniform-datapath SASS (UTCHMMA back to back), whereas `if (lane == 0)`
-// wraps every one of them in an ELECT / BRA.U.ANY loop over the possibly-active lanes (~20 SASS instructions per MMA, measured
-// 90-120 cycles per MMA in situ against ~30 for the tensor pipe itself).
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile("{\n\t.reg .pred P;\n\telect.sync _|P, 0xffffffff;\n\tselp.b32 %0, 1, 0, P;\n\t}" : "=r"(pred));
-  return pred != 0;
-}
-
-// ---- layer tables.  The generic kernel reads per-layer sizes and shared-memory offsets from TcArgs (uniform loads, runtime loop
-// bounds).  For the BASELINE architecture, feedforward_hourglass(64) = 64-53-43-32-32-43-53-64, the same numbers are compile-time
-// constants (STATIC instantiation): the layer loops unroll, MMA counts / descriptors / epilogue widths fold, and the control
-// warp's per-layer issue block is a handful of uniform adds between UTCHMMAs.  The table mirrors the host-side layout code in
-// gb_ffae_infer_score_tc, which verifies the match before choosing the STATIC kernel.
-template <int V> struct IC {};
-constexpr int HG_L = 7;
-constexpr int HG_DIMS[HG_L + 1] = {64, 53, 43, 32, 32, 43, 53, 64};
-constexpr int hg_ru(int v, int m) { return (v + m - 1) / m * m; }
-template <int l> struct HGL {
-  static constexpr int K = HG_DIMS[l], N = HG_DIMS[l + 1];
-  static constexpr int Np = hg_ru(N, 16), n8 = hg_ru(N, 8), k8 = hg_ru(K, 8) / 8, k16 = hg_ru(K, 16) / 16;
-  static constexpr int whi_bytes = l == 0 ? k8 * 8 * Np * 4 : k16 * 16 * Np * 2, wlo_bytes = k16 * 16 * Np * 2, whb_bytes = l == 0 ? k16 * 16 * Np * 2 : 0;
-  static constexpr int whi_ofs = HGL<l - 1>::end_ofs, wlo_ofs = whi_ofs + whi_bytes, whb_ofs = wlo_ofs + wlo_bytes, end_ofs = whb_ofs + whb_bytes;
-};
-template <> struct HGL<-1> { static constexpr int end_ofs = 0; };
-template <int l> constexpr int HG_BIAS_OFS = HGL<HG_L - 1>::end_ofs + 64 * 4 * l;  // biases follow the last weight image, 64 floats per layer
-
-struct LayerP { int K, N, Np, n8, k8, k16, whi_ofs, wlo_ofs, bias_ofs; };
-template <int V> __device__ __forceinline__ LayerP layer_of(const TcArgs&, IC<V>) {
-  return LayerP{HGL<V>::K, HGL<V>::N, HGL<V>::Np, HGL<V>::n8, HGL<V>::k8, HGL<V>::k16, HGL<V>::whi_ofs, HGL<V>::wlo_ofs, HG_BIAS_OFS<V>};
-}
-__device__ __forceinline__ LayerP layer_of(const TcArgs& a, int l) {
-  return LayerP{a.K[l], a.N[l], a.Np[l], a.n8[l], a.k8[l], a.k16[l], a.whi_ofs[l], a.wlo_ofs[l], a.bias_ofs[l]};
-}
-template <int V> __device__ __forceinline__ constexpr int layer_index(IC<V>) { return V; }
-__device__ __forceinline__ int layer_index(int l) { return l; }
-// f(l) for l = 0 .. n-1: compile-time indices (n == HG_L or HG_L - 1) in the STATIC kernel, a runtime loop otherwise
-template <bool STATIC, bool HIDDEN_ONLY, class F>
-__device__ __forceinline__ void for_layers(int n, F&& f) {
-  if constexpr (STATIC) {
-    f(IC<0>{}); f(IC<1>{}); f(IC<2>{}); f(IC<3>{}); f(IC<4>{}); f(IC<5>{});
-    if constexpr (!HIDDEN_ONLY) f(IC<6>{});
-  } else {
-    for (int l = 0; l < n; ++l) f(l);
-  }
+    for (int j = 0; j < C; ++j) fence_reg(f[i][j]);
 }
 
 // ------------------------------------------------------------------------------------------------ kernel
-// FULL: 64 tags (the row pitch and every column guard fold to constants -- the BASELINE workload); otherwise T < 64 rides in padded columns
-// STATIC (implies FULL): the feedforward_hourglass(64) stack with every layer constant folded (see the layer tables above)
-template <int NE, bool FULL, bool STATIC>
-__global__ void __launch_bounds__(NTHREADS, 1)
-ffae_tc_kernel(const __grid_constant__ TcArgs a, const __grid_constant__ CUtensorMap map_x) {
+__global__ void __launch_bounds__(NTHREADS, 1) ffae_tc_kernel(const __grid_constant__ TcArgs a) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  __shared__ uint32_t s_tmem_base;
-  __shared__ unsigned long long s_trace[4][TRACE_SLOTS];
-  int trace_cnt = 0;
-
   const int tid = threadIdx.x, lane = tid & 31;
-  if (a.trace != nullptr && tid == 0) {  // every CTA: start / end of its life in nanoseconds (how evenly the SMs finish)
-    unsigned long long ns;
-    asm volatile("mov.u64 %0, %globaltimer;" : "=l"(ns));
-    a.trace[8 + 4 * TRACE_SLOTS + 2 * blockIdx.x] = (long long)ns;
-    if (blockIdx.x == 0) {
-      a.trace[4 + 4 * TRACE_SLOTS + 0] = clock64();
-      a.trace[4 + 4 * TRACE_SLOTS + 2] = (long long)ns;
-    }
-  }
-  const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);  // warp-uniform by construction (lets the compiler use uniform registers)
-  const bool is_ctrl = warp >= EPI_WARPS, is_out = !is_ctrl && warp >= OUT0;
-  unsigned long long* ring = s_trace[is_ctrl ? (warp == EPI_WARPS ? 1 : 0) : (is_out ? (warp == EPI_WARPS - 1 ? 2 : 3) : 0)];
-  const int q = warp & 3, h = (warp >> 2) & 1;  // TMEM lane quadrant (rows 32q..) / column half
-  const int row = q * 32 + lane;                // tile row owned by this thread in the "one thread = one row" layout
+  const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
+  const int wg = warp >> 2, wq = warp & 3;  // warpgroup; warp inside it (rows 16 wq ..)
+  const int g = lane >> 2, t = lane & 3;    // fragment row / column pair
   const uint32_t sbase = smem_u32(smem);
-  // mbarriers, two of each (tile slot 0/1): x_full, a_ready, d_ready (hidden-layer MMAs), f_ready (output-layer MMAs), d_free
-  const uint32_t bars = sbase + a.bar_ofs;
-  const uint32_t BX = 0, BA = 24, BD = 48, BF = 72, BE = 96, BW = 120, BA0 = 128;  // 8 bytes per tile slot each; BW: bulk copy of a slot's parameter vector; BA0: layer-0 operands ready (DEDICATED)
+  const int TP = a.T, L = a.L;
   const bool has_y = a.y != nullptr;
-  const int TP = FULL ? W : a.T;  // tags per row = row pitch of x / y / per-tag outputs
-  const int L = STATIC ? HG_L : a.last_layer + 1;
+  const bool totals = has_y && (a.o_tots || a.o_totu || a.o_totconf);
+  const float inv_w = 1.0f / (float)TP;
 
-  if (tid == 0) {
-    for (int s = 0; s < NSLOT; ++s) {
-      mbar_init(bars + BX + 8 * s, 1);
-      mbar_init(bars + BA + 8 * s, MAIN_WARPS);
-      mbar_init(bars + BA0 + 8 * s, MAIN_WARPS);
-      mbar_init(bars + BD + 8 * s, 1);
-      mbar_init(bars + BF + 8 * s, 1);
-      mbar_init(bars + BE + 8 * s, OUT_WARPS);
-    }
-    mbar_init(bars + BW, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == EPI_WARPS) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem_base)), "n"(TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = __shfl_sync(0xffffffffu, s_tmem_base, 0);
-  const uint32_t lane_base = tmem + ((uint32_t)(q * 32) << 16);
-
-  // phase parities (each role uses the subset it waits on)
-  uint32_t ph_x = 0, ph_d = 0, ph_f = 0;  // one parity bit per tile slot
-  uint32_t ph_a = 0, ph_a0 = 0, ph_e = 0, ph_w = 0;
-  int cur_slot = -1;
   // Work distribution.  Tiles are numbered job by job (global tile G = job * tiles_per_job + tile) and handed out from a global
-  // counter in contiguous ranges: whole jobs, in order, for most of the launch -- every change of job costs a pipeline drain +
-  // refill (~30k cycles, measured), and neighbouring CTAs streaming neighbouring jobs keep the TLB footprint small (cutting the
-  // fleet into gridDim.x distant static ranges measured 18 % slower) -- then thirds and sixths of a job for the last ~1.5 jobs per
-  // CTA.  Why dynamic: with an equal static share per CTA the SMs finish up to 14 % apart (measured per-CTA lifetimes 2.83 / 2.94 /
-  // 3.29 ms min / mean / max at the BASELINE size: SMs differ in their distance to the memory partitions) and the launch lasts as
-  // long as its slowest CTA; but ranges must stay long -- a first version that shrank them to 8 tiles spent more in drains than it won.
-  // The scheduler state lives in shared memory (thread 0 only touches it between items): registers are what this kernel is short of.
-  __shared__ int s_item[4];  // [0] job, [1] first tile, [2] end tile of the item all threads work on next; [3] unused
+  // counter in contiguous ranges: whole jobs, in order, for most of the launch (a change of job restages the weights), then
+  // thirds and sixths of a job for the last ~1.5 jobs per CTA, so that the SMs finish close together.
+  __shared__ int s_item[3];   // job, first tile, end tile of the item all threads work on next
   __shared__ int s_range[2];  // thread 0: tiles [g, g_end) of the range it holds
   if (tid == 0) s_range[0] = s_range[1] = 0;
+  int cur_slot = -1;
 
   while (true) {
     if (tid == 0) {
       const int tpj = a.tiles_per_job, g_total = a.n_jobs * tpj;  // (the launcher refuses fleets beyond 2^31 tiles)
-      int g = s_range[0], g_end = s_range[1];
-      if (g >= g_end) {
+      int gg = s_range[0], g_end = s_range[1];
+      if (gg >= g_end) {
         const int seen = (int)*reinterpret_cast<volatile unsigned int*>(a.work_ctr);
         const int left = g_total - seen, per_cta = left / (int)gridDim.x;
         int size = per_cta * 2 >= 3 * tpj ? tpj : (per_cta >= tpj / 3 ? (tpj + 2) / 3 : (tpj + 5) / 6);
         if (size < 1) size = 1;
         if (seen % tpj != 0 && size > tpj - seen % tpj) size = tpj - seen % tpj;  // ranges end at job boundaries (a stale `seen` at worst mis-sizes one)
-        g = (int)atomicAdd(a.work_ctr, (unsigned int)size);
-        g_end = g + size < g_total ? g + size : g_total;
+        gg = (int)atomicAdd(a.work_ctr, (unsigned int)size);
+        g_end = gg + size < g_total ? gg + size : g_total;
       }
-      if (g >= g_total) {
+      if (gg >= g_total) {
         s_item[0] = -1;
       } else {
-        const int job_id = g / tpj, tile_begin = g - job_id * tpj;
-        const int tile_end = min(tpj, tile_begin + (g_end - g));
+        const int job_id = gg / tpj, tile_begin = gg - job_id * tpj;
+        const int tile_end = min(tpj, tile_begin + (g_end - gg));
         s_item[0] = job_id; s_item[1] = tile_begin; s_item[2] = tile_end;
-        g += tile_end - tile_begin;
+        gg += tile_end - tile_begin;
       }
-      s_range[0] = g; s_range[1] = g_end;
+      s_range[0] = gg; s_range[1] = g_end;
     }
     __syncthreads();
     const int job_id = s_item[0], tile_begin = s_item[1], tile_end = s_item[2];
     if (job_id < 0) break;
-    // (s_item is rewritten only after the item's closing __syncthreads)
     const gb_job job = a.jobs[job_id];
     const int row_begin = tile_begin * TILE;
     if (row_begin >= job.n_rows) {  // uniform across the CTA
@@ -498,489 +209,192 @@ ffae_tc_kernel(const __grid_constant__ TcArgs a, const __grid_constant__ CUtenso
     const int row_end = min(job.n_rows, tile_end * TILE);
     const int n_tiles = (row_end - row_begin + TILE - 1) / TILE;
 
-    if (tid == 0) trace_ev(a, ring, trace_cnt, 13, 0xfff, 0, 0);
-    // ---- stage this slot's weights: split (layer 0: TF32-hi / BF16-lo, others: FP16 + FP16) and lay out as UMMA K-major operands
+    // ---- stage this slot's weights: split (layer 0: TF32-hi + BF16 hi / lo, others: FP16 pair) as K-major wgmma B operands
     if (job.slot != cur_slot) {
       cur_slot = job.slot;
       const float* P = a.params + (long)job.slot * a.pstride;
-      // The whole parameter vector comes in with ONE bulk copy into the (idle between work items) x-box + staging area and is
-      // re-laid-out from shared memory: staging layer by layer straight from global memory was a chain of exposed load
-      // latencies (~23 us per work item, measured).  Unaligned or oversized parameter vectors take per-element loads.
-      float* scratch = reinterpret_cast<float*>(smem + a.xbox_ofs);
-      if (a.bulk_params) {
-        if (tid == 0) {
-          mbar_expect_tx(bars + BW, (uint32_t)a.param_bytes);
-          asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(scratch)), "l"(P),
-                       "r"((uint32_t)a.param_bytes), "r"(bars + BW)
-                       : "memory");
-        }
-      } else {
-        for (int i = tid; i < a.param_bytes / 4; i += NTHREADS) scratch[i] = __ldg(P + i);
-      }
-      const float v_scale = (tid < TP && a.scale) ? __ldg(a.scale + (long)job.slot * TP + tid) : 0.f;
-      const float v_thr = (tid < TP && a.feat_thr) ? __ldg(a.feat_thr + (long)job.slot * TP + tid) : 1.f;
       for (int i = tid; i < a.w_bytes / 16; i += NTHREADS) reinterpret_cast<uint4*>(smem)[i] = make_uint4(0, 0, 0, 0);
       __syncthreads();
-      if (a.bulk_params) {
-        mbar_wait(bars + BW, ph_w);
-        ph_w ^= 1;
-      }
       for (int l = 0; l < L; ++l) {
         const int K = a.K[l], N = a.N[l], Np = a.Np[l], KN = K * N;
-        const float* Ws = scratch + a.pofs[l];
-        float* whi = reinterpret_cast<float*>(smem + a.whi_ofs[l]);
-        __nv_bfloat16* wlo = reinterpret_cast<__nv_bfloat16*>(smem + a.wlo_ofs[l]);
-        __nv_bfloat16* whb = reinterpret_cast<__nv_bfloat16*>(smem + a.whb_ofs);
-        // one warp per weight row k, lanes over n: coalesced reads of the scratch copy, no index division
-        for (int k = warp; k < K; k += NTHREADS / 32) {
-          const float w0 = lane < N ? Ws[k * N + lane] : 0.f, w1v = lane + 32 < N ? Ws[k * N + lane + 32] : 0.f;
+        const float* Ws = P + a.pofs[l];
+        for (int i = tid; i < KN; i += NTHREADS) {
+          const int k = i / N, n = i - k * N;
+          const float w = __ldg(Ws + i);
+          const int i8 = ((k >> 3) * Np + n) * 8 + (k & 7);  // [K/8][Np][8] 16-bit images
+          if (l == 0) {
+            const float hi = __uint_as_float((__float_as_uint(w) + 0x1000u) & 0xffffe000u);  // round to nearest TF32
+            const int kt = tf32_row(k);
+            reinterpret_cast<float*>(smem + a.img0_ofs[0])[((kt >> 2) * Np + n) * 4 + (kt & 3)] = hi;
+            reinterpret_cast<__nv_bfloat16*>(smem + a.img1_ofs[0])[i8] = __float2bfloat16_rn(hi);
+            reinterpret_cast<__nv_bfloat16*>(smem + a.img2_ofs[0])[i8] = __float2bfloat16_rn(w - hi);
+          } else {
+            const __half w1 = __float2half_rn(w);
+            reinterpret_cast<__half*>(smem + a.img0_ofs[l])[i8] = w1;
+            reinterpret_cast<__half*>(smem + a.img1_ofs[l])[i8] = __float2half_rn(w - __half2float(w1));
+          }
+        }
+        const float bscale = (l + 1 < L) ? TANH_ARG_SCALE : 1.0f;  // hidden layers: bias folded into the tanh argument scale
+        for (int n = tid; n < N; n += NTHREADS) reinterpret_cast<float*>(smem + a.bias_ofs[l])[n] = __ldg(Ws + KN + n) * bscale;
+      }
+      float* vec = reinterpret_cast<float*>(smem + a.vec_ofs);  // [0,64): scale, [64,128): 1/feat_thr
+      if (tid < W) {
+        vec[tid] = (tid < TP && a.scale) ? __ldg(a.scale + (long)job.slot * TP + tid) : 0.f;
+        vec[W + tid] = (tid < TP && a.feat_thr) ? 1.0f / __ldg(a.feat_thr + (long)job.slot * TP + tid) : 0.f;
+      }
+      fence_proxy_async();  // generic-proxy writes above are read by the tensor cores (async proxy)
+    }
+    __syncthreads();
+
+    // ---- the tiles of this item, warpgroup by warpgroup
+    const float* vec = reinterpret_cast<const float*>(smem + a.vec_ofs);
+    float xr[2][16];  // this thread's x: rows g, g+8 of its warp; per 16 columns the pairs 2t, 2t+1 and 2t+8, 2t+9
+    auto load_x = [&](int tt) {
+      const int r = row_begin + tt * TILE + wq * 16 + g;
 #pragma unroll
-          for (int u = 0; u < 2; ++u) {
-            const int n = lane + 32 * u;
-            const float w = u ? w1v : w0;
-            if (n < N) {
-              if (l == 0) {
-                const float hi = __uint_as_float((__float_as_uint(w) + 0x1000u) & 0xffffe000u);  // round to nearest TF32
-                whi[((k >> 2) * Np + n) * 4 + (k & 3)] = hi;
-                wlo[((k >> 3) * Np + n) * 8 + (k & 7)] = __float2bfloat16_rn(w - hi);
-                whb[((k >> 3) * Np + n) * 8 + (k & 7)] = __float2bfloat16_rn(hi);
-              } else {  // two FP16 images, both [K/8][Np][8]
-                const __half w1 = __float2half_rn(w);
-                reinterpret_cast<__half*>(whi)[((k >> 3) * Np + n) * 8 + (k & 7)] = w1;
-                reinterpret_cast<__half*>(wlo)[((k >> 3) * Np + n) * 8 + (k & 7)] = __float2half_rn(w - __half2float(w1));
+      for (int hr = 0; hr < 2; ++hr) {
+        const int rr = min(r + 8 * hr, row_end - 1);  // rows past the end compute on a copy of the last row and store nothing
+        const float* xrow = a.x + (job.x_row + rr) * (long)TP;
+#pragma unroll
+        for (int c = 0; c < 8; ++c) {
+          const int col = 8 * c + 2 * t;
+          const float2 v = col < TP ? __ldg(reinterpret_cast<const float2*>(xrow + col)) : make_float2(0.f, 0.f);
+          xr[hr][2 * c] = v.x;
+          xr[hr][2 * c + 1] = v.y;
+        }
+        if (has_y && 32 * t < TP) asm volatile("prefetch.global.L2 [%0];" ::"l"(a.y + (job.x_row + rr) * (long)TP + 32 * t));  // read ~7 layers later
+      }
+    };
+    if (wg < n_tiles) load_x(wg);
+    for (int tt = wg; tt < n_tiles; tt += NWG) {
+      float d[32];
+      uint32_t a1[4][4] = {}, a2[4][4] = {};
+      // ---- layer 0
+      {
+        uint32_t xhi[4][8], alo[4][4], abf[4][4];
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) {
+#pragma unroll
+          for (int hh = 0; hh < 2; ++hh) {  // TF32 step 2 kk + hh: registers {row g, row g+8} x {col 2t, col 2t+1} of the pair 8 hh
+            xhi[kk][4 * hh + 0] = __float_as_uint(trunc_tf32(xr[0][4 * kk + 2 * hh]));
+            xhi[kk][4 * hh + 1] = __float_as_uint(trunc_tf32(xr[1][4 * kk + 2 * hh]));
+            xhi[kk][4 * hh + 2] = __float_as_uint(trunc_tf32(xr[0][4 * kk + 2 * hh + 1]));
+            xhi[kk][4 * hh + 3] = __float_as_uint(trunc_tf32(xr[1][4 * kk + 2 * hh + 1]));
+          }
+#pragma unroll
+          for (int q = 0; q < 4; ++q) {  // 16-bit fragment: q = 0 (row g, cols 2t..), 1 (row g+8), 2 (row g, cols 2t+8..), 3 (row g+8, +8)
+            const float v0 = xr[q & 1][4 * kk + 2 * (q >> 1)], v1 = xr[q & 1][4 * kk + 2 * (q >> 1) + 1];
+            alo[kk][q] = pack_bf16(v0 - trunc_tf32(v0), v1 - trunc_tf32(v1));
+            abf[kk][q] = pack_bf16(v0, v1);
+          }
+        }
+        const int k16 = a.k16[0];
+        const uint32_t i0 = sbase + a.img0_ofs[0], i1 = sbase + a.img1_ofs[0], i2 = sbase + a.img2_ofs[0];
+        wgmma_fence();
+        switch (a.Np[0]) {
+          case 16: mma_layer0<16>(d, xhi, alo, abf, i0, i1, i2, k16); break;
+          case 32: mma_layer0<32>(d, xhi, alo, abf, i0, i1, i2, k16); break;
+          case 48: mma_layer0<48>(d, xhi, alo, abf, i0, i1, i2, k16); break;
+          default: mma_layer0<64>(d, xhi, alo, abf, i0, i1, i2, k16); break;
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        fence_acc(d);
+        fence_frag(xhi);
+        fence_frag(alo);
+        fence_frag(abf);
+      }
+      if (tt + NWG < n_tiles) load_x(tt + NWG);  // the registers of x are free again: the next tile's rows load behind the hidden layers
+
+      // ---- hidden layers, then the output layer
+      for (int l = 0; l < L; ++l) {
+        if (l > 0) {
+          const uint32_t i0 = sbase + a.img0_ofs[l], i1 = sbase + a.img1_ofs[l];
+          const int k16 = a.k16[l];
+          wgmma_fence();
+          switch (a.Np[l]) {
+            case 16: mma_hidden<16>(d, a1, a2, i0, i1, k16); break;
+            case 32: mma_hidden<32>(d, a1, a2, i0, i1, k16); break;
+            case 48: mma_hidden<48>(d, a1, a2, i0, i1, k16); break;
+            default: mma_hidden<64>(d, a1, a2, i0, i1, k16); break;
+          }
+          wgmma_commit();
+          wgmma_wait<0>();
+          fence_acc(d);
+          fence_frag(a1);
+          fence_frag(a2);
+        }
+        if (l + 1 == L) break;
+        // epilogue of hidden layer l: bias, tanh, FP16 pair -> A fragment of layer l + 1 (columns past N are 0: zero weights and bias)
+        const float* bl = reinterpret_cast<const float*>(smem + a.bias_ofs[l]);
+        const int nt = a.Np[l] >> 3;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          if (j < nt) {
+            const float2 b = *reinterpret_cast<const float2*>(bl + 8 * j + 2 * t);
+            const float v0 = tanh_from_scaled(fmaf(d[4 * j], TANH_ARG_SCALE, b.x)), v1 = tanh_from_scaled(fmaf(d[4 * j + 1], TANH_ARG_SCALE, b.y));
+            const float v2 = tanh_from_scaled(fmaf(d[4 * j + 2], TANH_ARG_SCALE, b.x)), v3 = tanh_from_scaled(fmaf(d[4 * j + 3], TANH_ARG_SCALE, b.y));
+            // n-tile j = columns 8j.. of the next layer's K: k-step j/2, fragment registers (j%2)*2 + {0: row g, 1: row g+8}
+            split_f16(v0, v1, a1[j >> 1][2 * (j & 1)], a2[j >> 1][2 * (j & 1)]);
+            split_f16(v2, v3, a1[j >> 1][2 * (j & 1) + 1], a2[j >> 1][2 * (j & 1) + 1]);
+          }
+        }
+      }
+
+      // ---- output layer: model output and every anomaly column, straight from the accumulator fragment
+      const float* bo = reinterpret_cast<const float*>(smem + a.bias_ofs[L - 1]);
+      const int trow = row_begin + tt * TILE + wq * 16 + g;  // row inside the job of fragment row g
+      const int nt = a.Np[L - 1] >> 3;
+      float ss[2] = {0.f, 0.f}, su[2] = {0.f, 0.f};
+#pragma unroll
+      for (int hr = 0; hr < 2; ++hr) {
+        const int r = trow + 8 * hr;
+        const bool live = r < row_end;
+        const long go = (job.out_row + r) * (long)TP, gy = (job.x_row + min(r, row_end - 1)) * (long)TP;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const int col = 8 * j + 2 * t;
+          if (j < nt && col < TP) {  // T is a multiple of 4: col + 1 < T too
+            const float2 b = *reinterpret_cast<const float2*>(bo + col);
+            const float2 yh = make_float2(d[4 * j + 2 * hr] + b.x, d[4 * j + 2 * hr + 1] + b.y);
+            if (live) __stcs(reinterpret_cast<float2*>(a.o_model + go + col), yh);  // written once, never re-read: streaming stores
+            if (has_y) {
+              const float2 yv = __ldg(reinterpret_cast<const float2*>(a.y + gy + col));
+              const float2 sc = *reinterpret_cast<const float2*>(vec + col);
+              const float2 df = make_float2(fabsf(yh.x - yv.x), fabsf(yh.y - yv.y));
+              const float2 e = make_float2(df.x * sc.x, df.y * sc.y);
+              su[hr] += df.x * df.x + df.y * df.y;
+              ss[hr] += e.x * e.x + e.y * e.y;
+              if (live && a.o_tu) __stcs(reinterpret_cast<float2*>(a.o_tu + go + col), df);
+              if (live && a.o_ts) __stcs(reinterpret_cast<float2*>(a.o_ts + go + col), e);
+              if (live && a.o_conf) {
+                const float2 rt = *reinterpret_cast<const float2*>(vec + W + col);
+                __stcs(reinterpret_cast<float2*>(a.o_conf + go + col), make_float2(df.x * rt.x, df.y * rt.y));
               }
             }
           }
         }
-        float* bl = reinterpret_cast<float*>(smem + a.bias_ofs[l]);
-        const float bscale = (l + 1 < L) ? TANH_ARG_SCALE : 1.0f;  // hidden layers: bias folded into the tanh argument scale
-        for (int n = tid; n < N; n += NTHREADS) bl[n] = Ws[KN + n] * bscale;
       }
-      float* vec = reinterpret_cast<float*>(smem + a.vec_ofs);  // [0,64): scale, [64,128): 1/feat_thr
-      if (tid < W) {
-        vec[tid] = v_scale;
-        vec[W + tid] = (a.feat_thr && tid < TP) ? 1.0f / v_thr : 0.f;
-      }
-      fence_proxy_async();  // generic-proxy writes above are read by the tensor core (async proxy)
-    }
-    __syncthreads();
-    if (tid == 0) trace_ev(a, ring, trace_cnt, 14, 0xfff, 0, 0);
-
-    // x -> A operand of layer 0 of tile `tt` (slot tt % NSLOT): done by the output warps (shared layer group: they have the slack) or
-    // by the slot's own layer warps (DEDICATED); one thread = one row, warp/4 = column half in either group
-    auto split_wait_x = [&](int tt) {  // the x boxes of tile tt have landed
-      const int s = tt % NSLOT;
-      mbar_wait(bars + BX + 8 * s, (ph_x >> s) & 1u);
-      ph_x ^= 1u << s;
-    };
-    auto split_piece = [&](int tt, int piece) {  // 8 columns of this thread's row: BF16 images of A_lo and A into the slot's layer-0 columns
-      const int s = tt % NSLOT;
-      const uint32_t xbox = sbase + a.xbox_ofs + (2 * s + h) * BOX_BYTES + (uint32_t)row * 128u;
-      float v[8];
+      if (totals) {
 #pragma unroll
-      for (int c = 0; c < 2; ++c) {
-        const uint32_t addr = xbox + ((uint32_t)((piece * 2 + c) ^ (row & 7)) << 4);
-        asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(v[4 * c]), "=f"(v[4 * c + 1]), "=f"(v[4 * c + 2]), "=f"(v[4 * c + 3]) : "r"(addr));
-      }
-      store_a_operands<8>(lane_base + s * SLOT_COLS, h * 32 + piece * 8, v);
-    };
-    auto split_done = [&](int tt) {  // operands visible to the tensor core; one arrival per warp
-      const int s = tt % NSLOT;
-      tmem_wait_st();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bars + (GB_TC_DEDICATED ? BA0 : BA) + 8 * s);
-      if (lane == 0 && (warp == OUT0 || (GB_TC_DEDICATED && warp == 0))) trace_ev(a, ring, trace_cnt, 3, tt, 0, s);
-    };
-    auto split_x = [&](int tt) {
-      split_wait_x(tt);
-#pragma unroll
-      for (int piece = 0; piece < 4; ++piece) split_piece(tt, piece);  // 8 columns at a time keeps the register footprint small
-      split_done(tt);
-    };
-    if (is_ctrl) {
-      // =========================================== control warp of tile slot s: TMA producer + MMA issuer.
-      // The whole warp walks the (warp-uniform) control flow; one elected lane issues the asynchronous instructions.
-      const int s = warp - EPI_WARPS;
-      const long xrow0 = job.x_row + row_begin;
-      const uint32_t bar_x = bars + BX + 8 * s, bar_a = bars + BA + 8 * s, bar_d = bars + BD + 8 * s, bar_f = bars + BF + 8 * s,
-                     bar_e = bars + BE + 8 * s;
-      const uint32_t xdst = sbase + a.xbox_ofs + s * 2 * BOX_BYTES;
-      const uint32_t tb = tmem + s * SLOT_COLS;
-      const uint32_t whb_ofs = STATIC ? HGL<0>::whb_ofs : a.whb_ofs;
-      auto prefetch_y = [&](int t) {
-        if (has_y) {
-          const int nrows = min(TILE, row_end - (row_begin + t * TILE));
-          asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(a.y + (xrow0 + (long)t * TILE) * TP), "r"((uint32_t)(nrows * TP * 4)) : "memory");
-        }
-      };
-      // x boxes of tile t by TMA; its y rows are read ~7 layers later: ask for them in L2 ahead of time, so the output warps' loads do not wait on DRAM
-      auto fetch_tile = [&](int t) {
-        mbar_expect_tx(bar_x, 2 * BOX_BYTES);
-        tma_load_2d(xdst, &map_x, 0, (int)(xrow0 + (long)t * TILE), bar_x);
-        tma_load_2d(xdst + BOX_BYTES, &map_x, 32, (int)(xrow0 + (long)t * TILE), bar_x);
-        if (GB_TC_YPREF == 1) prefetch_y(t);
-      };
-      if (s < n_tiles && elect_one()) fetch_tile(s);
-      __syncwarp();
-      for (int t = s; t < n_tiles; t += NSLOT) {
-        for_layers<STATIC, false>(L, [&](auto lc) {
-          const int l = layer_index(lc);
-          const LayerP P = layer_of(a, lc);
-          const int Np = P.Np, k8 = P.k8, k16 = P.k16;
-          const uint32_t id32 = make_idesc(2, Np), id16 = make_idesc(l == 0 ? 1 : 0, Np);  // kind::f16 inputs: BF16 (layer 0) / FP16
-          const uint32_t lbo = (uint32_t)Np * 16u;
-          const uint32_t dstep = 2u * (uint32_t)Np;  // K-step in 16-byte units (two chunks); stays inside the address field
-          const uint64_t dhi = make_bdesc(sbase + P.whi_ofs, lbo, 128), dlo = make_bdesc(sbase + P.wlo_ofs, lbo, 128), dhb = make_bdesc(sbase + whb_ofs, lbo, 128);
-          if (GB_TC_DEDICATED && l == 0) {  // the slot's layer warps prepared this tile's layer-0 operands during the previous tile
-            mbar_wait(bars + BA0 + 8 * s, ph_a0);
-            ph_a0 ^= 1;
-          } else {
-            mbar_wait(bar_a, ph_a);
-            ph_a ^= 1;
-          }
-          // the output warps must have drained the accumulator this MMA chain overwrites: slot 0 reuses its own D for every
-          // layer (wait before layer 0); the other slots send only their output layer to a spare accumulator (wait before that layer)
-          // (DEDICATED: every slot sends its output layer to a spare accumulator -- the output warps take the tiles strictly in turn
-          // there and may park a tile late)
-          if (t >= NSLOT && l == ((s == 0 && !GB_TC_DEDICATED) ? 0 : L - 1)) {
-            mbar_wait(bar_e, ph_e);
-            ph_e ^= 1;
-          }
-          const uint32_t dcol = (l == L - 1 && (GB_TC_DEDICATED || s >= 1)) ? tmem + COL_DX + (uint32_t)(GB_TC_DEDICATED ? s : s - 1) * 64u : tb + COL_D;
-          tc_fence_after();
-          if (elect_one()) {
-            if (s == 0) trace_ev(a, ring, trace_cnt, 1, t, l, s);
-            if (GB_TC_YPREF == 2 && l == (L > GB_TC_YPREF_LAYER ? GB_TC_YPREF_LAYER : 0)) prefetch_y(t);
-            if (l == 1 && t + NSLOT < n_tiles) fetch_tile(t + NSLOT);  // layer 0's MMAs (which read the x boxes) are complete => the boxes are free
-            if (l == 0) {
-#pragma unroll
-              for (int ks = 0; ks < 8; ++ks)  // A_hi * W_hi: A is the x box (SWIZZLE_128B, 32 columns per box, 32 bytes per K step); first MMA overwrites
-                if (ks < k8) mma_tf32_ss(dcol, make_adesc_sw128(xdst + (ks >> 2) * BOX_BYTES) + (uint64_t)((ks & 3) * 2), dhi + (uint64_t)(ks * dstep), id32, ks > 0);
-#pragma unroll
-              for (int ks = 0; ks < 4; ++ks)  // bf16(A_lo) * bf16(W_hi)
-                if (ks < k16) mma_bf16_ts(dcol, tb + COL_ALB + ks * 8, dhb + (uint64_t)(ks * dstep), id16, 1);
-#pragma unroll
-              for (int ks = 0; ks < 4; ++ks)  // bf16(A) * bf16(W_lo)
-                if (ks < k16) mma_bf16_ts(dcol, tb + COL_ABF + ks * 8, dlo + (uint64_t)(ks * dstep), id16, 1);
-            } else {
-#pragma unroll
-              for (int ks = 0; ks < 4; ++ks)  // a2 * w1 (first MMA overwrites the accumulator)
-                if (ks < k16) mma_bf16_ts(dcol, tb + COL_A2 + ks * 8, dhi + (uint64_t)(ks * dstep), id16, ks > 0);
-#pragma unroll
-              for (int ks = 0; ks < 4; ++ks)  // a1 * w2
-                if (ks < k16) mma_bf16_ts(dcol, tb + COL_A1 + ks * 8, dlo + (uint64_t)(ks * dstep), id16, 1);
-#pragma unroll
-              for (int ks = 0; ks < 4; ++ks)  // a1 * w1
-                if (ks < k16) mma_bf16_ts(dcol, tb + COL_A1 + ks * 8, dhi + (uint64_t)(ks * dstep), id16, 1);
-            }
-            if (l + 1 < L) {
-              mma_commit(bar_d);
-            } else {
-              mma_commit(bar_f);  // output layer: watched by the output warps (accumulator) and the layer warps (A regions reusable)
-            }
-            if (s == 0) trace_ev(a, ring, trace_cnt, 2, t, l, s);
-          }
-          __syncwarp();
-        });
-      }
-      if (s < n_tiles) ph_e ^= 1;  // the last tile's d_free phase completes before the item-end barrier and is never waited on
-    } else if (!is_out) {
-      // =========================================== layer-epilogue warps (SFU-bound): hidden layers only
-      // D -> bias, tanh -> next layer's A operand.  A dedicated group owns slot `grp` (tiles grp, grp + NSLOT, ...); a shared group
-      // visits the slots in turn, layer by layer (one slot's epilogue then overlaps the other slot's MMAs).
-      const int grp = GB_TC_DEDICATED ? warp / MAIN_WARPS : 0;
-      // one hidden layer `lc` of the tile `t` in slot `s`: accumulator -> bias, tanh -> FP16-pair A operand of the next layer
-      auto serve = [&](int s, int t, auto lc) {
-        const int l = layer_index(lc);
-        const LayerP P = layer_of(a, lc);
-        const int half = P.n8 >> 1;  // columns this warp owns: [h*half, (h+1)*half), a multiple of 4, as two chunks
-        const float* bl = reinterpret_cast<const float*>(smem + P.bias_ofs);
-        tc_fence_after();
-        if (tid == 0) trace_ev(a, ring, trace_cnt, 5, t, l, s);
-        const uint32_t sl = lane_base + s * SLOT_COLS;
-        const int c0 = h * half;
-        switch (half) {
-          case 32: hidden_epilogue_pair<16, 16, NE>(sl, c0, bl); break;
-          case 28: hidden_epilogue_pair<16, 12, NE>(sl, c0, bl); break;
-          case 24: hidden_epilogue_pair<12, 12, NE>(sl, c0, bl); break;
-          case 20: hidden_epilogue_pair<12, 8, NE>(sl, c0, bl); break;
-          case 16: hidden_epilogue_pair<8, 8, NE>(sl, c0, bl); break;
-          case 12: hidden_epilogue_pair<8, 4, NE>(sl, c0, bl); break;
-          case 8: hidden_epilogue_pair<4, 4, NE>(sl, c0, bl); break;
-          default: hidden_epilogue_pair<4, 0, NE>(sl, c0, bl); break;
-        }
-        if (h == 1 && P.n8 < P.Np) {  // K padding of the next layer (8 columns): zeros, so stale operands never meet the MMA
-          const uint32_t z[4] = {0u, 0u, 0u, 0u};
-          tmem_st4(sl + COL_A1 + (P.n8 >> 1), z);
-          tmem_st4(sl + COL_A2 + (P.n8 >> 1), z);
-        }
-        tmem_wait_st();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bars + BA + 8 * s);
-        if (tid == 0) trace_ev(a, ring, trace_cnt, 6, t, l, s);
-      };
-      // Fixed service order: slot by slot, layer by layer.  Serving whichever slot has committed (each warp polling on its own, or
-      // warp 0 picking and a named barrier publishing the pick) measured 15-25 % slower with two slots and did not cure the
-      // three-slot convoy either (profiles/r02_kernel_experiments.md).
-      if (GB_TC_DEDICATED) {
-        // This group owns slot `grp`.  It also prepares the layer-0 operands of its tiles -- for the NEXT tile already while the
-        // current one is in its hidden layers (a quarter of the row after each of the middle layers' epilogues, into columns of
-        // their own) -- so that the control warp can issue layer 0 of the next tile right behind the output layer of this one:
-        // neither the output layer nor the operand preparation is on the tile-to-tile chain of the slot any more.
-        const int H = L - 1;  // hidden layers
-        if (grp < n_tiles) split_x(grp);
-        for (int t = grp; t < n_tiles; t += NSLOT) {
-          const bool more = t + NSLOT < n_tiles;
-          for_layers<STATIC, true>(H, [&](auto lc) {
-            const int l = layer_index(lc);
-            mbar_wait(bars + BD + 8 * grp, (ph_d >> grp) & 1u);
-            ph_d ^= 1u << grp;
-            if (l == 0 && t >= NSLOT) {  // the previous tile's output-layer MMAs are complete: nothing reads the FP16 operand columns any more
-              mbar_wait(bars + BF + 8 * grp, (ph_f >> grp) & 1u);
-              ph_f ^= 1u << grp;
-            }
-            serve(grp, t, lc);
-            if (more) {
-              const int first = H > 1 ? 1 : 0;                                   // pieces go behind the epilogues of layers first .. H-1
-              const int lo = H > 1 ? 4 * (l - 1) / (H - 1) : 0, hi = H > 1 ? 4 * l / (H - 1) : 4;
-              if (l == first) split_wait_x(t + NSLOT);
-              if (l >= first)
-                for (int piece = lo; piece < hi; ++piece) split_piece(t + NSLOT, piece);
-              if (l == H - 1) split_done(t + NSLOT);
-            }
-          });
-        }
-        if (grp < n_tiles) {  // consume the last tile's output-layer phase too, so that the parity is right in the next work item
-          mbar_wait(bars + BF + 8 * grp, (ph_f >> grp) & 1u);
-          ph_f ^= 1u << grp;
-        }
-      } else {
-        for (int t0 = 0; t0 < n_tiles; t0 += NSLOT) {
-          for_layers<STATIC, true>(L - 1, [&](auto lc) {
-#pragma unroll
-            for (int s = 0; s < NSLOT; ++s) {
-              if (t0 + s >= n_tiles) continue;
-              if (tid == 0) trace_ev(a, ring, trace_cnt, 4, t0 + s, layer_index(lc), s);
-              mbar_wait(bars + BD + 8 * s, (ph_d >> s) & 1u);
-              ph_d ^= 1u << s;
-              serve(s, t0 + s, lc);
-            }
-          });
-        }
-      }
-    } else {
-      // =========================================== output warps (LSU-bound): last layer -> model output + anomaly columns
-      // Global traffic is row-major with 8 lanes per 128-byte row segment ("transposed" layout: row = i*4 + tr, 16-byte chunk tc).
-      // Only the accumulator has to change layout (TMEM gives one thread = one row): it goes once through this warp's swizzled
-      // staging box; y is loaded straight into the transposed layout and every output column is formed and stored there.
-      const float* vec = reinterpret_cast<const float*>(smem + a.vec_ofs);
-      const uint32_t stage = sbase + a.stage_ofs + (warp - OUT0) * OBOX_BYTES;  // transpose staging of the accumulator
-      float* pair = reinterpret_cast<float*>(smem + a.pair_ofs);  // [2 halves][2][TILE] row sums
-      const int tr = lane >> 3, tc = lane & 7;
-      const float4 sc4 = *reinterpret_cast<const float4*>(vec + h * 32 + tc * 4);
-      const float4 rt4 = *reinterpret_cast<const float4*>(vec + W + h * 32 + tc * 4);
-      const float4 b4 = *reinterpret_cast<const float4*>(reinterpret_cast<const float*>(smem + (STATIC ? HG_BIAS_OFS<HG_L - 1> : a.bias_ofs[L - 1])) + h * 32 + tc * 4);
-      const float inv_w = 1.0f / (float)TP;
-      const bool in_cols = FULL || h * 32 + tc * 4 < TP;  // this lane's four columns exist (T is a multiple of 4)
-      const bool totals = has_y && (a.o_tots || a.o_totu || a.o_totconf);
-
-      // accumulator of the output layer -> this warp's staging box ("one thread = one row" -> row-major lines), accumulator freed
-      auto park = [&](int s, int t) {
-        float acc[32];
-        const uint32_t sl = lane_base + ((GB_TC_DEDICATED || s >= 1) ? COL_DX + (uint32_t)(GB_TC_DEDICATED ? s : s - 1) * 64u : COL_D) + h * 32;
-#pragma unroll
-        for (int c = 0; c < 4; ++c) tmem_ld8_nowait(sl + 8 * c, acc + 8 * c);
-#pragma unroll
-        for (int c = 0; c < 4; ++c) tmem_wait_ld8(acc + 8 * c);
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bars + BE + 8 * s);  // the slot's accumulator may be overwritten by the next tile
-        if (lane == 0 && (warp == OUT0 || warp == EPI_WARPS - 1)) trace_ev(a, ring, trace_cnt, 10, t, L - 1, s);
-#pragma unroll
-        for (int c = 0; c < 8; ++c) {
-          const uint32_t addr = stage + (uint32_t)lane * 128u + ((uint32_t)(c ^ (lane & 7)) << 4);
-          asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" ::"r"(addr), "f"(acc[4 * c]), "f"(acc[4 * c + 1]), "f"(acc[4 * c + 2]), "f"(acc[4 * c + 3]) : "memory");
-        }
-        __syncwarp();
-      };
-      // y rows in the transposed layout: row i*4 + tr of this warp's 32, 16-byte chunk tc of this column half
-      auto y_row = [&](int t, int i) -> float4 {
-        const int trow = row_begin + t * TILE;
-        const int r = min(q * 32 + i * 4 + tr, min(TILE, row_end - trow) - 1);
-        return in_cols ? __ldg(reinterpret_cast<const float4*>(a.y + (job.x_row + trow + r) * (long)TP + h * 32) + tc) : make_float4(0.f, 0.f, 0.f, 0.f);
-      };
-      constexpr int YW = 3;  // DEDICATED: rolling window of y rows (the L2 prefetch makes three iterations of lookahead enough; 12 registers, not 32)
-      float4 yt[GB_TC_DEDICATED ? YW : 8];
-      // every output column of tile t from the staged accumulator against y (registers: all eight rows requested before the
-      // accumulator is ready, or the rolling window)
-      auto emit = [&](int t) {
-        const int trow = row_begin + t * TILE;
-        const int nrows = min(TILE, row_end - trow);
-        const long grow0 = job.out_row + trow;
-        const int wrow0 = q * 32;
-        float ss[8], su[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const int r = i * 4 + tr;
-          float4 yh, yv = yt[GB_TC_DEDICATED ? i % YW : i];
-          if (GB_TC_DEDICATED && has_y && i + YW < 8) yt[i % YW] = y_row(t, i + YW);
-          const uint32_t addr = stage + (uint32_t)r * 128u + ((uint32_t)(tc ^ (r & 7)) << 4);
-          asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(yh.x), "=f"(yh.y), "=f"(yh.z), "=f"(yh.w) : "r"(addr));
-          if (!in_cols) yv = make_float4(0.f, 0.f, 0.f, 0.f);  // zero-padded columns (T < 64): model output is 0 there too
-          yh.x += b4.x; yh.y += b4.y; yh.z += b4.z; yh.w += b4.w;  // output layer is linear
-          if (!in_cols) yh = make_float4(0.f, 0.f, 0.f, 0.f);     // columns beyond T: the accumulator holds stale values there
-          const bool live = wrow0 + r < nrows && in_cols && !(a.flags & FLAG_NO_STORES);
-          const long g = (grow0 + wrow0 + r) * (long)TP + h * 32 + tc * 4;
-          if (live) __stcs(reinterpret_cast<float4*>(a.o_model + g), yh);  // written once, never re-read by this kernel: streaming stores
-          ss[i] = 0.f; su[i] = 0.f;
-          if (has_y) {
-            float4 d, e;
-            d.x = fabsf(yh.x - yv.x); d.y = fabsf(yh.y - yv.y); d.z = fabsf(yh.z - yv.z); d.w = fabsf(yh.w - yv.w);
-            su[i] = d.x * d.x + d.y * d.y + d.z * d.z + d.w * d.w;
-            if (live && a.o_tu) __stcs(reinterpret_cast<float4*>(a.o_tu + g), d);
-            e.x = d.x * sc4.x; e.y = d.y * sc4.y; e.z = d.z * sc4.z; e.w = d.w * sc4.w;
-            ss[i] = e.x * e.x + e.y * e.y + e.z * e.z + e.w * e.w;
-            if (live && a.o_ts) __stcs(reinterpret_cast<float4*>(a.o_ts + g), e);
-            if (live && a.o_conf) __stcs(reinterpret_cast<float4*>(a.o_conf + g), make_float4(d.x * rt4.x, d.y * rt4.y, d.z * rt4.z, d.w * rt4.w));
+        for (int hr = 0; hr < 2; ++hr) {
+          ss[hr] += __shfl_xor_sync(0xffffffffu, ss[hr], 1);
+          ss[hr] += __shfl_xor_sync(0xffffffffu, ss[hr], 2);
+          su[hr] += __shfl_xor_sync(0xffffffffu, su[hr], 1);
+          su[hr] += __shfl_xor_sync(0xffffffffu, su[hr], 2);
+          const int r = trow + 8 * hr;
+          if (t == 0 && r < row_end) {
+            const long go = job.out_row + r;
+            const float ts_ = ss[hr] * inv_w, tu_ = su[hr] * inv_w;
+            if (a.o_tots) a.o_tots[go] = ts_;
+            if (a.o_totu) a.o_totu[go] = tu_;
+            if (a.o_totconf) a.o_totconf[go] = ts_ / __ldg(a.agg_thr + job.slot);
           }
         }
-        __syncwarp();  // staging box reusable
-        if (lane == 0 && (warp == OUT0 || warp == EPI_WARPS - 1)) trace_ev(a, ring, trace_cnt, 12, t, L - 1, t % NSLOT);
-        if (totals) {
-          // row sums: 8 lanes (tc) hold the 32 columns of this half; halves meet in shared memory
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-#pragma unroll
-            for (int o = 1; o < 8; o <<= 1) {
-              ss[i] += __shfl_xor_sync(0xffffffffu, ss[i], o);
-              su[i] += __shfl_xor_sync(0xffffffffu, su[i], o);
-            }
-            if (tc == 0) {
-              pair[h * 2 * TILE + wrow0 + i * 4 + tr] = ss[i];
-              pair[h * 2 * TILE + TILE + wrow0 + i * 4 + tr] = su[i];
-            }
-          }
-          named_bar_sync(1 + q, 64);
-          if (h == 0 && row < nrows) {
-            const float ts_ = (pair[row] + pair[2 * TILE + row]) * inv_w, tu_ = (pair[TILE + row] + pair[3 * TILE + row]) * inv_w;
-            if (a.o_tots) a.o_tots[grow0 + row] = ts_;
-            if (a.o_totu) a.o_totu[grow0 + row] = tu_;
-            if (a.o_totconf) a.o_totconf[grow0 + row] = ts_ / __ldg(a.agg_thr + job.slot);
-          }
-          named_bar_sync(1 + q, 64);
-        }
-        if (lane == 0 && (warp == OUT0 || warp == EPI_WARPS - 1)) trace_ev(a, ring, trace_cnt, 9, t, L - 1, t % NSLOT);
-      };
-
-      // y rows of tile t -> registers, requested as early as the registers are free
-      auto load_y = [&](int t) {
-#pragma unroll
-        for (int i = 0; i < (GB_TC_DEDICATED ? YW : 8); ++i) yt[i] = y_row(t, i);
-      };
-      auto wait_f = [&](int s, int t) {
-        mbar_wait(bars + BF + 8 * s, (ph_f >> s) & 1u);
-        ph_f ^= 1u << s;
-        tc_fence_after();
-        if (lane == 0 && (warp == OUT0 || warp == EPI_WARPS - 1)) trace_ev(a, ring, trace_cnt, 8, t, L - 1, s);
-      };
-
-      if (GB_TC_DEDICATED) {
-        // the slots' own layer warps feed the pipeline; these warps take the finished tiles strictly in turn
-        for (int t = 0; t < n_tiles; ++t) {
-          const int s = t % NSLOT;
-          if (has_y) load_y(t);
-          wait_f(s, t);
-          park(s, t);
-          emit(t);
-        }
-      } else {
-      split_x(0);
-      if (n_tiles > 1) split_x(1);
-      if (NSLOT > 2 && n_tiles > 2) split_x(2);
-
-      for (int t0 = 0; t0 < n_tiles; t0 += NSLOT) {
-        const int n_in = min(NSLOT, n_tiles - t0);
-        if (has_y) load_y(t0);  // requested before the tile's accumulator is ready
-        // ---- first what the layer pipeline waits for: free slot 0's accumulator, feed every slot its next tile
-        if (lane == 0 && (warp == OUT0 || warp == EPI_WARPS - 1)) trace_ev(a, ring, trace_cnt, 7, t0, L - 1, 0);
-        wait_f(0, t0);
-        park(0, t0);
-        if (t0 + NSLOT < n_tiles) split_x(t0 + NSLOT);  // the output-layer MMA of tile t0 is complete: nothing reads slot 0's A operands
-        if (n_in > 1) {
-          wait_f(1, t0 + 1);
-          if (t0 + NSLOT + 1 < n_tiles) split_x(t0 + NSLOT + 1);  // slots 1 and 2 keep their output in a spare accumulator until parked below
-        }
-        if (n_in > 2) {
-          wait_f(2, t0 + 2);
-          if (t0 + NSLOT + 2 < n_tiles) split_x(t0 + NSLOT + 2);
-        }
-        // ---- then the stores
-        emit(t0);
-        if (n_in > 1) {
-          if (has_y) load_y(t0 + 1);
-          park(1, t0 + 1);
-          emit(t0 + 1);
-        }
-        if (n_in > 2) {
-          if (has_y) load_y(t0 + 2);
-          park(2, t0 + 2);
-          emit(t0 + 2);
-        }
-      }
       }
     }
-    fence_proxy_async();  // this item's generic accesses to the x boxes / staging precede the next item's bulk copy and TMA loads
-    __syncthreads();
+    __syncthreads();  // every warpgroup is done with this item's weights before the next item restages them
   }
-
-  if (a.trace != nullptr && tid == 0) {  // SM clock actually delivered over the kernel: cycles and nanoseconds
-    unsigned long long ns;
-    asm volatile("mov.u64 %0, %globaltimer;" : "=l"(ns));
-    a.trace[8 + 4 * TRACE_SLOTS + 2 * blockIdx.x + 1] = (long long)ns;
-    if (blockIdx.x == 0) {
-      a.trace[4 + 4 * TRACE_SLOTS + 1] = clock64();
-      a.trace[4 + 4 * TRACE_SLOTS + 3] = (long long)ns;
-    }
-  }
-  if (a.trace != nullptr && blockIdx.x == 0 && lane == 0 && (warp == 0 || warp == OUT0 || warp == EPI_WARPS - 1 || warp == EPI_WARPS)) {
-    const int role = is_ctrl ? 1 : (is_out ? (warp == EPI_WARPS - 1 ? 2 : 3) : 0);
-    a.trace[role] = trace_cnt;
-    for (int i = 0; i < trace_cnt; ++i) a.trace[4 + role * TRACE_SLOTS + i] = (long long)ring[i];
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == EPI_WARPS) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "n"(TMEM_COLS) : "memory");
-}
-
-// ------------------------------------------------------------------------------------------------ host side
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-EncodeTiledFn get_encode_fn() {
-  static EncodeTiledFn fn = nullptr;
-  if (fn) return fn;
-  void* p = nullptr;
-  cudaDriverEntryPointQueryResult qres;
-  if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) != cudaSuccess || qres != cudaDriverEntryPointSuccess) return nullptr;
-  fn = reinterpret_cast<EncodeTiledFn>(p);
-  return fn;
-}
-
-// [rows][64] fp32 row-major viewed as a 2-D tensor; box = 32 columns x box_rows rows, SWIZZLE_128B
-int make_map(CUtensorMap* map, const void* base, int64_t rows, int box_rows, int T) {
-  EncodeTiledFn fn = get_encode_fn();
-  GB_REQUIRE(fn != nullptr, GB_E_CUDA, "cuTensorMapEncodeTiled is not available from the driver");
-  cuuint64_t dims[2] = {(cuuint64_t)T, (cuuint64_t)(rows > 0 ? rows : 1)};  // columns T..63 of a box are out of bounds: TMA fills zeros
-  cuuint64_t strides[1] = {(cuuint64_t)T * sizeof(float)};
-  cuuint32_t box[2] = {32, (cuuint32_t)box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                  CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  GB_REQUIRE(r == CUDA_SUCCESS, GB_E_CUDA, "cuTensorMapEncodeTiled failed with CUresult %d", (int)r);
-  return GB_OK;
 }
 
 // tile counters of the launches in flight: a ring of static device words, one per launch, zeroed stream-ordered before the kernel
@@ -988,41 +402,28 @@ int make_map(CUtensorMap* map, const void* base, int64_t rows, int box_rows, int
 constexpr int WORK_CTRS = 1024;
 __device__ unsigned int g_work_ctr[WORK_CTRS];
 
-long long* g_trace = nullptr;  // 4 + 4*TRACE_SLOTS int64
-int g_trace_cap = 0;
-
 }  // namespace
-
-// debug aid (not part of the public header): timeline of CTA 0 into a device buffer of 8 + 4*gb_debug_trace_slots() + 2*grid int64
-// (zeroed by the caller): per-role event counts, events, CTA 0's clock/ns at start and end, then every CTA's start/end in ns
-extern "C" int gb_debug_trace_slots(void) { return TRACE_SLOTS; }
-extern "C" int gb_debug_set_trace(void* dev_buf, int capacity) {
-  g_trace = static_cast<long long*>(dev_buf);
-  g_trace_cap = capacity;
-  return GB_OK;
-}
 
 extern "C" int gb_ffae_tc_supported(const gb_ffnet* net) {
   if (gb::validate_ffnet(net) != GB_OK) return GB_E_SHAPE;
   const int L = net->n_layers;
   if (L < 2 || L > MAXL || net->dims[0] != net->dims[L] || net->dims[0] > W || net->dims[0] < 24 || (net->dims[0] & 3)) {
-    gb::set_error("tcgen05 variant covers autoencoders of 24..%d tags (a multiple of 4) with at most %d layers", W, MAXL);
+    gb::set_error("tensor-core variant covers autoencoders of 24..%d tags (a multiple of 4) with at most %d layers", W, MAXL);
     return GB_E_SHAPE;
   }
   for (int l = 1; l < L; ++l)
     if (net->dims[l] > W) {
-      gb::set_error("tcgen05 variant needs hidden widths <= %d", W);
+      gb::set_error("tensor-core variant needs hidden widths <= %d", W);
       return GB_E_SHAPE;
     }
   for (int l = 0; l < L; ++l)
     if (net->act[l] != (l + 1 < L ? GB_ACT_TANH : GB_ACT_LINEAR)) {
-      gb::set_error("tcgen05 variant is specialised for tanh hidden layers and a linear output (the factory defaults)");
+      gb::set_error("tensor-core variant is specialised for tanh hidden layers and a linear output (the factory defaults)");
       return GB_E_SHAPE;
     }
   return GB_OK;
 }
 
-// rows of x / y and of the output arrays are needed for the TMA tensor maps
 extern "C" int gb_ffae_infer_score_tc(const gb_ffnet* net, const float* params, const gb_job* jobs, int32_t n_jobs, int32_t max_rows,
                                       int64_t n_x_rows, int64_t n_out_rows, const float* x, const float* y, const float* scale,
                                       const float* feat_thr, const float* agg_thr, float* out_model, float* out_tag_scaled,
@@ -1030,97 +431,63 @@ extern "C" int gb_ffae_infer_score_tc(const gb_ffnet* net, const float* params, 
                                       float* out_total_conf, int32_t flags, void* stream) {
   int rc = gb_ffae_tc_supported(net);
   if (rc != GB_OK) return rc;
-  GB_REQUIRE(n_x_rows > 0 && n_out_rows > 0, GB_E_ARG, "the tcgen05 variant needs the row counts of x and of the outputs");
+  GB_REQUIRE(flags == 0, GB_E_ARG, "variant bits above the low byte must be 0");
+  GB_REQUIRE(n_x_rows > 0 && n_out_rows > 0, GB_E_ARG, "the tensor-core variant needs the row counts of x and of the outputs");
   TcArgs a{};
   const int L = net->n_layers;
-  a.n_layers = L;
+  a.L = L;
   a.T = net->dims[0];
-  const int dbg_last = (flags >> 8) & 0xff;
-  a.last_layer = (dbg_last > 0 && dbg_last <= L) ? dbg_last - 1 : L - 1;
-  a.flags = flags & 0xff;
   int ofs = 0, pofs = 0;
   for (int l = 0; l < L; ++l) {
     a.K[l] = net->dims[l];
     a.N[l] = net->dims[l + 1];
     a.Np[l] = gb::round_up(a.N[l], 16);
-    a.n8[l] = gb::round_up(a.N[l], 8);
-    a.k8[l] = gb::round_up(a.K[l], 8) / 8;
     a.k16[l] = gb::round_up(a.K[l], 16) / 16;
-    a.act[l] = net->act[l];
     a.pofs[l] = pofs;
     pofs += a.K[l] * a.N[l] + a.N[l];
-    a.whi_ofs[l] = ofs;  // layer 0: TF32 image [K/4][Np][4] + BF16 image [K/8][Np][8]; layers >= 1: two FP16 images [K/8][Np][8]
-    ofs += l == 0 ? a.k8[l] * 8 * a.Np[l] * 4 : a.k16[l] * 16 * a.Np[l] * 2;
-    a.wlo_ofs[l] = ofs;
-    ofs += a.k16[l] * 16 * a.Np[l] * 2;
+    const int kp = a.k16[l] * 16;
+    a.img0_ofs[l] = ofs;  // layer 0: TF32 image [K/4][Np][4]; layers >= 1: FP16 w1 [K/8][Np][8]
+    ofs += kp * a.Np[l] * (l == 0 ? 4 : 2);
+    a.img1_ofs[l] = ofs;  // layer 0: BF16 of W_hi; layers >= 1: FP16 w2
+    ofs += kp * a.Np[l] * 2;
     if (l == 0) {
-      a.whb_ofs = ofs;
-      ofs += a.k16[l] * 16 * a.Np[l] * 2;
+      a.img2_ofs[l] = ofs;  // layer 0: BF16 of W - W_hi
+      ofs += kp * a.Np[l] * 2;
     }
   }
   for (int l = 0; l < L; ++l) {
     a.bias_ofs[l] = ofs;
-    ofs += 64 * 4;  // padded to the widest layer so float4 reads never leave the zero-filled region
+    ofs += W * 4;  // padded to the widest layer: the padded columns read zeros
   }
   a.w_bytes = gb::round_up(ofs, 16);
   ofs = a.w_bytes;
   a.vec_ofs = ofs; ofs += 2 * W * 4;
-  a.pair_ofs = ofs; ofs += 4 * TILE * 4;
-  a.bar_ofs = ofs; ofs += 192;
-  ofs = gb::round_up(ofs, 1024);
-  a.xbox_ofs = ofs; ofs += 2 * NSLOT * BOX_BYTES;    // NSLOT tile slots x two 32-column boxes
-  a.stage_ofs = ofs; ofs += OUT_WARPS * OBOX_BYTES;  // per output warp: a 32-row x 32-column staging box
   const size_t smem = (size_t)ofs;
-  GB_REQUIRE(smem + 4 * TRACE_SLOTS * 8 + 64 <= 227 * 1024, GB_E_SMEM, "architecture needs %zu bytes of shared memory in the tcgen05 variant", smem);
+  GB_REQUIRE(smem <= 227 * 1024, GB_E_SMEM, "architecture needs %zu bytes of shared memory in the tensor-core variant", smem);
 
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   GB_CUDA_CHECK(cudaGetDevice(&dev));
   GB_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   const int tiles_per_job = (max_rows + TILE - 1) / TILE;
   a.tiles_per_job = tiles_per_job;
   a.n_jobs = n_jobs;
   a.pstride = (long)gb_ffnet_param_stride(net);
-  a.param_bytes = (int)(gb_ffnet_param_stride(net) * sizeof(float));  // stride is a multiple of 4 floats
-  GB_REQUIRE(a.param_bytes <= 2 * NSLOT * BOX_BYTES + OUT_WARPS * OBOX_BYTES, GB_E_SMEM, "parameter vector of %d bytes exceeds the staging scratch", a.param_bytes);
-  a.bulk_params = (reinterpret_cast<uintptr_t>(params) % 16 == 0) ? 1 : 0;
-  a.params = params; a.jobs = jobs; a.y = y; a.scale = scale; a.feat_thr = feat_thr; a.agg_thr = agg_thr;
+  a.params = params; a.jobs = jobs; a.x = x; a.y = y; a.scale = scale; a.feat_thr = feat_thr; a.agg_thr = agg_thr;
   a.o_model = out_model; a.o_ts = out_tag_scaled; a.o_tu = out_tag_unscaled; a.o_conf = out_conf;
   a.o_tots = out_total_scaled; a.o_totu = out_total_unscaled; a.o_totconf = out_total_conf;
-  a.trace = g_trace; a.trace_cap = g_trace_cap;
-  if (const char* e = getenv("GB_TC_TRACE_FROM")) a.trace_from = atoi(e);  // debug trace window (scratch/dbg_trace.py)
-  if (const char* e = getenv("GB_TC_TRACE_HEAD")) a.trace_head = atoi(e);
-
-  CUtensorMap mx;
-  if ((rc = make_map(&mx, x, n_x_rows, TILE, a.T)) != GB_OK) return rc;
 
   const long g_total = (long)n_jobs * tiles_per_job;
+  GB_REQUIRE(g_total < (1L << 31), GB_E_ARG, "%ld tiles in one launch: split the fleet", g_total);
   const int grid = (int)(g_total < sms ? g_total : sms);
   {
     static std::atomic<unsigned> next_ctr{0};
     void* base = nullptr;
     GB_CUDA_CHECK(cudaGetSymbolAddress(&base, g_work_ctr));
-    GB_REQUIRE(g_total < (1L << 31), GB_E_ARG, "%ld tiles in one launch: split the fleet", g_total);
     a.work_ctr = static_cast<unsigned int*>(base) + (next_ctr.fetch_add(1) % WORK_CTRS);
     GB_CUDA_CHECK(cudaMemsetAsync(a.work_ctr, 0, sizeof(unsigned int), (cudaStream_t)stream));
   }
-  auto launch = [&](auto kern) -> int {
-    GB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    kern<<<grid, NTHREADS, smem, (cudaStream_t)stream>>>(a, mx);
-    return GB_OK;
-  };
-  // the BASELINE stack runs the constant-folded instantiation when the host layout above equals the compile-time table
-  bool hg = GB_TC_STATIC && L == HG_L && a.last_layer == L - 1 && a.whb_ofs == HGL<0>::whb_ofs;
-  for (int l = 0; hg && l <= L; ++l) hg = net->dims[l] == HG_DIMS[l];
-  {
-    const int want_whi[HG_L] = {HGL<0>::whi_ofs, HGL<1>::whi_ofs, HGL<2>::whi_ofs, HGL<3>::whi_ofs, HGL<4>::whi_ofs, HGL<5>::whi_ofs, HGL<6>::whi_ofs};
-    const int want_wlo[HG_L] = {HGL<0>::wlo_ofs, HGL<1>::wlo_ofs, HGL<2>::wlo_ofs, HGL<3>::wlo_ofs, HGL<4>::wlo_ofs, HGL<5>::wlo_ofs, HGL<6>::wlo_ofs};
-    const int want_bias[HG_L] = {HG_BIAS_OFS<0>, HG_BIAS_OFS<1>, HG_BIAS_OFS<2>, HG_BIAS_OFS<3>, HG_BIAS_OFS<4>, HG_BIAS_OFS<5>, HG_BIAS_OFS<6>};
-    for (int l = 0; hg && l < L; ++l) hg = a.whi_ofs[l] == want_whi[l] && a.wlo_ofs[l] == want_wlo[l] && a.bias_ofs[l] == want_bias[l];
-  }
-  // NE = 2..4 (part of the tanh evaluations on the FMA pipe) measured 1-5 % slower
-  rc = hg ? launch(ffae_tc_kernel<DEFAULT_NE, true, true>)
-          : (a.T == W ? launch(ffae_tc_kernel<DEFAULT_NE, true, false>) : launch(ffae_tc_kernel<DEFAULT_NE, false, false>));
-  if (rc != GB_OK) return rc;
+  GB_CUDA_CHECK(cudaFuncSetAttribute(ffae_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  ffae_tc_kernel<<<grid, NTHREADS, smem, (cudaStream_t)stream>>>(a);
   GB_CUDA_CHECK(cudaGetLastError());
   return GB_OK;
 }

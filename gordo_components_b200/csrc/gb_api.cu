@@ -66,7 +66,7 @@ int gb_device_check(int device, int* sm_count) {
   cudaDeviceProp p;
   GB_CUDA_CHECK(cudaGetDeviceProperties(&p, device));
   if (sm_count) *sm_count = p.multiProcessorCount;
-  GB_REQUIRE(p.major == 10, GB_E_DEVICE, "device %d is sm_%d%d; this library is built for sm_100a only", device,
+  GB_REQUIRE(p.major == 9 && p.minor == 0, GB_E_DEVICE, "device %d is sm_%d%d; this library is built for sm_90a (H100) only", device,
              p.major, p.minor);
   return GB_OK;
 }

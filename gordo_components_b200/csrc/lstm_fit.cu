@@ -15,7 +15,7 @@
 //                                        [dx_t | dh_{t-1}] = dz_t [K; U]^T  (dx_t is the layer below's dh_t)
 //   weights   d[K; U] = sum_t [x_t | h_{t-1}]^T dz_t  (one GEMM per layer with reduction length L * batch), db
 //   Adam      m += (g-m)(1-b1); v += (g^2-v)(1-b2); w -= lr sqrt(1-b2^t)/(1-b1^t) m/(sqrt(v)+eps)   [3P keras]
-// fp32 CUDA cores throughout (the tcgen05 path for these GEMMs is the next step for this kernel family).
+// fp32 CUDA cores throughout (a tensor-core path for these GEMMs is the next step for this kernel family).
 #include "gb_common.cuh"
 
 namespace {

@@ -1,4 +1,4 @@
-// K3, variant 2: LSTM autoencoder prediction on the 5th-gen tensor cores (tcgen05 / TMEM / TMA), machine-batched.
+// K3, variant 2: LSTM autoencoder prediction on the Hopper tensor cores (warpgroup MMA, TMA), machine-batched.
 //
 // Replaces KerasLSTMBaseEstimator.predict (gordo/machine/model/models.py:618-660) for the stacks of
 // factories/lstm_autoencoder.py:72-103 (layer widths are padded to multiples of 64 internally; lstm_symmetric's 256/128/64
@@ -7,11 +7,11 @@
 // 335 MFLOP per 144 x 128 window is tensor-core work.  One launch advances EVERY window of EVERY job by one (layer,
 // timestep): a CTA owns a tile of 128 windows x 64 units and computes the four gate pre-activations
 //      z[128, 4 x 64] = [h_below,t | h_own,t-1] (128 x K)  .  [K; U]^T (K x 256)
-// as tcgen05.mma with both operands brought to shared memory by TMA (SWIZZLE_128B K-major boxes), accumulates in TMEM, and
-// finishes the cell in the epilogue: gates, c_t, h_t, with h_t written straight back as the next launches' A operand.  By default
-// two CTAs on neighbouring window tiles form a pair (cluster of 2) and run ONE cta_group::2 MMA (M=256, N=256, K=16 per instruction):
-// each keeps its own 128 windows and half of the weight box, a stage is 64 KB and the ring three deep (GB_LSTM_PAIR below).  The recurrent state of all windows lives in HBM (h as an FP16
-// pair, c in fp32): per timestep that is a few GB of traffic against tens of TFLOP of contraction.
+// as wgmma (m64n256k16, two consumer warpgroups of 64 windows each) with both operands brought to shared memory by TMA
+// (SWIZZLE_128B K-major boxes, a ring of STAGES chunks of K = 64 fed by a producer warp), accumulates in registers, and
+// finishes the cell in the epilogue: gates, c_t, h_t, with h_t written straight back as the next launches' A operand.  The
+// recurrent state of all windows lives in HBM (h as an FP16 pair, c in fp32): per timestep that is a few GB of traffic
+// against tens of TFLOP of contraction.
 //
 // Numerics (1e-4 parity): h in (-1, 1) and the weights are split into FP16 pairs (a = a1 + a2, 22 significant bits) and
 // every product is formed as a2*w1 + a1*w2 + a1*w1 with fp32 accumulation -- the scheme of ffae_infer_tc.cu's layers >= 1.
@@ -20,168 +20,36 @@
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include "gb_common.cuh"
+#include "gb_sm90.cuh"
 
 namespace {
 
+using namespace gb::sm90;
+
 constexpr int TILE = 128;            // windows per CTA
 constexpr int UB = 64;               // units per CTA
-constexpr int NCOL = 4 * UB;         // gate columns per CTA (accumulator width in TMEM)
-#ifndef GB_LSTM_KC
-#define GB_LSTM_KC 64
-#endif
-// K elements per pipeline chunk = one swizzle row of FP16 (64: SWIZZLE_128B; 32: SWIZZLE_64B, twice as many stages of half the size --
-// the same shared memory, the TMA producer further ahead of the MMAs; measured 2 % slower)
-constexpr int KC = GB_LSTM_KC;
-static_assert(KC == 64 || KC == 32, "chunk = one 128- or 64-byte swizzle row");
+constexpr int NCOL = 4 * UB;         // gate columns per CTA (wgmma N)
+constexpr int KC = 64;               // K elements per pipeline chunk = one 128-byte swizzle row of FP16
 constexpr int ROW_BYTES = KC * 2;
-#ifndef GB_LSTM_PAIR
-#define GB_LSTM_PAIR 2
-#endif
-// How the two CTAs of a thread-block cluster of 2 (neighbouring window tiles of the SAME job and unit block, hence the same weights)
-// cooperate.  The wide layers are bound by the operand stream: with a 96 KB stage only two stages fit, so the TMA of chunk c+2 cannot
-// start before the MMAs of chunk c have finished, and a 96 KB load (latency + transfer ~2.5 k cycles) is longer than the 1.6 k cycles
-// of MMAs of one chunk (ncu: tensor pipe 57-64 % on those layers).
-//   0  no pairing (one CTA = one tile, cta_group::1)
-//   1  each CTA fetches half of the weight box and TMA multicasts it into both CTAs' stages (L2 reads of the weights halved; the stage
-//      stays 96 KB and the ring two deep: +3.5 %)
-//   2  tcgen05 pair MMA (cta_group::2, M = 256): each CTA keeps only ITS half of the weight box (128 of the 256 gate rows) and its own
-//      128 windows of the state; the leader CTA issues the MMAs for both, the accumulator of a CTA's windows lands in its own TMEM.
-//      A stage is 64 KB and the ring three deep.
-constexpr int PAIR_MODE = GB_LSTM_PAIR;
-constexpr int PAIR = PAIR_MODE ? 2 : 1;
-constexpr bool TWO_SM = PAIR_MODE == 2;
-constexpr int B_PART_ROWS = NCOL / PAIR;          // gate rows of the weight box one CTA fetches
-constexpr int B_PART = B_PART_ROWS * ROW_BYTES;   // bytes
-constexpr int A_BOX = TILE * ROW_BYTES;           // bytes: 128 rows x KC FP16
-constexpr int B_BOX = NCOL * ROW_BYTES;           // bytes: 256 rows x KC FP16
-constexpr int B_STAGE = TWO_SM ? B_PART : B_BOX;  // bytes of one weight image (hi or lo) a CTA's stage holds
-constexpr int STAGE_BYTES = 2 * A_BOX + 2 * B_STAGE;
-constexpr int STAGES = (KC == 64 ? 2 : 4) * (TWO_SM ? 3 : 2) / 2;
-constexpr int EPI_WARPS = 16;        // epilogue: warp % 4 = TMEM lane quadrant (32 windows), warp / 4 = which UH of the 64 units
-constexpr int UH = UB / (EPI_WARPS / 4);  // units per epilogue thread and pass (with NG epilogue groups a thread covers NG * UH units of its item in NG passes)
-constexpr int SL = 4;                // units per software-pipeline slice (registers: 576 threads leave 112 each)
-constexpr int NTHREADS = (EPI_WARPS + 2) * 32;  // + warp 8: TMA producer, warp 9: MMA issuer
+constexpr int A_BOX = TILE * ROW_BYTES;  // bytes: 128 rows x KC FP16
+constexpr int B_BOX = NCOL * ROW_BYTES;  // bytes: 256 rows x KC FP16
+constexpr int STAGE_BYTES = 2 * A_BOX + 2 * B_BOX;  // hi and lo images of both operands: 96 KB
+constexpr int STAGES = 2;
+constexpr int CONSUMERS = 2;                         // warpgroups: windows 0..63 and 64..127 of the tile
+constexpr int NTHREADS = 128 * CONSUMERS + 32;       // + one producer warp
 
 struct TcLayerArgs {
   int u, kc_below, kc_own;           // units; K chunks coming from the layer below / from this layer's own h
-  int act, is_first;
-  int tiles_per_job, pairs_per_job, t, lookback, n_items;  // n_items counts (tile group of PAIR, unit block)
+  int act;
+  int tiles_per_job, t, n_items;     // n_items counts (window tile, unit block)
   const gb_job* jobs;
   const float* bias;                 // [n_slots][4u] reordered (layers >= 1; layer 0's bias lives in xk)
   const float* xk;                   // layer 0: input projection, row-blocked [x row / 128][4u reordered][128]
   long xk_rows;
-  float* c;                          // [rows][u]
+  float* c;                          // [tile][u][128 windows]
   __half *h_out_hi, *h_out_lo;       // [rows][u]
-  long long* trace;                  // debug (gb_debug_set_lstm_trace): timeline of CTA 0, three recorder threads; NULL in production
-  int trace_cap;
 };
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count)); }
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "WAIT_%=:\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1, %2;\n\t"
-      "@p bra DONE_%=;\n\t"
-      "bra WAIT_%=;\n\t"
-      "DONE_%=:\n\t"
-      "}" ::"r"(bar), "r"(parity), "r"(0x989680u)
-      : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, int c0, int c1, uint32_t bar) {
-  asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(dst),
-               "l"(map), "r"(c0), "r"(c1), "r"(bar)
-               : "memory");
-}
-// the same box into the same shared-memory offset of every CTA of the cluster named by mask; each destination's mbarrier (same offset)
-// receives the bytes
-__device__ __forceinline__ void tma_load_2d_mc(uint32_t dst, const CUtensorMap* map, int c0, int c1, uint32_t bar, uint16_t mask) {
-  asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%2, %3}], [%4], %5;" ::"r"(dst),
-               "l"(map), "r"(c0), "r"(c1), "r"(bar), "h"(mask)
-               : "memory");
-}
-__device__ __forceinline__ uint32_t cluster_rank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc], FP16 inputs, fp32 accumulate
-__device__ __forceinline__ void mma_f16_ss(uint32_t d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void mma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// pair MMA (issued by the leader CTA of the pair only): M = 256 -- rows 0..127 are the leader's A tile, rows 128..255 the partner's (same
-// shared-memory offset in its CTA); the N = 256 columns of B are split, 128 from each CTA's stage; D rows land in the owning CTA's TMEM
-__device__ __forceinline__ void mma_f16_ss_2sm(uint32_t d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void mma_commit_2sm(uint32_t bar, uint16_t mask) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar), "h"(mask) : "memory");
-}
-// arrive on the barrier at this offset in CTA `rank` of the cluster.  What these arrivals order lives in tensor memory or is written by
-// the async proxy (TMA), ordered by tcgen05.fence / the barrier's own completion; a cluster-scope acquire on the waiting side makes ptxas
-// invalidate L1 (CCTL.IVALL, 13 % of the stall samples of the epilogue when it was tried), so the waits stay at the default scope.
-__device__ __forceinline__ void mbar_arrive_remote(uint32_t bar, uint32_t rank) {
-  uint32_t raddr;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(raddr) : "r"(bar), "r"(rank));
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(raddr) : "memory");
-}
-// one arrival on the barrier at this offset in every CTA of the cluster named by mask, when the MMAs issued so far have completed
-__device__ __forceinline__ void mma_commit_mc(uint32_t bar, uint16_t mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar), "h"(mask) : "memory");
-}
-// K-major SWIZZLE_128B operand: rows of 128 bytes, 8-row groups 1024 bytes apart (SBO); the K step inside the swizzle
-// row is taken by advancing the start address (32 bytes per K=16 FP16 step)
-__device__ __forceinline__ uint64_t make_desc_sw128(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-  d |= (uint64_t)((8 * ROW_BYTES) >> 4) << 32;  // SBO: 8-row groups
-  d |= (uint64_t)1 << 46;                       // descriptor version (Blackwell)
-  d |= (uint64_t)(KC == 64 ? 2 : 4) << 61;      // SWIZZLE_128B / SWIZZLE_64B
-  return d;
-}
-__device__ __forceinline__ uint32_t make_idesc_f16(int m, int n) {  // D fp32, A/B FP16, both K-major
-  return (1u << 4) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
-}
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, float* v) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=f"(v[0]), "=f"(v[1]), "=f"(v[2]), "=f"(v[3]), "=f"(v[4]), "=f"(v[5]), "=f"(v[6]), "=f"(v[7])
-               : "r"(taddr)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld4(uint32_t taddr, float* v) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0,%1,%2,%3}, [%4];" : "=f"(v[0]), "=f"(v[1]), "=f"(v[2]), "=f"(v[3]) : "r"(taddr) : "memory");
-}
-template <int N>
-__device__ __forceinline__ void tmem_ldn(uint32_t taddr, float* v) {
-  if (N == 8) tmem_ld8(taddr, v); else tmem_ld4(taddr, v);
-}
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 // sigmoid through ex2.approx + rcp.approx (~2e-7 absolute error, exact limits); used by the cells whose activation is not tanh
 __device__ __forceinline__ float sigm(float z) {
   float e, r;
@@ -189,8 +57,7 @@ __device__ __forceinline__ float sigm(float z) {
   asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(e + 1.0f));
   return r;
 }
-// The tanh cell (every factory default) with the quotients merged: the epilogue is bound by the MUFU pipe (16 results per clock and SM;
-// trace: 6.6 k cycles of gate arithmetic per item against a floor of 5.1 k for ten MUFU per cell), so
+// The tanh cell (every factory default) with the quotients merged: the epilogue is bound by the MUFU pipe, so
 //   c' = f*c + i*g = [c*(1+ei)*(1+eg) + (eg-1)*(1+ef)] / [(1+ef)*(1+ei)*(1+eg)],   h = o*tanh(c') = (ec-1) / [(1+eo)*(1+ec)]
 // with ei = e^-zi, ef = e^-zf, eo = e^-zo, eg = e^2zg, ec = e^2c' costs five ex2 and two rcp instead of five and five.  The
 // exponentials are capped at 2^30 (sigmoid <= 1e-9 / tanh = 1 to fp32 there) so that the products stay finite; min.NaN keeps a NaN a NaN.
@@ -211,374 +78,151 @@ __device__ __forceinline__ void tanh_cell(float zi, float zf, float zg, float zo
   asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r2) : "f"(po * (ec + 1.0f)));
   h = (ec - 1.0f) * r2;
 }
-__device__ __forceinline__ void st_global_256(void* p, const uint32_t (&v)[8]) {  // 32-byte aligned
-  asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]),
-               "r"(v[6]), "r"(v[7])
-               : "memory");
-}
-// one lane of a converged warp (lets ptxas emit the tcgen05 / TMA issue as straight-line uniform code, see ffae_infer_tc.cu)
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile("{\n\t.reg .pred P;\n\telect.sync _|P, 0xffffffff;\n\tselp.b32 %0, 1, 0, P;\n\t}" : "=r"(pred));
-  return pred != 0;
-}
-
-// debug timeline: role r (0 producer, 1 MMA issuer, 2 epilogue thread 0) of CTA 0 appends (clock << 20 | item ordinal << 8 | chunk << 4 | code)
-// to its region of the buffer [3 counts][3][cap]
-__device__ __forceinline__ void trace_ev(const TcLayerArgs& a, int role, int& cnt, int code, int n, int c) {
-  if (a.trace == nullptr || blockIdx.x != 0 || cnt >= a.trace_cap) return;
-  a.trace[3 + (long)role * a.trace_cap + cnt] = (long long)(((unsigned long long)clock64() << 20) | ((unsigned long long)(n & 0xfff) << 8) | ((c & 0xf) << 4) | (code & 0xf));
-  a.trace[role] = ++cnt;
-}
 
 // ------------------------------------------------------------------------------------------------ one (layer, timestep) for all windows
-// Persistent: gridDim.x CTAs walk the work items (window tile, unit block); the accumulator is double-buffered in TMEM (2 x 256
-// columns), so the MMAs of item i+1 run while the epilogue warps finish the cell of item i; the TMA ring runs ahead across items.
+// Persistent: gridDim.x CTAs walk the work items (window tile, unit block) in a fixed stride; the producer warp's TMA ring runs
+// ahead across items.  An item whose tile holds no window is skipped by every role alike.
 // FIRST: layer 0 (the additive term is the per-row input projection, read from global memory); TANH: tanh cell / output activation.
-// Both are compile-time so that the epilogue -- the phase an item's time is made of (12-14 us per item whatever K) -- is branch-free:
-// as runtime switches they cost 35 CALLs, ~390 branches and local-memory traffic in the SASS of this kernel.
+// Both are compile-time so that the epilogue is branch-free.
 template <bool FIRST, bool TANH>
 __global__ void __launch_bounds__(NTHREADS, 1)
-lstm_tc_step_kernel(const TcLayerArgs a, const __grid_constant__ CUtensorMap m_below_hi, const __grid_constant__ CUtensorMap m_below_lo,
+lstm_tc_step_kernel(const __grid_constant__ TcLayerArgs a, const __grid_constant__ CUtensorMap m_below_hi, const __grid_constant__ CUtensorMap m_below_lo,
                     const __grid_constant__ CUtensorMap m_own_hi, const __grid_constant__ CUtensorMap m_own_lo,
                     const __grid_constant__ CUtensorMap m_w_hi, const __grid_constant__ CUtensorMap m_w_lo) {
-  // Epilogue groups: NG groups of 16 / NG warps, group g drains the items whose ordinal is g (mod NG).  Two groups run half an item apart,
-  // so one evaluates gates (MUFU bound) while the other is in its requests / stores / waits -- but a group then holds its accumulator
-  // twice as long, and the MMAs of the item after next wait for it.  Trace, cycles per item (one group / two groups): layer 0 (the input
-  // projection streams from HBM in the gate loop) 10.2 k / 11.5 k; the other layers 10.9 / 9.9 k (K = 384) and 9.0 / 8.4 k (K = 128).
-  constexpr int NG = FIRST ? 1 : 2;
-  constexpr int EPI_GROUP = EPI_WARPS / NG * 32;  // threads of one epilogue group
-  extern __shared__ __align__(1024) uint8_t smem[];
-  __shared__ uint32_t s_tmem;
-  __shared__ __align__(8) unsigned long long s_bar[3 * STAGES + 4];
-  __shared__ __align__(16) float s_bias[2][2][NCOL];  // [epilogue group][double buffer]
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  __shared__ __align__(8) unsigned long long s_bar[2 * STAGES];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));  // SWIZZLE_128B boxes: 1 KB aligned
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const uint32_t sbase = smem_u32(smem);
-  const uint32_t bar_full = smem_u32(&s_bar[0]), bar_empty = smem_u32(&s_bar[STAGES]), bar_done = smem_u32(&s_bar[2 * STAGES]),
-                 bar_free = smem_u32(&s_bar[2 * STAGES + 2]), bar_peer = smem_u32(&s_bar[2 * STAGES + 4]);  // bar_peer: the partner's stage s has landed (leader only)
+  const uint32_t bar_full = smem_u32(&s_bar[0]), bar_empty = smem_u32(&s_bar[STAGES]);
   const int u = a.u;
   if (tid == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(bar_full + 8 * s, 1);
-      mbar_init(bar_empty + 8 * s, PAIR_MODE == 1 ? 2 : 1);  // multicast mode: one tcgen05.commit per CTA of the pair, a stage is written by both CTAs' TMA
-      mbar_init(bar_peer + 8 * s, 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(bar_done + 8 * b, 1);
-      mbar_init(bar_free + 8 * b, (TWO_SM ? 2 : 1) * EPI_WARPS / NG);  // one arrival per warp of the group that drains it (pair MMA: of both CTAs, on the leader's barrier)
+      mbar_init(bar_empty + 8 * s, CONSUMERS);  // one arrival per consumer warpgroup when its MMAs on the stage are complete
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == EPI_WARPS + 1) {
-    if (TWO_SM) {
-      asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem)), "n"(2 * NCOL) : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    } else {
-      asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem)), "n"(2 * NCOL) : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-  }
-  tc_fence_before();
   __syncthreads();
-  if (PAIR > 1) cluster_sync_all();  // the partner's barriers are initialised before anything of ours can reach them
-  tc_fence_after();
-  const uint32_t tmem = s_tmem;
   const int n_chunks = a.kc_below + a.kc_own;
   const int nub = u / UB;
-  const int rank = PAIR > 1 ? (int)cluster_rank() : 0;
-  const int first_item = PAIR > 1 ? (int)(blockIdx.x / PAIR) : (int)blockIdx.x, item_step = (int)(gridDim.x / PAIR);
-  // work item -> (tile, ub): the unit blocks of one window tile are neighbours, so CTAs running side by side read the same A
-  // operand and it comes from L2.  Items whose tile holds no real window are skipped by every role alike.
-  // An item is a group of PAIR neighbouring tiles of one job x one unit block; this CTA takes tile rank of the group.  `real`: the
-  // group holds windows (every CTA of the pair runs the item's pipeline then -- the partner needs this CTA's half of the weights and
-  // its release of the stages); `mine`: this CTA's own tile holds windows (otherwise it computes on the group's first tile and
-  // writes nothing).
-  // The job record of an item is a global load (L2 latency) that every role needs before it can do anything for the item: each
-  // role requests the record of its NEXT item while it works on the current one and looks at it only when that item's turn comes
-  // (ncu: the exposed load was ~20 % of the stall samples of the narrow layers).
-  struct Item {
-    int item;                  // work item index (< 0: past the end); the rest of the coordinates are recomputed from it by resolve()
-    int slot, n_rows;          // the job record as loaded (the part this kernel uses)
-    long x_row;
-    int tile, ub, tj;          // filled in by resolve()
-    bool real, mine;
-    struct { int slot, n_rows; long x_row; } job;
-  };
-  auto fetch_item = [&](int item) -> Item {  // index arithmetic + the load; nothing here waits for the record
+  // item -> (tile, ub): the unit blocks of one window tile are neighbours, so CTAs running side by side read the same A operand from L2
+  struct Item { int tile, tj, ub, slot, n_rows; long x_row; bool real; };
+  auto item_of = [&](int item) -> Item {
     Item it;
-    it.item = -1;
-    it.slot = it.n_rows = 0;
-    it.x_row = 0;
-    if (item < a.n_items) {
-      const gb_job* jp = a.jobs + (item / nub) / a.pairs_per_job;
-      it.item = item;
-      const int2 sn = __ldg(reinterpret_cast<const int2*>(jp));  // slot, n_rows
-      it.slot = sn.x; it.n_rows = sn.y;
-      it.x_row = FIRST ? (long)__ldg(reinterpret_cast<const long long*>(&jp->x_row)) : 0;
-    }
+    const int grp = item / nub;
+    it.ub = item - grp * nub;
+    const int job_id = grp / a.tiles_per_job;
+    it.tj = grp - job_id * a.tiles_per_job;
+    it.tile = grp;
+    const gb_job* jp = a.jobs + job_id;
+    const int2 sn = __ldg(reinterpret_cast<const int2*>(jp));  // slot, n_rows
+    it.slot = sn.x; it.n_rows = sn.y;
+    it.x_row = FIRST ? (long)__ldg(reinterpret_cast<const long long*>(&jp->x_row)) : 0;
+    it.real = it.tj * TILE < it.n_rows;
     return it;
   };
-  auto resolve = [&](Item& it) {
-    it.real = it.mine = false;
-    if (it.item < 0) return;
-    const int grp = it.item / nub;
-    it.ub = it.item - grp * nub;
-    const int job_id = grp / a.pairs_per_job, tj0 = (grp - job_id * a.pairs_per_job) * PAIR;
-    it.job.slot = it.slot; it.job.n_rows = it.n_rows; it.job.x_row = it.x_row;
-    it.tj = tj0 + rank;
-    it.mine = it.tj < a.tiles_per_job && it.tj * TILE < it.n_rows;
-    if (!it.mine) it.tj = tj0;
-    it.tile = job_id * a.tiles_per_job + it.tj;
-    it.real = tj0 * TILE < it.n_rows;
-  };
 
-  if (warp == EPI_WARPS) {
-    // ============================== TMA producer
-    if (elect_one()) {
+  if (warp == CONSUMERS * 4) {
+    // ============================== TMA producer (one lane)
+    if (lane == 0) {
       int cc = 0;  // chunks issued so far (ring position)
-      int tr = 0, tn = 0;
-      Item nxt = fetch_item(first_item);
-      for (int item = first_item; item < a.n_items; item += item_step) {
-        Item cur = nxt;
-        resolve(cur);
-        nxt = fetch_item(item + item_step);
-        if (!cur.real) continue;
-        const int tile = cur.tile, ub = cur.ub;
-        const int row0 = tile * TILE, wrow0 = cur.slot * 4 * u + ub * NCOL;
+      for (int item = blockIdx.x; item < a.n_items; item += gridDim.x) {
+        const Item it = item_of(item);
+        if (!it.real) continue;
+        const int row0 = it.tile * TILE, wrow0 = it.slot * 4 * u + it.ub * NCOL;
         for (int c = 0; c < n_chunks; ++c, ++cc) {
           const int s = cc % STAGES, round = cc / STAGES;
           if (round > 0) mbar_wait(bar_empty + 8 * s, (round - 1) & 1);
-          trace_ev(a, 0, tr, 1, tn, c);
           const uint32_t st = sbase + s * STAGE_BYTES;
           mbar_expect_tx(bar_full + 8 * s, STAGE_BYTES);
           const bool below = c < a.kc_below;
           const int acol = (below ? c : c - a.kc_below) * KC;
           tma_load_2d(st, below ? &m_below_hi : &m_own_hi, acol, row0, bar_full + 8 * s);
           tma_load_2d(st + A_BOX, below ? &m_below_lo : &m_own_lo, acol, row0, bar_full + 8 * s);
-          if (TWO_SM) {  // this CTA's half of the weight box, into its own stage: the pair MMA reads 128 gate rows from each CTA
-            tma_load_2d(st + 2 * A_BOX, &m_w_hi, c * KC, wrow0 + rank * B_PART_ROWS, bar_full + 8 * s);
-            tma_load_2d(st + 2 * A_BOX + B_STAGE, &m_w_lo, c * KC, wrow0 + rank * B_PART_ROWS, bar_full + 8 * s);
-          } else if (PAIR_MODE == 1) {  // this CTA's half of the weight box, into both CTAs
-            tma_load_2d_mc(st + 2 * A_BOX + rank * B_PART, &m_w_hi, c * KC, wrow0 + rank * B_PART_ROWS, bar_full + 8 * s, (uint16_t)3);
-            tma_load_2d_mc(st + 2 * A_BOX + B_BOX + rank * B_PART, &m_w_lo, c * KC, wrow0 + rank * B_PART_ROWS, bar_full + 8 * s, (uint16_t)3);
-          } else {
-            tma_load_2d(st + 2 * A_BOX, &m_w_hi, c * KC, wrow0, bar_full + 8 * s);
-            tma_load_2d(st + 2 * A_BOX + B_BOX, &m_w_lo, c * KC, wrow0, bar_full + 8 * s);
-          }
-          trace_ev(a, 0, tr, 2, tn, c);
+          tma_load_2d(st + 2 * A_BOX, &m_w_hi, c * KC, wrow0, bar_full + 8 * s);
+          tma_load_2d(st + 2 * A_BOX + B_BOX, &m_w_lo, c * KC, wrow0, bar_full + 8 * s);
         }
-        ++tn;
       }
     }
-  } else if (warp == EPI_WARPS + 1) {
-    // ============================== MMA issuer (pair MMA: the leader CTA issues for both; the partner's warp reports its stages)
-    const uint32_t idesc = make_idesc_f16(TWO_SM ? 2 * TILE : TILE, NCOL);
-    int cc = 0, n = 0;  // chunks consumed, items started
-    int tr = 0;
-    Item nxt = fetch_item(first_item);
-    for (int item = first_item; item < a.n_items; item += item_step) {
-      Item cur = nxt;
-      resolve(cur);
-      nxt = fetch_item(item + item_step);
-      if (!cur.real) continue;
-      const int buf = n & 1;
-      if (TWO_SM && rank != 0) {
-        // partner of the pair: when a stage of ours has landed, tell the leader (its MMAs read our shared memory)
-        for (int c = 0; c < n_chunks; ++c, ++cc) {
-          const int s = cc % STAGES, round = cc / STAGES;
-          mbar_wait(bar_full + 8 * s, round & 1);
-          if (elect_one()) mbar_arrive_remote(bar_peer + 8 * s, 0);
-          __syncwarp();
-        }
-        ++n;
-        continue;
-      }
-      if (n >= 2) mbar_wait(bar_free + 8 * buf, ((n >> 1) - 1) & 1);  // the epilogue has drained this accumulator (pair MMA: in both CTAs)
-      tc_fence_after();
-      if (lane == 0) trace_ev(a, 1, tr, 3, n, 0);
-      const uint32_t dcol = tmem + buf * NCOL;
+  } else {
+    // ============================== consumer warpgroup: MMAs of its 64 windows, then gates, cell, h
+    // Fragment layout (gb_sm90.cuh): this thread holds windows r0 and r0 + 8 and, for every gate, the unit pairs 8jj + 2t + {0,1}
+    // (jj = 0..7) -- accumulator register 4 (8 G + jj) + 2 hr + e is gate G of unit 8jj + 2t + e of window r0 + 8 hr.
+    const int wg = warp >> 2, wq = warp & 3, g = lane >> 2, t = lane & 3;
+    const int r0 = wg * 64 + wq * 16 + g;  // window row in the tile
+    int cc = 0;
+    for (int item = blockIdx.x; item < a.n_items; item += gridDim.x) {
+      const Item it = item_of(item);
+      if (!it.real) continue;
+      float d[128];
       for (int c = 0; c < n_chunks; ++c, ++cc) {
         const int s = cc % STAGES, round = cc / STAGES;
         mbar_wait(bar_full + 8 * s, round & 1);
-        if (TWO_SM) mbar_wait(bar_peer + 8 * s, round & 1);
-        tc_fence_after();
-        if (lane == 0) trace_ev(a, 1, tr, 4, n, c);
-        if (elect_one()) {
-          const uint32_t st = sbase + s * STAGE_BYTES;
-          const uint64_t a_hi = make_desc_sw128(st), a_lo = make_desc_sw128(st + A_BOX);
-          const uint64_t b_hi = make_desc_sw128(st + 2 * A_BOX), b_lo = make_desc_sw128(st + 2 * A_BOX + B_STAGE);
+        const uint32_t st = sbase + s * STAGE_BYTES;
+        const uint32_t a_hi = st + wg * 64 * ROW_BYTES, a_lo = st + A_BOX + wg * 64 * ROW_BYTES;
+        const uint32_t b_hi = st + 2 * A_BOX, b_lo = st + 2 * A_BOX + B_BOX;
+        wgmma_fence();
 #pragma unroll
-          for (int ks = 0; ks < KC / 16; ++ks) {
-            const uint64_t adv = (uint64_t)(ks * 2);  // 32 bytes per K step, in 16-byte units of the address field
-            const uint32_t acc = (c > 0 || ks > 0) ? 1u : 0u;
-            if (TWO_SM) {
-              mma_f16_ss_2sm(dcol, a_lo + adv, b_hi + adv, idesc, acc);
-              mma_f16_ss_2sm(dcol, a_hi + adv, b_lo + adv, idesc, 1u);
-              mma_f16_ss_2sm(dcol, a_hi + adv, b_hi + adv, idesc, 1u);
-            } else {
-              mma_f16_ss(dcol, a_lo + adv, b_hi + adv, idesc, acc);
-              mma_f16_ss(dcol, a_hi + adv, b_lo + adv, idesc, 1u);
-              mma_f16_ss(dcol, a_hi + adv, b_hi + adv, idesc, 1u);
-            }
-          }
-          if (TWO_SM) {  // the stage is free, and at the end of the item the accumulator ready, in BOTH CTAs
-            mma_commit_2sm(bar_empty + 8 * s, (uint16_t)3);
-            if (c + 1 == n_chunks) mma_commit_2sm(bar_done + 8 * buf, (uint16_t)3);
-          } else {
-            if (PAIR_MODE == 1) mma_commit_mc(bar_empty + 8 * s, (uint16_t)3); else mma_commit(bar_empty + 8 * s);
-            if (c + 1 == n_chunks) mma_commit(bar_done + 8 * buf);
-          }
+        for (int ks = 0; ks < KC / 16; ++ks) {
+          const uint32_t adv = ks * 32;  // 32 bytes per K step inside the 128-byte swizzle row
+          wgmma_ss_f16_n256(d, desc_sw128(a_lo + adv), desc_sw128(b_hi + adv), (c > 0 || ks > 0) ? 1u : 0u);
+          wgmma_ss_f16_n256(d, desc_sw128(a_hi + adv), desc_sw128(b_lo + adv), 1u);
+          wgmma_ss_f16_n256(d, desc_sw128(a_hi + adv), desc_sw128(b_hi + adv), 1u);
         }
-        __syncwarp();
-        if (lane == 0) trace_ev(a, 1, tr, 5, n, c);
-      }
-      ++n;
-    }
-  } else {
-    // ============================== epilogue: gates, cell, h (one thread = one window x NG * UH units, in NG passes of UH)
-    // Everything that does not depend on the accumulator is requested while the MMAs run (c_{t-1}, the first input-projection
-    // slice), and inside the loop the next slice's TMEM / global loads are in flight while the current one is evaluated.
-    const int grp = warp / (EPI_WARPS / NG), wg = warp % (EPI_WARPS / NG), tg = tid & (EPI_GROUP - 1);
-    const int r = tid & (TILE - 1), ublk = wg >> 2;  // window row 0..127; which block of NG * UH units this warp evaluates
-    int n = 0, tr = 0;                                 // items seen (real ones)
-    bool bias_staged = false;  // the previous item of this group already put this item's bias into its buffer
-    Item q0 = fetch_item(first_item), q1 = fetch_item(first_item + item_step);  // two records ahead: a skipped item costs no load latency
-    for (int item = first_item; item < a.n_items; item += item_step) {
-      Item cur_item = q0;
-      resolve(cur_item);
-      q0 = q1;
-      q1 = fetch_item(item + 2 * item_step);
-      if (!cur_item.real) continue;
-      if (NG > 1 && (n % NG) != grp) { ++n; continue; }
-      const int tile = cur_item.tile, ub = cur_item.ub, tj = cur_item.tj;
-      const auto job = cur_item.job;
-      const int buf = n & 1, m = n / NG;                   // accumulator; ordinal of the item inside this group
-      if (tid == 0) trace_ev(a, 2, tr, 6, n, 0);
-      const int w = tj * TILE + r;                         // window index inside the job (may exceed n_rows in the last tile)
-      const long row = (long)tile * TILE + r;
-      float* sbuf = s_bias[grp][m & 1];
-      float bias_next = 0.f;
-      if (!FIRST) {
-        // this buffer's previous readers (this group's item m-2) finished before the group barrier of item m-1
-        if (!bias_staged) {
-          for (int i = tg; i < NCOL; i += EPI_GROUP) sbuf[i] = __ldg(a.bias + (long)job.slot * 4 * u + ub * NCOL + i);
+        wgmma_commit();
+        if (c > 0) {  // the previous chunk's MMAs are complete: its stage goes back to the producer
+          wgmma_wait<1>();
+          if ((tid & 127) == 0) mbar_arrive(bar_empty + 8 * ((cc - 1) % STAGES));
         }
-        if (grp == 0) asm volatile("bar.sync 1, %0;" ::"n"(EPI_GROUP) : "memory");
-        else asm volatile("bar.sync 2, %0;" ::"n"(EPI_GROUP) : "memory");
-        // request the bias of this group's NEXT item (NG items ahead) now, store it when this item's arithmetic is done.  Only when
-        // the following NG items all hold windows (otherwise the next item of the group is not known yet: it loads its bias itself).
-        Item p0 = q0, p1 = q1;
-        resolve(p0);
-        resolve(p1);
-        const Item& pn = NG == 1 ? p0 : p1;
-        bias_staged = p0.real && pn.real && tg < NCOL;
-        if (bias_staged)  // volatile: ptxas would otherwise sink the load to its use at the end of the item
-          asm volatile("ld.global.nc.f32 %0, [%1];" : "=f"(bias_next) : "l"(a.bias + (long)pn.job.slot * 4 * u + pn.ub * NCOL + tg));
       }
-      bool waited = false;
-#pragma unroll 1
-      for (int pass = 0; pass < NG; ++pass) {
-        const int unit0 = ublk * (NG * UH) + pass * UH;  // first of the UH units of this pass
-        const uint32_t lane_base = tmem + buf * NCOL + ((uint32_t)((warp & 3) * 32) << 16) + unit0;
+      wgmma_wait<0>();
+      if ((tid & 127) == 0) mbar_arrive(bar_empty + 8 * ((cc - 1) % STAGES));
+#pragma unroll
+      for (int i = 0; i < 128; ++i) fence_reg(d[i]);
+
+#pragma unroll
+      for (int hr = 0; hr < 2; ++hr) {
+        const int r = r0 + 8 * hr;
+        const int w = it.tj * TILE + r;  // window index inside the job (may exceed n_rows in the last tile)
+        const long row = (long)it.tile * TILE + r;
         const float* xk = nullptr;
-        if (FIRST) {  // xk is stored row-blocked, [row / 128][4u reordered][128]: windows (threads) run along the fastest axis
-          const long xr = min(job.x_row + min(w, job.n_rows - 1) + a.t, a.xk_rows - 1);
-          xk = a.xk + ((xr >> 7) * (long)(4 * u) + ub * NCOL + unit0) * TILE + (xr & (TILE - 1));
+        if (FIRST) {  // xk is stored row-blocked, [row / 128][4u reordered][128]
+          const long xr = min(it.x_row + min(w, it.n_rows - 1) + a.t, a.xk_rows - 1);
+          xk = a.xk + ((xr >> 7) * (long)(4 * u) + it.ub * NCOL) * TILE + (xr & (TILE - 1));
         }
-        // c is stored tile-blocked, [tile][unit][128 windows]: consecutive threads (windows) touch consecutive floats and an item's
-        // slice is one contiguous 32 KB block (a row-major layout costs a 32-byte sector per thread and access)
-        float* ccol = a.c + ((long)tile * u + ub * UB + unit0) * TILE + r;  // unit j of this window: ccol[j * TILE]
-        __half* hh = a.h_out_hi + row * u + ub * UB + unit0;
-        __half* hl = a.h_out_lo + row * u + ub * UB + unit0;
-        const float* sb = sbuf + unit0;
-        float cp[UH];
+        const float* bias = FIRST ? nullptr : a.bias + (long)it.slot * 4 * u + it.ub * NCOL;
+        float* ccol = a.c + ((long)it.tile * u + it.ub * UB) * TILE + r;  // unit j of this window: ccol[j * TILE]
+        __half2* hh = reinterpret_cast<__half2*>(a.h_out_hi + row * u + it.ub * UB);
+        __half2* hl = reinterpret_cast<__half2*>(a.h_out_lo + row * u + it.ub * UB);
 #pragma unroll
-        for (int i = 0; i < UH; ++i) cp[i] = a.t == 0 ? 0.f : ccol[i * TILE];
-        if (NG > 1 && pass == 0 && a.t != 0) {  // the second pass's state: towards L2 now
+        for (int jj = 0; jj < 8; ++jj) {
+          float hv[2];
 #pragma unroll
-          for (int i = 0; i < UH; ++i) asm volatile("prefetch.global.L2 [%0];" ::"l"(ccol + (UH + i) * TILE));
-        }
-        float ad[2][4][SL];  // [buffer][gate][unit]: the additive term (bias, or layer 0's input projection incl. bias)
-        auto load_add = [&](int b2, int j0) {
+          for (int e = 0; e < 2; ++e) {
+            const int unit = 8 * jj + 2 * t + e;
+            float z[4];
 #pragma unroll
-          for (int g = 0; g < 4; ++g)
-#pragma unroll
-            for (int i = 0; i < SL; ++i) ad[b2][g][i] = FIRST ? __ldg(xk + (g * UB + j0 + i) * TILE) : sb[g * UB + j0 + i];
-        };
-        load_add(0, 0);
-        if (!waited) {
-          if (tid == 0) trace_ev(a, 2, tr, 7, n, 0);
-          mbar_wait(bar_done + 8 * buf, (n >> 1) & 1);
-          tc_fence_after();
-          if (tid == 0) trace_ev(a, 2, tr, 8, n, 0);
-          waited = true;
-        }
-        float z[2][4][SL];
-        uint32_t hp1[UH / 2], hp2[UH / 2];
-#pragma unroll
-        for (int g = 0; g < 4; ++g) tmem_ldn<SL>(lane_base + g * UB, z[0][g]);
-#pragma unroll
-        for (int it = 0; it < UH / SL; ++it) {
-          const int j0 = it * SL, cur = it & 1;
-          tmem_wait_ld();
-          if (it + 1 < UH / SL) {
-#pragma unroll
-            for (int g = 0; g < 4; ++g) tmem_ldn<SL>(lane_base + g * UB + j0 + SL, z[cur ^ 1][g]);
-            load_add(cur ^ 1, j0 + SL);
-          } else if (pass == NG - 1) {
-            tc_fence_before();  // last slice of the accumulator is in registers: hand the buffer back to the MMA warp
-            __syncwarp();
-            if (lane == 0) {
-              if (TWO_SM && rank != 0) mbar_arrive_remote(bar_free + 8 * buf, 0);  // the leader issues the next MMAs into both CTAs' accumulators
-              else asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar_free + 8 * buf) : "memory");
-            }
-          }
-          float cn[SL], hv[SL];
-#pragma unroll
-          for (int i = 0; i < SL; ++i) {
+            for (int G = 0; G < 4; ++G) z[G] = d[4 * (8 * G + jj) + 2 * hr + e] + (FIRST ? __ldg(xk + (G * UB + unit) * TILE) : __ldg(bias + G * UB + unit));
+            const float cp = a.t == 0 ? 0.f : ccol[unit * TILE];
+            float cn;
             if (TANH) {
-              tanh_cell(z[cur][0][i] + ad[cur][0][i], z[cur][1][i] + ad[cur][1][i], z[cur][2][i] + ad[cur][2][i], z[cur][3][i] + ad[cur][3][i],
-                        cp[j0 + i], cn[i], hv[i]);
+              tanh_cell(z[0], z[1], z[2], z[3], cp, cn, hv[e]);
             } else {
-              const float ig = sigm(z[cur][0][i] + ad[cur][0][i]), fg = sigm(z[cur][1][i] + ad[cur][1][i]);
-              const float gg = gb::apply_act(a.act, z[cur][2][i] + ad[cur][2][i]), og = sigm(z[cur][3][i] + ad[cur][3][i]);
-              cn[i] = fmaf(fg, cp[j0 + i], ig * gg);
-              hv[i] = og * gb::apply_act(a.act, cn[i]);
+              const float ig = sigm(z[0]), fg = sigm(z[1]), gg = gb::apply_act(a.act, z[2]), og = sigm(z[3]);
+              cn = fmaf(fg, cp, ig * gg);
+              hv[e] = og * gb::apply_act(a.act, cn);
             }
+            ccol[unit * TILE] = cn;
           }
-          if (cur_item.mine) {
-#pragma unroll
-            for (int i = 0; i < SL; ++i) ccol[(j0 + i) * TILE] = cn[i];
-          }
-#pragma unroll
-          for (int i = 0; i < SL / 2; ++i) {  // FP16 pair h = h1 + h2, packed in registers: a pass's UH units are one full 32-byte sector per image
-            const __half2 p1 = __floats2half2_rn(hv[2 * i], hv[2 * i + 1]);  // low half = even unit
-            const float2 f1 = __half22float2(p1);
-            const __half2 p2 = __floats2half2_rn(hv[2 * i] - f1.x, hv[2 * i + 1] - f1.y);
-            hp1[(j0 >> 1) + i] = *reinterpret_cast<const uint32_t*>(&p1);
-            hp2[(j0 >> 1) + i] = *reinterpret_cast<const uint32_t*>(&p2);
-          }
-        }
-        if (cur_item.mine) {  // a CTA without a tile of its own ran the item for its partner's sake (weights, stage release) on the group's first tile
-          // one 256-bit store per image: a pass's UH units are exactly one 32-byte sector of the row (two 128-bit stores cost the LSU two
-          // half-filled sector transactions each; trace: 2.2 k cycles to issue an item's h stores when all warps reach them together)
-          static_assert(UH == 16, "a pass's units = one 32-byte sector of FP16");
-          st_global_256(hh, hp1);
-          st_global_256(hl, hp2);
+          // FP16 pair h = h1 + h2 (low half = even unit)
+          const __half2 p1 = __floats2half2_rn(hv[0], hv[1]);
+          const float2 f1 = __half22float2(p1);
+          hh[4 * jj + t] = p1;
+          hl[4 * jj + t] = __floats2half2_rn(hv[0] - f1.x, hv[1] - f1.y);
         }
       }
-      if (tid == 0) trace_ev(a, 2, tr, 9, n, 0);
-      if (!FIRST && bias_staged) s_bias[grp][(m & 1) ^ 1][tg] = bias_next;
-      if (tid == 0) trace_ev(a, 2, tr, 10, n, 0);
-      ++n;
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (PAIR > 1) cluster_sync_all();  // nothing of the partner's (multicast bytes, barrier arrivals) may still be on its way into this CTA
-  if (warp == EPI_WARPS + 1) {
-    if (TWO_SM) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem), "n"(2 * NCOL) : "memory");
-    else asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "n"(2 * NCOL) : "memory");
   }
 }
 
@@ -704,7 +348,7 @@ int make_map_f16(CUtensorMap* map, const void* base, long rows, long cols, int b
   cuuint32_t box[2] = {KC, (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1, 1};
   CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                  KC == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                  CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   GB_REQUIRE(r == CUDA_SUCCESS, GB_E_CUDA, "cuTensorMapEncodeTiled (fp16) failed with CUresult %d", (int)r);
   return GB_OK;
 }
@@ -752,25 +396,13 @@ void make_plan(const gb_lstmnet* net, int n_slots, long rows_pad, long x_rows, P
   p->total = ofs;
 }
 
-long long* g_lstm_trace = nullptr;
-int g_lstm_trace_cap = 0, g_lstm_trace_layer = -1;
-
 }  // namespace
-
-// debug aid (not part of the public header): timeline of CTA 0 of the step kernel of `layer` at the last timestep into a device buffer of
-// 3 + 3 * capacity int64 (zeroed by the caller)
-extern "C" int gb_debug_set_lstm_trace(void* dev_buf, int capacity, int layer) {
-  g_lstm_trace = static_cast<long long*>(dev_buf);
-  g_lstm_trace_cap = capacity;
-  g_lstm_trace_layer = layer;
-  return GB_OK;
-}
 
 extern "C" int gb_lstm_tc_supported(const gb_lstmnet* net) {
   GB_REQUIRE(net != nullptr, GB_E_ARG, "net is NULL");
   GB_REQUIRE(net->n_layers >= 1 && net->n_layers <= GB_MAX_LAYERS, GB_E_SHAPE, "n_layers=%d outside [1,%d]", net->n_layers, GB_MAX_LAYERS);
   for (int l = 0; l < net->n_layers; ++l)
-    GB_REQUIRE(net->units[l] >= 1 && net->units[l] <= 512, GB_E_SHAPE, "tcgen05 LSTM variant covers layer widths 1..512, units[%d]=%d", l, net->units[l]);
+    GB_REQUIRE(net->units[l] >= 1 && net->units[l] <= 512, GB_E_SHAPE, "tensor-core LSTM variant covers layer widths 1..512, units[%d]=%d", l, net->units[l]);
   GB_REQUIRE(net->n_features >= 1 && net->n_features <= 512 && net->n_features_out >= 1 && net->n_features_out <= 512, GB_E_SHAPE, "bad feature counts");
   GB_REQUIRE(net->lookback >= 1, GB_E_ARG, "lookback=%d must be >= 1", net->lookback);
   return GB_OK;
@@ -818,11 +450,11 @@ extern "C" int gb_lstm_infer_tc(const gb_lstmnet* net, const float* params, int3
       if ((rc = make_map_f16(&m_h[l][b][0], ws + p.h_hi[l][b], rows_pad, p.u[l], TILE)) != GB_OK) return rc;
       if ((rc = make_map_f16(&m_h[l][b][1], ws + p.h_lo[l][b], rows_pad, p.u[l], TILE)) != GB_OK) return rc;
     }
-    if ((rc = make_map_f16(&m_w[l][0], ws + p.w_hi[l], (long)n_slots * 4 * p.u[l], p.kp[l], B_PART_ROWS)) != GB_OK) return rc;
-    if ((rc = make_map_f16(&m_w[l][1], ws + p.w_lo[l], (long)n_slots * 4 * p.u[l], p.kp[l], B_PART_ROWS)) != GB_OK) return rc;
+    if ((rc = make_map_f16(&m_w[l][0], ws + p.w_hi[l], (long)n_slots * 4 * p.u[l], p.kp[l], NCOL)) != GB_OK) return rc;
+    if ((rc = make_map_f16(&m_w[l][1], ws + p.w_lo[l], (long)n_slots * 4 * p.u[l], p.kp[l], NCOL)) != GB_OK) return rc;
   }
-  const size_t smem = (size_t)STAGES * STAGE_BYTES + 1024;
-  int dev = 0, sms = 148;
+  const size_t smem = (size_t)STAGES * STAGE_BYTES + 1024;  // + alignment slack of the 1 KB aligned ring
+  int dev = 0, sms = 132;
   GB_CUDA_CHECK(cudaGetDevice(&dev));
   GB_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   using StepKernel = void (*)(const TcLayerArgs, const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap);
@@ -836,31 +468,19 @@ extern "C" int gb_lstm_infer_tc(const gb_lstmnet* net, const float* params, int3
     const int wr = t & 1, rd = wr ^ 1;
     for (int l = 0; l < p.nl; ++l) {
       TcLayerArgs a{};
-      a.u = p.u[l]; a.kc_below = p.kp_below[l] / KC; a.kc_own = p.u[l] / KC; a.act = net->act[l]; a.is_first = l == 0;
-      a.tiles_per_job = tiles_per_job; a.t = t; a.lookback = p.L; a.jobs = jobs;
+      a.u = p.u[l]; a.kc_below = p.kp_below[l] / KC; a.kc_own = p.u[l] / KC; a.act = net->act[l];
+      a.tiles_per_job = tiles_per_job; a.t = t; a.jobs = jobs;
       a.bias = reinterpret_cast<const float*>(ws + p.bias[l]);
       a.xk = reinterpret_cast<const float*>(ws + p.xk); a.xk_rows = x_rows;
       a.c = reinterpret_cast<float*>(ws + p.c[l]);
       a.h_out_hi = reinterpret_cast<__half*>(ws + p.h_hi[l][wr]);
       a.h_out_lo = reinterpret_cast<__half*>(ws + p.h_lo[l][wr]);
-      a.trace = (g_lstm_trace != nullptr && l == g_lstm_trace_layer && t == p.L - 1) ? g_lstm_trace : nullptr;
-      a.trace_cap = g_lstm_trace_cap;
       const int lb = l > 0 ? l - 1 : 0;
-      a.pairs_per_job = (tiles_per_job + PAIR - 1) / PAIR;
-      a.n_items = n_jobs * a.pairs_per_job * (p.u[l] / UB);
-      const int groups = a.n_items < sms / PAIR ? a.n_items : sms / PAIR;
-      cudaLaunchConfig_t cfg{};
-      cfg.gridDim = dim3(groups * PAIR);
-      cfg.blockDim = dim3(NTHREADS);
-      cfg.dynamicSmemBytes = smem;
-      cfg.stream = st;
-      cudaLaunchAttribute attr[1];
-      attr[0].id = cudaLaunchAttributeClusterDimension;
-      attr[0].val.clusterDim.x = PAIR; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-      cfg.attrs = attr;
-      cfg.numAttrs = 1;
-      GB_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kernels[l == 0][net->act[l] == GB_ACT_TANH], a, m_h[lb][wr][0], m_h[lb][wr][1], m_h[l][rd][0], m_h[l][rd][1],
-                                       m_w[l][0], m_w[l][1]));
+      a.n_items = n_jobs * tiles_per_job * (p.u[l] / UB);
+      const int grid = a.n_items < sms ? a.n_items : sms;
+      kernels[l == 0][net->act[l] == GB_ACT_TANH]<<<grid, NTHREADS, smem, st>>>(a, m_h[lb][wr][0], m_h[lb][wr][1], m_h[l][rd][0], m_h[l][rd][1],
+                                                                              m_w[l][0], m_w[l][1]);
+      GB_CUDA_CHECK(cudaGetLastError());
     }
   }
   const int top = p.nl - 1, fin = (p.L - 1) & 1;

@@ -36,7 +36,7 @@ def cuda_device(device=None):
     """Resolve a CUDA device or fail loudly -- there is no CPU path."""
     torch = _torch()
     if not torch.cuda.is_available():
-        raise _cabi.GordoB200Error("no CUDA device visible: gordo_components_b200 runs on B200 (sm_100a) only, there is no CPU fallback")
+        raise _cabi.GordoB200Error("no CUDA device visible: gordo_components_b200 runs on H100 (sm_90a) only, there is no CPU fallback")
     dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
     if dev.index is None:
         dev = torch.device("cuda", torch.cuda.current_device())
@@ -422,7 +422,7 @@ class LSTMEngine:
     def infer(self, params, jobs_dev, n_jobs, max_windows, x, out_rows, variant: int = 0):
         """
         out[j] = net(x[j : j + lookback]) for every job's windows (jobs' n_rows counts windows).
-        variant 0 = tcgen05 kernel when the layer widths allow it, 1 = fp32 CUDA-core kernel, 2 = tcgen05 (error if unsupported).
+        variant 0 = tensor-core (wgmma) kernel when the layer widths allow it, 1 = fp32 CUDA-core kernel, 2 = tensor-core kernel (error if unsupported).
         """
         torch = _torch()
         out = torch.empty((int(out_rows), self.n_out), dtype=torch.float32, device=self.device)

@@ -1,4 +1,4 @@
-"""Network specifications produced by the factories and consumed by the B200 engine."""
+"""Network specifications produced by the factories and consumed by the CUDA engine."""
 from dataclasses import dataclass, field
 from typing import Any, Dict, List
 
@@ -7,17 +7,17 @@ SUPPORTED_ACTIVATIONS = ("tanh", "relu", "sigmoid", "linear")
 
 def _check_act(name):
     if name not in SUPPORTED_ACTIVATIONS:
-        raise ValueError(f"activation {name!r} is not supported by the B200 kernels {SUPPORTED_ACTIVATIONS}")
+        raise ValueError(f"activation {name!r} is not supported by the CUDA kernels {SUPPORTED_ACTIVATIONS}")
     return name
 
 
 def _optimizer(optimizer, optimizer_kwargs, compile_kwargs):
     """Only what the kernels implement is accepted: Adam + mean squared error."""
     if not isinstance(optimizer, str) or optimizer.lower() != "adam":
-        raise ValueError(f"optimizer {optimizer!r}: the B200 fit kernel implements Adam only")
+        raise ValueError(f"optimizer {optimizer!r}: the CUDA fit kernel implements Adam only")
     loss = (compile_kwargs or {}).get("loss", "mse")
     if loss not in ("mse", "mean_squared_error"):
-        raise ValueError(f"loss {loss!r}: the B200 fit kernel implements mean squared error only")
+        raise ValueError(f"loss {loss!r}: the CUDA fit kernel implements mean squared error only")
     kw = dict(optimizer_kwargs or {})
     out = {
         "lr": float(kw.pop("learning_rate", kw.pop("lr", 1e-3))),

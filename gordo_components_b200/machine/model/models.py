@@ -3,7 +3,7 @@ sklearn-style model wrappers with the public surface of gordo/machine/model/mode
 (KerasBaseEstimator :36-357, KerasAutoEncoder :360-398, KerasLSTMBaseEstimator :463-698,
 KerasLSTMForecast :701-704, KerasLSTMAutoEncoder :707-710, create_keras_timeseriesgenerator :713-793)
 -- same class names, constructor arguments, methods, return types and exceptions -- whose fit and
-predict run as CUDA kernels on a B200 through ``gordo_components_b200.engine``.
+predict run as CUDA kernels on an H100 through ``gordo_components_b200.engine``.
 
 The class names keep their "Keras" prefix on purpose: gordo model definitions, the factory registry
 (``register_model_builder.factories["KerasAutoEncoder"]``) and stored metadata key on them.  There is no
@@ -146,7 +146,7 @@ def build_callbacks(definitions) -> list:
             out.append(EarlyStopping(**{k: getattr(cb, k) for k in ("monitor", "min_delta", "patience", "baseline", "restore_best_weights",
                                                                     "start_from_epoch") if hasattr(cb, k)}))
         else:
-            logger.warning("callback %s is not supported by the B200 fit loop and is ignored", cb)
+            logger.warning("callback %s is not supported by the CUDA fit loop and is ignored", cb)
     return out
 
 
@@ -266,7 +266,7 @@ class KerasBaseEstimator(BaseEstimator, GordoBase):
         spec = self._factory()(**self.sk_params)
         if not isinstance(spec, (FFNetSpec, LSTMNetSpec)):
             raise ValueError(
-                f"factory {self.kind!r} returned {type(spec).__name__}; B200 factories must return an FFNetSpec or LSTMNetSpec"
+                f"factory {self.kind!r} returned {type(spec).__name__}; factories must return an FFNetSpec or LSTMNetSpec"
             )
         return spec
 

@@ -3,7 +3,7 @@ Factory registry ``{type: {kind: function}}`` (mirror of gordo/machine/model/reg
 
 A registered factory takes ``n_features`` (plus keyword arguments from the model definition)
 and returns a network *specification* (``factories.specs.FFNetSpec`` / ``LSTMNetSpec``) -- the
-B200 engine compiles nothing per model, so there is no framework graph object to build.
+CUDA engine compiles nothing per model, so there is no framework graph object to build.
 """
 import inspect
 from typing import Callable, Dict

@@ -13,7 +13,7 @@ builder that runs where gordo itself is not installed needs the same three thing
 * ``dump`` / ``load`` / ``load_metadata`` / ``load_info``: ``model.pkl`` + ``metadata.json`` + ``info.json``.
 
 Class paths written for the reference (``gordo.machine.model...``, and the pre-1.0 ``gordo_components.model...``) resolve to
-this package's classes, so production configs load unchanged; Keras callback paths resolve to the callbacks of the B200 fit
+this package's classes, so production configs load unchanged; Keras callback paths resolve to the callbacks of the CUDA fit
 loop.
 """
 import copy

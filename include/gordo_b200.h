@@ -1,5 +1,5 @@
 /*
- * gordo_b200.h -- C ABI of the B200 (sm_100a) implementation of gordo's per-machine
+ * gordo_b200.h -- C ABI of the H100 (sm_90a) implementation of gordo's per-machine
  * autoencoder train-and-score hot path.
  *
  * The reference (equinor/gordo-components) has no native FFI: its plug-in boundary is a
@@ -43,7 +43,7 @@ typedef enum gb_status {
   GB_E_ALIGN = -3,   /* pointer not 16-byte aligned                            -> ValueError  */
   GB_E_SMEM = -4,    /* architecture does not fit in shared memory             -> ValueError  */
   GB_E_CUDA = -5,    /* CUDA runtime error (message has cudaGetErrorString)    -> RuntimeError*/
-  GB_E_DEVICE = -6   /* no sm_100 device                                       -> RuntimeError*/
+  GB_E_DEVICE = -6   /* no sm_90 device                                        -> RuntimeError*/
 } gb_status;
 
 typedef enum gb_act { GB_ACT_LINEAR = 0, GB_ACT_TANH = 1, GB_ACT_RELU = 2, GB_ACT_SIGMOID = 3 } gb_act;
@@ -71,7 +71,7 @@ typedef struct gb_job {
 /* ---- library ------------------------------------------------------------------------ */
 int gb_abi_version(void);
 const char* gb_last_error(void);
-/* 0 if `device` is an sm_100 part; GB_E_DEVICE otherwise.  Fills sm count if non-null. */
+/* 0 if `device` is an sm_90 (H100) part; GB_E_DEVICE otherwise.  Fills sm count if non-null. */
 int gb_device_check(int device, int* sm_count);
 
 /* ---- parameter layout ---------------------------------------------------------------
@@ -97,8 +97,8 @@ size_t gb_ffnet_param_stride(const gb_ffnet* net);
  * params: [n_slots][param_stride]; scale, feat_thr: [n_slots][n_out]; agg_thr: [n_slots].
  * jobs: DEVICE array of n_jobs gb_job; max_rows = max n_rows over jobs (host value, sizes the grid).
  * n_x_rows / n_out_rows: number of rows of the x (and y) array and of the output arrays (TMA tensor extents).
- * variant (low byte): 0 = auto (tcgen05 kernel for the stacks it covers, the row-per-thread kernel for stacks whose widths are
- * all <= 16, else the generic one), 1 = generic fp32 CUDA-core kernel, 2 = tcgen05 split-precision kernel, 3 = row-per-thread
+ * variant (low byte): 0 = auto (tensor-core kernel for the stacks it covers, the row-per-thread kernel for stacks whose widths are
+ * all <= 16, else the generic one), 1 = generic fp32 CUDA-core kernel, 2 = tensor-core (wgmma) split-precision kernel, 3 = row-per-thread
  * fp32 kernel (2 / 3: GB_E_SHAPE if the architecture is outside their range); higher bytes are debug knobs and must be 0. */
 int gb_ffae_infer_score(const gb_ffnet* net, const float* params, const gb_job* jobs, int32_t n_jobs,
                         int32_t max_rows, int64_t n_x_rows, int64_t n_out_rows, const float* x, const float* y, const float* scale,
@@ -107,7 +107,7 @@ int gb_ffae_infer_score(const gb_ffnet* net, const float* params, const gb_job* 
                         float* out_total_unscaled, float* out_conf, float* out_total_conf,
                         int32_t variant, void* stream);
 
-/* GB_OK if the tcgen05 (variant 2) kernel covers this architecture, else GB_E_SHAPE. */
+/* GB_OK if the tensor-core (variant 2) kernel covers this architecture, else GB_E_SHAPE. */
 int gb_ffae_tc_supported(const gb_ffnet* net);
 
 /* ---- K4 alone: anomaly score of predictions that already exist ----------------------------
@@ -241,9 +241,9 @@ size_t gb_lstm_workspace_bytes(const gb_lstmnet* net, int32_t n_jobs, int32_t ma
 int gb_lstm_infer(const gb_lstmnet* net, const float* params, const gb_job* jobs, int32_t n_jobs,
                   int32_t max_rows, const float* x, float* out_model, void* workspace, void* stream);
 
-/* ---- K3 on tcgen05 (layer widths 1..512, padded to multiples of 64 internally).  One launch per
+/* ---- K3 on the tensor cores, wgmma (layer widths 1..512, padded to multiples of 64 internally).  One launch per
  * (layer, timestep) advances every window of every job: [h_below,t | h_own,t-1] . [K; U]^T on the tensor cores
- * (FP16-pair split operands, fp32 accumulation in TMEM), LSTM cell in the epilogue, recurrent state in `workspace`
+ * (FP16-pair split operands, fp32 accumulation), LSTM cell in the epilogue, recurrent state in `workspace`
  * (gb_lstm_tc_workspace_bytes; x_rows = rows of the x array, n_slots = rows of params). */
 int gb_lstm_tc_supported(const gb_lstmnet* net);
 size_t gb_lstm_tc_workspace_bytes(const gb_lstmnet* net, int32_t n_slots, int32_t n_jobs, int32_t max_windows, int64_t x_rows);

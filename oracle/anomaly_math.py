@@ -5,7 +5,7 @@ cpu_baseline / ``--impl reference`` legs may import this module.
 
 PARITY STATUS: **pinned.**  Every function here is checked against outputs of the
 reference's own, unmodified ``gordo/machine/model/anomaly/diff.py`` executed from
-``/root/reference`` (``oracle/reference_loader.py``; fixtures committed under
+the reference project (``oracle/reference_loader.py``; fixtures committed under
 ``tests/golden/`` by ``tests/golden/make_golden.py``), and against the formula pins in
 ``tests/gordo/machine/model/anomaly/test_anomaly_detectors.py:94-110, 252-348``.
 

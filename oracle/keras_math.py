@@ -5,7 +5,7 @@ gordo autoencoder hot path.  Only ``tests/``, ``__graft_entry__.smoke()`` and
 product package (``gordo_components_b200``) never does and has no CPU fallback.
 
 PARITY STATUS: **parity unpinned at the TF/Keras boundary.**  The arithmetic restated
-here lives in third-party packages that are not vendored under ``/root/reference`` and
+here lives in third-party packages that are not vendored in the reference project and
 are not installable in this image: tensorflow==2.16.2, keras==3.3.3, scikeras==0.13.0
 (reference ``requirements/full_requirements.txt:449,201,406``).  No reference test pins
 a numerical output of Keras ``fit``/``predict`` (SURVEY.md section 8c), so this file

@@ -1,8 +1,8 @@
 """
 TEST INFRASTRUCTURE ONLY -- never imported by the product package.
 
-Loads the parts of the *unmodified* reference that can execute in this container
-straight from ``/root/reference`` (read-only), so that golden vectors under
+Loads the parts of the *unmodified* reference that can execute without its heavy dependencies
+straight from a checkout of equinor/gordo-components named by ``GORDO_REFERENCE_ROOT`` (read-only), so that golden vectors under
 ``tests/golden/`` are produced by the reference's own code, not by our restatement:
 
 * ``gordo/machine/model/anomaly/diff.py``  (DiffBasedAnomalyDetector, KFCV variant)
@@ -11,8 +11,8 @@ straight from ``/root/reference`` (read-only), so that golden vectors under
 
 TensorFlow / Keras / scikeras / xarray / gordo_core are not installed here, so the
 modules they would provide are replaced by inert stubs *before* import; none of the
-stubbed symbols take part in the anomaly arithmetic.  ``/root/reference`` does not
-exist on the GPU box: everything that runs there uses the committed fixtures instead.
+stubbed symbols take part in the anomaly arithmetic.  Only tests/golden/make_golden.py loads
+the reference; the test suite reads the fixtures it stored.
 
 Nothing is copied: the reference files are executed where they lie.
 """
@@ -25,11 +25,12 @@ import os
 import sys
 import types
 
-REFERENCE_ROOT = os.environ.get("GORDO_REFERENCE_ROOT", "/root/reference")
+REFERENCE_ROOT = os.environ.get("GORDO_REFERENCE_ROOT", "")
 
 
 def reference_available() -> bool:
-    return os.path.isfile(
+    """True when GORDO_REFERENCE_ROOT names a reference checkout (never a path relative to the working directory)."""
+    return bool(REFERENCE_ROOT) and os.path.isfile(
         os.path.join(REFERENCE_ROOT, "gordo", "machine", "model", "anomaly", "diff.py")
     )
 
@@ -145,7 +146,7 @@ def load_reference():
         return types.SimpleNamespace(**_loaded)
     if not reference_available():
         raise FileNotFoundError(
-            f"reference tree not found under {REFERENCE_ROOT}; use tests/golden fixtures"
+            f"no reference checkout at GORDO_REFERENCE_ROOT={REFERENCE_ROOT!r}; set it to a gordo-components checkout (the tests use tests/golden fixtures)"
         )
     _install_stubs()
     _install_pandas_append_shim()
@@ -238,7 +239,7 @@ class _Record:
 
 def load_reference_callers():
     """
-    The reference's own code either side of the hot path, executed from /root/reference for the golden fixtures of
+    The reference's own code either side of the hot path, executed from the reference checkout for the golden fixtures of
     tests/golden/make_golden.py (callers_* files):
 
     * ``gordo/serializer/{from_definition,into_definition,serializer,utils}.py`` -> ``from_definition, into_definition, dump, load ...``

@@ -1,9 +1,9 @@
 """
 Regenerates the golden fixtures in this directory by running the **reference's own code**
-(unmodified, from /root/reference, via oracle/reference_loader.py).  Run in the build
-container only -- /root/reference does not exist on the GPU box:
+(unmodified, from a checkout of equinor/gordo-components named by GORDO_REFERENCE_ROOT, via
+oracle/reference_loader.py).  The tests read only the stored fixtures:
 
-    python tests/golden/make_golden.py
+    GORDO_REFERENCE_ROOT=<gordo-components checkout> python tests/golden/make_golden.py
 
 Fixtures written:
   hourglass_dims.json        reference hourglass_calc_dims over a grid + the reference test table
@@ -11,6 +11,8 @@ Fixtures written:
                              block of DiffBasedAnomalyDetector.anomaly() from the reference
   ffnet_anomaly.npz          the same, with the base estimator being a fixed-weight hourglass
                              net (oracle/keras_math.ff_forward): pins net -> anomaly end to end
+  live_detector_<seed>.npz   a reference DiffBasedAnomalyDetector (LinearRegression base, sma smoothing) after
+                             cross_validate + fit: X, y, its predictions, thresholds and every anomaly() column block
 """
 from __future__ import annotations
 
@@ -301,6 +303,24 @@ def callers_fixture():
     print("callers ok:", len(out["expansions"]), "expansions;", {k: len(v["build_metadata"]["model"]["cross_validation"]["scores"]) for k, v in out["build"].items()})
 
 
+def live_detector_fixture(seed):
+    rng = np.random.default_rng(seed)
+    X = pd.DataFrame(rng.random((240, 5)))
+    y = pd.DataFrame(rng.random((240, 5)) * 3.0)
+    det = ref.DiffBasedAnomalyDetector(base_estimator=MultiOutputRegressor(LinearRegression()), scaler=MinMaxScaler(), window=10, smoothing_method="sma")
+    det.cross_validate(X=X, y=y)
+    det.fit(X, y)
+    frame = det.anomaly(X, y)
+    pred = det.predict(X)
+    np.testing.assert_array_equal(frame["model-output"].values, pred)
+    save = {"pred": pred, "feature_thresholds": det.feature_thresholds_.values,  # X and y are regenerated from the seed
+            "aggregate_threshold": np.float64(det.aggregate_threshold_), "hourglass_0.5_3_64": np.asarray(ref.hourglass_calc_dims(0.5, 3, 64))}
+    for k in dict.fromkeys(frame.columns.get_level_values(0)):
+        if k not in ("start", "end", "model-input", "model-output"):
+            save["frame/" + k] = frame[k].values.astype(np.float64)
+    np.savez_compressed(os.path.join(HERE, f"live_detector_{seed}.npz"), **save)
+
+
 if __name__ == "__main__":
     dims_fixture()
     kfcv_fixture("kfcv_smm", 300, 3, 12, "smm", 0.99, seed=6)
@@ -312,3 +332,5 @@ if __name__ == "__main__":
     anomaly_fixture("ffnet_anomaly", 400, 8, None, None, True, base="net", seed=4)
     anomaly_fixture("ffnet_anomaly_t64", 200, 64, None, None, True, base="net", seed=5)
     callers_fixture()
+    live_detector_fixture(11)
+    live_detector_fixture(12)

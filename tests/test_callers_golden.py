@@ -1,6 +1,6 @@
 """
 The path's callers against the reference's own code (no GPU needed): tests/golden/callers.{json,npz} were produced by
-tests/golden/make_golden.py running /root/reference's serializer, ModelBuilder._build, server wire helpers and InfImputer
+tests/golden/make_golden.py running the reference's serializer, ModelBuilder._build, server wire helpers and InfImputer
 (through oracle/reference_loader.load_reference_callers); here the same inputs go through this package.
 """
 import json

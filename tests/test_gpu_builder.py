@@ -19,7 +19,7 @@ def torch():
     import torch as t
 
     if not t.cuda.is_available():
-        pytest.skip("needs a B200")
+        pytest.skip("needs an H100")
     import __graft_entry__ as ge
 
     ge.build()
@@ -182,16 +182,37 @@ def test_fleet_model_builder_end_to_end(engine, torch, tmp_path):
     assert set(m["metadata"]["build_metadata"]["model"]) == {"cross_validation"} and m["metadata"]["build_metadata"]["model"]["cross_validation"]["scores"]
 
 
+def frame(rows=160, tags=4, seed=5):
+    """The data of the tests/golden/dropin.json build."""
+    rng = np.random.default_rng(seed)
+    t = np.linspace(0, 12, rows)[:, None]
+    values = (0.5 + 0.4 * np.sin(t * rng.uniform(0.5, 2, tags) + rng.uniform(0, 3, tags)) + rng.normal(0, 0.03, (rows, tags))) * rng.uniform(1, 30, tags)
+    return pd.DataFrame(values, index=pd.date_range("2020-03-01", periods=rows, freq="10min", tz="UTC"), columns=[f"TAG {i}" for i in range(tags)])
+
+
+def key_tree(obj):
+    """Nested keys with leaf *types* -- what a consumer of metadata.json can rely on."""
+    if isinstance(obj, dict):
+        return {str(k): key_tree(v) for k, v in sorted(obj.items(), key=lambda kv: str(kv[0]))}
+    if isinstance(obj, (list, tuple)):
+        return [f"list[{len(obj)}]", key_tree(obj[0]) if obj else None]
+    if isinstance(obj, (bool, np.bool_)):
+        return "bool"
+    if isinstance(obj, (int, np.integer)):
+        return "int"
+    if isinstance(obj, (float, np.floating)):
+        return "float"
+    return type(obj).__name__
+
+
 def test_dropin_definition_on_the_gpu(engine, torch):
     """
-    tests/test_reference_dropin.py runs the INTEGRATION.md definition through the REFERENCE'S from_definition / ModelBuilder._build /
-    serializer.dumps+loads (possible only where /root/reference exists, with the kernels mocked by the oracle) and commits the metadata
-    key tree and the anomaly frame's columns it produced (tests/golden/dropin.json).  Here the same definition and data run on the
-    real kernels -- per machine (`ModelBuilder`) and through the batched fleet path -- and must produce the same tree and columns.
+    tests/golden/dropin.json holds the metadata key tree and the anomaly frame's columns that the INTEGRATION.md definition produced
+    when the REFERENCE'S from_definition / ModelBuilder._build / serializer.dumps+loads drove this package's classes (kernels mocked
+    by the oracle).  Here the same definition and data run on the real kernels -- per machine (`ModelBuilder`) and through the
+    batched fleet path -- and must produce the same tree and columns.
     """
     import pickle
-
-    from test_reference_dropin import frame, key_tree
 
     from gordo_components_b200 import builder
 

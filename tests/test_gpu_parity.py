@@ -25,7 +25,7 @@ def torch():
     import torch as t
 
     if not t.cuda.is_available():
-        pytest.skip("needs a B200")
+        pytest.skip("needs an H100")
     import __graft_entry__ as ge
 
     ge.build()
@@ -39,7 +39,7 @@ def engine(torch):
     return e
 
 
-FLOOR = 2e-5  # absolute part of the tolerance, in units of the data magnitude: the tcgen05 split-precision path measures ~2e-6
+FLOOR = 2e-5  # absolute part of the tolerance, in units of the data magnitude: the tensor-core split-precision path measures ~2e-6
 
 
 def close(got, want, mag=1.0, rtol=RTOL, name="", atol=0.0, floor=FLOOR):
@@ -72,7 +72,7 @@ def run_infer(engine, torch, spec, weights_per_slot, X, y, jobs_h, scale=None, f
 # ------------------------------------------------------------------------------------------------ K1 + K4
 @pytest.mark.parametrize("T,variant", [(4, 1), (8, 1), (10, 1), (64, 1), (64, 2), (128, 1), (4, 3), (8, 3), (10, 3), (16, 3), (8, 0), (48, 2), (36, 2), (24, 2), (60, 0)])  # 3: row-per-thread kernel; 2 with T < 64: zero-padded columns
 def test_ffae_infer_score_matches_oracle(engine, torch, T, variant):
-    """variant 1 = fp32 CUDA-core kernel (any architecture), variant 2 = tcgen05 split-precision kernel (64-tag nets)."""
+    """variant 1 = fp32 CUDA-core kernel (any architecture), variant 2 = tensor-core (wgmma) split-precision kernel (64-tag nets)."""
     from oracle import anomaly_math as am
     from oracle import keras_math as km
 
@@ -161,7 +161,7 @@ def test_every_registered_factory_with_its_defaults(engine, torch, cls_name, kin
 
 
 def test_tc_work_split_many_ragged_jobs(engine, torch):
-    """More jobs than SMs with ragged lengths (whole-job waves + a split tail, empty tiles, jobs shorter than a tile): the tcgen05
+    """More jobs than SMs with ragged lengths (whole-job waves + a split tail, empty tiles, jobs shorter than a tile): the tensor-core
     kernel against the generic fp32 kernel (itself checked against the oracle above) on every output."""
     from gordo_components_b200 import fleet
     from oracle import keras_math as km
@@ -187,7 +187,7 @@ def test_tc_work_split_many_ragged_jobs(engine, torch):
     a = eng.infer_score(params, jobs, M, int(n_rows.max()), x, y, scale, feat, agg, variant=2)
     b = eng.infer_score(params, jobs, M, int(n_rows.max()), x, y, scale, feat, agg, variant=1)
     for k in b:
-        close(a[k].cpu().numpy(), b[k].cpu().numpy(), mag=float(b[k].abs().max()), name=f"tcgen05 vs fp32: {k}")
+        close(a[k].cpu().numpy(), b[k].cpu().numpy(), mag=float(b[k].abs().max()), name=f"tensor cores vs fp32: {k}")
 
 
 def test_more_jobs_than_a_grid_dimension(engine, torch):
@@ -539,7 +539,7 @@ def test_lstm_infer_matches_oracle(engine, torch, F, units, lookback):
                                                           (7, [128], 9, [400], 1000.0), (5, [7, 9, 3], 4, [50, 133], 1.0),
                                                           (128, [107, 85, 64, 64, 85, 107], 12, [150], 1.0),  # widths padded to 64 internally
                                                           (128, [256, 128, 64, 64, 128, 256], 144, [144 + 39, 144 + 130], 1.0),  # BASELINE configs[3]: error growth over 144 steps
-                                                          (4, [64, 64], 3, [19100, 18950], 1.0)])  # 149 + 148 tiles: every CTA pair walks several items (ring, accumulators, bias buffers wrap)
+                                                          (4, [64, 64], 3, [19100, 18950], 1.0)])  # 150 + 149 tiles on 132 SMs: every CTA walks several items (the TMA ring wraps across items)
 def test_lstm_infer_tcgen05_matches_oracle(engine, torch, F, units, lookback, rows, scale):
     """gb_lstm_infer_tc: FP16-pair split operands on the tensor cores, state in HBM, one launch per (layer, timestep).
     Jobs of different lengths (tiles with padding rows), machines sharing the launch, raw inputs of large magnitude (the
@@ -566,7 +566,7 @@ def test_lstm_infer_tcgen05_matches_oracle(engine, torch, F, units, lookback, ro
     got_fma = eng.infer(params, jobs, M, max(nwin), x, sum(nwin), variant=1).cpu().numpy()
     for m in range(M):
         want = km.lstm_predict(spec, ws[m], Xs[m], dtype=np.float64)
-        close(got_tc[outs[m]:outs[m] + nwin[m]], want, 1.0, name="tcgen05 lstm output")
+        close(got_tc[outs[m]:outs[m] + nwin[m]], want, 1.0, name="tensor-core lstm output")
         close(got_fma[outs[m]:outs[m] + nwin[m]], want, 1.0, name="fp32 lstm output")
 
 
@@ -886,7 +886,7 @@ def test_kfcv_detector_thresholds(engine, torch, n_rows, window, method, q):
 @pytest.mark.parametrize("case", ["kfcv_smm", "kfcv_ewma"])
 def test_kfcv_detector_against_reference_generated_fixture(engine, torch, case):
     """Thresholds and frame columns of the reference's own DiffBasedKFCVAnomalyDetector (tests/golden/make_golden.py ran it
-    from /root/reference with a LinearRegression base estimator) against ours with the same base estimator."""
+    from the reference with a LinearRegression base estimator) against ours with the same base estimator."""
     from sklearn.linear_model import LinearRegression
     from sklearn.multioutput import MultiOutputRegressor
     from sklearn.preprocessing import MinMaxScaler
@@ -949,7 +949,7 @@ def test_error_paths_raise_like_the_reference(engine, torch):
         eng.fit(params, jobs, 1, 18, x, x, epochs=1, batch_size=64)
     with pytest.raises(ValueError):  # pandas: "percentiles should all be in the interval [0, 1]"
         engine.quantile(engine.jobs_to_device(engine.make_jobs([0], [10], [0]), dev), 1, 10, torch.zeros((10, 1), device=dev), 1.5)
-    # fused kernel: the tcgen05 variant refuses architectures it does not cover
+    # fused kernel: the tensor-core variant refuses architectures it does not cover
     ff = km.ff_hourglass_spec(10)
     e2 = engine.FFEngine(ff.dims, ff.acts, ff.l1)
     p2 = e2.pack_params([km.init_ff_weights(ff, np.random.default_rng(0))])

@@ -19,7 +19,7 @@ def torch():
     import torch as t
 
     if not t.cuda.is_available():
-        pytest.skip("needs a B200")
+        pytest.skip("needs an H100")
     import __graft_entry__ as ge
 
     ge.build()
