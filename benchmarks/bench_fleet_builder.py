@@ -6,11 +6,24 @@ one at a time, gordo/builder/build_model.py:192-339 on the GPU estimators).  Wal
 number a `gordo build` user sees.
 
     python benchmarks/bench_fleet_builder.py [--machines 125] [--rows 10000] [--tags 64] [--epochs 10] [--scaled] [--single 3]
+    python benchmarks/bench_fleet_builder.py --lstm [--lookback 24] --machines 16 --rows 2000 --tags 16 --epochs 1 --single 16
 
-Not measured on the H100; the code paths it times are covered by tests/test_gpu_builder.py.
+``--lstm`` builds DiffBasedAnomalyDetector(KerasLSTMAutoEncoder(lstm_hourglass)) machines instead (batched by
+fleet.build_lstm_fleet).  Measured numbers and the card they were measured on are in DESIGN.md §7.
 """
 import argparse, json, os, sys, tempfile, time
 sys.path.insert(0, os.path.abspath(os.path.join(os.path.dirname(__file__), "..")))
+
+
+def _power_limit():
+    """The card's power limit in watts, read-only query (None when nvidia-smi is not available)."""
+    import subprocess
+
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader,nounits", "-i", "0"], capture_output=True, text=True, timeout=30)
+        return float(out.stdout.strip().splitlines()[0])
+    except Exception:
+        return None
 
 
 def main():
@@ -21,6 +34,8 @@ def main():
     ap.add_argument("--epochs", type=int, default=10)
     ap.add_argument("--scaled", action="store_true", help="Pipeline([MinMaxScaler, AE]) as in gordo's example config")
     ap.add_argument("--single", type=int, default=3, help="machines to also build one at a time for comparison")
+    ap.add_argument("--lstm", action="store_true", help="LSTM autoencoder machines (lstm_hourglass) instead of the feed-forward hourglass")
+    ap.add_argument("--lookback", type=int, default=24, help="lookback_window of the LSTM machines")
     a = ap.parse_args()
     import numpy as np
     import pandas as pd
@@ -29,7 +44,10 @@ def main():
     ge.build()
     from gordo_components_b200 import builder
 
-    ae = {"gordo.machine.model.models.KerasAutoEncoder": {"kind": "feedforward_hourglass", "epochs": a.epochs}}
+    if a.lstm:
+        ae = {"gordo.machine.model.models.KerasLSTMAutoEncoder": {"kind": "lstm_hourglass", "lookback_window": a.lookback, "epochs": a.epochs}}
+    else:
+        ae = {"gordo.machine.model.models.KerasAutoEncoder": {"kind": "feedforward_hourglass", "epochs": a.epochs}}
     base = {"sklearn.pipeline.Pipeline": {"steps": ["sklearn.preprocessing.MinMaxScaler", ae]}} if a.scaled else ae
     model = {"gordo.machine.model.anomaly.diff.DiffBasedAnomalyDetector": {"base_estimator": base}}
     rng = np.random.default_rng(0)
@@ -57,8 +75,10 @@ def main():
         torch.cuda.synchronize()
         single_s = (time.perf_counter() - t0) / a.single
     scores = results[0][1]["metadata"]["build_metadata"]["model"]["cross_validation"]["scores"]
+    net = f"LSTM hourglass (lookback {a.lookback})" if a.lstm else "hourglass"
     print(json.dumps({
-        "workload": f"{a.machines} machines x {a.tags}-tag hourglass{' behind MinMaxScaler' if a.scaled else ''}, {a.rows} rows, {a.epochs} epochs: "
+        "gpu": torch.cuda.get_device_name(0), "power_limit_w": _power_limit(),
+        "workload": f"{a.machines} machines x {a.tags}-tag {net}{' behind MinMaxScaler' if a.scaled else ''}, {a.rows} rows, {a.epochs} epochs: "
                     "definition -> 3-fold CV + fit + thresholds + scores metadata -> model.pkl/metadata.json",
         "fleet_builder_s": fleet_s, "machines_per_s": a.machines / fleet_s, "bytes_written": size,
         "model_builder_s_per_machine": single_s, "speedup_per_machine": None if single_s is None else single_s / (fleet_s / a.machines),

@@ -24,6 +24,7 @@ EXPORTS = (
     "gb_abi_version", "gb_last_error", "gb_device_check", "gb_ffnet_param_count", "gb_ffnet_param_stride",
     "gb_ffae_infer_score", "gb_ffae_tc_supported", "gb_anomaly_score", "gb_anomaly_score_f64", "gb_minmax_fit", "gb_minmax_f64", "gb_thresholds", "gb_thresholds_f64", "gb_cv_moments", "gb_smooth", "gb_quantile", "gb_affine_f64", "gb_ffae_fit_state_stride", "gb_ffae_fit",
     "gb_lstm_param_count", "gb_lstm_param_stride", "gb_lstm_workspace_bytes", "gb_lstm_infer", "gb_lstm_tc_supported", "gb_lstm_tc_workspace_bytes", "gb_lstm_infer_tc", "gb_lstm_fit_workspace_bytes", "gb_lstm_fit",
+    "gb_orthonormal_rows",
 )
 
 
@@ -112,6 +113,8 @@ def _declare(lib):
     lib.gb_lstm_fit_workspace_bytes.argtypes = [C.POINTER(GbLstmNet), C.c_int32]
     lib.gb_lstm_fit.argtypes = [C.POINTER(GbLstmNet), _P, _P, _P, _P, _P, C.c_int32, C.c_int32, _P, _P, C.POINTER(GbLstmFitHParams), _P, _P, _P, _P]
     lib.gb_lstm_fit.restype = C.c_int
+    lib.gb_orthonormal_rows.argtypes = [_P, C.c_int32, C.c_int32, C.c_int32, _P, C.c_int64, C.c_int64, _P]
+    lib.gb_orthonormal_rows.restype = C.c_int
     for name in ("gb_device_check", "gb_ffae_infer_score", "gb_ffae_tc_supported", "gb_anomaly_score", "gb_minmax_fit", "gb_thresholds", "gb_smooth", "gb_ffae_fit", "gb_lstm_infer"):
         getattr(lib, name).restype = C.c_int
 

@@ -7,10 +7,13 @@ definition -> cross validation with the evaluation metrics -> final fit -> offse
 ``FleetModelBuilder`` is where the batched kernels pay off: machines whose definition is the canonical
 ``DiffBasedAnomalyDetector(base_estimator=KerasAutoEncoder(<feed-forward kind>), scaler=MinMaxScaler())`` -- the network bare or
 behind one ``MinMaxScaler`` in a Pipeline, as in gordo's example configs -- are bucketed by architecture and training length, and every bucket is built by ``fleet.build_fleet`` -- all final fits and all CV folds
-in one ``gb_ffae_fit`` launch, fold scoring / thresholds / scaler statistics / metric moments one launch each.  The
+in one ``gb_ffae_fit`` launch, fold scoring / thresholds / scaler statistics / metric moments one launch each.  The LSTM form
+of the same definition (``KerasLSTMAutoEncoder`` / ``KerasLSTMForecast``, ``_canonical_lstm``) is bucketed by architecture,
+lookback, lookahead and training length and built by ``fleet.build_lstm_fleet``: all fits as jobs of ``gb_lstm_fit`` (in
+chunks that fit a workspace budget), every fold model's test block in one LSTM inference launch, float64 scoring.  The
 cross-validation ``scores`` block of the metadata is then assembled on the host from ``gb_cv_moments``' five sums per
-(fold, tag).  Any other definition (other transformers in a Pipeline, LSTM models, K-fold detectors, custom metrics ...) goes
-through ``ModelBuilder``: one machine at a time, still on the GPU through the estimators' own fit / predict.
+(fold, tag).  Any other definition (other transformers in a Pipeline, LSTM fits with callbacks, K-fold detectors, custom
+metrics ...) goes through ``ModelBuilder``: one machine at a time, still on the GPU through the estimators' own fit / predict.
 
 Machines are plain dicts in the layout of ``Machine.to_dict()`` (gordo/machine/machine.py:226-246): ``name``, ``model`` (a
 definition), ``dataset``, and optionally ``project_name``, ``evaluation``, ``metadata``, ``runtime``.  ``dataset`` is
@@ -383,6 +386,95 @@ def _canonical(index, machine) -> Optional[_Canonical]:
     return _Canonical(index, machine, model, spec, X, y, dataset_meta, query_sec, fit, split_obj.n_splits, evaluation, input_scaler)
 
 
+class _CanonicalLSTM(_Canonical):
+    """A machine whose LSTM detector can take the batched path (``fleet.build_lstm_fleet``)."""
+
+    def __init__(self, *args, lookahead: int):
+        super().__init__(*args)
+        self.lookahead = lookahead
+
+    def bucket(self):
+        s = self.spec
+        return (s.key(), tuple(sorted(s.adam.items())), tuple(s.metrics), self.lookahead, len(self.X), self.fit["epochs"], self.fit["batch_size"],
+                self.n_splits, int(self.evaluation.get("seed", 0)), self.input_scaler)
+
+
+def _is_lstm_definition(machine) -> bool:
+    """True when the machine's model is a DiffBasedAnomalyDetector around an LSTM estimator (bare or last Pipeline step)."""
+    from .machine.model.anomaly.diff import DiffBasedAnomalyDetector
+    from .machine.model.models import KerasLSTMBaseEstimator
+
+    try:
+        model = serializer.from_definition(machine["model"])
+    except Exception:  # ModelBuilder raises the definition's own error
+        return False
+    est = getattr(model, "base_estimator", None) if isinstance(model, DiffBasedAnomalyDetector) else None
+    if isinstance(est, Pipeline) and est.steps:
+        est = est.steps[-1][1]
+    return isinstance(est, KerasLSTMBaseEstimator)
+
+
+def _canonical_lstm(index, machine) -> Optional[_CanonicalLSTM]:
+    """
+    The LSTM form of the canonical definition -- ``DiffBasedAnomalyDetector(KerasLSTMAutoEncoder | KerasLSTMForecast)``, the network bare
+    or behind one default ``MinMaxScaler``, under the evaluation ``_canonical`` accepts -- as a candidate for the batched path, or
+    ``None`` with the reason logged.  Machines too short for the CV folds go to ``ModelBuilder``, which raises the reference's errors.
+    """
+    from .machine.model.anomaly.diff import DiffBasedAnomalyDetector
+    from .machine.model.factories.specs import LSTMNetSpec
+    from .machine.model.models import KerasLSTMAutoEncoder, KerasLSTMForecast
+
+    def no(reason):
+        logger.info("machine %s takes the per-machine path: %s", machine["name"], reason)
+        return None
+
+    evaluation = {**DEFAULT_EVALUATION, **(machine.get("evaluation") or {})}
+    if str(evaluation["cv_mode"]).lower() != "full_build":
+        return no(f"cv_mode {evaluation['cv_mode']}")
+    if any(m.rpartition(".")[2] not in MOMENT_METRICS or ("." in m and not m.startswith("sklearn.metrics.")) for m in evaluation["metrics"]):
+        return no("evaluation metrics beyond the four moment metrics")
+    scoring = evaluation.get("scoring_scaler")
+    if scoring:
+        scoring = serializer.from_definition(scoring) if isinstance(scoring, (str, dict)) else scoring
+        if not _default_minmax(scoring):
+            return no("scoring_scaler is not a default MinMaxScaler")
+    split_obj = serializer.from_definition(evaluation.get("cv", DEFAULT_CV))
+    if type(split_obj) is not TimeSeriesSplit or split_obj.max_train_size is not None or split_obj.test_size is not None or split_obj.gap:
+        return no("cv is not a plain TimeSeriesSplit")
+
+    model = serializer.from_definition(machine["model"])
+    if type(model) is not DiffBasedAnomalyDetector or model.window is not None or model.shuffle:
+        return no("model is not a plain DiffBasedAnomalyDetector")
+    if not _default_minmax(model.scaler):
+        return no("detector scaler is not a default MinMaxScaler")
+    est, input_scaler = model.base_estimator, False
+    if type(est) is Pipeline and len(est.steps) == 2 and _default_minmax(est.steps[0][1]):
+        est, input_scaler = est.steps[1][1], True
+    if type(est) not in (KerasLSTMAutoEncoder, KerasLSTMForecast):
+        return no("base_estimator is not a KerasLSTMAutoEncoder / KerasLSTMForecast, bare or behind one default MinMaxScaler")
+    fit_args = est.extract_supported_fit_args(est.kwargs)
+    if fit_args.get("validation_split") or fit_args.get("callbacks"):
+        return no("validation_split / callbacks need the per-epoch loop")
+    batch_size = int(est.batch_size)
+    if not 1 <= batch_size <= 32:
+        return no(f"batch_size {batch_size}: the batched LSTM fit takes at most 32 windows per batch")
+
+    t0 = time.time()
+    X, y, dataset_meta = _get_data(machine["dataset"])
+    query_sec = time.time() - t0
+    est.kwargs.update({"n_features": X.shape[1], "n_features_out": y.shape[1]})
+    spec = est._build_spec()
+    if not isinstance(spec, LSTMNetSpec):
+        return no("not an LSTM network")
+    L, la, K = int(est.lookback_window), int(est.lookahead), split_obj.n_splits
+    test = len(X) // (K + 1)
+    first_train = len(X) - K * test
+    if len(X) != len(y) or test <= L + la or first_train <= L or first_train - L + 1 - la < 1:
+        return no("too few rows for the CV folds at this lookback_window")
+    fit = {"epochs": int(fit_args.get("epochs", 1)), "batch_size": batch_size, "shuffle": False}
+    return _CanonicalLSTM(index, machine, model, spec, X, y, dataset_meta, query_sec, fit, K, evaluation, input_scaler, lookahead=la)
+
+
 class FleetModelBuilder:
     """
     Build every machine of a project: ``FleetModelBuilder(machines).build(output_dir)`` -> ``[(model, machine_dict), ...]`` in
@@ -409,7 +501,7 @@ class FleetModelBuilder:
         results: List[Optional[Tuple[Any, dict]]] = [None] * len(self.machines)
         buckets: Dict[tuple, List[_Canonical]] = {}
         for i, machine in enumerate(self.machines):
-            c = _canonical(i, machine)
+            c = _canonical_lstm(i, machine) if _is_lstm_definition(machine) else _canonical(i, machine)
             if c is None:
                 results[i] = ModelBuilder(machine).build()
             else:
@@ -429,6 +521,8 @@ class FleetModelBuilder:
 
     @staticmethod
     def _build_bucket(members: List[_Canonical]) -> List[Tuple[Any, dict]]:
+        if isinstance(members[0], _CanonicalLSTM):
+            return FleetModelBuilder._build_lstm_bucket(members)
         from . import engine, fleet
 
         first = members[0]
@@ -465,6 +559,42 @@ class FleetModelBuilder:
             }
             dataset_block = {"query_duration_sec": c.query_sec, "dataset_meta": c.dataset_meta}
             out.append((model, _machine_out(c.machine, {"model": model_block, "dataset": dataset_block})))
+        return out
+
+    @staticmethod
+    def _build_lstm_bucket(members: List[_CanonicalLSTM]) -> List[Tuple[Any, dict]]:
+        from . import engine, fleet
+
+        first = members[0]
+        eng = engine.lstm_engine_for(first.spec)
+        rows, K = len(first.X), first.n_splits
+        t0 = time.time()
+        xd = engine._torch().from_numpy(np.concatenate([np.ascontiguousarray(c.X.values, dtype=np.float64) for c in members])).to(eng.device)
+        same_y = all(c.y is c.X for c in members)
+        yd = xd if same_y else engine._torch().from_numpy(np.concatenate([np.ascontiguousarray(c.y.values, dtype=np.float64) for c in members])).to(eng.device)
+        fb = fleet.build_lstm_fleet(eng, xd, yd, rows, lookahead=first.lookahead, epochs=first.fit["epochs"], batch_size=first.fit["batch_size"],
+                                    n_splits=K, seed=int(first.evaluation.get("seed", 0)), adam=first.spec.adam, input_scaler=first.input_scaler)
+        engine._torch().cuda.synchronize()
+        share = (time.time() - t0) / len(members)  # the bucket's wall time, spread evenly: there is no per-machine time any more
+        split_obj = TimeSeriesSplit(n_splits=K)
+        out = []
+        for m, c in enumerate(members):
+            tags = list(c.y.columns)
+            model = fb.detector(m, tags=tags, template=c.model, input_tags=list(c.X.columns))
+            names = [s.rpartition(".")[2] for s in c.evaluation["metrics"]]
+            scoring_scale = model.scaler.scale_ if c.evaluation.get("scoring_scaler") else None  # the scoring scaler sees all targets too
+            scores = scores_block(scores_from_moments(fb.cv_moments[m], fb.n_test, scoring_scale, names), tags)
+            model_block = {
+                "model_offset": eng.lookback - 1 + c.lookahead,  # the first prediction answers row lookback_window - 1 + lookahead
+                "model_creation_date": _now(),
+                "model_builder_version": __version__,
+                "model_training_duration_sec": share * 1.0 / (K + 1),
+                "cross_validation": {"scores": scores, "cv_duration_sec": share * K / (K + 1), "splits": build_split_dict(c.X, split_obj)},
+                "model_meta": extract_metadata_from_model(model),
+            }
+            dataset_block = {"query_duration_sec": c.query_sec, "dataset_meta": c.dataset_meta}
+            out.append((model, _machine_out(c.machine, {"model": model_block, "dataset": dataset_block})))
+        logger.info("built %d LSTM machines in one batched bucket", len(members))
         return out
 
 

@@ -376,6 +376,43 @@ __global__ void lstm_epoch_kernel(const gb_job* jobs, int n_jobs, float* loss_su
   hit_sum[j] = 0.f;
 }
 
+// ---------------------------------------------------------------------------------------------- orthogonal initialiser
+// Keras' Orthogonal for a recurrent kernel [u, 4u] [3P]: QR of a [4u, u] standard-normal draw, Q's columns sign-corrected so that
+// diag(R) > 0, transposed.  That Q is what Gram-Schmidt gives, so: one CTA per matrix orthonormalises the rows of its own
+// [rows, cols] normal draw `g` in place (float64, modified Gram-Schmidt) and writes them rounded to float32.
+__global__ void __launch_bounds__(256) orthonormal_rows_kernel(double* g, int rows, int cols, float* out, long out_stride) {
+  __shared__ double s_red[8];
+  double* a = g + (long)blockIdx.x * rows * cols;
+  float* o = out + (long)blockIdx.x * out_stride;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int i = 0; i < rows; ++i) {
+    double* ri = a + (long)i * cols;
+    double s = 0.;
+    for (int c = threadIdx.x; c < cols; c += 256) s += ri[c] * ri[c];
+    for (int k = 16; k > 0; k >>= 1) s += __shfl_xor_sync(0xffffffffu, s, k);
+    if (lane == 0) s_red[warp] = s;
+    __syncthreads();
+    double norm2 = 0.;
+#pragma unroll
+    for (int w = 0; w < 8; ++w) norm2 += s_red[w];
+    const double inv = 1. / sqrt(norm2);
+    for (int c = threadIdx.x; c < cols; c += 256) {
+      const double v = ri[c] * inv;
+      ri[c] = v;
+      o[(long)i * cols + c] = (float)v;
+    }
+    __syncthreads();
+    for (int j = i + 1 + warp; j < rows; j += 8) {  // take row i out of every later row: one warp per row
+      double* rj = a + (long)j * cols;
+      double d = 0.;
+      for (int c = lane; c < cols; c += 32) d += rj[c] * ri[c];
+      for (int k = 16; k > 0; k >>= 1) d += __shfl_xor_sync(0xffffffffu, d, k);
+      for (int c = lane; c < cols; c += 32) rj[c] -= d * ri[c];
+    }
+    __syncthreads();
+  }
+}
+
 int validate(const gb_lstmnet* net) {
   GB_REQUIRE(net != nullptr, GB_E_ARG, "net is NULL");
   GB_REQUIRE(net->n_layers >= 1 && net->n_layers <= GB_MAX_LAYERS, GB_E_SHAPE, "n_layers=%d outside [1,%d]", net->n_layers, GB_MAX_LAYERS);
@@ -524,6 +561,17 @@ int gb_lstm_fit(const gb_lstmnet* net, float* params, float* adam_m, float* adam
     lstm_epoch_kernel<<<jb, 128, 0, st>>>(jobs, n_jobs, a.loss_sum, a.hit_sum, out_loss, out_acc, e, hp->epochs);
   }
   cudaGraphExecDestroy(gexec);  // the enqueued replays keep what they need
+  GB_CUDA_CHECK(cudaGetLastError());
+  return GB_OK;
+}
+
+int gb_orthonormal_rows(double* g, int32_t n_mats, int32_t rows, int32_t cols, float* out, int64_t out_offset, int64_t out_stride,
+                        void* stream) {
+  GB_REQUIRE(g && out, GB_E_ARG, "g/out must be non-NULL");
+  GB_REQUIRE(n_mats >= 0 && rows >= 1 && cols >= rows, GB_E_SHAPE, "rows=%d cols=%d: need 1 <= rows <= cols", rows, cols);
+  GB_REQUIRE(out_offset >= 0 && out_stride >= (int64_t)rows * cols, GB_E_ARG, "out_stride=%lld is shorter than one matrix", (long long)out_stride);
+  if (n_mats == 0) return GB_OK;
+  orthonormal_rows_kernel<<<n_mats, 256, 0, (cudaStream_t)stream>>>(g, rows, cols, out + out_offset, out_stride);
   GB_CUDA_CHECK(cudaGetLastError());
   return GB_OK;
 }

@@ -322,6 +322,21 @@ def affine_f64(jobs_dev, n_jobs, max_rows, x64, a, b, out_rows=None):
     return out
 
 
+def orthonormal_rows(g, out, out_offset: int, out_stride: int):
+    """
+    Keras' Orthogonal initialiser for every float64 standard-normal draw ``g`` [n, rows, cols] (overwritten): the rows
+    orthonormalised, written as float32 into the dense tensor ``out`` at element ``out_offset + i * out_stride`` for matrix i.
+    """
+    lib = _cabi.load_library()
+    n, rows, cols = (int(d) for d in g.shape)
+    if g.dtype != _torch().float64 or out.dtype != _torch().float32:
+        raise ValueError(f"orthonormal_rows takes float64 draws and a float32 output, got {g.dtype} / {out.dtype}")
+    if n and int(out_offset) + (n - 1) * int(out_stride) + rows * cols > out.numel():
+        raise ValueError("orthonormal_rows: the matrices do not fit into out")
+    p = _cabi.ptr
+    _cabi.check(lib.gb_orthonormal_rows(p(g), n, rows, cols, p(out), int(out_offset), int(out_stride), _stream_ptr()))
+
+
 SMOOTH_METHODS = {"smm": 0, "sma": 1, "ewma": 2}
 
 
@@ -371,6 +386,32 @@ class LSTMEngine:
             host[s, : vec.size] = vec
         return torch.from_numpy(host).to(self.device)
 
+    def initial_params(self, n_slots: int, generator, draw_bytes: int = 256 << 20):
+        """
+        Fresh networks on the device with Keras' LSTM initialisers, as ``KerasBaseEstimator._initial_weights`` draws them: kernels
+        glorot-uniform, recurrent kernels orthogonal (gb_orthonormal_rows on standard-normal draws, ``draw_bytes`` of them at a
+        time), biases zero except a forget-gate bias of 1.  Returns [n_slots, param_stride] float32.
+        """
+        torch = _torch()
+        params = torch.zeros((int(n_slots), self.param_stride), dtype=torch.float32, device=self.device)
+        ofs, i = 0, self.n_features
+        for u in self.units:
+            lim = math.sqrt(6.0 / (i + 4 * u))
+            params[:, ofs:ofs + i * 4 * u].uniform_(-lim, lim, generator=generator)
+            ofs += i * 4 * u
+            block = max(1, int(draw_bytes) // (u * 4 * u * 8))
+            for s0 in range(0, int(n_slots), block):
+                n = min(block, int(n_slots) - s0)
+                g = torch.randn((n, u, 4 * u), dtype=torch.float64, device=self.device, generator=generator)
+                orthonormal_rows(g, params, s0 * self.param_stride + ofs, self.param_stride)
+            ofs += u * 4 * u
+            params[:, ofs + u:ofs + 2 * u] = 1.0  # gate order i, f, c, o: unit_forget_bias
+            ofs += 4 * u
+            i = u
+        lim = math.sqrt(6.0 / (i + self.n_out))
+        params[:, ofs:ofs + i * self.n_out].uniform_(-lim, lim, generator=generator)
+        return params
+
     def unpack_params(self, params):
         """device [n_slots, stride] -> per slot ([(kernel, recurrent, bias) per layer], (Wd, bd)) as host arrays."""
         host = params.detach().cpu().numpy()
@@ -386,6 +427,10 @@ class LSTMEngine:
             Wd = vec[ofs:ofs + i * self.n_out].reshape(i, self.n_out).copy(); ofs += i * self.n_out
             out.append((layers, (Wd, vec[ofs:ofs + self.n_out].copy())))
         return out
+
+    def fit_workspace_bytes(self, n_jobs: int) -> int:
+        """Device scratch one ``fit`` launch of ``n_jobs`` jobs allocates (gb_lstm_fit_workspace_bytes)."""
+        return int(self.lib.gb_lstm_fit_workspace_bytes(C.byref(self.net), int(n_jobs)))
 
     def fit(self, params, jobs_dev, n_jobs, max_windows, x, y, epochs: int = 1, batch_size: int = 32, lookahead: int = 0,
             primer: bool = True, adam: Optional[Dict[str, float]] = None, state=None):

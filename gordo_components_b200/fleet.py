@@ -10,6 +10,7 @@ summaries -- there is no exchange step inside fit, predict or anomaly.
 """
 from __future__ import annotations
 
+import math
 import time
 from typing import Dict, List, Optional, Sequence
 
@@ -350,3 +351,214 @@ def build_fleet(eng: "engine.FFEngine", x, y, rows: int, epochs: int = 1, batch_
                       fold_in_scale=None if in_scale is None else in_scale[M:].view(K, M, -1).permute(1, 0, 2).contiguous(),
                       fold_in_offset=None if in_offset is None else in_offset[M:].view(K, M, -1).permute(1, 0, 2).contiguous(),
                       steps_per_epoch=(N + int(batch_size) - 1) // int(batch_size))
+
+
+# ------------------------------------------------------------------------------------------------ fleet build of LSTM detectors
+def _minmax_attributes(lo: np.ndarray, hi: np.ndarray):
+    """(scale_, min_) of a MinMaxScaler (feature_range (0, 1)) from float64 column extrema, with sklearn's own arithmetic."""
+    denom = hi - lo
+    denom[denom < 10 * np.finfo(np.float64).eps] = 1.0  # _handle_zeros_in_scale
+    scale = 1.0 / denom
+    return scale, 0.0 - lo * scale
+
+
+def _fill_minmax_from_extrema(sc, lo, hi, n_samples, names):
+    """Give a MinMaxScaler exactly the attributes sklearn's ``fit`` leaves for data with column extrema ``lo`` / ``hi``."""
+    sc.n_samples_seen_, sc.n_features_in_ = int(n_samples), len(lo)
+    sc.data_min_, sc.data_max_, sc.data_range_ = lo.copy(), hi.copy(), hi - lo
+    sc.scale_, sc.min_ = _minmax_attributes(lo, hi)
+    if names is not None and all(isinstance(n, str) for n in names):
+        sc.feature_names_in_ = np.asarray(names, dtype=object)
+    return sc
+
+
+class LSTMFleetBuild:
+    """
+    Result of ``build_lstm_fleet``: what ``ModelBuilder._build`` produces for one LSTM machine -- final weights, target scaler,
+    CV thresholds per fold and final, loss histories, CV metric moments -- for all machines of a bucket.  Slot layout of
+    ``init_params``: final models at [0, M), fold k of machine m at M + k*M + m.  Arrays named ``fold_*`` are [M, K, ...].
+    """
+
+    def __init__(self, eng, n_machines, n_splits, rows, lookahead, batch_size, starts, n_test, params, fold_params, init_params, loss, acc,
+                 fold_loss, fold_acc, y_min, y_max, fold_y_min, fold_y_max, feat_thr, agg_thr, fold_feat_thr, fold_agg_thr, cv_moments,
+                 fold_predictions, in_min=None, in_max=None, fold_in_min=None, fold_in_max=None):
+        self.eng, self.n_machines, self.n_splits, self.rows = eng, n_machines, n_splits, rows
+        self.lookahead, self.batch_size = lookahead, batch_size
+        self.steps_per_epoch = math.ceil((rows - eng.lookback + 1 - lookahead) / batch_size)  # of the final fit (History.params["steps"])
+        self.starts, self.n_test = starts, n_test            # first test row of every fold; predictions per test block
+        self.params, self.fold_params, self.init_params = params, fold_params, init_params  # device float32 ([S, stride] or None)
+        self.loss, self.acc, self.fold_loss, self.fold_acc = loss, acc, fold_loss, fold_acc   # [M, epochs], [M, K, epochs]
+        # float64 column extrema of the targets (final fit on all rows, fold k on its training prefix): the detector scalers
+        self.y_min, self.y_max, self.fold_y_min, self.fold_y_max = y_min, y_max, fold_y_min, fold_y_max
+        # the same for the MinMaxScaler in front of the network (None without one)
+        self.in_min, self.in_max, self.fold_in_min, self.fold_in_max = in_min, in_max, fold_in_min, fold_in_max
+        self.feat_thr, self.agg_thr = feat_thr, agg_thr                                # [M, T], [M] float64 (last fold)
+        self.fold_feat_thr, self.fold_agg_thr = fold_feat_thr, fold_agg_thr            # [M, K, T], [M, K] float64
+        self.cv_moments = cv_moments                                                   # [M, K, 5, T] float64
+        self.fold_predictions = fold_predictions                                       # [M, K, n_test, T] float32 (device)
+
+    def detector(self, m: int, tags=None, template=None, input_tags=None):
+        """
+        Machine ``m`` as a picklable ``DiffBasedAnomalyDetector`` around a ``KerasLSTMAutoEncoder`` / ``KerasLSTMForecast``, with the
+        attributes the per-machine build leaves.  ``template``: an unfitted detector from the machine's own definition, filled in
+        so that the estimator class, ``kind`` and the other constructor arguments survive.
+        """
+        import pandas as pd
+        from sklearn.pipeline import Pipeline
+        from sklearn.preprocessing import MinMaxScaler
+
+        from .machine.model.anomaly.diff import DiffBasedAnomalyDetector
+        from .machine.model.models import FittedNet, History, KerasLSTMAutoEncoder, KerasLSTMForecast
+
+        eng = self.eng
+        T, K = eng.n_out, self.n_splits
+        tags = list(tags) if tags is not None else list(range(T))
+        if template is not None:
+            det = template
+            est = det.base_estimator
+            lstm = est.steps[-1][1] if isinstance(est, Pipeline) else est
+            if isinstance(est, Pipeline) != (self.in_min is not None):
+                raise ValueError("the template's input scaler and the fleet's do not match")
+            if lstm.lookahead != self.lookahead:
+                raise ValueError("the template's lookahead differs from the fleet's")
+            lstm.kwargs.update({"n_features": eng.n_features, "n_features_out": T})
+            spec = lstm._build_spec()
+            if spec.key() != ("lstm", eng.n_features, tuple(eng.units), tuple(eng.acts), T, eng.out_func, eng.lookback):
+                raise ValueError("template architecture differs from the fleet's")
+            if isinstance(est, Pipeline):
+                _fill_minmax_from_extrema(est.steps[0][1], self.in_min[m], self.in_max[m], self.rows, input_tags)
+        else:
+            cls = KerasLSTMForecast if self.lookahead else KerasLSTMAutoEncoder
+            lstm = cls(kind="lstm_model", lookback_window=eng.lookback, batch_size=self.batch_size, encoding_dim=tuple(eng.units),
+                       encoding_func=tuple(eng.acts), decoding_dim=(), decoding_func=(), out_func=eng.out_func, n_features=eng.n_features,
+                       n_features_out=T)
+            spec = lstm._build_spec()
+            det = DiffBasedAnomalyDetector(base_estimator=lstm, scaler=MinMaxScaler())
+        lstm.model = FittedNet(spec, eng.unpack_params(self.params[m : m + 1])[0])
+        hist = {"loss": [float(v) for v in self.loss[m]]}
+        if "accuracy" in spec.metrics:
+            hist["accuracy"] = [float(v) for v in self.acc[m]]
+        lstm._history = History(hist, {"verbose": 0, "epochs": len(hist["loss"]), "steps": self.steps_per_epoch}, list(range(len(hist["loss"]))))
+        lstm.model.history = lstm._history
+        _fill_minmax_from_extrema(det.scaler, self.y_min[m], self.y_max[m], self.rows, tags)
+        det.feature_thresholds_ = pd.Series(self.feat_thr[m].copy(), index=tags, name=f"fold-{K - 1}")
+        det.aggregate_threshold_ = float(self.agg_thr[m])
+        det.feature_thresholds_per_fold_ = pd.DataFrame(self.fold_feat_thr[m].copy(), columns=tags, index=[f"fold-{k}" for k in range(K)])
+        det.aggregate_thresholds_per_fold_ = {f"fold-{k}": float(self.fold_agg_thr[m, k]) for k in range(K)}
+        det.smooth_feature_thresholds_per_fold_ = pd.DataFrame()
+        det.smooth_aggregate_thresholds_per_fold_ = {}
+        det.smooth_aggregate_threshold_ = None
+        det.smooth_feature_thresholds_ = None
+        return det
+
+
+def build_lstm_fleet(eng: "engine.LSTMEngine", x, y, rows: int, lookahead: int = 0, epochs: int = 1, batch_size: int = 32, n_splits: int = 3,
+                     seed: int = 0, adam: Optional[Dict[str, float]] = None, input_scaler: bool = False, memory_budget: int = 8 << 30,
+                     keep_init_params: bool = False, generator=None) -> LSTMFleetBuild:
+    """
+    The batched ``gordo build`` of one bucket of LSTM machines (``DiffBasedAnomalyDetector(KerasLSTMAutoEncoder | KerasLSTMForecast)``,
+    the network bare or behind one MinMaxScaler): for every machine the TimeSeriesSplit cross validation and the final fit, as
+    ``(n_splits + 1) * n_machines`` jobs of gb_lstm_fit (primer step, ordered batches), then one gb_lstm_infer(_tc) launch for
+    every fold model's test block and float64 scoring, thresholds, scaler extrema and metric moments, one launch each.
+
+    x, y: float64 device tensors [n_machines * rows, T]; machine m owns rows [m*rows, (m+1)*rows).  ``y`` may be ``x``.
+
+    ``memory_budget``: bytes of fit workspace (gb_lstm_fit_workspace_bytes) one gb_lstm_fit launch may take.  Machines are
+    trained in chunks that fit it -- all ``n_splits + 1`` fits of a machine in the same chunk; every job's result is the same
+    whatever the chunking.  ``keep_init_params``: keep the initial parameters of every slot on the result (``init_params``).
+    """
+    torch = engine._torch()
+    dev = eng.device
+    if x.dtype != torch.float64 or y.dtype != torch.float64:
+        raise ValueError(f"build_lstm_fleet takes float64 x and y, got {x.dtype} / {y.dtype}")
+    M, K, N, T = x.shape[0] // rows, int(n_splits), int(rows), eng.n_out
+    L, la = eng.lookback, int(lookahead)
+    test = N // (K + 1)
+    if test == 0:
+        raise ValueError("Too many splits for number of samples")
+    starts = [N - (K - k) * test for k in range(K)]  # sklearn TimeSeriesSplit: fold k trains on [0, starts[k]), tests the next `test` rows
+    train_rows = [N] + starts                        # final fit, then fold k
+    windows = [n - L + 1 - la for n in train_rows]   # the estimator's window count
+    n_test = test - L + 1 - la                       # predictions per test block
+    if min(windows) < 1 or starts[0] <= L or n_test < 1:
+        raise ValueError(f"{N} rows leave fold 0 without a training window or a test block without a prediction at lookback_window {L}, lookahead {la}")
+    S = M * (K + 1)
+    g = generator or torch.Generator(device=dev).manual_seed(int(seed))
+    params = eng.initial_params(S, g)
+    init_params = params.clone() if keep_init_params else None
+    # per slot: training rows / windows and the first row of its machine
+    slot_rows, slot_windows = np.repeat(train_rows, M).astype(np.int64), np.repeat(windows, M).astype(np.int64)
+    base = np.tile(np.arange(M, dtype=np.int64) * N, K + 1)
+
+    def host(t):
+        return t.cpu().numpy()
+
+    def extrema(a):
+        jobs = engine.jobs_to_device(engine.make_jobs(np.arange(S), slot_rows, base), dev)
+        lo, hi = (host(t) for t in engine.minmax_f64(jobs, S, N, a, S))
+        if not (np.isfinite(lo).all() and np.isfinite(hi).all()):
+            raise ValueError("a column without finite values in a training block")
+        return lo, hi
+
+    # target scalers: final on all rows, fold k on its training prefix (diff.py:173 inside each CV clone), float64 like _fit_scaler
+    y_lo, y_hi = extrema(y)
+    y32 = y.to(torch.float32)
+    in_lo = in_hi = None
+    if input_scaler:
+        # every fold clone fits the Pipeline's MinMaxScaler on its own prefix: slot s trains on its own float64-scaled copy of its
+        # machine's rows, at rows [s*N, (s+1)*N) of the replicated arrays (gb_affine_f64: sklearn's transform, rounded once)
+        in_lo, in_hi = (y_lo, y_hi) if y is x else extrema(x)
+        a, b = (torch.from_numpy(np.ascontiguousarray(v)).to(dev) for v in _minmax_attributes(in_lo, in_hi))
+        copy_jobs = engine.jobs_to_device(engine.make_jobs(np.arange(S), N, base, np.arange(S, dtype=np.int64) * N), dev)
+        xf = engine.affine_f64(copy_jobs, S, N, x, a, b, out_rows=S * N)
+        yf = y32.view(M, N, T).repeat(K + 1, 1, 1).view(S * N, T)
+        x_row = np.arange(S, dtype=np.int64) * N
+    else:
+        xf = y32 if y is x else x.to(torch.float32)
+        yf, x_row = y32, base
+
+    # fits: chunks of whole machines (final + K folds) whose workspace fits the budget
+    chunk = max(1, min(M, int(memory_budget) // max(eng.fit_workspace_bytes(K + 1), 1), 65535 // (K + 1)))
+    loss = torch.empty((S, epochs), dtype=torch.float32, device=dev)
+    acc = torch.empty_like(loss)
+    for m0 in range(0, M, chunk):
+        ms = np.arange(m0, min(M, m0 + chunk))
+        slots = np.concatenate([j * M + ms for j in range(K + 1)])
+        idx = torch.from_numpy(slots).to(dev)
+        p = params.index_select(0, idx)
+        jobs = engine.jobs_to_device(engine.make_jobs(np.arange(len(slots)), slot_windows[slots], x_row[slots]), dev)
+        cl, ca, _ = eng.fit(p, jobs, len(slots), int(slot_windows[slots].max()), xf, yf, epochs=epochs, batch_size=batch_size, lookahead=la,
+                            primer=True, adam=adam)
+        params.index_copy_(0, idx, p)
+        loss.index_copy_(0, idx, cl)
+        acc.index_copy_(0, idx, ca)
+
+    # fold scoring: fold k of machine m (job k*M + m) predicts the windows inside its test block, in one launch
+    KM = K * M
+    fk, fm = np.repeat(np.arange(K), M), np.tile(np.arange(M), K)
+    test_start = np.asarray(starts, dtype=np.int64)[fk]
+    out0 = np.arange(KM, dtype=np.int64) * n_test
+    infer_jobs = engine.jobs_to_device(engine.make_jobs(M + np.arange(KM), n_test, x_row[M:] + test_start, out0), dev)
+    pred = eng.infer(params, infer_jobs, KM, n_test, xf, KM * n_test)
+    # targets tail-aligned to the predictions, scored in float64 as the per-machine detector scores LSTM output (diff.py:350-385)
+    score_jobs = engine.jobs_to_device(engine.make_jobs(np.arange(KM), n_test, fm * N + test_start + L - 1 + la, out0), dev)
+    y_scale, _ = _minmax_attributes(y_lo, y_hi)
+    fold_scale = torch.from_numpy(np.ascontiguousarray(y_scale[M:])).to(dev)
+    res = engine.anomaly_score(score_jobs, KM, n_test, pred.to(torch.float64), y, T, scale=fold_scale, want=("tag-anomaly-unscaled", "total-anomaly-scaled"))
+    feat, agg = engine.thresholds(score_jobs, KM, n_test, res["tag-anomaly-unscaled"], res["total-anomaly-scaled"], T, KM, 6, dev)
+    # the evaluation metrics of ModelBuilder's cross validation reduce to five sums per (fold, tag)
+    moments = host(engine.cv_moments(score_jobs, KM, pred, y32, T)).reshape(K, M, 5, T).transpose(1, 0, 2, 3)
+    fold_feat = host(feat).reshape(K, M, T).transpose(1, 0, 2)
+    fold_agg = host(agg).reshape(K, M).T
+    loss_h, acc_h = host(loss), host(acc)
+
+    def folds(a):  # slot-ordered [S, ...] -> the folds of every machine [M, K, ...]
+        return np.ascontiguousarray(np.swapaxes(a[M:].reshape((K, M) + a.shape[1:]), 0, 1))
+
+    return LSTMFleetBuild(
+        eng, M, K, N, la, int(batch_size), starts, n_test, params[:M].contiguous(), params[M:].view(K, M, -1).permute(1, 0, 2).contiguous(),
+        init_params, loss_h[:M], acc_h[:M], folds(loss_h), folds(acc_h), y_lo[:M], y_hi[:M], folds(y_lo), folds(y_hi),
+        np.ascontiguousarray(fold_feat[:, K - 1]), np.ascontiguousarray(fold_agg[:, K - 1]), np.ascontiguousarray(fold_feat),
+        np.ascontiguousarray(fold_agg), np.ascontiguousarray(moments), pred.view(K, M, n_test, T).permute(1, 0, 2, 3),
+        in_min=None if in_lo is None else in_lo[:M], in_max=None if in_hi is None else in_hi[:M],
+        fold_in_min=None if in_lo is None else folds(in_lo), fold_in_max=None if in_hi is None else folds(in_hi))

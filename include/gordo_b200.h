@@ -271,6 +271,12 @@ int gb_lstm_fit(const gb_lstmnet* net, float* params, float* adam_m, float* adam
                 const gb_job* jobs, int32_t n_jobs, int32_t max_windows, const float* x, const float* y,
                 const gb_lstm_fit_hparams* hp, void* workspace, float* out_loss, float* out_acc, void* stream);
 
+/* Keras' Orthogonal initialiser for recurrent kernels: g holds n_mats standard-normal [rows][cols] draws (float64, rows <= cols,
+ * overwritten); matrix i's rows are orthonormalised (Gram-Schmidt, the sign convention of Keras' QR) and written as float32 to
+ * out + out_offset + i * out_stride, row-major. */
+int gb_orthonormal_rows(double* g, int32_t n_mats, int32_t rows, int32_t cols, float* out, int64_t out_offset, int64_t out_stride,
+                        void* stream);
+
 #ifdef __cplusplus
 }
 #endif
