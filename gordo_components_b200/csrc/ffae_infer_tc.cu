@@ -15,11 +15,13 @@
 //
 // One persistent CTA per SM, NWG warpgroups.  Per work item (a range of one job's rows) the slot's weights are split and
 // laid out once in shared memory as K-major wgmma B operands.  A warpgroup owns a 64-row tile at a time, one thread per
-// (row pair, column pair) as the wgmma fragments lay it out: x is loaded from global memory straight into the A fragment of
+// (row pair, column pair) as the wgmma fragments lay it out: x is read from a shared-memory tile into the A fragment of
 // layer 0, and every layer's accumulator becomes the next layer's A fragment in registers (bias, tanh, FP16 split), so
-// activations never leave the register file.  The output layer's accumulator is scored against y in the same fragment
-// layout and every output array is stored from there (each access of a warp fills whole 32-byte sectors).  The warpgroups
-// of an SM overlap one another's tensor-core waits, and each prefetches its next tile's x while the hidden layers run.
+// activations never leave the register file.  The output layer's accumulator is scored against y, read from a second
+// shared-memory tile in the same fragment layout, and every output array is stored from there (each access of a warp fills
+// whole 32-byte sectors).  Each warpgroup owns one x and one y tile buffer, filled by TMA: the next tile's x is requested as
+// soon as layer 0 has read the current one, the next tile's y as soon as the output stage has read the current one, so both
+// loads are in flight behind a whole tile of MMAs.  The warpgroups of an SM overlap one another's tensor-core waits.
 //
 // Reference arithmetic replaced: keras Dense under Model.predict (gordo/machine/model/models.py:289-300) and
 // DiffBasedAnomalyDetector.anomaly (gordo/machine/model/anomaly/diff.py:350-385, 420-444).
@@ -34,12 +36,18 @@ namespace {
 using namespace gb::sm90;
 
 constexpr int TILE = 64;  // rows per warpgroup tile (wgmma M)
-constexpr int NWG = 3;    // warpgroups per CTA (168 registers per thread)
+constexpr int NWG = 3;    // warpgroups per CTA
 constexpr int NTHREADS = 128 * NWG;
 constexpr int MAXL = 8;
 constexpr int W = 64;  // widest feature / hidden width
+// x / y tiles in shared memory: 64 rows x 64 columns of fp32 as two TMA boxes of 32 columns (128-byte rows, SWIZZLE_128B)
+constexpr int BOX_COLS = 32;
+constexpr int BOX_BYTES = TILE * BOX_COLS * 4;
+constexpr int TILE_BYTES = 2 * BOX_BYTES;
+constexpr int STAGE_BYTES = 2 * TILE_BYTES * NWG;  // per warpgroup: one x and one y tile
 
 struct TcArgs {
+  CUtensorMap tm_x, tm_y;  // x and y as [n_x_rows][T], boxes of BOX_COLS x TILE, zeros outside (tm_y unused without y)
   int T;  // tags per row of x / y / every per-tag output (row pitch); <= W, multiple of 4
   int L;  // layers
   int N[MAXL], Np[MAXL], k16[MAXL];                  // Np = N rounded up to 16 (wgmma N), k16 = K steps of 16
@@ -49,11 +57,12 @@ struct TcArgs {
   int K[MAXL];
   int w_bytes;  // bytes of the weight+bias region (zero-filled before staging)
   int vec_ofs;
+  int stage_ofs;  // x / y tile buffers: the first 1024-byte boundary at or after this offset (SWIZZLE_128B boxes)
   int n_jobs, tiles_per_job;
   long pstride;
   const float* params;
   const gb_job* jobs;
-  const float *x, *y, *scale, *feat_thr, *agg_thr;
+  const float *y, *scale, *feat_thr, *agg_thr;  // (x and y are read through tm_x / tm_y; y != nullptr says whether it is given)
   float *o_model, *o_ts, *o_tu, *o_conf, *o_tots, *o_totu, *o_totconf;
   unsigned int* work_ctr;  // global tile counter of this launch (zeroed by the launcher, stream-ordered)
 };
@@ -140,6 +149,13 @@ __device__ __forceinline__ void mma_hidden(float* d, const uint32_t (&a1)[4][4],
     if (ks < k16) mma_f16<N>(d, a1[ks], desc_noswizzle(img0 + ks * step, lbo, 128), 1);
 }
 
+// Byte offset inside a staged tile of the float pair (row r, columns col, col + 1), col even.  SWIZZLE_128B stores the 16-byte
+// chunk c of a box row r at chunk c ^ (r % 8), so the eight rows g of a warp's fragment access fall in different chunks: each
+// 8-byte access of a warp touches every bank exactly twice (two wavefronts, the least for 256 bytes).
+__device__ __forceinline__ int tile_ofs(int r, int col) { return (col >> 5) * BOX_BYTES + r * 128 + ((((col & 31) >> 2) ^ (r & 7)) << 4) + ((col & 3) << 2); }
+
+__device__ __forceinline__ void warpgroup_sync(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(wg + 1) : "memory"); }
+
 __device__ __forceinline__ void fence_acc(float (&d)[32]) {
 #pragma unroll
   for (int i = 0; i < 32; ++i) fence_reg(d[i]);
@@ -165,6 +181,20 @@ __global__ void __launch_bounds__(NTHREADS, 1) ffae_tc_kernel(const __grid_const
   const bool has_y = a.y != nullptr;
   const bool totals = has_y && (a.o_tots || a.o_totu || a.o_totconf);
   const float inv_w = 1.0f / (float)TP;
+
+  // this warpgroup's x and y tiles, and the mbarriers their TMA loads complete on; thread 0 of the warpgroup issues the loads
+  __shared__ __align__(8) unsigned long long s_bar[2 * NWG];
+  const uint32_t stage = (sbase + a.stage_ofs + 1023) & ~1023u;
+  const uint32_t xbuf = stage + wg * 2 * TILE_BYTES, ybuf = xbuf + TILE_BYTES;
+  const uint8_t* xs = smem + (xbuf - sbase);
+  const uint8_t* ys = smem + (ybuf - sbase);
+  const uint32_t bar_x = smem_u32(&s_bar[wg]), bar_y = smem_u32(&s_bar[NWG + wg]);
+  const bool leader = (tid & 127) == 0;
+  uint32_t x_phase = 0, y_phase = 0;
+  if (tid == 0) {
+    for (int i = 0; i < 2 * NWG; ++i) mbar_init(smem_u32(&s_bar[i]), 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
 
   // Work distribution.  Tiles are numbered job by job (global tile G = job * tiles_per_job + tile) and handed out from a global
   // counter in contiguous ranges: whole jobs, in order, for most of the launch (a change of job restages the weights), then
@@ -248,29 +278,37 @@ __global__ void __launch_bounds__(NTHREADS, 1) ffae_tc_kernel(const __grid_const
 
     // ---- the tiles of this item, warpgroup by warpgroup
     const float* vec = reinterpret_cast<const float*>(smem + a.vec_ofs);
-    float xr[2][16];  // this thread's x: rows g, g+8 of its warp; per 16 columns the pairs 2t, 2t+1 and 2t+8, 2t+9
-    auto load_x = [&](int tt) {
-      const int r = row_begin + tt * TILE + wq * 16 + g;
-#pragma unroll
-      for (int hr = 0; hr < 2; ++hr) {
-        const int rr = min(r + 8 * hr, row_end - 1);  // rows past the end compute on a copy of the last row and store nothing
-        const float* xrow = a.x + (job.x_row + rr) * (long)TP;
-#pragma unroll
-        for (int c = 0; c < 8; ++c) {
-          const int col = 8 * c + 2 * t;
-          const float2 v = col < TP ? __ldg(reinterpret_cast<const float2*>(xrow + col)) : make_float2(0.f, 0.f);
-          xr[hr][2 * c] = v.x;
-          xr[hr][2 * c + 1] = v.y;
-        }
-        if (has_y && 32 * t < TP) asm volatile("prefetch.global.L2 [%0];" ::"l"(a.y + (job.x_row + rr) * (long)TP + 32 * t));  // read ~7 layers later
-      }
+    // One 64-row tile of x or y for this warpgroup (thread 0 of the warpgroup).  Columns past T and rows past the end of the array
+    // arrive as zeros; rows past the end of the job are its neighbour's rows.  Those rows run through the MMAs like any other (the
+    // rows of an MMA are independent) and nothing of them is stored.
+    auto load_tile = [&](const CUtensorMap* m, uint32_t buf, uint32_t bar, int tt) {
+      const int row = (int)(job.x_row + row_begin + tt * TILE);
+      mbar_expect_tx(bar, TILE_BYTES);
+      tma_load_2d(buf, m, 0, row, bar);
+      tma_load_2d(buf + BOX_BYTES, m, BOX_COLS, row, bar);
     };
-    if (wg < n_tiles) load_x(wg);
+    if (leader && wg < n_tiles) {
+      load_tile(&a.tm_x, xbuf, bar_x, wg);
+      if (has_y) load_tile(&a.tm_y, ybuf, bar_y, wg);
+    }
     for (int tt = wg; tt < n_tiles; tt += NWG) {
       float d[32];
       uint32_t a1[4][4] = {}, a2[4][4] = {};
       // ---- layer 0
       {
+        float xr[2][16];  // this thread's x: rows g, g+8 of its warp; per 16 columns the pairs 2t, 2t+1 and 2t+8, 2t+9
+        mbar_wait(bar_x, x_phase);
+        x_phase ^= 1;
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr)
+#pragma unroll
+          for (int c = 0; c < 8; ++c) {
+            const float2 v = *reinterpret_cast<const float2*>(xs + tile_ofs(wq * 16 + g + 8 * hr, 8 * c + 2 * t));
+            xr[hr][2 * c] = v.x;
+            xr[hr][2 * c + 1] = v.y;
+          }
+        warpgroup_sync(wg);  // the whole warpgroup has read x: the buffer takes the next tile's rows, which load behind this tile's layers
+        if (leader && tt + NWG < n_tiles) load_tile(&a.tm_x, xbuf, bar_x, tt + NWG);
         uint32_t xhi[4][8], alo[4][4], abf[4][4];
 #pragma unroll
         for (int kk = 0; kk < 4; ++kk) {
@@ -304,7 +342,6 @@ __global__ void __launch_bounds__(NTHREADS, 1) ffae_tc_kernel(const __grid_const
         fence_frag(alo);
         fence_frag(abf);
       }
-      if (tt + NWG < n_tiles) load_x(tt + NWG);  // the registers of x are free again: the next tile's rows load behind the hidden layers
 
       // ---- hidden layers, then the output layer
       for (int l = 0; l < L; ++l) {
@@ -346,11 +383,22 @@ __global__ void __launch_bounds__(NTHREADS, 1) ffae_tc_kernel(const __grid_const
       const int trow = row_begin + tt * TILE + wq * 16 + g;  // row inside the job of fragment row g
       const int nt = a.Np[L - 1] >> 3;
       float ss[2] = {0.f, 0.f}, su[2] = {0.f, 0.f};
+      float2 yr[2][8];  // y in the accumulator's layout: rows g, g+8; columns 8j + 2t, + 1
+      if (has_y) {
+        mbar_wait(bar_y, y_phase);
+        y_phase ^= 1;
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr)
+#pragma unroll
+          for (int j = 0; j < 8; ++j) yr[hr][j] = *reinterpret_cast<const float2*>(ys + tile_ofs(wq * 16 + g + 8 * hr, 8 * j + 2 * t));
+        warpgroup_sync(wg);  // the whole warpgroup has read y: the next tile's y loads behind the stores below and the next tile's layers
+        if (leader && tt + NWG < n_tiles) load_tile(&a.tm_y, ybuf, bar_y, tt + NWG);
+      }
 #pragma unroll
       for (int hr = 0; hr < 2; ++hr) {
         const int r = trow + 8 * hr;
         const bool live = r < row_end;
-        const long go = (job.out_row + r) * (long)TP, gy = (job.x_row + min(r, row_end - 1)) * (long)TP;
+        const long go = (job.out_row + r) * (long)TP;
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
           const int col = 8 * j + 2 * t;
@@ -359,7 +407,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) ffae_tc_kernel(const __grid_const
             const float2 yh = make_float2(d[4 * j + 2 * hr] + b.x, d[4 * j + 2 * hr + 1] + b.y);
             if (live) __stcs(reinterpret_cast<float2*>(a.o_model + go + col), yh);  // written once, never re-read: streaming stores
             if (has_y) {
-              const float2 yv = __ldg(reinterpret_cast<const float2*>(a.y + gy + col));
+              const float2 yv = yr[hr][j];
               const float2 sc = *reinterpret_cast<const float2*>(vec + col);
               const float2 df = make_float2(fabsf(yh.x - yv.x), fabsf(yh.y - yv.y));
               const float2 e = make_float2(df.x * sc.x, df.y * sc.y);
@@ -402,38 +450,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) ffae_tc_kernel(const __grid_const
 constexpr int WORK_CTRS = 1024;
 __device__ unsigned int g_work_ctr[WORK_CTRS];
 
-}  // namespace
-
-extern "C" int gb_ffae_tc_supported(const gb_ffnet* net) {
-  if (gb::validate_ffnet(net) != GB_OK) return GB_E_SHAPE;
-  const int L = net->n_layers;
-  if (L < 2 || L > MAXL || net->dims[0] != net->dims[L] || net->dims[0] > W || net->dims[0] < 24 || (net->dims[0] & 3)) {
-    gb::set_error("tensor-core variant covers autoencoders of 24..%d tags (a multiple of 4) with at most %d layers", W, MAXL);
-    return GB_E_SHAPE;
-  }
-  for (int l = 1; l < L; ++l)
-    if (net->dims[l] > W) {
-      gb::set_error("tensor-core variant needs hidden widths <= %d", W);
-      return GB_E_SHAPE;
-    }
-  for (int l = 0; l < L; ++l)
-    if (net->act[l] != (l + 1 < L ? GB_ACT_TANH : GB_ACT_LINEAR)) {
-      gb::set_error("tensor-core variant is specialised for tanh hidden layers and a linear output (the factory defaults)");
-      return GB_E_SHAPE;
-    }
-  return GB_OK;
-}
-
-extern "C" int gb_ffae_infer_score_tc(const gb_ffnet* net, const float* params, const gb_job* jobs, int32_t n_jobs, int32_t max_rows,
-                                      int64_t n_x_rows, int64_t n_out_rows, const float* x, const float* y, const float* scale,
-                                      const float* feat_thr, const float* agg_thr, float* out_model, float* out_tag_scaled,
-                                      float* out_tag_unscaled, float* out_total_scaled, float* out_total_unscaled, float* out_conf,
-                                      float* out_total_conf, int32_t flags, void* stream) {
-  int rc = gb_ffae_tc_supported(net);
-  if (rc != GB_OK) return rc;
-  GB_REQUIRE(flags == 0, GB_E_ARG, "variant bits above the low byte must be 0");
-  GB_REQUIRE(n_x_rows > 0 && n_out_rows > 0, GB_E_ARG, "the tensor-core variant needs the row counts of x and of the outputs");
-  TcArgs a{};
+// Shared-memory layout of the kernel for this architecture (fills the shape and offset fields of `a`); returns its bytes.
+int plan_smem(const gb_ffnet* net, TcArgs& a) {
   const int L = net->n_layers;
   a.L = L;
   a.T = net->dims[0];
@@ -462,8 +480,56 @@ extern "C" int gb_ffae_infer_score_tc(const gb_ffnet* net, const float* params, 
   a.w_bytes = gb::round_up(ofs, 16);
   ofs = a.w_bytes;
   a.vec_ofs = ofs; ofs += 2 * W * 4;
-  const size_t smem = (size_t)ofs;
-  GB_REQUIRE(smem <= 227 * 1024, GB_E_SMEM, "architecture needs %zu bytes of shared memory in the tensor-core variant", smem);
+  a.stage_ofs = ofs; ofs += 1024 + STAGE_BYTES;  // (the kernel aligns the tiles up to 1024 bytes inside this slack)
+  return ofs;
+}
+
+}  // namespace
+
+extern "C" int gb_ffae_tc_supported(const gb_ffnet* net) {
+  if (gb::validate_ffnet(net) != GB_OK) return GB_E_SHAPE;
+  const int L = net->n_layers;
+  if (L < 2 || L > MAXL || net->dims[0] != net->dims[L] || net->dims[0] > W || net->dims[0] < 24 || (net->dims[0] & 3)) {
+    gb::set_error("tensor-core variant covers autoencoders of 24..%d tags (a multiple of 4) with at most %d layers", W, MAXL);
+    return GB_E_SHAPE;
+  }
+  for (int l = 1; l < L; ++l)
+    if (net->dims[l] > W) {
+      gb::set_error("tensor-core variant needs hidden widths <= %d", W);
+      return GB_E_SHAPE;
+    }
+  for (int l = 0; l < L; ++l)
+    if (net->act[l] != (l + 1 < L ? GB_ACT_TANH : GB_ACT_LINEAR)) {
+      gb::set_error("tensor-core variant is specialised for tanh hidden layers and a linear output (the factory defaults)");
+      return GB_E_SHAPE;
+    }
+  TcArgs a{};
+  const int smem = plan_smem(net, a);
+  if (smem > 227 * 1024) {
+    gb::set_error("tensor-core variant: the weights and x / y tiles of this stack need %d bytes of shared memory (227 KB per SM)", smem);
+    return GB_E_SHAPE;
+  }
+  return GB_OK;
+}
+
+extern "C" int gb_ffae_infer_score_tc(const gb_ffnet* net, const float* params, const gb_job* jobs, int32_t n_jobs, int32_t max_rows,
+                                      int64_t n_x_rows, int64_t n_out_rows, const float* x, const float* y, const float* scale,
+                                      const float* feat_thr, const float* agg_thr, float* out_model, float* out_tag_scaled,
+                                      float* out_tag_unscaled, float* out_total_scaled, float* out_total_unscaled, float* out_conf,
+                                      float* out_total_conf, int32_t flags, void* stream) {
+  int rc = gb_ffae_tc_supported(net);
+  if (rc != GB_OK) return rc;
+  GB_REQUIRE(flags == 0, GB_E_ARG, "variant bits above the low byte must be 0");
+  GB_REQUIRE(n_x_rows > 0 && n_out_rows > 0, GB_E_ARG, "the tensor-core variant needs the row counts of x and of the outputs");
+  TcArgs a{};
+  const size_t smem = (size_t)plan_smem(net, a);
+  GB_REQUIRE(n_x_rows < (1L << 31), GB_E_ARG, "%ld rows of x: TMA row coordinates are 32-bit", (long)n_x_rows);
+  {
+    CUresult r = gb::sm90::encode_map_2d(&a.tm_x, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, x, n_x_rows, a.T, BOX_COLS, TILE);
+    if (r == CUDA_SUCCESS && y) r = gb::sm90::encode_map_2d(&a.tm_y, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, y, n_x_rows, a.T, BOX_COLS, TILE);
+    GB_REQUIRE(r != CUDA_ERROR_NOT_FOUND, GB_E_CUDA, "cuTensorMapEncodeTiled is not available from the driver");
+    GB_REQUIRE(r == CUDA_SUCCESS, GB_E_CUDA, "cuTensorMapEncodeTiled (x / y) failed with CUresult %d", (int)r);
+  }
 
   int dev = 0, sms = 132;
   GB_CUDA_CHECK(cudaGetDevice(&dev));
@@ -472,7 +538,7 @@ extern "C" int gb_ffae_infer_score_tc(const gb_ffnet* net, const float* params, 
   a.tiles_per_job = tiles_per_job;
   a.n_jobs = n_jobs;
   a.pstride = (long)gb_ffnet_param_stride(net);
-  a.params = params; a.jobs = jobs; a.x = x; a.y = y; a.scale = scale; a.feat_thr = feat_thr; a.agg_thr = agg_thr;
+  a.params = params; a.jobs = jobs; a.y = y; a.scale = scale; a.feat_thr = feat_thr; a.agg_thr = agg_thr;
   a.o_model = out_model; a.o_ts = out_tag_scaled; a.o_tu = out_tag_unscaled; a.o_conf = out_conf;
   a.o_tots = out_total_scaled; a.o_totu = out_total_unscaled; a.o_totconf = out_total_conf;
 

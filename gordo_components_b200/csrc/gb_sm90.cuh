@@ -56,6 +56,28 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
                : "memory");
 }
 
+// Host: TMA map of a row-major [rows][cols] tensor with boxes of box_cols x box_rows elements, SWIZZLE_128B (box_cols * elem_bytes
+// must be 128), zeros outside the tensor.  CUDA_ERROR_NOT_FOUND when the driver does not export cuTensorMapEncodeTiled.
+inline CUresult encode_map_2d(CUtensorMap* map, CUtensorMapDataType type, int elem_bytes, const void* base, long rows, long cols, int box_cols,
+                              int box_rows) {
+  typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
+                                    const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+  static EncodeTiledFn fn = nullptr;
+  if (!fn) {
+    void* p = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess)
+      return CUDA_ERROR_NOT_FOUND;
+    fn = reinterpret_cast<EncodeTiledFn>(p);
+  }
+  const cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
+  const cuuint64_t strides[1] = {(cuuint64_t)cols * elem_bytes};
+  const cuuint32_t box[2] = {(cuuint32_t)box_cols, (cuuint32_t)box_rows};
+  const cuuint32_t estr[2] = {1, 1};
+  return fn(map, type, 2, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+            CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+}
+
 __device__ __forceinline__ void wgmma_rs_f16_n16(float* d, const uint32_t* a, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
       "{\n.reg .pred p;\nsetp.ne.b32 p, %13, 0;\n"

@@ -329,26 +329,10 @@ __global__ void __launch_bounds__(128) lstm_tc_head_kernel(const gb_job* __restr
   }
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
-                                  const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiledFn encode_fn() {
-  static EncodeTiledFn fn = nullptr;
-  if (fn) return fn;
-  void* p = nullptr;
-  cudaDriverEntryPointQueryResult q;
-  if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess) return nullptr;
-  return fn = reinterpret_cast<EncodeTiledFn>(p);
-}
 // [rows][cols] FP16 row-major, box = 64 columns x box_rows rows, SWIZZLE_128B
 int make_map_f16(CUtensorMap* map, const void* base, long rows, long cols, int box_rows) {
-  EncodeTiledFn fn = encode_fn();
-  GB_REQUIRE(fn != nullptr, GB_E_CUDA, "cuTensorMapEncodeTiled is not available from the driver");
-  cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)cols * sizeof(__half)};
-  cuuint32_t box[2] = {KC, (cuuint32_t)box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                  CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  const CUresult r = encode_map_2d(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, sizeof(__half), base, rows, cols, KC, box_rows);
+  GB_REQUIRE(r != CUDA_ERROR_NOT_FOUND, GB_E_CUDA, "cuTensorMapEncodeTiled is not available from the driver");
   GB_REQUIRE(r == CUDA_SUCCESS, GB_E_CUDA, "cuTensorMapEncodeTiled (fp16) failed with CUresult %d", (int)r);
   return GB_OK;
 }
