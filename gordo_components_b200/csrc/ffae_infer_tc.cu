@@ -18,10 +18,13 @@
 // (row pair, column pair) as the wgmma fragments lay it out: x is read from a shared-memory tile into the A fragment of
 // layer 0, and every layer's accumulator becomes the next layer's A fragment in registers (bias, tanh, FP16 split), so
 // activations never leave the register file.  The output layer's accumulator is scored against y, read from a second
-// shared-memory tile in the same fragment layout, and every output array is stored from there (each access of a warp fills
-// whole 32-byte sectors).  Each warpgroup owns one x and one y tile buffer, filled by TMA: the next tile's x is requested as
-// soon as layer 0 has read the current one, the next tile's y as soon as the output stage has read the current one, so both
-// loads are in flight behind a whole tile of MMAs.  The warpgroups of an SM overlap one another's tensor-core waits.
+// shared-memory tile in the same fragment layout.  Each warpgroup owns one x and one y tile buffer, filled by TMA: the next
+// tile's x is requested as soon as layer 0 has read the current one, so it loads behind a whole tile of MMAs.  Every per-tag
+// output goes out through shared memory: each warp writes its 16 rows x 32 columns of an array into a 2 KB box and one lane
+// hands the box to a TMA store, so the writes reach HBM as whole lines and the warp moves on while they drain.  The warp's
+// two boxes are its two slices of the y tile (free once y is in registers), so y of a tile is requested only after layer 0 of
+// that tile, once the previous tile's stores have read their boxes; it loads behind layers 1 ..  The warpgroups of an SM
+// overlap one another's tensor-core waits.
 //
 // Reference arithmetic replaced: keras Dense under Model.predict (gordo/machine/model/models.py:289-300) and
 // DiffBasedAnomalyDetector.anomaly (gordo/machine/model/anomaly/diff.py:350-385, 420-444).
@@ -45,9 +48,13 @@ constexpr int BOX_COLS = 32;
 constexpr int BOX_BYTES = TILE * BOX_COLS * 4;
 constexpr int TILE_BYTES = 2 * BOX_BYTES;
 constexpr int STAGE_BYTES = 2 * TILE_BYTES * NWG;  // per warpgroup: one x and one y tile
+// output staging: a warp's 16 rows x 32 columns of one array (rows 16 wq .. of a SWIZZLE_128B box: a 1024-aligned slice)
+constexpr int OBOX_ROWS = 16;
+constexpr int OBOX_BYTES = OBOX_ROWS * BOX_COLS * 4;
 
 struct TcArgs {
   CUtensorMap tm_x, tm_y;  // x and y as [n_x_rows][T], boxes of BOX_COLS x TILE, zeros outside (tm_y unused without y)
+  CUtensorMap tm_o[4];     // model output, tag-anomaly-unscaled, -scaled, confidence as [n_out_rows][T], boxes of BOX_COLS x OBOX_ROWS
   int T;  // tags per row of x / y / every per-tag output (row pitch); <= W, multiple of 4
   int L;  // layers
   int N[MAXL], Np[MAXL], k16[MAXL];                  // Np = N rounded up to 16 (wgmma N), k16 = K steps of 16
@@ -152,7 +159,9 @@ __device__ __forceinline__ void mma_hidden(float* d, const uint32_t (&a1)[4][4],
 // Byte offset inside a staged tile of the float pair (row r, columns col, col + 1), col even.  SWIZZLE_128B stores the 16-byte
 // chunk c of a box row r at chunk c ^ (r % 8), so the eight rows g of a warp's fragment access fall in different chunks: each
 // 8-byte access of a warp touches every bank exactly twice (two wavefronts, the least for 256 bytes).
-__device__ __forceinline__ int tile_ofs(int r, int col) { return (col >> 5) * BOX_BYTES + r * 128 + ((((col & 31) >> 2) ^ (r & 7)) << 4) + ((col & 3) << 2); }
+// The same inside one box (col < 32); the output staging boxes use it too.
+__device__ __forceinline__ int box_ofs(int r, int col) { return r * 128 + (((col >> 2) ^ (r & 7)) << 4) + ((col & 3) << 2); }
+__device__ __forceinline__ int tile_ofs(int r, int col) { return (col >> 5) * BOX_BYTES + box_ofs(r, col & 31); }
 
 __device__ __forceinline__ void warpgroup_sync(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(wg + 1) : "memory"); }
 
@@ -191,6 +200,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) ffae_tc_kernel(const __grid_const
   const uint32_t bar_x = smem_u32(&s_bar[wg]), bar_y = smem_u32(&s_bar[NWG + wg]);
   const bool leader = (tid & 127) == 0;
   uint32_t x_phase = 0, y_phase = 0;
+  // this warp's output staging boxes (lane 0 issues their TMA stores)
+  const uint32_t obox0 = ybuf + wq * OBOX_BYTES, obox1 = obox0 + BOX_BYTES;
   if (tid == 0) {
     for (int i = 0; i < 2 * NWG; ++i) mbar_init(smem_u32(&s_bar[i]), 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -287,10 +298,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) ffae_tc_kernel(const __grid_const
       tma_load_2d(buf, m, 0, row, bar);
       tma_load_2d(buf + BOX_BYTES, m, BOX_COLS, row, bar);
     };
-    if (leader && wg < n_tiles) {
-      load_tile(&a.tm_x, xbuf, bar_x, wg);
-      if (has_y) load_tile(&a.tm_y, ybuf, bar_y, wg);
-    }
+    if (leader && wg < n_tiles) load_tile(&a.tm_x, xbuf, bar_x, wg);
     for (int tt = wg; tt < n_tiles; tt += NWG) {
       float d[32];
       uint32_t a1[4][4] = {}, a2[4][4] = {};
@@ -307,8 +315,13 @@ __global__ void __launch_bounds__(NTHREADS, 1) ffae_tc_kernel(const __grid_const
             xr[hr][2 * c] = v.x;
             xr[hr][2 * c + 1] = v.y;
           }
+        // the y tile holds the staged outputs of the previous tile: every warp's stores must have read them before y is refilled
+        if (lane == 0) bulk_wait_read<0>();
         warpgroup_sync(wg);  // the whole warpgroup has read x: the buffer takes the next tile's rows, which load behind this tile's layers
-        if (leader && tt + NWG < n_tiles) load_tile(&a.tm_x, xbuf, bar_x, tt + NWG);
+        if (leader) {
+          if (tt + NWG < n_tiles) load_tile(&a.tm_x, xbuf, bar_x, tt + NWG);
+          if (has_y) load_tile(&a.tm_y, ybuf, bar_y, tt);  // behind layers 1 ..
+        }
         uint32_t xhi[4][8], alo[4][4], abf[4][4];
 #pragma unroll
         for (int kk = 0; kk < 4; ++kk) {
@@ -378,11 +391,11 @@ __global__ void __launch_bounds__(NTHREADS, 1) ffae_tc_kernel(const __grid_const
         }
       }
 
-      // ---- output layer: model output and every anomaly column, straight from the accumulator fragment
+      // ---- output layer: model output and every anomaly column, from the accumulator fragment
       const float* bo = reinterpret_cast<const float*>(smem + a.bias_ofs[L - 1]);
-      const int trow = row_begin + tt * TILE + wq * 16 + g;  // row inside the job of fragment row g
+      const int wrow = row_begin + tt * TILE + wq * 16;  // row inside the job of the warp's first row
+      const int trow = wrow + g;                         // ... and of fragment row g
       const int nt = a.Np[L - 1] >> 3;
-      float ss[2] = {0.f, 0.f}, su[2] = {0.f, 0.f};
       float2 yr[2][8];  // y in the accumulator's layout: rows g, g+8; columns 8j + 2t, + 1
       if (has_y) {
         mbar_wait(bar_y, y_phase);
@@ -391,39 +404,81 @@ __global__ void __launch_bounds__(NTHREADS, 1) ffae_tc_kernel(const __grid_const
         for (int hr = 0; hr < 2; ++hr)
 #pragma unroll
           for (int j = 0; j < 8; ++j) yr[hr][j] = *reinterpret_cast<const float2*>(ys + tile_ofs(wq * 16 + g + 8 * hr, 8 * j + 2 * t));
-        warpgroup_sync(wg);  // the whole warpgroup has read y: the next tile's y loads behind the stores below and the next tile's layers
-        if (leader && tt + NWG < n_tiles) load_tile(&a.tm_y, ybuf, bar_y, tt + NWG);
       }
+      // model output of fragment rows g + 8 hr, columns 8j + 2t, + 1 (the output layer's MMAs write no columns past Np)
+      auto model_out = [&](int hr, int j) {
+        const float2 b = *reinterpret_cast<const float2*>(bo + 8 * j + 2 * t);
+        return j < nt ? make_float2(d[4 * j + 2 * hr] + b.x, d[4 * j + 2 * hr + 1] + b.y) : make_float2(0.f, 0.f);
+      };
+
+      // Per-tag outputs: for each array the warp asked for, and each half of 32 columns, the fragment goes into one of the warp's
+      // two staging boxes, in turn, and lane 0 hands the box to a TMA store.  A store clips at the array's edges but not at
+      // the end of the job, whose next rows may belong to another job written by another CTA: a warp whose 16 rows are not all
+      // inside the job copies its live rows out of the box itself.
+      const int n_live = min(row_end - wrow, OBOX_ROWS);
+      if (n_live > 0) {
+        int k = 0;  // boxes staged in this tile
 #pragma unroll
-      for (int hr = 0; hr < 2; ++hr) {
-        const int r = trow + 8 * hr;
-        const bool live = r < row_end;
-        const long go = (job.out_row + r) * (long)TP;
+        for (int arr = 0; arr < 4; ++arr) {
+          float* o = arr == 0 ? a.o_model : arr == 1 ? a.o_tu : arr == 2 ? a.o_ts : a.o_conf;
+          if (o == nullptr || (arr > 0 && !has_y)) continue;
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const int col = 8 * j + 2 * t;
-          if (j < nt && col < TP) {  // T is a multiple of 4: col + 1 < T too
-            const float2 b = *reinterpret_cast<const float2*>(bo + col);
-            const float2 yh = make_float2(d[4 * j + 2 * hr] + b.x, d[4 * j + 2 * hr + 1] + b.y);
-            if (live) __stcs(reinterpret_cast<float2*>(a.o_model + go + col), yh);  // written once, never re-read: streaming stores
-            if (has_y) {
-              const float2 yv = yr[hr][j];
+          for (int h = 0; h < 2; ++h) {
+            if (h == 1 && TP <= BOX_COLS) break;
+            const uint32_t box = (k & 1) ? obox1 : obox0;
+            if (k >= 2 && lane == 0) bulk_wait_read<1>();  // the store that last used this box has read it
+            __syncwarp();
+            uint8_t* bs = smem + (box - sbase);
+#pragma unroll
+            for (int hr = 0; hr < 2; ++hr)
+#pragma unroll
+              for (int jj = 0; jj < 4; ++jj) {
+                const int j = 4 * h + jj, col = 8 * j + 2 * t;
+                float2 v = model_out(hr, j);
+                if (arr > 0) {
+                  const float2 yv = yr[hr][j];
+                  v = make_float2(fabsf(v.x - yv.x), fabsf(v.y - yv.y));
+                  const float2 s = *reinterpret_cast<const float2*>(vec + (arr == 3 ? W : 0) + col);
+                  if (arr > 1) v = make_float2(v.x * s.x, v.y * s.y);
+                }
+                *reinterpret_cast<float2*>(bs + box_ofs(g + 8 * hr, 8 * jj + 2 * t)) = v;
+              }
+            fence_proxy_async();  // the box is read by the TMA store (async proxy)
+            __syncwarp();
+            if (n_live == OBOX_ROWS) {
+              if (lane == 0) {
+                tma_store_2d(&a.tm_o[arr], box, BOX_COLS * h, (int)(job.out_row + wrow));
+                bulk_commit();
+              }
+            } else {
+              const int cols = min(BOX_COLS, TP - BOX_COLS * h);
+              for (int i = lane; i < n_live * 8; i += 32) {  // 16-byte chunk c of row r: coalesced along the row
+                const int r = i >> 3, c = i & 7;
+                if (4 * c < cols)
+                  __stcs(reinterpret_cast<float4*>(o + (job.out_row + wrow + r) * (long)TP + BOX_COLS * h + 4 * c),
+                         *reinterpret_cast<const float4*>(bs + box_ofs(r, 4 * c)));
+              }
+            }
+            ++k;
+          }
+        }
+      }
+      if (totals) {
+        float ss[2] = {0.f, 0.f}, su[2] = {0.f, 0.f};
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr)
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            const int col = 8 * j + 2 * t;
+            if (j < nt && col < TP) {  // T is a multiple of 4: col + 1 < T too
+              const float2 yh = model_out(hr, j), yv = yr[hr][j];
               const float2 sc = *reinterpret_cast<const float2*>(vec + col);
               const float2 df = make_float2(fabsf(yh.x - yv.x), fabsf(yh.y - yv.y));
               const float2 e = make_float2(df.x * sc.x, df.y * sc.y);
               su[hr] += df.x * df.x + df.y * df.y;
               ss[hr] += e.x * e.x + e.y * e.y;
-              if (live && a.o_tu) __stcs(reinterpret_cast<float2*>(a.o_tu + go + col), df);
-              if (live && a.o_ts) __stcs(reinterpret_cast<float2*>(a.o_ts + go + col), e);
-              if (live && a.o_conf) {
-                const float2 rt = *reinterpret_cast<const float2*>(vec + W + col);
-                __stcs(reinterpret_cast<float2*>(a.o_conf + go + col), make_float2(df.x * rt.x, df.y * rt.y));
-              }
             }
           }
-        }
-      }
-      if (totals) {
 #pragma unroll
         for (int hr = 0; hr < 2; ++hr) {
           ss[hr] += __shfl_xor_sync(0xffffffffu, ss[hr], 1);
@@ -443,6 +498,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) ffae_tc_kernel(const __grid_const
     }
     __syncthreads();  // every warpgroup is done with this item's weights before the next item restages them
   }
+  if (lane == 0) bulk_wait<0>();  // shared memory must outlive the stores' reads of it
 }
 
 // tile counters of the launches in flight: a ring of static device words, one per launch, zeroed stream-ordered before the kernel
@@ -524,11 +580,15 @@ extern "C" int gb_ffae_infer_score_tc(const gb_ffnet* net, const float* params, 
   TcArgs a{};
   const size_t smem = (size_t)plan_smem(net, a);
   GB_REQUIRE(n_x_rows < (1L << 31), GB_E_ARG, "%ld rows of x: TMA row coordinates are 32-bit", (long)n_x_rows);
+  GB_REQUIRE(n_out_rows < (1L << 31), GB_E_ARG, "%ld output rows: TMA row coordinates are 32-bit", (long)n_out_rows);
   {
     CUresult r = gb::sm90::encode_map_2d(&a.tm_x, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, x, n_x_rows, a.T, BOX_COLS, TILE);
     if (r == CUDA_SUCCESS && y) r = gb::sm90::encode_map_2d(&a.tm_y, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, y, n_x_rows, a.T, BOX_COLS, TILE);
+    float* const outs[4] = {out_model, out_tag_unscaled, out_tag_scaled, out_conf};  // the order of TcArgs::tm_o
+    for (int i = 0; i < 4; ++i)
+      if (r == CUDA_SUCCESS && outs[i]) r = gb::sm90::encode_map_2d(&a.tm_o[i], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, outs[i], n_out_rows, a.T, BOX_COLS, OBOX_ROWS);
     GB_REQUIRE(r != CUDA_ERROR_NOT_FOUND, GB_E_CUDA, "cuTensorMapEncodeTiled is not available from the driver");
-    GB_REQUIRE(r == CUDA_SUCCESS, GB_E_CUDA, "cuTensorMapEncodeTiled (x / y) failed with CUresult %d", (int)r);
+    GB_REQUIRE(r == CUDA_SUCCESS, GB_E_CUDA, "cuTensorMapEncodeTiled (x / y / outputs) failed with CUresult %d", (int)r);
   }
 
   int dev = 0, sms = 132;

@@ -55,9 +55,21 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
                "r"(c0), "r"(c1), "r"(bar)
                : "memory");
 }
+// TMA store of one box from shared memory (the writes to it are made visible to the async proxy by fence_proxy_async first);
+// the issuing thread tracks it in its bulk groups
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(map), "r"(src), "r"(c0), "r"(c1) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// at most N of this thread's bulk groups still read their shared-memory source
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+// at most N of this thread's bulk groups are still in flight
+template <int N>
+__device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
 
 // Host: TMA map of a row-major [rows][cols] tensor with boxes of box_cols x box_rows elements, SWIZZLE_128B (box_cols * elem_bytes
-// must be 128), zeros outside the tensor.  CUDA_ERROR_NOT_FOUND when the driver does not export cuTensorMapEncodeTiled.
+// must be 128), zeros outside the tensor (loads) or clipped at its edges (stores).  CUDA_ERROR_NOT_FOUND when the driver does not export cuTensorMapEncodeTiled.
 inline CUresult encode_map_2d(CUtensorMap* map, CUtensorMapDataType type, int elem_bytes, const void* base, long rows, long cols, int box_cols,
                               int box_rows) {
   typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
