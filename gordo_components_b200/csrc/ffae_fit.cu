@@ -528,6 +528,42 @@ int odd_pitch(int width) {
   return p4 * 4;
 }
 
+// Memory plan of a fit: the first of five layouts that fits.  Everything in shared memory; else the weight image in the slot's
+// L2-resident state area; then, one by one, the dz buffers in L2 as well (at most as many as the two spare thirds of the Adam-v
+// area hold).  Fills the layout fields of `a` (net, image, widths, offsets, pitches, d_global) and the dynamic shared memory.
+int plan_fit(const gb_ffnet* net, FitArgs& a, bool& w_global, size_t& smem) {
+  a.net = *net;
+  a.im = gb::make_ff_image(net, 4);
+  const int L = net->n_layers;
+  a.n_in = net->dims[0];
+  a.n_out = net->dims[L];
+  a.wfloats = gb::round_up(a.im.total, 4);
+  smem = 0;
+  w_global = false;
+  for (int pass = 0; pass < 5; ++pass) {
+    w_global = pass >= 1;
+    a.d_global = pass >= 2 ? pass - 1 : 0;
+    int ofs = w_global ? 0 : a.wfloats;
+    a.apitch[0] = odd_pitch(a.im.kp[0]);
+    for (int l = 1; l <= L; ++l) {
+      a.apitch[l] = odd_pitch(a.im.np[l - 1]);
+      a.aofs[l] = ofs;
+      ofs += BR * a.apitch[l];
+    }
+    for (int b = 0; b < 2; ++b) { a.xofs[b] = ofs; ofs += BR * a.apitch[0]; }
+    a.ypitch = odd_pitch(gb::round_up(a.n_out, 4));
+    for (int b = 0; b < 2; ++b) { a.yofs[b] = ofs; ofs += BR * a.ypitch; }
+    a.dpitch = odd_pitch(a.im.max_np);
+    for (int b = 0; b < 3 - a.d_global; ++b) { a.dofs[b] = ofs; ofs += BR * a.dpitch; }
+    a.smem_floats = ofs;
+    smem = (size_t)ofs * sizeof(float);
+    if (smem <= 227 * 1024 && (long)a.d_global * BR * a.dpitch <= 2L * a.wfloats) break;
+  }
+  GB_REQUIRE(smem <= 227 * 1024 && (long)a.d_global * BR * a.dpitch <= 2L * a.wfloats, GB_E_SMEM,
+             "architecture needs %zu bytes of shared memory for the activations of one mini-batch chunk", smem);
+  return GB_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -535,6 +571,18 @@ extern "C" {
 size_t gb_ffae_fit_state_stride(const gb_ffnet* net) {
   if (gb::validate_ffnet(net) != GB_OK) return 0;
   return 3 * (size_t)gb::round_up(gb::make_ff_image(net, 4).total, 4);  // moments + gradient scratch of multi-chunk mini-batches + weight image of wide stacks
+}
+
+int gb_ffae_fit_plan(const gb_ffnet* net, int32_t* weights_in_l2, int32_t* dz_in_l2) {
+  const int rc = gb::validate_ffnet(net);
+  if (rc != GB_OK) return rc;
+  FitArgs a{};
+  size_t smem = 0;
+  bool w_global = false;
+  if (plan_fit(net, a, w_global, smem) != GB_OK) return GB_E_SMEM;
+  if (weights_in_l2) *weights_in_l2 = w_global ? 1 : 0;
+  if (dz_in_l2) *dz_in_l2 = a.d_global;
+  return GB_OK;
 }
 
 // debug aid (not part of the public header): per-phase cycle sums of CTA 0 into a device buffer of 2*GB_MAX_LAYERS+4 int64
@@ -561,46 +609,21 @@ int gb_ffae_fit(const gb_ffnet* net, float* params, float* adam_m, float* adam_v
   if (n_jobs == 0 || max_rows == 0) return GB_OK;
 
   FitArgs a{};
-  a.net = *net;
-  a.im = gb::make_ff_image(net, 4);
+  size_t smem = 0;
+  bool w_global = false;
+  rc = plan_fit(net, a, w_global, smem);
+  if (rc != GB_OK) return rc;
   a.hp = *hp;
   const int L = net->n_layers;
-  a.n_in = net->dims[0];
-  a.n_out = net->dims[L];
   a.max_rows = max_rows;
   a.pstride = (long)gb_ffnet_param_stride(net);
   a.sstride = (long)gb_ffae_fit_state_stride(net);
-  a.wfloats = gb::round_up(a.im.total, 4);
   a.gather_layer = 0;
   for (int l = 1; l < L; ++l)
     if (a.im.np[l] <= a.im.np[a.gather_layer]) a.gather_layer = l;  // the last of the narrowest layers
   a.gather_layer2 = a.gather_layer;
   for (int l = 0, best = 1 << 30; l < L; ++l)
     if (l != a.gather_layer && a.im.np[l] < best) { best = a.im.np[l]; a.gather_layer2 = l; }  // the narrowest of the others
-  size_t smem = 0;
-  bool w_global = false;
-  // first everything in shared memory; if that does not fit, the weight image in L2; then, one by one, the dz buffers in L2 as well
-  for (int pass = 0; pass < 5; ++pass) {
-    w_global = pass >= 1;
-    a.d_global = pass >= 2 ? pass - 1 : 0;
-    int ofs = w_global ? 0 : a.wfloats;
-    a.apitch[0] = odd_pitch(a.im.kp[0]);
-    for (int l = 1; l <= L; ++l) {
-      a.apitch[l] = odd_pitch(a.im.np[l - 1]);
-      a.aofs[l] = ofs;
-      ofs += BR * a.apitch[l];
-    }
-    for (int b = 0; b < 2; ++b) { a.xofs[b] = ofs; ofs += BR * a.apitch[0]; }
-    a.ypitch = odd_pitch(gb::round_up(a.n_out, 4));
-    for (int b = 0; b < 2; ++b) { a.yofs[b] = ofs; ofs += BR * a.ypitch; }
-    a.dpitch = odd_pitch(a.im.max_np);
-    for (int b = 0; b < 3 - a.d_global; ++b) { a.dofs[b] = ofs; ofs += BR * a.dpitch; }
-    a.smem_floats = ofs;
-    smem = (size_t)ofs * sizeof(float);
-    if (smem <= 227 * 1024 && (long)a.d_global * BR * a.dpitch <= 2L * a.wfloats) break;
-  }
-  GB_REQUIRE(smem <= 227 * 1024 && (long)a.d_global * BR * a.dpitch <= 2L * a.wfloats, GB_E_SMEM,
-             "architecture needs %zu bytes of shared memory for the activations of one mini-batch chunk", smem);
   a.params = params; a.adam_m = adam_m; a.adam_v = adam_v; a.jobs = jobs; a.x = x; a.y = y; a.perm = perm;
   a.out_loss = out_loss; a.out_acc = out_acc;
   a.trace = g_fit_trace;

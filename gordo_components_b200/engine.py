@@ -452,13 +452,14 @@ class LSTMEngine:
             m, v, t = state
         ws_bytes = int(self.lib.gb_lstm_fit_workspace_bytes(C.byref(self.net), int(n_jobs)))
         ws = torch.empty((ws_bytes + 3) // 4, dtype=torch.float32, device=self.device)
-        loss = torch.zeros((n_jobs, max(epochs, 1)), dtype=torch.float32, device=self.device)[:, :epochs]
-        acc = torch.zeros((n_jobs, max(epochs, 1)), dtype=torch.float32, device=self.device)[:, :epochs]
-        loss, acc = loss.contiguous(), acc.contiguous()
+        # a primer-only fit (epochs = 0) writes no history, but the kernel takes the outputs as non-NULL pointers and a tensor with
+        # no elements has none: the buffers keep one column and the caller gets the empty slice
+        loss = torch.zeros((n_jobs, max(epochs, 1)), dtype=torch.float32, device=self.device)
+        acc = torch.zeros((n_jobs, max(epochs, 1)), dtype=torch.float32, device=self.device)
         p = _cabi.ptr
         _cabi.check(self.lib.gb_lstm_fit(C.byref(self.net), p(params), p(m), p(v), p(t), p(jobs_dev), int(n_jobs), int(max_windows), p(x), p(y),
                                          C.byref(hp), p(ws), p(loss), p(acc), _stream_ptr()))
-        return loss, acc, (m, v, t)
+        return loss[:, :epochs], acc[:, :epochs], (m, v, t)
 
     @property
     def tc_supported(self) -> bool:

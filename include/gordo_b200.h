@@ -216,6 +216,12 @@ int gb_ffae_fit(const gb_ffnet* net, float* params, float* adam_m, float* adam_v
                 int32_t n_jobs, int32_t max_rows, const float* x, const float* y, const int32_t* perm,
                 const gb_fit_hparams* hp, float* out_loss, float* out_acc, void* stream);
 
+/* The memory plan gb_ffae_fit uses for this architecture (host only, no device needed).  The first of five that fits in
+ * 227 KB of shared memory: everything in shared memory; the weight image in the slot's L2-resident state area
+ * (*weights_in_l2 = 1); then one, two or three of the three dz buffers there as well (*dz_in_l2).  GB_E_SMEM if none fits
+ * (gb_ffae_fit refuses the architecture with the same status); either output may be NULL. */
+int gb_ffae_fit_plan(const gb_ffnet* net, int32_t* weights_in_l2, int32_t* dz_in_l2);
+
 /* ---- K3: LSTM autoencoder predict --------------------------------------------------------
  * lstm_model / lstm_symmetric / lstm_hourglass (factories/lstm_autoencoder.py:72-103):
  * LSTM layers (gate order i,f,c,o; sigmoid recurrent activation; zero initial state per

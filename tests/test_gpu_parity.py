@@ -13,11 +13,11 @@ import os
 import numpy as np
 import pandas as pd
 import pytest
+from parity_helpers import close, random_net
 
 pytestmark = pytest.mark.gpu
 
 GOLDEN = os.path.join(os.path.dirname(__file__), "golden")
-RTOL = 1e-4
 
 
 @pytest.fixture(scope="module")
@@ -37,26 +37,6 @@ def engine(torch):
     from gordo_components_b200 import engine as e
 
     return e
-
-
-FLOOR = 2e-5  # absolute part of the tolerance, in units of the data magnitude: the tensor-core split-precision path measures ~2e-6
-
-
-def close(got, want, mag=1.0, rtol=RTOL, name="", atol=0.0, floor=FLOOR):
-    got, want = np.asarray(got, dtype=np.float64), np.asarray(want, dtype=np.float64)
-    assert got.shape == want.shape, (name, got.shape, want.shape)
-    err = np.abs(got - want)
-    tol = rtol * np.abs(want) + floor * mag + atol
-    bad = ~(err <= tol) & ~(np.isnan(got) & np.isnan(want))
-    assert not bad.any(), f"{name}: {bad.sum()} of {bad.size} outside tolerance; max err {err[bad].max():.3e} (tol {tol[bad].min():.3e})"
-
-
-def random_net(km, dims_or_T, seed, acts=None):
-    rng = np.random.default_rng(seed)
-    spec = km.ff_hourglass_spec(dims_or_T) if isinstance(dims_or_T, int) else km.FFSpec(list(dims_or_T), acts or ["tanh"] * (len(dims_or_T) - 2) + ["linear"])
-    w = km.init_ff_weights(spec, rng)
-    w = [(W, rng.uniform(-0.2, 0.2, b.shape).astype(np.float32)) for W, b in w]
-    return spec, w
 
 
 def run_infer(engine, torch, spec, weights_per_slot, X, y, jobs_h, scale=None, feat=None, agg=None, out_rows=None, variant=0):
