@@ -7,9 +7,12 @@ number a `gordo build` user sees.
 
     python benchmarks/bench_fleet_builder.py [--machines 125] [--rows 10000] [--tags 64] [--epochs 10] [--scaled] [--single 3]
     python benchmarks/bench_fleet_builder.py --lstm [--lookback 24] --machines 16 --rows 2000 --tags 16 --epochs 1 --single 16
+    python benchmarks/bench_fleet_builder.py --example-config --machines 125 --rows 10000 --tags 64 --epochs 10 --single 3
 
 ``--lstm`` builds DiffBasedAnomalyDetector(KerasLSTMAutoEncoder(lstm_hourglass)) machines instead (batched by
-fleet.build_lstm_fleet).  Measured numbers and the card they were measured on are in DESIGN.md §7.
+fleet.build_lstm_fleet).  ``--example-config`` builds the model of gordo's examples/model-configuration.yaml:
+DiffBasedAnomalyDetector(shuffle=True) around Pipeline([MinMaxScaler, KerasAutoEncoder(feedforward_hourglass, compression_factor
+0.6, 1 encoding layer, batch 128, validation_split 0.1)]) under TimeSeriesSplit(5).  Measured numbers and the card they were measured on are in DESIGN.md §7.
 """
 import argparse, json, os, sys, tempfile, time
 sys.path.insert(0, os.path.abspath(os.path.join(os.path.dirname(__file__), "..")))
@@ -36,6 +39,7 @@ def main():
     ap.add_argument("--single", type=int, default=3, help="machines to also build one at a time for comparison")
     ap.add_argument("--lstm", action="store_true", help="LSTM autoencoder machines (lstm_hourglass) instead of the feed-forward hourglass")
     ap.add_argument("--lookback", type=int, default=24, help="lookback_window of the LSTM machines")
+    ap.add_argument("--example-config", action="store_true", help="the model and evaluation of gordo's examples/model-configuration.yaml")
     a = ap.parse_args()
     import numpy as np
     import pandas as pd
@@ -50,6 +54,15 @@ def main():
         ae = {"gordo.machine.model.models.KerasAutoEncoder": {"kind": "feedforward_hourglass", "epochs": a.epochs}}
     base = {"sklearn.pipeline.Pipeline": {"steps": ["sklearn.preprocessing.MinMaxScaler", ae]}} if a.scaled else ae
     model = {"gordo.machine.model.anomaly.diff.DiffBasedAnomalyDetector": {"base_estimator": base}}
+    evaluation, n_splits = {}, 3
+    if a.example_config:
+        ae = {"gordo.machine.model.models.KerasAutoEncoder": {
+            "batch_size": 128, "compression_factor": 0.6, "encoding_layers": 1, "epochs": a.epochs, "func": "tanh", "kind": "feedforward_hourglass",
+            "loss": "mse", "optimizer": "Adam", "out_func": "linear", "validation_split": 0.1}}
+        model = {"gordo.machine.model.anomaly.diff.DiffBasedAnomalyDetector": {
+            "base_estimator": {"sklearn.pipeline.Pipeline": {"steps": ["sklearn.preprocessing.MinMaxScaler", ae]}},
+            "scaler": "sklearn.preprocessing.MinMaxScaler", "shuffle": True, "smoothing_method": "smm"}}
+        evaluation, n_splits = {"cv": {"sklearn.model_selection.TimeSeriesSplit": {"n_splits": 5}}}, 5
     rng = np.random.default_rng(0)
     idx = pd.date_range("2019-01-01", periods=a.rows, freq="10min", tz="UTC")
     t = np.linspace(0, 60, a.rows)[:, None]
@@ -57,7 +70,7 @@ def main():
     for m in range(a.machines):
         values = 0.5 + 0.4 * np.sin(t * rng.uniform(0.5, 2, a.tags) + rng.uniform(0, 6, a.tags)) + rng.normal(0, 0.02, (a.rows, a.tags))
         frame = pd.DataFrame(values.astype(np.float32), index=idx, columns=[f"tag-{i}" for i in range(a.tags)])
-        machines.append({"name": f"machine-{m}", "model": model, "dataset": {"X": frame, "y": frame}})
+        machines.append({"name": f"machine-{m}", "model": model, "dataset": {"X": frame, "y": frame}, "evaluation": evaluation})
 
     builder.FleetModelBuilder(machines[:2]).build()  # warm-up: library load, first launches
     torch.cuda.synchronize()
@@ -76,10 +89,12 @@ def main():
         single_s = (time.perf_counter() - t0) / a.single
     scores = results[0][1]["metadata"]["build_metadata"]["model"]["cross_validation"]["scores"]
     net = f"LSTM hourglass (lookback {a.lookback})" if a.lstm else "hourglass"
+    if a.example_config:
+        net = "hourglass (compression 0.6, 1 encoding layer, batch 128, validation_split 0.1) in a shuffling detector"
     print(json.dumps({
         "gpu": torch.cuda.get_device_name(0), "power_limit_w": _power_limit(),
-        "workload": f"{a.machines} machines x {a.tags}-tag {net}{' behind MinMaxScaler' if a.scaled else ''}, {a.rows} rows, {a.epochs} epochs: "
-                    "definition -> 3-fold CV + fit + thresholds + scores metadata -> model.pkl/metadata.json",
+        "workload": f"{a.machines} machines x {a.tags}-tag {net}{' behind MinMaxScaler' if a.scaled or a.example_config else ''}, {a.rows} rows, {a.epochs} epochs: "
+                    f"definition -> {n_splits}-fold CV + fit + thresholds + scores metadata -> model.pkl/metadata.json",
         "fleet_builder_s": fleet_s, "machines_per_s": a.machines / fleet_s, "bytes_written": size,
         "model_builder_s_per_machine": single_s, "speedup_per_machine": None if single_s is None else single_s / (fleet_s / a.machines),
         "r2_fold_mean_machine_0": scores["r2-score"]["fold-mean"],

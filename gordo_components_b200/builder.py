@@ -25,6 +25,7 @@ import copy
 import datetime
 import importlib
 import logging
+import math
 import os
 import random
 import time
@@ -319,8 +320,10 @@ class ModelBuilder:
 class _Canonical:
     """What ``FleetModelBuilder`` needs to know about a machine that can take the batched path."""
 
-    def __init__(self, index, machine, model, spec, X, y, dataset_meta, query_sec, fit, n_splits, evaluation, input_scaler):
+    def __init__(self, index, machine, model, spec, X, y, dataset_meta, query_sec, fit, n_splits, evaluation, input_scaler,
+                 split=(False, 0.0, None)):
         self.index, self.machine, self.model, self.spec, self.input_scaler = index, machine, model, spec, input_scaler
+        self.split = split  # (detector shuffle, keras validation_split, validation batch size or None without a split)
         self.X, self.y, self.dataset_meta, self.query_sec = X, y, dataset_meta, query_sec
         self.fit, self.n_splits, self.evaluation = fit, n_splits, evaluation
 
@@ -328,7 +331,7 @@ class _Canonical:
         s = self.spec
         return (tuple(s.dims), tuple(s.acts), tuple(float(v) for v in s.l1), tuple(sorted(s.adam.items())), tuple(s.metrics),
                 len(self.X), self.fit["epochs"], self.fit["batch_size"], self.fit["shuffle"], self.n_splits, int(self.evaluation.get("seed", 0)),
-                self.input_scaler)
+                self.split, self.input_scaler)
 
 
 def _default_minmax(scaler) -> bool:
@@ -360,7 +363,7 @@ def _canonical(index, machine) -> Optional[_Canonical]:
         return no("cv is not a plain TimeSeriesSplit")
 
     model = serializer.from_definition(machine["model"])
-    if type(model) is not DiffBasedAnomalyDetector or model.window is not None or model.shuffle:
+    if type(model) is not DiffBasedAnomalyDetector or model.window is not None:
         return no("model is not a plain DiffBasedAnomalyDetector")
     if not _default_minmax(model.scaler):
         return no("detector scaler is not a default MinMaxScaler")
@@ -370,8 +373,11 @@ def _canonical(index, machine) -> Optional[_Canonical]:
     if type(ae) is not KerasAutoEncoder:
         return no("base_estimator is not a KerasAutoEncoder, bare or behind one default MinMaxScaler")
     fit_args = ae.extract_supported_fit_args(ae.kwargs)
-    if fit_args.get("validation_split") or fit_args.get("callbacks"):
-        return no("validation_split / callbacks need the per-epoch loop")
+    if fit_args.get("callbacks"):
+        return no("callbacks need the per-epoch loop")
+    vsplit = float(fit_args.get("validation_split") or 0.0)
+    if vsplit and not 0.0 < vsplit < 1.0:
+        return no(f"validation_split {vsplit} is outside (0, 1)")
 
     t0 = time.time()
     X, y, dataset_meta = _get_data(machine["dataset"])
@@ -380,10 +386,14 @@ def _canonical(index, machine) -> Optional[_Canonical]:
     spec = ae._build_spec()
     if not isinstance(spec, FFNetSpec):
         return no("not a feed-forward network")
-    if len(X) != len(y) or len(X) // (split_obj.n_splits + 1) == 0:
+    test = len(X) // (split_obj.n_splits + 1)
+    if len(X) != len(y) or test == 0:
         return no("too few rows for the CV folds")
+    if vsplit and math.floor((len(X) - split_obj.n_splits * test) * (1.0 - vsplit)) < 1:  # the smallest fold: keras' split (models.py)
+        return no(f"validation_split {vsplit} leaves the first CV fold without a training row")
     fit = {"epochs": int(fit_args.get("epochs", 1)), "batch_size": int(fit_args.get("batch_size") or 32), "shuffle": bool(fit_args.get("shuffle", True))}
-    return _Canonical(index, machine, model, spec, X, y, dataset_meta, query_sec, fit, split_obj.n_splits, evaluation, input_scaler)
+    split = (bool(model.shuffle), vsplit, int(fit_args.get("validation_batch_size") or fit["batch_size"]) if vsplit else None)
+    return _Canonical(index, machine, model, spec, X, y, dataset_meta, query_sec, fit, split_obj.n_splits, evaluation, input_scaler, split)
 
 
 class _CanonicalLSTM(_Canonical):
@@ -535,7 +545,8 @@ class FleetModelBuilder:
         yd = xd if same_y else engine.to_device_f32(np.concatenate([np.ascontiguousarray(c.y.values, dtype=np.float32) for c in members]), eng.device)
         fb = fleet.build_fleet(eng, xd, yd, rows, epochs=first.fit["epochs"], batch_size=first.fit["batch_size"], n_splits=K,
                                seed=int(first.evaluation.get("seed", 0)), adam=first.spec.adam, shuffle=first.fit["shuffle"],
-                               input_scaler=first.input_scaler)
+                               input_scaler=first.input_scaler, detector_shuffle=first.split[0], validation_split=first.split[1],
+                               validation_batch_size=first.split[2])
         moments = fb.cv_moments.cpu().numpy()
         scale = fb.scale.cpu().numpy().astype(np.float64)
         engine._torch().cuda.synchronize()

@@ -45,6 +45,11 @@ struct FitArgs {
   const int32_t* perm;
   float *out_loss, *out_acc;
   long long* trace;  // debug (gb_debug_set_fit_trace): cycles of CTA 0 per phase, summed over the fit; NULL in production
+  // gb_ffae_fit_split only (appended, so that the fields above keep their offsets in the parameter block of every kernel)
+  const gb_fit_split* split;  // per job: held-out positions and row map; NULL = none
+  const int32_t* row_map;
+  int val_batch;
+  float *out_val_loss, *out_val_acc;
 };
 
 __device__ __forceinline__ uint32_t mix32(uint32_t h) {
@@ -111,7 +116,11 @@ __device__ __forceinline__ void quarter_reduce(const float (&acc)[4][4], int lan
 // WG = false: the slot's padded weight image lives in shared memory for the whole fit (every 64-tag stack).  WG = true: the image does
 // not fit beside the activations (e.g. the 128-tag hourglass, 245 KB) and lives in the slot's L2-resident state area instead; the
 // code is the same, the loads become global.
-template <bool WG, bool DG>  // DG: some dz buffers live in global memory too (kept apart so that the usual case addresses them as shared memory)
+// SPLIT (gb_ffae_fit_split): a job's rows are positions.  Training visits positions [0, n_rows); every epoch then ends with
+// forward-only mini-batches of val_batch rows over the held-out positions [n_rows, n_rows + n_val), in order, whose loss and
+// accuracy are the epoch's validation statistics.  Position p reads row x_row + row_map[map_ofs + p] (x_row + p without a map).
+// The held-out batches are more chunks of the same visiting order, so the cp.async prefetch runs across them as well.
+template <bool WG, bool DG, bool SPLIT = false>  // DG: some dz buffers live in global memory too (kept apart so that the usual case addresses them as shared memory)
 __global__ void __launch_bounds__(THREADS, 1) ffae_fit_kernel(const FitArgs a) {
   extern __shared__ __align__(16) float smem[];
   __shared__ float s_red[3][NWARPS];
@@ -159,6 +168,16 @@ __global__ void __launch_bounds__(THREADS, 1) ffae_fit_kernel(const FitArgs a) {
   const float* xbase = a.x + job.x_row * (long)n_in;
   const float* ybase = a.y + job.x_row * (long)n_out;
   const int steps = (n + B - 1) / B;
+  int nv = 0;           // held-out positions
+  long map_ofs = -1;
+  if (SPLIT && a.split != nullptr) {
+    nv = a.split[job_id].n_val;
+    if (a.row_map != nullptr) map_ofs = a.split[job_id].map_ofs;
+  }
+  const int VB = a.val_batch;
+  const int vsteps = SPLIT && nv > 0 ? (nv + VB - 1) / VB : 0;  // mini-batches s in [steps, steps + vsteps) are held-out ones
+  auto held_out = [&](int s) -> bool { return SPLIT && s >= steps; };
+  auto batch_rows = [&](int s) -> int { return held_out(s) ? min(VB, nv - (s - steps) * VB) : min(B, n - s * B); };
   const uint32_t key_base = mix32((uint32_t)a.hp.seed ^ mix32((uint32_t)(a.hp.seed >> 32) + 0x632be5abU * (uint32_t)(job.slot + 1)));
 
   auto row_index = [&](int e, int i) -> int {
@@ -166,9 +185,15 @@ __global__ void __launch_bounds__(THREADS, 1) ffae_fit_kernel(const FitArgs a) {
     if (a.hp.shuffle == 2) return a.perm[((long)job_id * a.hp.epochs + e) * a.max_rows + i];
     return (int)permute_index((uint32_t)i, (uint32_t)n, mix32(key_base + (uint32_t)e * 0x9e3779b9U));
   };
+  // row (relative to x_row) of row i of mini-batch s of epoch e
+  auto batch_row = [&](int e, int s, int i) -> int {
+    if (!SPLIT) return row_index(e, s * B + i);
+    const int p = held_out(s) ? n + (s - steps) * VB + i : row_index(e, s * B + i);
+    return map_ofs >= 0 ? a.row_map[map_ofs + p] : p;
+  };
   // rows [r_lo, r_hi) of chunk c (32 rows) of mini-batch s of epoch e, by n_warps warps
   auto gather = [&](int buf, int e, int s, int c, int first_warp, int n_warps, int r_lo = 0, int r_hi = BR) {
-    const int nb = min(BR, min(B, n - s * B) - c * BR);
+    const int nb = min(BR, batch_rows(s) - c * BR);
     float* xs = smem + a.xofs[buf];
     float* ys = smem + a.yofs[buf];
     for (int r = r_lo + warp - first_warp; r < min(nb, r_hi); r += n_warps) {
@@ -195,13 +220,13 @@ __global__ void __launch_bounds__(THREADS, 1) ffae_fit_kernel(const FitArgs a) {
   // the visiting order is resolved one chunk ahead of its gather by the last warp (a row per lane): the keyed permutation costs a
   // few hundred instructions per row, which every warp would otherwise repeat in front of its cp.async
   auto advance = [&](int& e, int& s, int& c) -> bool {  // next chunk in visiting order; false past the last epoch
-    const int nch = (min(B, n - s * B) + BR - 1) / BR;
-    if (++c == nch) { c = 0; if (++s == steps) { s = 0; ++e; } }
+    const int nch = (batch_rows(s) + BR - 1) / BR;
+    if (++c == nch) { c = 0; if (++s == steps + vsteps) { s = 0; ++e; } }
     return e < a.hp.epochs;
   };
   auto stage_indices = [&](int buf, int e, int s, int c) {
-    const int nb = min(BR, min(B, n - s * B) - c * BR);
-    if (lane < nb) s_idx[buf][lane] = row_index(e, s * B + c * BR + lane);
+    const int nb = min(BR, batch_rows(s) - c * BR);
+    if (lane < nb) s_idx[buf][lane] = batch_row(e, s, c * BR + lane);
   };
   auto adam_alpha = [&](int t_int) -> float {  // lr * sqrt(1 - b2^t) / (1 - b1^t)
     const double t = (double)t_int;
@@ -224,12 +249,35 @@ __global__ void __launch_bounds__(THREADS, 1) ffae_fit_kernel(const FitArgs a) {
     return b < 3 - a.d_global ? smem + a.dofs[b] : Vg + a.wfloats + (long)(b - (3 - a.d_global)) * BR * a.dpitch;
   };
 
+  // ---- epoch statistics (keras History: sample-weighted mean of the per-batch total loss) -------------
+  auto epoch_stats = [&](float v0, float v1, float v2, float* out_l, float* out_a, int rows, int e) {
+    for (int o = 16; o > 0; o >>= 1) {
+      v0 += __shfl_xor_sync(0xffffffffu, v0, o);
+      v1 += __shfl_xor_sync(0xffffffffu, v1, o);
+      v2 += __shfl_xor_sync(0xffffffffu, v2, o);
+    }
+    if (lane == 0) { s_red[0][warp] = v0; s_red[1][warp] = v1; s_red[2][warp] = v2; }
+    __syncthreads();
+    if (tid == 0) {
+      float q0 = 0.f, q1 = 0.f, q2 = 0.f;
+      for (int w = 0; w < NWARPS; ++w) { q0 += s_red[0][w]; q1 += s_red[1][w]; q2 += s_red[2][w]; }
+      out_l[(long)job_id * a.hp.epochs + e] = (q0 / (float)n_out + q1) / (float)rows;
+      if (out_a) out_a[(long)job_id * a.hp.epochs + e] = q2 / (float)rows;
+    }
+    __syncthreads();
+  };
+
   for (int e = 0; e < a.hp.epochs; ++e) {
     float acc_sq = 0.f, acc_reg = 0.f, acc_hit = 0.f;
-    for (int s = 0; s < steps; ++s) {
-      const int nbt = min(B, n - s * B);          // rows of this mini-batch
+    for (int s = 0; s < steps + vsteps; ++s) {
+      const bool val = held_out(s);               // forward only: loss statistics, no optimizer step
+      if (val && s == steps) {                    // the training statistics are complete: the held-out ones start from zero
+        epoch_stats(acc_sq, acc_reg, acc_hit, a.out_loss, a.out_acc, n, e);
+        acc_sq = acc_reg = acc_hit = 0.f;
+      }
+      const int nbt = batch_rows(s);              // rows of this mini-batch
       const int nchunks = (nbt + BR - 1) / BR;
-      ++t_step;
+      if (!val) ++t_step;
      for (int c = 0; c < nchunks; ++c) {
       const int nb = min(BR, nbt - c * BR);        // rows of this chunk
       const bool first_chunk = c == 0, last_chunk = c + 1 == nchunks;
@@ -260,7 +308,7 @@ __global__ void __launch_bounds__(THREADS, 1) ffae_fit_kernel(const FitArgs a) {
         }
         if (l == 0) {  // the last two warps have no tile in the first layer of a 64-tag hourglass (14 tiles): they prepare the next step
           if (warp == NWARPS - 1 && more2) stage_indices(cur, ne, ns, nc);  // read by the gather at the top of the next chunk
-          if (warp == NWARPS - 2 && first_chunk && lane == 0) s_alpha[(t_step + 1) & 1] = adam_alpha(t_step + 1);  // read after the loss barrier of step t+1
+          if (warp == NWARPS - 2 && first_chunk && !val && lane == 0) s_alpha[(t_step + 1) & 1] = adam_alpha(t_step + 1);  // read after the loss barrier of step t+1
         }
         // A warp owns 32 rows x 4 output columns; lane = (row group p, K quarter kq): rows p, p+8, p+16, p+24 against every fourth
         // block of four k.  Per block a lane loads 4 + 4 float4 for 64 FMA (a row per lane with the whole K needs 1 + 4 for 16: the
@@ -475,32 +523,20 @@ __global__ void __launch_bounds__(THREADS, 1) ffae_fit_kernel(const FitArgs a) {
           sW[off] = w; Mg[off] = m; Vg[off] = v;
         }
       };
-      for (int p = L - 1; p >= 0; --p) {
-        if (p > 0) input_grad(p);
-        if (p + 1 < L) weight_step(p + 1);
-        if (p == 0) weight_step(0);
-        __syncthreads();
-        stamp(L + 2 + (L - 1 - p));
+      if (!val) {
+        for (int p = L - 1; p >= 0; --p) {
+          if (p > 0) input_grad(p);
+          if (p + 1 < L) weight_step(p + 1);
+          if (p == 0) weight_step(0);
+          __syncthreads();
+          stamp(L + 2 + (L - 1 - p));
+        }
       }
       cur ^= 1;
      }  // chunks
     }
-    // ---- epoch statistics (keras History: sample-weighted mean of the per-batch total loss) -------------
-    float v0 = acc_sq, v1 = acc_reg, v2 = acc_hit;
-    for (int o = 16; o > 0; o >>= 1) {
-      v0 += __shfl_xor_sync(0xffffffffu, v0, o);
-      v1 += __shfl_xor_sync(0xffffffffu, v1, o);
-      v2 += __shfl_xor_sync(0xffffffffu, v2, o);
-    }
-    if (lane == 0) { s_red[0][warp] = v0; s_red[1][warp] = v1; s_red[2][warp] = v2; }
-    __syncthreads();
-    if (tid == 0) {
-      float q0 = 0.f, q1 = 0.f, q2 = 0.f;
-      for (int w = 0; w < NWARPS; ++w) { q0 += s_red[0][w]; q1 += s_red[1][w]; q2 += s_red[2][w]; }
-      a.out_loss[(long)job_id * a.hp.epochs + e] = (q0 / (float)n_out + q1) / (float)n;
-      if (a.out_acc) a.out_acc[(long)job_id * a.hp.epochs + e] = q2 / (float)n;
-    }
-    __syncthreads();
+    if (vsteps > 0) epoch_stats(acc_sq, acc_reg, acc_hit, a.out_val_loss, a.out_val_acc, nv, e);
+    else epoch_stats(acc_sq, acc_reg, acc_hit, a.out_loss, a.out_acc, n, e);
   }
 
   // ---- trained weights back to the canonical layout ------------------------------------------------------
@@ -564,37 +600,11 @@ int plan_fit(const gb_ffnet* net, FitArgs& a, bool& w_global, size_t& smem) {
   return GB_OK;
 }
 
-}  // namespace
-
-extern "C" {
-
-size_t gb_ffae_fit_state_stride(const gb_ffnet* net) {
-  if (gb::validate_ffnet(net) != GB_OK) return 0;
-  return 3 * (size_t)gb::round_up(gb::make_ff_image(net, 4).total, 4);  // moments + gradient scratch of multi-chunk mini-batches + weight image of wide stacks
-}
-
-int gb_ffae_fit_plan(const gb_ffnet* net, int32_t* weights_in_l2, int32_t* dz_in_l2) {
-  const int rc = gb::validate_ffnet(net);
-  if (rc != GB_OK) return rc;
-  FitArgs a{};
-  size_t smem = 0;
-  bool w_global = false;
-  if (plan_fit(net, a, w_global, smem) != GB_OK) return GB_E_SMEM;
-  if (weights_in_l2) *weights_in_l2 = w_global ? 1 : 0;
-  if (dz_in_l2) *dz_in_l2 = a.d_global;
-  return GB_OK;
-}
-
-// debug aid (not part of the public header): per-phase cycle sums of CTA 0 into a device buffer of 2*GB_MAX_LAYERS+4 int64
-// (0 gather wait, 1..L forward layers, L+1 loss, L+2.. backward phases, 2L+2 set-up, 2L+3 tail); NULL switches it off
-int gb_debug_set_fit_trace(void* dev_buf) {
-  g_fit_trace = static_cast<long long*>(dev_buf);
-  return GB_OK;
-}
-
-int gb_ffae_fit(const gb_ffnet* net, float* params, float* adam_m, float* adam_v, const gb_job* jobs, int32_t n_jobs,
-                int32_t max_rows, const float* x, const float* y, const int32_t* perm, const gb_fit_hparams* hp,
-                float* out_loss, float* out_acc, void* stream) {
+// gb_ffae_fit (with_split = false: the kernels without the held-out pass) and gb_ffae_fit_split
+int launch_fit(const gb_ffnet* net, float* params, float* adam_m, float* adam_v, const gb_job* jobs, const gb_fit_split* split,
+               int32_t n_jobs, int32_t max_rows, const float* x, const float* y, const int32_t* row_map, const int32_t* perm,
+               const gb_fit_hparams* hp, int32_t val_batch, float* out_loss, float* out_acc, float* out_val_loss, float* out_val_acc,
+               bool with_split, void* stream) {
   int rc = gb::validate_ffnet(net);
   if (rc != GB_OK) return rc;
   GB_REQUIRE(params && adam_m && adam_v && jobs && x && y && hp && out_loss, GB_E_ARG,
@@ -627,17 +637,69 @@ int gb_ffae_fit(const gb_ffnet* net, float* params, float* adam_m, float* adam_v
   a.params = params; a.adam_m = adam_m; a.adam_v = adam_v; a.jobs = jobs; a.x = x; a.y = y; a.perm = perm;
   a.out_loss = out_loss; a.out_acc = out_acc;
   a.trace = g_fit_trace;
+  a.split = split; a.row_map = row_map; a.val_batch = val_batch; a.out_val_loss = out_val_loss; a.out_val_acc = out_val_acc;
   auto launch = [&](auto kernel) -> int {
     GB_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     kernel<<<n_jobs, THREADS, smem, (cudaStream_t)stream>>>(a);
     return GB_OK;
   };
-  if (a.d_global > 0) rc = launch(ffae_fit_kernel<true, true>);
-  else if (w_global) rc = launch(ffae_fit_kernel<true, false>);
-  else rc = launch(ffae_fit_kernel<false, false>);
+  if (with_split) {
+    if (a.d_global > 0) rc = launch(ffae_fit_kernel<true, true, true>);
+    else if (w_global) rc = launch(ffae_fit_kernel<true, false, true>);
+    else rc = launch(ffae_fit_kernel<false, false, true>);
+  } else {
+    if (a.d_global > 0) rc = launch(ffae_fit_kernel<true, true>);
+    else if (w_global) rc = launch(ffae_fit_kernel<true, false>);
+    else rc = launch(ffae_fit_kernel<false, false>);
+  }
   if (rc != GB_OK) return rc;
   GB_CUDA_CHECK(cudaGetLastError());
   return GB_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+size_t gb_ffae_fit_state_stride(const gb_ffnet* net) {
+  if (gb::validate_ffnet(net) != GB_OK) return 0;
+  return 3 * (size_t)gb::round_up(gb::make_ff_image(net, 4).total, 4);  // moments + gradient scratch of multi-chunk mini-batches + weight image of wide stacks
+}
+
+int gb_ffae_fit_plan(const gb_ffnet* net, int32_t* weights_in_l2, int32_t* dz_in_l2) {
+  const int rc = gb::validate_ffnet(net);
+  if (rc != GB_OK) return rc;
+  FitArgs a{};
+  size_t smem = 0;
+  bool w_global = false;
+  if (plan_fit(net, a, w_global, smem) != GB_OK) return GB_E_SMEM;
+  if (weights_in_l2) *weights_in_l2 = w_global ? 1 : 0;
+  if (dz_in_l2) *dz_in_l2 = a.d_global;
+  return GB_OK;
+}
+
+// debug aid (not part of the public header): per-phase cycle sums of CTA 0 into a device buffer of 2*GB_MAX_LAYERS+4 int64
+// (0 gather wait, 1..L forward layers, L+1 loss, L+2.. backward phases, 2L+2 set-up, 2L+3 tail); NULL switches it off
+int gb_debug_set_fit_trace(void* dev_buf) {
+  g_fit_trace = static_cast<long long*>(dev_buf);
+  return GB_OK;
+}
+
+int gb_ffae_fit(const gb_ffnet* net, float* params, float* adam_m, float* adam_v, const gb_job* jobs, int32_t n_jobs,
+                int32_t max_rows, const float* x, const float* y, const int32_t* perm, const gb_fit_hparams* hp,
+                float* out_loss, float* out_acc, void* stream) {
+  return launch_fit(net, params, adam_m, adam_v, jobs, nullptr, n_jobs, max_rows, x, y, nullptr, perm, hp, 1, out_loss, out_acc,
+                    nullptr, nullptr, false, stream);
+}
+
+int gb_ffae_fit_split(const gb_ffnet* net, float* params, float* adam_m, float* adam_v, const gb_job* jobs,
+                      const gb_fit_split* split, int32_t n_jobs, int32_t max_rows, const float* x, const float* y,
+                      const int32_t* row_map, const int32_t* perm, const gb_fit_hparams* hp, int32_t val_batch,
+                      float* out_loss, float* out_acc, float* out_val_loss, float* out_val_acc, void* stream) {
+  GB_REQUIRE(!split || out_val_loss, GB_E_ARG, "split needs out_val_loss");
+  GB_REQUIRE(!split || val_batch >= 1, GB_E_ARG, "val_batch=%d must be >= 1", val_batch);
+  return launch_fit(net, params, adam_m, adam_v, jobs, split, n_jobs, max_rows, x, y, row_map, perm, hp, split ? val_batch : 1,
+                    out_loss, out_acc, out_val_loss, out_val_acc, true, stream);
 }
 
 }  // extern "C"

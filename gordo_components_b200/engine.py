@@ -166,20 +166,8 @@ class FFEngine:
         ``perm`` (int32 [n_jobs, epochs, max_rows]) pins the visiting order (parity tests).
         """
         torch = _torch()
-        adam = adam or {}
-        hp = _cabi.GbFitHParams()
-        hp.epochs, hp.batch_size = int(epochs), int(batch_size)
-        hp.shuffle = 2 if perm is not None else (1 if shuffle else 0)
-        hp.l1_div_batch = int(bool(l1_div_batch))
-        hp.lr, hp.beta1 = float(adam.get("lr", 1e-3)), float(adam.get("beta1", 0.9))
-        hp.beta2, hp.eps = float(adam.get("beta2", 0.999)), float(adam.get("eps", 1e-7))
-        hp.seed, hp.step0 = int(seed) & (2**64 - 1), int(step0)
-        n_slots = params.shape[0]
-        if state is None:
-            m = torch.zeros((n_slots, self.state_stride), dtype=torch.float32, device=self.device)
-            v = torch.zeros_like(m)
-        else:
-            m, v = state
+        hp = _fit_hparams(epochs, batch_size, shuffle, perm, adam, seed, l1_div_batch, step0)
+        m, v = self._fit_state(params, state)
         loss = torch.empty((n_jobs, epochs), dtype=torch.float32, device=self.device)
         acc = torch.empty((n_jobs, epochs), dtype=torch.float32, device=self.device)
         p = _cabi.ptr
@@ -187,12 +175,68 @@ class FFEngine:
                                          p(perm), C.byref(hp), p(loss), p(acc), _stream_ptr()))
         return loss, acc, (m, v)
 
+    def fit_split(self, params, jobs_dev, n_jobs: int, max_rows: int, x, y, split=None, row_map=None, val_batch: Optional[int] = None,
+                  epochs: int = 1, batch_size: int = 32, shuffle=True, perm=None, adam: Optional[Dict[str, float]] = None, seed: int = 0,
+                  l1_div_batch: bool = False, state=None, step0: int = 0):
+        """
+        ``fit`` over row *positions* with Keras' ``validation_split``, in one launch (gb_ffae_fit_split).  Job i trains on its
+        positions [0, n_rows) exactly as ``fit`` trains on its rows, and after every epoch runs the network forward over the held-out
+        positions [n_rows, n_rows + split[i].n_val) in batches of ``val_batch`` (default ``batch_size``) rows -- what Keras reports as
+        ``val_loss`` / ``val_accuracy``.  Position p reads row x_row + row_map[map_ofs + p] (x_row + p where map_ofs is -1).
+
+        ``split``: ``make_split`` records [n_jobs] (host array or device bytes), None = no held-out positions and no map.
+        ``row_map``: int32 device tensor of row indices relative to a job's x_row, shared by the jobs through map_ofs.
+        Returns (loss, accuracy, val_loss, val_accuracy, (m, v)), each [n_jobs, epochs]; val_* rows of jobs without held-out
+        positions are NaN.
+        """
+        torch = _torch()
+        hp = _fit_hparams(epochs, batch_size, shuffle, perm, adam, seed, l1_div_batch, step0)
+        m, v = self._fit_state(params, state)
+        if split is not None and isinstance(split, np.ndarray):
+            split = jobs_to_device(split, self.device)
+        out = [torch.empty((n_jobs, epochs), dtype=torch.float32, device=self.device) for _ in range(2)]
+        out += [torch.full((n_jobs, epochs), float("nan"), dtype=torch.float32, device=self.device) for _ in range(2)]
+        vb = int(val_batch if val_batch is not None else batch_size)
+        p = _cabi.ptr
+        _cabi.check(self.lib.gb_ffae_fit_split(C.byref(self.net), p(params), p(m), p(v), p(jobs_dev), p(split), int(n_jobs), int(max_rows),
+                                               p(x), p(y), p(row_map), p(perm), C.byref(hp), vb, *(p(t) for t in out), _stream_ptr()))
+        return (*out, (m, v))
+
+    def _fit_state(self, params, state):
+        """Adam (m, v) of every slot: the given pair, or zeros for a fresh fit."""
+        if state is not None:
+            return state
+        torch = _torch()
+        m = torch.zeros((params.shape[0], self.state_stride), dtype=torch.float32, device=self.device)
+        return m, torch.zeros_like(m)
+
     # ------------------------------------------------------------------ K7 / K5 / K4-alone (architecture independent)
     def minmax_fit(self, jobs_dev, n_jobs, max_rows, y, n_slots):
         return minmax_fit(jobs_dev, n_jobs, max_rows, y, self.n_out, n_slots, self.device)
 
     def thresholds(self, jobs_dev, n_jobs, max_rows, tag_unscaled, total_scaled, n_slots, window=6):
         return thresholds(jobs_dev, n_jobs, max_rows, tag_unscaled, total_scaled, self.n_out, n_slots, window, self.device)
+
+
+def _fit_hparams(epochs, batch_size, shuffle, perm, adam, seed, l1_div_batch, step0) -> "_cabi.GbFitHParams":
+    adam = adam or {}
+    hp = _cabi.GbFitHParams()
+    hp.epochs, hp.batch_size = int(epochs), int(batch_size)
+    hp.shuffle = 2 if perm is not None else (1 if shuffle else 0)
+    hp.l1_div_batch = int(bool(l1_div_batch))
+    hp.lr, hp.beta1 = float(adam.get("lr", 1e-3)), float(adam.get("beta1", 0.9))
+    hp.beta2, hp.eps = float(adam.get("beta2", 0.999)), float(adam.get("eps", 1e-7))
+    hp.seed, hp.step0 = int(seed) & (2**64 - 1), int(step0)
+    return hp
+
+
+def make_split(n_val, map_ofs=-1) -> np.ndarray:
+    """Structured array of gb_fit_split records (per job: held-out positions, offset of its row map or -1)."""
+    n_val = np.atleast_1d(np.asarray(n_val))
+    split = np.zeros(len(n_val), dtype=_cabi.SPLIT_DTYPE)
+    split["n_val"] = n_val
+    split["map_ofs"] = map_ofs
+    return split
 
 
 def minmax_fit(jobs_dev, n_jobs, max_rows, y, n_out, n_slots, device, return_minmax=False):

@@ -15,6 +15,7 @@ import time
 from typing import Dict, List, Optional, Sequence
 
 import numpy as np
+from sklearn.utils import shuffle as sk_shuffle
 
 from . import engine
 
@@ -164,7 +165,10 @@ class FleetBuild:
     """
 
     def __init__(self, eng, n_machines, n_splits, params, scale, offset, feat_thr, agg_thr, loss, acc, fold_loss, fold_feat_thr, fold_agg_thr,
-                 fold_params=None, cv_moments=None, in_scale=None, in_offset=None, fold_in_scale=None, fold_in_offset=None, steps_per_epoch=None):
+                 fold_params=None, cv_moments=None, in_scale=None, in_offset=None, fold_in_scale=None, fold_in_offset=None, steps_per_epoch=None,
+                 val_loss=None, val_acc=None, fold_val_loss=None, fold_val_acc=None):
+        # Keras validation_split: per-epoch loss / accuracy on the held-out tail ([M, epochs]; per CV fold [M, K, epochs]); None without one
+        self.val_loss, self.val_acc, self.fold_val_loss, self.fold_val_acc = val_loss, val_acc, fold_val_loss, fold_val_acc
         self.steps_per_epoch = steps_per_epoch                                 # optimizer steps per epoch of the final fit (keras History.params["steps"])
         # float64 scale_ / min_ of the MinMaxScaler in front of the network ([M, T]; per CV fold [M, K, T]); None without one
         self.in_scale, self.in_offset, self.fold_in_scale, self.fold_in_offset = in_scale, in_offset, fold_in_scale, fold_in_offset
@@ -223,6 +227,9 @@ class FleetBuild:
             spec = FFNetSpec(list(eng.dims), list(eng.acts), list(eng.l1))
             ae.model = FittedNet(spec, eng.unpack_params(self.params[m : m + 1])[0])
         hist = {"loss": [float(v) for v in self.loss[m].cpu().numpy()], "accuracy": [float(v) for v in self.acc[m].cpu().numpy()]}
+        if self.val_loss is not None:  # the keys and their order of the per-machine History
+            hist["val_loss"] = [float(v) for v in self.val_loss[m].cpu().numpy()]
+            hist["val_accuracy"] = [float(v) for v in self.val_acc[m].cpu().numpy()]
         ae._history = History(hist, {"verbose": 0, "epochs": len(hist["loss"]), "steps": self.steps_per_epoch}, list(range(len(hist["loss"]))))
         sc = self._fill_minmax(MinMaxScaler(), self.scale[m].cpu().numpy().astype(np.float64), self.offset[m].cpu().numpy().astype(np.float64), None)
         if template is not None:
@@ -275,7 +282,8 @@ def dump_fleet(fb: "FleetBuild", root: str, names: Sequence[str], tags: Optional
 
 
 def build_fleet(eng: "engine.FFEngine", x, y, rows: int, epochs: int = 1, batch_size: int = 32, n_splits: int = 3, seed: int = 0,
-                adam: Optional[Dict[str, float]] = None, shuffle: bool = True, generator=None, input_scaler: bool = False) -> FleetBuild:
+                adam: Optional[Dict[str, float]] = None, shuffle: bool = True, generator=None, input_scaler: bool = False,
+                detector_shuffle: bool = False, validation_split: float = 0.0, validation_batch_size: Optional[int] = None) -> FleetBuild:
     """
     The batched form of ``gordo build`` for one architecture bucket: for every machine the 3-fold TimeSeriesSplit
     cross-validation (fit on each prefix, thresholds from the following test block: diff.py:176-266) and the final fit on
@@ -288,6 +296,14 @@ def build_fleet(eng: "engine.FFEngine", x, y, rows: int, epochs: int = 1, batch_
     gordo's example configs, examples/config.yaml:74-81).  Inside cross validation every fold clone fits that scaler on its
     own training prefix, so every fit slot gets its own scaled copy of its machine's rows -- sklearn's float64 arithmetic on
     the exact column extrema (``gb_minmax_fit`` finds them, ``gb_affine_f64`` applies them), rounded to float32 once.
+
+    ``detector_shuffle``: ``DiffBasedAnomalyDetector(shuffle=True)``, which hands its estimator its rows in the order of
+    ``sklearn.utils.shuffle(X, y, random_state=0)`` (the final fit on all rows, every CV clone on its own prefix).  The fits read
+    the rows through that order (a row map; one per slot length, shared by every machine) instead of a shuffled copy.
+    ``validation_split``: Keras' hold-out of the estimator: of a slot's ``n`` (shuffled) rows it trains on the first
+    ``floor(n * (1 - validation_split))`` and reports the loss and accuracy of the rest after every epoch (``val_loss``,
+    ``val_accuracy``; in batches of ``validation_batch_size``, default ``batch_size``), computed inside the same fit launch.
+    The scalers still see all ``n`` rows of a slot, as the detector's and the Pipeline's do.
     """
     torch = engine._torch()
     dev = eng.device
@@ -306,13 +322,26 @@ def build_fleet(eng: "engine.FFEngine", x, y, rows: int, epochs: int = 1, batch_
         params[:, ofs:ofs + o] = 0
         ofs += o
     base = np.arange(M, dtype=np.int64) * N
+    slot_n = [N] + starts  # rows of the final fit, then of fold k
+    vsplit = float(validation_split or 0.0)
+    n_train = [int(math.floor(n * (1.0 - vsplit))) if 0.0 < vsplit < 1.0 else n for n in slot_n]  # keras' split (models.py)
+    if min(n_train) < 1:
+        raise ValueError(f"validation_split {vsplit} leaves the {min(slot_n)}-row slot without a training row")
     fit_slots = np.concatenate([np.arange(M)] + [M + k * M + np.arange(M) for k in range(K)])
-    fit_rows = np.concatenate([np.full(M, N)] + [np.full(M, starts[k]) for k in range(K)])
+    all_rows = np.repeat(slot_n, M)     # every row of a slot: what its scalers see
+    fit_rows = np.repeat(n_train, M)    # the positions its optimizer steps visit
     fit_x = np.concatenate([base] * (K + 1))
+    split = row_map = None
+    if detector_shuffle or n_train != slot_n:
+        maps = [sk_shuffle(np.arange(n), random_state=0) if detector_shuffle else None for n in slot_n]
+        map_ofs = np.cumsum([0] + slot_n[:-1]) if detector_shuffle else np.full(K + 1, -1)
+        split = engine.make_split(all_rows - fit_rows, np.repeat(map_ofs, M))
+        if detector_shuffle:
+            row_map = torch.from_numpy(np.concatenate(maps).astype(np.int32)).to(dev)
     in_scale = in_offset = None
     if input_scaler:
         S = M * (K + 1)
-        prefix_jobs = engine.jobs_to_device(engine.make_jobs(fit_slots, fit_rows, fit_x), dev)
+        prefix_jobs = engine.jobs_to_device(engine.make_jobs(fit_slots, all_rows, fit_x), dev)
         _, _, lo, hi = engine.minmax_fit(prefix_jobs, S, N, x, eng.n_in, S, dev, return_minmax=True)
         lo, span = lo.double(), hi.double() - lo.double()
         span[~(span >= 10 * np.finfo(np.float64).eps)] = 1.0  # sklearn _handle_zeros_in_scale (also catches all-NaN columns)
@@ -327,9 +356,18 @@ def build_fleet(eng: "engine.FFEngine", x, y, rows: int, epochs: int = 1, batch_
     else:
         base_of = lambda k: base  # noqa: E731
     fit_jobs = engine.jobs_to_device(engine.make_jobs(fit_slots, fit_rows, fit_x), dev)
-    loss, acc, _ = eng.fit(params, fit_jobs, len(fit_slots), N, x, y, epochs=epochs, batch_size=batch_size, shuffle=shuffle, adam=adam, seed=seed)
-    # scalers: final on all rows, fold k on its training prefix (diff.py:173 inside each CV clone)
-    scale, offset = eng.minmax_fit(fit_jobs, len(fit_slots), N, y, M * (K + 1))
+    val_loss = val_acc = None
+    if split is None:
+        loss, acc, _ = eng.fit(params, fit_jobs, len(fit_slots), N, x, y, epochs=epochs, batch_size=batch_size, shuffle=shuffle, adam=adam, seed=seed)
+    else:
+        loss, acc, val_loss, val_acc, _ = eng.fit_split(params, fit_jobs, len(fit_slots), N, x, y, split=split, row_map=row_map,
+                                                        val_batch=validation_batch_size or batch_size, epochs=epochs, batch_size=batch_size,
+                                                        shuffle=shuffle, adam=adam, seed=seed)
+        if n_train == slot_n:  # shuffled, nothing held out
+            val_loss = val_acc = None
+    # scalers: final on all rows, fold k on its training prefix (diff.py:173 inside each CV clone), held-out rows included
+    all_jobs = fit_jobs if n_train == slot_n else engine.jobs_to_device(engine.make_jobs(fit_slots, all_rows, fit_x), dev)
+    scale, offset = eng.minmax_fit(all_jobs, len(fit_slots), N, y, M * (K + 1))
     # fold scoring on the test blocks: compact output rows [(k*M + m)*test, ...)
     sc_slots = np.concatenate([M + k * M + np.arange(M) for k in range(K)])
     sc_x = np.concatenate([base_of(k) + starts[k] for k in range(K)])
@@ -344,13 +382,16 @@ def build_fleet(eng: "engine.FFEngine", x, y, rows: int, epochs: int = 1, batch_
     fold_feat = feat[M:].view(K, M, T).permute(1, 0, 2).contiguous()
     fold_agg = agg[M:].view(K, M).t().contiguous()
     E = loss.shape[1]
+    folds = lambda t: None if t is None else t[M:].view(K, M, E).permute(1, 0, 2)  # noqa: E731
     return FleetBuild(eng, M, K, params[:M].contiguous(), scale[:M].contiguous(), offset[:M].contiguous(), fold_feat[:, K - 1].contiguous(),
                       fold_agg[:, K - 1].contiguous(), loss[:M], acc[:M], loss[M:].view(K, M, E).permute(1, 0, 2), fold_feat, fold_agg,
                       fold_params=fold_params, cv_moments=moments,
                       in_scale=None if in_scale is None else in_scale[:M].contiguous(), in_offset=None if in_offset is None else in_offset[:M].contiguous(),
                       fold_in_scale=None if in_scale is None else in_scale[M:].view(K, M, -1).permute(1, 0, 2).contiguous(),
                       fold_in_offset=None if in_offset is None else in_offset[M:].view(K, M, -1).permute(1, 0, 2).contiguous(),
-                      steps_per_epoch=(N + int(batch_size) - 1) // int(batch_size))
+                      steps_per_epoch=(n_train[0] + int(batch_size) - 1) // int(batch_size),
+                      val_loss=None if val_loss is None else val_loss[:M], val_acc=None if val_acc is None else val_acc[:M],
+                      fold_val_loss=folds(val_loss), fold_val_acc=folds(val_acc))
 
 
 # ------------------------------------------------------------------------------------------------ fleet build of LSTM detectors

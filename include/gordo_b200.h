@@ -216,6 +216,26 @@ int gb_ffae_fit(const gb_ffnet* net, float* params, float* adam_m, float* adam_v
                 int32_t n_jobs, int32_t max_rows, const float* x, const float* y, const int32_t* perm,
                 const gb_fit_hparams* hp, float* out_loss, float* out_acc, void* stream);
 
+/* gb_ffae_fit with Keras' validation_split and a row map (a detector that shuffles its rows before the fit).  A job's rows are
+ * *positions*: the job trains on positions [0, n_rows) exactly as gb_ffae_fit trains on its rows (sequential order, keyed
+ * permutation or `perm` permute positions), and position p reads row x_row + row_map[map_ofs + p] of x and y
+ * (x_row + p when map_ofs is -1 or row_map is NULL).  After the last optimizer step of every epoch the job runs the network
+ * forward over the held-out positions [n_rows, n_rows + n_val), in order, in batches of val_batch rows, and writes their
+ * loss and accuracy, accumulated as the training ones are, to out_val_loss / out_val_acc [n_jobs][epochs]; weights and
+ * Adam state are not touched by that pass.  Rows of jobs with n_val 0 are left as they are.  split: [n_jobs] device array,
+ * or NULL (no job has held-out positions or a map); several jobs may share one map.  Without a map and held-out
+ * positions, the results are those of gb_ffae_fit; with a map, those of gb_ffae_fit on the gathered copy x[map], y[map]. */
+typedef struct gb_fit_split {
+  int32_t n_val;     /* held-out positions after the job's n_rows training positions */
+  int32_t reserved;
+  int64_t map_ofs;   /* position p of the job reads row x_row + row_map[map_ofs + p]; -1 = row x_row + p */
+} gb_fit_split;
+
+int gb_ffae_fit_split(const gb_ffnet* net, float* params, float* adam_m, float* adam_v, const gb_job* jobs,
+                      const gb_fit_split* split, int32_t n_jobs, int32_t max_rows, const float* x, const float* y,
+                      const int32_t* row_map, const int32_t* perm, const gb_fit_hparams* hp, int32_t val_batch,
+                      float* out_loss, float* out_acc, float* out_val_loss, float* out_val_acc, void* stream);
+
 /* The memory plan gb_ffae_fit uses for this architecture (host only, no device needed).  The first of five that fits in
  * 227 KB of shared memory: everything in shared memory; the weight image in the slot's L2-resident state area
  * (*weights_in_l2 = 1); then one, two or three of the three dz buffers there as well (*dz_in_l2).  GB_E_SMEM if none fits
