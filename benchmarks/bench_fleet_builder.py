@@ -8,11 +8,16 @@ number a `gordo build` user sees.
     python benchmarks/bench_fleet_builder.py [--machines 125] [--rows 10000] [--tags 64] [--epochs 10] [--scaled] [--single 3]
     python benchmarks/bench_fleet_builder.py --lstm [--lookback 24] --machines 16 --rows 2000 --tags 16 --epochs 1 --single 16
     python benchmarks/bench_fleet_builder.py --example-config --machines 125 --rows 10000 --tags 64 --epochs 10 --single 3
+    python benchmarks/bench_fleet_builder.py --early-stopping --machines 125 --rows 10000 --tags 64 --epochs 100 --single 1
 
 ``--lstm`` builds DiffBasedAnomalyDetector(KerasLSTMAutoEncoder(lstm_hourglass)) machines instead (batched by
 fleet.build_lstm_fleet).  ``--example-config`` builds the model of gordo's examples/model-configuration.yaml:
 DiffBasedAnomalyDetector(shuffle=True) around Pipeline([MinMaxScaler, KerasAutoEncoder(feedforward_hourglass, compression_factor
-0.6, 1 encoding layer, batch 128, validation_split 0.1)]) under TimeSeriesSplit(5).  Measured numbers and the card they were measured on are in DESIGN.md §7.
+0.6, 1 encoding layer, batch 128, validation_split 0.1)]) under TimeSeriesSplit(5).  ``--early-stopping`` adds the callback of
+the reference's production definition to that model, EarlyStopping(monitor=val_loss, patience=10, restore_best_weights=True), and
+also reports the epochs each fit ran (min / median / max over all final and CV-fold fits) and the time of the bucket's fit
+launch with the rule against the same launch with patience = epochs (never stops), alternating, CUDA events around the launch
+after a warm-up.  Measured numbers and the card they were measured on are in DESIGN.md §7.
 """
 import argparse, json, os, sys, tempfile, time
 sys.path.insert(0, os.path.abspath(os.path.join(os.path.dirname(__file__), "..")))
@@ -40,6 +45,9 @@ def main():
     ap.add_argument("--lstm", action="store_true", help="LSTM autoencoder machines (lstm_hourglass) instead of the feed-forward hourglass")
     ap.add_argument("--lookback", type=int, default=24, help="lookback_window of the LSTM machines")
     ap.add_argument("--example-config", action="store_true", help="the model and evaluation of gordo's examples/model-configuration.yaml")
+    ap.add_argument("--early-stopping", action="store_true", help="--example-config with EarlyStopping(val_loss, patience=10, restore_best_weights)")
+    ap.add_argument("--launch-runs", type=int, default=3, help="--early-stopping: timed fit launches of each kind")
+    ap.add_argument("--min-delta", type=float, default=0.0, help="--early-stopping: the callback's min_delta (the reference's definition has none)")
     a = ap.parse_args()
     import numpy as np
     import pandas as pd
@@ -55,10 +63,13 @@ def main():
     base = {"sklearn.pipeline.Pipeline": {"steps": ["sklearn.preprocessing.MinMaxScaler", ae]}} if a.scaled else ae
     model = {"gordo.machine.model.anomaly.diff.DiffBasedAnomalyDetector": {"base_estimator": base}}
     evaluation, n_splits = {}, 3
-    if a.example_config:
+    stopping = {"monitor": "val_loss", "patience": 10, "restore_best_weights": True, "min_delta": a.min_delta}
+    if a.example_config or a.early_stopping:
         ae = {"gordo.machine.model.models.KerasAutoEncoder": {
             "batch_size": 128, "compression_factor": 0.6, "encoding_layers": 1, "epochs": a.epochs, "func": "tanh", "kind": "feedforward_hourglass",
             "loss": "mse", "optimizer": "Adam", "out_func": "linear", "validation_split": 0.1}}
+        if a.early_stopping:
+            ae["gordo.machine.model.models.KerasAutoEncoder"]["callbacks"] = [{"tensorflow.keras.callbacks.EarlyStopping": stopping}]
         model = {"gordo.machine.model.anomaly.diff.DiffBasedAnomalyDetector": {
             "base_estimator": {"sklearn.pipeline.Pipeline": {"steps": ["sklearn.preprocessing.MinMaxScaler", ae]}},
             "scaler": "sklearn.preprocessing.MinMaxScaler", "shuffle": True, "smoothing_method": "smm"}}
@@ -72,11 +83,11 @@ def main():
         frame = pd.DataFrame(values.astype(np.float32), index=idx, columns=[f"tag-{i}" for i in range(a.tags)])
         machines.append({"name": f"machine-{m}", "model": model, "dataset": {"X": frame, "y": frame}, "evaluation": evaluation})
 
-    builder.FleetModelBuilder(machines[:2]).build()  # warm-up: library load, first launches
+    builder.FleetModelBuilder(machines[:2], early_stopping=a.early_stopping).build()  # warm-up: library load, first launches
     torch.cuda.synchronize()
     with tempfile.TemporaryDirectory() as out:
         t0 = time.perf_counter()
-        results = builder.FleetModelBuilder(machines).build(out)
+        results = builder.FleetModelBuilder(machines, early_stopping=a.early_stopping).build(out)
         torch.cuda.synchronize()
         fleet_s = time.perf_counter() - t0
         size = sum(os.path.getsize(os.path.join(out, m["name"], f)) for _, m in results for f in ("model.pkl", "metadata.json"))
@@ -89,16 +100,70 @@ def main():
         single_s = (time.perf_counter() - t0) / a.single
     scores = results[0][1]["metadata"]["build_metadata"]["model"]["cross_validation"]["scores"]
     net = f"LSTM hourglass (lookback {a.lookback})" if a.lstm else "hourglass"
-    if a.example_config:
+    if a.example_config or a.early_stopping:
         net = "hourglass (compression 0.6, 1 encoding layer, batch 128, validation_split 0.1) in a shuffling detector"
-    print(json.dumps({
+    if a.early_stopping:
+        net += f", EarlyStopping(val_loss, patience 10, min_delta {a.min_delta:g}, restore_best_weights)"
+    out = {
         "gpu": torch.cuda.get_device_name(0), "power_limit_w": _power_limit(),
-        "workload": f"{a.machines} machines x {a.tags}-tag {net}{' behind MinMaxScaler' if a.scaled or a.example_config else ''}, {a.rows} rows, {a.epochs} epochs: "
-                    f"definition -> {n_splits}-fold CV + fit + thresholds + scores metadata -> model.pkl/metadata.json",
+        "workload": f"{a.machines} machines x {a.tags}-tag {net}{' behind MinMaxScaler' if a.scaled or a.example_config or a.early_stopping else ''}, "
+                    f"{a.rows} rows, {a.epochs} epochs: definition -> {n_splits}-fold CV + fit + thresholds + scores metadata -> model.pkl/metadata.json",
         "fleet_builder_s": fleet_s, "machines_per_s": a.machines / fleet_s, "bytes_written": size,
         "model_builder_s_per_machine": single_s, "speedup_per_machine": None if single_s is None else single_s / (fleet_s / a.machines),
         "r2_fold_mean_machine_0": scores["r2-score"]["fold-mean"],
-    }))
+    }
+    if a.early_stopping:
+        out.update(_stop_launches(a, machines, stopping))
+    print(json.dumps(out))
+
+
+def _stop_launches(a, machines, stopping):
+    """
+    The bucket's fit launch (build_fleet as FleetModelBuilder calls it) with the EarlyStopping rule, against the same launch with
+    patience = epochs, which never stops: CUDA events around the fit launch alone, alternating, after one warm-up of each.
+    """
+    import numpy as np
+    import torch
+
+    from gordo_components_b200 import engine, fleet
+    from gordo_components_b200.machine.model.models import EarlyStopping
+    from gordo_components_b200.machine.model.factories.feedforward_autoencoder import feedforward_hourglass
+
+    class TimedEngine:  # the engine, with CUDA events around its fit launch
+        def __init__(self, eng):
+            self.eng, self.ms = eng, None
+
+        def __getattr__(self, name):
+            return getattr(self.eng, name)
+
+        def fit_split(self, *args, **kw):
+            ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
+            ev[0].record()
+            res = self.eng.fit_split(*args, **kw)
+            ev[1].record()
+            torch.cuda.synchronize()
+            self.ms = ev[0].elapsed_time(ev[1])
+            return res
+
+    spec = feedforward_hourglass(n_features=a.tags, compression_factor=0.6, encoding_layers=1, func="tanh", out_func="linear")
+    eng = TimedEngine(engine.ff_engine_for(spec))
+    x = engine.to_device_f32(np.concatenate([m["dataset"]["X"].values for m in machines]), eng.device)
+    never = dict(stopping, patience=a.epochs)
+
+    def launch(rule):
+        fb = fleet.build_fleet(eng, x, x, a.rows, epochs=a.epochs, batch_size=128, n_splits=5, adam=spec.adam, input_scaler=True,
+                               detector_shuffle=True, validation_split=0.1, early_stopping=EarlyStopping(**rule))
+        return eng.ms, fb
+
+    launch(stopping), launch(never)  # warm-up
+    rule_ms, never_ms = [], []
+    for _ in range(a.launch_runs):
+        ms, fb = launch(stopping)
+        rule_ms.append(ms)
+        never_ms.append(launch(never)[0])
+    ran = torch.cat([fb.epochs_run.flatten(), fb.fold_epochs_run.flatten()]).cpu().numpy()
+    return {"epochs_run_min": int(ran.min()), "epochs_run_median": float(np.median(ran)), "epochs_run_max": int(ran.max()),
+            "fit_slots": int(ran.size), "fit_launch_ms_with_rule": rule_ms, "fit_launch_ms_never_stopping": never_ms}
 
 
 if __name__ == "__main__":

@@ -7,13 +7,16 @@ definition -> cross validation with the evaluation metrics -> final fit -> offse
 ``FleetModelBuilder`` is where the batched kernels pay off: machines whose definition is the canonical
 ``DiffBasedAnomalyDetector(base_estimator=KerasAutoEncoder(<feed-forward kind>), scaler=MinMaxScaler())`` -- the network bare or
 behind one ``MinMaxScaler`` in a Pipeline, as in gordo's example configs -- are bucketed by architecture and training length, and every bucket is built by ``fleet.build_fleet`` -- all final fits and all CV folds
-in one ``gb_ffae_fit`` launch, fold scoring / thresholds / scaler statistics / metric moments one launch each.  The LSTM form
+in one ``gb_ffae_fit`` launch, fold scoring / thresholds / scaler statistics / metric moments one launch each.  With
+``FleetModelBuilder(early_stopping=True)`` an estimator with one Keras ``EarlyStopping`` callback on a metric its fit reports
+(loss, accuracy, and their ``val_*`` forms with a ``validation_split``) is batched as well: every fit applies the rule inside the
+launch (``gb_ffae_fit_stop``), and machines that differ only in the callback's parameters share a bucket.  The LSTM form
 of the same definition (``KerasLSTMAutoEncoder`` / ``KerasLSTMForecast``, ``_canonical_lstm``) is bucketed by architecture,
 lookback, lookahead and training length and built by ``fleet.build_lstm_fleet``: all fits as jobs of ``gb_lstm_fit`` (in
 chunks that fit a workspace budget), every fold model's test block in one LSTM inference launch, float64 scoring.  The
 cross-validation ``scores`` block of the metadata is then assembled on the host from ``gb_cv_moments``' five sums per
-(fold, tag).  Any other definition (other transformers in a Pipeline, LSTM fits with callbacks, K-fold detectors, custom
-metrics ...) goes through ``ModelBuilder``: one machine at a time, still on the GPU through the estimators' own fit / predict.
+(fold, tag).  Any other definition (other transformers in a Pipeline, callbacks unless batched as above, LSTM fits with
+callbacks, K-fold detectors, custom metrics ...) goes through ``ModelBuilder``: one machine at a time, still on the GPU through the estimators' own fit / predict.
 
 Machines are plain dicts in the layout of ``Machine.to_dict()`` (gordo/machine/machine.py:226-246): ``name``, ``model`` (a
 definition), ``dataset``, and optionally ``project_name``, ``evaluation``, ``metadata``, ``runtime``.  ``dataset`` is
@@ -321,9 +324,10 @@ class _Canonical:
     """What ``FleetModelBuilder`` needs to know about a machine that can take the batched path."""
 
     def __init__(self, index, machine, model, spec, X, y, dataset_meta, query_sec, fit, n_splits, evaluation, input_scaler,
-                 split=(False, 0.0, None)):
+                 split=(False, 0.0, None), early_stopping=None):
         self.index, self.machine, self.model, self.spec, self.input_scaler = index, machine, model, spec, input_scaler
         self.split = split  # (detector shuffle, keras validation_split, validation batch size or None without a split)
+        self.early_stopping = early_stopping  # the estimator's one EarlyStopping callback, or None
         self.X, self.y, self.dataset_meta, self.query_sec = X, y, dataset_meta, query_sec
         self.fit, self.n_splits, self.evaluation = fit, n_splits, evaluation
 
@@ -331,18 +335,22 @@ class _Canonical:
         s = self.spec
         return (tuple(s.dims), tuple(s.acts), tuple(float(v) for v in s.l1), tuple(sorted(s.adam.items())), tuple(s.metrics),
                 len(self.X), self.fit["epochs"], self.fit["batch_size"], self.fit["shuffle"], self.n_splits, int(self.evaluation.get("seed", 0)),
-                self.split, self.input_scaler)
+                self.split, self.early_stopping is not None, self.input_scaler)  # EarlyStopping's parameters are per-job records
 
 
 def _default_minmax(scaler) -> bool:
     return type(scaler) is MinMaxScaler and tuple(scaler.feature_range) == (0, 1) and not getattr(scaler, "clip", False)
 
 
-def _canonical(index, machine) -> Optional[_Canonical]:
-    """The machine as a candidate for the batched path, or ``None`` with the reason logged."""
+def _canonical(index, machine, early_stopping: bool = False) -> Optional[_Canonical]:
+    """
+    The machine as a candidate for the batched path, or ``None`` with the reason logged.  ``early_stopping``: also take an
+    estimator with one Keras ``EarlyStopping`` callback on a metric its fit reports (``FleetModelBuilder(early_stopping=True)``);
+    without it any callback sends the machine to ``ModelBuilder``.
+    """
     from .machine.model.anomaly.diff import DiffBasedAnomalyDetector
     from .machine.model.factories.specs import FFNetSpec
-    from .machine.model.models import KerasAutoEncoder
+    from .machine.model.models import KerasAutoEncoder, build_callbacks
 
     def no(reason):
         logger.info("machine %s takes the per-machine path: %s", machine["name"], reason)
@@ -373,8 +381,16 @@ def _canonical(index, machine) -> Optional[_Canonical]:
     if type(ae) is not KerasAutoEncoder:
         return no("base_estimator is not a KerasAutoEncoder, bare or behind one default MinMaxScaler")
     fit_args = ae.extract_supported_fit_args(ae.kwargs)
+    stopping = None
     if fit_args.get("callbacks"):
-        return no("callbacks need the per-epoch loop")
+        if not early_stopping:
+            return no("callbacks need the per-epoch loop (FleetModelBuilder(early_stopping=True) batches one EarlyStopping)")
+        definitions = fit_args["callbacks"]
+        definitions = list(definitions) if isinstance(definitions, (list, tuple)) else [definitions]
+        callbacks = build_callbacks(definitions)
+        if len(definitions) != 1 or len(callbacks) != 1:  # several callbacks, or one the fit loop does not know
+            return no("callbacks other than one EarlyStopping need the per-epoch loop")
+        stopping = callbacks[0]
     vsplit = float(fit_args.get("validation_split") or 0.0)
     if vsplit and not 0.0 < vsplit < 1.0:
         return no(f"validation_split {vsplit} is outside (0, 1)")
@@ -391,9 +407,16 @@ def _canonical(index, machine) -> Optional[_Canonical]:
         return no("too few rows for the CV folds")
     if vsplit and math.floor((len(X) - split_obj.n_splits * test) * (1.0 - vsplit)) < 1:  # the smallest fold: keras' split (models.py)
         return no(f"validation_split {vsplit} leaves the first CV fold without a training row")
+    if stopping is not None:
+        available = {"loss"} | ({"accuracy"} if "accuracy" in spec.metrics else set())
+        if vsplit:
+            available |= {"val_" + k for k in available}
+        if stopping.monitor not in available:
+            return no(f"EarlyStopping monitors {stopping.monitor!r}, which this fit does not report")
     fit = {"epochs": int(fit_args.get("epochs", 1)), "batch_size": int(fit_args.get("batch_size") or 32), "shuffle": bool(fit_args.get("shuffle", True))}
     split = (bool(model.shuffle), vsplit, int(fit_args.get("validation_batch_size") or fit["batch_size"]) if vsplit else None)
-    return _Canonical(index, machine, model, spec, X, y, dataset_meta, query_sec, fit, split_obj.n_splits, evaluation, input_scaler, split)
+    return _Canonical(index, machine, model, spec, X, y, dataset_meta, query_sec, fit, split_obj.n_splits, evaluation, input_scaler, split,
+                      stopping)
 
 
 class _CanonicalLSTM(_Canonical):
@@ -490,9 +513,15 @@ class FleetModelBuilder:
     Build every machine of a project: ``FleetModelBuilder(machines).build(output_dir)`` -> ``[(model, machine_dict), ...]`` in
     input order, each written to ``<output_dir>/<name>/`` when ``output_dir`` is given.  Results per machine are what
     ``ModelBuilder`` gives (same detector attributes and metadata keys); only the launch count differs.
+
+    ``early_stopping``: also batch feed-forward machines whose estimator has one Keras ``EarlyStopping`` callback on a metric its
+    fit reports (``loss``, ``accuracy``, their ``val_*`` forms with a ``validation_split``) -- the reference's production
+    definition.  Every fit then applies the rule inside the fit launch (``fleet.build_fleet(early_stopping=...)``).  Off by
+    default: such machines then build through ``ModelBuilder``, one epoch launch at a time, as they always have.
     """
 
-    def __init__(self, machines: Sequence):
+    def __init__(self, machines: Sequence, early_stopping: bool = False):
+        self.early_stopping = bool(early_stopping)
         self.machines = [_machine_dict(m) for m in machines]
         names = [m["name"] for m in self.machines]
         if len(set(names)) != len(names):
@@ -505,13 +534,13 @@ class FleetModelBuilder:
         """
         from . import fleet
 
-        return FleetModelBuilder([self.machines[i] for i in fleet.partition(len(self.machines), world)[rank]])
+        return FleetModelBuilder([self.machines[i] for i in fleet.partition(len(self.machines), world)[rank]], early_stopping=self.early_stopping)
 
     def build(self, output_dir: Optional[str] = None) -> List[Tuple[Any, dict]]:
         results: List[Optional[Tuple[Any, dict]]] = [None] * len(self.machines)
         buckets: Dict[tuple, List[_Canonical]] = {}
         for i, machine in enumerate(self.machines):
-            c = _canonical_lstm(i, machine) if _is_lstm_definition(machine) else _canonical(i, machine)
+            c = _canonical_lstm(i, machine) if _is_lstm_definition(machine) else _canonical(i, machine, early_stopping=self.early_stopping)
             if c is None:
                 results[i] = ModelBuilder(machine).build()
             else:
@@ -546,7 +575,8 @@ class FleetModelBuilder:
         fb = fleet.build_fleet(eng, xd, yd, rows, epochs=first.fit["epochs"], batch_size=first.fit["batch_size"], n_splits=K,
                                seed=int(first.evaluation.get("seed", 0)), adam=first.spec.adam, shuffle=first.fit["shuffle"],
                                input_scaler=first.input_scaler, detector_shuffle=first.split[0], validation_split=first.split[1],
-                               validation_batch_size=first.split[2])
+                               validation_batch_size=first.split[2],
+                               early_stopping=None if first.early_stopping is None else [c.early_stopping for c in members])
         moments = fb.cv_moments.cpu().numpy()
         scale = fb.scale.cpu().numpy().astype(np.float64)
         engine._torch().cuda.synchronize()
@@ -726,14 +756,15 @@ def machines_from_config(config, project_name: str = "local-build", datasets=Non
     return machines
 
 
-def local_build(config_str, datasets=None, batched: bool = True):
+def local_build(config_str, datasets=None, batched: bool = True, early_stopping: bool = False):
     """
     Build the model(s) of a bare gordo config locally and yield ``(model, machine)`` per machine, in config order
-    (gordo/builder/local_build.py:15-80).  ``batched=False`` builds one machine at a time like the reference does.
+    (gordo/builder/local_build.py:15-80).  ``batched=False`` builds one machine at a time like the reference does;
+    ``early_stopping`` is ``FleetModelBuilder``'s.
     """
     machines = machines_from_config(config_str, datasets=datasets)
     if batched:
-        yield from FleetModelBuilder(machines).build()
+        yield from FleetModelBuilder(machines, early_stopping=early_stopping).build()
     else:
         for machine in machines:
             yield ModelBuilder(machine).build()

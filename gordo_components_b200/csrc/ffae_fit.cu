@@ -16,6 +16,7 @@
 // The two products with the batch rows as the outer dimension (a.W and dz.W^T) give a lane four rows and a quarter of the reduction
 // index (4x4 register tile, reduce-scatter over the four quarters); the weight gradient gives a thread a 4x2 block of W.
 #include <cuda_pipeline.h>
+#include <math_constants.h>
 #include "gb_common.cuh"
 
 namespace {
@@ -50,6 +51,10 @@ struct FitArgs {
   const int32_t* row_map;
   int val_batch;
   float *out_val_loss, *out_val_acc;
+  // gb_ffae_fit_stop only (appended too)
+  const gb_fit_stop* stop;  // per job: the EarlyStopping rule; NULL = none
+  float* best_params;       // [n_slots][pstride]: the snapshots
+  int32_t *out_epochs, *out_best_epoch;
 };
 
 __device__ __forceinline__ uint32_t mix32(uint32_t h) {
@@ -120,7 +125,11 @@ __device__ __forceinline__ void quarter_reduce(const float (&acc)[4][4], int lan
 // forward-only mini-batches of val_batch rows over the held-out positions [n_rows, n_rows + n_val), in order, whose loss and
 // accuracy are the epoch's validation statistics.  Position p reads row x_row + row_map[map_ofs + p] (x_row + p without a map).
 // The held-out batches are more chunks of the same visiting order, so the cp.async prefetch runs across them as well.
-template <bool WG, bool DG, bool SPLIT = false>  // DG: some dz buffers live in global memory too (kept apart so that the usual case addresses them as shared memory)
+// STOP (gb_ffae_fit_stop, with SPLIT): Keras' EarlyStopping at the end of every epoch.  Thread 0 applies the job's rule to the
+// monitored history entry it has just written and posts the decision (snapshot, stop) in s_red, free between two epoch_stats;
+// one barrier shares it.  A snapshot is the weight image written to best_params in canonical layout; a job that stops drains
+// its cp.async prefetch and leaves, so its SM takes the next job of the launch.
+template <bool WG, bool DG, bool SPLIT = false, bool STOP = false>  // DG: some dz buffers live in global memory too (kept apart so that the usual case addresses them as shared memory)
 __global__ void __launch_bounds__(THREADS, 1) ffae_fit_kernel(const FitArgs a) {
   extern __shared__ __align__(16) float smem[];
   __shared__ float s_red[3][NWARPS];
@@ -131,7 +140,11 @@ __global__ void __launch_bounds__(THREADS, 1) ffae_fit_kernel(const FitArgs a) {
   const int job_id = blockIdx.x;
   const gb_job job = a.jobs[job_id];
   const int n = job.n_rows;
-  if (n <= 0) return;
+  const bool stopping = STOP && a.stop != nullptr;
+  if (n <= 0) {
+    if (stopping && threadIdx.x == 0) { a.out_epochs[job_id] = 0; a.out_best_epoch[job_id] = -1; }
+    return;
+  }
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int L = a.net.n_layers, n_in = a.n_in, n_out = a.n_out;
   const bool tracing = a.trace != nullptr && blockIdx.x == 0 && tid == 0;
@@ -266,6 +279,28 @@ __global__ void __launch_bounds__(THREADS, 1) ffae_fit_kernel(const FitArgs a) {
     }
     __syncthreads();
   };
+
+  // ---- the weight image in canonical layout (the slot's parameter vector), by every thread -----------------
+  auto write_image = [&](float* dst) {
+    for (int l = 0; l < L; ++l) {
+      const int K = a.net.dims[l], N = a.net.dims[l + 1], Np = a.im.np[l];
+      float* Wg = dst + a.im.pofs[l];
+      const float* src = sW + a.im.wofs[l];
+      for (int idx = tid; idx < K * N; idx += THREADS) {
+        const int k = idx / N, nn = idx - k * N;
+        Wg[idx] = src[k * Np + nn];
+      }
+      for (int nn = tid; nn < N; nn += THREADS) Wg[K * N + nn] = sW[a.im.bofs[l] + nn];
+    }
+  };
+
+  // ---- EarlyStopping (keras 3 EarlyStopping.on_epoch_end, models.py EarlyStopping.update) ------------------------------
+  // Thread 0 owns the state, three registers across the epoch loop: the record is re-read from global memory at each epoch's
+  // end.  `best` is +-inf or a monitored float32 value, so a float holds it exactly; with restore_best a snapshot exists once
+  // an epoch has counted, i.e. when best_epoch >= 0.
+  float best = stopping && a.stop[job_id].mode > 0 ? CUDART_INF_F : -CUDART_INF_F;
+  int wait = 0, best_epoch = -1;
+  if (stopping && tid == 0) a.out_epochs[job_id] = a.hp.epochs;  // rewritten by an early stop
 
   for (int e = 0; e < a.hp.epochs; ++e) {
     float acc_sq = 0.f, acc_reg = 0.f, acc_hit = 0.f;
@@ -537,18 +572,59 @@ __global__ void __launch_bounds__(THREADS, 1) ffae_fit_kernel(const FitArgs a) {
     }
     if (vsteps > 0) epoch_stats(acc_sq, acc_reg, acc_hit, a.out_val_loss, a.out_val_acc, nv, e);
     else epoch_stats(acc_sq, acc_reg, acc_hit, a.out_loss, a.out_acc, n, e);
+    if (stopping) {
+      // the history entries of epoch e are written (by thread 0, after the last barrier of epoch_stats): apply the rule to the
+      // monitored one, widened to double as Python compares it.  Bit 0 of the decision: snapshot; bit 1: stop.
+      if (tid == 0) {
+        const gb_fit_stop rule = a.stop[job_id];
+        const float* monitored = rule.monitor == 0 ? a.out_loss : rule.monitor == 1 ? a.out_acc
+                               : vsteps == 0 ? nullptr : rule.monitor == 2 ? a.out_val_loss : rule.monitor == 3 ? a.out_val_acc : nullptr;
+        auto improves = [&](double v, double ref) -> bool {
+          return rule.mode > 0 ? v + rule.min_delta < ref : v - rule.min_delta > ref;
+        };
+        int act = 0;
+        if (monitored != nullptr && e >= rule.start_from_epoch) {
+          const float v = monitored[(long)job_id * a.hp.epochs + e];
+          if (rule.restore_best && best_epoch < 0) { act |= 1; best_epoch = e; }
+          ++wait;
+          if (improves(v, best)) {
+            best = v;
+            best_epoch = e;
+            if (rule.restore_best) act |= 1;
+            if (!rule.has_baseline || improves(v, rule.baseline)) wait = 0;
+          } else if (wait >= rule.patience && e > 0) {
+            act |= 2;
+          }
+        }
+        if (act & 2) { a.out_epochs[job_id] = e + 1; }
+        reinterpret_cast<volatile int*>(s_red[0])[0] = act;
+      }
+      __syncthreads();
+      const int act = reinterpret_cast<volatile int*>(s_red[0])[0];
+      if (act & 1) write_image(a.best_params + (long)job.slot * a.pstride);
+      if (act & 2) {
+        __pipeline_wait_prior(0);  // the next epoch's first chunk is in flight
+        break;
+      }
+    }
   }
 
-  // ---- trained weights back to the canonical layout ------------------------------------------------------
-  for (int l = 0; l < L; ++l) {
-    const int K = a.net.dims[l], N = a.net.dims[l + 1], Np = a.im.np[l];
-    float* Wg = P + a.im.pofs[l];
-    const float* src = sW + a.im.wofs[l];
-    for (int idx = tid; idx < K * N; idx += THREADS) {
-      const int k = idx / N, nn = idx - k * N;
-      Wg[idx] = src[k * Np + nn];
+  // ---- trained weights (or, with restore_best, the snapshot) back to the canonical layout ------------------------------
+  if (stopping) {
+    bool restore = false;
+    if (tid == 0) {
+      restore = a.stop[job_id].restore_best && best_epoch >= 0;
+      a.out_best_epoch[job_id] = best_epoch;
     }
-    for (int nn = tid; nn < N; nn += THREADS) Wg[K * N + nn] = sW[a.im.bofs[l] + nn];
+    if (__syncthreads_or(restore)) {  // the snapshot's threads are not this copy's
+      const float* B = a.best_params + (long)job.slot * a.pstride;
+      const int count = a.im.pofs[L - 1] + a.net.dims[L - 1] * a.net.dims[L] + a.net.dims[L];
+      for (int i = tid; i < count; i += THREADS) P[i] = B[i];
+    } else {
+      write_image(P);
+    }
+  } else {
+    write_image(P);
   }
   if (tracing) {
     stamp(2 * L + 3);  // epoch statistics + write-back
@@ -600,11 +676,14 @@ int plan_fit(const gb_ffnet* net, FitArgs& a, bool& w_global, size_t& smem) {
   return GB_OK;
 }
 
-// gb_ffae_fit (with_split = false: the kernels without the held-out pass) and gb_ffae_fit_split
+enum FitEntry { FIT_PLAIN, FIT_SPLIT, FIT_STOP };
+
+// gb_ffae_fit (FIT_PLAIN: the kernels without the held-out pass), gb_ffae_fit_split and gb_ffae_fit_stop
 int launch_fit(const gb_ffnet* net, float* params, float* adam_m, float* adam_v, const gb_job* jobs, const gb_fit_split* split,
                int32_t n_jobs, int32_t max_rows, const float* x, const float* y, const int32_t* row_map, const int32_t* perm,
                const gb_fit_hparams* hp, int32_t val_batch, float* out_loss, float* out_acc, float* out_val_loss, float* out_val_acc,
-               bool with_split, void* stream) {
+               const gb_fit_stop* stop, float* best_params, int32_t* out_epochs, int32_t* out_best_epoch, FitEntry entry,
+               void* stream) {
   int rc = gb::validate_ffnet(net);
   if (rc != GB_OK) return rc;
   GB_REQUIRE(params && adam_m && adam_v && jobs && x && y && hp && out_loss, GB_E_ARG,
@@ -638,12 +717,17 @@ int launch_fit(const gb_ffnet* net, float* params, float* adam_m, float* adam_v,
   a.out_loss = out_loss; a.out_acc = out_acc;
   a.trace = g_fit_trace;
   a.split = split; a.row_map = row_map; a.val_batch = val_batch; a.out_val_loss = out_val_loss; a.out_val_acc = out_val_acc;
+  a.stop = stop; a.best_params = best_params; a.out_epochs = out_epochs; a.out_best_epoch = out_best_epoch;
   auto launch = [&](auto kernel) -> int {
     GB_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     kernel<<<n_jobs, THREADS, smem, (cudaStream_t)stream>>>(a);
     return GB_OK;
   };
-  if (with_split) {
+  if (entry == FIT_STOP) {
+    if (a.d_global > 0) rc = launch(ffae_fit_kernel<true, true, true, true>);
+    else if (w_global) rc = launch(ffae_fit_kernel<true, false, true, true>);
+    else rc = launch(ffae_fit_kernel<false, false, true, true>);
+  } else if (entry == FIT_SPLIT) {
     if (a.d_global > 0) rc = launch(ffae_fit_kernel<true, true, true>);
     else if (w_global) rc = launch(ffae_fit_kernel<true, false, true>);
     else rc = launch(ffae_fit_kernel<false, false, true>);
@@ -689,7 +773,7 @@ int gb_ffae_fit(const gb_ffnet* net, float* params, float* adam_m, float* adam_v
                 int32_t max_rows, const float* x, const float* y, const int32_t* perm, const gb_fit_hparams* hp,
                 float* out_loss, float* out_acc, void* stream) {
   return launch_fit(net, params, adam_m, adam_v, jobs, nullptr, n_jobs, max_rows, x, y, nullptr, perm, hp, 1, out_loss, out_acc,
-                    nullptr, nullptr, false, stream);
+                    nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, FIT_PLAIN, stream);
 }
 
 int gb_ffae_fit_split(const gb_ffnet* net, float* params, float* adam_m, float* adam_v, const gb_job* jobs,
@@ -699,7 +783,21 @@ int gb_ffae_fit_split(const gb_ffnet* net, float* params, float* adam_m, float* 
   GB_REQUIRE(!split || out_val_loss, GB_E_ARG, "split needs out_val_loss");
   GB_REQUIRE(!split || val_batch >= 1, GB_E_ARG, "val_batch=%d must be >= 1", val_batch);
   return launch_fit(net, params, adam_m, adam_v, jobs, split, n_jobs, max_rows, x, y, row_map, perm, hp, split ? val_batch : 1,
-                    out_loss, out_acc, out_val_loss, out_val_acc, true, stream);
+                    out_loss, out_acc, out_val_loss, out_val_acc, nullptr, nullptr, nullptr, nullptr, FIT_SPLIT, stream);
+}
+
+int gb_ffae_fit_stop(const gb_ffnet* net, float* params, float* adam_m, float* adam_v, const gb_job* jobs,
+                     const gb_fit_split* split, int32_t n_jobs, int32_t max_rows, const float* x, const float* y,
+                     const int32_t* row_map, const int32_t* perm, const gb_fit_hparams* hp, int32_t val_batch,
+                     float* out_loss, float* out_acc, float* out_val_loss, float* out_val_acc, const gb_fit_stop* stop,
+                     float* best_params, int32_t* out_epochs, int32_t* out_best_epoch, void* stream) {
+  GB_REQUIRE(!split || out_val_loss, GB_E_ARG, "split needs out_val_loss");
+  GB_REQUIRE(!split || val_batch >= 1, GB_E_ARG, "val_batch=%d must be >= 1", val_batch);
+  GB_REQUIRE(!stop || (best_params && out_epochs && out_best_epoch), GB_E_ARG,
+             "stop needs best_params, out_epochs and out_best_epoch");
+  GB_REQUIRE(!stop || gb::aligned16(best_params), GB_E_ARG, "best_params must be 16-byte aligned");
+  return launch_fit(net, params, adam_m, adam_v, jobs, split, n_jobs, max_rows, x, y, row_map, perm, hp, split ? val_batch : 1,
+                    out_loss, out_acc, out_val_loss, out_val_acc, stop, best_params, out_epochs, out_best_epoch, FIT_STOP, stream);
 }
 
 }  // extern "C"

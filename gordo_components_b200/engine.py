@@ -177,7 +177,7 @@ class FFEngine:
 
     def fit_split(self, params, jobs_dev, n_jobs: int, max_rows: int, x, y, split=None, row_map=None, val_batch: Optional[int] = None,
                   epochs: int = 1, batch_size: int = 32, shuffle=True, perm=None, adam: Optional[Dict[str, float]] = None, seed: int = 0,
-                  l1_div_batch: bool = False, state=None, step0: int = 0):
+                  l1_div_batch: bool = False, state=None, step0: int = 0, stop=None):
         """
         ``fit`` over row *positions* with Keras' ``validation_split``, in one launch (gb_ffae_fit_split).  Job i trains on its
         positions [0, n_rows) exactly as ``fit`` trains on its rows, and after every epoch runs the network forward over the held-out
@@ -188,19 +188,36 @@ class FFEngine:
         ``row_map``: int32 device tensor of row indices relative to a job's x_row, shared by the jobs through map_ofs.
         Returns (loss, accuracy, val_loss, val_accuracy, (m, v)), each [n_jobs, epochs]; val_* rows of jobs without held-out
         positions are NaN.
+
+        ``stop``: ``make_stop`` records [n_jobs] (host array or device bytes): every job applies its Keras EarlyStopping rule at the
+        end of each epoch inside the launch (gb_ffae_fit_stop) and leaves the kernel when it fires; with ``restore_best_weights``
+        its slot of ``params`` ends with the weights of its best epoch.  Returns (loss, accuracy, val_loss, val_accuracy,
+        epochs_run, best_epoch, (m, v)): epochs_run / best_epoch are int32 [n_jobs] (best_epoch -1 when no epoch improved and no
+        snapshot was taken), and every history entry past a job's epochs_run is NaN.
         """
         torch = _torch()
         hp = _fit_hparams(epochs, batch_size, shuffle, perm, adam, seed, l1_div_batch, step0)
         m, v = self._fit_state(params, state)
         if split is not None and isinstance(split, np.ndarray):
             split = jobs_to_device(split, self.device)
-        out = [torch.empty((n_jobs, epochs), dtype=torch.float32, device=self.device) for _ in range(2)]
+        make = torch.empty if stop is None else (lambda shape, **kw: torch.full(shape, float("nan"), **kw))  # noqa: E731
+        out = [make((n_jobs, epochs), dtype=torch.float32, device=self.device) for _ in range(2)]
         out += [torch.full((n_jobs, epochs), float("nan"), dtype=torch.float32, device=self.device) for _ in range(2)]
         vb = int(val_batch if val_batch is not None else batch_size)
         p = _cabi.ptr
-        _cabi.check(self.lib.gb_ffae_fit_split(C.byref(self.net), p(params), p(m), p(v), p(jobs_dev), p(split), int(n_jobs), int(max_rows),
-                                               p(x), p(y), p(row_map), p(perm), C.byref(hp), vb, *(p(t) for t in out), _stream_ptr()))
-        return (*out, (m, v))
+        if stop is None:
+            _cabi.check(self.lib.gb_ffae_fit_split(C.byref(self.net), p(params), p(m), p(v), p(jobs_dev), p(split), int(n_jobs), int(max_rows),
+                                                   p(x), p(y), p(row_map), p(perm), C.byref(hp), vb, *(p(t) for t in out), _stream_ptr()))
+            return (*out, (m, v))
+        if isinstance(stop, np.ndarray):
+            stop = jobs_to_device(stop, self.device)
+        best = torch.empty_like(params)  # snapshot area
+        epochs_run = torch.zeros((n_jobs,), dtype=torch.int32, device=self.device)
+        best_epoch = torch.full((n_jobs,), -1, dtype=torch.int32, device=self.device)
+        _cabi.check(self.lib.gb_ffae_fit_stop(C.byref(self.net), p(params), p(m), p(v), p(jobs_dev), p(split), int(n_jobs), int(max_rows),
+                                              p(x), p(y), p(row_map), p(perm), C.byref(hp), vb, *(p(t) for t in out), p(stop), p(best),
+                                              p(epochs_run), p(best_epoch), _stream_ptr()))
+        return (*out, epochs_run, best_epoch, (m, v))
 
     def _fit_state(self, params, state):
         """Adam (m, v) of every slot: the given pair, or zeros for a fresh fit."""
@@ -237,6 +254,30 @@ def make_split(n_val, map_ofs=-1) -> np.ndarray:
     split["n_val"] = n_val
     split["map_ofs"] = map_ofs
     return split
+
+
+STOP_ARGS = ("monitor", "min_delta", "patience", "mode", "baseline", "restore_best_weights", "start_from_epoch")
+
+
+def make_stop(callbacks_per_job) -> np.ndarray:
+    """
+    Structured array of gb_fit_stop records, one per job, from Keras EarlyStopping callbacks: ``EarlyStopping`` objects (ours or
+    anything with its attributes) or dicts of its constructor arguments.  Each goes through ``EarlyStopping.__init__``, so
+    ``mode="auto"`` and the sign of ``min_delta`` resolve exactly as the per-machine fit loop resolves them.  The monitor must be
+    one the fit kernel writes: loss, accuracy, val_loss or val_accuracy.
+    """
+    from .machine.model.models import EarlyStopping
+
+    stop = np.zeros(len(callbacks_per_job), dtype=_cabi.STOP_DTYPE)
+    for j, cb in enumerate(callbacks_per_job):
+        kw = dict(cb) if isinstance(cb, dict) else {k: getattr(cb, k) for k in STOP_ARGS if hasattr(cb, k)}
+        cb = EarlyStopping(**kw)
+        if cb.monitor not in _cabi.STOP_MONITORS:
+            raise ValueError(f"EarlyStopping monitor {cb.monitor!r} is not one of {sorted(_cabi.STOP_MONITORS)}")
+        stop[j] = (_cabi.STOP_MONITORS[cb.monitor], 1 if cb.mode == "min" else -1, cb.patience, cb.start_from_epoch,
+                   int(cb.restore_best_weights), int(cb.baseline is not None), cb.min_delta,
+                   0.0 if cb.baseline is None else float(cb.baseline))
+    return stop
 
 
 def minmax_fit(jobs_dev, n_jobs, max_rows, y, n_out, n_slots, device, return_minmax=False):

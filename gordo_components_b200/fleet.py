@@ -166,7 +166,12 @@ class FleetBuild:
 
     def __init__(self, eng, n_machines, n_splits, params, scale, offset, feat_thr, agg_thr, loss, acc, fold_loss, fold_feat_thr, fold_agg_thr,
                  fold_params=None, cv_moments=None, in_scale=None, in_offset=None, fold_in_scale=None, fold_in_offset=None, steps_per_epoch=None,
-                 val_loss=None, val_acc=None, fold_val_loss=None, fold_val_acc=None):
+                 val_loss=None, val_acc=None, fold_val_loss=None, fold_val_acc=None, epochs=None, epochs_run=None, best_epoch=None,
+                 fold_epochs_run=None, fold_best_epoch=None):
+        # EarlyStopping: epochs each fit ran and its best epoch (-1: none) ([M]; per CV fold [M, K]); None without the callback.
+        # History entries past a fit's epochs_run are NaN.  `epochs` is the configured count (keras History.params["epochs"]).
+        self.epochs = epochs
+        self.epochs_run, self.best_epoch, self.fold_epochs_run, self.fold_best_epoch = epochs_run, best_epoch, fold_epochs_run, fold_best_epoch
         # Keras validation_split: per-epoch loss / accuracy on the held-out tail ([M, epochs]; per CV fold [M, K, epochs]); None without one
         self.val_loss, self.val_acc, self.fold_val_loss, self.fold_val_acc = val_loss, val_acc, fold_val_loss, fold_val_acc
         self.steps_per_epoch = steps_per_epoch                                 # optimizer steps per epoch of the final fit (keras History.params["steps"])
@@ -230,7 +235,12 @@ class FleetBuild:
         if self.val_loss is not None:  # the keys and their order of the per-machine History
             hist["val_loss"] = [float(v) for v in self.val_loss[m].cpu().numpy()]
             hist["val_accuracy"] = [float(v) for v in self.val_acc[m].cpu().numpy()]
-        ae._history = History(hist, {"verbose": 0, "epochs": len(hist["loss"]), "steps": self.steps_per_epoch}, list(range(len(hist["loss"]))))
+        if self.epochs_run is None:
+            ae._history = History(hist, {"verbose": 0, "epochs": len(hist["loss"]), "steps": self.steps_per_epoch}, list(range(len(hist["loss"]))))
+        else:  # as the per-machine fit loop leaves it: the epochs run, against the configured count
+            ran = int(self.epochs_run[m])
+            hist = {k: v[:ran] for k, v in hist.items()}
+            ae._history = History(hist, {"verbose": 0, "epochs": int(self.epochs), "steps": self.steps_per_epoch}, list(range(ran)))
         sc = self._fill_minmax(MinMaxScaler(), self.scale[m].cpu().numpy().astype(np.float64), self.offset[m].cpu().numpy().astype(np.float64), None)
         if template is not None:
             det = template
@@ -283,7 +293,8 @@ def dump_fleet(fb: "FleetBuild", root: str, names: Sequence[str], tags: Optional
 
 def build_fleet(eng: "engine.FFEngine", x, y, rows: int, epochs: int = 1, batch_size: int = 32, n_splits: int = 3, seed: int = 0,
                 adam: Optional[Dict[str, float]] = None, shuffle: bool = True, generator=None, input_scaler: bool = False,
-                detector_shuffle: bool = False, validation_split: float = 0.0, validation_batch_size: Optional[int] = None) -> FleetBuild:
+                detector_shuffle: bool = False, validation_split: float = 0.0, validation_batch_size: Optional[int] = None,
+                early_stopping=None) -> FleetBuild:
     """
     The batched form of ``gordo build`` for one architecture bucket: for every machine the 3-fold TimeSeriesSplit
     cross-validation (fit on each prefix, thresholds from the following test block: diff.py:176-266) and the final fit on
@@ -304,6 +315,10 @@ def build_fleet(eng: "engine.FFEngine", x, y, rows: int, epochs: int = 1, batch_
     ``floor(n * (1 - validation_split))`` and reports the loss and accuracy of the rest after every epoch (``val_loss``,
     ``val_accuracy``; in batches of ``validation_batch_size``, default ``batch_size``), computed inside the same fit launch.
     The scalers still see all ``n`` rows of a slot, as the detector's and the Pipeline's do.
+    ``early_stopping``: the estimator's Keras ``EarlyStopping`` callback -- one for every machine, or a sequence of one per machine
+    (``engine.make_stop`` takes any form).  Every slot of machine m, the final fit and each CV fold, applies m's rule at the end of
+    each of its epochs inside the fit launch (gb_ffae_fit_stop), as sklearn's clone hands every fold the same callbacks.  The
+    result then carries ``epochs_run`` / ``best_epoch``; history entries past a fit's ``epochs_run`` are NaN.
     """
     torch = engine._torch()
     dev = eng.device
@@ -356,8 +371,18 @@ def build_fleet(eng: "engine.FFEngine", x, y, rows: int, epochs: int = 1, batch_
     else:
         base_of = lambda k: base  # noqa: E731
     fit_jobs = engine.jobs_to_device(engine.make_jobs(fit_slots, fit_rows, fit_x), dev)
-    val_loss = val_acc = None
-    if split is None:
+    val_loss = val_acc = epochs_run = best_epoch = None
+    if early_stopping is not None:
+        per_machine = list(early_stopping) if isinstance(early_stopping, (list, tuple)) else [early_stopping] * M
+        if len(per_machine) != M:
+            raise ValueError(f"early_stopping: {len(per_machine)} callbacks for {M} machines")
+        stop = engine.make_stop([per_machine[j % M] for j in range(len(fit_slots))])  # job j trains a slot of machine j mod M
+        loss, acc, val_loss, val_acc, epochs_run, best_epoch, _ = eng.fit_split(
+            params, fit_jobs, len(fit_slots), N, x, y, split=split, row_map=row_map, val_batch=validation_batch_size or batch_size, epochs=epochs,
+            batch_size=batch_size, shuffle=shuffle, adam=adam, seed=seed, stop=stop)
+        if n_train == slot_n:  # nothing held out
+            val_loss = val_acc = None
+    elif split is None:
         loss, acc, _ = eng.fit(params, fit_jobs, len(fit_slots), N, x, y, epochs=epochs, batch_size=batch_size, shuffle=shuffle, adam=adam, seed=seed)
     else:
         loss, acc, val_loss, val_acc, _ = eng.fit_split(params, fit_jobs, len(fit_slots), N, x, y, split=split, row_map=row_map,
@@ -383,6 +408,7 @@ def build_fleet(eng: "engine.FFEngine", x, y, rows: int, epochs: int = 1, batch_
     fold_agg = agg[M:].view(K, M).t().contiguous()
     E = loss.shape[1]
     folds = lambda t: None if t is None else t[M:].view(K, M, E).permute(1, 0, 2)  # noqa: E731
+    fold_jobs = lambda t: None if t is None else t[M:].view(K, M).t()  # noqa: E731
     return FleetBuild(eng, M, K, params[:M].contiguous(), scale[:M].contiguous(), offset[:M].contiguous(), fold_feat[:, K - 1].contiguous(),
                       fold_agg[:, K - 1].contiguous(), loss[:M], acc[:M], loss[M:].view(K, M, E).permute(1, 0, 2), fold_feat, fold_agg,
                       fold_params=fold_params, cv_moments=moments,
@@ -391,7 +417,9 @@ def build_fleet(eng: "engine.FFEngine", x, y, rows: int, epochs: int = 1, batch_
                       fold_in_offset=None if in_offset is None else in_offset[M:].view(K, M, -1).permute(1, 0, 2).contiguous(),
                       steps_per_epoch=(n_train[0] + int(batch_size) - 1) // int(batch_size),
                       val_loss=None if val_loss is None else val_loss[:M], val_acc=None if val_acc is None else val_acc[:M],
-                      fold_val_loss=folds(val_loss), fold_val_acc=folds(val_acc))
+                      fold_val_loss=folds(val_loss), fold_val_acc=folds(val_acc), epochs=int(epochs),
+                      epochs_run=None if epochs_run is None else epochs_run[:M], best_epoch=None if best_epoch is None else best_epoch[:M],
+                      fold_epochs_run=fold_jobs(epochs_run), fold_best_epoch=fold_jobs(best_epoch))
 
 
 # ------------------------------------------------------------------------------------------------ fleet build of LSTM detectors

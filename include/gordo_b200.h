@@ -236,6 +236,35 @@ int gb_ffae_fit_split(const gb_ffnet* net, float* params, float* adam_m, float* 
                       const int32_t* row_map, const int32_t* perm, const gb_fit_hparams* hp, int32_t val_batch,
                       float* out_loss, float* out_acc, float* out_val_loss, float* out_val_acc, void* stream);
 
+/* gb_ffae_fit_split with Keras' EarlyStopping callback (keras 3 EarlyStopping.on_epoch_end; models.py EarlyStopping.update), applied
+ * by every job at the end of each of its epochs, inside the launch.  The monitored value is the float32 history entry the epoch
+ * wrote, widened to double; "better" is v + min_delta < best (mode +1) or v - min_delta > best (mode -1), in double, so a NaN never
+ * improves.  Epochs below start_from_epoch are skipped.  With restore_best, the first epoch that is not skipped takes a snapshot,
+ * and so does every improvement; `wait` counts the epochs since the last improvement that also beat the baseline; the job stops
+ * after the epoch at which wait >= patience and epoch > 0.  At the end, with restore_best and a snapshot, params get the snapshot,
+ * whether or not the job stopped early; the Adam state is that of the last epoch run.  A val_* monitor on a job with n_val 0 (or
+ * a NULL history array for the monitor) is unavailable: the job never stops and takes no snapshot.
+ * stop: [n_jobs] device array, or NULL (then this is gb_ffae_fit_split).  best_params: [n_slots][param_stride], 16-byte aligned,
+ * the snapshot area (overwritten where snapshots are taken).  out_epochs: [n_jobs] epochs each job ran; history entries past it
+ * are left as they are.  out_best_epoch: [n_jobs] the epoch of the best monitored value (with restore_best: the snapshot's),
+ * -1 when no epoch improved and no snapshot was taken.  NULL best_params, out_epochs or out_best_epoch with a stop array, or a
+ * misaligned best_params, is GB_E_ARG. */
+typedef struct gb_fit_stop {
+  int32_t monitor;          /* 0 loss, 1 accuracy, 2 val_loss, 3 val_accuracy */
+  int32_t mode;             /* +1 lower is better ("min"), -1 higher is better ("max"); "auto" is resolved by the caller */
+  int32_t patience, start_from_epoch;
+  int32_t restore_best;     /* the job's final params are those of its best epoch */
+  int32_t has_baseline;
+  double min_delta;         /* >= 0 */
+  double baseline;
+} gb_fit_stop;
+
+int gb_ffae_fit_stop(const gb_ffnet* net, float* params, float* adam_m, float* adam_v, const gb_job* jobs,
+                     const gb_fit_split* split, int32_t n_jobs, int32_t max_rows, const float* x, const float* y,
+                     const int32_t* row_map, const int32_t* perm, const gb_fit_hparams* hp, int32_t val_batch,
+                     float* out_loss, float* out_acc, float* out_val_loss, float* out_val_acc, const gb_fit_stop* stop,
+                     float* best_params, int32_t* out_epochs, int32_t* out_best_epoch, void* stream);
+
 /* The memory plan gb_ffae_fit uses for this architecture (host only, no device needed).  The first of five that fits in
  * 227 KB of shared memory: everything in shared memory; the weight image in the slot's L2-resident state area
  * (*weights_in_l2 = 1); then one, two or three of the three dz buffers there as well (*dz_in_l2).  GB_E_SMEM if none fits
