@@ -22,7 +22,7 @@ ACT_CODES = {"linear": 0, None: 0, "tanh": 1, "relu": 2, "sigmoid": 3}
 
 EXPORTS = (
     "gb_abi_version", "gb_last_error", "gb_device_check", "gb_ffnet_param_count", "gb_ffnet_param_stride",
-    "gb_ffae_infer_score", "gb_ffae_tc_supported", "gb_anomaly_score", "gb_anomaly_score_f64", "gb_minmax_fit", "gb_minmax_f64", "gb_thresholds", "gb_thresholds_f64", "gb_cv_moments", "gb_smooth", "gb_quantile", "gb_affine_f64", "gb_ffae_fit_state_stride", "gb_ffae_fit", "gb_ffae_fit_split", "gb_ffae_fit_stop", "gb_ffae_fit_plan",
+    "gb_ffae_infer_score", "gb_ffae_tc_supported", "gb_ffae_infer_plan", "gb_anomaly_score", "gb_anomaly_score_f64", "gb_minmax_fit", "gb_minmax_f64", "gb_thresholds", "gb_thresholds_f64", "gb_cv_moments", "gb_smooth", "gb_quantile", "gb_affine_f64", "gb_ffae_fit_state_stride", "gb_ffae_fit", "gb_ffae_fit_split", "gb_ffae_fit_stop", "gb_ffae_fit_plan",
     "gb_lstm_param_count", "gb_lstm_param_stride", "gb_lstm_workspace_bytes", "gb_lstm_infer", "gb_lstm_tc_supported", "gb_lstm_tc_workspace_bytes", "gb_lstm_infer_tc", "gb_lstm_fit_workspace_bytes", "gb_lstm_fit",
     "gb_orthonormal_rows",
 )
@@ -126,6 +126,8 @@ def _declare(lib):
     lib.gb_ffae_fit_stop.argtypes = lib.gb_ffae_fit_split.argtypes[:-1] + [_P] * 5
     lib.gb_ffae_fit_plan.argtypes = [C.POINTER(GbFFNet), C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
     lib.gb_ffae_fit_plan.restype = C.c_int
+    lib.gb_ffae_infer_plan.argtypes = [C.POINTER(GbFFNet), C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
+    lib.gb_ffae_infer_plan.restype = C.c_int
     lib.gb_lstm_infer.argtypes = [C.POINTER(GbLstmNet), _P, _P, C.c_int32, C.c_int32, _P, _P, _P, _P]
     lib.gb_lstm_tc_supported.argtypes = [C.POINTER(GbLstmNet)]
     lib.gb_lstm_tc_supported.restype = C.c_int
@@ -139,7 +141,7 @@ def _declare(lib):
     lib.gb_lstm_fit.restype = C.c_int
     lib.gb_orthonormal_rows.argtypes = [_P, C.c_int32, C.c_int32, C.c_int32, _P, C.c_int64, C.c_int64, _P]
     lib.gb_orthonormal_rows.restype = C.c_int
-    for name in ("gb_device_check", "gb_ffae_infer_score", "gb_ffae_tc_supported", "gb_anomaly_score", "gb_minmax_fit", "gb_thresholds", "gb_smooth", "gb_ffae_fit", "gb_ffae_fit_split", "gb_ffae_fit_stop", "gb_lstm_infer"):
+    for name in ("gb_device_check", "gb_ffae_infer_score", "gb_ffae_tc_supported", "gb_ffae_infer_plan", "gb_anomaly_score", "gb_minmax_fit", "gb_thresholds", "gb_smooth", "gb_ffae_fit", "gb_ffae_fit_split", "gb_ffae_fit_stop", "gb_lstm_infer"):
         getattr(lib, name).restype = C.c_int
 
 

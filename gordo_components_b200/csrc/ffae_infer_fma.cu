@@ -25,6 +25,7 @@ struct Args {
   int pitch;        // floats between consecutive rows of an activation buffer (pitch/4 odd)
   int wfloats;      // floats reserved for weights in smem
   int resident;     // all layers resident (1) or staged layer by layer (0)
+  int col_block;    // staged: output columns of a layer staged at a time (>= every padded width unless a layer is too large)
   int n_in, n_out;
   int rows_per_chunk;
   long pstride;
@@ -34,20 +35,23 @@ struct Args {
   float *o_model, *o_ts, *o_tu, *o_tots, *o_totu, *o_conf, *o_totconf;
 };
 
-__device__ __forceinline__ void stage_layer(float* dst, const float* P, const Args& a, int l, int tid) {
-  const int K = a.net.dims[l], N = a.net.dims[l + 1], Kp = a.im.kp[l], Np = a.im.np[l];
+// output columns [c0, c0 + nb) of layer l as a padded [Kp][nb] image followed by their nb biases
+__device__ __forceinline__ void stage_layer(float* dst, const float* P, const Args& a, int l, int c0, int nb, int tid) {
+  const int K = a.net.dims[l], N = a.net.dims[l + 1], Kp = a.im.kp[l];
   const float* Wg = P + a.im.pofs[l];
   const float* bg = Wg + K * N;
-  for (int idx = tid; idx < Kp * Np; idx += THREADS) {
-    const int k = idx / Np, n = idx - k * Np;
+  for (int idx = tid; idx < Kp * nb; idx += THREADS) {
+    const int k = idx / nb, n = c0 + idx - k * nb;
     dst[idx] = (k < K && n < N) ? __ldg(Wg + k * N + n) : 0.f;
   }
-  for (int n = tid; n < Np; n += THREADS) dst[Kp * Np + n] = n < N ? __ldg(bg + n) : 0.f;
+  for (int n = tid; n < nb; n += THREADS) dst[Kp * nb + n] = c0 + n < N ? __ldg(bg + c0 + n) : 0.f;
 }
 
 // RT row groups of 32 per thread: tiles of 128 rows (RT = 4) for the usual stacks, 64 / 32 rows when wide layers (up to 256: the
-// defaults of feedforward_model / feedforward_symmetric) leave less shared memory for the activation buffers
-template <int RT>
+// defaults of feedforward_model / feedforward_symmetric) leave less shared memory for the activation buffers.  BLOCKED: staged
+// layers go in blocks of a.col_block output columns (only with 32-row tiles, for layers too large to stage whole); a separate
+// instantiation so that every other plan runs the single-block code.
+template <int RT, bool BLOCKED>
 __global__ void __launch_bounds__(THREADS) ffae_infer_fma_kernel(const Args a) {
   constexpr int ROWS = 32 * RT;
   extern __shared__ __align__(16) float smem[];
@@ -65,7 +69,7 @@ __global__ void __launch_bounds__(THREADS) ffae_infer_fma_kernel(const Args a) {
   const int pitch = a.pitch, n_in = a.n_in, n_out = a.n_out, L = a.net.n_layers;
 
   if (a.resident) {
-    for (int l = 0; l < L; ++l) stage_layer(sW + a.im.wofs[l], P, a, l, tid);
+    for (int l = 0; l < L; ++l) stage_layer(sW + a.im.wofs[l], P, a, l, 0, a.im.np[l], tid);
   }
   __syncthreads();
 
@@ -97,51 +101,58 @@ __global__ void __launch_bounds__(THREADS) ffae_infer_fma_kernel(const Args a) {
     float* out = buf1;
     for (int l = 0; l < L; ++l) {
       const int Kp = a.im.kp[l], Np = a.im.np[l], act = a.net.act[l];
-      const float* Wl;
-      if (a.resident) {
-        Wl = sW + a.im.wofs[l];
-      } else {
-        stage_layer(sW, P, a, l, tid);
-        __syncthreads();
-        Wl = sW;
-      }
-      const float* bl = Wl + Kp * Np;
-      for (int task = warp; task < (Np >> 2); task += NWARPS) {
-        const int n0 = task << 2;
-        const float4 b4 = *reinterpret_cast<const float4*>(bl + n0);
-        float4 acc[RT];
+      const int cb = BLOCKED ? min(Np, a.col_block) : Np;
+      int c0 = 0;
+      do {
+        const int nb = BLOCKED ? min(cb, Np - c0) : Np;
+        const float* Wl;
+        if (a.resident) {
+          Wl = sW + a.im.wofs[l];
+        } else {
+          if (BLOCKED && c0 > 0) __syncthreads();  // every warp is done with the previous column block
+          stage_layer(sW, P, a, l, c0, nb, tid);
+          __syncthreads();
+          Wl = sW;
+        }
+        const float* bl = Wl + Kp * nb;
+        for (int task = warp; task < (nb >> 2); task += NWARPS) {
+          const int n0 = task << 2;
+          const float4 b4 = *reinterpret_cast<const float4*>(bl + n0);
+          float4 acc[RT];
 #pragma unroll
-        for (int i = 0; i < RT; ++i) acc[i] = b4;
-        const float* arow = in + lane * pitch;
-        const float* wcol = Wl + n0;
-        for (int k = 0; k < Kp; k += 4) {
-          float4 av[RT];
+          for (int i = 0; i < RT; ++i) acc[i] = b4;
+          const float* arow = in + lane * pitch;
+          const float* wcol = Wl + n0;
+          for (int k = 0; k < Kp; k += 4) {
+            float4 av[RT];
 #pragma unroll
-          for (int i = 0; i < RT; ++i) av[i] = *reinterpret_cast<const float4*>(arow + i * 32 * pitch + k);
-          const float4 w0 = *reinterpret_cast<const float4*>(wcol + (k + 0) * Np);
-          const float4 w1 = *reinterpret_cast<const float4*>(wcol + (k + 1) * Np);
-          const float4 w2 = *reinterpret_cast<const float4*>(wcol + (k + 2) * Np);
-          const float4 w3 = *reinterpret_cast<const float4*>(wcol + (k + 3) * Np);
+            for (int i = 0; i < RT; ++i) av[i] = *reinterpret_cast<const float4*>(arow + i * 32 * pitch + k);
+            const float4 w0 = *reinterpret_cast<const float4*>(wcol + (k + 0) * nb);
+            const float4 w1 = *reinterpret_cast<const float4*>(wcol + (k + 1) * nb);
+            const float4 w2 = *reinterpret_cast<const float4*>(wcol + (k + 2) * nb);
+            const float4 w3 = *reinterpret_cast<const float4*>(wcol + (k + 3) * nb);
+#pragma unroll
+            for (int i = 0; i < RT; ++i) {
+              acc[i].x = fmaf(av[i].x, w0.x, acc[i].x); acc[i].y = fmaf(av[i].x, w0.y, acc[i].y);
+              acc[i].z = fmaf(av[i].x, w0.z, acc[i].z); acc[i].w = fmaf(av[i].x, w0.w, acc[i].w);
+              acc[i].x = fmaf(av[i].y, w1.x, acc[i].x); acc[i].y = fmaf(av[i].y, w1.y, acc[i].y);
+              acc[i].z = fmaf(av[i].y, w1.z, acc[i].z); acc[i].w = fmaf(av[i].y, w1.w, acc[i].w);
+              acc[i].x = fmaf(av[i].z, w2.x, acc[i].x); acc[i].y = fmaf(av[i].z, w2.y, acc[i].y);
+              acc[i].z = fmaf(av[i].z, w2.z, acc[i].z); acc[i].w = fmaf(av[i].z, w2.w, acc[i].w);
+              acc[i].x = fmaf(av[i].w, w3.x, acc[i].x); acc[i].y = fmaf(av[i].w, w3.y, acc[i].y);
+              acc[i].z = fmaf(av[i].w, w3.z, acc[i].z); acc[i].w = fmaf(av[i].w, w3.w, acc[i].w);
+            }
+          }
 #pragma unroll
           for (int i = 0; i < RT; ++i) {
-            acc[i].x = fmaf(av[i].x, w0.x, acc[i].x); acc[i].y = fmaf(av[i].x, w0.y, acc[i].y);
-            acc[i].z = fmaf(av[i].x, w0.z, acc[i].z); acc[i].w = fmaf(av[i].x, w0.w, acc[i].w);
-            acc[i].x = fmaf(av[i].y, w1.x, acc[i].x); acc[i].y = fmaf(av[i].y, w1.y, acc[i].y);
-            acc[i].z = fmaf(av[i].y, w1.z, acc[i].z); acc[i].w = fmaf(av[i].y, w1.w, acc[i].w);
-            acc[i].x = fmaf(av[i].z, w2.x, acc[i].x); acc[i].y = fmaf(av[i].z, w2.y, acc[i].y);
-            acc[i].z = fmaf(av[i].z, w2.z, acc[i].z); acc[i].w = fmaf(av[i].z, w2.w, acc[i].w);
-            acc[i].x = fmaf(av[i].w, w3.x, acc[i].x); acc[i].y = fmaf(av[i].w, w3.y, acc[i].y);
-            acc[i].z = fmaf(av[i].w, w3.z, acc[i].z); acc[i].w = fmaf(av[i].w, w3.w, acc[i].w);
+            float4 o;
+            o.x = gb::apply_act(act, acc[i].x); o.y = gb::apply_act(act, acc[i].y);
+            o.z = gb::apply_act(act, acc[i].z); o.w = gb::apply_act(act, acc[i].w);
+            *reinterpret_cast<float4*>(out + (lane + 32 * i) * pitch + c0 + n0) = o;
           }
         }
-#pragma unroll
-        for (int i = 0; i < RT; ++i) {
-          float4 o;
-          o.x = gb::apply_act(act, acc[i].x); o.y = gb::apply_act(act, acc[i].y);
-          o.z = gb::apply_act(act, acc[i].z); o.w = gb::apply_act(act, acc[i].w);
-          *reinterpret_cast<float4*>(out + (lane + 32 * i) * pitch + n0) = o;
-        }
-      }
+        c0 += cb;
+      } while (BLOCKED && c0 < Np);
       __syncthreads();
       float* t = in; in = out; out = t;
     }
@@ -234,7 +245,66 @@ __global__ void __launch_bounds__(THREADS) ffae_infer_fma_kernel(const Args a) {
   }
 }
 
+// The launch plan of an architecture: the largest row tile (128, 64 or 32 rows) whose activation buffers fit next to the weights,
+// all layers resident when they fit the budget, else staged layer by layer.  A layer whose whole image does not fit next to even
+// the 32-row buffers (a 256 x 256 layer, or 256 x 172 in the feedforward_symmetric default at 172 tags) is staged in blocks of
+// output columns.  Fills a.im, a.pitch, a.resident, a.col_block, a.wfloats; returns the row tile and the dynamic shared memory.
+int make_plan(const gb_ffnet* net, Args& a, size_t* smem_out) {
+  constexpr size_t SMEM_MAX = 227 * 1024;
+  a.net = *net;
+  a.im = gb::make_ff_image(net, 4);
+  int p4 = a.im.max_np / 4 + 1;
+  if ((p4 & 1) == 0) ++p4;  // odd number of 16-byte units per row -> conflict-free LDS.128/STS.128
+  a.pitch = p4 * 4;
+  a.col_block = a.im.max_np;
+  int max_layer = 0, max_kp = 0;
+  for (int l = 0; l < net->n_layers; ++l) {
+    max_layer = max(max_layer, a.im.kp[l] * a.im.np[l] + a.im.np[l]);
+    max_kp = max(max_kp, a.im.kp[l]);
+  }
+  const size_t budget = 220 * 1024;
+  int rt = 4;
+  size_t smem = 0, act_bytes = 0;
+  for (;; rt >>= 1) {  // the largest row tile whose activation buffers fit next to the (resident or per-layer staged) weights
+    const int rows = 32 * rt;
+    act_bytes = (size_t)(2 * rows * a.pitch + 2 * rows) * sizeof(float);
+    a.resident = ((size_t)a.im.total * sizeof(float) + act_bytes) <= budget;
+    a.wfloats = gb::round_up(a.resident ? a.im.total : max_layer, 4);
+    smem = (size_t)a.wfloats * sizeof(float) + act_bytes;
+    if (smem <= SMEM_MAX || rt == 1) break;
+  }
+  if (smem > SMEM_MAX && act_bytes < SMEM_MAX) {  // column blocks: a multiple of 32 columns (whole warp-task rounds) where possible
+    int cb = (int)((SMEM_MAX - act_bytes) / sizeof(float) / (max_kp + 1));
+    cb = cb >= 32 ? cb / 32 * 32 : cb / 4 * 4;
+    if (cb >= 4) {
+      a.col_block = cb;
+      int wf = 0;
+      for (int l = 0; l < net->n_layers; ++l) {
+        const int nb = min(a.im.np[l], cb);
+        wf = max(wf, a.im.kp[l] * nb + nb);
+      }
+      a.wfloats = gb::round_up(wf, 4);
+      smem = (size_t)a.wfloats * sizeof(float) + act_bytes;
+    }
+  }
+  GB_REQUIRE(smem <= SMEM_MAX, GB_E_SMEM, "architecture needs %zu bytes of shared memory", smem);
+  *smem_out = smem;
+  return 32 * rt;
+}
+
 }  // namespace
+
+extern "C" int gb_ffae_infer_plan(const gb_ffnet* net, int32_t* rows_per_tile, int32_t* resident) {
+  int rc = gb::validate_ffnet(net);
+  if (rc != GB_OK) return rc;
+  Args a{};
+  size_t smem = 0;
+  const int rows = make_plan(net, a, &smem);
+  if (rows < 0) return rows;
+  if (rows_per_tile) *rows_per_tile = rows;
+  if (resident) *resident = a.resident;
+  return GB_OK;
+}
 
 extern "C" int gb_ffae_infer_score_fma(const gb_ffnet* net, const float* params, const gb_job* jobs, int32_t n_jobs,
                                        int32_t max_rows, const float* x, const float* y, const float* scale,
@@ -243,28 +313,12 @@ extern "C" int gb_ffae_infer_score_fma(const gb_ffnet* net, const float* params,
                                        float* out_total_unscaled, float* out_conf, float* out_total_conf,
                                        void* stream) {
   Args a{};
-  a.net = *net;
-  a.im = gb::make_ff_image(net, 4);
-  int p4 = a.im.max_np / 4 + 1;
-  if ((p4 & 1) == 0) ++p4;  // odd number of 16-byte units per row -> conflict-free LDS.128/STS.128
-  a.pitch = p4 * 4;
+  size_t smem = 0;
+  const int ROWS = make_plan(net, a, &smem);
+  if (ROWS < 0) return ROWS;
+  const int rt = ROWS / 32;
   a.n_in = net->dims[0];
   a.n_out = net->dims[net->n_layers];
-  int max_layer = 0;
-  for (int l = 0; l < net->n_layers; ++l) max_layer = max(max_layer, a.im.kp[l] * a.im.np[l] + a.im.np[l]);
-  const size_t budget = 220 * 1024;
-  int rt = 4;
-  size_t smem = 0;
-  for (;; rt >>= 1) {  // the largest row tile whose activation buffers fit next to the (resident or per-layer staged) weights
-    const int rows = 32 * rt;
-    const size_t act_bytes = (size_t)(2 * rows * a.pitch + 2 * rows) * sizeof(float);
-    a.resident = ((size_t)a.im.total * sizeof(float) + act_bytes) <= budget;
-    a.wfloats = gb::round_up(a.resident ? a.im.total : max_layer, 4);
-    smem = (size_t)a.wfloats * sizeof(float) + act_bytes;
-    if (smem <= 227 * 1024 || rt == 1) break;
-  }
-  GB_REQUIRE(smem <= 227 * 1024, GB_E_SMEM, "architecture needs %zu bytes of shared memory", smem);
-  const int ROWS = 32 * rt;
   a.pstride = (long)gb_ffnet_param_stride(net);
   a.params = params; a.jobs = jobs; a.x = x; a.y = y; a.scale = scale; a.feat_thr = feat_thr; a.agg_thr = agg_thr;
   a.o_model = out_model; a.o_ts = out_tag_scaled; a.o_tu = out_tag_unscaled; a.o_tots = out_total_scaled;
@@ -287,7 +341,9 @@ extern "C" int gb_ffae_infer_score_fma(const gb_ffnet* net, const float* params,
     }
     return GB_OK;
   };
-  int rc = rt == 4 ? launch(ffae_infer_fma_kernel<4>) : rt == 2 ? launch(ffae_infer_fma_kernel<2>) : launch(ffae_infer_fma_kernel<1>);
+  const bool blocked = a.col_block < a.im.max_np;
+  int rc = rt == 4 ? launch(ffae_infer_fma_kernel<4, false>) : rt == 2 ? launch(ffae_infer_fma_kernel<2, false>)
+           : blocked ? launch(ffae_infer_fma_kernel<1, true>) : launch(ffae_infer_fma_kernel<1, false>);
   if (rc != GB_OK) return rc;
   GB_CUDA_CHECK(cudaGetLastError());
   return GB_OK;

@@ -223,7 +223,7 @@ int gb_lstm_infer(const gb_lstmnet* net, const float* params, const gb_job* jobs
   int rc = validate_lstm(net);
   if (rc != GB_OK) return rc;
   GB_REQUIRE(params && jobs && x && out_model, GB_E_ARG, "params/jobs/x/out_model must be non-NULL");
-  GB_REQUIRE(n_jobs >= 0 && n_jobs <= 65535 && max_rows >= 0, GB_E_ARG, "bad n_jobs/max_rows");
+  GB_REQUIRE(n_jobs >= 0 && max_rows >= 0, GB_E_ARG, "bad n_jobs/max_rows");
   if (n_jobs == 0 || max_rows == 0) return GB_OK;
   LstmArgs a{};
   a.net = *net;
@@ -250,7 +250,10 @@ int gb_lstm_infer(const gb_lstmnet* net, const float* params, const gb_job* jobs
   GB_REQUIRE(smem <= 227 * 1024, GB_E_SMEM, "LSTM stack needs %zu bytes of shared memory for its state", smem);
   GB_CUDA_CHECK(cudaFuncSetAttribute(lstm_infer_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const int blocks = (max_rows + BW - 1) / BW;
-  lstm_infer_kernel<<<dim3(blocks, n_jobs), THREADS, smem, (cudaStream_t)stream>>>(a);
+  for (int j0 = 0; j0 < n_jobs; j0 += 65535) {  // gridDim.y carries the job index: larger fleets go out as several launches
+    a.jobs = jobs + j0;
+    lstm_infer_kernel<<<dim3(blocks, n_jobs - j0 < 65535 ? n_jobs - j0 : 65535), THREADS, smem, (cudaStream_t)stream>>>(a);
+  }
   GB_CUDA_CHECK(cudaGetLastError());
   return GB_OK;
 }

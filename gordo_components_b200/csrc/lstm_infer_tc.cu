@@ -15,8 +15,11 @@
 //
 // Numerics (1e-4 parity): h in (-1, 1) and the weights are split into FP16 pairs (a = a1 + a2, 22 significant bits) and
 // every product is formed as a2*w1 + a1*w2 + a1*w1 with fp32 accumulation -- the scheme of ffae_infer_tc.cu's layers >= 1.
-// The raw input x (any magnitude) never enters an FP16 operand: its projection x.K0 + b0 is computed once per ROW (not
-// per window) in fp32 on the CUDA cores and added in layer 0's epilogue.
+// That bound on h holds for tanh and sigmoid cells only: relu and linear cells have an unbounded h that overflows FP16, so
+// gb_lstm_tc_supported refuses them (they run on the fp32 kernel, lstm_infer.cu).
+// The raw input x (any magnitude) never enters an FP16 operand: its projection x.K0 + b0 is computed once per x row of each
+// job (not per window) in fp32 on the CUDA cores and added in layer 0's epilogue.  Each job keeps its own projection, made with
+// its own slot's weights, so jobs of different slots may read the same x rows.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include "gb_common.cuh"
@@ -44,8 +47,8 @@ struct TcLayerArgs {
   int tiles_per_job, t, n_items;     // n_items counts (window tile, unit block)
   const gb_job* jobs;
   const float* bias;                 // [n_slots][4u] reordered (layers >= 1; layer 0's bias lives in xk)
-  const float* xk;                   // layer 0: input projection, row-blocked [x row / 128][4u reordered][128]
-  long xk_rows;
+  const float* xk;                   // layer 0: input projection of each job's own x rows, [job][row in job / 128][4u reordered][128]
+  int xk_blocks;                     // 128-row blocks per job in xk
   float* c;                          // [tile][u][128 windows]
   __half *h_out_hi, *h_out_lo;       // [rows][u]
 };
@@ -107,18 +110,16 @@ lstm_tc_step_kernel(const __grid_constant__ TcLayerArgs a, const __grid_constant
   const int n_chunks = a.kc_below + a.kc_own;
   const int nub = u / UB;
   // item -> (tile, ub): the unit blocks of one window tile are neighbours, so CTAs running side by side read the same A operand from L2
-  struct Item { int tile, tj, ub, slot, n_rows; long x_row; bool real; };
+  struct Item { int tile, tj, ub, slot, n_rows, job; bool real; };
   auto item_of = [&](int item) -> Item {
     Item it;
     const int grp = item / nub;
     it.ub = item - grp * nub;
-    const int job_id = grp / a.tiles_per_job;
-    it.tj = grp - job_id * a.tiles_per_job;
+    it.job = grp / a.tiles_per_job;
+    it.tj = grp - it.job * a.tiles_per_job;
     it.tile = grp;
-    const gb_job* jp = a.jobs + job_id;
-    const int2 sn = __ldg(reinterpret_cast<const int2*>(jp));  // slot, n_rows
+    const int2 sn = __ldg(reinterpret_cast<const int2*>(a.jobs + it.job));  // slot, n_rows
     it.slot = sn.x; it.n_rows = sn.y;
-    it.x_row = FIRST ? (long)__ldg(reinterpret_cast<const long long*>(&jp->x_row)) : 0;
     it.real = it.tj * TILE < it.n_rows;
     return it;
   };
@@ -187,9 +188,9 @@ lstm_tc_step_kernel(const __grid_constant__ TcLayerArgs a, const __grid_constant
         const int w = it.tj * TILE + r;  // window index inside the job (may exceed n_rows in the last tile)
         const long row = (long)it.tile * TILE + r;
         const float* xk = nullptr;
-        if (FIRST) {  // xk is stored row-blocked, [row / 128][4u reordered][128]
-          const long xr = min(it.x_row + min(w, it.n_rows - 1) + a.t, a.xk_rows - 1);
-          xk = a.xk + ((xr >> 7) * (long)(4 * u) + it.ub * NCOL) * TILE + (xr & (TILE - 1));
+        if (FIRST) {  // xk is stored per job and row-blocked, [job][row / 128][4u reordered][128]
+          const int xr = min(w, it.n_rows - 1) + a.t;  // x row relative to the job's x_row
+          xk = a.xk + (((long)it.job * a.xk_blocks + (xr >> 7)) * (4 * u) + it.ub * NCOL) * TILE + (xr & (TILE - 1));
         }
         const float* bias = FIRST ? nullptr : a.bias + (long)it.slot * 4 * u + it.ub * NCOL;
         float* ccol = a.c + ((long)it.tile * u + it.ub * UB) * TILE + r;  // unit j of this window: ccol[j * TILE]
@@ -235,10 +236,10 @@ __device__ __forceinline__ int keras_col(int np, int u) {
   return unit < u ? g * u + unit : -1;
 }
 
-// weight images of one layer: rows n' (4u per slot), K contiguous: [below part padded to 64 | own part], FP16 pair
+// weight images of one layer: rows n' (4u per slot), K contiguous: [below part padded to 64 | own part], FP16 pair; slots from slot0
 __global__ void lstm_tc_weights_kernel(const float* __restrict__ params, long pstride, long kofs, int in, int u, int up, int kp_below, int kp,
-                                       int use_below, __half* __restrict__ w_hi, __half* __restrict__ w_lo, float* __restrict__ bias) {
-  const int slot = blockIdx.y;
+                                       int use_below, int slot0, __half* __restrict__ w_hi, __half* __restrict__ w_lo, float* __restrict__ bias) {
+  const int slot = slot0 + blockIdx.y;
   const float* P = params + (long)slot * pstride + kofs;  // kernel [in][4u], recurrent [u][4u], bias [4u]  (real widths)
   const int u4 = 4 * u, up4 = 4 * up;
   for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < (long)up4 * kp; i += (long)gridDim.x * blockDim.x) {
@@ -263,10 +264,13 @@ __global__ void lstm_tc_weights_kernel(const float* __restrict__ params, long ps
     }
 }
 
-// layer 0 input projection per ROW: xk[row][n'] = x[row] . K0[:, col(n')] + b0[col(n')]; grid (ceil(rows/32), 4u/64, jobs)
-__global__ void __launch_bounds__(256) lstm_tc_xk_kernel(const gb_job* __restrict__ jobs, const float* __restrict__ x, int F, int u, int up, int lookback,
-                                                         const float* __restrict__ params, long pstride, float* __restrict__ xk) {
-  const gb_job job = jobs[blockIdx.z];
+// layer 0 input projection per x row of a job: xk[job][r][n'] = x[x_row + r] . K0[:, col(n')] + b0[col(n')] with the job's slot;
+// grid (ceil(rows/32), 4u/64, jobs from job0)
+__global__ void __launch_bounds__(256) lstm_tc_xk_kernel(const gb_job* __restrict__ jobs, int job0, const float* __restrict__ x, int F, int u, int up,
+                                                         int lookback, const float* __restrict__ params, long pstride, int xk_blocks,
+                                                         float* __restrict__ xk) {
+  const long job_id = job0 + blockIdx.z;
+  const gb_job job = jobs[job_id];
   const int n_x = job.n_rows + lookback - 1;  // x rows this job's windows touch
   const int r0 = blockIdx.x * 32;
   if (r0 >= n_x) return;
@@ -299,27 +303,26 @@ __global__ void __launch_bounds__(256) lstm_tc_xk_kernel(const gb_job* __restric
     __syncthreads();
   }
   const float b = kc >= 0 ? __ldg(P + (long)(F + u) * u4 + kc) : 0.f;
-  // out: row-blocked [row / 128][4 * up][128]; staged through shared memory so that lanes run along rows (128-byte segments)
+  // out: the job's rows, row-blocked [row / 128][4 * up][128]; staged through shared memory so that lanes run along rows (128-byte segments)
 #pragma unroll
   for (int i = 0; i < 8; ++i) sW[rg + 4 * i][col] = acc[i] + b;  // sW reused as [32 rows][64 columns]
   __syncthreads();
+  float* xj = xk + job_id * xk_blocks * (4L * up) * TILE;
   for (int i = tid; i < 64 * 32; i += 256) {
     const int c = i >> 5, rr = i & 31, r = r0 + rr;
-    if (r < n_x) {
-      const long xr = job.x_row + r;
-      xk[((xr >> 7) * (long)(4 * up) + c0 + c) * TILE + (xr & (TILE - 1))] = sW[rr][c];
-    }
+    if (r < n_x) xj[((r >> 7) * (long)(4 * up) + c0 + c) * TILE + (r & (TILE - 1))] = sW[rr][c];
   }
 }
 
-// Dense head on the last layer's final h: out[w][o] = act(sum_k h[w][k] Wd[k][o] + bd[o]); grid (tiles, jobs)
-__global__ void __launch_bounds__(128) lstm_tc_head_kernel(const gb_job* __restrict__ jobs, int tiles_per_job, const __half* __restrict__ h_hi,
+// Dense head on the last layer's final h: out[w][o] = act(sum_k h[w][k] Wd[k][o] + bd[o]); grid (tiles, jobs from job0)
+__global__ void __launch_bounds__(128) lstm_tc_head_kernel(const gb_job* __restrict__ jobs, int job0, int tiles_per_job, const __half* __restrict__ h_hi,
                                                            const __half* __restrict__ h_lo, int u, int up, int n_out, int out_act,
                                                            const float* __restrict__ params, long pstride, long dofs, float* __restrict__ out) {
-  const gb_job job = jobs[blockIdx.y];
+  const long job_id = job0 + blockIdx.y;
+  const gb_job job = jobs[job_id];
   const int w = blockIdx.x * TILE + threadIdx.x;
   if (w >= job.n_rows) return;
-  const long row = ((long)blockIdx.y * tiles_per_job + blockIdx.x) * TILE + threadIdx.x;
+  const long row = (job_id * tiles_per_job + blockIdx.x) * TILE + threadIdx.x;
   const float* Wd = params + (long)job.slot * pstride + dofs;
   const float* bd = Wd + (long)u * n_out;
   for (int o = 0; o < n_out; ++o) {
@@ -341,6 +344,7 @@ struct Plan {
   int nl, F, n_out, L;
   int u[GB_MAX_LAYERS], ur[GB_MAX_LAYERS], in[GB_MAX_LAYERS], kp_below[GB_MAX_LAYERS], kp[GB_MAX_LAYERS];  // u: padded to 64, ur / in: real widths
   long kofs[GB_MAX_LAYERS], dofs;
+  int xk_blocks;  // 128-row blocks of each job's input projection: its windows touch max_windows + lookback - 1 x rows
   // workspace offsets (bytes)
   size_t w_hi[GB_MAX_LAYERS], w_lo[GB_MAX_LAYERS], bias[GB_MAX_LAYERS], h_hi[GB_MAX_LAYERS][2], h_lo[GB_MAX_LAYERS][2], c[GB_MAX_LAYERS], xk, total;
   size_t state_begin, state_end;
@@ -348,8 +352,11 @@ struct Plan {
 
 size_t align256(size_t v) { return (v + 255) / 256 * 256; }
 
-void make_plan(const gb_lstmnet* net, int n_slots, long rows_pad, long x_rows, Plan* p) {
+void make_plan(const gb_lstmnet* net, int n_slots, int n_jobs, int max_windows, Plan* p) {
   p->nl = net->n_layers; p->F = net->n_features; p->n_out = net->n_features_out; p->L = net->lookback;
+  const long tiles_per_job = (max_windows + TILE - 1) / TILE;
+  const long rows_pad = (long)n_jobs * tiles_per_job * TILE;
+  p->xk_blocks = (int)(((long)max_windows + p->L - 1 + TILE - 1) / TILE);
   long pofs = 0;
   int in = net->n_features;
   size_t ofs = 0;
@@ -366,7 +373,7 @@ void make_plan(const gb_lstmnet* net, int n_slots, long rows_pad, long x_rows, P
     in = ur;
   }
   p->dofs = pofs;
-  p->xk = ofs; ofs = align256(ofs + (size_t)((x_rows + TILE - 1) / TILE * TILE) * 4 * p->u[0] * sizeof(float));
+  p->xk = ofs; ofs = align256(ofs + (size_t)n_jobs * p->xk_blocks * TILE * 4 * p->u[0] * sizeof(float));
   p->state_begin = ofs;
   for (int l = 0; l < p->nl; ++l) {
     const size_t hb = (size_t)rows_pad * p->u[l] * sizeof(__half);
@@ -389,15 +396,17 @@ extern "C" int gb_lstm_tc_supported(const gb_lstmnet* net) {
     GB_REQUIRE(net->units[l] >= 1 && net->units[l] <= 512, GB_E_SHAPE, "tensor-core LSTM variant covers layer widths 1..512, units[%d]=%d", l, net->units[l]);
   GB_REQUIRE(net->n_features >= 1 && net->n_features <= 512 && net->n_features_out >= 1 && net->n_features_out <= 512, GB_E_SHAPE, "bad feature counts");
   GB_REQUIRE(net->lookback >= 1, GB_E_ARG, "lookback=%d must be >= 1", net->lookback);
+  for (int l = 0; l < net->n_layers; ++l)  // h is carried as an FP16 pair: only cells with |h| < 1
+    GB_REQUIRE(net->act[l] == GB_ACT_TANH || net->act[l] == GB_ACT_SIGMOID, GB_E_SHAPE,
+               "tensor-core LSTM variant covers tanh and sigmoid cells (a relu or linear cell's h overflows FP16), act[%d]=%d", l, net->act[l]);
   return GB_OK;
 }
 
-// x_rows: rows of the x array (the input projection is indexed by absolute x row)
-extern "C" size_t gb_lstm_tc_workspace_bytes(const gb_lstmnet* net, int32_t n_slots, int32_t n_jobs, int32_t max_windows, int64_t x_rows) {
+// x_rows: rows of the x array (not needed for the size: each job's input projection covers its own max_windows + lookback - 1 rows)
+extern "C" size_t gb_lstm_tc_workspace_bytes(const gb_lstmnet* net, int32_t n_slots, int32_t n_jobs, int32_t max_windows, int64_t /*x_rows*/) {
   if (gb_lstm_tc_supported(net) != GB_OK || n_jobs < 0 || max_windows < 0 || n_slots < 0) return 0;
   Plan p;
-  const long tiles_per_job = (max_windows + TILE - 1) / TILE;
-  make_plan(net, n_slots, (long)n_jobs * tiles_per_job * TILE, x_rows, &p);
+  make_plan(net, n_slots, n_jobs, max_windows, &p);
   return p.total;
 }
 
@@ -406,25 +415,28 @@ extern "C" int gb_lstm_infer_tc(const gb_lstmnet* net, const float* params, int3
   int rc = gb_lstm_tc_supported(net);
   if (rc != GB_OK) return rc;
   GB_REQUIRE(params && jobs && x && out_model && workspace, GB_E_ARG, "params/jobs/x/out_model/workspace must be non-NULL");
-  GB_REQUIRE(n_jobs >= 0 && n_jobs <= 65535 && max_windows >= 0 && n_slots >= 1 && x_rows >= 1, GB_E_ARG, "bad n_jobs/max_windows/n_slots/x_rows");
+  GB_REQUIRE(n_jobs >= 0 && max_windows >= 0 && n_slots >= 1 && x_rows >= 1, GB_E_ARG, "bad n_jobs/max_windows/n_slots/x_rows");
   GB_REQUIRE(gb::aligned16(workspace), GB_E_ALIGN, "workspace must be 16-byte aligned");
   if (n_jobs == 0 || max_windows == 0) return GB_OK;
   cudaStream_t st = (cudaStream_t)stream;
   const int tiles_per_job = (max_windows + TILE - 1) / TILE;
   const long rows_pad = (long)n_jobs * tiles_per_job * TILE;
   Plan p;
-  make_plan(net, n_slots, rows_pad, x_rows, &p);
+  make_plan(net, n_slots, n_jobs, max_windows, &p);
   uint8_t* ws = static_cast<uint8_t*>(workspace);
   const long pstride = (long)gb_lstm_param_stride(net);
+  constexpr int GRID_YZ = 65535;  // gridDim.y / z carry slots and jobs: larger fleets go out as several launches
 
   // ---- operands that do not depend on the timestep
   for (int l = 0; l < p.nl; ++l)
-    lstm_tc_weights_kernel<<<dim3(64, n_slots), 256, 0, st>>>(params, pstride, p.kofs[l], p.in[l], p.ur[l], p.u[l], p.kp_below[l], p.kp[l], l > 0,
-                                                               reinterpret_cast<__half*>(ws + p.w_hi[l]), reinterpret_cast<__half*>(ws + p.w_lo[l]),
-                                                               reinterpret_cast<float*>(ws + p.bias[l]));
+    for (int s0 = 0; s0 < n_slots; s0 += GRID_YZ)
+      lstm_tc_weights_kernel<<<dim3(64, min(n_slots - s0, GRID_YZ)), 256, 0, st>>>(params, pstride, p.kofs[l], p.in[l], p.ur[l], p.u[l], p.kp_below[l],
+                                                                                  p.kp[l], l > 0, s0, reinterpret_cast<__half*>(ws + p.w_hi[l]),
+                                                                                  reinterpret_cast<__half*>(ws + p.w_lo[l]), reinterpret_cast<float*>(ws + p.bias[l]));
   const int xr_max = max_windows + p.L - 1;
-  lstm_tc_xk_kernel<<<dim3((xr_max + 31) / 32, 4 * p.u[0] / 64, n_jobs), 256, 0, st>>>(jobs, x, p.F, p.ur[0], p.u[0], p.L, params, pstride,
-                                                                                       reinterpret_cast<float*>(ws + p.xk));
+  for (int j0 = 0; j0 < n_jobs; j0 += GRID_YZ)
+    lstm_tc_xk_kernel<<<dim3((xr_max + 31) / 32, 4 * p.u[0] / 64, min(n_jobs - j0, GRID_YZ)), 256, 0, st>>>(jobs, j0, x, p.F, p.ur[0], p.u[0], p.L, params,
+                                                                                                        pstride, p.xk_blocks, reinterpret_cast<float*>(ws + p.xk));
   GB_CUDA_CHECK(cudaMemsetAsync(ws + p.state_begin, 0, p.state_end - p.state_begin, st));
   GB_CUDA_CHECK(cudaGetLastError());
 
@@ -455,7 +467,7 @@ extern "C" int gb_lstm_infer_tc(const gb_lstmnet* net, const float* params, int3
       a.u = p.u[l]; a.kc_below = p.kp_below[l] / KC; a.kc_own = p.u[l] / KC; a.act = net->act[l];
       a.tiles_per_job = tiles_per_job; a.t = t; a.jobs = jobs;
       a.bias = reinterpret_cast<const float*>(ws + p.bias[l]);
-      a.xk = reinterpret_cast<const float*>(ws + p.xk); a.xk_rows = x_rows;
+      a.xk = reinterpret_cast<const float*>(ws + p.xk); a.xk_blocks = p.xk_blocks;
       a.c = reinterpret_cast<float*>(ws + p.c[l]);
       a.h_out_hi = reinterpret_cast<__half*>(ws + p.h_hi[l][wr]);
       a.h_out_lo = reinterpret_cast<__half*>(ws + p.h_lo[l][wr]);
@@ -468,9 +480,10 @@ extern "C" int gb_lstm_infer_tc(const gb_lstmnet* net, const float* params, int3
     }
   }
   const int top = p.nl - 1, fin = (p.L - 1) & 1;
-  lstm_tc_head_kernel<<<dim3(tiles_per_job, n_jobs), TILE, 0, st>>>(jobs, tiles_per_job, reinterpret_cast<const __half*>(ws + p.h_hi[top][fin]),
-                                                                     reinterpret_cast<const __half*>(ws + p.h_lo[top][fin]), p.ur[top], p.u[top], p.n_out, net->out_act,
-                                                                     params, pstride, p.dofs, out_model);
+  for (int j0 = 0; j0 < n_jobs; j0 += GRID_YZ)
+    lstm_tc_head_kernel<<<dim3(tiles_per_job, min(n_jobs - j0, GRID_YZ)), TILE, 0, st>>>(jobs, j0, tiles_per_job, reinterpret_cast<const __half*>(ws + p.h_hi[top][fin]),
+                                                                                          reinterpret_cast<const __half*>(ws + p.h_lo[top][fin]), p.ur[top], p.u[top],
+                                                                                          p.n_out, net->out_act, params, pstride, p.dofs, out_model);
   GB_CUDA_CHECK(cudaGetLastError());
   return GB_OK;
 }

@@ -110,6 +110,12 @@ int gb_ffae_infer_score(const gb_ffnet* net, const float* params, const gb_job* 
 /* GB_OK if the tensor-core (variant 2) kernel covers this architecture, else GB_E_SHAPE. */
 int gb_ffae_tc_supported(const gb_ffnet* net);
 
+/* The launch plan of the generic (variant 1) kernel for this architecture, without launching: rows per tile (128, 64 or 32)
+ * and whether every layer's weights stay resident in shared memory (1) or are staged layer by layer (0; a layer too large to
+ * stage whole next to the activations is staged in blocks of output columns).  GB_E_SMEM exactly when gb_ffae_infer_score
+ * would refuse the architecture on variant 1 for shared memory; either output may be NULL. */
+int gb_ffae_infer_plan(const gb_ffnet* net, int32_t* rows_per_tile, int32_t* resident);
+
 /* ---- K4 alone: anomaly score of predictions that already exist ----------------------------
  * Same outputs as gb_ffae_infer_score, for a `yhat` produced elsewhere (a base estimator that is not
  * one of ours, e.g. the sklearn regressors the reference's detector tests use; an LSTM prediction from
@@ -296,7 +302,8 @@ size_t gb_lstm_workspace_bytes(const gb_lstmnet* net, int32_t n_jobs, int32_t ma
 int gb_lstm_infer(const gb_lstmnet* net, const float* params, const gb_job* jobs, int32_t n_jobs,
                   int32_t max_rows, const float* x, float* out_model, void* workspace, void* stream);
 
-/* ---- K3 on the tensor cores, wgmma (layer widths 1..512, padded to multiples of 64 internally).  One launch per
+/* ---- K3 on the tensor cores, wgmma (layer widths 1..512, padded to multiples of 64 internally; tanh and sigmoid cells
+ * only, since h is carried as an FP16 pair and a relu or linear cell's h is unbounded).  One launch per
  * (layer, timestep) advances every window of every job: [h_below,t | h_own,t-1] . [K; U]^T on the tensor cores
  * (FP16-pair split operands, fp32 accumulation), LSTM cell in the epilogue, recurrent state in `workspace`
  * (gb_lstm_tc_workspace_bytes; x_rows = rows of the x array, n_slots = rows of params). */
