@@ -9,6 +9,7 @@ number a `gordo build` user sees.
     python benchmarks/bench_fleet_builder.py --lstm [--lookback 24] --machines 16 --rows 2000 --tags 16 --epochs 1 --single 16
     python benchmarks/bench_fleet_builder.py --example-config --machines 125 --rows 10000 --tags 64 --epochs 10 --single 3
     python benchmarks/bench_fleet_builder.py --early-stopping --machines 125 --rows 10000 --tags 64 --epochs 100 --single 1
+    python benchmarks/bench_fleet_builder.py --kfcv --machines 125 --rows 10000 --tags 64 --epochs 20 --single 1
 
 ``--lstm`` builds DiffBasedAnomalyDetector(KerasLSTMAutoEncoder(lstm_hourglass)) machines instead (batched by
 fleet.build_lstm_fleet).  ``--example-config`` builds the model of gordo's examples/model-configuration.yaml:
@@ -17,7 +18,13 @@ DiffBasedAnomalyDetector(shuffle=True) around Pipeline([MinMaxScaler, KerasAutoE
 the reference's production definition to that model, EarlyStopping(monitor=val_loss, patience=10, restore_best_weights=True), and
 also reports the epochs each fit ran (min / median / max over all final and CV-fold fits) and the time of the bucket's fit
 launch with the rule against the same launch with patience = epochs (never stops), alternating, CUDA events around the launch
-after a warm-up.  Measured numbers and the card they were measured on are in DESIGN.md §7.
+after a warm-up.  ``--kfcv`` builds the reference's production definition: DiffBasedKFCVAnomalyDetector(window 144, shuffle,
+threshold_percentile 0.975) around TransformedTargetRegressor(MinMaxScaler, Pipeline([MinMaxScaler, KerasAutoEncoder(feedforward_hourglass,
+compression_factor 0.5, 1 encoding layer, batch 128, validation_split 0.1, EarlyStopping(val_loss, patience 10, restore_best_weights))]))
+under KFold(5, shuffle=True, random_state=0), with FleetModelBuilder(early_stopping=True, kfcv=True); it also reports the device
+time of the K-fold threshold stage (errors back to time order, smoothing, percentile, metric moments: the launches
+fleet.build_kfold_fleet makes after the fold scoring, on arrays of the bucket's shape), CUDA events, after a warm-up.
+Measured numbers and the card they were measured on are in DESIGN.md §5b and §7.
 """
 import argparse, json, os, sys, tempfile, time
 sys.path.insert(0, os.path.abspath(os.path.join(os.path.dirname(__file__), "..")))
@@ -48,6 +55,7 @@ def main():
     ap.add_argument("--early-stopping", action="store_true", help="--example-config with EarlyStopping(val_loss, patience=10, restore_best_weights)")
     ap.add_argument("--launch-runs", type=int, default=3, help="--early-stopping: timed fit launches of each kind")
     ap.add_argument("--min-delta", type=float, default=0.0, help="--early-stopping: the callback's min_delta (the reference's definition has none)")
+    ap.add_argument("--kfcv", action="store_true", help="the reference's production definition: a K-fold detector under KFold(5, shuffle, random_state=0)")
     a = ap.parse_args()
     import numpy as np
     import pandas as pd
@@ -74,6 +82,17 @@ def main():
             "base_estimator": {"sklearn.pipeline.Pipeline": {"steps": ["sklearn.preprocessing.MinMaxScaler", ae]}},
             "scaler": "sklearn.preprocessing.MinMaxScaler", "shuffle": True, "smoothing_method": "smm"}}
         evaluation, n_splits = {"cv": {"sklearn.model_selection.TimeSeriesSplit": {"n_splits": 5}}}, 5
+    if a.kfcv:
+        ae = {"gordo.machine.model.models.KerasAutoEncoder": {
+            "kind": "feedforward_hourglass", "batch_size": 128, "compression_factor": 0.5, "encoding_layers": 1, "func": "tanh", "out_func": "linear",
+            "epochs": a.epochs, "validation_split": 0.1, "callbacks": [{"tensorflow.keras.callbacks.EarlyStopping": stopping}]}}
+        model = {"gordo.machine.model.anomaly.diff.DiffBasedKFCVAnomalyDetector": {
+            "base_estimator": {"sklearn.compose.TransformedTargetRegressor": {
+                "transformer": "sklearn.preprocessing.MinMaxScaler",
+                "regressor": {"sklearn.pipeline.Pipeline": {"steps": ["sklearn.preprocessing.MinMaxScaler", ae]}}}},
+            "scaler": "sklearn.preprocessing.MinMaxScaler", "window": 144, "shuffle": True, "threshold_percentile": 0.975}}
+        evaluation, n_splits = {"cv": {"sklearn.model_selection.KFold": {"n_splits": 5, "shuffle": True, "random_state": 0}}}, 5
+    flags = dict(early_stopping=a.early_stopping or a.kfcv, kfcv=a.kfcv)
     rng = np.random.default_rng(0)
     idx = pd.date_range("2019-01-01", periods=a.rows, freq="10min", tz="UTC")
     t = np.linspace(0, 60, a.rows)[:, None]
@@ -83,11 +102,11 @@ def main():
         frame = pd.DataFrame(values.astype(np.float32), index=idx, columns=[f"tag-{i}" for i in range(a.tags)])
         machines.append({"name": f"machine-{m}", "model": model, "dataset": {"X": frame, "y": frame}, "evaluation": evaluation})
 
-    builder.FleetModelBuilder(machines[:2], early_stopping=a.early_stopping).build()  # warm-up: library load, first launches
+    builder.FleetModelBuilder(machines[:2], **flags).build()  # warm-up: library load, first launches
     torch.cuda.synchronize()
     with tempfile.TemporaryDirectory() as out:
         t0 = time.perf_counter()
-        results = builder.FleetModelBuilder(machines, early_stopping=a.early_stopping).build(out)
+        results = builder.FleetModelBuilder(machines, **flags).build(out)
         torch.cuda.synchronize()
         fleet_s = time.perf_counter() - t0
         size = sum(os.path.getsize(os.path.join(out, m["name"], f)) for _, m in results for f in ("model.pkl", "metadata.json"))
@@ -102,7 +121,10 @@ def main():
     net = f"LSTM hourglass (lookback {a.lookback})" if a.lstm else "hourglass"
     if a.example_config or a.early_stopping:
         net = "hourglass (compression 0.6, 1 encoding layer, batch 128, validation_split 0.1) in a shuffling detector"
-    if a.early_stopping:
+    if a.kfcv:
+        net = ("K-fold detector (window 144, percentile 0.975) around TransformedTargetRegressor(MinMaxScaler) of a hourglass (compression 0.5, "
+               "1 encoding layer, batch 128, validation_split 0.1), KFold(5, shuffle, random_state=0)")
+    if a.early_stopping or a.kfcv:
         net += f", EarlyStopping(val_loss, patience 10, min_delta {a.min_delta:g}, restore_best_weights)"
     out = {
         "gpu": torch.cuda.get_device_name(0), "power_limit_w": _power_limit(),
@@ -114,7 +136,60 @@ def main():
     }
     if a.early_stopping:
         out.update(_stop_launches(a, machines, stopping))
+    if a.kfcv:
+        ran = np.asarray([len(r.base_estimator.regressor_.steps[-1][1]._history.epoch) for r, _ in results])
+        out.update({"final_fit_epochs_run_min": int(ran.min()), "final_fit_epochs_run_median": float(np.median(ran)), "final_fit_epochs_run_max": int(ran.max())})
+        out.update(_kfold_threshold_stage(a))
     print(json.dumps(out))
+
+
+def _kfold_threshold_stage(a, runs: int = 5):
+    """
+    Device time of the K-fold threshold stage of fleet.build_kfold_fleet for this bucket's shape, the same launches in the same
+    order: the float64 fold errors (per tag and aggregate) back to time order as float32, rolling median over 144 rows, the 0.975
+    quantile, and the metric moments of the K*M test blocks.  CUDA events around the stage, after one warm-up.
+    """
+    import numpy as np
+    import torch
+    from sklearn.model_selection import KFold
+
+    from gordo_components_b200 import engine, fleet
+
+    dev = engine.cuda_device()
+    M, N, T = a.machines, a.rows, a.tags
+    tests, _, _, inverse = fleet.kfold_layout(KFold(5, shuffle=True, random_state=0), N)
+    K = len(tests)
+    n_test = np.asarray([len(t) for t in tests])
+    o = np.concatenate([[0], np.cumsum(n_test)[:-1]])
+    g = torch.Generator(device=dev).manual_seed(0)
+    tag_err = torch.rand((M * N, T), dtype=torch.float64, device=dev, generator=g)
+    tot_err = torch.rand((M * N,), dtype=torch.float64, device=dev, generator=g)
+    pred = torch.rand((M * N, T), dtype=torch.float32, device=dev, generator=g)
+    y32 = torch.rand((M * N, T), dtype=torch.float32, device=dev, generator=g)
+    whole = engine.jobs_to_device(engine.make_jobs(np.arange(M), N, np.arange(M) * N), dev)
+    fk, fm = np.repeat(np.arange(K), M), np.tile(np.arange(M), K)
+    blocks = engine.jobs_to_device(engine.make_jobs(M + np.arange(K * M), n_test[fk], fm * N + o[fk]), dev)
+    to_time = torch.from_numpy(inverse.astype(np.int32)).to(dev)
+
+    def stage():
+        tag_t = engine.gather_rows(whole, M, N, to_time, tag_err, M * N, to_f32=True)
+        tot_t = engine.gather_rows(whole, M, N, to_time, tot_err, M * N, to_f32=True)
+        tag_t = engine.smooth(whole, M, tag_t, 144, "smm", max_rows=N)
+        tot_t = engine.smooth(whole, M, tot_t, 144, "smm", max_rows=N)
+        engine.quantile(whole, M, N, tag_t, 0.975)
+        engine.quantile(whole, M, N, tot_t, 0.975)
+        engine.cv_moments(blocks, K * M, pred, y32, T)
+
+    stage()
+    ms = []
+    for _ in range(runs):
+        ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
+        ev[0].record()
+        stage()
+        ev[1].record()
+        torch.cuda.synchronize()
+        ms.append(ev[0].elapsed_time(ev[1]))
+    return {"threshold_stage_ms": ms}
 
 
 def _stop_launches(a, machines, stopping):

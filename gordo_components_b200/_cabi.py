@@ -22,7 +22,7 @@ ACT_CODES = {"linear": 0, None: 0, "tanh": 1, "relu": 2, "sigmoid": 3}
 
 EXPORTS = (
     "gb_abi_version", "gb_last_error", "gb_device_check", "gb_ffnet_param_count", "gb_ffnet_param_stride",
-    "gb_ffae_infer_score", "gb_ffae_tc_supported", "gb_ffae_infer_plan", "gb_anomaly_score", "gb_anomaly_score_f64", "gb_minmax_fit", "gb_minmax_f64", "gb_thresholds", "gb_thresholds_f64", "gb_cv_moments", "gb_smooth", "gb_quantile", "gb_affine_f64", "gb_ffae_fit_state_stride", "gb_ffae_fit", "gb_ffae_fit_split", "gb_ffae_fit_stop", "gb_ffae_fit_plan",
+    "gb_ffae_infer_score", "gb_ffae_tc_supported", "gb_ffae_infer_plan", "gb_anomaly_score", "gb_anomaly_score_f64", "gb_minmax_fit", "gb_minmax_f64", "gb_thresholds", "gb_thresholds_f64", "gb_cv_moments", "gb_smooth", "gb_quantile", "gb_affine_f64", "gb_gather_rows", "gb_minmax_inverse_f32", "gb_ffae_fit_state_stride", "gb_ffae_fit", "gb_ffae_fit_split", "gb_ffae_fit_stop", "gb_ffae_fit_plan",
     "gb_lstm_param_count", "gb_lstm_param_stride", "gb_lstm_workspace_bytes", "gb_lstm_infer", "gb_lstm_tc_supported", "gb_lstm_tc_workspace_bytes", "gb_lstm_infer_tc", "gb_lstm_fit_workspace_bytes", "gb_lstm_fit",
     "gb_orthonormal_rows",
 )
@@ -119,6 +119,10 @@ def _declare(lib):
     lib.gb_quantile.restype = C.c_int
     lib.gb_affine_f64.argtypes = [_P, C.c_int32, C.c_int32, _P, C.c_int32, _P, _P, _P, _P]
     lib.gb_affine_f64.restype = C.c_int
+    lib.gb_gather_rows.argtypes = [_P, C.c_int32, C.c_int32, _P, _P, C.c_int32, C.c_int32, C.c_int32, _P, _P]
+    lib.gb_gather_rows.restype = C.c_int
+    lib.gb_minmax_inverse_f32.argtypes = [_P, C.c_int32, C.c_int32, _P, C.c_int32, _P, _P, _P, _P, _P]
+    lib.gb_minmax_inverse_f32.restype = C.c_int
     lib.gb_ffae_fit.argtypes = [C.POINTER(GbFFNet), _P, _P, _P, _P, C.c_int32, C.c_int32, _P, _P, _P,
                                 C.POINTER(GbFitHParams), _P, _P, _P]
     lib.gb_ffae_fit_split.argtypes = [C.POINTER(GbFFNet), _P, _P, _P, _P, _P, C.c_int32, C.c_int32, _P, _P, _P, _P,

@@ -16,7 +16,8 @@ lookback, lookahead and training length and built by ``fleet.build_lstm_fleet``:
 chunks that fit a workspace budget), every fold model's test block in one LSTM inference launch, float64 scoring.  The
 cross-validation ``scores`` block of the metadata is then assembled on the host from ``gb_cv_moments``' five sums per
 (fold, tag).  Any other definition (other transformers in a Pipeline, callbacks unless batched as above, LSTM fits with
-callbacks, K-fold detectors, custom metrics ...) goes through ``ModelBuilder``: one machine at a time, still on the GPU through the estimators' own fit / predict.
+callbacks, K-fold detectors unless ``FleetModelBuilder(kfcv=True)`` batches them under a KFold cv through ``fleet.build_kfold_fleet``,
+custom metrics ...) goes through ``ModelBuilder``: one machine at a time, still on the GPU through the estimators' own fit / predict.
 
 Machines are plain dicts in the layout of ``Machine.to_dict()`` (gordo/machine/machine.py:226-246): ``name``, ``model`` (a
 definition), ``dataset``, and optionally ``project_name``, ``evaluation``, ``metadata``, ``runtime``.  ``dataset`` is
@@ -38,7 +39,8 @@ import numpy as np
 import pandas as pd
 from sklearn import metrics as sk_metrics
 from sklearn.base import BaseEstimator
-from sklearn.model_selection import TimeSeriesSplit, cross_validate
+from sklearn.compose import TransformedTargetRegressor
+from sklearn.model_selection import KFold, TimeSeriesSplit, cross_validate
 from sklearn.pipeline import Pipeline
 from sklearn.preprocessing import MinMaxScaler
 
@@ -156,17 +158,18 @@ def extract_metadata_from_model(model, metadata: Optional[dict] = None) -> dict:
     return out
 
 
-def scores_from_moments(moments: np.ndarray, n_rows: int, scoring_scale: Optional[np.ndarray] = None,
+def scores_from_moments(moments: np.ndarray, n_rows, scoring_scale: Optional[np.ndarray] = None,
                         metrics: Sequence[str] = MOMENT_METRICS) -> Dict[str, Tuple[np.ndarray, np.ndarray]]:
     """
     The four evaluation metrics of one machine from ``gb_cv_moments``: ``moments`` is ``[folds, 5, tags]`` (sum e, sum e^2,
     sum |e|, sum (y-y0), sum (y-y0)^2 over the fold's ``n_rows`` test rows, e = prediction - target), ``scoring_scale`` the
     per-tag ``scale_`` of the scoring scaler fitted on all targets (an affine map per tag: errors scale by it, the two
-    ratio metrics do not change).  Returns ``{metric: (per_tag [folds, tags], averaged [folds])}`` with sklearn's
+    ratio metrics do not change).  ``n_rows``: the test rows of every fold (an int), or one count per fold (KFold folds differ
+    in size by one row).  Returns ``{metric: (per_tag [folds, tags], averaged [folds])}`` with sklearn's
     conventions: uniform average over tags; a constant target scores 1 when predicted exactly and 0 otherwise.
     """
     m = np.asarray(moments, dtype=np.float64)
-    n = float(n_rows)
+    n = float(n_rows) if np.ndim(n_rows) == 0 else np.asarray(n_rows, dtype=np.float64).reshape(-1, 1)  # per fold, against [folds, tags]
     se, see, sae, sc, scc = (m[..., q, :] for q in range(5))
     s = 1.0 if scoring_scale is None else np.asarray(scoring_scale, dtype=np.float64)
 
@@ -350,22 +353,15 @@ def _canonical(index, machine, early_stopping: bool = False) -> Optional[_Canoni
     """
     from .machine.model.anomaly.diff import DiffBasedAnomalyDetector
     from .machine.model.factories.specs import FFNetSpec
-    from .machine.model.models import KerasAutoEncoder, build_callbacks
 
     def no(reason):
         logger.info("machine %s takes the per-machine path: %s", machine["name"], reason)
         return None
 
     evaluation = {**DEFAULT_EVALUATION, **(machine.get("evaluation") or {})}
-    if str(evaluation["cv_mode"]).lower() != "full_build":
-        return no(f"cv_mode {evaluation['cv_mode']}")
-    if any(m.rpartition(".")[2] not in MOMENT_METRICS or ("." in m and not m.startswith("sklearn.metrics.")) for m in evaluation["metrics"]):
-        return no("evaluation metrics beyond the four moment metrics")
-    scoring = evaluation.get("scoring_scaler")
-    if scoring:
-        scoring = serializer.from_definition(scoring) if isinstance(scoring, (str, dict)) else scoring
-        if not _default_minmax(scoring):
-            return no("scoring_scaler is not a default MinMaxScaler")
+    reason = _evaluation_refusal(evaluation)
+    if reason:
+        return no(reason)
     split_obj = serializer.from_definition(evaluation.get("cv", DEFAULT_CV))
     if type(split_obj) is not TimeSeriesSplit or split_obj.max_train_size is not None or split_obj.test_size is not None or split_obj.gap:
         return no("cv is not a plain TimeSeriesSplit")
@@ -375,25 +371,12 @@ def _canonical(index, machine, early_stopping: bool = False) -> Optional[_Canoni
         return no("model is not a plain DiffBasedAnomalyDetector")
     if not _default_minmax(model.scaler):
         return no("detector scaler is not a default MinMaxScaler")
-    ae, input_scaler = model.base_estimator, False
-    if type(ae) is Pipeline and len(ae.steps) == 2 and _default_minmax(ae.steps[0][1]):
-        ae, input_scaler = ae.steps[1][1], True  # Pipeline([MinMaxScaler(), KerasAutoEncoder]): gordo's example config
-    if type(ae) is not KerasAutoEncoder:
+    ae, input_scaler = _ff_network(model.base_estimator)
+    if ae is None:
         return no("base_estimator is not a KerasAutoEncoder, bare or behind one default MinMaxScaler")
-    fit_args = ae.extract_supported_fit_args(ae.kwargs)
-    stopping = None
-    if fit_args.get("callbacks"):
-        if not early_stopping:
-            return no("callbacks need the per-epoch loop (FleetModelBuilder(early_stopping=True) batches one EarlyStopping)")
-        definitions = fit_args["callbacks"]
-        definitions = list(definitions) if isinstance(definitions, (list, tuple)) else [definitions]
-        callbacks = build_callbacks(definitions)
-        if len(definitions) != 1 or len(callbacks) != 1:  # several callbacks, or one the fit loop does not know
-            return no("callbacks other than one EarlyStopping need the per-epoch loop")
-        stopping = callbacks[0]
-    vsplit = float(fit_args.get("validation_split") or 0.0)
-    if vsplit and not 0.0 < vsplit < 1.0:
-        return no(f"validation_split {vsplit} is outside (0, 1)")
+    reason, fit_args, stopping, vsplit = _ff_fit_arguments(ae, early_stopping)
+    if reason:
+        return no(reason)
 
     t0 = time.time()
     X, y, dataset_meta = _get_data(machine["dataset"])
@@ -407,16 +390,70 @@ def _canonical(index, machine, early_stopping: bool = False) -> Optional[_Canoni
         return no("too few rows for the CV folds")
     if vsplit and math.floor((len(X) - split_obj.n_splits * test) * (1.0 - vsplit)) < 1:  # the smallest fold: keras' split (models.py)
         return no(f"validation_split {vsplit} leaves the first CV fold without a training row")
-    if stopping is not None:
-        available = {"loss"} | ({"accuracy"} if "accuracy" in spec.metrics else set())
-        if vsplit:
-            available |= {"val_" + k for k in available}
-        if stopping.monitor not in available:
-            return no(f"EarlyStopping monitors {stopping.monitor!r}, which this fit does not report")
+    reason = _monitor_refusal(stopping, spec, vsplit)
+    if reason:
+        return no(reason)
     fit = {"epochs": int(fit_args.get("epochs", 1)), "batch_size": int(fit_args.get("batch_size") or 32), "shuffle": bool(fit_args.get("shuffle", True))}
     split = (bool(model.shuffle), vsplit, int(fit_args.get("validation_batch_size") or fit["batch_size"]) if vsplit else None)
     return _Canonical(index, machine, model, spec, X, y, dataset_meta, query_sec, fit, split_obj.n_splits, evaluation, input_scaler, split,
                       stopping)
+
+
+def _evaluation_refusal(evaluation: dict) -> Optional[str]:
+    """Why the batched path cannot reproduce this evaluation's metadata (cv aside), or None."""
+    if str(evaluation["cv_mode"]).lower() != "full_build":
+        return f"cv_mode {evaluation['cv_mode']}"
+    if any(m.rpartition(".")[2] not in MOMENT_METRICS or ("." in m and not m.startswith("sklearn.metrics.")) for m in evaluation["metrics"]):
+        return "evaluation metrics beyond the four moment metrics"
+    scoring = evaluation.get("scoring_scaler")
+    if scoring:
+        scoring = serializer.from_definition(scoring) if isinstance(scoring, (str, dict)) else scoring
+        if not _default_minmax(scoring):
+            return "scoring_scaler is not a default MinMaxScaler"
+    return None
+
+
+def _ff_network(est):
+    """(the KerasAutoEncoder, whether a default MinMaxScaler is in front of it) of a bare AE or ``Pipeline([MinMaxScaler(), AE])``; (None, False) otherwise."""
+    from .machine.model.models import KerasAutoEncoder
+
+    input_scaler = False
+    if type(est) is Pipeline and len(est.steps) == 2 and _default_minmax(est.steps[0][1]):
+        est, input_scaler = est.steps[1][1], True  # Pipeline([MinMaxScaler(), KerasAutoEncoder]): gordo's example config
+    return (est, input_scaler) if type(est) is KerasAutoEncoder else (None, False)
+
+
+def _ff_fit_arguments(ae, early_stopping: bool):
+    """(refusal or None, fit arguments, the one EarlyStopping callback or None, validation_split) of a feed-forward estimator."""
+    from .machine.model.models import build_callbacks
+
+    fit_args = ae.extract_supported_fit_args(ae.kwargs)
+    stopping = None
+    if fit_args.get("callbacks"):
+        if not early_stopping:
+            return "callbacks need the per-epoch loop (FleetModelBuilder(early_stopping=True) batches one EarlyStopping)", fit_args, None, 0.0
+        definitions = fit_args["callbacks"]
+        definitions = list(definitions) if isinstance(definitions, (list, tuple)) else [definitions]
+        callbacks = build_callbacks(definitions)
+        if len(definitions) != 1 or len(callbacks) != 1:  # several callbacks, or one the fit loop does not know
+            return "callbacks other than one EarlyStopping need the per-epoch loop", fit_args, None, 0.0
+        stopping = callbacks[0]
+    vsplit = float(fit_args.get("validation_split") or 0.0)
+    if vsplit and not 0.0 < vsplit < 1.0:
+        return f"validation_split {vsplit} is outside (0, 1)", fit_args, stopping, vsplit
+    return None, fit_args, stopping, vsplit
+
+
+def _monitor_refusal(stopping, spec, vsplit: float) -> Optional[str]:
+    """Why the fit cannot apply this EarlyStopping callback (a monitor it does not report), or None."""
+    if stopping is None:
+        return None
+    available = {"loss"} | ({"accuracy"} if "accuracy" in spec.metrics else set())
+    if vsplit:
+        available |= {"val_" + k for k in available}
+    if stopping.monitor not in available:
+        return f"EarlyStopping monitors {stopping.monitor!r}, which this fit does not report"
+    return None
 
 
 class _CanonicalLSTM(_Canonical):
@@ -508,6 +545,94 @@ def _canonical_lstm(index, machine) -> Optional[_CanonicalLSTM]:
     return _CanonicalLSTM(index, machine, model, spec, X, y, dataset_meta, query_sec, fit, K, evaluation, input_scaler, lookahead=la)
 
 
+class _CanonicalKFold(_Canonical):
+    """A machine whose ``DiffBasedKFCVAnomalyDetector`` can take the batched path (``fleet.build_kfold_fleet``)."""
+
+    def __init__(self, *args, cv, target_scaler: bool):
+        super().__init__(*args)
+        self.cv, self.target_scaler = cv, target_scaler
+
+    def bucket(self):
+        m = self.model  # every field below is a scalar of the shared row maps or of the gb_smooth / gb_quantile launches
+        return super().bucket() + ((self.cv.n_splits, bool(self.cv.shuffle), self.cv.random_state), m.window, m.smoothing_method,
+                                   float(m.threshold_percentile), bool(m.shuffle), self.target_scaler)
+
+
+def _is_kfcv_definition(machine) -> bool:
+    from .machine.model.anomaly.diff import DiffBasedKFCVAnomalyDetector
+
+    try:
+        return type(serializer.from_definition(machine["model"])) is DiffBasedKFCVAnomalyDetector
+    except Exception:  # ModelBuilder raises the definition's own error
+        return False
+
+
+def _canonical_kfcv(index, machine, early_stopping: bool = False) -> Optional[_CanonicalKFold]:
+    """
+    A ``DiffBasedKFCVAnomalyDetector`` machine as a candidate for the batched path (``FleetModelBuilder(kfcv=True)``), or ``None``
+    with the reason logged.  The detector has a default MinMaxScaler, an int or no ``window`` and smm / sma / ewma smoothing; its
+    estimator is a feed-forward ``KerasAutoEncoder``, bare or behind one default MinMaxScaler, optionally inside a
+    ``TransformedTargetRegressor`` with a default MinMaxScaler transformer; the fit arguments are those ``_canonical`` takes; the
+    evaluation's cv is a ``KFold`` that is unshuffled or seeded with an int, so every machine of a bucket gets the same folds.
+    """
+    import numbers
+
+    from .machine.model.factories.specs import FFNetSpec
+
+    def no(reason):
+        logger.info("machine %s takes the per-machine path: %s", machine["name"], reason)
+        return None
+
+    evaluation = {**DEFAULT_EVALUATION, **(machine.get("evaluation") or {})}
+    reason = _evaluation_refusal(evaluation)
+    if reason:
+        return no(reason)
+    cv = serializer.from_definition(evaluation.get("cv", DEFAULT_CV))
+    if type(cv) is not KFold:
+        return no("a K-fold detector is batched under a KFold cv only")
+    if cv.shuffle and (not isinstance(cv.random_state, numbers.Integral) or isinstance(cv.random_state, bool)):
+        return no("a shuffled KFold without an int random_state gives every machine other folds")
+
+    model = serializer.from_definition(machine["model"])
+    if not _default_minmax(model.scaler):
+        return no("detector scaler is not a default MinMaxScaler")
+    if model.window is not None and (not isinstance(model.window, numbers.Integral) or isinstance(model.window, bool) or model.window < 1):
+        return no(f"window {model.window!r} is not a positive int")
+    if model.window is not None and model.smoothing_method not in ("smm", "sma", "ewma"):
+        return no(f"smoothing_method {model.smoothing_method!r}")
+    est, target_scaler = model.base_estimator, False
+    if type(est) is TransformedTargetRegressor:
+        if est.func is not None or est.inverse_func is not None or est.transformer is None or not _default_minmax(est.transformer):
+            return no("TransformedTargetRegressor without a default MinMaxScaler transformer")
+        est, target_scaler = est.regressor, True
+    ae, input_scaler = _ff_network(est)
+    if ae is None:
+        return no("the estimator is not a KerasAutoEncoder, bare or behind one default MinMaxScaler")
+    reason, fit_args, stopping, vsplit = _ff_fit_arguments(ae, early_stopping)
+    if reason:
+        return no(reason)
+
+    t0 = time.time()
+    X, y, dataset_meta = _get_data(machine["dataset"])
+    query_sec = time.time() - t0
+    ae.kwargs.update({"n_features": X.shape[1], "n_features_out": y.shape[1]})
+    spec = ae._build_spec()
+    if not isinstance(spec, FFNetSpec):
+        return no("not a feed-forward network")
+    if len(X) != len(y) or len(X) < cv.n_splits:
+        return no("too few rows for the CV folds")
+    smallest = len(X) - math.ceil(len(X) / cv.n_splits)  # the training rows of the largest test fold
+    if vsplit and math.floor(smallest * (1.0 - vsplit)) < 1:
+        return no(f"validation_split {vsplit} leaves a CV fold without a training row")
+    reason = _monitor_refusal(stopping, spec, vsplit)
+    if reason:
+        return no(reason)
+    fit = {"epochs": int(fit_args.get("epochs", 1)), "batch_size": int(fit_args.get("batch_size") or 32), "shuffle": bool(fit_args.get("shuffle", True))}
+    split = (bool(model.shuffle), vsplit, int(fit_args.get("validation_batch_size") or fit["batch_size"]) if vsplit else None)
+    return _CanonicalKFold(index, machine, model, spec, X, y, dataset_meta, query_sec, fit, cv.n_splits, evaluation, input_scaler, split, stopping,
+                           cv=cv, target_scaler=target_scaler)
+
+
 class FleetModelBuilder:
     """
     Build every machine of a project: ``FleetModelBuilder(machines).build(output_dir)`` -> ``[(model, machine_dict), ...]`` in
@@ -518,10 +643,15 @@ class FleetModelBuilder:
     fit reports (``loss``, ``accuracy``, their ``val_*`` forms with a ``validation_split``) -- the reference's production
     definition.  Every fit then applies the rule inside the fit launch (``fleet.build_fleet(early_stopping=...)``).  Off by
     default: such machines then build through ``ModelBuilder``, one epoch launch at a time, as they always have.
+
+    ``kfcv``: also batch ``DiffBasedKFCVAnomalyDetector`` machines under a ``KFold`` cv (``_canonical_kfcv``; the reference's
+    production definition), built by ``fleet.build_kfold_fleet``.  Off by default for the same reason: the batched fits draw their
+    initial weights per fleet, so without the flag these machines build through ``ModelBuilder`` as before.
     """
 
-    def __init__(self, machines: Sequence, early_stopping: bool = False):
+    def __init__(self, machines: Sequence, early_stopping: bool = False, kfcv: bool = False):
         self.early_stopping = bool(early_stopping)
+        self.kfcv = bool(kfcv)
         self.machines = [_machine_dict(m) for m in machines]
         names = [m["name"] for m in self.machines]
         if len(set(names)) != len(names):
@@ -534,13 +664,19 @@ class FleetModelBuilder:
         """
         from . import fleet
 
-        return FleetModelBuilder([self.machines[i] for i in fleet.partition(len(self.machines), world)[rank]], early_stopping=self.early_stopping)
+        return FleetModelBuilder([self.machines[i] for i in fleet.partition(len(self.machines), world)[rank]], early_stopping=self.early_stopping,
+                                 kfcv=self.kfcv)
 
     def build(self, output_dir: Optional[str] = None) -> List[Tuple[Any, dict]]:
         results: List[Optional[Tuple[Any, dict]]] = [None] * len(self.machines)
         buckets: Dict[tuple, List[_Canonical]] = {}
         for i, machine in enumerate(self.machines):
-            c = _canonical_lstm(i, machine) if _is_lstm_definition(machine) else _canonical(i, machine, early_stopping=self.early_stopping)
+            if _is_lstm_definition(machine):
+                c = _canonical_lstm(i, machine)
+            elif self.kfcv and _is_kfcv_definition(machine):
+                c = _canonical_kfcv(i, machine, early_stopping=self.early_stopping)
+            else:
+                c = _canonical(i, machine, early_stopping=self.early_stopping)
             if c is None:
                 results[i] = ModelBuilder(machine).build()
             else:
@@ -562,6 +698,8 @@ class FleetModelBuilder:
     def _build_bucket(members: List[_Canonical]) -> List[Tuple[Any, dict]]:
         if isinstance(members[0], _CanonicalLSTM):
             return FleetModelBuilder._build_lstm_bucket(members)
+        if isinstance(members[0], _CanonicalKFold):
+            return FleetModelBuilder._build_kfold_bucket(members)
         from . import engine, fleet
 
         first = members[0]
@@ -636,6 +774,47 @@ class FleetModelBuilder:
             dataset_block = {"query_duration_sec": c.query_sec, "dataset_meta": c.dataset_meta}
             out.append((model, _machine_out(c.machine, {"model": model_block, "dataset": dataset_block})))
         logger.info("built %d LSTM machines in one batched bucket", len(members))
+        return out
+
+    @staticmethod
+    def _build_kfold_bucket(members: List[_CanonicalKFold]) -> List[Tuple[Any, dict]]:
+        from . import engine, fleet
+
+        first = members[0]
+        eng = engine.ff_engine_for(first.spec)
+        rows, K = len(first.X), first.n_splits
+        torch = engine._torch()
+        t0 = time.time()
+        xd = torch.from_numpy(np.concatenate([np.ascontiguousarray(c.X.values, dtype=np.float64) for c in members])).to(eng.device)
+        same_y = all(c.y is c.X for c in members)
+        yd = xd if same_y else torch.from_numpy(np.concatenate([np.ascontiguousarray(c.y.values, dtype=np.float64) for c in members])).to(eng.device)
+        det = first.model
+        fb = fleet.build_kfold_fleet(eng, xd, yd, rows, first.cv, epochs=first.fit["epochs"], batch_size=first.fit["batch_size"],
+                                     seed=int(first.evaluation.get("seed", 0)), adam=first.spec.adam, shuffle=first.fit["shuffle"],
+                                     input_scaler=first.input_scaler, target_scaler=first.target_scaler, detector_shuffle=first.split[0],
+                                     validation_split=first.split[1], validation_batch_size=first.split[2],
+                                     early_stopping=None if first.early_stopping is None else [c.early_stopping for c in members],
+                                     window=det.window, smoothing_method=det.smoothing_method, threshold_percentile=det.threshold_percentile)
+        torch.cuda.synchronize()
+        share = (time.time() - t0) / len(members)  # the bucket's wall time, spread evenly: there is no per-machine time any more
+        out = []
+        for m, c in enumerate(members):
+            tags = list(c.y.columns)
+            model = fb.detector(m, c.model, tags=tags, input_tags=list(c.X.columns))
+            names = [s.rpartition(".")[2] for s in c.evaluation["metrics"]]
+            scoring_scale = model.scaler.scale_ if c.evaluation.get("scoring_scaler") else None  # the scoring scaler sees all targets too
+            scores = scores_block(scores_from_moments(fb.cv_moments[m], fb.n_test, scoring_scale, names), tags)
+            model_block = {
+                "model_offset": 0,  # a Dense stack answers every row
+                "model_creation_date": _now(),
+                "model_builder_version": __version__,
+                "model_training_duration_sec": share * 1.0 / (K + 1),
+                "cross_validation": {"scores": scores, "cv_duration_sec": share * K / (K + 1), "splits": build_split_dict(c.X, c.cv)},
+                "model_meta": extract_metadata_from_model(model),
+            }
+            dataset_block = {"query_duration_sec": c.query_sec, "dataset_meta": c.dataset_meta}
+            out.append((model, _machine_out(c.machine, {"model": model_block, "dataset": dataset_block})))
+        logger.info("built %d K-fold machines in one batched bucket", len(members))
         return out
 
 
@@ -756,15 +935,15 @@ def machines_from_config(config, project_name: str = "local-build", datasets=Non
     return machines
 
 
-def local_build(config_str, datasets=None, batched: bool = True, early_stopping: bool = False):
+def local_build(config_str, datasets=None, batched: bool = True, early_stopping: bool = False, kfcv: bool = False):
     """
     Build the model(s) of a bare gordo config locally and yield ``(model, machine)`` per machine, in config order
     (gordo/builder/local_build.py:15-80).  ``batched=False`` builds one machine at a time like the reference does;
-    ``early_stopping`` is ``FleetModelBuilder``'s.
+    ``early_stopping`` and ``kfcv`` are ``FleetModelBuilder``'s.
     """
     machines = machines_from_config(config_str, datasets=datasets)
     if batched:
-        yield from FleetModelBuilder(machines, early_stopping=early_stopping).build()
+        yield from FleetModelBuilder(machines, early_stopping=early_stopping, kfcv=kfcv).build()
     else:
         for machine in machines:
             yield ModelBuilder(machine).build()

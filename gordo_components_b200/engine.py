@@ -407,6 +407,50 @@ def affine_f64(jobs_dev, n_jobs, max_rows, x64, a, b, out_rows=None):
     return out
 
 
+def gather_rows(jobs_dev, n_jobs, max_rows, row_map, src, out_rows: int, to_f32: bool = False, out=None):
+    """
+    Row permutation per job (gb_gather_rows): out[out_row + p] = src[x_row + row_map[p]] for p < n_rows.  ``src``: [rows, cols]
+    or [rows] tensor of 4- or 8-byte elements; ``to_f32`` narrows float64 to float32 in the same pass.  ``row_map``: int32 device
+    tensor shared by every job.  Returns ``out`` ([out_rows, ...], allocated when not given).
+    """
+    torch = _torch()
+    lib = _cabi.load_library()
+    if row_map.dtype != torch.int32:
+        raise ValueError(f"gather_rows takes an int32 row map, got {row_map.dtype}")
+    if to_f32 and src.dtype != torch.float64:
+        raise ValueError(f"gather_rows narrows float64 to float32, got {src.dtype}")
+    n_cols = 1 if src.dim() == 1 else int(src.shape[1])
+    dtype = torch.float32 if to_f32 else src.dtype
+    if out is None:
+        out = torch.empty((int(out_rows),) + tuple(src.shape[1:]), dtype=dtype, device=src.device)
+    if out.dtype != dtype:
+        raise ValueError(f"gather_rows: out is {out.dtype}, expected {dtype}")
+    p = _cabi.ptr
+    _cabi.check(lib.gb_gather_rows(p(jobs_dev), int(n_jobs), int(max_rows), p(row_map), p(src), n_cols, int(src.element_size()), int(bool(to_f32)),
+                                   p(out), _stream_ptr()))
+    return out
+
+
+def minmax_inverse_f32(jobs_dev, n_jobs, max_rows, pred, scale, min_, out_rows=None, want=("f32", "f64")):
+    """
+    ``MinMaxScaler.inverse_transform`` of float32 predictions as sklearn computes it on a float32 array (gb_minmax_inverse_f32):
+    per job, rows of ``pred`` at x_row with the float64 ``scale_`` / ``min_`` of its slot, to rows at out_row.  Returns the
+    requested forms, ``{"f32": float32 tensor, "f64": the same values as float64}``.
+    """
+    torch = _torch()
+    lib = _cabi.load_library()
+    total = int(out_rows if out_rows is not None else pred.shape[0])
+    res = {}
+    if "f32" in want:
+        res["f32"] = torch.empty((total, pred.shape[1]), dtype=torch.float32, device=pred.device)
+    if "f64" in want:
+        res["f64"] = torch.empty((total, pred.shape[1]), dtype=torch.float64, device=pred.device)
+    p = _cabi.ptr
+    _cabi.check(lib.gb_minmax_inverse_f32(p(jobs_dev), int(n_jobs), int(max_rows), p(pred), int(pred.shape[1]), p(scale), p(min_), p(res.get("f32")),
+                                          p(res.get("f64")), _stream_ptr()))
+    return res
+
+
 def orthonormal_rows(g, out, out_offset: int, out_stride: int):
     """
     Keras' Orthogonal initialiser for every float64 standard-normal draw ``g`` [n, rows, cols] (overwritten): the rows

@@ -291,6 +291,42 @@ def dump_fleet(fb: "FleetBuild", root: str, names: Sequence[str], tags: Optional
     return out
 
 
+def _keras_initial_params(eng: "engine.FFEngine", n_slots: int, generator):
+    """Fresh Dense stacks for ``n_slots`` fits: glorot-uniform kernels and, as Keras initialises them, zero biases."""
+    params = random_glorot_params(eng, n_slots, generator)
+    ofs = 0
+    for i, o in zip(eng.dims[:-1], eng.dims[1:]):
+        ofs += i * o
+        params[:, ofs:ofs + o] = 0
+        ofs += o
+    return params
+
+
+def _fit_slots(eng, params, fit_jobs, n_jobs, max_rows, x, y, split, row_map, n_machines, epochs, batch_size, shuffle, adam, seed,
+               validation_batch_size, early_stopping):
+    """
+    The one fit launch of a bucket (job j trains a slot of machine j mod n_machines): gb_ffae_fit without held-out positions or a
+    row map, gb_ffae_fit_split with them, gb_ffae_fit_stop with an EarlyStopping callback (one for all machines or one per machine).
+    Returns (loss, acc, val_loss, val_acc, epochs_run, best_epoch); the last four None where the launch has none.
+    """
+    val_loss = val_acc = epochs_run = best_epoch = None
+    vb = validation_batch_size or batch_size
+    if early_stopping is not None:
+        per_machine = list(early_stopping) if isinstance(early_stopping, (list, tuple)) else [early_stopping] * n_machines
+        if len(per_machine) != n_machines:
+            raise ValueError(f"early_stopping: {len(per_machine)} callbacks for {n_machines} machines")
+        stop = engine.make_stop([per_machine[j % n_machines] for j in range(n_jobs)])
+        loss, acc, val_loss, val_acc, epochs_run, best_epoch, _ = eng.fit_split(
+            params, fit_jobs, n_jobs, max_rows, x, y, split=split, row_map=row_map, val_batch=vb, epochs=epochs, batch_size=batch_size,
+            shuffle=shuffle, adam=adam, seed=seed, stop=stop)
+    elif split is None:
+        loss, acc, _ = eng.fit(params, fit_jobs, n_jobs, max_rows, x, y, epochs=epochs, batch_size=batch_size, shuffle=shuffle, adam=adam, seed=seed)
+    else:
+        loss, acc, val_loss, val_acc, _ = eng.fit_split(params, fit_jobs, n_jobs, max_rows, x, y, split=split, row_map=row_map, val_batch=vb,
+                                                        epochs=epochs, batch_size=batch_size, shuffle=shuffle, adam=adam, seed=seed)
+    return loss, acc, val_loss, val_acc, epochs_run, best_epoch
+
+
 def build_fleet(eng: "engine.FFEngine", x, y, rows: int, epochs: int = 1, batch_size: int = 32, n_splits: int = 3, seed: int = 0,
                 adam: Optional[Dict[str, float]] = None, shuffle: bool = True, generator=None, input_scaler: bool = False,
                 detector_shuffle: bool = False, validation_split: float = 0.0, validation_batch_size: Optional[int] = None,
@@ -329,13 +365,7 @@ def build_fleet(eng: "engine.FFEngine", x, y, rows: int, epochs: int = 1, batch_
     starts = [N - (K - k) * test for k in range(K)]  # sklearn TimeSeriesSplit: fold k trains on [0, starts[k]), tests the next `test` rows
     g = generator or torch.Generator(device=dev).manual_seed(seed)
     # slots: [0, M) final models, then fold k of machine m at M + k*M + m
-    params = random_glorot_params(eng, M * (K + 1), g)
-    # Keras initialises biases to zero
-    ofs = 0
-    for i, o in zip(eng.dims[:-1], eng.dims[1:]):
-        ofs += i * o
-        params[:, ofs:ofs + o] = 0
-        ofs += o
+    params = _keras_initial_params(eng, M * (K + 1), g)
     base = np.arange(M, dtype=np.int64) * N
     slot_n = [N] + starts  # rows of the final fit, then of fold k
     vsplit = float(validation_split or 0.0)
@@ -371,25 +401,10 @@ def build_fleet(eng: "engine.FFEngine", x, y, rows: int, epochs: int = 1, batch_
     else:
         base_of = lambda k: base  # noqa: E731
     fit_jobs = engine.jobs_to_device(engine.make_jobs(fit_slots, fit_rows, fit_x), dev)
-    val_loss = val_acc = epochs_run = best_epoch = None
-    if early_stopping is not None:
-        per_machine = list(early_stopping) if isinstance(early_stopping, (list, tuple)) else [early_stopping] * M
-        if len(per_machine) != M:
-            raise ValueError(f"early_stopping: {len(per_machine)} callbacks for {M} machines")
-        stop = engine.make_stop([per_machine[j % M] for j in range(len(fit_slots))])  # job j trains a slot of machine j mod M
-        loss, acc, val_loss, val_acc, epochs_run, best_epoch, _ = eng.fit_split(
-            params, fit_jobs, len(fit_slots), N, x, y, split=split, row_map=row_map, val_batch=validation_batch_size or batch_size, epochs=epochs,
-            batch_size=batch_size, shuffle=shuffle, adam=adam, seed=seed, stop=stop)
-        if n_train == slot_n:  # nothing held out
-            val_loss = val_acc = None
-    elif split is None:
-        loss, acc, _ = eng.fit(params, fit_jobs, len(fit_slots), N, x, y, epochs=epochs, batch_size=batch_size, shuffle=shuffle, adam=adam, seed=seed)
-    else:
-        loss, acc, val_loss, val_acc, _ = eng.fit_split(params, fit_jobs, len(fit_slots), N, x, y, split=split, row_map=row_map,
-                                                        val_batch=validation_batch_size or batch_size, epochs=epochs, batch_size=batch_size,
-                                                        shuffle=shuffle, adam=adam, seed=seed)
-        if n_train == slot_n:  # shuffled, nothing held out
-            val_loss = val_acc = None
+    loss, acc, val_loss, val_acc, epochs_run, best_epoch = _fit_slots(
+        eng, params, fit_jobs, len(fit_slots), N, x, y, split, row_map, M, epochs, batch_size, shuffle, adam, seed, validation_batch_size, early_stopping)
+    if n_train == slot_n:  # nothing held out
+        val_loss = val_acc = None
     # scalers: final on all rows, fold k on its training prefix (diff.py:173 inside each CV clone), held-out rows included
     all_jobs = fit_jobs if n_train == slot_n else engine.jobs_to_device(engine.make_jobs(fit_slots, all_rows, fit_x), dev)
     scale, offset = eng.minmax_fit(all_jobs, len(fit_slots), N, y, M * (K + 1))
@@ -631,3 +646,281 @@ def build_lstm_fleet(eng: "engine.LSTMEngine", x, y, rows: int, lookahead: int =
         np.ascontiguousarray(fold_agg), np.ascontiguousarray(moments), pred.view(K, M, n_test, T).permute(1, 0, 2, 3),
         in_min=None if in_lo is None else in_lo[:M], in_max=None if in_hi is None else in_hi[:M],
         fold_in_min=None if in_lo is None else folds(in_lo), fold_in_max=None if in_hi is None else folds(in_hi))
+
+
+# ------------------------------------------------------------------------------------------------ fleet build of K-fold detectors
+class KFoldFleetBuild:
+    """
+    Result of ``build_kfold_fleet``: what ``ModelBuilder._build`` produces for one ``DiffBasedKFCVAnomalyDetector`` machine -- final
+    weights, target (and input) scaler extrema, the K-fold percentile thresholds, loss histories, CV metric moments -- for all
+    machines of a bucket.  Slot layout of ``params`` / ``init_params`` and of every ``slot_*`` array: final models at [0, M), fold k
+    of machine m at M + k*M + m.  Host arrays except ``params`` / ``init_params`` (device float32 [S, stride]).
+    """
+
+    def __init__(self, eng, n_machines, n_splits, rows, n_test, params, init_params, loss, acc, val_loss, val_acc, epochs, epochs_run,
+                 best_epoch, slot_steps, y_min, y_max, in_min, in_max, target_scaler, feat_thr, agg_thr, cv_moments):
+        self.eng, self.n_machines, self.n_splits, self.rows = eng, n_machines, n_splits, rows
+        self.n_test = n_test                                  # [K] test rows of every fold (KFold folds differ by one row at most)
+        self.params, self.init_params = params, init_params
+        # per slot [S, epochs] (val_* None without a validation_split; NaN past a fit's epochs_run with EarlyStopping)
+        self.loss, self.acc, self.val_loss, self.val_acc = loss, acc, val_loss, val_acc
+        self.epochs, self.epochs_run, self.best_epoch = epochs, epochs_run, best_epoch  # epochs_run / best_epoch [S] or None
+        self.slot_steps = slot_steps                          # [S] optimizer steps per epoch of every fit (History.params["steps"])
+        self.steps_per_epoch = int(slot_steps[0])             # ... of the final fits
+        # float64 column extrema per slot [S, T] of the targets (the detector's scaler and the TransformedTargetRegressor's
+        # transformer) and of the inputs (the Pipeline's MinMaxScaler; None without one)
+        self.y_min, self.y_max, self.in_min, self.in_max = y_min, y_max, in_min, in_max
+        self.target_scaler = target_scaler                    # the estimator is a TransformedTargetRegressor(MinMaxScaler)
+        self.feat_thr, self.agg_thr = feat_thr, agg_thr       # [M, T], [M] float64: feature_thresholds_ / aggregate_threshold_
+        self.cv_moments = cv_moments                          # [M, K, 5, T] float64 (gb_cv_moments of every fold's test block)
+
+    def detector(self, m: int, template, tags=None, input_tags=None):
+        """
+        Machine ``m`` as its fitted ``DiffBasedKFCVAnomalyDetector``: ``template`` is an unfitted detector from the machine's own
+        definition, filled in with the attributes the per-machine build leaves (picklable, servable).
+        """
+        import pandas as pd
+
+        det = self._fill(m, template, tags, input_tags)
+        det.feature_thresholds_ = pd.Series(self.feat_thr[m].copy(), index=list(tags) if tags is not None else list(range(self.eng.n_out)))
+        det.aggregate_threshold_ = float(self.agg_thr[m])
+        return det
+
+    def fold_detector(self, m: int, k: int, template, tags=None, input_tags=None):
+        """Fold k's detector of machine m (a ``cross_validate`` estimator: fitted on fold k's training rows, no thresholds)."""
+        return self._fill(self.n_machines + k * self.n_machines + m, template, tags, input_tags)
+
+    def _fill(self, s: int, template, tags, input_tags):
+        """``template`` with the fitted state of slot ``s``: scalers, weights, History, the target transformer."""
+        from sklearn.base import clone
+        from sklearn.compose import TransformedTargetRegressor
+        from sklearn.pipeline import Pipeline
+
+        from .machine.model.models import History
+
+        eng, M = self.eng, self.n_machines
+        n_rows = self.rows if s < M else self.rows - int(self.n_test[(s - M) // M])  # the rows the slot's scalers saw
+        T = eng.n_out
+        tags = list(tags) if tags is not None else list(range(T))
+        det = template
+        est = det.base_estimator
+        ttr = est if isinstance(est, TransformedTargetRegressor) else None
+        if (ttr is not None) != self.target_scaler:
+            raise ValueError("the template's target transformer and the fleet's do not match")
+        reg = clone(ttr.regressor) if ttr is not None else est
+        ae = reg.steps[-1][1] if isinstance(reg, Pipeline) else reg
+        if isinstance(reg, Pipeline) != (self.in_min is not None):
+            raise ValueError("the template's input scaler and the fleet's do not match")
+        if isinstance(reg, Pipeline):
+            _fill_minmax_from_extrema(reg.steps[0][1], self.in_min[s], self.in_max[s], n_rows, input_tags)
+        ae.kwargs.update({"n_features": eng.n_in, "n_features_out": T})
+        ae._prepare_model()
+        if list(ae.model.spec.dims) != list(eng.dims) or list(ae.model.spec.acts) != list(eng.acts):
+            raise ValueError("template architecture differs from the fleet's")
+        ae.model.weights = eng.unpack_params(self.params[s : s + 1])[0]
+        ran = int(self.epochs_run[s]) if self.epochs_run is not None else self.loss.shape[1]
+        hist = {"loss": [float(v) for v in self.loss[s, :ran]], "accuracy": [float(v) for v in self.acc[s, :ran]]}
+        if self.val_loss is not None:  # the keys and their order of the per-machine History
+            hist["val_loss"] = [float(v) for v in self.val_loss[s, :ran]]
+            hist["val_accuracy"] = [float(v) for v in self.val_acc[s, :ran]]
+        ae._history = History(hist, {"verbose": 0, "epochs": int(self.epochs), "steps": int(self.slot_steps[s])}, list(range(ran)))
+        ae.model.history = ae._history
+        if ttr is not None:  # what TransformedTargetRegressor.fit leaves: the transformer fitted on the target array, a fitted clone
+            ttr._training_dim = 2
+            ttr.transformer_ = _fill_minmax_from_extrema(clone(ttr.transformer), self.y_min[s], self.y_max[s], n_rows, None)
+            ttr.regressor_ = reg
+            if hasattr(reg, "feature_names_in_"):
+                ttr.feature_names_in_ = reg.feature_names_in_
+        _fill_minmax_from_extrema(det.scaler, self.y_min[s], self.y_max[s], n_rows, tags)
+        return det
+
+
+def kfold_layout(cv, rows: int):
+    """
+    The row layout of a K-fold bucket from ``cv.split`` over ``rows`` rows: (tests, trains, order, inverse), where ``order`` is the
+    concatenation of the folds' test rows (fold order: fold k tests a contiguous block) and ``inverse[t]`` is the fold-order
+    position of row t.  ValueError unless the folds test every row exactly once.
+    """
+    folds = [(np.asarray(tr, dtype=np.int64), np.asarray(te, dtype=np.int64)) for tr, te in cv.split(np.arange(rows))]
+    trains, tests = [f[0] for f in folds], [f[1] for f in folds]
+    order = np.concatenate(tests) if tests else np.zeros(0, np.int64)
+    if len(tests) < 2 or len(order) != rows or not np.array_equal(np.sort(order), np.arange(rows)):
+        raise ValueError("K-fold thresholds need a cv whose test folds cover every row exactly once (KFold)")
+    inverse = np.empty(rows, dtype=np.int64)
+    inverse[order] = np.arange(rows)
+    return tests, trains, order, inverse
+
+
+def kfold_row_maps(trains, inverse, rows: int, detector_shuffle: bool):
+    """
+    The K + 1 row maps of a K-fold bucket, in fold-order rows: the final fit's positions (all rows, in time order) and fold k's
+    (its training rows) -- each in the order ``sklearn.utils.shuffle(..., random_state=0)`` gives when the detector shuffles.
+    """
+    orders = [np.arange(rows)] + list(trains)
+    if detector_shuffle:
+        orders = [sk_shuffle(t, random_state=0) for t in orders]
+    return [inverse[t] for t in orders]
+
+
+def combine_fold_extrema(lo, hi):
+    """
+    Column extrema per slot from those of the K test blocks (``lo`` / ``hi``: [K, M, T]): the final slot's over all blocks, fold
+    k's over every block but k.  Min and max do not depend on order, so these are exactly the extrema of the slot's rows.
+    Returns ([S, T], [S, T]) in the slot layout (finals, then fold k of machine m at M + k*M + m).
+    """
+    K, M = lo.shape[:2]
+    s_lo = np.empty(((K + 1) * M,) + lo.shape[2:], dtype=lo.dtype)
+    s_hi = np.empty_like(s_lo)
+    s_lo[:M], s_hi[:M] = lo.min(axis=0), hi.max(axis=0)
+    for k in range(K):
+        others = [j for j in range(K) if j != k]
+        s_lo[M + k * M : M + (k + 1) * M] = lo[others].min(axis=0)
+        s_hi[M + k * M : M + (k + 1) * M] = hi[others].max(axis=0)
+    return s_lo, s_hi
+
+
+def build_kfold_fleet(eng: "engine.FFEngine", x, y, rows: int, cv, epochs: int = 1, batch_size: int = 32, seed: int = 0,
+                      adam: Optional[Dict[str, float]] = None, shuffle: bool = True, generator=None, input_scaler: bool = False,
+                      target_scaler: bool = False, detector_shuffle: bool = False, validation_split: float = 0.0,
+                      validation_batch_size: Optional[int] = None, early_stopping=None, window: Optional[int] = None,
+                      smoothing_method: Optional[str] = None, threshold_percentile: float = 0.99,
+                      keep_init_params: bool = False) -> KFoldFleetBuild:
+    """
+    The batched ``gordo build`` of one bucket of ``DiffBasedKFCVAnomalyDetector`` machines (diff.py:566-635 in the reference):
+    for every machine the K-fold cross validation under ``cv`` (a KFold) and the final fit -- ``(K + 1) * n_machines`` fits in one
+    fit launch -- then every fold model's test block scored in one launch, the errors brought back to time order, smoothed and
+    reduced to the ``threshold_percentile`` quantile, and the CV metric moments.
+
+    x, y: float64 device tensors [n_machines * rows, T]; machine m owns rows [m*rows, (m+1)*rows).  ``y`` may be ``x``.
+
+    Every machine of a bucket has the same rows, so the KFold split and every row map are the same for all of them.  x and y are
+    laid out once in fold order (the folds' test rows one after the other, gb_gather_rows), where fold k's test rows are one
+    contiguous block; the fits read their rows through K + 1 shared maps.  ``input_scaler``: the network is behind a MinMaxScaler
+    (``Pipeline([MinMaxScaler(), KerasAutoEncoder])``); ``target_scaler``: the estimator is ``TransformedTargetRegressor(transformer=
+    MinMaxScaler(), regressor=...)``, so every slot trains on its own MinMax-scaled targets and the fold models' predictions are
+    mapped back by sklearn's float32 inverse (gb_minmax_inverse_f32) and scored in float64, as the per-machine detector scores a
+    foreign estimator.  Every scaler's extrema come from gb_minmax_f64 over the test blocks (a slot's rows are a union of blocks)
+    with sklearn's float64 attribute arithmetic.  ``detector_shuffle``, ``validation_split``, ``early_stopping`` as in ``build_fleet``.
+    """
+    torch = engine._torch()
+    dev = eng.device
+    if x.dtype != torch.float64 or y.dtype != torch.float64:
+        raise ValueError(f"build_kfold_fleet takes float64 x and y, got {x.dtype} / {y.dtype}")
+    x, y = x.contiguous(), (None if y is x else y.contiguous())
+    y = x if y is None else y
+    M, N, T = x.shape[0] // rows, int(rows), eng.n_out
+    tests, trains, order, inverse = kfold_layout(cv, N)
+    K, S, KM = len(tests), M * (len(tests) + 1), M * len(tests)
+    n_test = np.asarray([len(t) for t in tests], dtype=np.int64)
+    o = np.concatenate([[0], np.cumsum(n_test)[:-1]])           # first fold-order row of fold k's test block
+    max_test = int(n_test.max())
+    base = np.arange(M, dtype=np.int64) * N
+
+    def i32(a):
+        return torch.from_numpy(np.ascontiguousarray(a, dtype=np.int32)).to(dev)
+
+    def jobs(slots, n, x_row, out_row=None):
+        return engine.jobs_to_device(engine.make_jobs(slots, n, x_row, out_row), dev)
+
+    def f64(a):
+        return torch.from_numpy(np.ascontiguousarray(a, dtype=np.float64)).to(dev)
+
+    # 1. fold order: one gather per array
+    whole = jobs(np.arange(M), N, base)
+    to_fold = i32(order)
+    xq = engine.gather_rows(whole, M, N, to_fold, x, M * N)
+    yq = xq if y is x else engine.gather_rows(whole, M, N, to_fold, y, M * N)
+
+    # 2. scaler extrema: one reduction over the K*M test blocks (job k*M + m), combined per slot on the host
+    fk, fm = np.repeat(np.arange(K), M), np.tile(np.arange(M), K)
+    blocks = jobs(np.arange(KM), n_test[fk], fm * N + o[fk])
+
+    def slot_extrema(a):
+        lo, hi = (t.cpu().numpy().reshape(K, M, -1) for t in engine.minmax_f64(blocks, KM, max_test, a, KM))
+        s_lo, s_hi = combine_fold_extrema(lo, hi)
+        if not (np.isfinite(s_lo).all() and np.isfinite(s_hi).all()):
+            raise ValueError("a column without finite values in a training set")
+        return s_lo, s_hi
+
+    y_lo, y_hi = slot_extrema(yq)
+    y_scale, y_offset = _minmax_attributes(y_lo, y_hi)
+    in_lo = in_hi = None
+    if input_scaler:
+        in_lo, in_hi = (y_lo, y_hi) if y is x else slot_extrema(xq)
+
+    # 3. the fits' inputs: with a scaler in front of the network or on the targets, slot s owns rows [s*N, (s+1)*N) of x and y
+    per_slot = input_scaler or target_scaler
+    slot_x = np.arange(S, dtype=np.int64) * N if per_slot else np.tile(base, K + 1)  # first row of slot s in x / y
+    machine_of = np.tile(base, K + 1)
+    copy_jobs = jobs(np.arange(S), N, machine_of, slot_x)
+    if input_scaler:
+        a, b = _minmax_attributes(in_lo, in_hi)
+        xf = engine.affine_f64(copy_jobs, S, N, xq, f64(a), f64(b), out_rows=S * N)
+    else:
+        xf = engine.gather_rows(copy_jobs if per_slot else whole, S if per_slot else M, N, to_fold, x, S * N if per_slot else M * N, to_f32=True)
+    if target_scaler:
+        yf = xf if (input_scaler and y is x) else engine.affine_f64(copy_jobs, S, N, yq, f64(y_scale), f64(y_offset), out_rows=S * N)
+    elif per_slot:
+        yf = engine.gather_rows(copy_jobs, S, N, to_fold, y, S * N, to_f32=True)
+    else:
+        yf = xf if y is x else engine.gather_rows(whole, M, N, to_fold, y, M * N, to_f32=True)
+
+    maps = kfold_row_maps(trains, inverse, N, detector_shuffle)
+    slot_n = [N] + [N - int(n) for n in n_test]                    # rows each slot's estimator receives
+    vsplit = float(validation_split or 0.0)
+    n_train = [int(math.floor(n * (1.0 - vsplit))) if 0.0 < vsplit < 1.0 else n for n in slot_n]  # keras' split (models.py)
+    if min(n_train) < 1:
+        raise ValueError(f"validation_split {vsplit} leaves the {min(slot_n)}-row slot without a training row")
+    map_ofs = np.cumsum([0] + slot_n[:-1])
+    split = engine.make_split(np.repeat(slot_n, M) - np.repeat(n_train, M), np.repeat(map_ofs, M))
+    row_map = i32(np.concatenate(maps))
+    g = generator or torch.Generator(device=dev).manual_seed(seed)
+    params = _keras_initial_params(eng, S, g)
+    init_params = params.clone() if keep_init_params else None
+    fit_jobs = jobs(np.arange(S), np.repeat(n_train, M), slot_x)
+    loss, acc, val_loss, val_acc, epochs_run, best_epoch = _fit_slots(
+        eng, params, fit_jobs, S, N, xf, yf, split, row_map, M, epochs, batch_size, shuffle, adam, seed, validation_batch_size, early_stopping)
+    if n_train == slot_n:  # nothing held out
+        val_loss = val_acc = None
+
+    # 4. fold errors in fold order, by the route the per-machine detector takes (DiffBasedAnomalyDetector._score)
+    sc_slots = M + np.arange(KM)
+    out0 = fm * N + o[fk]                                           # fold-order rows of the test block in machine layout
+    sc_jobs = jobs(sc_slots, n_test[fk], slot_x[sc_slots] + o[fk], out0)
+    mult = (y_scale + y_offset) - y_offset                          # _scaler_multiplier: transform(1) - transform(0)
+    want = ("tag-anomaly-unscaled", "total-anomaly-scaled")
+    if not target_scaler:  # fused predict + score, fp32, with the fold detector's multiplier
+        res = eng.infer_score(params, sc_jobs, KM, max_test, xf, yf, torch.from_numpy(mult.astype(np.float32)).to(dev), out_rows=M * N, want=want)
+        pred32, tag_err, tot_err = res["model-output"], res["tag-anomaly-unscaled"], res["total-anomaly-scaled"]
+        mom_jobs, y32 = sc_jobs, yf
+    else:  # predict, sklearn's float32 inverse of the slot's transformer, float64 scoring against the float64 targets
+        pred = eng.infer_score(params, sc_jobs, KM, max_test, xf, out_rows=M * N)["model-output"]
+        mom_jobs = jobs(sc_slots, n_test[fk], out0, out0)
+        back = engine.minmax_inverse_f32(mom_jobs, KM, max_test, pred, f64(y_scale), f64(y_offset), out_rows=M * N)
+        pred32 = back["f32"]
+        res = engine.anomaly_score(mom_jobs, KM, max_test, back["f64"], yq, T, scale=f64(mult), want=want)
+        tag_err, tot_err = res["tag-anomaly-unscaled"], res["total-anomaly-scaled"]
+        y32 = engine.gather_rows(whole, M, N, to_fold, y, M * N, to_f32=True)
+
+    # 5. K-fold thresholds: errors back in time order (float32, as the detector stores them), smoothed, the percentile
+    to_time = i32(inverse)
+    narrow = tag_err.dtype == torch.float64
+    tag_t = engine.gather_rows(whole, M, N, to_time, tag_err, M * N, to_f32=narrow)
+    tot_t = engine.gather_rows(whole, M, N, to_time, tot_err, M * N, to_f32=narrow)
+    if window is not None and smoothing_method is not None:
+        tag_t = engine.smooth(whole, M, tag_t, int(window), smoothing_method, max_rows=N)
+        tot_t = engine.smooth(whole, M, tot_t, int(window), smoothing_method, max_rows=N)
+    q = float(threshold_percentile)
+    feat = engine.quantile(whole, M, N, tag_t, q)
+    agg = engine.quantile(whole, M, N, tot_t, q)[:, 0]
+
+    # 6. the evaluation metrics of ModelBuilder's cross validation, in the targets' own units
+    moments = engine.cv_moments(mom_jobs, KM, pred32, y32, T)
+
+    def host(t):
+        return None if t is None else t.cpu().numpy()
+
+    return KFoldFleetBuild(
+        eng, M, K, N, n_test, params, init_params, host(loss), host(acc), host(val_loss), host(val_acc), int(epochs), host(epochs_run),
+        host(best_epoch), (np.repeat(n_train, M) + int(batch_size) - 1) // int(batch_size), y_lo, y_hi, in_lo, in_hi, bool(target_scaler),
+        host(feat).astype(np.float64), host(agg).astype(np.float64), host(moments).reshape(K, M, 5, T).transpose(1, 0, 2, 3).copy())

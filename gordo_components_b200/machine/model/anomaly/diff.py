@@ -481,18 +481,27 @@ class DiffBasedKFCVAnomalyDetector(DiffBasedAnomalyDetector):
     def cross_validate(self, *, X, y, cv=None, **kwargs):
         from sklearn.model_selection import KFold
 
-        from .... import engine
-
         cv = cv if cv is not None else KFold(n_splits=5, shuffle=True, random_state=0)
         kwargs.update(dict(return_estimator=True, cv=cv))
         cv_output = sk_cross_validate(self, X=X, y=y, **kwargs)
+        feature_thresholds, self.aggregate_threshold_ = self.kfold_thresholds(X, y, kwargs["cv"], cv_output["estimator"])
+        self.feature_thresholds_ = feature_thresholds
+        return cv_output
+
+    def kfold_thresholds(self, X, y, cv, fold_estimators):
+        """
+        ``(feature_thresholds_, aggregate_threshold_)`` from fitted fold detectors (``cross_validate``'s ``estimator`` list, in the
+        order of ``cv.split``): every row scored by the fold model that did not see it, smoothed, the ``threshold_percentile``
+        quantile.
+        """
+        from .... import engine
 
         yv = _values(y)
         n, t = yv.shape
         columns = list(y.columns) if hasattr(y, "columns") else list(range(t))
         abs_err = np.zeros((n, t), dtype=np.float32)
         val_mse = np.full((n,), np.nan, dtype=np.float32)
-        for (_, test_idxs), fold in zip(kwargs["cv"].split(X, y), cv_output["estimator"]):
+        for (_, test_idxs), fold in zip(cv.split(X, y), fold_estimators):
             X_test = X.iloc[test_idxs] if isinstance(X, pd.DataFrame) else X[test_idxs]
             y_test = y.iloc[test_idxs] if isinstance(y, pd.DataFrame) else y[test_idxs]
             res = self._score(fold, X_test, y_test, fold.scaler, want=("tag-anomaly-unscaled", "total-anomaly-scaled"))
@@ -512,6 +521,5 @@ class DiffBasedKFCVAnomalyDetector(DiffBasedAnomalyDetector):
                 a = engine.smooth(jobs, 1, a, int(self.window), self.smoothing_method)
             return engine.quantile(jobs, 1, n, a, q)[0].cpu().numpy().astype(np.float64)
 
-        self.aggregate_threshold_ = float(threshold(val_mse)[0])
-        self.feature_thresholds_ = pd.Series(threshold(abs_err), index=columns)
-        return cv_output
+        aggregate = float(threshold(val_mse)[0])
+        return pd.Series(threshold(abs_err), index=columns), aggregate

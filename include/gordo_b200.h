@@ -192,6 +192,20 @@ int gb_quantile(const gb_job* jobs, int32_t n_jobs, int32_t max_rows, const floa
 int gb_affine_f64(const gb_job* jobs, int32_t n_jobs, int32_t max_rows, const double* x, int32_t n_cols, const double* a,
                   const double* b, float* out, void* stream);
 
+/* ---- row permutations of the batched K-fold build (DiffBasedKFCVAnomalyDetector.cross_validate, diff.py:566-635) ----
+ * Per job: dst row out_row + p = src row x_row + row_map[p] for p < n_rows; one map shared by every job (a KFold split is the
+ * same for every machine of a bucket).  src / dst: [rows][n_cols] of elem_bytes (4 or 8) each; to_f32 = 1 reads float64 and
+ * writes float32 (round to nearest), in the same pass.  Rows that are whole 16-byte units are copied 16 bytes at a time. */
+int gb_gather_rows(const gb_job* jobs, int32_t n_jobs, int32_t max_rows, const int32_t* row_map, const void* src, int32_t n_cols,
+                   int32_t elem_bytes, int32_t to_f32, void* dst, void* stream);
+
+/* MinMaxScaler.inverse_transform of float32 predictions, as sklearn does it inside TransformedTargetRegressor.predict: the
+ * array stays float32 and each in-place step rounds to it, t = (float)((double)p - min_), v = (float)((double)t / scale_).
+ * p indexed by x_row, outputs by out_row; scale / min_: [n_slots][n_cols] double.  out_f32 gets v, out_f64 gets (double)v;
+ * either may be NULL, not both. */
+int gb_minmax_inverse_f32(const gb_job* jobs, int32_t n_jobs, int32_t max_rows, const float* p, int32_t n_cols, const double* scale,
+                          const double* min_, float* out_f32, double* out_f64, void* stream);
+
 /* ---- K2: fit ---------------------------------------------------------------------------
  * Replaces scikeras KerasRegressor.fit -> keras Model.fit (models.py:284) for the Dense
  * stacks above: per job, `epochs` passes over rows [x_row, x_row+n_rows) in batches of
