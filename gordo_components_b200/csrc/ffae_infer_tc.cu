@@ -51,6 +51,8 @@ constexpr int STAGE_BYTES = 2 * TILE_BYTES * NWG;  // per warpgroup: one x and o
 // output staging: a warp's 16 rows x 32 columns of one array (rows 16 wq .. of a SWIZZLE_128B box: a 1024-aligned slice)
 constexpr int OBOX_ROWS = 16;
 constexpr int OBOX_BYTES = OBOX_ROWS * BOX_COLS * 4;
+constexpr int RESTAGE_BATCH = 11;  // parameter loads per thread and layer when the weights are restaged
+static_assert(RESTAGE_BATCH * NTHREADS >= W * W + W, "a layer's kernel and bias are one batch of loads");
 
 struct TcArgs {
   CUtensorMap tm_x, tm_y;  // x and y as [n_x_rows][T], boxes of BOX_COLS x TILE, zeros outside (tm_y unused without y)
@@ -250,18 +252,56 @@ __global__ void __launch_bounds__(NTHREADS, 1) ffae_tc_kernel(const __grid_const
     const int row_end = min(job.n_rows, tile_end * TILE);
     const int n_tiles = (row_end - row_begin + TILE - 1) / TILE;
 
+    // One 64-row tile of x or y for this warpgroup (thread 0 of the warpgroup).  Columns past T and rows past the end of the array
+    // arrive as zeros; rows past the end of the job are its neighbour's rows.  Those rows run through the MMAs like any other (the
+    // rows of an MMA are independent) and nothing of them is stored.
+    auto load_tile = [&](const CUtensorMap* m, uint32_t buf, uint32_t bar, int tt) {
+      const int row = (int)(job.x_row + row_begin + tt * TILE);
+      mbar_expect_tx(bar, TILE_BYTES);
+      tma_load_2d(buf, m, 0, row, bar);
+      tma_load_2d(buf + BOX_BYTES, m, BOX_COLS, row, bar);
+    };
+    // the x buffer is free between items (the last tile requested no successor): the first tile loads behind the restage
+    if (leader && wg < n_tiles) load_tile(&a.tm_x, xbuf, bar_x, wg);
+
     // ---- stage this slot's weights: split (layer 0: TF32-hi + BF16 hi / lo, others: FP16 pair) as K-major wgmma B operands
     if (job.slot != cur_slot) {
       cur_slot = job.slot;
       const float* P = a.params + (long)job.slot * a.pstride;
+      // The restage is bound by the latency of its loads (the SM streams no tiles meanwhile).  A layer's kernel [K][N] and bias
+      // [N] (contiguous in the parameter vector, K * N + N <= RESTAGE_BATCH * NTHREADS) are one batch of loads per thread, and the
+      // batch of layer l + 1 is requested before layer l is split, so it arrives while that layer is written.  Layer 0's batch
+      // and the per-tag vectors are requested ahead of the zero fill.
+      float v[RESTAGE_BATCH], vn[RESTAGE_BATCH];
+      auto fetch = [&](float (&dst)[RESTAGE_BATCH], int l) {
+        const float* Ws = P + a.pofs[l];
+        const int n_l = a.K[l] * a.N[l] + a.N[l];
+#pragma unroll
+        for (int u = 0; u < RESTAGE_BATCH; ++u) {
+          const int i = tid + u * NTHREADS;
+          dst[u] = i < n_l ? __ldg(Ws + i) : 0.f;
+        }
+      };
+      fetch(v, 0);
+      const bool vt = tid < TP;
+      const float sc = vt && a.scale ? __ldg(a.scale + (long)job.slot * TP + tid) : 0.f;
+      const float ft = vt && a.feat_thr ? __ldg(a.feat_thr + (long)job.slot * TP + tid) : 0.f;
       for (int i = tid; i < a.w_bytes / 16; i += NTHREADS) reinterpret_cast<uint4*>(smem)[i] = make_uint4(0, 0, 0, 0);
       __syncthreads();
       for (int l = 0; l < L; ++l) {
+        if (l + 1 < L) fetch(vn, l + 1);
         const int K = a.K[l], N = a.N[l], Np = a.Np[l], KN = K * N;
-        const float* Ws = P + a.pofs[l];
-        for (int i = tid; i < KN; i += NTHREADS) {
+        const float bscale = (l + 1 < L) ? TANH_ARG_SCALE : 1.0f;  // hidden layers: bias folded into the tanh argument scale
+#pragma unroll
+        for (int u = 0; u < RESTAGE_BATCH; ++u) {
+          const int i = tid + u * NTHREADS;
+          if (i >= KN + N) break;
+          if (i >= KN) {
+            reinterpret_cast<float*>(smem + a.bias_ofs[l])[i - KN] = v[u] * bscale;
+            continue;
+          }
           const int k = i / N, n = i - k * N;
-          const float w = __ldg(Ws + i);
+          const float w = v[u];
           const int i8 = ((k >> 3) * Np + n) * 8 + (k & 7);  // [K/8][Np][8] 16-bit images
           if (l == 0) {
             const float hi = __uint_as_float((__float_as_uint(w) + 0x1000u) & 0xffffe000u);  // round to nearest TF32
@@ -275,13 +315,13 @@ __global__ void __launch_bounds__(NTHREADS, 1) ffae_tc_kernel(const __grid_const
             reinterpret_cast<__half*>(smem + a.img1_ofs[l])[i8] = __float2half_rn(w - __half2float(w1));
           }
         }
-        const float bscale = (l + 1 < L) ? TANH_ARG_SCALE : 1.0f;  // hidden layers: bias folded into the tanh argument scale
-        for (int n = tid; n < N; n += NTHREADS) reinterpret_cast<float*>(smem + a.bias_ofs[l])[n] = __ldg(Ws + KN + n) * bscale;
+#pragma unroll
+        for (int u = 0; u < RESTAGE_BATCH; ++u) v[u] = vn[u];
       }
       float* vec = reinterpret_cast<float*>(smem + a.vec_ofs);  // [0,64): scale, [64,128): 1/feat_thr
       if (tid < W) {
-        vec[tid] = (tid < TP && a.scale) ? __ldg(a.scale + (long)job.slot * TP + tid) : 0.f;
-        vec[W + tid] = (tid < TP && a.feat_thr) ? 1.0f / __ldg(a.feat_thr + (long)job.slot * TP + tid) : 0.f;
+        vec[tid] = sc;
+        vec[W + tid] = vt && a.feat_thr ? 1.0f / ft : 0.f;
       }
       fence_proxy_async();  // generic-proxy writes above are read by the tensor cores (async proxy)
     }
@@ -289,16 +329,6 @@ __global__ void __launch_bounds__(NTHREADS, 1) ffae_tc_kernel(const __grid_const
 
     // ---- the tiles of this item, warpgroup by warpgroup
     const float* vec = reinterpret_cast<const float*>(smem + a.vec_ofs);
-    // One 64-row tile of x or y for this warpgroup (thread 0 of the warpgroup).  Columns past T and rows past the end of the array
-    // arrive as zeros; rows past the end of the job are its neighbour's rows.  Those rows run through the MMAs like any other (the
-    // rows of an MMA are independent) and nothing of them is stored.
-    auto load_tile = [&](const CUtensorMap* m, uint32_t buf, uint32_t bar, int tt) {
-      const int row = (int)(job.x_row + row_begin + tt * TILE);
-      mbar_expect_tx(bar, TILE_BYTES);
-      tma_load_2d(buf, m, 0, row, bar);
-      tma_load_2d(buf + BOX_BYTES, m, BOX_COLS, row, bar);
-    };
-    if (leader && wg < n_tiles) load_tile(&a.tm_x, xbuf, bar_x, wg);
     for (int tt = wg; tt < n_tiles; tt += NWG) {
       float d[32];
       uint32_t a1[4][4] = {}, a2[4][4] = {};
