@@ -2,7 +2,7 @@
 BASELINE configs[2] (scaled): batched training of 64-tag feedforward_hourglass autoencoders, one persistent CTA per machine.
 Reports row-epochs/s, microseconds per optimizer step and the CPU oracle (NumPy Keras-style loop) on a small sample.
 
-    python benchmarks/bench_fit.py [--machines 296] [--rows 10000] [--epochs 3] [--batch 32]
+    python benchmarks/bench_fit.py [--machines 296] [--rows 10000] [--epochs 3] [--batch 32] [--loss mse]
 """
 import argparse, json, os, sys, time
 import numpy as np
@@ -17,6 +17,7 @@ def main():
     ap.add_argument("--batch", type=int, default=32)
     ap.add_argument("--tags", type=int, default=64)
     ap.add_argument("--cpu", type=int, default=1)
+    ap.add_argument("--loss", default="mse", help="training loss (a canonical name: mse, mae, mape, msle, huber, log_cosh)")
     a = ap.parse_args()
     import torch
     import __graft_entry__ as ge
@@ -33,11 +34,11 @@ def main():
     params = fleet.random_glorot_params(eng, M, g)
     jobs = engine.jobs_to_device(engine.uniform_jobs(M, N), dev)
     p0 = params.clone()
-    eng.fit(p0, jobs, M, N, x, x, epochs=1, batch_size=B)  # warm-up
+    eng.fit(p0, jobs, M, N, x, x, epochs=1, batch_size=B, loss=a.loss)  # warm-up
     torch.cuda.synchronize()
     ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     ev0.record()
-    loss, acc, _ = eng.fit(params, jobs, M, N, x, x, epochs=E, batch_size=B)
+    loss, acc, _ = eng.fit(params, jobs, M, N, x, x, epochs=E, batch_size=B, loss=a.loss)
     ev1.record()
     torch.cuda.synchronize()
     ms = ev0.elapsed_time(ev1)
@@ -45,7 +46,7 @@ def main():
     sms = 132
     waves = (M + sms - 1) // sms
     out = {
-        "workload": f"{M} machines x {a.tags}-tag hourglass, {N} rows, {E} epochs, batch {B}",
+        "workload": f"{M} machines x {a.tags}-tag hourglass, {N} rows, {E} epochs, batch {B}, loss {a.loss}",
         "ms": ms, "row_epochs_per_s": M * N * E / (ms * 1e-3), "us_per_step_per_cta": ms * 1e3 / (steps * waves),
         "steps_per_fit": steps, "waves": waves, "loss_first_last": [float(loss[:, 0].mean()), float(loss[:, -1].mean())],
         "algorithmic_tflops": M * N * E * 90708 / (ms * 1e-3) / 1e12,

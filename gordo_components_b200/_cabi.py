@@ -19,11 +19,21 @@ LIB_PATH = os.path.join(_HERE, "csrc", "libgordo_b200.so")
 GB_MAX_LAYERS = 16
 GB_MAX_WIDTH = 256
 ACT_CODES = {"linear": 0, None: 0, "tanh": 1, "relu": 2, "sigmoid": 3}
+GB_LOSS_MSE, GB_LOSS_MAE, GB_LOSS_MAPE, GB_LOSS_MSLE, GB_LOSS_HUBER, GB_LOSS_LOG_COSH = range(6)  # gb_loss
+LOSS_CODES = {"mse": GB_LOSS_MSE, "mae": GB_LOSS_MAE, "mape": GB_LOSS_MAPE, "msle": GB_LOSS_MSLE, "huber": GB_LOSS_HUBER,
+              "log_cosh": GB_LOSS_LOG_COSH}
+
+
+def loss_code(loss: str) -> int:
+    """gb_loss id of a canonical loss name (``factories.specs.resolve_loss`` maps the Keras spellings to these)."""
+    if loss not in LOSS_CODES:
+        raise ValueError(f"loss {loss!r} is not one the CUDA fit kernels implement {sorted(LOSS_CODES)}")
+    return LOSS_CODES[loss]
 
 EXPORTS = (
     "gb_abi_version", "gb_last_error", "gb_device_check", "gb_ffnet_param_count", "gb_ffnet_param_stride",
     "gb_ffae_infer_score", "gb_ffae_tc_supported", "gb_ffae_infer_plan", "gb_anomaly_score", "gb_anomaly_score_f64", "gb_minmax_fit", "gb_minmax_f64", "gb_thresholds", "gb_thresholds_f64", "gb_cv_moments", "gb_smooth", "gb_quantile", "gb_affine_f64", "gb_gather_rows", "gb_minmax_inverse_f32", "gb_ffae_fit_state_stride", "gb_ffae_fit", "gb_ffae_fit_split", "gb_ffae_fit_stop", "gb_ffae_fit_plan",
-    "gb_lstm_param_count", "gb_lstm_param_stride", "gb_lstm_workspace_bytes", "gb_lstm_infer", "gb_lstm_tc_supported", "gb_lstm_tc_workspace_bytes", "gb_lstm_infer_tc", "gb_lstm_fit_workspace_bytes", "gb_lstm_fit",
+    "gb_lstm_param_count", "gb_lstm_param_stride", "gb_lstm_workspace_bytes", "gb_lstm_infer", "gb_lstm_tc_supported", "gb_lstm_tc_workspace_bytes", "gb_lstm_infer_tc", "gb_lstm_fit_workspace_bytes", "gb_lstm_fit", "gb_lstm_fit_loss",
     "gb_orthonormal_rows",
 )
 
@@ -44,7 +54,7 @@ assert JOB_DTYPE.itemsize == C.sizeof(GbJob) == 24
 class GbFitHParams(C.Structure):
     _fields_ = [("epochs", C.c_int32), ("batch_size", C.c_int32), ("shuffle", C.c_int32), ("l1_div_batch", C.c_int32),
                 ("lr", C.c_float), ("beta1", C.c_float), ("beta2", C.c_float), ("eps", C.c_float),
-                ("seed", C.c_uint64), ("step0", C.c_int32), ("reserved", C.c_int32)]
+                ("seed", C.c_uint64), ("step0", C.c_int32), ("loss", C.c_int32)]
 
 
 class GbFitSplit(C.Structure):
@@ -143,6 +153,8 @@ def _declare(lib):
     lib.gb_lstm_fit_workspace_bytes.argtypes = [C.POINTER(GbLstmNet), C.c_int32]
     lib.gb_lstm_fit.argtypes = [C.POINTER(GbLstmNet), _P, _P, _P, _P, _P, C.c_int32, C.c_int32, _P, _P, C.POINTER(GbLstmFitHParams), _P, _P, _P, _P]
     lib.gb_lstm_fit.restype = C.c_int
+    lib.gb_lstm_fit_loss.argtypes = lib.gb_lstm_fit.argtypes[:-1] + [C.c_int32, _P]
+    lib.gb_lstm_fit_loss.restype = C.c_int
     lib.gb_orthonormal_rows.argtypes = [_P, C.c_int32, C.c_int32, C.c_int32, _P, C.c_int64, C.c_int64, _P]
     lib.gb_orthonormal_rows.restype = C.c_int
     for name in ("gb_device_check", "gb_ffae_infer_score", "gb_ffae_tc_supported", "gb_ffae_infer_plan", "gb_anomaly_score", "gb_minmax_fit", "gb_thresholds", "gb_smooth", "gb_ffae_fit", "gb_ffae_fit_split", "gb_ffae_fit_stop", "gb_lstm_infer"):

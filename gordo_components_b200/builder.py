@@ -336,7 +336,7 @@ class _Canonical:
 
     def bucket(self):
         s = self.spec
-        return (tuple(s.dims), tuple(s.acts), tuple(float(v) for v in s.l1), tuple(sorted(s.adam.items())), tuple(s.metrics),
+        return (tuple(s.dims), tuple(s.acts), tuple(float(v) for v in s.l1), tuple(sorted(s.adam.items())), tuple(s.metrics), s.loss,
                 len(self.X), self.fit["epochs"], self.fit["batch_size"], self.fit["shuffle"], self.n_splits, int(self.evaluation.get("seed", 0)),
                 self.split, self.early_stopping is not None, self.input_scaler)  # EarlyStopping's parameters are per-job records
 
@@ -465,7 +465,7 @@ class _CanonicalLSTM(_Canonical):
 
     def bucket(self):
         s = self.spec
-        return (s.key(), tuple(sorted(s.adam.items())), tuple(s.metrics), self.lookahead, len(self.X), self.fit["epochs"], self.fit["batch_size"],
+        return (s.key(), tuple(sorted(s.adam.items())), tuple(s.metrics), s.loss, self.lookahead, len(self.X), self.fit["epochs"], self.fit["batch_size"],
                 self.n_splits, int(self.evaluation.get("seed", 0)), self.input_scaler)
 
 
@@ -714,7 +714,7 @@ class FleetModelBuilder:
                                seed=int(first.evaluation.get("seed", 0)), adam=first.spec.adam, shuffle=first.fit["shuffle"],
                                input_scaler=first.input_scaler, detector_shuffle=first.split[0], validation_split=first.split[1],
                                validation_batch_size=first.split[2],
-                               early_stopping=None if first.early_stopping is None else [c.early_stopping for c in members])
+                               early_stopping=None if first.early_stopping is None else [c.early_stopping for c in members], loss=first.spec.loss)
         moments = fb.cv_moments.cpu().numpy()
         scale = fb.scale.cpu().numpy().astype(np.float64)
         engine._torch().cuda.synchronize()
@@ -752,7 +752,8 @@ class FleetModelBuilder:
         same_y = all(c.y is c.X for c in members)
         yd = xd if same_y else engine._torch().from_numpy(np.concatenate([np.ascontiguousarray(c.y.values, dtype=np.float64) for c in members])).to(eng.device)
         fb = fleet.build_lstm_fleet(eng, xd, yd, rows, lookahead=first.lookahead, epochs=first.fit["epochs"], batch_size=first.fit["batch_size"],
-                                    n_splits=K, seed=int(first.evaluation.get("seed", 0)), adam=first.spec.adam, input_scaler=first.input_scaler)
+                                    n_splits=K, seed=int(first.evaluation.get("seed", 0)), adam=first.spec.adam, input_scaler=first.input_scaler,
+                                    loss=first.spec.loss)
         engine._torch().cuda.synchronize()
         share = (time.time() - t0) / len(members)  # the bucket's wall time, spread evenly: there is no per-machine time any more
         split_obj = TimeSeriesSplit(n_splits=K)
@@ -794,7 +795,8 @@ class FleetModelBuilder:
                                      input_scaler=first.input_scaler, target_scaler=first.target_scaler, detector_shuffle=first.split[0],
                                      validation_split=first.split[1], validation_batch_size=first.split[2],
                                      early_stopping=None if first.early_stopping is None else [c.early_stopping for c in members],
-                                     window=det.window, smoothing_method=det.smoothing_method, threshold_percentile=det.threshold_percentile)
+                                     window=det.window, smoothing_method=det.smoothing_method, threshold_percentile=det.threshold_percentile,
+                                     loss=first.spec.loss)
         torch.cuda.synchronize()
         share = (time.time() - t0) / len(members)  # the bucket's wall time, spread evenly: there is no per-machine time any more
         out = []

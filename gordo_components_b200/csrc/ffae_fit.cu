@@ -2,7 +2,8 @@
 //
 // Replaces scikeras KerasRegressor.fit -> keras Model.fit (gordo/machine/model/models.py:284) for
 // the networks of factories/feedforward_autoencoder.py:65-104:
-//   loss = mean((net(x)-y)^2) + sum_l l1[l]*sum|a_l|,  Adam(lr, b1, b2, eps) [keras defaults 1e-3/.9/.999/1e-7],
+//   loss = mean(f(net(x), y)) + sum_l l1[l]*sum|a_l|,  Adam(lr, b1, b2, eps) [keras defaults 1e-3/.9/.999/1e-7],
+//   f = (net(x)-y)^2 or another Keras regression loss (hp.loss, gb::loss_value / gb::loss_grad),
 //   every epoch visits a permutation of the job's rows in batches of batch_size (last partial batch kept).
 //
 // A fit is a chain of epochs*ceil(n/batch) dependent optimizer steps of ~3 MFLOP each, so it is latency bound,
@@ -17,6 +18,7 @@
 // index (4x4 register tile, reduce-scatter over the four quarters); the weight gradient gives a thread a 4x2 block of W.
 #include <cuda_pipeline.h>
 #include <math_constants.h>
+#include <type_traits>
 #include "gb_common.cuh"
 
 namespace {
@@ -129,7 +131,9 @@ __device__ __forceinline__ void quarter_reduce(const float (&acc)[4][4], int lan
 // monitored history entry it has just written and posts the decision (snapshot, stop) in s_red, free between two epoch_stats;
 // one barrier shares it.  A snapshot is the weight image written to best_params in canonical layout; a job that stops drains
 // its cp.async prefetch and leaves, so its SM takes the next job of the launch.
-template <bool WG, bool DG, bool SPLIT = false, bool STOP = false>  // DG: some dz buffers live in global memory too (kept apart so that the usual case addresses them as shared memory)
+// LOSS (a fit whose hp.loss is not MSE): the output layer takes f / f' from gb::loss_value / gb::loss_grad.  Kept apart so that
+// the MSE fits keep the exact code of the kernels without it.
+template <bool WG, bool DG, bool SPLIT = false, bool STOP = false, bool LOSS = false>  // DG: some dz buffers live in global memory too (kept apart so that the usual case addresses them as shared memory)
 __global__ void __launch_bounds__(THREADS, 1) ffae_fit_kernel(const FitArgs a) {
   extern __shared__ __align__(16) float smem[];
   __shared__ float s_red[3][NWARPS];
@@ -399,6 +403,8 @@ __global__ void __launch_bounds__(THREADS, 1) ffae_fit_kernel(const FitArgs a) {
         const int NpL = a.im.np[L - 1], actL = a.net.act[L - 1];
         const float cL = a.net.l1[L - 1] / (a.hp.l1_div_batch ? (float)nbt : 1.f);
         const float gscale = 2.f / ((float)nbt * (float)n_out);
+        const int loss = LOSS ? a.hp.loss : GB_LOSS_MSE;  // launch-uniform; MSE keeps its own arithmetic (d * d, gscale * d)
+        const float lscale = 1.f / ((float)nbt * (float)n_out);
         for (int r = warp; r < BR; r += NWARPS) {
           // keras "accuracy" on 2-D float targets: argmax match (binary if width 1); first maximum wins, as np.argmax.  The
           // values are compared as order-preserving integer keys so that the warp-wide maximum is one REDUX.
@@ -408,9 +414,14 @@ __global__ void __launch_bounds__(THREADS, 1) ffae_fit_kernel(const FitArgs a) {
             float g = 0.f;
             if (r < nb && j < n_out) {
               const float ao = yh[r * yp + j], t = yt[r * a.ypitch + j];
-              const float d = ao - t;
-              acc_sq += d * d;
-              g = gscale * d;
+              if (loss == GB_LOSS_MSE) {
+                const float d = ao - t;
+                acc_sq += d * d;
+                g = gscale * d;
+              } else {
+                acc_sq += gb::loss_value(loss, ao, t);
+                g = lscale * gb::loss_grad(loss, ao, t);
+              }
               if (cL != 0.f) g += cL * ((ao > 0.f) ? 1.f : ((ao < 0.f) ? -1.f : 0.f));
               g *= gb::act_grad_from_output(actL, ao);
               const unsigned ka = order_key(ao), kb = order_key(t);
@@ -692,6 +703,7 @@ int launch_fit(const gb_ffnet* net, float* params, float* adam_m, float* adam_v,
   GB_REQUIRE(hp->batch_size >= 1, GB_E_ARG, "batch_size=%d must be >= 1", hp->batch_size);
   GB_REQUIRE(hp->shuffle >= 0 && hp->shuffle <= 2, GB_E_ARG, "shuffle=%d unknown", hp->shuffle);
   GB_REQUIRE(hp->shuffle != 2 || perm, GB_E_ARG, "shuffle=2 needs perm");
+  GB_REQUIRE(hp->loss >= GB_LOSS_MSE && hp->loss <= GB_LOSS_LOG_COSH, GB_E_ARG, "loss=%d unknown (gb_loss: 0..5)", hp->loss);
   GB_REQUIRE(gb::aligned16(params) && gb::aligned16(adam_m) && gb::aligned16(adam_v) && gb::aligned16(x) &&
                  gb::aligned16(y),
              GB_E_ALIGN, "params/adam/x/y must be 16-byte aligned");
@@ -723,19 +735,23 @@ int launch_fit(const gb_ffnet* net, float* params, float* adam_m, float* adam_v,
     kernel<<<n_jobs, THREADS, smem, (cudaStream_t)stream>>>(a);
     return GB_OK;
   };
-  if (entry == FIT_STOP) {
-    if (a.d_global > 0) rc = launch(ffae_fit_kernel<true, true, true, true>);
-    else if (w_global) rc = launch(ffae_fit_kernel<true, false, true, true>);
-    else rc = launch(ffae_fit_kernel<false, false, true, true>);
-  } else if (entry == FIT_SPLIT) {
-    if (a.d_global > 0) rc = launch(ffae_fit_kernel<true, true, true>);
-    else if (w_global) rc = launch(ffae_fit_kernel<true, false, true>);
-    else rc = launch(ffae_fit_kernel<false, false, true>);
-  } else {
-    if (a.d_global > 0) rc = launch(ffae_fit_kernel<true, true>);
-    else if (w_global) rc = launch(ffae_fit_kernel<true, false>);
-    else rc = launch(ffae_fit_kernel<false, false>);
-  }
+  auto dispatch = [&](auto any_loss) -> int {
+    constexpr bool LS = decltype(any_loss)::value;
+    if (entry == FIT_STOP) {
+      if (a.d_global > 0) return launch(ffae_fit_kernel<true, true, true, true, LS>);
+      if (w_global) return launch(ffae_fit_kernel<true, false, true, true, LS>);
+      return launch(ffae_fit_kernel<false, false, true, true, LS>);
+    }
+    if (entry == FIT_SPLIT) {
+      if (a.d_global > 0) return launch(ffae_fit_kernel<true, true, true, false, LS>);
+      if (w_global) return launch(ffae_fit_kernel<true, false, true, false, LS>);
+      return launch(ffae_fit_kernel<false, false, true, false, LS>);
+    }
+    if (a.d_global > 0) return launch(ffae_fit_kernel<true, true, false, false, LS>);
+    if (w_global) return launch(ffae_fit_kernel<true, false, false, false, LS>);
+    return launch(ffae_fit_kernel<false, false, false, false, LS>);
+  };
+  rc = hp->loss == GB_LOSS_MSE ? dispatch(std::false_type{}) : dispatch(std::true_type{});
   if (rc != GB_OK) return rc;
   GB_CUDA_CHECK(cudaGetLastError());
   return GB_OK;

@@ -3,7 +3,7 @@
 // Replaces KerasLSTMBaseEstimator.fit (gordo/machine/model/models.py:557-616): a primer Adam step on the single window
 // X[:L], then `epochs` passes over the lookback windows IN ORDER (shuffle=False, :612-615) in batches of `batch_size`,
 // for the stacks of factories/lstm_autoencoder.py:72-103 (every LSTM returns sequences except the last; Dense head;
-// MSE; Adam with the Keras defaults).  Windows are never materialised (models.py:713-793): window j of a job is the x rows
+// MSE or, through gb_lstm_fit_loss, another Keras regression loss; Adam with the Keras defaults).  Windows are never materialised (models.py:713-793): window j of a job is the x rows
 // [x_row + j, x_row + j + L) and its target is y row x_row + j + L - 1 + lookahead.
 //
 // Unlike the Dense autoencoders (one CTA trains one machine with its weights in shared memory), one LSTM stack is
@@ -48,6 +48,7 @@ struct FitArgs {
   const int* step;            // device: {first window, nominal batch size} of the optimizer step being replayed (the launch
                               // sequence of one step is captured once as a CUDA graph; only these two numbers change)
   float lr, b1, b2, eps;
+  int loss;                   // gb_loss of the head
 };
 
 __device__ __forceinline__ float sigm(float z) { return 1.f / (1.f + expf(-z)); }
@@ -144,6 +145,7 @@ __global__ void __launch_bounds__(256) lstm_head_kernel(const FitArgs a) {
   for (int i = tid; i < nb * u; i += 256) sh[i] = H[i];
   __syncthreads();
   const float inv = 2.0f / (float)(nb * T);
+  const float linv = 1.0f / (float)(nb * T);
   float lsum = 0.f;
   for (int i = tid; i < nb * T; i += 256) {
     const int b = i / T, o = i - b * T;
@@ -151,10 +153,15 @@ __global__ void __launch_bounds__(256) lstm_head_kernel(const FitArgs a) {
     for (int k = 0; k < u; ++k) z = fmaf(sh[b * u + k], __ldg(P + (long)k * T + o), z);
     const float yh = gb::apply_act(a.out_act, z);
     const float tgt = __ldg(a.y + (job.x_row + a.step[0] + b + a.L - 1 + a.lookahead) * (long)T + o);
-    const float d = yh - tgt;
-    lsum += d * d;
     sy[i] = yh;
-    sd[i] = inv * d * gb::act_grad_from_output(a.out_act, yh);
+    if (a.loss == GB_LOSS_MSE) {  // the MSE arithmetic of gb_lstm_fit, unchanged
+      const float d = yh - tgt;
+      lsum += d * d;
+      sd[i] = inv * d * gb::act_grad_from_output(a.out_act, yh);
+    } else {
+      lsum += gb::loss_value(a.loss, yh, tgt);
+      sd[i] = linv * gb::loss_grad(a.loss, yh, tgt) * gb::act_grad_from_output(a.out_act, yh);
+    }
   }
   red[tid] = lsum;
   __syncthreads();
@@ -463,8 +470,16 @@ size_t gb_lstm_fit_workspace_bytes(const gb_lstmnet* net, int32_t n_jobs) {
 int gb_lstm_fit(const gb_lstmnet* net, float* params, float* adam_m, float* adam_v, int32_t* adam_t, const gb_job* jobs, int32_t n_jobs,
                 int32_t max_windows, const float* x, const float* y, const gb_lstm_fit_hparams* hp, void* workspace, float* out_loss,
                 float* out_acc, void* stream) {
+  return gb_lstm_fit_loss(net, params, adam_m, adam_v, adam_t, jobs, n_jobs, max_windows, x, y, hp, workspace, out_loss, out_acc,
+                          GB_LOSS_MSE, stream);
+}
+
+int gb_lstm_fit_loss(const gb_lstmnet* net, float* params, float* adam_m, float* adam_v, int32_t* adam_t, const gb_job* jobs,
+                     int32_t n_jobs, int32_t max_windows, const float* x, const float* y, const gb_lstm_fit_hparams* hp, void* workspace,
+                     float* out_loss, float* out_acc, int32_t loss, void* stream) {
   int rc = validate(net);
   if (rc != GB_OK) return rc;
+  GB_REQUIRE(loss >= GB_LOSS_MSE && loss <= GB_LOSS_LOG_COSH, GB_E_ARG, "loss=%d unknown (gb_loss: 0..5)", loss);
   GB_REQUIRE(params && adam_m && adam_v && adam_t && jobs && x && y && hp && workspace && out_loss && out_acc, GB_E_ARG, "NULL argument");
   GB_REQUIRE(n_jobs >= 0 && n_jobs <= 65535 && max_windows >= 0, GB_E_ARG, "bad n_jobs/max_windows");
   GB_REQUIRE(hp->epochs >= 0 && hp->batch_size >= 1, GB_E_ARG, "epochs=%d batch_size=%d", hp->epochs, hp->batch_size);
@@ -482,6 +497,7 @@ int gb_lstm_fit(const gb_lstmnet* net, float* params, float* adam_m, float* adam
   a.loss_sum = a.ws + a.ws_stride * n_jobs;
   a.hit_sum = a.loss_sum + n_jobs;
   a.lr = hp->lr; a.b1 = hp->beta1; a.b2 = hp->beta2; a.eps = hp->eps;
+  a.loss = loss;
   const long n_params = (long)gb_lstm_param_count(net);
   const int u_top = net->units[net->n_layers - 1];
   const size_t head_smem = (size_t)(MAXB * u_top + 2 * MAXB * net->n_features_out) * sizeof(float);

@@ -160,24 +160,25 @@ class FFEngine:
     # ------------------------------------------------------------------ K2
     def fit(self, params, jobs_dev, n_jobs: int, max_rows: int, x, y, epochs: int = 1, batch_size: int = 32, shuffle=True,
             perm=None, adam: Optional[Dict[str, float]] = None, seed: int = 0, l1_div_batch: bool = False, state=None,
-            step0: int = 0):
+            step0: int = 0, loss: str = "mse"):
         """
         Trains every job's slot in place (``params`` is updated).  Returns (loss [n_jobs, epochs], accuracy, (m, v)).
-        ``perm`` (int32 [n_jobs, epochs, max_rows]) pins the visiting order (parity tests).
+        ``perm`` (int32 [n_jobs, epochs, max_rows]) pins the visiting order (parity tests).  ``loss``: canonical Keras loss name
+        (``_cabi.LOSS_CODES``) the fit minimises and reports.
         """
         torch = _torch()
-        hp = _fit_hparams(epochs, batch_size, shuffle, perm, adam, seed, l1_div_batch, step0)
+        hp = _fit_hparams(epochs, batch_size, shuffle, perm, adam, seed, l1_div_batch, step0, loss)
         m, v = self._fit_state(params, state)
-        loss = torch.empty((n_jobs, epochs), dtype=torch.float32, device=self.device)
+        hist = torch.empty((n_jobs, epochs), dtype=torch.float32, device=self.device)
         acc = torch.empty((n_jobs, epochs), dtype=torch.float32, device=self.device)
         p = _cabi.ptr
         _cabi.check(self.lib.gb_ffae_fit(C.byref(self.net), p(params), p(m), p(v), p(jobs_dev), int(n_jobs), int(max_rows), p(x), p(y),
-                                         p(perm), C.byref(hp), p(loss), p(acc), _stream_ptr()))
-        return loss, acc, (m, v)
+                                         p(perm), C.byref(hp), p(hist), p(acc), _stream_ptr()))
+        return hist, acc, (m, v)
 
     def fit_split(self, params, jobs_dev, n_jobs: int, max_rows: int, x, y, split=None, row_map=None, val_batch: Optional[int] = None,
                   epochs: int = 1, batch_size: int = 32, shuffle=True, perm=None, adam: Optional[Dict[str, float]] = None, seed: int = 0,
-                  l1_div_batch: bool = False, state=None, step0: int = 0, stop=None):
+                  l1_div_batch: bool = False, state=None, step0: int = 0, stop=None, loss: str = "mse"):
         """
         ``fit`` over row *positions* with Keras' ``validation_split``, in one launch (gb_ffae_fit_split).  Job i trains on its
         positions [0, n_rows) exactly as ``fit`` trains on its rows, and after every epoch runs the network forward over the held-out
@@ -194,9 +195,11 @@ class FFEngine:
         its slot of ``params`` ends with the weights of its best epoch.  Returns (loss, accuracy, val_loss, val_accuracy,
         epochs_run, best_epoch, (m, v)): epochs_run / best_epoch are int32 [n_jobs] (best_epoch -1 when no epoch improved and no
         snapshot was taken), and every history entry past a job's epochs_run is NaN.
+
+        ``loss``: as in ``fit``; the held-out statistics report the same loss.
         """
         torch = _torch()
-        hp = _fit_hparams(epochs, batch_size, shuffle, perm, adam, seed, l1_div_batch, step0)
+        hp = _fit_hparams(epochs, batch_size, shuffle, perm, adam, seed, l1_div_batch, step0, loss)
         m, v = self._fit_state(params, state)
         if split is not None and isinstance(split, np.ndarray):
             split = jobs_to_device(split, self.device)
@@ -235,7 +238,7 @@ class FFEngine:
         return thresholds(jobs_dev, n_jobs, max_rows, tag_unscaled, total_scaled, self.n_out, n_slots, window, self.device)
 
 
-def _fit_hparams(epochs, batch_size, shuffle, perm, adam, seed, l1_div_batch, step0) -> "_cabi.GbFitHParams":
+def _fit_hparams(epochs, batch_size, shuffle, perm, adam, seed, l1_div_batch, step0, loss="mse") -> "_cabi.GbFitHParams":
     adam = adam or {}
     hp = _cabi.GbFitHParams()
     hp.epochs, hp.batch_size = int(epochs), int(batch_size)
@@ -244,6 +247,7 @@ def _fit_hparams(epochs, batch_size, shuffle, perm, adam, seed, l1_div_batch, st
     hp.lr, hp.beta1 = float(adam.get("lr", 1e-3)), float(adam.get("beta1", 0.9))
     hp.beta2, hp.eps = float(adam.get("beta2", 0.999)), float(adam.get("eps", 1e-7))
     hp.seed, hp.step0 = int(seed) & (2**64 - 1), int(step0)
+    hp.loss = _cabi.loss_code(loss)
     return hp
 
 
@@ -562,11 +566,13 @@ class LSTMEngine:
         return int(self.lib.gb_lstm_fit_workspace_bytes(C.byref(self.net), int(n_jobs)))
 
     def fit(self, params, jobs_dev, n_jobs, max_windows, x, y, epochs: int = 1, batch_size: int = 32, lookahead: int = 0,
-            primer: bool = True, adam: Optional[Dict[str, float]] = None, state=None):
+            primer: bool = True, adam: Optional[Dict[str, float]] = None, state=None, loss: str = "mse"):
         """
         Trains every job's slot in place by back-propagation through time (``jobs`` count windows; target of window j is
-        y[x_row + j + lookback - 1 + lookahead]).  Returns (loss [n_jobs, epochs], accuracy, (m, v, t)).
+        y[x_row + j + lookback - 1 + lookahead]).  Returns (loss [n_jobs, epochs], accuracy, (m, v, t)).  ``loss``: canonical
+        Keras loss name (``_cabi.LOSS_CODES``), for the primer step too (gb_lstm_fit_loss).
         """
+        code = _cabi.loss_code(loss)
         torch = _torch()
         adam = adam or {}
         hp = _cabi.GbLstmFitHParams()
@@ -583,12 +589,12 @@ class LSTMEngine:
         ws = torch.empty((ws_bytes + 3) // 4, dtype=torch.float32, device=self.device)
         # a primer-only fit (epochs = 0) writes no history, but the kernel takes the outputs as non-NULL pointers and a tensor with
         # no elements has none: the buffers keep one column and the caller gets the empty slice
-        loss = torch.zeros((n_jobs, max(epochs, 1)), dtype=torch.float32, device=self.device)
+        hist = torch.zeros((n_jobs, max(epochs, 1)), dtype=torch.float32, device=self.device)
         acc = torch.zeros((n_jobs, max(epochs, 1)), dtype=torch.float32, device=self.device)
         p = _cabi.ptr
-        _cabi.check(self.lib.gb_lstm_fit(C.byref(self.net), p(params), p(m), p(v), p(t), p(jobs_dev), int(n_jobs), int(max_windows), p(x), p(y),
-                                         C.byref(hp), p(ws), p(loss), p(acc), _stream_ptr()))
-        return loss[:, :epochs], acc[:, :epochs], (m, v, t)
+        _cabi.check(self.lib.gb_lstm_fit_loss(C.byref(self.net), p(params), p(m), p(v), p(t), p(jobs_dev), int(n_jobs), int(max_windows), p(x),
+                                              p(y), C.byref(hp), p(ws), p(hist), p(acc), code, _stream_ptr()))
+        return hist[:, :epochs], acc[:, :epochs], (m, v, t)
 
     @property
     def tc_supported(self) -> bool:

@@ -303,7 +303,7 @@ def _keras_initial_params(eng: "engine.FFEngine", n_slots: int, generator):
 
 
 def _fit_slots(eng, params, fit_jobs, n_jobs, max_rows, x, y, split, row_map, n_machines, epochs, batch_size, shuffle, adam, seed,
-               validation_batch_size, early_stopping):
+               validation_batch_size, early_stopping, loss="mse"):
     """
     The one fit launch of a bucket (job j trains a slot of machine j mod n_machines): gb_ffae_fit without held-out positions or a
     row map, gb_ffae_fit_split with them, gb_ffae_fit_stop with an EarlyStopping callback (one for all machines or one per machine).
@@ -316,21 +316,22 @@ def _fit_slots(eng, params, fit_jobs, n_jobs, max_rows, x, y, split, row_map, n_
         if len(per_machine) != n_machines:
             raise ValueError(f"early_stopping: {len(per_machine)} callbacks for {n_machines} machines")
         stop = engine.make_stop([per_machine[j % n_machines] for j in range(n_jobs)])
-        loss, acc, val_loss, val_acc, epochs_run, best_epoch, _ = eng.fit_split(
+        hist, acc, val_loss, val_acc, epochs_run, best_epoch, _ = eng.fit_split(
             params, fit_jobs, n_jobs, max_rows, x, y, split=split, row_map=row_map, val_batch=vb, epochs=epochs, batch_size=batch_size,
-            shuffle=shuffle, adam=adam, seed=seed, stop=stop)
+            shuffle=shuffle, adam=adam, seed=seed, stop=stop, loss=loss)
     elif split is None:
-        loss, acc, _ = eng.fit(params, fit_jobs, n_jobs, max_rows, x, y, epochs=epochs, batch_size=batch_size, shuffle=shuffle, adam=adam, seed=seed)
+        hist, acc, _ = eng.fit(params, fit_jobs, n_jobs, max_rows, x, y, epochs=epochs, batch_size=batch_size, shuffle=shuffle, adam=adam, seed=seed,
+                               loss=loss)
     else:
-        loss, acc, val_loss, val_acc, _ = eng.fit_split(params, fit_jobs, n_jobs, max_rows, x, y, split=split, row_map=row_map, val_batch=vb,
-                                                        epochs=epochs, batch_size=batch_size, shuffle=shuffle, adam=adam, seed=seed)
-    return loss, acc, val_loss, val_acc, epochs_run, best_epoch
+        hist, acc, val_loss, val_acc, _ = eng.fit_split(params, fit_jobs, n_jobs, max_rows, x, y, split=split, row_map=row_map, val_batch=vb,
+                                                        epochs=epochs, batch_size=batch_size, shuffle=shuffle, adam=adam, seed=seed, loss=loss)
+    return hist, acc, val_loss, val_acc, epochs_run, best_epoch
 
 
 def build_fleet(eng: "engine.FFEngine", x, y, rows: int, epochs: int = 1, batch_size: int = 32, n_splits: int = 3, seed: int = 0,
                 adam: Optional[Dict[str, float]] = None, shuffle: bool = True, generator=None, input_scaler: bool = False,
                 detector_shuffle: bool = False, validation_split: float = 0.0, validation_batch_size: Optional[int] = None,
-                early_stopping=None) -> FleetBuild:
+                early_stopping=None, loss: str = "mse") -> FleetBuild:
     """
     The batched form of ``gordo build`` for one architecture bucket: for every machine the 3-fold TimeSeriesSplit
     cross-validation (fit on each prefix, thresholds from the following test block: diff.py:176-266) and the final fit on
@@ -355,6 +356,7 @@ def build_fleet(eng: "engine.FFEngine", x, y, rows: int, epochs: int = 1, batch_
     (``engine.make_stop`` takes any form).  Every slot of machine m, the final fit and each CV fold, applies m's rule at the end of
     each of its epochs inside the fit launch (gb_ffae_fit_stop), as sklearn's clone hands every fold the same callbacks.  The
     result then carries ``epochs_run`` / ``best_epoch``; history entries past a fit's ``epochs_run`` are NaN.
+    ``loss``: the estimator's canonical Keras loss name (``FFNetSpec.loss``), trained on and reported by every fit.
     """
     torch = engine._torch()
     dev = eng.device
@@ -401,8 +403,9 @@ def build_fleet(eng: "engine.FFEngine", x, y, rows: int, epochs: int = 1, batch_
     else:
         base_of = lambda k: base  # noqa: E731
     fit_jobs = engine.jobs_to_device(engine.make_jobs(fit_slots, fit_rows, fit_x), dev)
-    loss, acc, val_loss, val_acc, epochs_run, best_epoch = _fit_slots(
-        eng, params, fit_jobs, len(fit_slots), N, x, y, split, row_map, M, epochs, batch_size, shuffle, adam, seed, validation_batch_size, early_stopping)
+    hist, acc, val_loss, val_acc, epochs_run, best_epoch = _fit_slots(
+        eng, params, fit_jobs, len(fit_slots), N, x, y, split, row_map, M, epochs, batch_size, shuffle, adam, seed, validation_batch_size, early_stopping,
+        loss)
     if n_train == slot_n:  # nothing held out
         val_loss = val_acc = None
     # scalers: final on all rows, fold k on its training prefix (diff.py:173 inside each CV clone), held-out rows included
@@ -421,11 +424,11 @@ def build_fleet(eng: "engine.FFEngine", x, y, rows: int, epochs: int = 1, batch_
     fold_params = params[M:].view(K, M, -1).permute(1, 0, 2).contiguous()
     fold_feat = feat[M:].view(K, M, T).permute(1, 0, 2).contiguous()
     fold_agg = agg[M:].view(K, M).t().contiguous()
-    E = loss.shape[1]
+    E = hist.shape[1]
     folds = lambda t: None if t is None else t[M:].view(K, M, E).permute(1, 0, 2)  # noqa: E731
     fold_jobs = lambda t: None if t is None else t[M:].view(K, M).t()  # noqa: E731
     return FleetBuild(eng, M, K, params[:M].contiguous(), scale[:M].contiguous(), offset[:M].contiguous(), fold_feat[:, K - 1].contiguous(),
-                      fold_agg[:, K - 1].contiguous(), loss[:M], acc[:M], loss[M:].view(K, M, E).permute(1, 0, 2), fold_feat, fold_agg,
+                      fold_agg[:, K - 1].contiguous(), hist[:M], acc[:M], hist[M:].view(K, M, E).permute(1, 0, 2), fold_feat, fold_agg,
                       fold_params=fold_params, cv_moments=moments,
                       in_scale=None if in_scale is None else in_scale[:M].contiguous(), in_offset=None if in_offset is None else in_offset[:M].contiguous(),
                       fold_in_scale=None if in_scale is None else in_scale[M:].view(K, M, -1).permute(1, 0, 2).contiguous(),
@@ -538,7 +541,7 @@ class LSTMFleetBuild:
 
 def build_lstm_fleet(eng: "engine.LSTMEngine", x, y, rows: int, lookahead: int = 0, epochs: int = 1, batch_size: int = 32, n_splits: int = 3,
                      seed: int = 0, adam: Optional[Dict[str, float]] = None, input_scaler: bool = False, memory_budget: int = 8 << 30,
-                     keep_init_params: bool = False, generator=None) -> LSTMFleetBuild:
+                     keep_init_params: bool = False, generator=None, loss: str = "mse") -> LSTMFleetBuild:
     """
     The batched ``gordo build`` of one bucket of LSTM machines (``DiffBasedAnomalyDetector(KerasLSTMAutoEncoder | KerasLSTMForecast)``,
     the network bare or behind one MinMaxScaler): for every machine the TimeSeriesSplit cross validation and the final fit, as
@@ -550,6 +553,7 @@ def build_lstm_fleet(eng: "engine.LSTMEngine", x, y, rows: int, lookahead: int =
     ``memory_budget``: bytes of fit workspace (gb_lstm_fit_workspace_bytes) one gb_lstm_fit launch may take.  Machines are
     trained in chunks that fit it -- all ``n_splits + 1`` fits of a machine in the same chunk; every job's result is the same
     whatever the chunking.  ``keep_init_params``: keep the initial parameters of every slot on the result (``init_params``).
+    ``loss``: the estimator's canonical Keras loss name (``LSTMNetSpec.loss``).
     """
     torch = engine._torch()
     dev = eng.device
@@ -603,8 +607,8 @@ def build_lstm_fleet(eng: "engine.LSTMEngine", x, y, rows: int, lookahead: int =
 
     # fits: chunks of whole machines (final + K folds) whose workspace fits the budget
     chunk = max(1, min(M, int(memory_budget) // max(eng.fit_workspace_bytes(K + 1), 1), 65535 // (K + 1)))
-    loss = torch.empty((S, epochs), dtype=torch.float32, device=dev)
-    acc = torch.empty_like(loss)
+    hist = torch.empty((S, epochs), dtype=torch.float32, device=dev)
+    acc = torch.empty_like(hist)
     for m0 in range(0, M, chunk):
         ms = np.arange(m0, min(M, m0 + chunk))
         slots = np.concatenate([j * M + ms for j in range(K + 1)])
@@ -612,9 +616,9 @@ def build_lstm_fleet(eng: "engine.LSTMEngine", x, y, rows: int, lookahead: int =
         p = params.index_select(0, idx)
         jobs = engine.jobs_to_device(engine.make_jobs(np.arange(len(slots)), slot_windows[slots], x_row[slots]), dev)
         cl, ca, _ = eng.fit(p, jobs, len(slots), int(slot_windows[slots].max()), xf, yf, epochs=epochs, batch_size=batch_size, lookahead=la,
-                            primer=True, adam=adam)
+                            primer=True, adam=adam, loss=loss)
         params.index_copy_(0, idx, p)
-        loss.index_copy_(0, idx, cl)
+        hist.index_copy_(0, idx, cl)
         acc.index_copy_(0, idx, ca)
 
     # fold scoring: fold k of machine m (job k*M + m) predicts the windows inside its test block, in one launch
@@ -634,7 +638,7 @@ def build_lstm_fleet(eng: "engine.LSTMEngine", x, y, rows: int, lookahead: int =
     moments = host(engine.cv_moments(score_jobs, KM, pred, y32, T)).reshape(K, M, 5, T).transpose(1, 0, 2, 3)
     fold_feat = host(feat).reshape(K, M, T).transpose(1, 0, 2)
     fold_agg = host(agg).reshape(K, M).T
-    loss_h, acc_h = host(loss), host(acc)
+    loss_h, acc_h = host(hist), host(acc)
 
     def folds(a):  # slot-ordered [S, ...] -> the folds of every machine [M, K, ...]
         return np.ascontiguousarray(np.swapaxes(a[M:].reshape((K, M) + a.shape[1:]), 0, 1))
@@ -784,7 +788,7 @@ def build_kfold_fleet(eng: "engine.FFEngine", x, y, rows: int, cv, epochs: int =
                       target_scaler: bool = False, detector_shuffle: bool = False, validation_split: float = 0.0,
                       validation_batch_size: Optional[int] = None, early_stopping=None, window: Optional[int] = None,
                       smoothing_method: Optional[str] = None, threshold_percentile: float = 0.99,
-                      keep_init_params: bool = False) -> KFoldFleetBuild:
+                      keep_init_params: bool = False, loss: str = "mse") -> KFoldFleetBuild:
     """
     The batched ``gordo build`` of one bucket of ``DiffBasedKFCVAnomalyDetector`` machines (diff.py:566-635 in the reference):
     for every machine the K-fold cross validation under ``cv`` (a KFold) and the final fit -- ``(K + 1) * n_machines`` fits in one
@@ -800,7 +804,8 @@ def build_kfold_fleet(eng: "engine.FFEngine", x, y, rows: int, cv, epochs: int =
     MinMaxScaler(), regressor=...)``, so every slot trains on its own MinMax-scaled targets and the fold models' predictions are
     mapped back by sklearn's float32 inverse (gb_minmax_inverse_f32) and scored in float64, as the per-machine detector scores a
     foreign estimator.  Every scaler's extrema come from gb_minmax_f64 over the test blocks (a slot's rows are a union of blocks)
-    with sklearn's float64 attribute arithmetic.  ``detector_shuffle``, ``validation_split``, ``early_stopping`` as in ``build_fleet``.
+    with sklearn's float64 attribute arithmetic.  ``detector_shuffle``, ``validation_split``, ``early_stopping``, ``loss`` as in
+    ``build_fleet``.
     """
     torch = engine._torch()
     dev = eng.device
@@ -878,8 +883,9 @@ def build_kfold_fleet(eng: "engine.FFEngine", x, y, rows: int, cv, epochs: int =
     params = _keras_initial_params(eng, S, g)
     init_params = params.clone() if keep_init_params else None
     fit_jobs = jobs(np.arange(S), np.repeat(n_train, M), slot_x)
-    loss, acc, val_loss, val_acc, epochs_run, best_epoch = _fit_slots(
-        eng, params, fit_jobs, S, N, xf, yf, split, row_map, M, epochs, batch_size, shuffle, adam, seed, validation_batch_size, early_stopping)
+    hist, acc, val_loss, val_acc, epochs_run, best_epoch = _fit_slots(
+        eng, params, fit_jobs, S, N, xf, yf, split, row_map, M, epochs, batch_size, shuffle, adam, seed, validation_batch_size, early_stopping,
+        loss)
     if n_train == slot_n:  # nothing held out
         val_loss = val_acc = None
 
@@ -921,6 +927,6 @@ def build_kfold_fleet(eng: "engine.FFEngine", x, y, rows: int, cv, epochs: int =
         return None if t is None else t.cpu().numpy()
 
     return KFoldFleetBuild(
-        eng, M, K, N, n_test, params, init_params, host(loss), host(acc), host(val_loss), host(val_acc), int(epochs), host(epochs_run),
+        eng, M, K, N, n_test, params, init_params, host(hist), host(acc), host(val_loss), host(val_acc), int(epochs), host(epochs_run),
         host(best_epoch), (np.repeat(n_train, M) + int(batch_size) - 1) // int(batch_size), y_lo, y_hi, in_lo, in_hi, bool(target_scaler),
         host(feat).astype(np.float64), host(agg).astype(np.float64), host(moments).reshape(K, M, 5, T).transpose(1, 0, 2, 3).copy())

@@ -4,12 +4,12 @@ gordo/machine/model/factories/feedforward_autoencoder.py:15-251, returning an ``
 
 Topology (reference :65-104): encoder Dense layers (the first one plain, the following ones with an
 l1(10e-5) activity regulariser), decoder Dense layers, then ``Dense(n_features_out, out_func)``;
-compiled with Adam / mean squared error / metrics ["accuracy"].
+compiled with Adam / metrics ["accuracy"] and ``compile_kwargs["loss"]``, mean squared error by default (``specs.resolve_loss``).
 """
 from typing import Any, Dict, Optional, Tuple
 
 from ..register import register_model_builder
-from .specs import FFNetSpec, _check_act, _optimizer
+from .specs import FFNetSpec, _check_act, _optimizer, resolve_loss
 from .utils import check_dim_func_len, hourglass_calc_dims
 
 __all__ = ["feedforward_model", "feedforward_symmetric", "feedforward_hourglass"]
@@ -38,7 +38,7 @@ def feedforward_model(
     acts = [_check_act(f) for f in (*encoding_func, *decoding_func, out_func)]
     l1 = [0.0 if i == 0 else ACTIVITY_L1 for i in range(len(encoding_dim))] + [0.0] * (len(decoding_dim) + 1)
     metrics = list((compile_kwargs or {}).get("metrics", ["accuracy"]))
-    return FFNetSpec(dims, acts, l1, _optimizer(optimizer, optimizer_kwargs, compile_kwargs), metrics)
+    return FFNetSpec(dims, acts, l1, _optimizer(optimizer, optimizer_kwargs), metrics, resolve_loss(compile_kwargs))
 
 
 @register_model_builder(type="KerasAutoEncoder")

@@ -6,7 +6,7 @@ Registered for both wrapper types, like the reference (:15-16, :106-107, :177-17
 from typing import Any, Dict, Optional, Tuple
 
 from ..register import register_model_builder
-from .specs import LSTMNetSpec, _check_act, _optimizer
+from .specs import LSTMNetSpec, _check_act, _optimizer, resolve_loss
 from .utils import check_dim_func_len, hourglass_calc_dims
 
 __all__ = ["lstm_model", "lstm_symmetric", "lstm_hourglass"]
@@ -34,7 +34,7 @@ def lstm_model(
     units = [*map(int, encoding_dim), *map(int, decoding_dim)]
     acts = [_check_act(f) for f in (*encoding_func, *decoding_func)]
     return LSTMNetSpec(int(n_features), units, acts, int(n_features_out), _check_act(out_func), int(lookback_window),
-                       _optimizer(optimizer, optimizer_kwargs, compile_kwargs), list((compile_kwargs or {}).get("metrics", [])))
+                       _optimizer(optimizer, optimizer_kwargs), list((compile_kwargs or {}).get("metrics", [])), resolve_loss(compile_kwargs))
 
 
 @register_model_builder(type="KerasLSTMAutoEncoder")

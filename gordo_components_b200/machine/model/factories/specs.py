@@ -11,13 +11,34 @@ def _check_act(name):
     return name
 
 
-def _optimizer(optimizer, optimizer_kwargs, compile_kwargs):
-    """Only what the kernels implement is accepted: Adam + mean squared error."""
+# The Keras 3 loss names the fit kernels implement (the spellings keras.losses.get resolves [3P keras 3.3.3]) -> canonical
+# name, which is what a spec stores and what engine / _cabi.LOSS_CODES take.  Per-element definitions: include/gordo_b200.h gb_loss.
+LOSS_NAMES = {
+    **dict.fromkeys(("mse", "MSE", "mean_squared_error", "MeanSquaredError"), "mse"),
+    **dict.fromkeys(("mae", "MAE", "mean_absolute_error", "MeanAbsoluteError"), "mae"),
+    **dict.fromkeys(("mape", "MAPE", "mean_absolute_percentage_error", "MeanAbsolutePercentageError"), "mape"),
+    **dict.fromkeys(("msle", "MSLE", "mean_squared_logarithmic_error", "MeanSquaredLogarithmicError"), "msle"),
+    **dict.fromkeys(("huber", "Huber"), "huber"),
+    **dict.fromkeys(("log_cosh", "LogCosh"), "log_cosh"),
+}
+
+
+def resolve_loss(compile_kwargs) -> str:
+    """
+    Canonical name of ``compile_kwargs["loss"]`` (mean squared error when absent, as the reference's factories default it).
+    Only names are accepted: a loss object or dict (e.g. a Huber with another delta) and every loss the kernels do not
+    implement are refused.
+    """
+    loss = (compile_kwargs or {}).get("loss", "mse")
+    if not isinstance(loss, str) or loss not in LOSS_NAMES:
+        raise ValueError(f"loss {loss!r}: the CUDA fit kernels implement the losses {sorted(LOSS_NAMES)}")
+    return LOSS_NAMES[loss]
+
+
+def _optimizer(optimizer, optimizer_kwargs):
+    """Only what the kernels implement is accepted: Adam."""
     if not isinstance(optimizer, str) or optimizer.lower() != "adam":
         raise ValueError(f"optimizer {optimizer!r}: the CUDA fit kernel implements Adam only")
-    loss = (compile_kwargs or {}).get("loss", "mse")
-    if loss not in ("mse", "mean_squared_error"):
-        raise ValueError(f"loss {loss!r}: the CUDA fit kernel implements mean squared error only")
     kw = dict(optimizer_kwargs or {})
     out = {
         "lr": float(kw.pop("learning_rate", kw.pop("lr", 1e-3))),
@@ -39,6 +60,7 @@ class FFNetSpec:
     l1: List[float]
     adam: Dict[str, float] = field(default_factory=lambda: {"lr": 1e-3, "beta1": 0.9, "beta2": 0.999, "eps": 1e-7})
     metrics: List[str] = field(default_factory=lambda: ["accuracy"])
+    loss: str = "mse"  # canonical name (resolve_loss); a plain default, so a spec pickled before the field existed loads as MSE
 
     @property
     def n_layers(self):
@@ -68,6 +90,7 @@ class LSTMNetSpec:
     lookback_window: int
     adam: Dict[str, float] = field(default_factory=lambda: {"lr": 1e-3, "beta1": 0.9, "beta2": 0.999, "eps": 1e-7})
     metrics: List[str] = field(default_factory=list)
+    loss: str = "mse"  # as FFNetSpec.loss
 
     @property
     def units(self):

@@ -364,15 +364,15 @@ class KerasBaseEstimator(BaseEstimator, GordoBase):
             frozen = dict(spec.adam, lr=0.0)
             for e in range(epochs):
                 loss, acc, state = eng.fit(params, jobs, 1, n_train, xd, yd, epochs=1, batch_size=batch_size, shuffle=shuffle,
-                                           adam=spec.adam, seed=seed + e, state=state, step0=step0)
+                                           adam=spec.adam, seed=seed + e, state=state, step0=step0, loss=spec.loss)
                 step0 += steps
                 logs = {"loss": float(loss[0, 0])}
                 if "accuracy" in history:
                     logs["accuracy"] = float(acc[0, 0])
                 if n_val:
-                    # keras evaluates the *total* loss (MSE + activity regularisation) on the held-out tail in batches: the fit
+                    # keras evaluates the *total* loss (the compiled loss + activity regularisation) on the held-out tail in batches: the fit
                     # kernel with a zero learning rate on a throw-away optimizer state computes exactly that and moves nothing
-                    vl, va, _ = eng.fit(params, vjobs, 1, n_val, xd, yd, epochs=1, batch_size=vbatch, shuffle=False, adam=frozen)
+                    vl, va, _ = eng.fit(params, vjobs, 1, n_val, xd, yd, epochs=1, batch_size=vbatch, shuffle=False, adam=frozen, loss=spec.loss)
                     logs["val_loss"] = float(vl[0, 0])
                     if "accuracy" in history:
                         logs["val_accuracy"] = float(va[0, 0])
@@ -386,7 +386,7 @@ class KerasBaseEstimator(BaseEstimator, GordoBase):
             epochs_run = len(history["loss"])
         else:
             loss, acc, _ = eng.fit(params, jobs, 1, n_train, xd, yd, epochs=epochs, batch_size=batch_size, shuffle=shuffle,
-                                   adam=spec.adam, seed=seed)
+                                   adam=spec.adam, seed=seed, loss=spec.loss)
             history["loss"] = [float(v) for v in loss[0].cpu().numpy()]
             if "accuracy" in history:
                 history["accuracy"] = [float(v) for v in acc[0].cpu().numpy()]
@@ -512,7 +512,7 @@ class KerasLSTMBaseEstimator(KerasBaseEstimator, TransformerMixin, metaclass=abc
             state = None
             for e in range(epochs):
                 loss, acc, state = eng.fit(params, jobs, 1, n_win, xd, yd, epochs=1, batch_size=batch_size, lookahead=self.lookahead,
-                                           primer=(e == 0), adam=getattr(spec, "adam", None), state=state)
+                                           primer=(e == 0), adam=getattr(spec, "adam", None), state=state, loss=spec.loss)
                 logs = {"loss": float(loss[0, 0])}
                 if want_acc:
                     logs["accuracy"] = float(acc[0, 0])
@@ -525,7 +525,7 @@ class KerasLSTMBaseEstimator(KerasBaseEstimator, TransformerMixin, metaclass=abc
                     params = cb.best_weights
         else:
             loss, acc, _ = eng.fit(params, jobs, 1, n_win, xd, yd, epochs=epochs, batch_size=batch_size, lookahead=self.lookahead,
-                                   primer=True, adam=getattr(spec, "adam", None))
+                                   primer=True, adam=getattr(spec, "adam", None), loss=spec.loss)
             history["loss"] = [float(v) for v in loss[0].cpu().numpy()]
             if want_acc:
                 history["accuracy"] = [float(v) for v in acc[0].cpu().numpy()]

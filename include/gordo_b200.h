@@ -48,6 +48,20 @@ typedef enum gb_status {
 
 typedef enum gb_act { GB_ACT_LINEAR = 0, GB_ACT_TANH = 1, GB_ACT_RELU = 2, GB_ACT_SIGMOID = 3 } gb_act;
 
+/* Training loss (the `loss` of the reference's compile_kwargs, a Keras 3 loss name).  With e = yhat - y and eps = 1e-7, each is a
+ * per-element f averaged over all B * n_out elements of a mini-batch (Keras' per-sample mean, then sum_over_batch_size):
+ *   MSE e^2;  MAE |e|;  MAPE 100 |e| / max(|y|, eps);  MSLE (log(max(yhat, eps) + 1) - log(max(y, eps) + 1))^2;
+ *   HUBER 0.5 e^2 if |e| <= 1 else |e| - 0.5 (delta 1);  LOG_COSH e + softplus(-2 e) - log 2.
+ * Gradients follow TF: sign(0) = 0 for MAE / MAPE, and MSLE passes none where yhat < eps. */
+typedef enum gb_loss {
+  GB_LOSS_MSE = 0,
+  GB_LOSS_MAE = 1,
+  GB_LOSS_MAPE = 2,
+  GB_LOSS_MSLE = 3,
+  GB_LOSS_HUBER = 4,
+  GB_LOSS_LOG_COSH = 5
+} gb_loss;
+
 /* Dense stack built by feedforward_model / feedforward_symmetric / feedforward_hourglass
  * (gordo/machine/model/factories/feedforward_autoencoder.py:65-104).  dims[0] = n_features,
  * dims[l+1] = units of Dense layer l; l1[l] = activity_regularizer l1 coefficient of layer l
@@ -209,7 +223,8 @@ int gb_minmax_inverse_f32(const gb_job* jobs, int32_t n_jobs, int32_t max_rows, 
 /* ---- K2: fit ---------------------------------------------------------------------------
  * Replaces scikeras KerasRegressor.fit -> keras Model.fit (models.py:284) for the Dense
  * stacks above: per job, `epochs` passes over rows [x_row, x_row+n_rows) in batches of
- * `batch_size`, loss = mean((net(x)-y)^2) + sum_l l1[l]*sum|a_l|, Adam (Keras defaults).
+ * `batch_size`, loss = mean(f(net(x), y)) + sum_l l1[l]*sum|a_l| with f the gb_loss of hp->loss (mean squared error by
+ * default), Adam (Keras defaults).  The history and the held-out statistics report the same loss.
  * One CTA per job trains the whole fit with weights resident in shared memory. */
 typedef struct gb_fit_hparams {
   int32_t epochs;
@@ -220,7 +235,7 @@ typedef struct gb_fit_hparams {
   float lr, beta1, beta2, eps;
   uint64_t seed;
   int32_t step0;          /* Adam step count already taken (warm start); 0 for a fresh fit */
-  int32_t reserved;
+  int32_t loss;           /* gb_loss; 0 = GB_LOSS_MSE.  Outside 0..5: GB_E_ARG, nothing enqueued */
 } gb_fit_hparams;
 
 /* Adam moments are opaque optimizer state in the kernel's padded layout: gb_ffae_fit_state_stride() floats per slot. */
@@ -346,6 +361,12 @@ size_t gb_lstm_fit_workspace_bytes(const gb_lstmnet* net, int32_t n_jobs);
 int gb_lstm_fit(const gb_lstmnet* net, float* params, float* adam_m, float* adam_v, int32_t* adam_t,
                 const gb_job* jobs, int32_t n_jobs, int32_t max_windows, const float* x, const float* y,
                 const gb_lstm_fit_hparams* hp, void* workspace, float* out_loss, float* out_acc, void* stream);
+/* gb_lstm_fit on the gb_loss `loss` (primer step and history included): loss = mean(f(net(window), target)).
+ * gb_lstm_fit is this with GB_LOSS_MSE.  Outside 0..5: GB_E_ARG, nothing enqueued. */
+int gb_lstm_fit_loss(const gb_lstmnet* net, float* params, float* adam_m, float* adam_v, int32_t* adam_t,
+                     const gb_job* jobs, int32_t n_jobs, int32_t max_windows, const float* x, const float* y,
+                     const gb_lstm_fit_hparams* hp, void* workspace, float* out_loss, float* out_acc, int32_t loss,
+                     void* stream);
 
 /* Keras' Orthogonal initialiser for recurrent kernels: g holds n_mats standard-normal [rows][cols] draws (float64, rows <= cols,
  * overwritten); matrix i's rows are orthonormalised (Gram-Schmidt, the sign convention of Keras' QR) and written as float32 to
