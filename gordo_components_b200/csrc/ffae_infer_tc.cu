@@ -435,52 +435,83 @@ __global__ void __launch_bounds__(NTHREADS, 1) ffae_tc_kernel(const __grid_const
 #pragma unroll
           for (int j = 0; j < 8; ++j) yr[hr][j] = *reinterpret_cast<const float2*>(ys + tile_ofs(wq * 16 + g + 8 * hr, 8 * j + 2 * t));
       }
-      // model output of fragment rows g + 8 hr, columns 8j + 2t, + 1 (the output layer's MMAs write no columns past Np)
+      // model output of fragment rows g + 8 hr, columns 8j + 2t, + 1 (the output layer's MMAs write no columns past Np).  The
+      // accumulator registers are only read here: a write to them outside the MMAs makes ptxas serialise the wgmma chains.
       auto model_out = [&](int hr, int j) {
         const float2 b = *reinterpret_cast<const float2*>(bo + 8 * j + 2 * t);
         return j < nt ? make_float2(d[4 * j + 2 * hr] + b.x, d[4 * j + 2 * hr + 1] + b.y) : make_float2(0.f, 0.f);
       };
 
-      // Per-tag outputs: for each array the warp asked for, and each half of 32 columns, the fragment goes into one of the warp's
-      // two staging boxes, in turn, and lane 0 hands the box to a TMA store.  A store clips at the array's edges but not at
-      // the end of the job, whose next rows may belong to another job written by another CTA: a warp whose 16 rows are not all
-      // inside the job copies its live rows out of the box itself.
+      // Per-tag outputs, one pass per array: model output, |y^ - y| (which then replaces y in registers), the same scaled, and
+      // the same over the feature thresholds.  The passes over the unscaled and scaled arrays also sum the row totals, even when
+      // the array itself is not asked for.  A pass stages its array's fragment in the warp's two 2 KB boxes, one per half of
+      // 32 columns (with T <= 32 one box, the two boxes taking the arrays in turn), and lane 0 hands them to TMA stores.  A
+      // store clips at the array's edges but not at the end of the job, whose next rows may belong to another job written by
+      // another CTA: a warp whose 16 rows are not all inside the job copies its live rows out of the boxes itself.
       const int n_live = min(row_end - wrow, OBOX_ROWS);
+      const bool want_su = has_y && a.o_totu, want_ss = has_y && (a.o_tots || a.o_totconf);
+      float ss[2] = {0.f, 0.f}, su[2] = {0.f, 0.f};
       if (n_live > 0) {
-        int k = 0;  // boxes staged in this tile
+        const int nh = TP > BOX_COLS ? 2 : 1;  // halves of 32 columns in a row
+        int k = 0;                             // store groups issued in this tile
 #pragma unroll
         for (int arr = 0; arr < 4; ++arr) {
+          if (arr == 1 && has_y) {
+#pragma unroll
+            for (int hr = 0; hr < 2; ++hr)
+#pragma unroll
+              for (int j = 0; j < 8; ++j) {
+                const float2 m = model_out(hr, j);
+                yr[hr][j] = make_float2(fabsf(m.x - yr[hr][j].x), fabsf(m.y - yr[hr][j].y));
+              }
+          }
           float* o = arr == 0 ? a.o_model : arr == 1 ? a.o_tu : arr == 2 ? a.o_ts : a.o_conf;
-          if (o == nullptr || (arr > 0 && !has_y)) continue;
+          const bool put = o != nullptr && (arr == 0 || has_y);
+          const bool acc = arr == 1 ? want_su : arr == 2 ? want_ss : false;
+          if (!put && !acc) continue;
+          const float* sv = vec + (arr == 3 ? W : 0);
+          const uint32_t box0 = nh == 2 || (k & 1) == 0 ? obox0 : obox1;  // the box of columns 0..31; obox1 takes 32..63
+          if (put) {
+            if (lane == 0) {  // the stores that last used the box(es) have read them
+              if (nh == 2 && k >= 1) bulk_wait_read<0>();
+              if (nh == 1 && k >= 2) bulk_wait_read<1>();
+            }
+            __syncwarp();
+          }
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
-            if (h == 1 && TP <= BOX_COLS) break;
-            const uint32_t box = (k & 1) ? obox1 : obox0;
-            if (k >= 2 && lane == 0) bulk_wait_read<1>();  // the store that last used this box has read it
-            __syncwarp();
-            uint8_t* bs = smem + (box - sbase);
+            if (h == nh) break;
+            uint8_t* bs = smem + ((h ? obox1 : box0) - sbase);
 #pragma unroll
             for (int hr = 0; hr < 2; ++hr)
 #pragma unroll
               for (int jj = 0; jj < 4; ++jj) {
                 const int j = 4 * h + jj, col = 8 * j + 2 * t;
-                float2 v = model_out(hr, j);
-                if (arr > 0) {
-                  const float2 yv = yr[hr][j];
-                  v = make_float2(fabsf(v.x - yv.x), fabsf(v.y - yv.y));
-                  const float2 s = *reinterpret_cast<const float2*>(vec + (arr == 3 ? W : 0) + col);
-                  if (arr > 1) v = make_float2(v.x * s.x, v.y * s.y);
+                float2 v = arr == 0 ? model_out(hr, j) : yr[hr][j];
+                if (arr > 1) {
+                  const float2 s = *reinterpret_cast<const float2*>(sv + col);
+                  v = make_float2(v.x * s.x, v.y * s.y);
                 }
-                *reinterpret_cast<float2*>(bs + box_ofs(g + 8 * hr, 8 * jj + 2 * t)) = v;
+                if (acc && col < TP) {  // T is a multiple of 4: col + 1 < T too
+                  // rounding pinned to fma(x, x, y * y) and an add, so it does not depend on how the compiler contracts
+                  const float q = __fmaf_rn(v.x, v.x, __fmul_rn(v.y, v.y));
+                  if (arr == 1) su[hr] = __fadd_rn(su[hr], q);
+                  else ss[hr] = __fadd_rn(ss[hr], q);
+                }
+                if (put) *reinterpret_cast<float2*>(bs + box_ofs(g + 8 * hr, 8 * jj + 2 * t)) = v;
               }
-            fence_proxy_async();  // the box is read by the TMA store (async proxy)
-            __syncwarp();
-            if (n_live == OBOX_ROWS) {
-              if (lane == 0) {
-                tma_store_2d(&a.tm_o[arr], box, BOX_COLS * h, (int)(job.out_row + wrow));
-                bulk_commit();
-              }
-            } else {
+          }
+          if (!put) continue;
+          fence_proxy_async();  // the boxes are read by the TMA stores (async proxy)
+          __syncwarp();
+          if (n_live == OBOX_ROWS) {
+            if (lane == 0) {
+              for (int h = 0; h < nh; ++h) tma_store_2d(&a.tm_o[arr], h ? obox1 : box0, BOX_COLS * h, (int)(job.out_row + wrow));
+              bulk_commit();
+            }
+          } else {
+            for (int h = 0; h < nh; ++h) {
+              const uint8_t* bs = smem + ((h ? obox1 : box0) - sbase);
               const int cols = min(BOX_COLS, TP - BOX_COLS * h);
               for (int i = lane; i < n_live * 8; i += 32) {  // 16-byte chunk c of row r: coalesced along the row
                 const int r = i >> 3, c = i & 7;
@@ -489,26 +520,11 @@ __global__ void __launch_bounds__(NTHREADS, 1) ffae_tc_kernel(const __grid_const
                          *reinterpret_cast<const float4*>(bs + box_ofs(r, 4 * c)));
               }
             }
-            ++k;
           }
+          ++k;
         }
       }
       if (totals) {
-        float ss[2] = {0.f, 0.f}, su[2] = {0.f, 0.f};
-#pragma unroll
-        for (int hr = 0; hr < 2; ++hr)
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const int col = 8 * j + 2 * t;
-            if (j < nt && col < TP) {  // T is a multiple of 4: col + 1 < T too
-              const float2 yh = model_out(hr, j), yv = yr[hr][j];
-              const float2 sc = *reinterpret_cast<const float2*>(vec + col);
-              const float2 df = make_float2(fabsf(yh.x - yv.x), fabsf(yh.y - yv.y));
-              const float2 e = make_float2(df.x * sc.x, df.y * sc.y);
-              su[hr] += df.x * df.x + df.y * df.y;
-              ss[hr] += e.x * e.x + e.y * e.y;
-            }
-          }
 #pragma unroll
         for (int hr = 0; hr < 2; ++hr) {
           ss[hr] += __shfl_xor_sync(0xffffffffu, ss[hr], 1);
