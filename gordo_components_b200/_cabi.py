@@ -33,7 +33,7 @@ def loss_code(loss: str) -> int:
 EXPORTS = (
     "gb_abi_version", "gb_last_error", "gb_device_check", "gb_ffnet_param_count", "gb_ffnet_param_stride",
     "gb_ffae_infer_score", "gb_ffae_tc_supported", "gb_ffae_infer_plan", "gb_anomaly_score", "gb_anomaly_score_f64", "gb_minmax_fit", "gb_minmax_f64", "gb_thresholds", "gb_thresholds_f64", "gb_cv_moments", "gb_smooth", "gb_quantile", "gb_affine_f64", "gb_gather_rows", "gb_minmax_inverse_f32", "gb_ffae_fit_state_stride", "gb_ffae_fit", "gb_ffae_fit_split", "gb_ffae_fit_stop", "gb_ffae_fit_plan",
-    "gb_lstm_param_count", "gb_lstm_param_stride", "gb_lstm_workspace_bytes", "gb_lstm_infer", "gb_lstm_tc_supported", "gb_lstm_tc_workspace_bytes", "gb_lstm_infer_tc", "gb_lstm_fit_workspace_bytes", "gb_lstm_fit", "gb_lstm_fit_loss",
+    "gb_lstm_param_count", "gb_lstm_param_stride", "gb_lstm_workspace_bytes", "gb_lstm_infer", "gb_lstm_tc_supported", "gb_lstm_tc_workspace_bytes", "gb_lstm_infer_tc", "gb_lstm_fit_workspace_bytes", "gb_lstm_fit", "gb_lstm_fit_loss", "gb_lstm_fit_tc_workspace_bytes", "gb_lstm_fit_tc",
     "gb_orthonormal_rows",
 )
 
@@ -155,6 +155,10 @@ def _declare(lib):
     lib.gb_lstm_fit.restype = C.c_int
     lib.gb_lstm_fit_loss.argtypes = lib.gb_lstm_fit.argtypes[:-1] + [C.c_int32, _P]
     lib.gb_lstm_fit_loss.restype = C.c_int
+    lib.gb_lstm_fit_tc_workspace_bytes.restype = C.c_size_t
+    lib.gb_lstm_fit_tc_workspace_bytes.argtypes = [C.POINTER(GbLstmNet), C.c_int32, C.c_int32]
+    lib.gb_lstm_fit_tc.argtypes = lib.gb_lstm_fit_loss.argtypes
+    lib.gb_lstm_fit_tc.restype = C.c_int
     lib.gb_orthonormal_rows.argtypes = [_P, C.c_int32, C.c_int32, C.c_int32, _P, C.c_int64, C.c_int64, _P]
     lib.gb_orthonormal_rows.restype = C.c_int
     for name in ("gb_device_check", "gb_ffae_infer_score", "gb_ffae_tc_supported", "gb_ffae_infer_plan", "gb_anomaly_score", "gb_minmax_fit", "gb_thresholds", "gb_smooth", "gb_ffae_fit", "gb_ffae_fit_split", "gb_ffae_fit_stop", "gb_lstm_infer"):

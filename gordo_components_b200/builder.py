@@ -12,8 +12,8 @@ in one ``gb_ffae_fit`` launch, fold scoring / thresholds / scaler statistics / m
 (loss, accuracy, and their ``val_*`` forms with a ``validation_split``) is batched as well: every fit applies the rule inside the
 launch (``gb_ffae_fit_stop``), and machines that differ only in the callback's parameters share a bucket.  The LSTM form
 of the same definition (``KerasLSTMAutoEncoder`` / ``KerasLSTMForecast``, ``_canonical_lstm``) is bucketed by architecture,
-lookback, lookahead and training length and built by ``fleet.build_lstm_fleet``: all fits as jobs of ``gb_lstm_fit`` (in
-chunks that fit a workspace budget), every fold model's test block in one LSTM inference launch, float64 scoring.  The
+lookback, lookahead, batch size and training length and built by ``fleet.build_lstm_fleet``: all fits as jobs of ``gb_lstm_fit``
+(batches above 32 windows: ``gb_lstm_fit_tc``, with ``FleetModelBuilder(lstm_wide_batches=True)``; in chunks that fit a workspace budget), every fold model's test block in one LSTM inference launch, float64 scoring.  The
 cross-validation ``scores`` block of the metadata is then assembled on the host from ``gb_cv_moments``' five sums per
 (fold, tag).  Any other definition (other transformers in a Pipeline, callbacks unless batched as above, LSTM fits with
 callbacks, K-fold detectors unless ``FleetModelBuilder(kfcv=True)`` batches them under a KFold cv through ``fleet.build_kfold_fleet``,
@@ -484,13 +484,16 @@ def _is_lstm_definition(machine) -> bool:
     return isinstance(est, KerasLSTMBaseEstimator)
 
 
-def _canonical_lstm(index, machine) -> Optional[_CanonicalLSTM]:
+def _canonical_lstm(index, machine, wide_batches: bool = False) -> Optional[_CanonicalLSTM]:
     """
     The LSTM form of the canonical definition -- ``DiffBasedAnomalyDetector(KerasLSTMAutoEncoder | KerasLSTMForecast)``, the network bare
     or behind one default ``MinMaxScaler``, under the evaluation ``_canonical`` accepts -- as a candidate for the batched path, or
     ``None`` with the reason logged.  Machines too short for the CV folds go to ``ModelBuilder``, which raises the reference's errors.
+    ``wide_batches``: also take batch sizes above 32, up to ``LSTMEngine.TC_MAX_BATCH`` (the tensor-core fit family;
+    ``FleetModelBuilder(lstm_wide_batches=True)``).
     """
     from .machine.model.anomaly.diff import DiffBasedAnomalyDetector
+    from .engine import LSTMEngine
     from .machine.model.factories.specs import LSTMNetSpec
     from .machine.model.models import KerasLSTMAutoEncoder, KerasLSTMForecast
 
@@ -526,8 +529,11 @@ def _canonical_lstm(index, machine) -> Optional[_CanonicalLSTM]:
     if fit_args.get("validation_split") or fit_args.get("callbacks"):
         return no("validation_split / callbacks need the per-epoch loop")
     batch_size = int(est.batch_size)
-    if not 1 <= batch_size <= 32:
-        return no(f"batch_size {batch_size}: the batched LSTM fit takes at most 32 windows per batch")
+    if not 1 <= batch_size <= LSTMEngine.FP32_MAX_BATCH and not (wide_batches and 1 <= batch_size <= LSTMEngine.TC_MAX_BATCH):
+        if wide_batches:
+            return no(f"batch_size {batch_size}: the batched LSTM fit takes at most {LSTMEngine.TC_MAX_BATCH} windows per batch")
+        return no(f"batch_size {batch_size}: the batched LSTM fit takes at most {LSTMEngine.FP32_MAX_BATCH} windows per batch "
+                  "(FleetModelBuilder(lstm_wide_batches=True) batches up to 256)")
 
     t0 = time.time()
     X, y, dataset_meta = _get_data(machine["dataset"])
@@ -647,11 +653,16 @@ class FleetModelBuilder:
     ``kfcv``: also batch ``DiffBasedKFCVAnomalyDetector`` machines under a ``KFold`` cv (``_canonical_kfcv``; the reference's
     production definition), built by ``fleet.build_kfold_fleet``.  Off by default for the same reason: the batched fits draw their
     initial weights per fleet, so without the flag these machines build through ``ModelBuilder`` as before.
+
+    ``lstm_wide_batches``: also batch LSTM machines whose batch_size is above 32 (up to 256), trained by the tensor-core fit
+    family (``LSTMEngine.fit_tc``).  Off by default for the same reason: without it such machines build through ``ModelBuilder``,
+    whose estimator fit runs the same family one machine at a time.
     """
 
-    def __init__(self, machines: Sequence, early_stopping: bool = False, kfcv: bool = False):
+    def __init__(self, machines: Sequence, early_stopping: bool = False, kfcv: bool = False, lstm_wide_batches: bool = False):
         self.early_stopping = bool(early_stopping)
         self.kfcv = bool(kfcv)
+        self.lstm_wide_batches = bool(lstm_wide_batches)
         self.machines = [_machine_dict(m) for m in machines]
         names = [m["name"] for m in self.machines]
         if len(set(names)) != len(names):
@@ -665,14 +676,14 @@ class FleetModelBuilder:
         from . import fleet
 
         return FleetModelBuilder([self.machines[i] for i in fleet.partition(len(self.machines), world)[rank]], early_stopping=self.early_stopping,
-                                 kfcv=self.kfcv)
+                                 kfcv=self.kfcv, lstm_wide_batches=self.lstm_wide_batches)
 
     def build(self, output_dir: Optional[str] = None) -> List[Tuple[Any, dict]]:
         results: List[Optional[Tuple[Any, dict]]] = [None] * len(self.machines)
         buckets: Dict[tuple, List[_Canonical]] = {}
         for i, machine in enumerate(self.machines):
             if _is_lstm_definition(machine):
-                c = _canonical_lstm(i, machine)
+                c = _canonical_lstm(i, machine, wide_batches=self.lstm_wide_batches)
             elif self.kfcv and _is_kfcv_definition(machine):
                 c = _canonical_kfcv(i, machine, early_stopping=self.early_stopping)
             else:
@@ -937,15 +948,16 @@ def machines_from_config(config, project_name: str = "local-build", datasets=Non
     return machines
 
 
-def local_build(config_str, datasets=None, batched: bool = True, early_stopping: bool = False, kfcv: bool = False):
+def local_build(config_str, datasets=None, batched: bool = True, early_stopping: bool = False, kfcv: bool = False,
+                lstm_wide_batches: bool = False):
     """
     Build the model(s) of a bare gordo config locally and yield ``(model, machine)`` per machine, in config order
     (gordo/builder/local_build.py:15-80).  ``batched=False`` builds one machine at a time like the reference does;
-    ``early_stopping`` and ``kfcv`` are ``FleetModelBuilder``'s.
+    ``early_stopping``, ``kfcv`` and ``lstm_wide_batches`` are ``FleetModelBuilder``'s.
     """
     machines = machines_from_config(config_str, datasets=datasets)
     if batched:
-        yield from FleetModelBuilder(machines, early_stopping=early_stopping, kfcv=kfcv).build()
+        yield from FleetModelBuilder(machines, early_stopping=early_stopping, kfcv=kfcv, lstm_wide_batches=lstm_wide_batches).build()
     else:
         for machine in machines:
             yield ModelBuilder(machine).build()

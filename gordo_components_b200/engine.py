@@ -561,9 +561,26 @@ class LSTMEngine:
             out.append((layers, (Wd, vec[ofs:ofs + self.n_out].copy())))
         return out
 
+    FP32_MAX_BATCH = 32   # largest batch of the fp32 fit family (gb_lstm_fit_loss)
+    TC_MAX_BATCH = 256    # largest batch of the tensor-core fit family (gb_lstm_fit_tc)
+
     def fit_workspace_bytes(self, n_jobs: int) -> int:
         """Device scratch one ``fit`` launch of ``n_jobs`` jobs allocates (gb_lstm_fit_workspace_bytes)."""
         return int(self.lib.gb_lstm_fit_workspace_bytes(C.byref(self.net), int(n_jobs)))
+
+    def fit_tc_workspace_bytes(self, n_jobs: int, batch_size: int) -> int:
+        """Device scratch one ``fit_tc`` launch of ``n_jobs`` jobs at ``batch_size`` allocates (gb_lstm_fit_tc_workspace_bytes)."""
+        return int(self.lib.gb_lstm_fit_tc_workspace_bytes(C.byref(self.net), int(n_jobs), int(batch_size)))
+
+    def fit_for_batch(self, batch_size: int):
+        """The fit family for ``batch_size``: ``fit`` (fp32) up to FP32_MAX_BATCH windows, ``fit_tc`` above."""
+        return self.fit if int(batch_size) <= self.FP32_MAX_BATCH else self.fit_tc
+
+    def fit_workspace_bytes_for_batch(self, n_jobs: int, batch_size: int) -> int:
+        """Workspace of the launch ``fit_for_batch(batch_size)`` makes for ``n_jobs`` jobs."""
+        if int(batch_size) <= self.FP32_MAX_BATCH:
+            return self.fit_workspace_bytes(n_jobs)
+        return self.fit_tc_workspace_bytes(n_jobs, batch_size)
 
     def fit(self, params, jobs_dev, n_jobs, max_windows, x, y, epochs: int = 1, batch_size: int = 32, lookahead: int = 0,
             primer: bool = True, adam: Optional[Dict[str, float]] = None, state=None, loss: str = "mse"):
@@ -572,6 +589,25 @@ class LSTMEngine:
         y[x_row + j + lookback - 1 + lookahead]).  Returns (loss [n_jobs, epochs], accuracy, (m, v, t)).  ``loss``: canonical
         Keras loss name (``_cabi.LOSS_CODES``), for the primer step too (gb_lstm_fit_loss).
         """
+        ws_bytes = int(self.lib.gb_lstm_fit_workspace_bytes(C.byref(self.net), int(n_jobs)))
+        return self._fit_launch(self.lib.gb_lstm_fit_loss, ws_bytes, params, jobs_dev, n_jobs, max_windows, x, y, epochs, batch_size,
+                                lookahead, primer, adam, state, loss)
+
+    def fit_tc(self, params, jobs_dev, n_jobs, max_windows, x, y, epochs: int = 1, batch_size: int = 32, lookahead: int = 0,
+               primer: bool = True, adam: Optional[Dict[str, float]] = None, state=None, loss: str = "mse"):
+        """
+        ``fit`` on the tensor-core family (gb_lstm_fit_tc): the same training for batches of 1 .. TC_MAX_BATCH windows, the
+        GEMMs of each step on wgmma in split TF32.  Same arguments, return value and (m, v, t) state, which may be carried
+        between calls of either family.  A batch above TC_MAX_BATCH raises ValueError before anything is launched.
+        """
+        if not 1 <= int(batch_size) <= self.TC_MAX_BATCH:
+            raise ValueError(f"batch_size={int(batch_size)}: the LSTM fit handles batches of 1 to {self.TC_MAX_BATCH} windows")
+        ws_bytes = self.fit_tc_workspace_bytes(n_jobs, batch_size)
+        return self._fit_launch(self.lib.gb_lstm_fit_tc, ws_bytes, params, jobs_dev, n_jobs, max_windows, x, y, epochs, batch_size,
+                                lookahead, primer, adam, state, loss)
+
+    def _fit_launch(self, entry, ws_bytes, params, jobs_dev, n_jobs, max_windows, x, y, epochs, batch_size, lookahead, primer, adam, state,
+                    loss):
         code = _cabi.loss_code(loss)
         torch = _torch()
         adam = adam or {}
@@ -585,15 +621,14 @@ class LSTMEngine:
             t = torch.zeros((params.shape[0],), dtype=torch.int32, device=self.device)
         else:
             m, v, t = state
-        ws_bytes = int(self.lib.gb_lstm_fit_workspace_bytes(C.byref(self.net), int(n_jobs)))
         ws = torch.empty((ws_bytes + 3) // 4, dtype=torch.float32, device=self.device)
         # a primer-only fit (epochs = 0) writes no history, but the kernel takes the outputs as non-NULL pointers and a tensor with
         # no elements has none: the buffers keep one column and the caller gets the empty slice
         hist = torch.zeros((n_jobs, max(epochs, 1)), dtype=torch.float32, device=self.device)
         acc = torch.zeros((n_jobs, max(epochs, 1)), dtype=torch.float32, device=self.device)
         p = _cabi.ptr
-        _cabi.check(self.lib.gb_lstm_fit_loss(C.byref(self.net), p(params), p(m), p(v), p(t), p(jobs_dev), int(n_jobs), int(max_windows), p(x),
-                                              p(y), C.byref(hp), p(ws), p(hist), p(acc), code, _stream_ptr()))
+        _cabi.check(entry(C.byref(self.net), p(params), p(m), p(v), p(t), p(jobs_dev), int(n_jobs), int(max_windows), p(x), p(y), C.byref(hp),
+                          p(ws), p(hist), p(acc), code, _stream_ptr()))
         return hist[:, :epochs], acc[:, :epochs], (m, v, t)
 
     @property

@@ -550,7 +550,9 @@ def build_lstm_fleet(eng: "engine.LSTMEngine", x, y, rows: int, lookahead: int =
 
     x, y: float64 device tensors [n_machines * rows, T]; machine m owns rows [m*rows, (m+1)*rows).  ``y`` may be ``x``.
 
-    ``memory_budget``: bytes of fit workspace (gb_lstm_fit_workspace_bytes) one gb_lstm_fit launch may take.  Machines are
+    ``batch_size``: up to 32 windows on gb_lstm_fit, up to 256 on gb_lstm_fit_tc (``LSTMEngine.fit_for_batch``).
+    ``memory_budget``: bytes of fit workspace (gb_lstm_fit_workspace_bytes, or gb_lstm_fit_tc_workspace_bytes at the batch size)
+    one fit launch may take.  Machines are
     trained in chunks that fit it -- all ``n_splits + 1`` fits of a machine in the same chunk; every job's result is the same
     whatever the chunking.  ``keep_init_params``: keep the initial parameters of every slot on the result (``init_params``).
     ``loss``: the estimator's canonical Keras loss name (``LSTMNetSpec.loss``).
@@ -606,7 +608,9 @@ def build_lstm_fleet(eng: "engine.LSTMEngine", x, y, rows: int, lookahead: int =
         yf, x_row = y32, base
 
     # fits: chunks of whole machines (final + K folds) whose workspace fits the budget
-    chunk = max(1, min(M, int(memory_budget) // max(eng.fit_workspace_bytes(K + 1), 1), 65535 // (K + 1)))
+    # (batches above 32 windows train on the tensor-core family, whose workspace grows with the batch)
+    fit = eng.fit_for_batch(batch_size)
+    chunk = max(1, min(M, int(memory_budget) // max(eng.fit_workspace_bytes_for_batch(K + 1, batch_size), 1), 65535 // (K + 1)))
     hist = torch.empty((S, epochs), dtype=torch.float32, device=dev)
     acc = torch.empty_like(hist)
     for m0 in range(0, M, chunk):
@@ -615,8 +619,8 @@ def build_lstm_fleet(eng: "engine.LSTMEngine", x, y, rows: int, lookahead: int =
         idx = torch.from_numpy(slots).to(dev)
         p = params.index_select(0, idx)
         jobs = engine.jobs_to_device(engine.make_jobs(np.arange(len(slots)), slot_windows[slots], x_row[slots]), dev)
-        cl, ca, _ = eng.fit(p, jobs, len(slots), int(slot_windows[slots].max()), xf, yf, epochs=epochs, batch_size=batch_size, lookahead=la,
-                            primer=True, adam=adam, loss=loss)
+        cl, ca, _ = fit(p, jobs, len(slots), int(slot_windows[slots].max()), xf, yf, epochs=epochs, batch_size=batch_size, lookahead=la,
+                        primer=True, adam=adam, loss=loss)
         params.index_copy_(0, idx, p)
         hist.index_copy_(0, idx, cl)
         acc.index_copy_(0, idx, ca)

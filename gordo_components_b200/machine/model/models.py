@@ -480,7 +480,8 @@ class KerasLSTMBaseEstimator(KerasBaseEstimator, TransformerMixin, metaclass=abc
         """
         models.py:557-616: the network is built and initialised, takes the reference's primer Adam step on the first window,
         then ``epochs`` passes over the lookback windows in order (``shuffle=False``) in batches of ``self.batch_size``
-        (gb_lstm_fit, back-propagation through time on the GPU).
+        (gb_lstm_fit, back-propagation through time on the GPU).  Batches of up to 32 windows train on the fp32 kernel family,
+        larger ones (up to 256) on the tensor-core family (``LSTMEngine.fit_tc``).
         """
         from ... import engine
 
@@ -500,6 +501,7 @@ class KerasLSTMBaseEstimator(KerasBaseEstimator, TransformerMixin, metaclass=abc
         if n_win < 1:
             raise ValueError("no training windows")
         eng = self._engine()
+        fit = eng.fit_for_batch(batch_size)
         dev = eng.device
         xd, yd = engine.to_device_f32(X, dev), engine.to_device_f32(y, dev)
         params = eng.pack_params([self.model.weights])
@@ -511,8 +513,8 @@ class KerasLSTMBaseEstimator(KerasBaseEstimator, TransformerMixin, metaclass=abc
         if callbacks:  # one launch sequence per epoch, the callbacks in between (the generator fit has no validation data)
             state = None
             for e in range(epochs):
-                loss, acc, state = eng.fit(params, jobs, 1, n_win, xd, yd, epochs=1, batch_size=batch_size, lookahead=self.lookahead,
-                                           primer=(e == 0), adam=getattr(spec, "adam", None), state=state, loss=spec.loss)
+                loss, acc, state = fit(params, jobs, 1, n_win, xd, yd, epochs=1, batch_size=batch_size, lookahead=self.lookahead,
+                                       primer=(e == 0), adam=getattr(spec, "adam", None), state=state, loss=spec.loss)
                 logs = {"loss": float(loss[0, 0])}
                 if want_acc:
                     logs["accuracy"] = float(acc[0, 0])
@@ -524,8 +526,8 @@ class KerasLSTMBaseEstimator(KerasBaseEstimator, TransformerMixin, metaclass=abc
                 if cb.restore_best_weights and cb.best_weights is not None:
                     params = cb.best_weights
         else:
-            loss, acc, _ = eng.fit(params, jobs, 1, n_win, xd, yd, epochs=epochs, batch_size=batch_size, lookahead=self.lookahead,
-                                   primer=True, adam=getattr(spec, "adam", None), loss=spec.loss)
+            loss, acc, _ = fit(params, jobs, 1, n_win, xd, yd, epochs=epochs, batch_size=batch_size, lookahead=self.lookahead,
+                               primer=True, adam=getattr(spec, "adam", None), loss=spec.loss)
             history["loss"] = [float(v) for v in loss[0].cpu().numpy()]
             if want_acc:
                 history["accuracy"] = [float(v) for v in acc[0].cpu().numpy()]

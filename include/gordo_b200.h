@@ -352,7 +352,7 @@ int gb_lstm_infer_tc(const gb_lstmnet* net, const float* params, int32_t n_slots
  * workspace: gb_lstm_fit_workspace_bytes(net, n_jobs) bytes of device scratch (saved gates/states of
  * one batch per job).  One optimizer step is a sequence of launches over (tile, job) grids. */
 typedef struct gb_lstm_fit_hparams {
-  int32_t epochs, batch_size;   /* batch_size <= 32 */
+  int32_t epochs, batch_size;   /* batch_size <= 32 (gb_lstm_fit_tc: <= 256) */
   int32_t lookahead;            /* 0 = KerasLSTMAutoEncoder, 1 = KerasLSTMForecast */
   int32_t primer;               /* 1 = run the reference's primer step first */
   float lr, beta1, beta2, eps;
@@ -367,6 +367,16 @@ int gb_lstm_fit_loss(const gb_lstmnet* net, float* params, float* adam_m, float*
                      const gb_job* jobs, int32_t n_jobs, int32_t max_windows, const float* x, const float* y,
                      const gb_lstm_fit_hparams* hp, void* workspace, float* out_loss, float* out_acc, int32_t loss,
                      void* stream);
+/* gb_lstm_fit_loss for batches of 1..256 windows, on the tensor cores: the same steps, order, losses, history and Adam state,
+ * with the GEMMs of a step (forward gates, backward input, weight gradients) on wgmma in split TF32 (hi*hi + hi*lo + lo*hi,
+ * fp32 accumulation) over 64-window batch tiles.  workspace: gb_lstm_fit_tc_workspace_bytes(net, n_jobs, batch_size) bytes
+ * (grows with the batch rounded up to 64, x lookback x the units; 0 for an invalid net or batch_size outside 1..256).
+ * batch_size > 256: GB_E_SHAPE, nothing enqueued. */
+size_t gb_lstm_fit_tc_workspace_bytes(const gb_lstmnet* net, int32_t n_jobs, int32_t batch_size);
+int gb_lstm_fit_tc(const gb_lstmnet* net, float* params, float* adam_m, float* adam_v, int32_t* adam_t,
+                   const gb_job* jobs, int32_t n_jobs, int32_t max_windows, const float* x, const float* y,
+                   const gb_lstm_fit_hparams* hp, void* workspace, float* out_loss, float* out_acc, int32_t loss,
+                   void* stream);
 
 /* Keras' Orthogonal initialiser for recurrent kernels: g holds n_mats standard-normal [rows][cols] draws (float64, rows <= cols,
  * overwritten); matrix i's rows are orthonormalised (Gram-Schmidt, the sign convention of Keras' QR) and written as float32 to
