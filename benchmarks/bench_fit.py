@@ -2,7 +2,7 @@
 BASELINE configs[2] (scaled): batched training of 64-tag feedforward_hourglass autoencoders, one persistent CTA per machine.
 Reports row-epochs/s, microseconds per optimizer step and the CPU oracle (NumPy Keras-style loop) on a small sample.
 
-    python benchmarks/bench_fit.py [--machines 296] [--rows 10000] [--epochs 3] [--batch 32] [--loss mse]
+    python benchmarks/bench_fit.py [--machines 296] [--rows 10000] [--epochs 3] [--batch 32] [--loss mse] [--optimizer Nadam]
 """
 import argparse, json, os, sys, time
 import numpy as np
@@ -18,6 +18,8 @@ def main():
     ap.add_argument("--tags", type=int, default=64)
     ap.add_argument("--cpu", type=int, default=1)
     ap.add_argument("--loss", default="mse", help="training loss (a canonical name: mse, mae, mape, msle, huber, log_cosh)")
+    ap.add_argument("--optimizer", default=None, help="a Keras optimizer name (RMSprop, Adagrad, Adadelta, Adamax, Nadam, AdamW, Adam) "
+                    "with its default hyperparameters; without it, Adam through the Adam kernels")
     a = ap.parse_args()
     import torch
     import __graft_entry__ as ge
@@ -25,6 +27,9 @@ def main():
     from gordo_components_b200 import engine, fleet
     from oracle import keras_math as km
 
+    from gordo_components_b200.machine.model.factories.specs import resolve_optimizer
+
+    opt = None if a.optimizer is None else resolve_optimizer(a.optimizer, {})
     spec = km.ff_hourglass_spec(a.tags)
     eng = engine.FFEngine(spec.dims, spec.acts, spec.l1)
     dev = eng.device
@@ -34,11 +39,11 @@ def main():
     params = fleet.random_glorot_params(eng, M, g)
     jobs = engine.jobs_to_device(engine.uniform_jobs(M, N), dev)
     p0 = params.clone()
-    eng.fit(p0, jobs, M, N, x, x, epochs=1, batch_size=B, loss=a.loss)  # warm-up
+    eng.fit(p0, jobs, M, N, x, x, epochs=1, batch_size=B, loss=a.loss, optimizer=opt)  # warm-up
     torch.cuda.synchronize()
     ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     ev0.record()
-    loss, acc, _ = eng.fit(params, jobs, M, N, x, x, epochs=E, batch_size=B, loss=a.loss)
+    loss, acc, _ = eng.fit(params, jobs, M, N, x, x, epochs=E, batch_size=B, loss=a.loss, optimizer=opt)
     ev1.record()
     torch.cuda.synchronize()
     ms = ev0.elapsed_time(ev1)
@@ -46,7 +51,8 @@ def main():
     sms = 132
     waves = (M + sms - 1) // sms
     out = {
-        "workload": f"{M} machines x {a.tags}-tag hourglass, {N} rows, {E} epochs, batch {B}, loss {a.loss}",
+        "workload": f"{M} machines x {a.tags}-tag hourglass, {N} rows, {E} epochs, batch {B}, loss {a.loss}"
+                    + (f", optimizer {a.optimizer}" if a.optimizer else ""),
         "ms": ms, "row_epochs_per_s": M * N * E / (ms * 1e-3), "us_per_step_per_cta": ms * 1e3 / (steps * waves),
         "steps_per_fit": steps, "waves": waves, "loss_first_last": [float(loss[:, 0].mean()), float(loss[:, -1].mean())],
         "algorithmic_tflops": M * N * E * 90708 / (ms * 1e-3) / 1e12,

@@ -26,6 +26,7 @@ def main():
     ap.add_argument("--cpu", type=int, default=1)
     ap.add_argument("--variant", default=None, help="auto, fp32, tc or a comma list of them, timed alternately")
     ap.add_argument("--rounds", type=int, default=1)
+    ap.add_argument("--optimizer", default=None, help="a Keras optimizer name with its default hyperparameters; without it, Adam")
     a = ap.parse_args()
     import torch
     import __graft_entry__ as ge
@@ -33,6 +34,9 @@ def main():
     from gordo_components_b200 import engine
     from oracle import keras_math as km
 
+    from gordo_components_b200.machine.model.factories.specs import resolve_optimizer
+
+    opt = None if a.optimizer is None else resolve_optimizer(a.optimizer, {})
     spec = km.lstm_symmetric_spec(a.tags, lookback_window=a.lookback)
     eng = engine.LSTMEngine(spec.n_features, spec.units, spec.acts, spec.n_features_out, spec.out_func, spec.lookback_window)
     dev = eng.device
@@ -44,15 +48,17 @@ def main():
     params = eng.pack_params([w0] * M)
     jobs = engine.jobs_to_device(engine.make_jobs(np.arange(M), nwin, np.arange(M, dtype=np.int64) * N), dev)
     workload = f"{M} machines x {a.tags}-tag lstm_symmetric(256,128,64), lookback {a.lookback}, {nwin} windows, batch {a.batch}, 1 epoch"
+    if opt is not None:
+        workload += f", optimizer {a.optimizer}"
     steps = 1 + (nwin + a.batch - 1) // a.batch
 
     def timed(fit):
         p = params.clone()
-        fit(p.clone(), jobs, M, min(nwin, a.batch), x, x, epochs=1, batch_size=a.batch, primer=False)  # warm-up: one step
+        fit(p.clone(), jobs, M, min(nwin, a.batch), x, x, epochs=1, batch_size=a.batch, primer=False, optimizer=opt)  # warm-up: one step
         torch.cuda.synchronize()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
-        loss, acc, _ = fit(p, jobs, M, nwin, x, x, epochs=1, batch_size=a.batch, primer=True)
+        loss, acc, _ = fit(p, jobs, M, nwin, x, x, epochs=1, batch_size=a.batch, primer=True, optimizer=opt)
         e1.record()
         torch.cuda.synchronize()
         return e0.elapsed_time(e1), loss

@@ -30,10 +30,39 @@ def loss_code(loss: str) -> int:
         raise ValueError(f"loss {loss!r} is not one the CUDA fit kernels implement {sorted(LOSS_CODES)}")
     return LOSS_CODES[loss]
 
+GB_OPT_ADAM, GB_OPT_ADAMW, GB_OPT_RMSPROP, GB_OPT_ADAGRAD, GB_OPT_ADADELTA, GB_OPT_ADAMAX, GB_OPT_NADAM = range(7)  # gb_opt
+GB_OPT_CENTERED = 1
+OPT_CODES = {"adam": GB_OPT_ADAM, "adamw": GB_OPT_ADAMW, "rmsprop": GB_OPT_RMSPROP, "adagrad": GB_OPT_ADAGRAD, "adadelta": GB_OPT_ADADELTA,
+             "adamax": GB_OPT_ADAMAX, "nadam": GB_OPT_NADAM}
+
+
+class GbOptimizer(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("flags", C.c_int32), ("lr", C.c_float), ("beta1", C.c_float), ("beta2", C.c_float),
+                ("eps", C.c_float), ("momentum", C.c_float), ("initial_accumulator", C.c_float), ("weight_decay", C.c_float),
+                ("clipvalue", C.c_float)]
+
+
+def make_optimizer(name: str, cfg) -> GbOptimizer:
+    """gb_optimizer of a canonical optimizer name and its complete record (``factories.specs.resolve_optimizer``)."""
+    if name not in OPT_CODES:
+        raise ValueError(f"optimizer {name!r} is not one the CUDA fit kernels implement {sorted(OPT_CODES)}")
+    o = GbOptimizer()
+    o.kind = OPT_CODES[name]
+    o.flags = GB_OPT_CENTERED if cfg.get("centered") else 0
+    o.lr, o.eps = float(cfg["lr"]), float(cfg["eps"])
+    o.beta1 = float(cfg.get("beta1", cfg.get("rho", 0.0)))
+    o.beta2 = float(cfg.get("beta2", 0.0))
+    o.momentum = float(cfg.get("momentum", 0.0))
+    o.initial_accumulator = float(cfg.get("initial_accumulator_value", 0.0))
+    o.weight_decay = float(cfg.get("weight_decay") or 0.0)
+    o.clipvalue = float(cfg.get("clipvalue") or 0.0)
+    return o
+
+
 EXPORTS = (
     "gb_abi_version", "gb_last_error", "gb_device_check", "gb_ffnet_param_count", "gb_ffnet_param_stride",
-    "gb_ffae_infer_score", "gb_ffae_tc_supported", "gb_ffae_infer_plan", "gb_anomaly_score", "gb_anomaly_score_f64", "gb_minmax_fit", "gb_minmax_f64", "gb_thresholds", "gb_thresholds_f64", "gb_cv_moments", "gb_smooth", "gb_quantile", "gb_affine_f64", "gb_gather_rows", "gb_minmax_inverse_f32", "gb_ffae_fit_state_stride", "gb_ffae_fit", "gb_ffae_fit_split", "gb_ffae_fit_stop", "gb_ffae_fit_plan",
-    "gb_lstm_param_count", "gb_lstm_param_stride", "gb_lstm_workspace_bytes", "gb_lstm_infer", "gb_lstm_tc_supported", "gb_lstm_tc_workspace_bytes", "gb_lstm_infer_tc", "gb_lstm_fit_workspace_bytes", "gb_lstm_fit", "gb_lstm_fit_loss", "gb_lstm_fit_tc_workspace_bytes", "gb_lstm_fit_tc",
+    "gb_ffae_infer_score", "gb_ffae_tc_supported", "gb_ffae_infer_plan", "gb_anomaly_score", "gb_anomaly_score_f64", "gb_minmax_fit", "gb_minmax_f64", "gb_thresholds", "gb_thresholds_f64", "gb_cv_moments", "gb_smooth", "gb_quantile", "gb_affine_f64", "gb_gather_rows", "gb_minmax_inverse_f32", "gb_ffae_fit_state_stride", "gb_ffae_fit", "gb_ffae_fit_split", "gb_ffae_fit_stop", "gb_ffae_fit_plan", "gb_ffae_fit_opt",
+    "gb_lstm_param_count", "gb_lstm_param_stride", "gb_lstm_workspace_bytes", "gb_lstm_infer", "gb_lstm_tc_supported", "gb_lstm_tc_workspace_bytes", "gb_lstm_infer_tc", "gb_lstm_fit_workspace_bytes", "gb_lstm_fit", "gb_lstm_fit_loss", "gb_lstm_fit_tc_workspace_bytes", "gb_lstm_fit_tc", "gb_lstm_fit_opt", "gb_lstm_fit_tc_opt",
     "gb_orthonormal_rows",
 )
 
@@ -159,6 +188,11 @@ def _declare(lib):
     lib.gb_lstm_fit_tc_workspace_bytes.argtypes = [C.POINTER(GbLstmNet), C.c_int32, C.c_int32]
     lib.gb_lstm_fit_tc.argtypes = lib.gb_lstm_fit_loss.argtypes
     lib.gb_lstm_fit_tc.restype = C.c_int
+    lib.gb_ffae_fit_opt.argtypes = lib.gb_ffae_fit_stop.argtypes[:-1] + [C.POINTER(GbOptimizer), _P]
+    lib.gb_ffae_fit_opt.restype = C.c_int
+    for name in ("gb_lstm_fit_opt", "gb_lstm_fit_tc_opt"):
+        getattr(lib, name).argtypes = lib.gb_lstm_fit_loss.argtypes[:-1] + [C.POINTER(GbOptimizer), _P]
+        getattr(lib, name).restype = C.c_int
     lib.gb_orthonormal_rows.argtypes = [_P, C.c_int32, C.c_int32, C.c_int32, _P, C.c_int64, C.c_int64, _P]
     lib.gb_orthonormal_rows.restype = C.c_int
     for name in ("gb_device_check", "gb_ffae_infer_score", "gb_ffae_tc_supported", "gb_ffae_infer_plan", "gb_anomaly_score", "gb_minmax_fit", "gb_thresholds", "gb_smooth", "gb_ffae_fit", "gb_ffae_fit_split", "gb_ffae_fit_stop", "gb_lstm_infer"):

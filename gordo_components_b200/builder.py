@@ -46,6 +46,7 @@ from sklearn.preprocessing import MinMaxScaler
 
 from . import __version__, serializer
 from .machine.model.base import GordoBase
+from .machine.model.factories.specs import fit_optimizer, optimizer_key
 from .machine.model.utils import metric_wrapper
 
 logger = logging.getLogger(__name__)
@@ -338,7 +339,7 @@ class _Canonical:
         s = self.spec
         return (tuple(s.dims), tuple(s.acts), tuple(float(v) for v in s.l1), tuple(sorted(s.adam.items())), tuple(s.metrics), s.loss,
                 len(self.X), self.fit["epochs"], self.fit["batch_size"], self.fit["shuffle"], self.n_splits, int(self.evaluation.get("seed", 0)),
-                self.split, self.early_stopping is not None, self.input_scaler)  # EarlyStopping's parameters are per-job records
+                self.split, self.early_stopping is not None, self.input_scaler) + optimizer_key(s)  # EarlyStopping's parameters are per-job records
 
 
 def _default_minmax(scaler) -> bool:
@@ -466,7 +467,7 @@ class _CanonicalLSTM(_Canonical):
     def bucket(self):
         s = self.spec
         return (s.key(), tuple(sorted(s.adam.items())), tuple(s.metrics), s.loss, self.lookahead, len(self.X), self.fit["epochs"], self.fit["batch_size"],
-                self.n_splits, int(self.evaluation.get("seed", 0)), self.input_scaler)
+                self.n_splits, int(self.evaluation.get("seed", 0)), self.input_scaler) + optimizer_key(s)
 
 
 def _is_lstm_definition(machine) -> bool:
@@ -725,7 +726,7 @@ class FleetModelBuilder:
                                seed=int(first.evaluation.get("seed", 0)), adam=first.spec.adam, shuffle=first.fit["shuffle"],
                                input_scaler=first.input_scaler, detector_shuffle=first.split[0], validation_split=first.split[1],
                                validation_batch_size=first.split[2],
-                               early_stopping=None if first.early_stopping is None else [c.early_stopping for c in members], loss=first.spec.loss)
+                               early_stopping=None if first.early_stopping is None else [c.early_stopping for c in members], loss=first.spec.loss, optimizer=fit_optimizer(first.spec))
         moments = fb.cv_moments.cpu().numpy()
         scale = fb.scale.cpu().numpy().astype(np.float64)
         engine._torch().cuda.synchronize()
@@ -764,7 +765,7 @@ class FleetModelBuilder:
         yd = xd if same_y else engine._torch().from_numpy(np.concatenate([np.ascontiguousarray(c.y.values, dtype=np.float64) for c in members])).to(eng.device)
         fb = fleet.build_lstm_fleet(eng, xd, yd, rows, lookahead=first.lookahead, epochs=first.fit["epochs"], batch_size=first.fit["batch_size"],
                                     n_splits=K, seed=int(first.evaluation.get("seed", 0)), adam=first.spec.adam, input_scaler=first.input_scaler,
-                                    loss=first.spec.loss)
+                                    loss=first.spec.loss, optimizer=fit_optimizer(first.spec))
         engine._torch().cuda.synchronize()
         share = (time.time() - t0) / len(members)  # the bucket's wall time, spread evenly: there is no per-machine time any more
         split_obj = TimeSeriesSplit(n_splits=K)
@@ -807,7 +808,7 @@ class FleetModelBuilder:
                                      validation_split=first.split[1], validation_batch_size=first.split[2],
                                      early_stopping=None if first.early_stopping is None else [c.early_stopping for c in members],
                                      window=det.window, smoothing_method=det.smoothing_method, threshold_percentile=det.threshold_percentile,
-                                     loss=first.spec.loss)
+                                     loss=first.spec.loss, optimizer=fit_optimizer(first.spec))
         torch.cuda.synchronize()
         share = (time.time() - t0) / len(members)  # the bucket's wall time, spread evenly: there is no per-machine time any more
         out = []

@@ -57,6 +57,8 @@ struct FitArgs {
   const gb_fit_stop* stop;  // per job: the EarlyStopping rule; NULL = none
   float* best_params;       // [n_slots][pstride]: the snapshots
   int32_t *out_epochs, *out_best_epoch;
+  // gb_ffae_fit_opt only (appended too): the optimizer of the OPT kernels
+  gb_optimizer opt;
 };
 
 __device__ __forceinline__ uint32_t mix32(uint32_t h) {
@@ -133,11 +135,15 @@ __device__ __forceinline__ void quarter_reduce(const float (&acc)[4][4], int lan
 // its cp.async prefetch and leaves, so its SM takes the next job of the launch.
 // LOSS (a fit whose hp.loss is not MSE): the output layer takes f / f' from gb::loss_value / gb::loss_grad.  Kept apart so that
 // the MSE fits keep the exact code of the kernels without it.
-template <bool WG, bool DG, bool SPLIT = false, bool STOP = false, bool LOSS = false>  // DG: some dz buffers live in global memory too (kept apart so that the usual case addresses them as shared memory)
+// OPT (an optimizer other than plain Adam, gb_ffae_fit_opt; instantiated with LOSS only): the weight and bias updates are
+// gb::opt_update on the two state slots (the Adam m / v loads and stores), with the per-step scalars gb::OptStep in place of
+// the Adam step size, computed one step ahead as that is.
+template <bool WG, bool DG, bool SPLIT = false, bool STOP = false, bool LOSS = false, bool OPT = false>  // DG: some dz buffers live in global memory too (kept apart so that the usual case addresses them as shared memory)
 __global__ void __launch_bounds__(THREADS, 1) ffae_fit_kernel(const FitArgs a) {
   extern __shared__ __align__(16) float smem[];
   __shared__ float s_red[3][NWARPS];
   __shared__ float s_alpha[2];  // Adam step size of optimizer step t at [t & 1]: written one step ahead, off the critical path
+  __shared__ std::conditional_t<OPT, gb::OptStep, float> s_opt[2];  // OPT: the same for the optimizer's per-step scalars
   __shared__ int s_idx[2][BR];
   __shared__ long long s_phase[2 * GB_MAX_LAYERS + 4];
 
@@ -249,7 +255,11 @@ __global__ void __launch_bounds__(THREADS, 1) ffae_fit_kernel(const FitArgs a) {
     const double t = (double)t_int;
     return (float)((double)a.hp.lr * sqrt(1.0 - pow((double)a.hp.beta2, t)) / (1.0 - pow((double)a.hp.beta1, t)));
   };
-  if (tid == 0) s_alpha[(t_step + 1) & 1] = adam_alpha(t_step + 1);
+  if constexpr (OPT) {
+    if (tid == 0) s_opt[(t_step + 1) & 1] = gb::opt_step_at(a.opt, t_step + 1);
+  } else {
+    if (tid == 0) s_alpha[(t_step + 1) & 1] = adam_alpha(t_step + 1);
+  }
   if (warp == NWARPS - 1) {
     int e1 = 0, s1 = 0, c1 = 0;
     stage_indices(0, 0, 0, 0);
@@ -347,7 +357,10 @@ __global__ void __launch_bounds__(THREADS, 1) ffae_fit_kernel(const FitArgs a) {
         }
         if (l == 0) {  // the last two warps have no tile in the first layer of a 64-tag hourglass (14 tiles): they prepare the next step
           if (warp == NWARPS - 1 && more2) stage_indices(cur, ne, ns, nc);  // read by the gather at the top of the next chunk
-          if (warp == NWARPS - 2 && first_chunk && !val && lane == 0) s_alpha[(t_step + 1) & 1] = adam_alpha(t_step + 1);  // read after the loss barrier of step t+1
+          if (warp == NWARPS - 2 && first_chunk && !val && lane == 0) {  // read after the loss barrier of step t+1
+            if constexpr (OPT) s_opt[(t_step + 1) & 1] = gb::opt_step_next(a.opt, s_opt[t_step & 1]);
+            else s_alpha[(t_step + 1) & 1] = adam_alpha(t_step + 1);
+          }
         }
         // A warp owns 32 rows x 4 output columns; lane = (row group p, K quarter kq): rows p, p+8, p+16, p+24 against every fourth
         // block of four k.  Per block a lane loads 4 + 4 float4 for 64 FMA (a row per lane with the whole K needs 1 + 4 for 16: the
@@ -441,7 +454,9 @@ __global__ void __launch_bounds__(THREADS, 1) ffae_fit_kernel(const FitArgs a) {
       }
       __syncthreads();
       stamp(L + 1);
-      const float alpha = s_alpha[t_step & 1];
+      const float alpha = OPT ? 0.f : s_alpha[t_step & 1];
+      gb::OptStep ost{};
+      if constexpr (OPT) ost = s_opt[t_step & 1];
 
       // ---- backward + Adam, pipelined over the layers ------------------------------------------------------
       // dz of layer l lives in D buffer (L-1-l) % 3.  Phase p (one barrier each) runs, on disjoint data,
@@ -548,8 +563,13 @@ __global__ void __launch_bounds__(THREADS, 1) ffae_fit_kernel(const FitArgs a) {
               float2 w = *reinterpret_cast<float2*>(Wl + off);
               float2 m = mq[i];
               float2 v = vq[i];
-              adam_update(w.x, gs[i].x, m.x, v.x, alpha, omb1, omb2, eps);
-              adam_update(w.y, gs[i].y, m.y, v.y, alpha, omb1, omb2, eps);
+              if constexpr (OPT) {  // m / v: the optimizer's state slots 0 / 1
+                gb::opt_update(a.opt, ost, w.x, gs[i].x, m.x, v.x);
+                gb::opt_update(a.opt, ost, w.y, gs[i].y, m.y, v.y);
+              } else {
+                adam_update(w.x, gs[i].x, m.x, v.x, alpha, omb1, omb2, eps);
+                adam_update(w.y, gs[i].y, m.y, v.y, alpha, omb1, omb2, eps);
+              }
               *reinterpret_cast<float2*>(Wl + off) = w;
               *reinterpret_cast<float2*>(Ml + off) = m;
               *reinterpret_cast<float2*>(Vl + off) = v;
@@ -565,7 +585,8 @@ __global__ void __launch_bounds__(THREADS, 1) ffae_fit_kernel(const FitArgs a) {
             if (!last_chunk) { Gacc[off] = g; continue; }
           }
           float w = sW[off], m = Mg[off], v = Vg[off];
-          adam_update(w, g, m, v, alpha, omb1, omb2, eps);
+          if constexpr (OPT) gb::opt_update(a.opt, ost, w, g, m, v);
+          else adam_update(w, g, m, v, alpha, omb1, omb2, eps);
           sW[off] = w; Mg[off] = m; Vg[off] = v;
         }
       };
@@ -694,8 +715,10 @@ int launch_fit(const gb_ffnet* net, float* params, float* adam_m, float* adam_v,
                int32_t n_jobs, int32_t max_rows, const float* x, const float* y, const int32_t* row_map, const int32_t* perm,
                const gb_fit_hparams* hp, int32_t val_batch, float* out_loss, float* out_acc, float* out_val_loss, float* out_val_acc,
                const gb_fit_stop* stop, float* best_params, int32_t* out_epochs, int32_t* out_best_epoch, FitEntry entry,
-               void* stream) {
+               const gb_optimizer* opt, void* stream) {
   int rc = gb::validate_ffnet(net);
+  if (rc != GB_OK) return rc;
+  rc = gb::validate_optimizer(opt);
   if (rc != GB_OK) return rc;
   GB_REQUIRE(params && adam_m && adam_v && jobs && x && y && hp && out_loss, GB_E_ARG,
              "params/adam_m/adam_v/jobs/x/y/hp/out_loss must be non-NULL");
@@ -715,6 +738,11 @@ int launch_fit(const gb_ffnet* net, float* params, float* adam_m, float* adam_v,
   rc = plan_fit(net, a, w_global, smem);
   if (rc != GB_OK) return rc;
   a.hp = *hp;
+  const bool use_opt = !gb::plain_adam(opt);
+  if (opt != nullptr && !use_opt) {  // plain Adam runs the Adam kernels, from the optimizer's hyperparameters
+    a.hp.lr = opt->lr; a.hp.beta1 = opt->beta1; a.hp.beta2 = opt->beta2; a.hp.eps = opt->eps;
+  }
+  if (use_opt) a.opt = *opt;
   const int L = net->n_layers;
   a.max_rows = max_rows;
   a.pstride = (long)gb_ffnet_param_stride(net);
@@ -735,23 +763,25 @@ int launch_fit(const gb_ffnet* net, float* params, float* adam_m, float* adam_v,
     kernel<<<n_jobs, THREADS, smem, (cudaStream_t)stream>>>(a);
     return GB_OK;
   };
-  auto dispatch = [&](auto any_loss) -> int {
-    constexpr bool LS = decltype(any_loss)::value;
+  auto dispatch = [&](auto any_loss, auto any_opt) -> int {
+    constexpr bool LS = decltype(any_loss)::value, OP = decltype(any_opt)::value;
     if (entry == FIT_STOP) {
-      if (a.d_global > 0) return launch(ffae_fit_kernel<true, true, true, true, LS>);
-      if (w_global) return launch(ffae_fit_kernel<true, false, true, true, LS>);
-      return launch(ffae_fit_kernel<false, false, true, true, LS>);
+      if (a.d_global > 0) return launch(ffae_fit_kernel<true, true, true, true, LS, OP>);
+      if (w_global) return launch(ffae_fit_kernel<true, false, true, true, LS, OP>);
+      return launch(ffae_fit_kernel<false, false, true, true, LS, OP>);
     }
     if (entry == FIT_SPLIT) {
-      if (a.d_global > 0) return launch(ffae_fit_kernel<true, true, true, false, LS>);
-      if (w_global) return launch(ffae_fit_kernel<true, false, true, false, LS>);
-      return launch(ffae_fit_kernel<false, false, true, false, LS>);
+      if (a.d_global > 0) return launch(ffae_fit_kernel<true, true, true, false, LS, OP>);
+      if (w_global) return launch(ffae_fit_kernel<true, false, true, false, LS, OP>);
+      return launch(ffae_fit_kernel<false, false, true, false, LS, OP>);
     }
-    if (a.d_global > 0) return launch(ffae_fit_kernel<true, true, false, false, LS>);
-    if (w_global) return launch(ffae_fit_kernel<true, false, false, false, LS>);
-    return launch(ffae_fit_kernel<false, false, false, false, LS>);
+    if (a.d_global > 0) return launch(ffae_fit_kernel<true, true, false, false, LS, OP>);
+    if (w_global) return launch(ffae_fit_kernel<true, false, false, false, LS, OP>);
+    return launch(ffae_fit_kernel<false, false, false, false, LS, OP>);
   };
-  rc = hp->loss == GB_LOSS_MSE ? dispatch(std::false_type{}) : dispatch(std::true_type{});
+  // another optimizer than plain Adam takes the LOSS kernels (their loss switch covers MSE), so it adds 9 instantiations, not 18
+  if (use_opt) rc = dispatch(std::true_type{}, std::true_type{});
+  else rc = hp->loss == GB_LOSS_MSE ? dispatch(std::false_type{}, std::false_type{}) : dispatch(std::true_type{}, std::false_type{});
   if (rc != GB_OK) return rc;
   GB_CUDA_CHECK(cudaGetLastError());
   return GB_OK;
@@ -789,7 +819,7 @@ int gb_ffae_fit(const gb_ffnet* net, float* params, float* adam_m, float* adam_v
                 int32_t max_rows, const float* x, const float* y, const int32_t* perm, const gb_fit_hparams* hp,
                 float* out_loss, float* out_acc, void* stream) {
   return launch_fit(net, params, adam_m, adam_v, jobs, nullptr, n_jobs, max_rows, x, y, nullptr, perm, hp, 1, out_loss, out_acc,
-                    nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, FIT_PLAIN, stream);
+                    nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, FIT_PLAIN, nullptr, stream);
 }
 
 int gb_ffae_fit_split(const gb_ffnet* net, float* params, float* adam_m, float* adam_v, const gb_job* jobs,
@@ -799,7 +829,7 @@ int gb_ffae_fit_split(const gb_ffnet* net, float* params, float* adam_m, float* 
   GB_REQUIRE(!split || out_val_loss, GB_E_ARG, "split needs out_val_loss");
   GB_REQUIRE(!split || val_batch >= 1, GB_E_ARG, "val_batch=%d must be >= 1", val_batch);
   return launch_fit(net, params, adam_m, adam_v, jobs, split, n_jobs, max_rows, x, y, row_map, perm, hp, split ? val_batch : 1,
-                    out_loss, out_acc, out_val_loss, out_val_acc, nullptr, nullptr, nullptr, nullptr, FIT_SPLIT, stream);
+                    out_loss, out_acc, out_val_loss, out_val_acc, nullptr, nullptr, nullptr, nullptr, FIT_SPLIT, nullptr, stream);
 }
 
 int gb_ffae_fit_stop(const gb_ffnet* net, float* params, float* adam_m, float* adam_v, const gb_job* jobs,
@@ -813,7 +843,22 @@ int gb_ffae_fit_stop(const gb_ffnet* net, float* params, float* adam_m, float* a
              "stop needs best_params, out_epochs and out_best_epoch");
   GB_REQUIRE(!stop || gb::aligned16(best_params), GB_E_ARG, "best_params must be 16-byte aligned");
   return launch_fit(net, params, adam_m, adam_v, jobs, split, n_jobs, max_rows, x, y, row_map, perm, hp, split ? val_batch : 1,
-                    out_loss, out_acc, out_val_loss, out_val_acc, stop, best_params, out_epochs, out_best_epoch, FIT_STOP, stream);
+                    out_loss, out_acc, out_val_loss, out_val_acc, stop, best_params, out_epochs, out_best_epoch, FIT_STOP, nullptr, stream);
+}
+
+int gb_ffae_fit_opt(const gb_ffnet* net, float* params, float* adam_m, float* adam_v, const gb_job* jobs,
+                    const gb_fit_split* split, int32_t n_jobs, int32_t max_rows, const float* x, const float* y,
+                    const int32_t* row_map, const int32_t* perm, const gb_fit_hparams* hp, int32_t val_batch,
+                    float* out_loss, float* out_acc, float* out_val_loss, float* out_val_acc, const gb_fit_stop* stop,
+                    float* best_params, int32_t* out_epochs, int32_t* out_best_epoch, const gb_optimizer* opt, void* stream) {
+  GB_REQUIRE(!split || out_val_loss, GB_E_ARG, "split needs out_val_loss");
+  GB_REQUIRE(!split || val_batch >= 1, GB_E_ARG, "val_batch=%d must be >= 1", val_batch);
+  GB_REQUIRE(!stop || (best_params && out_epochs && out_best_epoch), GB_E_ARG,
+             "stop needs best_params, out_epochs and out_best_epoch");
+  GB_REQUIRE(!stop || gb::aligned16(best_params), GB_E_ARG, "best_params must be 16-byte aligned");
+  const FitEntry entry = stop ? FIT_STOP : split ? FIT_SPLIT : FIT_PLAIN;
+  return launch_fit(net, params, adam_m, adam_v, jobs, split, n_jobs, max_rows, x, y, row_map, perm, hp, split ? val_batch : 1,
+                    out_loss, out_acc, out_val_loss, out_val_acc, stop, best_params, out_epochs, out_best_epoch, entry, opt, stream);
 }
 
 }  // extern "C"

@@ -103,4 +103,141 @@ __device__ __forceinline__ float loss_grad(int loss, float yh, float t) {
   }
 }
 
+// ---- optimizers (include/gordo_b200.h gb_optimizer; keras 3.3.3 keras/src/optimizers/*.py [3P], restated, not verified against TF)
+// The fit kernels keep their own Adam for a NULL optimizer and for one that is plain Adam (no weight decay, no clipping), so
+// those fits stay bit-identical; every other optimizer goes through opt_update.
+inline int validate_optimizer(const gb_optimizer* o) {
+  if (o == nullptr) return GB_OK;
+  auto nonneg = [](float v) { return v >= 0.f && v < 3.0e38f; };  // false for NaN and inf
+  auto unit = [](float v) { return v >= 0.f && v < 1.f; };
+  GB_REQUIRE(o->kind >= GB_OPT_ADAM && o->kind <= GB_OPT_NADAM, GB_E_ARG, "optimizer kind=%d unknown (gb_opt: 0..6)", o->kind);
+  GB_REQUIRE((o->flags & ~GB_OPT_CENTERED) == 0, GB_E_ARG, "optimizer flags=%d unknown", o->flags);
+  GB_REQUIRE(!(o->flags & GB_OPT_CENTERED) || o->kind == GB_OPT_RMSPROP, GB_E_ARG, "optimizer flag GB_OPT_CENTERED is RMSprop's");
+  GB_REQUIRE(!(o->flags & GB_OPT_CENTERED) || o->momentum == 0.f, GB_E_ARG,
+             "optimizer: centered RMSprop with momentum needs a third state slot, which the fit kernels do not have");
+  GB_REQUIRE(nonneg(o->lr) && nonneg(o->eps) && nonneg(o->momentum) && nonneg(o->initial_accumulator) && nonneg(o->weight_decay) &&
+                 nonneg(o->clipvalue),
+             GB_E_ARG, "optimizer lr/eps/momentum/initial_accumulator/weight_decay/clipvalue must be finite and >= 0");
+  const bool two_betas = o->kind == GB_OPT_ADAM || o->kind == GB_OPT_ADAMW || o->kind == GB_OPT_ADAMAX || o->kind == GB_OPT_NADAM;
+  GB_REQUIRE(o->kind == GB_OPT_ADAGRAD || unit(o->beta1), GB_E_ARG, "optimizer beta1/rho=%g outside [0, 1)", (double)o->beta1);
+  GB_REQUIRE(!two_betas || unit(o->beta2), GB_E_ARG, "optimizer beta2=%g outside [0, 1)", (double)o->beta2);
+  return GB_OK;
+}
+// Adam(W) without weight decay or clipping: the kernels' own Adam runs it, from the optimizer's lr / beta1 / beta2 / eps
+inline bool plain_adam(const gb_optimizer* o) {
+  return o == nullptr || ((o->kind == GB_OPT_ADAM || o->kind == GB_OPT_ADAMW) && o->weight_decay == 0.f && o->clipvalue == 0.f);
+}
+
+// Per-step scalars of optimizer step t, computed once per step off the per-parameter path.  nadam_p / nadam_pi carry Nadam's
+// 0.96^t and the float32 product P_t, so that step t+1 follows from step t (opt_step_next) exactly as opt_step_at recomputes it
+// from step 1: a fit split over several launches takes the same steps as one launch.
+struct OptStep {
+  float c0, c1, c2;  // ADAM(W): alpha_t = lr sqrt(1 - b2^t) / (1 - b1^t); ADAMAX: 1 / (1 - b1^t);
+                     // NADAM: u_(t+1) / (1 - P_t u_(t+1)), (1 - u_t) / (1 - P_t), 1 / (1 - b2^t)
+  int first;         // t == 1 (ADAGRAD reads initial_accumulator in place of its stored state)
+  int t;
+  float nadam_pi;
+  double nadam_p;
+};
+
+__device__ __forceinline__ float nadam_u(float beta1, double p96) { return (float)((double)beta1 * (1.0 - 0.5 * p96)); }
+
+__device__ __forceinline__ void opt_scalars(const gb_optimizer& o, OptStep& s) {
+  const double t = (double)s.t;
+  s.first = s.t == 1;
+  switch (o.kind) {
+    case GB_OPT_ADAMAX: s.c0 = (float)(1.0 / (1.0 - pow((double)o.beta1, t))); break;
+    case GB_OPT_NADAM: {
+      const float ut = nadam_u(o.beta1, s.nadam_p), ut1 = nadam_u(o.beta1, s.nadam_p * 0.96);
+      s.c0 = ut1 / (1.f - s.nadam_pi * ut1);
+      s.c1 = (1.f - ut) / (1.f - s.nadam_pi);
+      s.c2 = (float)(1.0 / (1.0 - pow((double)o.beta2, t)));
+      break;
+    }
+    default:
+      s.c0 = (float)((double)o.lr * sqrt(1.0 - pow((double)o.beta2, t)) / (1.0 - pow((double)o.beta1, t)));
+  }
+}
+// step prev.t + 1 from step prev.t
+__device__ __forceinline__ OptStep opt_step_next(const gb_optimizer& o, const OptStep& prev) {
+  OptStep s = prev;
+  s.t = prev.t + 1;
+  if (o.kind == GB_OPT_NADAM) {
+    s.nadam_p = prev.nadam_p * 0.96;
+    s.nadam_pi = prev.nadam_pi * nadam_u(o.beta1, s.nadam_p);
+  }
+  opt_scalars(o, s);
+  return s;
+}
+// step t >= 1 from scratch: Nadam's product is taken from step 1, every other rule's scalars come from t alone
+__device__ __forceinline__ OptStep opt_step_at(const gb_optimizer& o, int t) {
+  OptStep s{};
+  s.t = t - 1;
+  s.nadam_pi = 1.f;  // P_0
+  s.nadam_p = 1.0;   // 0.96^0
+  if (o.kind == GB_OPT_NADAM)
+    for (int k = 1; k < t; ++k) {
+      s.nadam_p *= 0.96;
+      s.nadam_pi *= nadam_u(o.beta1, s.nadam_p);
+    }
+  return opt_step_next(o, s);
+}
+
+// One parameter's update: w, its gradient g (summed over the mini-batch) and its two state slots.  Padded weight lanes (w = 0,
+// g = 0) stay exactly zero under every rule.  The kind switch is uniform over a launch.
+__device__ __forceinline__ void opt_update(const gb_optimizer& o, const OptStep& s, float& w, float g, float& s0, float& s1) {
+  if (o.clipvalue > 0.f) g = fminf(fmaxf(g, -o.clipvalue), o.clipvalue);
+  if (o.weight_decay != 0.f) w = __fsub_rn(w, __fmul_rn(__fmul_rn(w, o.weight_decay), o.lr));  // keras: w - w * wd * lr
+  switch (o.kind) {
+    case GB_OPT_RMSPROP: {
+      s0 = o.beta1 * s0 + (1.f - o.beta1) * (g * g);
+      float d;
+      if (o.flags & GB_OPT_CENTERED) {
+        s1 = o.beta1 * s1 + (1.f - o.beta1) * g;
+        d = s0 - s1 * s1 + o.eps;
+      } else {
+        d = s0 + o.eps;
+      }
+      const float inc = o.lr * g / sqrtf(d);
+      if (o.momentum > 0.f) {
+        s1 = o.momentum * s1 + inc;
+        w -= s1;
+      } else {
+        w -= inc;
+      }
+      break;
+    }
+    case GB_OPT_ADAGRAD: {
+      s0 = (s.first ? o.initial_accumulator : s0) + g * g;
+      w -= o.lr * g / sqrtf(s0 + o.eps);
+      break;
+    }
+    case GB_OPT_ADADELTA: {
+      s0 = o.beta1 * s0 + (1.f - o.beta1) * (g * g);
+      const float dv = -(sqrtf(s1 + o.eps) * g / sqrtf(s0 + o.eps));
+      s1 = o.beta1 * s1 + (1.f - o.beta1) * (dv * dv);
+      w += o.lr * dv;
+      break;
+    }
+    case GB_OPT_ADAMAX: {
+      s0 += (g - s0) * (1.f - o.beta1);
+      s1 = fmaxf(o.beta2 * s1, fabsf(g));
+      w -= o.lr * s0 * s.c0 / (s1 + o.eps);
+      break;
+    }
+    case GB_OPT_NADAM: {
+      s0 += (g - s0) * (1.f - o.beta1);
+      s1 += (g * g - s1) * (1.f - o.beta2);
+      const float mhat = s.c0 * s0 + s.c1 * g;
+      w -= mhat * o.lr / (sqrtf(s1 * s.c2) + o.eps);
+      break;
+    }
+    default: {  // ADAM, ADAMW
+      s0 += (g - s0) * (1.f - o.beta1);
+      s1 += (g * g - s1) * (1.f - o.beta2);
+      w -= s0 * s.c0 / (sqrtf(s1) + o.eps);
+    }
+  }
+}
+
 }  // namespace gb

@@ -61,6 +61,7 @@ struct FitArgs {
   const int* step;            // device: {first window, batch size} of the optimizer step being replayed
   float lr, b1, b2, eps;
   int loss;
+  gb_optimizer opt;  // another optimizer than plain Adam (tc_opt_kernel)
 };
 
 __device__ __forceinline__ float sigm(float z) { return 1.f / (1.f + expf(-z)); }
@@ -462,6 +463,27 @@ __global__ void __launch_bounds__(256) tc_adam_kernel(const FitArgs a, long n_pa
     P[i] -= alpha * m / (sqrtf(v) + a.eps);
   }
 }
+// Every other optimizer than plain Adam (gb::opt_update; state slots 0 / 1 = adam_m / adam_v), captured in place of tc_adam_kernel.
+// The per-step scalars come from the slot's step count, once per CTA (for Nadam a product over the slot's steps, a few cycles each).
+__global__ void __launch_bounds__(256) tc_opt_kernel(const FitArgs a, long n_params) {
+  const gb_job job = a.jobs[blockIdx.y];
+  if (job_batch(job, a.step[0], a.step[1]) == 0) return;
+  __shared__ gb::OptStep s_st;
+  if (threadIdx.x == 0) s_st = gb::opt_step_at(a.opt, a.adam_t[job.slot] + 1);
+  __syncthreads();
+  const gb::OptStep st = s_st;
+  const float* G = a.ws + (long)blockIdx.y * a.ws_stride + a.gofs;
+  float* P = a.params + (long)job.slot * a.pstride;
+  float* S0 = a.adam_m + (long)job.slot * a.pstride;
+  float* S1 = a.adam_v + (long)job.slot * a.pstride;
+  for (long i = (long)blockIdx.x * 256 + threadIdx.x; i < n_params; i += (long)gridDim.x * 256) {
+    float w = P[i], s0 = S0[i], s1 = S1[i];
+    gb::opt_update(a.opt, st, w, G[i], s0, s1);
+    P[i] = w;
+    S0[i] = s0;
+    S1[i] = s1;
+  }
+}
 __global__ void tc_bump_kernel(const FitArgs a, int n_jobs) {
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
   if (j < n_jobs && job_batch(a.jobs[j], a.step[0], a.step[1]) > 0) a.adam_t[a.jobs[j].slot] += 1;
@@ -537,8 +559,16 @@ size_t gb_lstm_fit_tc_workspace_bytes(const gb_lstmnet* net, int32_t n_jobs, int
 int gb_lstm_fit_tc(const gb_lstmnet* net, float* params, float* adam_m, float* adam_v, int32_t* adam_t, const gb_job* jobs,
                    int32_t n_jobs, int32_t max_windows, const float* x, const float* y, const gb_lstm_fit_hparams* hp, void* workspace,
                    float* out_loss, float* out_acc, int32_t loss, void* stream) {
+  return gb_lstm_fit_tc_opt(net, params, adam_m, adam_v, adam_t, jobs, n_jobs, max_windows, x, y, hp, workspace, out_loss, out_acc, loss,
+                            nullptr, stream);
+}
+
+int gb_lstm_fit_tc_opt(const gb_lstmnet* net, float* params, float* adam_m, float* adam_v, int32_t* adam_t, const gb_job* jobs,
+                       int32_t n_jobs, int32_t max_windows, const float* x, const float* y, const gb_lstm_fit_hparams* hp, void* workspace,
+                       float* out_loss, float* out_acc, int32_t loss, const gb_optimizer* opt, void* stream) {
   int rc = validate(net);
   if (rc != GB_OK) return rc;
+  if ((rc = gb::validate_optimizer(opt)) != GB_OK) return rc;
   GB_REQUIRE(loss >= GB_LOSS_MSE && loss <= GB_LOSS_LOG_COSH, GB_E_ARG, "loss=%d unknown (gb_loss: 0..5)", loss);
   GB_REQUIRE(params && adam_m && adam_v && adam_t && jobs && x && y && hp && workspace && out_loss && out_acc, GB_E_ARG, "NULL argument");
   GB_REQUIRE(n_jobs >= 0 && n_jobs <= 65535 && max_windows >= 0, GB_E_ARG, "bad n_jobs/max_windows");
@@ -558,6 +588,9 @@ int gb_lstm_fit_tc(const gb_lstmnet* net, float* params, float* adam_m, float* a
   a.loss_sum = a.ws + a.ws_stride * n_jobs;
   a.hit_sum = a.loss_sum + n_jobs;
   a.lr = hp->lr; a.b1 = hp->beta1; a.b2 = hp->beta2; a.eps = hp->eps;
+  const bool use_opt = !gb::plain_adam(opt);
+  if (opt != nullptr && !use_opt) { a.lr = opt->lr; a.b1 = opt->beta1; a.b2 = opt->beta2; a.eps = opt->eps; }  // plain Adam: the Adam kernel
+  if (use_opt) a.opt = *opt;
   a.loss = loss;
   const long n_params = (long)gb_lstm_param_count(net);
   const int u_top = net->units[net->n_layers - 1], T = net->n_features_out;
@@ -598,7 +631,10 @@ int gb_lstm_fit_tc(const gb_lstmnet* net, float* params, float* adam_m, float* a
       const Lay& ly = a.lay[l];
       tc_wgrad_kernel<<<dim3((4 * ly.u + TN - 1) / TN, (ly.in + ly.u + 1 + TM - 1) / TM, n_jobs), 128, 0, st>>>(a, l);
     }
-    tc_adam_kernel<<<dim3((unsigned)((n_params + 256 * 8 - 1) / (256 * 8)), n_jobs), 256, 0, st>>>(a, n_params);
+    if (use_opt)
+      tc_opt_kernel<<<dim3((unsigned)((n_params + 256 * 8 - 1) / (256 * 8)), n_jobs), 256, 0, st>>>(a, n_params);
+    else
+      tc_adam_kernel<<<dim3((unsigned)((n_params + 256 * 8 - 1) / (256 * 8)), n_jobs), 256, 0, st>>>(a, n_params);
     tc_bump_kernel<<<jb, 128, 0, st>>>(a, n_jobs);
   }
   {

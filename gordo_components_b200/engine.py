@@ -160,11 +160,12 @@ class FFEngine:
     # ------------------------------------------------------------------ K2
     def fit(self, params, jobs_dev, n_jobs: int, max_rows: int, x, y, epochs: int = 1, batch_size: int = 32, shuffle=True,
             perm=None, adam: Optional[Dict[str, float]] = None, seed: int = 0, l1_div_batch: bool = False, state=None,
-            step0: int = 0, loss: str = "mse"):
+            step0: int = 0, loss: str = "mse", optimizer=None):
         """
         Trains every job's slot in place (``params`` is updated).  Returns (loss [n_jobs, epochs], accuracy, (m, v)).
         ``perm`` (int32 [n_jobs, epochs, max_rows]) pins the visiting order (parity tests).  ``loss``: canonical Keras loss name
-        (``_cabi.LOSS_CODES``) the fit minimises and reports.
+        (``_cabi.LOSS_CODES``) the fit minimises and reports.  ``optimizer``: None (Adam from ``adam``) or the (name, record) pair of
+        ``factories.specs.resolve_optimizer`` (gb_ffae_fit_opt); (m, v) are then its state slots 0 and 1.
         """
         torch = _torch()
         hp = _fit_hparams(epochs, batch_size, shuffle, perm, adam, seed, l1_div_batch, step0, loss)
@@ -172,13 +173,19 @@ class FFEngine:
         hist = torch.empty((n_jobs, epochs), dtype=torch.float32, device=self.device)
         acc = torch.empty((n_jobs, epochs), dtype=torch.float32, device=self.device)
         p = _cabi.ptr
+        if optimizer is not None:
+            opt = _cabi.make_optimizer(*optimizer)
+            _cabi.check(self.lib.gb_ffae_fit_opt(C.byref(self.net), p(params), p(m), p(v), p(jobs_dev), None, int(n_jobs), int(max_rows), p(x),
+                                                 p(y), None, p(perm), C.byref(hp), 1, p(hist), p(acc), None, None, None, None, None, None,
+                                                 C.byref(opt), _stream_ptr()))
+            return hist, acc, (m, v)
         _cabi.check(self.lib.gb_ffae_fit(C.byref(self.net), p(params), p(m), p(v), p(jobs_dev), int(n_jobs), int(max_rows), p(x), p(y),
                                          p(perm), C.byref(hp), p(hist), p(acc), _stream_ptr()))
         return hist, acc, (m, v)
 
     def fit_split(self, params, jobs_dev, n_jobs: int, max_rows: int, x, y, split=None, row_map=None, val_batch: Optional[int] = None,
                   epochs: int = 1, batch_size: int = 32, shuffle=True, perm=None, adam: Optional[Dict[str, float]] = None, seed: int = 0,
-                  l1_div_batch: bool = False, state=None, step0: int = 0, stop=None, loss: str = "mse"):
+                  l1_div_batch: bool = False, state=None, step0: int = 0, stop=None, loss: str = "mse", optimizer=None):
         """
         ``fit`` over row *positions* with Keras' ``validation_split``, in one launch (gb_ffae_fit_split).  Job i trains on its
         positions [0, n_rows) exactly as ``fit`` trains on its rows, and after every epoch runs the network forward over the held-out
@@ -196,7 +203,7 @@ class FFEngine:
         epochs_run, best_epoch, (m, v)): epochs_run / best_epoch are int32 [n_jobs] (best_epoch -1 when no epoch improved and no
         snapshot was taken), and every history entry past a job's epochs_run is NaN.
 
-        ``loss``: as in ``fit``; the held-out statistics report the same loss.
+        ``loss``, ``optimizer``: as in ``fit``; the held-out statistics report the same loss.
         """
         torch = _torch()
         hp = _fit_hparams(epochs, batch_size, shuffle, perm, adam, seed, l1_div_batch, step0, loss)
@@ -208,6 +215,12 @@ class FFEngine:
         out += [torch.full((n_jobs, epochs), float("nan"), dtype=torch.float32, device=self.device) for _ in range(2)]
         vb = int(val_batch if val_batch is not None else batch_size)
         p = _cabi.ptr
+        opt = None if optimizer is None else _cabi.make_optimizer(*optimizer)
+        if stop is None and opt is not None:
+            _cabi.check(self.lib.gb_ffae_fit_opt(C.byref(self.net), p(params), p(m), p(v), p(jobs_dev), p(split), int(n_jobs), int(max_rows),
+                                                 p(x), p(y), p(row_map), p(perm), C.byref(hp), vb, *(p(t) for t in out), None, None, None, None,
+                                                 C.byref(opt), _stream_ptr()))
+            return (*out, (m, v))
         if stop is None:
             _cabi.check(self.lib.gb_ffae_fit_split(C.byref(self.net), p(params), p(m), p(v), p(jobs_dev), p(split), int(n_jobs), int(max_rows),
                                                    p(x), p(y), p(row_map), p(perm), C.byref(hp), vb, *(p(t) for t in out), _stream_ptr()))
@@ -217,13 +230,18 @@ class FFEngine:
         best = torch.empty_like(params)  # snapshot area
         epochs_run = torch.zeros((n_jobs,), dtype=torch.int32, device=self.device)
         best_epoch = torch.full((n_jobs,), -1, dtype=torch.int32, device=self.device)
+        if opt is not None:
+            _cabi.check(self.lib.gb_ffae_fit_opt(C.byref(self.net), p(params), p(m), p(v), p(jobs_dev), p(split), int(n_jobs), int(max_rows),
+                                                 p(x), p(y), p(row_map), p(perm), C.byref(hp), vb, *(p(t) for t in out), p(stop), p(best),
+                                                 p(epochs_run), p(best_epoch), C.byref(opt), _stream_ptr()))
+            return (*out, epochs_run, best_epoch, (m, v))
         _cabi.check(self.lib.gb_ffae_fit_stop(C.byref(self.net), p(params), p(m), p(v), p(jobs_dev), p(split), int(n_jobs), int(max_rows),
                                               p(x), p(y), p(row_map), p(perm), C.byref(hp), vb, *(p(t) for t in out), p(stop), p(best),
                                               p(epochs_run), p(best_epoch), _stream_ptr()))
         return (*out, epochs_run, best_epoch, (m, v))
 
     def _fit_state(self, params, state):
-        """Adam (m, v) of every slot: the given pair, or zeros for a fresh fit."""
+        """Optimizer state slots (m, v) of every slot: the given pair, or zeros for a fresh fit."""
         if state is not None:
             return state
         torch = _torch()
@@ -583,18 +601,20 @@ class LSTMEngine:
         return self.fit_tc_workspace_bytes(n_jobs, batch_size)
 
     def fit(self, params, jobs_dev, n_jobs, max_windows, x, y, epochs: int = 1, batch_size: int = 32, lookahead: int = 0,
-            primer: bool = True, adam: Optional[Dict[str, float]] = None, state=None, loss: str = "mse"):
+            primer: bool = True, adam: Optional[Dict[str, float]] = None, state=None, loss: str = "mse", optimizer=None):
         """
         Trains every job's slot in place by back-propagation through time (``jobs`` count windows; target of window j is
         y[x_row + j + lookback - 1 + lookahead]).  Returns (loss [n_jobs, epochs], accuracy, (m, v, t)).  ``loss``: canonical
-        Keras loss name (``_cabi.LOSS_CODES``), for the primer step too (gb_lstm_fit_loss).
+        Keras loss name (``_cabi.LOSS_CODES``), for the primer step too (gb_lstm_fit_loss).  ``optimizer``: None (Adam from
+        ``adam``) or the (name, record) pair of ``factories.specs.resolve_optimizer`` (gb_lstm_fit_opt); m and v are its state slots.
         """
         ws_bytes = int(self.lib.gb_lstm_fit_workspace_bytes(C.byref(self.net), int(n_jobs)))
-        return self._fit_launch(self.lib.gb_lstm_fit_loss, ws_bytes, params, jobs_dev, n_jobs, max_windows, x, y, epochs, batch_size,
-                                lookahead, primer, adam, state, loss)
+        entry = self.lib.gb_lstm_fit_loss if optimizer is None else self.lib.gb_lstm_fit_opt
+        return self._fit_launch(entry, ws_bytes, params, jobs_dev, n_jobs, max_windows, x, y, epochs, batch_size,
+                                lookahead, primer, adam, state, loss, optimizer)
 
     def fit_tc(self, params, jobs_dev, n_jobs, max_windows, x, y, epochs: int = 1, batch_size: int = 32, lookahead: int = 0,
-               primer: bool = True, adam: Optional[Dict[str, float]] = None, state=None, loss: str = "mse"):
+               primer: bool = True, adam: Optional[Dict[str, float]] = None, state=None, loss: str = "mse", optimizer=None):
         """
         ``fit`` on the tensor-core family (gb_lstm_fit_tc): the same training for batches of 1 .. TC_MAX_BATCH windows, the
         GEMMs of each step on wgmma in split TF32.  Same arguments, return value and (m, v, t) state, which may be carried
@@ -603,12 +623,14 @@ class LSTMEngine:
         if not 1 <= int(batch_size) <= self.TC_MAX_BATCH:
             raise ValueError(f"batch_size={int(batch_size)}: the LSTM fit handles batches of 1 to {self.TC_MAX_BATCH} windows")
         ws_bytes = self.fit_tc_workspace_bytes(n_jobs, batch_size)
-        return self._fit_launch(self.lib.gb_lstm_fit_tc, ws_bytes, params, jobs_dev, n_jobs, max_windows, x, y, epochs, batch_size,
-                                lookahead, primer, adam, state, loss)
+        entry = self.lib.gb_lstm_fit_tc if optimizer is None else self.lib.gb_lstm_fit_tc_opt
+        return self._fit_launch(entry, ws_bytes, params, jobs_dev, n_jobs, max_windows, x, y, epochs, batch_size,
+                                lookahead, primer, adam, state, loss, optimizer)
 
     def _fit_launch(self, entry, ws_bytes, params, jobs_dev, n_jobs, max_windows, x, y, epochs, batch_size, lookahead, primer, adam, state,
-                    loss):
+                    loss, optimizer=None):
         code = _cabi.loss_code(loss)
+        opt = () if optimizer is None else (C.byref(_cabi.make_optimizer(*optimizer)),)
         torch = _torch()
         adam = adam or {}
         hp = _cabi.GbLstmFitHParams()
@@ -628,7 +650,7 @@ class LSTMEngine:
         acc = torch.zeros((n_jobs, max(epochs, 1)), dtype=torch.float32, device=self.device)
         p = _cabi.ptr
         _cabi.check(entry(C.byref(self.net), p(params), p(m), p(v), p(t), p(jobs_dev), int(n_jobs), int(max_windows), p(x), p(y), C.byref(hp),
-                          p(ws), p(hist), p(acc), code, _stream_ptr()))
+                          p(ws), p(hist), p(acc), code, *opt, _stream_ptr()))
         return hist[:, :epochs], acc[:, :epochs], (m, v, t)
 
     @property

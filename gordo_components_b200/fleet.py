@@ -303,7 +303,7 @@ def _keras_initial_params(eng: "engine.FFEngine", n_slots: int, generator):
 
 
 def _fit_slots(eng, params, fit_jobs, n_jobs, max_rows, x, y, split, row_map, n_machines, epochs, batch_size, shuffle, adam, seed,
-               validation_batch_size, early_stopping, loss="mse"):
+               validation_batch_size, early_stopping, loss="mse", optimizer=None):
     """
     The one fit launch of a bucket (job j trains a slot of machine j mod n_machines): gb_ffae_fit without held-out positions or a
     row map, gb_ffae_fit_split with them, gb_ffae_fit_stop with an EarlyStopping callback (one for all machines or one per machine).
@@ -318,20 +318,21 @@ def _fit_slots(eng, params, fit_jobs, n_jobs, max_rows, x, y, split, row_map, n_
         stop = engine.make_stop([per_machine[j % n_machines] for j in range(n_jobs)])
         hist, acc, val_loss, val_acc, epochs_run, best_epoch, _ = eng.fit_split(
             params, fit_jobs, n_jobs, max_rows, x, y, split=split, row_map=row_map, val_batch=vb, epochs=epochs, batch_size=batch_size,
-            shuffle=shuffle, adam=adam, seed=seed, stop=stop, loss=loss)
+            shuffle=shuffle, adam=adam, seed=seed, stop=stop, loss=loss, optimizer=optimizer)
     elif split is None:
         hist, acc, _ = eng.fit(params, fit_jobs, n_jobs, max_rows, x, y, epochs=epochs, batch_size=batch_size, shuffle=shuffle, adam=adam, seed=seed,
-                               loss=loss)
+                               loss=loss, optimizer=optimizer)
     else:
         hist, acc, val_loss, val_acc, _ = eng.fit_split(params, fit_jobs, n_jobs, max_rows, x, y, split=split, row_map=row_map, val_batch=vb,
-                                                        epochs=epochs, batch_size=batch_size, shuffle=shuffle, adam=adam, seed=seed, loss=loss)
+                                                        epochs=epochs, batch_size=batch_size, shuffle=shuffle, adam=adam, seed=seed, loss=loss,
+                                                        optimizer=optimizer)
     return hist, acc, val_loss, val_acc, epochs_run, best_epoch
 
 
 def build_fleet(eng: "engine.FFEngine", x, y, rows: int, epochs: int = 1, batch_size: int = 32, n_splits: int = 3, seed: int = 0,
                 adam: Optional[Dict[str, float]] = None, shuffle: bool = True, generator=None, input_scaler: bool = False,
                 detector_shuffle: bool = False, validation_split: float = 0.0, validation_batch_size: Optional[int] = None,
-                early_stopping=None, loss: str = "mse") -> FleetBuild:
+                early_stopping=None, loss: str = "mse", optimizer=None) -> FleetBuild:
     """
     The batched form of ``gordo build`` for one architecture bucket: for every machine the 3-fold TimeSeriesSplit
     cross-validation (fit on each prefix, thresholds from the following test block: diff.py:176-266) and the final fit on
@@ -357,6 +358,7 @@ def build_fleet(eng: "engine.FFEngine", x, y, rows: int, epochs: int = 1, batch_
     each of its epochs inside the fit launch (gb_ffae_fit_stop), as sklearn's clone hands every fold the same callbacks.  The
     result then carries ``epochs_run`` / ``best_epoch``; history entries past a fit's ``epochs_run`` are NaN.
     ``loss``: the estimator's canonical Keras loss name (``FFNetSpec.loss``), trained on and reported by every fit.
+    ``optimizer``: None (Adam from ``adam``) or the estimator's (name, record) (``factories.specs.fit_optimizer``), for every fit.
     """
     torch = engine._torch()
     dev = eng.device
@@ -405,7 +407,7 @@ def build_fleet(eng: "engine.FFEngine", x, y, rows: int, epochs: int = 1, batch_
     fit_jobs = engine.jobs_to_device(engine.make_jobs(fit_slots, fit_rows, fit_x), dev)
     hist, acc, val_loss, val_acc, epochs_run, best_epoch = _fit_slots(
         eng, params, fit_jobs, len(fit_slots), N, x, y, split, row_map, M, epochs, batch_size, shuffle, adam, seed, validation_batch_size, early_stopping,
-        loss)
+        loss, optimizer)
     if n_train == slot_n:  # nothing held out
         val_loss = val_acc = None
     # scalers: final on all rows, fold k on its training prefix (diff.py:173 inside each CV clone), held-out rows included
@@ -541,7 +543,7 @@ class LSTMFleetBuild:
 
 def build_lstm_fleet(eng: "engine.LSTMEngine", x, y, rows: int, lookahead: int = 0, epochs: int = 1, batch_size: int = 32, n_splits: int = 3,
                      seed: int = 0, adam: Optional[Dict[str, float]] = None, input_scaler: bool = False, memory_budget: int = 8 << 30,
-                     keep_init_params: bool = False, generator=None, loss: str = "mse") -> LSTMFleetBuild:
+                     keep_init_params: bool = False, generator=None, loss: str = "mse", optimizer=None) -> LSTMFleetBuild:
     """
     The batched ``gordo build`` of one bucket of LSTM machines (``DiffBasedAnomalyDetector(KerasLSTMAutoEncoder | KerasLSTMForecast)``,
     the network bare or behind one MinMaxScaler): for every machine the TimeSeriesSplit cross validation and the final fit, as
@@ -555,7 +557,7 @@ def build_lstm_fleet(eng: "engine.LSTMEngine", x, y, rows: int, lookahead: int =
     one fit launch may take.  Machines are
     trained in chunks that fit it -- all ``n_splits + 1`` fits of a machine in the same chunk; every job's result is the same
     whatever the chunking.  ``keep_init_params``: keep the initial parameters of every slot on the result (``init_params``).
-    ``loss``: the estimator's canonical Keras loss name (``LSTMNetSpec.loss``).
+    ``loss``: the estimator's canonical Keras loss name (``LSTMNetSpec.loss``).  ``optimizer``: as in ``build_fleet``.
     """
     torch = engine._torch()
     dev = eng.device
@@ -620,7 +622,7 @@ def build_lstm_fleet(eng: "engine.LSTMEngine", x, y, rows: int, lookahead: int =
         p = params.index_select(0, idx)
         jobs = engine.jobs_to_device(engine.make_jobs(np.arange(len(slots)), slot_windows[slots], x_row[slots]), dev)
         cl, ca, _ = fit(p, jobs, len(slots), int(slot_windows[slots].max()), xf, yf, epochs=epochs, batch_size=batch_size, lookahead=la,
-                        primer=True, adam=adam, loss=loss)
+                        primer=True, adam=adam, loss=loss, optimizer=optimizer)
         params.index_copy_(0, idx, p)
         hist.index_copy_(0, idx, cl)
         acc.index_copy_(0, idx, ca)
@@ -792,7 +794,7 @@ def build_kfold_fleet(eng: "engine.FFEngine", x, y, rows: int, cv, epochs: int =
                       target_scaler: bool = False, detector_shuffle: bool = False, validation_split: float = 0.0,
                       validation_batch_size: Optional[int] = None, early_stopping=None, window: Optional[int] = None,
                       smoothing_method: Optional[str] = None, threshold_percentile: float = 0.99,
-                      keep_init_params: bool = False, loss: str = "mse") -> KFoldFleetBuild:
+                      keep_init_params: bool = False, loss: str = "mse", optimizer=None) -> KFoldFleetBuild:
     """
     The batched ``gordo build`` of one bucket of ``DiffBasedKFCVAnomalyDetector`` machines (diff.py:566-635 in the reference):
     for every machine the K-fold cross validation under ``cv`` (a KFold) and the final fit -- ``(K + 1) * n_machines`` fits in one
@@ -889,7 +891,7 @@ def build_kfold_fleet(eng: "engine.FFEngine", x, y, rows: int, cv, epochs: int =
     fit_jobs = jobs(np.arange(S), np.repeat(n_train, M), slot_x)
     hist, acc, val_loss, val_acc, epochs_run, best_epoch = _fit_slots(
         eng, params, fit_jobs, S, N, xf, yf, split, row_map, M, epochs, batch_size, shuffle, adam, seed, validation_batch_size, early_stopping,
-        loss)
+        loss, optimizer)
     if n_train == slot_n:  # nothing held out
         val_loss = val_acc = None
 

@@ -38,7 +38,8 @@ def feedforward_model(
     acts = [_check_act(f) for f in (*encoding_func, *decoding_func, out_func)]
     l1 = [0.0 if i == 0 else ACTIVITY_L1 for i in range(len(encoding_dim))] + [0.0] * (len(decoding_dim) + 1)
     metrics = list((compile_kwargs or {}).get("metrics", ["accuracy"]))
-    return FFNetSpec(dims, acts, l1, _optimizer(optimizer, optimizer_kwargs), metrics, resolve_loss(compile_kwargs))
+    adam, opt, opt_cfg = _optimizer(optimizer, optimizer_kwargs)
+    return FFNetSpec(dims, acts, l1, adam, metrics, resolve_loss(compile_kwargs), opt, opt_cfg)
 
 
 @register_model_builder(type="KerasAutoEncoder")

@@ -33,8 +33,9 @@ def lstm_model(
     check_dim_func_len("decoding", decoding_dim, decoding_func)
     units = [*map(int, encoding_dim), *map(int, decoding_dim)]
     acts = [_check_act(f) for f in (*encoding_func, *decoding_func)]
+    adam, opt, opt_cfg = _optimizer(optimizer, optimizer_kwargs)
     return LSTMNetSpec(int(n_features), units, acts, int(n_features_out), _check_act(out_func), int(lookback_window),
-                       _optimizer(optimizer, optimizer_kwargs), list((compile_kwargs or {}).get("metrics", [])), resolve_loss(compile_kwargs))
+                       adam, list((compile_kwargs or {}).get("metrics", [])), resolve_loss(compile_kwargs), opt, opt_cfg)
 
 
 @register_model_builder(type="KerasLSTMAutoEncoder")

@@ -27,7 +27,7 @@ from sklearn.metrics import explained_variance_score
 
 from .base import GordoBase
 from .factories import *  # noqa: F401,F403  -- executes the @register_model_builder decorators
-from .factories.specs import FFNetSpec, LSTMNetSpec
+from .factories.specs import FFNetSpec, LSTMNetSpec, fit_optimizer
 from .register import register_model_builder
 
 logger = logging.getLogger(__name__)
@@ -325,6 +325,7 @@ class KerasBaseEstimator(BaseEstimator, GordoBase):
         if self.model is None:
             self._prepare_model()
         spec = self.model.spec
+        optimizer = fit_optimizer(spec)  # None: Adam from spec.adam
         if spec.dims[0] != X.shape[1] or spec.dims[-1] != y.shape[1]:
             raise ValueError(f"model was built for {spec.dims[0]}->{spec.dims[-1]} features, got X {X.shape} y {y.shape}")
         fit_args = {**self.extract_supported_fit_args(self.kwargs), **kwargs}
@@ -361,10 +362,10 @@ class KerasBaseEstimator(BaseEstimator, GordoBase):
                 vbatch = int(fit_args.get("validation_batch_size") or batch_size)
             state, step0 = None, 0
             steps = int(math.ceil(n_train / batch_size))
-            frozen = dict(spec.adam, lr=0.0)
+            frozen = dict(spec.adam, lr=0.0)  # an Adam pass at lr 0 whatever the fit's optimizer: it moves nothing
             for e in range(epochs):
                 loss, acc, state = eng.fit(params, jobs, 1, n_train, xd, yd, epochs=1, batch_size=batch_size, shuffle=shuffle,
-                                           adam=spec.adam, seed=seed + e, state=state, step0=step0, loss=spec.loss)
+                                           adam=spec.adam, seed=seed + e, state=state, step0=step0, loss=spec.loss, optimizer=optimizer)
                 step0 += steps
                 logs = {"loss": float(loss[0, 0])}
                 if "accuracy" in history:
@@ -386,7 +387,7 @@ class KerasBaseEstimator(BaseEstimator, GordoBase):
             epochs_run = len(history["loss"])
         else:
             loss, acc, _ = eng.fit(params, jobs, 1, n_train, xd, yd, epochs=epochs, batch_size=batch_size, shuffle=shuffle,
-                                   adam=spec.adam, seed=seed, loss=spec.loss)
+                                   adam=spec.adam, seed=seed, loss=spec.loss, optimizer=optimizer)
             history["loss"] = [float(v) for v in loss[0].cpu().numpy()]
             if "accuracy" in history:
                 history["accuracy"] = [float(v) for v in acc[0].cpu().numpy()]
@@ -491,6 +492,7 @@ class KerasLSTMBaseEstimator(KerasBaseEstimator, TransformerMixin, metaclass=abc
             y = y.reshape(-1, 1)
         self.initialize(X.shape[1], y.shape[1])
         spec = self.model.spec
+        optimizer = fit_optimizer(spec)  # None: Adam from spec.adam
         fit_args = {**self.extract_supported_fit_args(self.kwargs), **kwargs}
         epochs = int(fit_args.get("epochs", 1))
         callbacks = build_callbacks(fit_args.get("callbacks"))
@@ -514,7 +516,7 @@ class KerasLSTMBaseEstimator(KerasBaseEstimator, TransformerMixin, metaclass=abc
             state = None
             for e in range(epochs):
                 loss, acc, state = fit(params, jobs, 1, n_win, xd, yd, epochs=1, batch_size=batch_size, lookahead=self.lookahead,
-                                       primer=(e == 0), adam=getattr(spec, "adam", None), state=state, loss=spec.loss)
+                                       primer=(e == 0), adam=getattr(spec, "adam", None), state=state, loss=spec.loss, optimizer=optimizer)
                 logs = {"loss": float(loss[0, 0])}
                 if want_acc:
                     logs["accuracy"] = float(acc[0, 0])
@@ -527,7 +529,7 @@ class KerasLSTMBaseEstimator(KerasBaseEstimator, TransformerMixin, metaclass=abc
                     params = cb.best_weights
         else:
             loss, acc, _ = fit(params, jobs, 1, n_win, xd, yd, epochs=epochs, batch_size=batch_size, lookahead=self.lookahead,
-                               primer=True, adam=getattr(spec, "adam", None), loss=spec.loss)
+                               primer=True, adam=getattr(spec, "adam", None), loss=spec.loss, optimizer=optimizer)
             history["loss"] = [float(v) for v in loss[0].cpu().numpy()]
             if want_acc:
                 history["accuracy"] = [float(v) for v in acc[0].cpu().numpy()]

@@ -238,7 +238,48 @@ typedef struct gb_fit_hparams {
   int32_t loss;           /* gb_loss; 0 = GB_LOSS_MSE.  Outside 0..5: GB_E_ARG, nothing enqueued */
 } gb_fit_hparams;
 
-/* Adam moments are opaque optimizer state in the kernel's padded layout: gb_ffae_fit_state_stride() floats per slot. */
+/* Optimizer of a fit (the reference factories' `optimizer` / `optimizer_kwargs`, a Keras 3 optimizer; keras 3.3.3 update rules [3P],
+ * restated, not verified against TF).  g is the summed mini-batch gradient of one parameter, t the 1-based step count of its slot
+ * (hp->step0 / adam_t carry it across launches; the LSTM primer step counts), s0 / s1 the two state slots (adam_m / adam_v):
+ *   ADAM, ADAMW  s0 = m += (g - m)(1 - beta1); s1 = v += (g^2 - v)(1 - beta2); w -= lr sqrt(1 - beta2^t) / (1 - beta1^t) m / (sqrt(v) + eps)
+ *   RMSPROP      (rho = beta1) s0 = v = rho v + (1 - rho) g^2; d = v + eps, or with GB_OPT_CENTERED s1 = gbar = rho gbar + (1 - rho) g
+ *                and d = v - gbar^2 + eps; inc = lr g / sqrt(d); with momentum > 0, s1 = mom = momentum mom + inc and w -= mom,
+ *                else w -= inc.  Centered together with momentum would need a third slot: GB_E_ARG.
+ *   ADAGRAD      s0 = acc += g^2 (at t = 1 the stored s0 is not read: acc starts from initial_accumulator); w -= lr g / sqrt(acc + eps)
+ *   ADADELTA     (rho = beta1) s0 = Eg2 = rho Eg2 + (1 - rho) g^2; D = -sqrt(s1 + eps) g / sqrt(Eg2 + eps);
+ *                s1 = rho s1 + (1 - rho) D^2; w += lr D
+ *   ADAMAX       s0 = m += (g - m)(1 - beta1); s1 = u = max(beta2 u, |g|); w -= lr m / ((1 - beta1^t)(u + eps))
+ *   NADAM        u_t = beta1 (1 - 0.96^t / 2), P_t = P_(t-1) u_t (float32 product from P_0 = 1, recomputed from step 1 by every launch);
+ *                m, v as Adam; mhat = u_(t+1) m / (1 - P_t u_(t+1)) + (1 - u_t) g / (1 - P_t); w -= lr mhat / (sqrt(v / (1 - beta2^t)) + eps)
+ * Before the update, every optimizer: g = clip(g, -clipvalue, clipvalue) when clipvalue > 0, then w -= w * weight_decay * lr.
+ * Invalid (GB_E_ARG, nothing enqueued): an unknown kind or flag, a negative or non-finite lr, eps, momentum, initial_accumulator,
+ * weight_decay or clipvalue, beta1 / beta2 (the ones the kind reads) outside [0, 1), GB_OPT_CENTERED on another kind than RMSPROP. */
+typedef enum gb_opt {
+  GB_OPT_ADAM = 0,
+  GB_OPT_ADAMW = 1,
+  GB_OPT_RMSPROP = 2,
+  GB_OPT_ADAGRAD = 3,
+  GB_OPT_ADADELTA = 4,
+  GB_OPT_ADAMAX = 5,
+  GB_OPT_NADAM = 6
+} gb_opt;
+#define GB_OPT_CENTERED 1 /* gb_optimizer.flags: RMSprop(centered=True) */
+
+typedef struct gb_optimizer {
+  int32_t kind;               /* gb_opt */
+  int32_t flags;              /* GB_OPT_CENTERED or 0 */
+  float lr;
+  float beta1;                /* beta_1; rho of RMSPROP and ADADELTA */
+  float beta2;                /* beta_2 of ADAM, ADAMW, ADAMAX, NADAM */
+  float eps;
+  float momentum;             /* RMSPROP */
+  float initial_accumulator;  /* ADAGRAD */
+  float weight_decay;         /* 0 = none */
+  float clipvalue;            /* 0 = none */
+} gb_optimizer;
+
+/* The optimizer state (adam_m = slot 0, adam_v = slot 1) is opaque, in the kernel's padded layout: gb_ffae_fit_state_stride() floats
+ * per slot; all zero for a fresh fit whatever the optimizer. */
 size_t gb_ffae_fit_state_stride(const gb_ffnet* net);
 
 /* params: [n_slots][param_stride], updated in place.  adam_m / adam_v: [n_slots][state_stride], updated in place
@@ -299,6 +340,15 @@ int gb_ffae_fit_stop(const gb_ffnet* net, float* params, float* adam_m, float* a
                      const int32_t* row_map, const int32_t* perm, const gb_fit_hparams* hp, int32_t val_batch,
                      float* out_loss, float* out_acc, float* out_val_loss, float* out_val_acc, const gb_fit_stop* stop,
                      float* best_params, int32_t* out_epochs, int32_t* out_best_epoch, void* stream);
+
+/* gb_ffae_fit_stop with the optimizer `opt` in place of Adam from hp->lr / beta1 / beta2 / eps.  opt NULL: Adam from hp, bit-identical
+ * to gb_ffae_fit_stop; a NULL stop gives gb_ffae_fit_split and a NULL stop and split gb_ffae_fit (out_val_loss, out_val_acc,
+ * best_params, out_epochs and out_best_epoch may then be NULL).  hp->lr / beta1 / beta2 / eps are not read when opt is given. */
+int gb_ffae_fit_opt(const gb_ffnet* net, float* params, float* adam_m, float* adam_v, const gb_job* jobs,
+                    const gb_fit_split* split, int32_t n_jobs, int32_t max_rows, const float* x, const float* y,
+                    const int32_t* row_map, const int32_t* perm, const gb_fit_hparams* hp, int32_t val_batch,
+                    float* out_loss, float* out_acc, float* out_val_loss, float* out_val_acc, const gb_fit_stop* stop,
+                    float* best_params, int32_t* out_epochs, int32_t* out_best_epoch, const gb_optimizer* opt, void* stream);
 
 /* The memory plan gb_ffae_fit uses for this architecture (host only, no device needed).  The first of five that fits in
  * 227 KB of shared memory: everything in shared memory; the weight image in the slot's L2-resident state area
@@ -377,6 +427,16 @@ int gb_lstm_fit_tc(const gb_lstmnet* net, float* params, float* adam_m, float* a
                    const gb_job* jobs, int32_t n_jobs, int32_t max_windows, const float* x, const float* y,
                    const gb_lstm_fit_hparams* hp, void* workspace, float* out_loss, float* out_acc, int32_t loss,
                    void* stream);
+/* gb_lstm_fit_loss / gb_lstm_fit_tc with the gb_optimizer `opt` in place of Adam from hp->lr / beta1 / beta2 / eps (adam_m / adam_v
+ * are its state slots 0 / 1, adam_t its step counts).  opt NULL: Adam from hp, bit-identical to the entry point without _opt. */
+int gb_lstm_fit_opt(const gb_lstmnet* net, float* params, float* adam_m, float* adam_v, int32_t* adam_t,
+                    const gb_job* jobs, int32_t n_jobs, int32_t max_windows, const float* x, const float* y,
+                    const gb_lstm_fit_hparams* hp, void* workspace, float* out_loss, float* out_acc, int32_t loss,
+                    const gb_optimizer* opt, void* stream);
+int gb_lstm_fit_tc_opt(const gb_lstmnet* net, float* params, float* adam_m, float* adam_v, int32_t* adam_t,
+                       const gb_job* jobs, int32_t n_jobs, int32_t max_windows, const float* x, const float* y,
+                       const gb_lstm_fit_hparams* hp, void* workspace, float* out_loss, float* out_acc, int32_t loss,
+                       const gb_optimizer* opt, void* stream);
 
 /* Keras' Orthogonal initialiser for recurrent kernels: g holds n_mats standard-normal [rows][cols] draws (float64, rows <= cols,
  * overwritten); matrix i's rows are orthonormalised (Gram-Schmidt, the sign convention of Keras' QR) and written as float32 to
