@@ -13,12 +13,14 @@ constexpr int THREADS = 256;
 constexpr int NWARPS = THREADS / 32;
 constexpr int ROWS_PER_CTA = 1024;
 
+// The integer form follows the sign bit, not v >= 0: -0.0 is INT_MIN as a signed integer and must take the unsigned path
+// of the negative values, where it is the largest.
 __device__ __forceinline__ void atomic_max_float(float* addr, float v) {
-  if (v >= 0.f) atomicMax(reinterpret_cast<int*>(addr), __float_as_int(v));
+  if (!signbit(v)) atomicMax(reinterpret_cast<int*>(addr), __float_as_int(v));
   else atomicMin(reinterpret_cast<unsigned*>(addr), __float_as_uint(v));
 }
 __device__ __forceinline__ void atomic_min_float(float* addr, float v) {
-  if (v >= 0.f) atomicMin(reinterpret_cast<int*>(addr), __float_as_int(v));
+  if (!signbit(v)) atomicMin(reinterpret_cast<int*>(addr), __float_as_int(v));
   else atomicMax(reinterpret_cast<unsigned*>(addr), __float_as_uint(v));
 }
 
@@ -42,11 +44,11 @@ template <> struct RollBits<double> {
 __device__ __forceinline__ void atomic_max_fp(float* addr, float v) { atomic_max_float(addr, v); }
 __device__ __forceinline__ void atomic_min_fp(float* addr, float v) { atomic_min_float(addr, v); }
 __device__ __forceinline__ void atomic_max_fp(double* addr, double v) {
-  if (v >= 0.) atomicMax(reinterpret_cast<long long*>(addr), __double_as_longlong(v));
+  if (!signbit(v)) atomicMax(reinterpret_cast<long long*>(addr), __double_as_longlong(v));
   else atomicMin(reinterpret_cast<unsigned long long*>(addr), (unsigned long long)__double_as_longlong(v));
 }
 __device__ __forceinline__ void atomic_min_fp(double* addr, double v) {
-  if (v >= 0.) atomicMin(reinterpret_cast<long long*>(addr), __double_as_longlong(v));
+  if (!signbit(v)) atomicMin(reinterpret_cast<long long*>(addr), __double_as_longlong(v));
   else atomicMax(reinterpret_cast<unsigned long long*>(addr), (unsigned long long)__double_as_longlong(v));
 }
 
@@ -152,6 +154,7 @@ __global__ void __launch_bounds__(THREADS) rollmin_max_kernel(const gb_job* jobs
     T best = s_max[0][j];
 #pragma unroll
     for (int q = 1; q < NWARPS; ++q) best = s_max[q][j] > best ? s_max[q][j] : best;
+    best = best + (T)0;  // -0.0 -> +0.0: as an integer -0.0 would never beat the -1 marker
     if (best >= (T)0)
       atomicMax(reinterpret_cast<typename RollBits<T>::I*>(&out[(long)job.slot * n_cols + j]), RollBits<T>::bits(best));
   }
@@ -188,7 +191,7 @@ __global__ void __launch_bounds__(THREADS) anomaly_score_kernel(const gb_job* jo
     T ss = 0, su = 0;
     for (int j = lane; j < n_out; j += 32) {
       const T diff = __ldg(yhat + go + j) - __ldg(y + gy + j);
-      const T d = diff < (T)0 ? -diff : diff;
+      const T d = fabs(diff);  // +0.0 for yhat = -0.0, y = +0.0, as np.abs
       if (o_tu) o_tu[go + j] = d;
       su += d * d;
       if (sc) {
