@@ -143,11 +143,16 @@ __global__ void __launch_bounds__(THREADS) ffae_infer_fma_kernel(const Args a) {
               acc[i].z = fmaf(av[i].w, w3.z, acc[i].z); acc[i].w = fmaf(av[i].w, w3.w, acc[i].w);
             }
           }
+          // columns past the layer's width stay 0, as in the row-per-thread kernel: their zero weights times an infinite input are
+          // NaN, which the next layer would spread over the whole row
+          const int n_live = a.net.dims[l + 1] - (c0 + n0);
 #pragma unroll
           for (int i = 0; i < RT; ++i) {
             float4 o;
-            o.x = gb::apply_act(act, acc[i].x); o.y = gb::apply_act(act, acc[i].y);
-            o.z = gb::apply_act(act, acc[i].z); o.w = gb::apply_act(act, acc[i].w);
+            o.x = gb::apply_act(act, acc[i].x);
+            o.y = n_live > 1 ? gb::apply_act(act, acc[i].y) : 0.f;
+            o.z = n_live > 2 ? gb::apply_act(act, acc[i].z) : 0.f;
+            o.w = n_live > 3 ? gb::apply_act(act, acc[i].w) : 0.f;
             *reinterpret_cast<float4*>(out + (lane + 32 * i) * pitch + c0 + n0) = o;
           }
         }

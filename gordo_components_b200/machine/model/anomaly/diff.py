@@ -43,6 +43,31 @@ def _values(a) -> np.ndarray:
     return np.asarray(getattr(a, "values", a))
 
 
+def _has_inf(a: np.ndarray) -> bool:
+    return a.dtype.kind in "fc" and bool(np.isinf(a).any())
+
+
+def _refuse_infinity(a: np.ndarray):
+    """The error sklearn's scalers raise on ±inf (NaN passes): the reference scales y, the model output and, behind a scaler
+    pipeline, X with them, so a request holding ±inf in any of these is refused there too."""
+    if _has_inf(a):
+        raise ValueError(f"Input X contains infinity or a value too large for {a.dtype!r}.")
+
+
+def _total_skipna(total: np.ndarray, per_tag: np.ndarray, rows: np.ndarray) -> np.ndarray:
+    """
+    ``total`` (float64) with its ``rows`` (the NaN ones) recomputed as the reference computes the anomaly frame's totals,
+    ``np.square(tags).mean(axis=1)`` on a DataFrame (diff.py:366, :383): pandas skips NaN tags, and a row with no tag left is NaN.
+    The kernels average over every tag, the numpy mean that threshold fitting needs (diff.py:292), so only the frame is corrected.
+    """
+    sq = np.square(np.asarray(per_tag, dtype=np.float64)[rows])
+    cnt = (~np.isnan(sq)).sum(axis=1)
+    out = np.array(total, dtype=np.float64)
+    with np.errstate(invalid="ignore", divide="ignore"):
+        out[rows] = np.where(cnt > 0, np.nansum(sq, axis=1) / cnt, np.nan)
+    return out
+
+
 _MULTIPLIERS = weakref.WeakKeyDictionary()  # scaler object -> (fitted-state key, slope): a request does not re-probe a fitted scaler
 
 
@@ -255,6 +280,7 @@ class DiffBasedAnomalyDetector(AnomalyDetectorBase):
 
         dev = engine.cuda_device()
         yv = _values(y_true)
+        _refuse_infinity(yv)
         n_out = yv.shape[1]
         mult = _scaler_multiplier(scaler, n_out)
         torch = engine._torch()
@@ -269,9 +295,11 @@ class DiffBasedAnomalyDetector(AnomalyDetectorBase):
             pre, ae = fused
             eng = ae._engine()
             affine = _compose_affine(pre, eng.n_in)
+            variant = 0
             if pre and affine is not None:
                 # per-feature scalers in front of the network: one f64 pass on the device (gb_affine_f64) instead of sklearn on the host
                 Xv = np.ascontiguousarray(_values(X), dtype=np.float64)
+                _refuse_infinity(Xv)  # what the sklearn steps would have raised
                 n = len(Xv)
                 jobs = engine.jobs_to_device(engine.make_jobs([0], [n], [0]), dev)
                 a_d, b_d = (torch.from_numpy(v.reshape(1, -1)).to(dev) for v in affine)
@@ -284,11 +312,16 @@ class DiffBasedAnomalyDetector(AnomalyDetectorBase):
                 n = len(Xv)
                 jobs = engine.jobs_to_device(engine.make_jobs([0], [n], [0]), dev)
                 xd = engine.to_device_f32(Xv, dev)
+                if _has_inf(Xv):
+                    # tanh(±inf) = ±1 as in Keras on the fp32 kernels; the tensor-core kernel's split of x into TF32 + BF16 parts
+                    # turns ±inf into NaN, so an input holding ±inf is not given to it
+                    variant = 1
             yd = engine.to_device_f32(yv, dev)
-            res = eng.infer_score(ae._device_params(), jobs, 1, n, xd, yd, scale_d, ft_d, at_d, want=want)
+            res = eng.infer_score(ae._device_params(), jobs, 1, n, xd, yd, scale_d, ft_d, at_d, want=want, variant=variant)
         else:
             # diff.py:350-385: pandas arithmetic on float64 y and the (float32- or float64-valued) predictions widened to float64
             pred = np.asarray(estimator_owner.predict(X) if hasattr(estimator_owner, "predict") else estimator_owner.transform(X))
+            _refuse_infinity(pred)
             n = len(pred)
             p64 = np.ascontiguousarray(pred, dtype=np.float64)
             p64 = p64.reshape(n, -1)
@@ -297,7 +330,10 @@ class DiffBasedAnomalyDetector(AnomalyDetectorBase):
             jobs = engine.jobs_to_device(engine.make_jobs([0], [n], [0]), dev)
             res = engine.anomaly_score(jobs, 1, n, pd_, yd, n_out, scale_d, ft_d, at_d, want=want) if n else {}
             res["model-output"] = pred
-        return {k: (v.cpu().numpy() if hasattr(v, "cpu") else np.asarray(v)) for k, v in res.items()}
+        res = {k: (v.cpu().numpy() if hasattr(v, "cpu") else np.asarray(v)) for k, v in res.items()}
+        if fused is not None:
+            _refuse_infinity(res["model-output"])
+        return res
 
     # ------------------------------------------------------------------ cross validation -> thresholds
     def cross_validate(self, *, X, y, cv=TimeSeriesSplit(n_splits=3), **kwargs):
@@ -394,6 +430,18 @@ class DiffBasedAnomalyDetector(AnomalyDetectorBase):
         """``anomaly_blocks`` for score arrays that already exist (``res`` as ``_score`` returns it, e.g. out of a request coalescer)."""
         feat_thr, agg_thr = self._thresholds()
         res = dict(res)
+        # rows with a missing target tag: pandas' totals, and the total confidence from them, before anything is smoothed
+        for total, per_tag in (("total-anomaly-scaled", "tag-anomaly-scaled"), ("total-anomaly-unscaled", "tag-anomaly-unscaled")):
+            if total not in res or per_tag not in res:
+                continue
+            rows = np.isnan(res[total])
+            if not rows.any():
+                continue
+            res[total] = _total_skipna(res[total], res[per_tag], rows)
+            if total == "total-anomaly-scaled" and "total-anomaly-confidence" in res and agg_thr is not None:
+                conf = np.array(res["total-anomaly-confidence"], dtype=np.float64)
+                conf[rows] = res[total][rows] / float(agg_thr)
+                res["total-anomaly-confidence"] = conf
         out = res["model-output"]
         index, frame_blocks, frame_cols = model_utils.base_blocks(
             tags=X.columns, model_input=X.values, model_output=out, target_tag_list=y.columns,

@@ -556,7 +556,9 @@ class KerasLSTMBaseEstimator(KerasBaseEstimator, TransformerMixin, metaclass=abc
         if cache is None or cache[0] is not self.model.weights:
             cache = (self.model.weights, eng.pack_params([self.model.weights]))
             self.__dict__["_dev_cache"] = cache
-        return eng.infer(cache[1], jobs, 1, n_win, xd, n_win).cpu().numpy()
+        # ±inf in X: the fp32 kernel saturates the gates as Keras does; the tensor-core kernel's windows come out NaN
+        variant = 1 if np.asarray(X).dtype.kind == "f" and np.isinf(X).any() else 0
+        return eng.infer(cache[1], jobs, 1, n_win, xd, n_win, variant=variant).cpu().numpy()
 
     def score(self, X, y, sample_weight=None, **kwargs) -> float:
         if self.model is None:

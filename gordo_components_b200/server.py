@@ -292,8 +292,16 @@ class ResidentBucket:
         return True
 
     def anomaly_blocks(self, store: "ModelStore", name: str, X: pd.DataFrame, y: pd.DataFrame, frequency=None):
+        from .machine.model.anomaly.diff import _has_inf, _refuse_infinity, _values
+
+        model = store.model(name)
+        _refuse_infinity(_values(y))
+        if _has_inf(_values(X)):
+            # the coalescer's launch may run the tensor-core kernel, which does not take ±inf inputs: this request goes on its own
+            return model.anomaly_blocks(X, y, frequency=frequency)
         scores = self.coalescer.anomaly(self.slot[name], X, y)
-        return store.model(name).blocks_from_scores(scores, X, y, frequency)
+        _refuse_infinity(scores["model-output"])
+        return model.blocks_from_scores(scores, X, y, frequency)
 
     def close(self):
         self.coalescer.close()

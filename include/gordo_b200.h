@@ -113,7 +113,12 @@ size_t gb_ffnet_param_stride(const gb_ffnet* net);
  * n_x_rows / n_out_rows: number of rows of the x (and y) array and of the output arrays (TMA tensor extents).
  * variant (low byte): 0 = auto (tensor-core kernel for the stacks it covers, the row-per-thread kernel for stacks whose widths are
  * all <= 16, else the generic one), 1 = generic fp32 CUDA-core kernel, 2 = tensor-core (wgmma) split-precision kernel, 3 = row-per-thread
- * fp32 kernel (2 / 3: GB_E_SHAPE if the architecture is outside their range); higher bytes are debug knobs and must be 0. */
+ * fp32 kernel (2 / 3: GB_E_SHAPE if the architecture is outside their range); higher bytes are debug knobs and must be 0.
+ * Non-finite inputs stay in their own row.  The totals are the plain mean over all n_out tags (the numpy mean that threshold
+ * fitting uses, diff.py:292): a NaN tag gives a NaN total and an infinite tag an infinite one.  pandas' skip-NaN mean of the
+ * anomaly frame (diff.py:366, :383) is the caller's to apply.  NaN in x gives an all-NaN row.  On variants 1 and 3, ±inf in x
+ * propagates as IEEE arithmetic does (tanh(±inf) = ±1, as in Keras).  Variant 2 splits x into a TF32 part and a BF16 remainder,
+ * which is inf - inf = NaN, so ±inf in x gives an all-NaN row there: launch variant 1 for such rows. */
 int gb_ffae_infer_score(const gb_ffnet* net, const float* params, const gb_job* jobs, int32_t n_jobs,
                         int32_t max_rows, int64_t n_x_rows, int64_t n_out_rows, const float* x, const float* y, const float* scale,
                         const float* feat_thr, const float* agg_thr, float* out_model,
@@ -133,7 +138,8 @@ int gb_ffae_infer_plan(const gb_ffnet* net, int32_t* rows_per_tile, int32_t* res
 /* ---- K4 alone: anomaly score of predictions that already exist ----------------------------
  * Same outputs as gb_ffae_infer_score, for a `yhat` produced elsewhere (a base estimator that is not
  * one of ours, e.g. the sklearn regressors the reference's detector tests use; an LSTM prediction from
- * gb_lstm_infer).  yhat and all outputs are indexed by out_row, y by x_row. */
+ * gb_lstm_infer).  yhat and all outputs are indexed by out_row, y by x_row.  A NaN or ±inf in yhat or y reaches only
+ * its own (row, tag) cells and that row's totals, which are the plain mean over all tags as in gb_ffae_infer_score. */
 int gb_anomaly_score(const gb_job* jobs, int32_t n_jobs, int32_t max_rows, const float* yhat, const float* y,
                      int32_t n_out, const float* scale, const float* feat_thr, const float* agg_thr,
                      float* out_tag_scaled, float* out_tag_unscaled, float* out_total_scaled,

@@ -134,6 +134,19 @@ def fold_thresholds(y_true: np.ndarray, y_pred: np.ndarray, scale: np.ndarray, m
 # ------------------------------------------------------------------ anomaly()
 
 
+def row_mean_skipna(a: np.ndarray) -> np.ndarray:
+    """``DataFrame.mean(axis=1)`` (diff.py:366, :383): NaN cells are skipped, a row without any value is NaN.  Only the rows whose
+    plain mean is NaN are recomputed, so all-finite data costs one mean and one NaN scan."""
+    m = a.mean(axis=1)
+    bad = np.isnan(m)
+    if bad.any():
+        sub = a[bad]
+        cnt = (~np.isnan(sub)).sum(axis=1)
+        with np.errstate(invalid="ignore", divide="ignore"):
+            m[bad] = np.where(cnt > 0, np.nansum(sub, axis=1) / cnt, np.nan)
+    return m
+
+
 def anomaly_arrays(
     y_pred: np.ndarray,
     y: np.ndarray,
@@ -155,10 +168,10 @@ def anomaly_arrays(
     out: Dict[str, np.ndarray] = {"model-output": y_pred}
     tag_scaled = np.abs(minmax_transform(pred64, scale, min_) - minmax_transform(y, scale, min_))
     out["tag-anomaly-scaled"] = tag_scaled
-    out["total-anomaly-scaled"] = np.square(tag_scaled).mean(axis=1)
+    out["total-anomaly-scaled"] = row_mean_skipna(np.square(tag_scaled))
     tag_unscaled = np.abs(pred64 - y)
     out["tag-anomaly-unscaled"] = tag_unscaled
-    out["total-anomaly-unscaled"] = np.square(tag_unscaled).mean(axis=1)
+    out["total-anomaly-unscaled"] = row_mean_skipna(np.square(tag_unscaled))
     if window is not None and smoothing_method is not None:
         out["smooth-tag-anomaly-scaled"] = smoothing(tag_scaled, window, smoothing_method)
         out["smooth-total-anomaly-scaled"] = smoothing(out["total-anomaly-scaled"], window, smoothing_method)

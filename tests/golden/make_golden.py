@@ -11,6 +11,7 @@ Fixtures written:
                              block of DiffBasedAnomalyDetector.anomaly() from the reference
   ffnet_anomaly.npz          the same, with the base estimator being a fixed-weight hourglass
                              net (oracle/keras_math.ff_forward): pins net -> anomaly end to end
+  ffnet_anomaly_nan.npz      the fixed-weight net with sma smoothing on targets and inputs with missing (NaN) values
   live_detector_<seed>.npz   a reference DiffBasedAnomalyDetector (LinearRegression base, sma smoothing) after
                              cross_validate + fit: X, y, its predictions, thresholds and every anomaly() column block
 """
@@ -86,7 +87,21 @@ def dims_fixture():
         json.dump({"grid": table, "reference_test_table": ref_test_table}, f)
 
 
-def anomaly_fixture(name, n_rows, n_tags, window, method, datetime_index, base="linear", seed=0):
+def poison_with_nan(X, y, window, seed):
+    """Missing sensor values as requests carry them: scattered NaN targets, one row without any target, a NaN run in one target tag
+    longer than the smoothing window, and a few input rows without any value."""
+    rng = np.random.default_rng(seed + 100)
+    n, t = y.shape
+    yv, Xv = y.values.copy(), X.values.copy()
+    cells = rng.choice(n * t, size=12, replace=False)
+    yv.flat[cells] = np.nan
+    yv[n // 3] = np.nan
+    yv[n // 2: n // 2 + 2 * window, 1] = np.nan
+    Xv[[17, n // 4, n - 30, n - 1]] = np.nan
+    return pd.DataFrame(Xv, columns=X.columns, index=X.index), pd.DataFrame(yv, columns=y.columns, index=y.index)
+
+
+def anomaly_fixture(name, n_rows, n_tags, window, method, datetime_index, base="linear", seed=0, nan=False):
     rng = np.random.default_rng(seed)
     cols = [f"tag-{i}" for i in range(n_tags)]
     index = pd.date_range("2019-01-01", periods=n_rows, freq="10min", tz="UTC") if datetime_index else pd.RangeIndex(n_rows)
@@ -97,6 +112,8 @@ def anomaly_fixture(name, n_rows, n_tags, window, method, datetime_index, base="
     else:
         y = X.copy()
         est = FixedNet(n_features=n_tags, seed=seed)
+    if nan:
+        X, y = poison_with_nan(X, y, window, seed)
     det = ref.DiffBasedAnomalyDetector(base_estimator=est, scaler=MinMaxScaler(), window=window, smoothing_method=method)
     cv = TimeSeriesSplit(n_splits=3)
     cvo = det.cross_validate(X=X, y=y, cv=cv)
@@ -331,6 +348,7 @@ if __name__ == "__main__":
     anomaly_fixture("anomaly_ewma", 200, 4, 12, "ewma", False, seed=3)
     anomaly_fixture("ffnet_anomaly", 400, 8, None, None, True, base="net", seed=4)
     anomaly_fixture("ffnet_anomaly_t64", 200, 64, None, None, True, base="net", seed=5)
+    anomaly_fixture("ffnet_anomaly_nan", 400, 8, 6, "sma", True, base="net", seed=6, nan=True)
     callers_fixture()
     live_detector_fixture(11)
     live_detector_fixture(12)

@@ -351,3 +351,58 @@ def test_anomaly_frame_assembly_with_a_mocked_score(rows, offset, thresholds, wi
     assert list(got.columns) == list(want.columns) and list(got.dtypes) == list(want.dtypes) and len(got) == n
     pd.testing.assert_frame_equal(got, want, check_exact=True, check_freq=False)
     assert got.columns is not det.anomaly(X, X, frequency=freq).columns  # the cached column index is handed out as copies
+
+
+@pytest.mark.parametrize("window", [None, 4])
+def test_anomaly_frame_totals_skip_missing_target_tags(window):
+    """
+    Rows with NaN target tags, as requests with missing sensor values give them: the kernels' totals (numpy mean over every tag) are
+    NaN there, and the frame replaces them with pandas' mean over the tags that have a value (diff.py:366, :383) -- NaN only when no
+    tag has one -- and recomputes the total confidence from it.  Smoothing sees the corrected totals; every other row is untouched.
+    """
+    T, n = 4, 30
+    tags = [f"tag {i}" for i in range(T)]
+    rng = np.random.default_rng(7)
+    X = pd.DataFrame(rng.random((n, T)), index=pd.date_range("2019-01-01", periods=n, freq="10min", tz="UTC"), columns=tags)
+    det = DiffBasedAnomalyDetector(base_estimator=KerasAutoEncoder(kind="feedforward_hourglass"), window=window,
+                                   smoothing_method="sma" if window else None)
+    agg = 0.3
+    det.feature_thresholds_, det.aggregate_threshold_ = pd.Series(np.full(T, 0.5), index=tags), agg
+    tag_s, tag_u = rng.random((n, T)).astype(np.float32), rng.random((n, T)).astype(np.float32)
+    for a in (tag_s, tag_u):
+        a[3, 1] = a[10, [0, 2]] = a[11] = np.nan  # one tag, two tags, every tag
+        a[20:27, 3] = np.nan                      # a run longer than the window
+    tot_s, tot_u = np.square(tag_s).mean(axis=1), np.square(tag_u).mean(axis=1)
+    res = {"model-output": rng.random((n, T)).astype(np.float32), "tag-anomaly-scaled": tag_s, "total-anomaly-scaled": tot_s,
+           "tag-anomaly-unscaled": tag_u, "total-anomaly-unscaled": tot_u, "anomaly-confidence": tag_u / np.float32(0.5),
+           "total-anomaly-confidence": tot_s / np.float32(agg)}
+    det._score = lambda *a, **k: dict(res)
+    smoothed = []
+    det._smoothing = lambda metric: (smoothed.append(np.array(metric)), np.asarray(metric, dtype=np.float32) * 0.5)[1]
+    got = det.anomaly(X, X)
+
+    missing = np.isnan(tot_s)
+    assert missing.sum() == 10
+    with np.errstate(all="ignore"), __import__("warnings").catch_warnings():
+        __import__("warnings").simplefilter("ignore", RuntimeWarning)
+        want_s = pd.DataFrame(np.square(tag_s.astype(np.float64))).mean(axis=1).values
+        want_u = pd.DataFrame(np.square(tag_u.astype(np.float64))).mean(axis=1).values
+    for key, want, kernel in (("total-anomaly-scaled", want_s, tot_s), ("total-anomaly-unscaled", want_u, tot_u),
+                              ("total-anomaly-confidence", want_s / agg, tot_s / np.float32(agg))):
+        col = got[(key, "")].values
+        np.testing.assert_array_equal(col[~missing], kernel[~missing].astype(np.float64), err_msg=key)  # bit for bit
+        np.testing.assert_allclose(col[missing], want[missing], rtol=1e-12, err_msg=key)
+        assert np.isnan(col).tolist() == [i == 11 for i in range(n)], key  # NaN only where no tag has a value
+    np.testing.assert_array_equal(got["tag-anomaly-scaled"].values, tag_s.astype(np.float64))
+    if window:
+        # the smoothed totals are the smoothing of the corrected totals
+        assert len(smoothed) == 4
+        np.testing.assert_array_equal(smoothed[1], got[("total-anomaly-scaled", "")].values)
+        np.testing.assert_array_equal(smoothed[3], got[("total-anomaly-unscaled", "")].values)
+        corrected = np.where(missing, want_s, tot_s).astype(np.float32)
+        np.testing.assert_array_equal(got[("smooth-total-anomaly-scaled", "")].values, (corrected * 0.5).astype(np.float64))
+    # without a NaN row the totals pass through as the kernels computed them
+    clean = {k: np.nan_to_num(v, nan=0.25) for k, v in res.items()}
+    det._score = lambda *a, **k: dict(clean)
+    frame = det.anomaly(X, X)
+    np.testing.assert_array_equal(frame[("total-anomaly-scaled", "")].values, clean["total-anomaly-scaled"].astype(np.float64))

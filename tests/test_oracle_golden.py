@@ -137,7 +137,7 @@ def test_anomaly_oracle_matches_reference_fixture(case):
     assert level0 == expect
 
 
-@pytest.mark.parametrize("case", ["ffnet_anomaly", "ffnet_anomaly_t64"])
+@pytest.mark.parametrize("case", ["ffnet_anomaly", "ffnet_anomaly_t64", "ffnet_anomaly_nan"])
 def test_ffnet_fixture_prediction_is_oracle_forward(case):
     g = np.load(os.path.join(GOLDEN, case + ".npz"))
     dims = [int(d) for d in g["net_dims"]]
