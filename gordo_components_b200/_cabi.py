@@ -63,6 +63,7 @@ EXPORTS = (
     "gb_abi_version", "gb_last_error", "gb_device_check", "gb_ffnet_param_count", "gb_ffnet_param_stride",
     "gb_ffae_infer_score", "gb_ffae_tc_supported", "gb_ffae_infer_plan", "gb_anomaly_score", "gb_anomaly_score_f64", "gb_minmax_fit", "gb_minmax_f64", "gb_thresholds", "gb_thresholds_f64", "gb_cv_moments", "gb_smooth", "gb_quantile", "gb_affine_f64", "gb_gather_rows", "gb_minmax_inverse_f32", "gb_ffae_fit_state_stride", "gb_ffae_fit", "gb_ffae_fit_split", "gb_ffae_fit_stop", "gb_ffae_fit_plan", "gb_ffae_fit_opt",
     "gb_lstm_param_count", "gb_lstm_param_stride", "gb_lstm_workspace_bytes", "gb_lstm_infer", "gb_lstm_tc_supported", "gb_lstm_tc_workspace_bytes", "gb_lstm_infer_tc", "gb_lstm_fit_workspace_bytes", "gb_lstm_fit", "gb_lstm_fit_loss", "gb_lstm_fit_tc_workspace_bytes", "gb_lstm_fit_tc", "gb_lstm_fit_opt", "gb_lstm_fit_tc_opt",
+    "gb_lstm_fit_stop_state_bytes", "gb_lstm_fit_stop", "gb_lstm_fit_tc_stop",
     "gb_orthonormal_rows",
 )
 
@@ -192,6 +193,11 @@ def _declare(lib):
     lib.gb_ffae_fit_opt.restype = C.c_int
     for name in ("gb_lstm_fit_opt", "gb_lstm_fit_tc_opt"):
         getattr(lib, name).argtypes = lib.gb_lstm_fit_loss.argtypes[:-1] + [C.POINTER(GbOptimizer), _P]
+        getattr(lib, name).restype = C.c_int
+    lib.gb_lstm_fit_stop_state_bytes.restype = C.c_size_t
+    lib.gb_lstm_fit_stop_state_bytes.argtypes = [C.c_int32]
+    for name in ("gb_lstm_fit_stop", "gb_lstm_fit_tc_stop"):
+        getattr(lib, name).argtypes = lib.gb_lstm_fit_opt.argtypes[:-1] + [_P] * 5
         getattr(lib, name).restype = C.c_int
     lib.gb_orthonormal_rows.argtypes = [_P, C.c_int32, C.c_int32, C.c_int32, _P, C.c_int64, C.c_int64, _P]
     lib.gb_orthonormal_rows.restype = C.c_int

@@ -13,10 +13,12 @@ in one ``gb_ffae_fit`` launch, fold scoring / thresholds / scaler statistics / m
 launch (``gb_ffae_fit_stop``), and machines that differ only in the callback's parameters share a bucket.  The LSTM form
 of the same definition (``KerasLSTMAutoEncoder`` / ``KerasLSTMForecast``, ``_canonical_lstm``) is bucketed by architecture,
 lookback, lookahead, batch size and training length and built by ``fleet.build_lstm_fleet``: all fits as jobs of ``gb_lstm_fit``
-(batches above 32 windows: ``gb_lstm_fit_tc``, with ``FleetModelBuilder(lstm_wide_batches=True)``; in chunks that fit a workspace budget), every fold model's test block in one LSTM inference launch, float64 scoring.  The
+(batches above 32 windows: ``gb_lstm_fit_tc``, with ``FleetModelBuilder(lstm_wide_batches=True)``; in chunks that fit a workspace budget), every fold model's test block in one LSTM inference launch, float64 scoring.
+With ``FleetModelBuilder(lstm_early_stopping=True)`` an LSTM estimator with one ``EarlyStopping`` on ``loss`` (or a reported
+``accuracy``) is batched too: every fit applies the rule inside its launch (``gb_lstm_fit_stop`` / ``gb_lstm_fit_tc_stop``).  The
 cross-validation ``scores`` block of the metadata is then assembled on the host from ``gb_cv_moments``' five sums per
 (fold, tag).  Any other definition (other transformers in a Pipeline, callbacks unless batched as above, LSTM fits with
-callbacks, K-fold detectors unless ``FleetModelBuilder(kfcv=True)`` batches them under a KFold cv through ``fleet.build_kfold_fleet``,
+``validation_split``, K-fold detectors unless ``FleetModelBuilder(kfcv=True)`` batches them under a KFold cv through ``fleet.build_kfold_fleet``,
 custom metrics ...) goes through ``ModelBuilder``: one machine at a time, still on the GPU through the estimators' own fit / predict.
 
 Machines are plain dicts in the layout of ``Machine.to_dict()`` (gordo/machine/machine.py:226-246): ``name``, ``model`` (a
@@ -424,21 +426,28 @@ def _ff_network(est):
     return (est, input_scaler) if type(est) is KerasAutoEncoder else (None, False)
 
 
-def _ff_fit_arguments(ae, early_stopping: bool):
-    """(refusal or None, fit arguments, the one EarlyStopping callback or None, validation_split) of a feed-forward estimator."""
+def _early_stopping(fit_args, early_stopping: bool, flag: str):
+    """(refusal or None, the one EarlyStopping callback or None) of an estimator's fit arguments; ``flag`` names the builder option."""
     from .machine.model.models import build_callbacks
 
+    if not fit_args.get("callbacks"):
+        return None, None
+    if not early_stopping:
+        return f"callbacks need the per-epoch loop (FleetModelBuilder({flag}=True) batches one EarlyStopping)", None
+    definitions = fit_args["callbacks"]
+    definitions = list(definitions) if isinstance(definitions, (list, tuple)) else [definitions]
+    callbacks = build_callbacks(definitions)
+    if len(definitions) != 1 or len(callbacks) != 1:  # several callbacks, or one the fit loop does not know
+        return "callbacks other than one EarlyStopping need the per-epoch loop", None
+    return None, callbacks[0]
+
+
+def _ff_fit_arguments(ae, early_stopping: bool):
+    """(refusal or None, fit arguments, the one EarlyStopping callback or None, validation_split) of a feed-forward estimator."""
     fit_args = ae.extract_supported_fit_args(ae.kwargs)
-    stopping = None
-    if fit_args.get("callbacks"):
-        if not early_stopping:
-            return "callbacks need the per-epoch loop (FleetModelBuilder(early_stopping=True) batches one EarlyStopping)", fit_args, None, 0.0
-        definitions = fit_args["callbacks"]
-        definitions = list(definitions) if isinstance(definitions, (list, tuple)) else [definitions]
-        callbacks = build_callbacks(definitions)
-        if len(definitions) != 1 or len(callbacks) != 1:  # several callbacks, or one the fit loop does not know
-            return "callbacks other than one EarlyStopping need the per-epoch loop", fit_args, None, 0.0
-        stopping = callbacks[0]
+    reason, stopping = _early_stopping(fit_args, early_stopping, "early_stopping")
+    if reason:
+        return reason, fit_args, None, 0.0
     vsplit = float(fit_args.get("validation_split") or 0.0)
     if vsplit and not 0.0 < vsplit < 1.0:
         return f"validation_split {vsplit} is outside (0, 1)", fit_args, stopping, vsplit
@@ -467,7 +476,7 @@ class _CanonicalLSTM(_Canonical):
     def bucket(self):
         s = self.spec
         return (s.key(), tuple(sorted(s.adam.items())), tuple(s.metrics), s.loss, self.lookahead, len(self.X), self.fit["epochs"], self.fit["batch_size"],
-                self.n_splits, int(self.evaluation.get("seed", 0)), self.input_scaler) + optimizer_key(s)
+                self.n_splits, int(self.evaluation.get("seed", 0)), self.input_scaler, self.early_stopping is not None) + optimizer_key(s)  # EarlyStopping's parameters are per-job records
 
 
 def _is_lstm_definition(machine) -> bool:
@@ -485,13 +494,14 @@ def _is_lstm_definition(machine) -> bool:
     return isinstance(est, KerasLSTMBaseEstimator)
 
 
-def _canonical_lstm(index, machine, wide_batches: bool = False) -> Optional[_CanonicalLSTM]:
+def _canonical_lstm(index, machine, wide_batches: bool = False, early_stopping: bool = False) -> Optional[_CanonicalLSTM]:
     """
     The LSTM form of the canonical definition -- ``DiffBasedAnomalyDetector(KerasLSTMAutoEncoder | KerasLSTMForecast)``, the network bare
     or behind one default ``MinMaxScaler``, under the evaluation ``_canonical`` accepts -- as a candidate for the batched path, or
     ``None`` with the reason logged.  Machines too short for the CV folds go to ``ModelBuilder``, which raises the reference's errors.
     ``wide_batches``: also take batch sizes above 32, up to ``LSTMEngine.TC_MAX_BATCH`` (the tensor-core fit family;
-    ``FleetModelBuilder(lstm_wide_batches=True)``).
+    ``FleetModelBuilder(lstm_wide_batches=True)``).  ``early_stopping``: also take an estimator with one Keras ``EarlyStopping``
+    callback on a metric its fit reports, ``loss`` or (with the accuracy metric) ``accuracy`` (``FleetModelBuilder(lstm_early_stopping=True)``).
     """
     from .machine.model.anomaly.diff import DiffBasedAnomalyDetector
     from .engine import LSTMEngine
@@ -527,8 +537,11 @@ def _canonical_lstm(index, machine, wide_batches: bool = False) -> Optional[_Can
     if type(est) not in (KerasLSTMAutoEncoder, KerasLSTMForecast):
         return no("base_estimator is not a KerasLSTMAutoEncoder / KerasLSTMForecast, bare or behind one default MinMaxScaler")
     fit_args = est.extract_supported_fit_args(est.kwargs)
-    if fit_args.get("validation_split") or fit_args.get("callbacks"):
-        return no("validation_split / callbacks need the per-epoch loop")
+    if fit_args.get("validation_split"):
+        return no("validation_split needs the per-machine fit")
+    reason, stopping = _early_stopping(fit_args, early_stopping, "lstm_early_stopping")
+    if reason:
+        return no(reason)
     batch_size = int(est.batch_size)
     if not 1 <= batch_size <= LSTMEngine.FP32_MAX_BATCH and not (wide_batches and 1 <= batch_size <= LSTMEngine.TC_MAX_BATCH):
         if wide_batches:
@@ -548,8 +561,12 @@ def _canonical_lstm(index, machine, wide_batches: bool = False) -> Optional[_Can
     first_train = len(X) - K * test
     if len(X) != len(y) or test <= L + la or first_train <= L or first_train - L + 1 - la < 1:
         return no("too few rows for the CV folds at this lookback_window")
+    reason = _monitor_refusal(stopping, spec, 0.0)  # the generator fit has no validation data
+    if reason:
+        return no(reason)
     fit = {"epochs": int(fit_args.get("epochs", 1)), "batch_size": batch_size, "shuffle": False}
-    return _CanonicalLSTM(index, machine, model, spec, X, y, dataset_meta, query_sec, fit, K, evaluation, input_scaler, lookahead=la)
+    return _CanonicalLSTM(index, machine, model, spec, X, y, dataset_meta, query_sec, fit, K, evaluation, input_scaler, (False, 0.0, None), stopping,
+                          lookahead=la)
 
 
 class _CanonicalKFold(_Canonical):
@@ -658,12 +675,19 @@ class FleetModelBuilder:
     ``lstm_wide_batches``: also batch LSTM machines whose batch_size is above 32 (up to 256), trained by the tensor-core fit
     family (``LSTMEngine.fit_tc``).  Off by default for the same reason: without it such machines build through ``ModelBuilder``,
     whose estimator fit runs the same family one machine at a time.
+
+    ``lstm_early_stopping``: also batch LSTM machines whose estimator has one Keras ``EarlyStopping`` callback on ``loss`` or
+    ``accuracy`` (``_canonical_lstm``).  Every fit applies the rule inside its launch (``fleet.build_lstm_fleet(early_stopping=...)``)
+    and a fit that stops does no further work.  Off by default for the same reason as ``kfcv``: without it such machines build
+    through ``ModelBuilder``, one epoch launch at a time.  It combines with ``lstm_wide_batches``.
     """
 
-    def __init__(self, machines: Sequence, early_stopping: bool = False, kfcv: bool = False, lstm_wide_batches: bool = False):
+    def __init__(self, machines: Sequence, early_stopping: bool = False, kfcv: bool = False, lstm_wide_batches: bool = False,
+                 lstm_early_stopping: bool = False):
         self.early_stopping = bool(early_stopping)
         self.kfcv = bool(kfcv)
         self.lstm_wide_batches = bool(lstm_wide_batches)
+        self.lstm_early_stopping = bool(lstm_early_stopping)
         self.machines = [_machine_dict(m) for m in machines]
         names = [m["name"] for m in self.machines]
         if len(set(names)) != len(names):
@@ -677,14 +701,14 @@ class FleetModelBuilder:
         from . import fleet
 
         return FleetModelBuilder([self.machines[i] for i in fleet.partition(len(self.machines), world)[rank]], early_stopping=self.early_stopping,
-                                 kfcv=self.kfcv, lstm_wide_batches=self.lstm_wide_batches)
+                                 kfcv=self.kfcv, lstm_wide_batches=self.lstm_wide_batches, lstm_early_stopping=self.lstm_early_stopping)
 
     def build(self, output_dir: Optional[str] = None) -> List[Tuple[Any, dict]]:
         results: List[Optional[Tuple[Any, dict]]] = [None] * len(self.machines)
         buckets: Dict[tuple, List[_Canonical]] = {}
         for i, machine in enumerate(self.machines):
             if _is_lstm_definition(machine):
-                c = _canonical_lstm(i, machine, wide_batches=self.lstm_wide_batches)
+                c = _canonical_lstm(i, machine, wide_batches=self.lstm_wide_batches, early_stopping=self.lstm_early_stopping)
             elif self.kfcv and _is_kfcv_definition(machine):
                 c = _canonical_kfcv(i, machine, early_stopping=self.early_stopping)
             else:
@@ -765,7 +789,8 @@ class FleetModelBuilder:
         yd = xd if same_y else engine._torch().from_numpy(np.concatenate([np.ascontiguousarray(c.y.values, dtype=np.float64) for c in members])).to(eng.device)
         fb = fleet.build_lstm_fleet(eng, xd, yd, rows, lookahead=first.lookahead, epochs=first.fit["epochs"], batch_size=first.fit["batch_size"],
                                     n_splits=K, seed=int(first.evaluation.get("seed", 0)), adam=first.spec.adam, input_scaler=first.input_scaler,
-                                    loss=first.spec.loss, optimizer=fit_optimizer(first.spec))
+                                    loss=first.spec.loss, optimizer=fit_optimizer(first.spec),
+                                    early_stopping=None if first.early_stopping is None else [c.early_stopping for c in members])
         engine._torch().cuda.synchronize()
         share = (time.time() - t0) / len(members)  # the bucket's wall time, spread evenly: there is no per-machine time any more
         split_obj = TimeSeriesSplit(n_splits=K)

@@ -17,6 +17,7 @@
 //   Adam      m += (g-m)(1-b1); v += (g^2-v)(1-b2); w -= lr sqrt(1-b2^t)/(1-b1^t) m/(sqrt(v)+eps)   [3P keras]
 // fp32 CUDA cores throughout (a tensor-core path for these GEMMs is the next step for this kernel family).
 #include "gb_common.cuh"
+#include "lstm_fit_stop.cuh"
 
 namespace {
 
@@ -503,9 +504,11 @@ int gb_lstm_fit_loss(const gb_lstmnet* net, float* params, float* adam_m, float*
                          nullptr, stream);
 }
 
-int gb_lstm_fit_opt(const gb_lstmnet* net, float* params, float* adam_m, float* adam_v, int32_t* adam_t, const gb_job* jobs,
-                    int32_t n_jobs, int32_t max_windows, const float* x, const float* y, const gb_lstm_fit_hparams* hp, void* workspace,
-                    float* out_loss, float* out_acc, int32_t loss, const gb_optimizer* opt, void* stream) {
+// gb_lstm_fit_opt (stop NULL: the step graph and launches as they have always been) and gb_lstm_fit_stop
+static int launch_fit(const gb_lstmnet* net, float* params, float* adam_m, float* adam_v, int32_t* adam_t, const gb_job* jobs,
+                      int32_t n_jobs, int32_t max_windows, const float* x, const float* y, const gb_lstm_fit_hparams* hp, void* workspace,
+                      float* out_loss, float* out_acc, int32_t loss, const gb_optimizer* opt, const gb_fit_stop* stop, float* best_params,
+                      int32_t* out_epochs, int32_t* out_best_epoch, void* stream) {
   int rc = validate(net);
   if (rc != GB_OK) return rc;
   if ((rc = gb::validate_optimizer(opt)) != GB_OK) return rc;
@@ -515,6 +518,11 @@ int gb_lstm_fit_opt(const gb_lstmnet* net, float* params, float* adam_m, float* 
   GB_REQUIRE(hp->epochs >= 0 && hp->batch_size >= 1, GB_E_ARG, "epochs=%d batch_size=%d", hp->epochs, hp->batch_size);
   GB_REQUIRE(hp->batch_size <= MAXB, GB_E_SHAPE, "batch_size=%d: this kernel family handles batches of at most %d windows", hp->batch_size, MAXB);
   GB_REQUIRE(hp->lookahead >= 0, GB_E_ARG, "Value of `lookahead` can not be negative, is %d", hp->lookahead);
+  if (stop != nullptr) {
+    GB_REQUIRE(best_params && out_epochs && out_best_epoch, GB_E_ARG, "stop needs best_params, out_epochs and out_best_epoch");
+    GB_REQUIRE(gb::aligned16(best_params), GB_E_ARG, "best_params must be 16-byte aligned");
+    if ((rc = lstm_stop::validate(stop, n_jobs)) != GB_OK) return rc;
+  }
   if (n_jobs == 0) return GB_OK;
   cudaStream_t st = (cudaStream_t)stream;
   FitArgs a{};
@@ -540,22 +548,16 @@ int gb_lstm_fit_opt(const gb_lstmnet* net, float* params, float* adam_m, float* 
 
   int* d_step = reinterpret_cast<int*>(a.hit_sum + n_jobs);
   a.step = d_step;
+  const lstm_stop::Run run(workspace, gb_lstm_fit_workspace_bytes(net, n_jobs), jobs, n_jobs, hp->epochs, out_epochs, out_best_epoch,
+                           params, best_params, a.pstride, n_params);
+  if (stop != nullptr) {
+    run.init(stop, st);
+    a.jobs = run.job_copy;  // a job that stops gets n_rows 0 here, so job_batch gives it no windows
+  }
   // One optimizer step is ~2 600 small launches (18 per timestep): captured once as a CUDA graph and replayed per step, the
   // step's (first window, batch size) being read from device memory -- launch overhead was >90 % of a step for few machines.
-  cudaGraph_t graph = nullptr;
   cudaGraphExec_t gexec = nullptr;
-  cudaStream_t cap = nullptr;  // the caller's stream may be the legacy default stream, which cannot capture
-  GB_CUDA_CHECK(cudaStreamCreateWithFlags(&cap, cudaStreamNonBlocking));
-  {
-    const cudaError_t ce = cudaStreamBeginCapture(cap, cudaStreamCaptureModeThreadLocal);
-    if (ce != cudaSuccess) {
-      cudaStreamDestroy(cap);
-      gb::set_error("cudaStreamBeginCapture failed: %s", cudaGetErrorString(ce));
-      return GB_E_CUDA;
-    }
-  }
-  {
-    cudaStream_t st = cap;  // everything in this block is recorded, not run
+  rc = capture_step(&gexec, stop != nullptr ? run.live : nullptr, [&](cudaStream_t st) {
     for (int t = 0; t < a.L; ++t)
       for (int l = 0; l < a.n_layers; ++l) lstm_fwd_kernel<<<dim3((a.lay[l].u + 15) / 16, n_jobs), 256, 0, st>>>(a, l, t);
     lstm_head_kernel<<<n_jobs, 256, head_smem, st>>>(a);
@@ -575,23 +577,8 @@ int gb_lstm_fit_opt(const gb_lstmnet* net, float* params, float* adam_m, float* 
     else
       lstm_adam_kernel<<<dim3((unsigned)((n_params + 256 * 8 - 1) / (256 * 8)), n_jobs), 256, 0, st>>>(a, n_params);
     lstm_bump_kernel<<<jb, 128, 0, st>>>(a, n_jobs);
-  }
-  {
-    const cudaError_t ce = cudaStreamEndCapture(cap, &graph);
-    cudaStreamDestroy(cap);
-    if (ce != cudaSuccess || graph == nullptr) {
-      gb::set_error("capturing the LSTM optimizer step failed: %s", cudaGetErrorString(ce));
-      return GB_E_CUDA;
-    }
-  }
-  {
-    const cudaError_t ce = cudaGraphInstantiate(&gexec, graph, 0);
-    cudaGraphDestroy(graph);
-    if (ce != cudaSuccess) {
-      gb::set_error("cudaGraphInstantiate failed: %s", cudaGetErrorString(ce));
-      return GB_E_CUDA;
-    }
-  }
+  });
+  if (rc != GB_OK) return rc;
   auto step = [&](int win0, int bsz) -> int {
     lstm_set_step_kernel<<<1, 1, 0, st>>>(d_step, win0, bsz);
     const cudaError_t ce = cudaGraphLaunch(gexec, st);
@@ -610,12 +597,31 @@ int gb_lstm_fit_opt(const gb_lstmnet* net, float* params, float* adam_m, float* 
   for (int e = 0; e < hp->epochs; ++e) {
     for (int w = 0; w < max_windows; w += hp->batch_size)
       if ((rc = step(w, hp->batch_size)) != GB_OK) return rc;
-    lstm_epoch_kernel<<<jb, 128, 0, st>>>(jobs, n_jobs, a.loss_sum, a.hit_sum, out_loss, out_acc, e, hp->epochs);
+    if (stop != nullptr) run.end_epoch(e, a.loss_sum, a.hit_sum, out_loss, out_acc, st);
+    else lstm_epoch_kernel<<<jb, 128, 0, st>>>(jobs, n_jobs, a.loss_sum, a.hit_sum, out_loss, out_acc, e, hp->epochs);
   }
+  if (stop != nullptr) run.finish(st);
   cudaGraphExecDestroy(gexec);  // the enqueued replays keep what they need
   GB_CUDA_CHECK(cudaGetLastError());
   return GB_OK;
 }
+
+int gb_lstm_fit_opt(const gb_lstmnet* net, float* params, float* adam_m, float* adam_v, int32_t* adam_t, const gb_job* jobs,
+                    int32_t n_jobs, int32_t max_windows, const float* x, const float* y, const gb_lstm_fit_hparams* hp, void* workspace,
+                    float* out_loss, float* out_acc, int32_t loss, const gb_optimizer* opt, void* stream) {
+  return launch_fit(net, params, adam_m, adam_v, adam_t, jobs, n_jobs, max_windows, x, y, hp, workspace, out_loss, out_acc, loss, opt,
+                    nullptr, nullptr, nullptr, nullptr, stream);
+}
+
+int gb_lstm_fit_stop(const gb_lstmnet* net, float* params, float* adam_m, float* adam_v, int32_t* adam_t, const gb_job* jobs,
+                     int32_t n_jobs, int32_t max_windows, const float* x, const float* y, const gb_lstm_fit_hparams* hp, void* workspace,
+                     float* out_loss, float* out_acc, int32_t loss, const gb_optimizer* opt, const gb_fit_stop* stop, float* best_params,
+                     int32_t* out_epochs, int32_t* out_best_epoch, void* stream) {
+  return launch_fit(net, params, adam_m, adam_v, adam_t, jobs, n_jobs, max_windows, x, y, hp, workspace, out_loss, out_acc, loss, opt,
+                    stop, best_params, out_epochs, out_best_epoch, stream);
+}
+
+size_t gb_lstm_fit_stop_state_bytes(int32_t n_jobs) { return n_jobs < 0 ? 0 : lstm_stop::state_bytes(n_jobs); }
 
 int gb_orthonormal_rows(double* g, int32_t n_mats, int32_t rows, int32_t cols, float* out, int64_t out_offset, int64_t out_stride,
                         void* stream) {

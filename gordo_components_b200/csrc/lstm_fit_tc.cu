@@ -21,6 +21,7 @@
 // row order, and the slice sums added in slice order.  No atomics: every launch is deterministic.
 #include "gb_common.cuh"
 #include "gb_sm90.cuh"
+#include "lstm_fit_stop.cuh"
 
 namespace {
 
@@ -563,9 +564,11 @@ int gb_lstm_fit_tc(const gb_lstmnet* net, float* params, float* adam_m, float* a
                             nullptr, stream);
 }
 
-int gb_lstm_fit_tc_opt(const gb_lstmnet* net, float* params, float* adam_m, float* adam_v, int32_t* adam_t, const gb_job* jobs,
-                       int32_t n_jobs, int32_t max_windows, const float* x, const float* y, const gb_lstm_fit_hparams* hp, void* workspace,
-                       float* out_loss, float* out_acc, int32_t loss, const gb_optimizer* opt, void* stream) {
+// gb_lstm_fit_tc_opt (stop NULL: the step graph and launches as they have always been) and gb_lstm_fit_tc_stop
+static int launch_fit(const gb_lstmnet* net, float* params, float* adam_m, float* adam_v, int32_t* adam_t, const gb_job* jobs,
+                      int32_t n_jobs, int32_t max_windows, const float* x, const float* y, const gb_lstm_fit_hparams* hp, void* workspace,
+                      float* out_loss, float* out_acc, int32_t loss, const gb_optimizer* opt, const gb_fit_stop* stop, float* best_params,
+                      int32_t* out_epochs, int32_t* out_best_epoch, void* stream) {
   int rc = validate(net);
   if (rc != GB_OK) return rc;
   if ((rc = gb::validate_optimizer(opt)) != GB_OK) return rc;
@@ -576,6 +579,11 @@ int gb_lstm_fit_tc_opt(const gb_lstmnet* net, float* params, float* adam_m, floa
   GB_REQUIRE(hp->batch_size <= MAX_BATCH, GB_E_SHAPE, "batch_size=%d: the tensor-core LSTM fit handles batches of at most %d windows",
              hp->batch_size, MAX_BATCH);
   GB_REQUIRE(hp->lookahead >= 0, GB_E_ARG, "Value of `lookahead` can not be negative, is %d", hp->lookahead);
+  if (stop != nullptr) {
+    GB_REQUIRE(best_params && out_epochs && out_best_epoch, GB_E_ARG, "stop needs best_params, out_epochs and out_best_epoch");
+    GB_REQUIRE(gb::aligned16(best_params), GB_E_ARG, "best_params must be 16-byte aligned");
+    if ((rc = lstm_stop::validate(stop, n_jobs)) != GB_OK) return rc;
+  }
   if (n_jobs == 0) return GB_OK;
   cudaStream_t st = (cudaStream_t)stream;
   FitArgs a{};
@@ -601,21 +609,15 @@ int gb_lstm_fit_tc_opt(const gb_lstmnet* net, float* params, float* adam_m, floa
 
   int* d_step = reinterpret_cast<int*>(a.hit_sum + n_jobs);
   a.step = d_step;
-  // the launch sequence of one optimizer step, captured once and replayed per step as in gb_lstm_fit_loss
-  cudaGraph_t graph = nullptr;
-  cudaGraphExec_t gexec = nullptr;
-  cudaStream_t cap = nullptr;
-  GB_CUDA_CHECK(cudaStreamCreateWithFlags(&cap, cudaStreamNonBlocking));
-  {
-    const cudaError_t ce = cudaStreamBeginCapture(cap, cudaStreamCaptureModeThreadLocal);
-    if (ce != cudaSuccess) {
-      cudaStreamDestroy(cap);
-      gb::set_error("cudaStreamBeginCapture failed: %s", cudaGetErrorString(ce));
-      return GB_E_CUDA;
-    }
+  const lstm_stop::Run run(workspace, gb_lstm_fit_tc_workspace_bytes(net, n_jobs, hp->batch_size), jobs, n_jobs, hp->epochs, out_epochs,
+                           out_best_epoch, params, best_params, a.pstride, n_params);
+  if (stop != nullptr) {
+    run.init(stop, st);
+    a.jobs = run.job_copy;  // a job that stops gets n_rows 0 here, so job_batch gives it no windows
   }
-  {
-    cudaStream_t st = cap;  // everything in this block is recorded, not run
+  // the launch sequence of one optimizer step, captured once and replayed per step as in gb_lstm_fit_loss
+  cudaGraphExec_t gexec = nullptr;
+  rc = capture_step(&gexec, stop != nullptr ? run.live : nullptr, [&](cudaStream_t st) {
     for (int t = 0; t < a.L; ++t)
       for (int l = 0; l < a.n_layers; ++l) tc_fwd_kernel<<<dim3((a.lay[l].u + 15) / 16, nbt, n_jobs), 128, 0, st>>>(a, l, t);
     tc_head_rows_kernel<<<dim3(a.Bp / HEAD_ROWS, n_jobs), 256, head_smem, st>>>(a);
@@ -636,23 +638,8 @@ int gb_lstm_fit_tc_opt(const gb_lstmnet* net, float* params, float* adam_m, floa
     else
       tc_adam_kernel<<<dim3((unsigned)((n_params + 256 * 8 - 1) / (256 * 8)), n_jobs), 256, 0, st>>>(a, n_params);
     tc_bump_kernel<<<jb, 128, 0, st>>>(a, n_jobs);
-  }
-  {
-    const cudaError_t ce = cudaStreamEndCapture(cap, &graph);
-    cudaStreamDestroy(cap);
-    if (ce != cudaSuccess || graph == nullptr) {
-      gb::set_error("capturing the LSTM optimizer step failed: %s", cudaGetErrorString(ce));
-      return GB_E_CUDA;
-    }
-  }
-  {
-    const cudaError_t ce = cudaGraphInstantiate(&gexec, graph, 0);
-    cudaGraphDestroy(graph);
-    if (ce != cudaSuccess) {
-      gb::set_error("cudaGraphInstantiate failed: %s", cudaGetErrorString(ce));
-      return GB_E_CUDA;
-    }
-  }
+  });
+  if (rc != GB_OK) return rc;
   auto step = [&](int win0, int bsz) -> int {
     tc_set_step_kernel<<<1, 1, 0, st>>>(d_step, win0, bsz);
     const cudaError_t ce = cudaGraphLaunch(gexec, st);
@@ -672,11 +659,28 @@ int gb_lstm_fit_tc_opt(const gb_lstmnet* net, float* params, float* adam_m, floa
   for (int e = 0; e < hp->epochs; ++e) {
     for (int w = 0; w < max_windows; w += hp->batch_size)
       if ((rc = step(w, hp->batch_size)) != GB_OK) return rc;
-    tc_epoch_kernel<<<jb, 128, 0, st>>>(jobs, n_jobs, a.loss_sum, a.hit_sum, out_loss, out_acc, e, hp->epochs);
+    if (stop != nullptr) run.end_epoch(e, a.loss_sum, a.hit_sum, out_loss, out_acc, st);
+    else tc_epoch_kernel<<<jb, 128, 0, st>>>(jobs, n_jobs, a.loss_sum, a.hit_sum, out_loss, out_acc, e, hp->epochs);
   }
+  if (stop != nullptr) run.finish(st);
   cudaGraphExecDestroy(gexec);  // the enqueued replays keep what they need
   GB_CUDA_CHECK(cudaGetLastError());
   return GB_OK;
+}
+
+int gb_lstm_fit_tc_opt(const gb_lstmnet* net, float* params, float* adam_m, float* adam_v, int32_t* adam_t, const gb_job* jobs,
+                       int32_t n_jobs, int32_t max_windows, const float* x, const float* y, const gb_lstm_fit_hparams* hp, void* workspace,
+                       float* out_loss, float* out_acc, int32_t loss, const gb_optimizer* opt, void* stream) {
+  return launch_fit(net, params, adam_m, adam_v, adam_t, jobs, n_jobs, max_windows, x, y, hp, workspace, out_loss, out_acc, loss, opt,
+                    nullptr, nullptr, nullptr, nullptr, stream);
+}
+
+int gb_lstm_fit_tc_stop(const gb_lstmnet* net, float* params, float* adam_m, float* adam_v, int32_t* adam_t, const gb_job* jobs,
+                        int32_t n_jobs, int32_t max_windows, const float* x, const float* y, const gb_lstm_fit_hparams* hp, void* workspace,
+                        float* out_loss, float* out_acc, int32_t loss, const gb_optimizer* opt, const gb_fit_stop* stop, float* best_params,
+                        int32_t* out_epochs, int32_t* out_best_epoch, void* stream) {
+  return launch_fit(net, params, adam_m, adam_v, adam_t, jobs, n_jobs, max_windows, x, y, hp, workspace, out_loss, out_acc, loss, opt,
+                    stop, best_params, out_epochs, out_best_epoch, stream);
 }
 
 }  // extern "C"

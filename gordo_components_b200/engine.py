@@ -627,10 +627,39 @@ class LSTMEngine:
         return self._fit_launch(entry, ws_bytes, params, jobs_dev, n_jobs, max_windows, x, y, epochs, batch_size,
                                 lookahead, primer, adam, state, loss, optimizer)
 
+    def fit_stop(self, params, jobs_dev, n_jobs, max_windows, x, y, stop, epochs: int = 1, batch_size: int = 32, lookahead: int = 0,
+                 primer: bool = True, adam: Optional[Dict[str, float]] = None, state=None, loss: str = "mse", optimizer=None):
+        """
+        ``fit_for_batch(batch_size)`` with Keras' EarlyStopping inside the launch (gb_lstm_fit_stop, or gb_lstm_fit_tc_stop above
+        FP32_MAX_BATCH windows): every job applies its rule at the end of each epoch, a job that stops does no further work, and
+        with ``restore_best_weights`` its slot of ``params`` ends with the weights of its best epoch.  ``stop``: ``make_stop``
+        records, one per job (a host array).  Returns (loss, accuracy, epochs_run, best_epoch, (m, v, t)): epochs_run / best_epoch
+        are int32 [n_jobs] (best_epoch -1 when no epoch improved and no snapshot was taken), and every history entry past a job's
+        epochs_run is NaN.  The other arguments and (m, v, t) are ``fit``'s.
+        """
+        torch = _torch()
+        if not 1 <= int(batch_size) <= self.TC_MAX_BATCH:
+            raise ValueError(f"batch_size={int(batch_size)}: the LSTM fit handles batches of 1 to {self.TC_MAX_BATCH} windows")
+        stop = np.ascontiguousarray(stop, dtype=_cabi.STOP_DTYPE)
+        if stop.shape != (int(n_jobs),):
+            raise ValueError(f"stop holds {stop.shape} records for {int(n_jobs)} jobs")
+        tc = int(batch_size) > self.FP32_MAX_BATCH
+        ws_bytes = self.fit_workspace_bytes_for_batch(n_jobs, batch_size) + int(self.lib.gb_lstm_fit_stop_state_bytes(int(n_jobs)))
+        entry = self.lib.gb_lstm_fit_tc_stop if tc else self.lib.gb_lstm_fit_stop
+        epochs_run = torch.zeros((int(n_jobs),), dtype=torch.int32, device=self.device)
+        best_epoch = torch.full((int(n_jobs),), -1, dtype=torch.int32, device=self.device)
+        best = torch.empty_like(params)  # snapshot area
+        hist, acc, st = self._fit_launch(entry, ws_bytes, params, jobs_dev, n_jobs, max_windows, x, y, epochs, batch_size, lookahead, primer,
+                                         adam, state, loss, optimizer, stop=(stop, best, epochs_run, best_epoch))
+        return hist, acc, epochs_run, best_epoch, st
+
     def _fit_launch(self, entry, ws_bytes, params, jobs_dev, n_jobs, max_windows, x, y, epochs, batch_size, lookahead, primer, adam, state,
-                    loss, optimizer=None):
+                    loss, optimizer=None, stop=None):
         code = _cabi.loss_code(loss)
         opt = () if optimizer is None else (C.byref(_cabi.make_optimizer(*optimizer)),)
+        if stop is not None:  # the _stop entry points always take the optimizer argument, then the rule's arrays
+            records, best, epochs_run, best_epoch = stop
+            opt = (opt[0] if opt else None, records.ctypes.data_as(C.c_void_p), _cabi.ptr(best), _cabi.ptr(epochs_run), _cabi.ptr(best_epoch))
         torch = _torch()
         adam = adam or {}
         hp = _cabi.GbLstmFitHParams()
@@ -646,8 +675,9 @@ class LSTMEngine:
         ws = torch.empty((ws_bytes + 3) // 4, dtype=torch.float32, device=self.device)
         # a primer-only fit (epochs = 0) writes no history, but the kernel takes the outputs as non-NULL pointers and a tensor with
         # no elements has none: the buffers keep one column and the caller gets the empty slice
-        hist = torch.zeros((n_jobs, max(epochs, 1)), dtype=torch.float32, device=self.device)
-        acc = torch.zeros((n_jobs, max(epochs, 1)), dtype=torch.float32, device=self.device)
+        fill = 0.0 if stop is None else float("nan")  # with a stop rule, the entries past a job's epochs_run stay NaN
+        hist = torch.full((n_jobs, max(epochs, 1)), fill, dtype=torch.float32, device=self.device)
+        acc = torch.full((n_jobs, max(epochs, 1)), fill, dtype=torch.float32, device=self.device)
         p = _cabi.ptr
         _cabi.check(entry(C.byref(self.net), p(params), p(m), p(v), p(t), p(jobs_dev), int(n_jobs), int(max_windows), p(x), p(y), C.byref(hp),
                           p(ws), p(hist), p(acc), code, *opt, _stream_ptr()))

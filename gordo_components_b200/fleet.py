@@ -470,7 +470,12 @@ class LSTMFleetBuild:
 
     def __init__(self, eng, n_machines, n_splits, rows, lookahead, batch_size, starts, n_test, params, fold_params, init_params, loss, acc,
                  fold_loss, fold_acc, y_min, y_max, fold_y_min, fold_y_max, feat_thr, agg_thr, fold_feat_thr, fold_agg_thr, cv_moments,
-                 fold_predictions, in_min=None, in_max=None, fold_in_min=None, fold_in_max=None):
+                 fold_predictions, in_min=None, in_max=None, fold_in_min=None, fold_in_max=None, epochs=None, epochs_run=None, best_epoch=None,
+                 fold_epochs_run=None, fold_best_epoch=None):
+        # EarlyStopping: epochs each fit ran and its best epoch (-1: none) ([M]; per CV fold [M, K]) as int32 host arrays; None without
+        # the callback.  History entries past a fit's epochs_run are NaN.  `epochs` is the configured count (History.params["epochs"]).
+        self.epochs = epochs
+        self.epochs_run, self.best_epoch, self.fold_epochs_run, self.fold_best_epoch = epochs_run, best_epoch, fold_epochs_run, fold_best_epoch
         self.eng, self.n_machines, self.n_splits, self.rows = eng, n_machines, n_splits, rows
         self.lookahead, self.batch_size = lookahead, batch_size
         self.steps_per_epoch = math.ceil((rows - eng.lookback + 1 - lookahead) / batch_size)  # of the final fit (History.params["steps"])
@@ -527,7 +532,12 @@ class LSTMFleetBuild:
         hist = {"loss": [float(v) for v in self.loss[m]]}
         if "accuracy" in spec.metrics:
             hist["accuracy"] = [float(v) for v in self.acc[m]]
-        lstm._history = History(hist, {"verbose": 0, "epochs": len(hist["loss"]), "steps": self.steps_per_epoch}, list(range(len(hist["loss"]))))
+        if self.epochs_run is None:
+            lstm._history = History(hist, {"verbose": 0, "epochs": len(hist["loss"]), "steps": self.steps_per_epoch}, list(range(len(hist["loss"]))))
+        else:  # as the per-machine fit loop leaves it: the epochs run, against the configured count
+            ran = int(self.epochs_run[m])
+            hist = {k: v[:ran] for k, v in hist.items()}
+            lstm._history = History(hist, {"verbose": 0, "epochs": int(self.epochs), "steps": self.steps_per_epoch}, list(range(ran)))
         lstm.model.history = lstm._history
         _fill_minmax_from_extrema(det.scaler, self.y_min[m], self.y_max[m], self.rows, tags)
         det.feature_thresholds_ = pd.Series(self.feat_thr[m].copy(), index=tags, name=f"fold-{K - 1}")
@@ -543,7 +553,7 @@ class LSTMFleetBuild:
 
 def build_lstm_fleet(eng: "engine.LSTMEngine", x, y, rows: int, lookahead: int = 0, epochs: int = 1, batch_size: int = 32, n_splits: int = 3,
                      seed: int = 0, adam: Optional[Dict[str, float]] = None, input_scaler: bool = False, memory_budget: int = 8 << 30,
-                     keep_init_params: bool = False, generator=None, loss: str = "mse", optimizer=None) -> LSTMFleetBuild:
+                     keep_init_params: bool = False, generator=None, loss: str = "mse", optimizer=None, early_stopping=None) -> LSTMFleetBuild:
     """
     The batched ``gordo build`` of one bucket of LSTM machines (``DiffBasedAnomalyDetector(KerasLSTMAutoEncoder | KerasLSTMForecast)``,
     the network bare or behind one MinMaxScaler): for every machine the TimeSeriesSplit cross validation and the final fit, as
@@ -558,6 +568,11 @@ def build_lstm_fleet(eng: "engine.LSTMEngine", x, y, rows: int, lookahead: int =
     trained in chunks that fit it -- all ``n_splits + 1`` fits of a machine in the same chunk; every job's result is the same
     whatever the chunking.  ``keep_init_params``: keep the initial parameters of every slot on the result (``init_params``).
     ``loss``: the estimator's canonical Keras loss name (``LSTMNetSpec.loss``).  ``optimizer``: as in ``build_fleet``.
+    ``early_stopping``: the estimator's Keras ``EarlyStopping`` callback -- one for every machine, or a sequence of one per machine
+    (``engine.make_stop`` takes any form).  Every slot of machine m, the final fit and each CV fold, applies m's rule at the end of
+    each of its epochs inside the fit launch (``LSTMEngine.fit_stop``), as sklearn's clone hands every fold the same callbacks.  The
+    result then carries ``epochs_run`` / ``best_epoch``; history entries past a fit's ``epochs_run`` are NaN.  With
+    ``restore_best_weights`` the launch also holds a snapshot of every slot, which ``memory_budget`` counts.
     """
     torch = engine._torch()
     dev = eng.device
@@ -612,7 +627,18 @@ def build_lstm_fleet(eng: "engine.LSTMEngine", x, y, rows: int, lookahead: int =
     # fits: chunks of whole machines (final + K folds) whose workspace fits the budget
     # (batches above 32 windows train on the tensor-core family, whose workspace grows with the batch)
     fit = eng.fit_for_batch(batch_size)
-    chunk = max(1, min(M, int(memory_budget) // max(eng.fit_workspace_bytes_for_batch(K + 1, batch_size), 1), 65535 // (K + 1)))
+    per_machine_bytes = eng.fit_workspace_bytes_for_batch(K + 1, batch_size)
+    stop = epochs_run = best_epoch = None
+    if early_stopping is not None:
+        per_machine = list(early_stopping) if isinstance(early_stopping, (list, tuple)) else [early_stopping] * M
+        if len(per_machine) != M:
+            raise ValueError(f"early_stopping: {len(per_machine)} callbacks for {M} machines")
+        stop = engine.make_stop([per_machine[s % M] for s in range(S)])  # slot s belongs to machine s mod M
+        per_machine_bytes += int(eng.lib.gb_lstm_fit_stop_state_bytes(K + 1))
+        if stop["restore_best"].any():  # the snapshot area
+            per_machine_bytes += (K + 1) * eng.param_stride * 4
+        epochs_run, best_epoch = np.zeros(S, np.int32), np.zeros(S, np.int32)
+    chunk = max(1, min(M, int(memory_budget) // max(per_machine_bytes, 1), 65535 // (K + 1)))
     hist = torch.empty((S, epochs), dtype=torch.float32, device=dev)
     acc = torch.empty_like(hist)
     for m0 in range(0, M, chunk):
@@ -621,8 +647,13 @@ def build_lstm_fleet(eng: "engine.LSTMEngine", x, y, rows: int, lookahead: int =
         idx = torch.from_numpy(slots).to(dev)
         p = params.index_select(0, idx)
         jobs = engine.jobs_to_device(engine.make_jobs(np.arange(len(slots)), slot_windows[slots], x_row[slots]), dev)
-        cl, ca, _ = fit(p, jobs, len(slots), int(slot_windows[slots].max()), xf, yf, epochs=epochs, batch_size=batch_size, lookahead=la,
-                        primer=True, adam=adam, loss=loss, optimizer=optimizer)
+        args = (p, jobs, len(slots), int(slot_windows[slots].max()), xf, yf)
+        kw = dict(epochs=epochs, batch_size=batch_size, lookahead=la, primer=True, adam=adam, loss=loss, optimizer=optimizer)
+        if stop is None:
+            cl, ca, _ = fit(*args, **kw)
+        else:
+            cl, ca, er, be, _ = eng.fit_stop(*args, stop[slots], **kw)
+            epochs_run[slots], best_epoch[slots] = host(er), host(be)
         params.index_copy_(0, idx, p)
         hist.index_copy_(0, idx, cl)
         acc.index_copy_(0, idx, ca)
@@ -655,7 +686,10 @@ def build_lstm_fleet(eng: "engine.LSTMEngine", x, y, rows: int, lookahead: int =
         np.ascontiguousarray(fold_feat[:, K - 1]), np.ascontiguousarray(fold_agg[:, K - 1]), np.ascontiguousarray(fold_feat),
         np.ascontiguousarray(fold_agg), np.ascontiguousarray(moments), pred.view(K, M, n_test, T).permute(1, 0, 2, 3),
         in_min=None if in_lo is None else in_lo[:M], in_max=None if in_hi is None else in_hi[:M],
-        fold_in_min=None if in_lo is None else folds(in_lo), fold_in_max=None if in_hi is None else folds(in_hi))
+        fold_in_min=None if in_lo is None else folds(in_lo), fold_in_max=None if in_hi is None else folds(in_hi), epochs=int(epochs),
+        epochs_run=None if stop is None else epochs_run[:M], best_epoch=None if stop is None else best_epoch[:M],
+        fold_epochs_run=None if stop is None else epochs_run[M:].reshape(K, M).T.copy(),
+        fold_best_epoch=None if stop is None else best_epoch[M:].reshape(K, M).T.copy())
 
 
 # ------------------------------------------------------------------------------------------------ fleet build of K-fold detectors

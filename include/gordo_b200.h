@@ -443,6 +443,37 @@ int gb_lstm_fit_tc_opt(const gb_lstmnet* net, float* params, float* adam_m, floa
                        const gb_job* jobs, int32_t n_jobs, int32_t max_windows, const float* x, const float* y,
                        const gb_lstm_fit_hparams* hp, void* workspace, float* out_loss, float* out_acc, int32_t loss,
                        const gb_optimizer* opt, void* stream);
+/* gb_lstm_fit_opt / gb_lstm_fit_tc_opt with Keras' EarlyStopping callback (keras 3 EarlyStopping.on_epoch_end; models.py
+ * EarlyStopping.update), applied by every job at the end of each of its epochs, inside the call, as the per-machine fit loop applies
+ * it after each one-epoch launch (the primer step is not an epoch; epochs count from 0).  The monitored value is the float32
+ * history entry the epoch wrote, widened to double; "better" is v + min_delta < best (mode +1) or v - min_delta > best (mode -1),
+ * in double, so a NaN never improves.  Epochs below start_from_epoch are skipped.  With restore_best, the first epoch that is not
+ * skipped takes a snapshot, and so does every improvement; `wait` counts the epochs since the last improvement that also beat the
+ * baseline; the job stops after the epoch at which wait >= patience and epoch > 0.  From then on it does no work: its params,
+ * optimizer state and step count stay as the last epoch it ran left them, and once every job has stopped the remaining steps
+ * skip their kernels.  At the end, with restore_best and a snapshot, params get the snapshot, whether or not the job stopped
+ * early; the optimizer state is that of the last epoch run.  The LSTM fit reports loss and accuracy only, so a val_* monitor
+ * (2, 3) is unavailable: the job never stops and takes no snapshot.
+ * stop: [n_jobs] *host* array of gb_fit_stop, read before the call returns, or NULL (then this is the _opt entry point, bit for
+ * bit).  With a stop array the workspace is gb_lstm_fit_workspace_bytes(net, n_jobs) (gb_lstm_fit_tc_stop:
+ * gb_lstm_fit_tc_workspace_bytes(net, n_jobs, batch_size)) + gb_lstm_fit_stop_state_bytes(n_jobs) bytes: the rule's per-job
+ * state lives at its end.  best_params: [n_slots][param_stride] device, 16-byte aligned, the snapshot area (overwritten where
+ * snapshots are taken).  out_epochs: [n_jobs] device, epochs each job ran; history entries past it are left as they are.
+ * out_best_epoch: [n_jobs] device, the epoch of the best monitored value (with restore_best: the snapshot's), -1 when no epoch
+ * improved and no snapshot was taken.  GB_E_ARG, nothing enqueued and no device needed: NULL best_params, out_epochs or
+ * out_best_epoch with a stop array, a misaligned best_params, a monitor outside 0..3, a mode other than +1 / -1, a negative
+ * patience or a negative min_delta. */
+size_t gb_lstm_fit_stop_state_bytes(int32_t n_jobs);
+int gb_lstm_fit_stop(const gb_lstmnet* net, float* params, float* adam_m, float* adam_v, int32_t* adam_t,
+                     const gb_job* jobs, int32_t n_jobs, int32_t max_windows, const float* x, const float* y,
+                     const gb_lstm_fit_hparams* hp, void* workspace, float* out_loss, float* out_acc, int32_t loss,
+                     const gb_optimizer* opt, const gb_fit_stop* stop, float* best_params, int32_t* out_epochs,
+                     int32_t* out_best_epoch, void* stream);
+int gb_lstm_fit_tc_stop(const gb_lstmnet* net, float* params, float* adam_m, float* adam_v, int32_t* adam_t,
+                        const gb_job* jobs, int32_t n_jobs, int32_t max_windows, const float* x, const float* y,
+                        const gb_lstm_fit_hparams* hp, void* workspace, float* out_loss, float* out_acc, int32_t loss,
+                        const gb_optimizer* opt, const gb_fit_stop* stop, float* best_params, int32_t* out_epochs,
+                        int32_t* out_best_epoch, void* stream);
 
 /* Keras' Orthogonal initialiser for recurrent kernels: g holds n_mats standard-normal [rows][cols] draws (float64, rows <= cols,
  * overwritten); matrix i's rows are orthonormalised (Gram-Schmidt, the sign convention of Keras' QR) and written as float32 to
