@@ -429,7 +429,9 @@ __global__ void __launch_bounds__(THREADS, 1) ffae_fit_kernel(const FitArgs a) {
               const float ao = yh[r * yp + j], t = yt[r * a.ypitch + j];
               if (loss == GB_LOSS_MSE) {
                 const float d = ao - t;
-                acc_sq += d * d;
+                // one fused multiply-add, pinned: in the LOSS kernels the compiler may otherwise merge the two branches' sums into
+                // one add of a separately rounded d * d, and an MSE fit's loss there would differ in the last bits from the MSE kernels'
+                acc_sq = __fmaf_rn(d, d, acc_sq);
                 g = gscale * d;
               } else {
                 acc_sq += gb::loss_value(loss, ao, t);

@@ -1,6 +1,7 @@
 """
-The Keras regression losses on the training kernels: gb_ffae_fit (every memory plan, and the split / stop entry points) and
-gb_lstm_fit_loss against the loss oracle (tests/loss_oracle.py) from injected weights and visiting order; the edge cases of the
+The Keras regression losses on the training kernels: gb_ffae_fit in every memory plan at batches of 32 and 80 rows and
+gb_ffae_fit_split in every memory plan through a row map with a held-out tail, the split / stop entry points on a small stack, and
+gb_lstm_fit_loss, against the loss oracle (tests/loss_oracle.py) from injected weights and visiting order; the edge cases of the
 loss table (sign(0) = 0, MSLE below eps, MAPE near 0, Huber on both sides of delta); mean squared error bit-identical to the
 default call; and the loss through the estimators and the three batched fleet builds.
 """
@@ -12,7 +13,7 @@ import numpy as np
 import pandas as pd
 import pytest
 from loss_oracle import LOSSES
-from parity_helpers import close, random_net
+from parity_helpers import ENTRIES, close, crossed, ff_split_run, random_net
 
 pytestmark = pytest.mark.gpu
 
@@ -89,13 +90,16 @@ def ff_run(engine, torch, spec, w0s, X, Y, N, E, B, perm, adam, loss):
     return eng, eng.unpack_params(params), hist.cpu().numpy(), acc.cpu().numpy(), m.cpu().numpy(), v.cpu().numpy()
 
 
-def check_ff(lo, spec, w0s, Xs, Ys, perm, res, E, B, adam, loss, gradients=False, atol_w=0.0):
-    eng, got, hist, acc, m, v = res
+def check_ff(lo, spec, w0s, Xs, Ys, perm, res, E, B, adam, loss, gradients=False, atol_w=0.0, n_val=0):
+    """With n_val, Xs / Ys are the jobs' positions (training, then n_val held out) and res ends with val_loss / val_accuracy."""
+    eng, got, hist, acc, m, v, *val = res
     for j in range(len(w0s)):
-        n = len(Xs[j])
+        n = len(Xs[j]) - n_val
+        vsplit = n_val / len(Xs[j])
+        assert math.floor(len(Xs[j]) * (1.0 - vsplit)) == n  # the oracle's split is the launch's
         w_ref, h_ref, st = lo.ff_fit(spec, w0s[j], Xs[j], Ys[j], epochs=E, batch_size=B, perms=[perm[j, e, :n] for e in range(E)],
                                      lr=adam["lr"], b1=adam["beta1"], b2=adam["beta2"], eps=adam["eps"],
-                                     dtype=np.float64 if gradients else np.float32, loss=loss)
+                                     dtype=np.float64 if gradients else np.float32, loss=loss, validation_split=vsplit)
         for l, ((Wg, bg), (Wr, br), (W0, b0)) in enumerate(zip(got[j], w_ref, w0s[j])):
             if gradients:
                 for g_, r_, z_, what in ((Wg, Wr, W0, "W"), (bg, br, b0, "b")):
@@ -111,33 +115,43 @@ def check_ff(lo, spec, w0s, Xs, Ys, perm, res, E, B, adam, loss, gradients=False
                     close(sb, rb, mag=mag, rtol=1e-3, atol=1e-4 * mag, name=f"{loss} job {j} Adam {what} b{l}")
         close(hist[j], np.array(h_ref["loss"]), mag=0.0, rtol=5e-4, name=f"{loss} job {j} loss history")
         close(acc[j], np.array(h_ref["accuracy"]), mag=0, rtol=0, atol=2.0 / n, name=f"{loss} job {j} accuracy history")
+        if n_val:
+            close(val[0][j], np.array(h_ref["val_loss"]), mag=0.0, rtol=5e-4, name=f"{loss} job {j} val_loss history")
+            close(val[1][j], np.array(h_ref["val_accuracy"]), mag=0, rtol=0, atol=2.0 / n_val, name=f"{loss} job {j} val_accuracy history")
 
 
 # (weights in L2, dz buffers in L2) of the five fit plans (tests/test_fit_plan.py pins these shapes to them)
 PLANS = {"smem": ("hourglass", 64), "w_l2": ("symmetric", 10), "dz1": ("symmetric", 64), "dz2": ("symmetric", 96), "dz3": ("symmetric", 128)}
 
 
-@pytest.mark.parametrize("plan", list(PLANS))
+@pytest.mark.parametrize("plan,entry", crossed(PLANS, ENTRIES))
 @pytest.mark.parametrize("loss", LOSSES)
-def test_every_loss_in_every_memory_plan(engine, torch, km, lo, loss, plan):
+def test_every_loss_in_every_memory_plan(engine, torch, km, lo, loss, plan, entry):
     """Targets 3x - 0.3 of the inputs (0.12 .. 2.3): errors on both sides of the Huber delta, negative outputs.  Targets near 0, where
-    one MAPE term outweighs the rest of the batch, have their own test."""
+    one MAPE term outweighs the rest of the batch, have their own test.  At batch 80 the last mini-batch of an epoch is partial too
+    (170 = 80 + 80 + 10 rows); the split launch holds out 40 positions, one held-out batch of two chunks."""
     kind, T = PLANS[plan]
     spec = km.ff_hourglass_spec(T) if kind == "hourglass" else km.ff_symmetric_spec(T)
-    M, N, E, B = 2, 70, 2, 32
+    split, B = entry
+    M, N, E, NV = 2, 70 if B == 32 else 170, 2, 40 if split else 0
     atol_w = 0.0
     if loss in ("mae", "mape"):
         # sign(e) of an element within rounding of 0 can differ from the oracle's: two steps only.  And a gradient that is the
         # small residue of many +-100/|y| terms keeps few digits: a weight may end up to 1/50 of its two Adam steps apart.
-        N, E = 64, 1
+        N, E = 2 * B, 1
         atol_w = 0.02 * KERAS_ADAM["lr"] * 2
     rng = np.random.default_rng(T)
-    Xs = [waves(rng, N, T) for _ in range(M)]
+    Xs = [waves(rng, N + NV, T) for _ in range(M)]
     Ys = [3 * x - 0.3 for x in Xs]
     w0s = [random_net(km, spec.dims, 5 + m, spec.acts)[1] for m in range(M)]
     perm = perms(M, E, N, seed=T)
-    res = ff_run(engine, torch, spec, w0s, np.concatenate(Xs), np.concatenate(Ys), N, E, B, perm, KERAS_ADAM, loss)
-    check_ff(lo, spec, w0s, Xs, Ys, perm, res, E, B, KERAS_ADAM, loss, atol_w=atol_w)
+    if split:
+        maps = [np.random.default_rng(50 + m).permutation(N + NV) for m in range(M)]
+        res = ff_split_run(engine, torch, spec, w0s, Xs, Ys, maps, NV, E, B, perm, adam=KERAS_ADAM, loss=loss)
+        Xs, Ys = [x[mp] for x, mp in zip(Xs, maps)], [y[mp] for y, mp in zip(Ys, maps)]  # the gathered copies
+    else:
+        res = ff_run(engine, torch, spec, w0s, np.concatenate(Xs), np.concatenate(Ys), N, E, B, perm, KERAS_ADAM, loss)
+    check_ff(lo, spec, w0s, Xs, Ys, perm, res, E, B, KERAS_ADAM, loss, atol_w=atol_w, n_val=NV)
 
 
 @pytest.mark.parametrize("loss", LOSSES)

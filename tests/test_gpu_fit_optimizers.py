@@ -1,9 +1,10 @@
 """
-The Keras optimizers on the training kernels: gb_ffae_fit_opt in every memory plan (plain, split and stop launches), gb_lstm_fit_opt
-and gb_lstm_fit_tc_opt against the optimizer oracle (tests/optimizer_oracle.py) from injected weights and visiting order, on the
-weights, both state slots and the history; clipvalue on the summed gradient of a mini-batch above 32 rows; weight decay; padded
-lanes; per-epoch launches equal to one launch; NULL and plain Adam equal to the Adam entry points; and the optimizer through the
-estimators and the three batched fleet builds.
+The Keras optimizers on the training kernels: gb_ffae_fit_opt in every memory plan (plain launches at batches of 32 and 80 rows, and
+split launches through a row map with a held-out tail), gb_lstm_fit_opt and gb_lstm_fit_tc_opt against the optimizer oracle
+(tests/optimizer_oracle.py) from injected weights and visiting order, on the weights, both state slots and the history; split and stop
+launches on a small stack; clipvalue on the summed gradient of a mini-batch above 32 rows; weight decay; padded lanes; per-epoch
+launches equal to one launch; NULL and plain Adam equal to the Adam entry points; and the optimizer through the estimators and the
+three batched fleet builds.  The stop launches in every memory plan are compared with the split ones in tests/test_gpu_fit_stop.py.
 """
 import ctypes as C
 import math
@@ -12,7 +13,7 @@ import numpy as np
 import pandas as pd
 import pytest
 from optimizer_oracle import OPTIMIZERS
-from parity_helpers import close, random_net
+from parity_helpers import ENTRIES, close, crossed, ff_split_run, random_net
 
 pytestmark = pytest.mark.gpu
 
@@ -60,8 +61,8 @@ def opt(name, **kw):
 
 # a larger rate than Keras' default, so that every rule moves the weights well beyond their float32 rounding in a few steps (Adadelta,
 # whose steps are ~sqrt(eps / (1 - rho)) = 1.4e-3 times the rate, at the rate its users run it with)
-def fast_opt(name):
-    return opt(name, learning_rate=1.0 if name == "adadelta" else 0.01, **({"momentum": 0.5} if name == "rmsprop" else {}))
+def fast_opt(name, **kw):
+    return opt(name, learning_rate=1.0 if name == "adadelta" else 0.01, **({"momentum": 0.5} if name == "rmsprop" else {}), **kw)
 
 
 
@@ -102,14 +103,17 @@ def ff_run(engine, torch, spec, w0s, X, Y, N, E, B, perm, optimizer, loss="mse")
     return eng, eng.unpack_params(params), hist.cpu().numpy(), acc.cpu().numpy(), m.cpu().numpy(), v.cpu().numpy()
 
 
-def check_ff(oo, spec, w0s, Xs, Ys, perm, res, E, B, optimizer, loss="mse"):
+def check_ff(oo, spec, w0s, Xs, Ys, perm, res, E, B, optimizer, loss="mse", n_val=0):
     """The tolerances of the loss tests on the weights and the history, with a wider absolute part where the rules normalise g: an
-    element whose summed gradient nearly cancels carries its rounding into its step and its state at their own scale."""
-    eng, got, hist, acc, m, v = res
+    element whose summed gradient nearly cancels carries its rounding into its step and its state at their own scale.  With n_val,
+    Xs / Ys are the jobs' positions (training, then n_val held out) and res ends with val_loss / val_accuracy."""
+    eng, got, hist, acc, m, v, *val = res
     for j in range(len(w0s)):
-        n = len(Xs[j])
+        n = len(Xs[j]) - n_val
+        vsplit = n_val / len(Xs[j])
+        assert math.floor(len(Xs[j]) * (1.0 - vsplit)) == n  # the oracle's split is the launch's
         w_ref, h_ref, st = oo.ff_fit(spec, w0s[j], Xs[j], Ys[j], optimizer, epochs=E, batch_size=B, perms=[perm[j, e, :n] for e in range(E)],
-                                     loss=loss)
+                                     loss=loss, validation_split=vsplit)
         for l, ((Wg, bg), (Wr, br), (W0, b0)) in enumerate(zip(got[j], w_ref, w0s[j])):
             # plus 0.5 % of the array's largest move: Adam's, Adamax's, Nadam's and RMSprop's steps are normalised, so an element whose
             # summed gradient nearly cancels moves by up to a full step in a direction its rounding decides
@@ -122,6 +126,9 @@ def check_ff(oo, spec, w0s, Xs, Ys, perm, res, E, B, optimizer, loss="mse"):
                 close(sb, rb, mag=mag, rtol=1e-3, atol=1e-2 * mag, name=f"{optimizer[0]} job {j} {what} b{l}")
         close(hist[j], np.array(h_ref["loss"]), mag=0.0, rtol=5e-4, name=f"{optimizer[0]} job {j} loss history")
         close(acc[j], np.array(h_ref["accuracy"]), mag=0, rtol=0, atol=2.0 / n, name=f"{optimizer[0]} job {j} accuracy history")
+        if n_val:
+            close(val[0][j], np.array(h_ref["val_loss"]), mag=0.0, rtol=5e-4, name=f"{optimizer[0]} job {j} val_loss history")
+            close(val[1][j], np.array(h_ref["val_accuracy"]), mag=0, rtol=0, atol=2.0 / n_val, name=f"{optimizer[0]} job {j} val_accuracy history")
 
 
 # (weights in L2, dz buffers in L2) of the five fit plans (tests/test_fit_plan.py pins these shapes to them)
@@ -138,15 +145,28 @@ def _plan_case(km, plan, M=2, N=70, seed=0):
     return spec, Xs, Ys, w0s
 
 
-@pytest.mark.parametrize("plan", list(PLANS))
+@pytest.mark.parametrize("plan,entry", crossed(PLANS, ENTRIES))
 @pytest.mark.parametrize("name", OPTIMIZERS)
-def test_every_optimizer_in_every_memory_plan(engine, torch, km, oo, name, plan):
-    spec, Xs, Ys, w0s = _plan_case(km, plan)
-    M, N, E, B = 2, 70, 2, 32
+def test_every_optimizer_in_every_memory_plan(engine, torch, km, oo, name, plan, entry):
+    """At batch 80 the last mini-batch of an epoch is partial too (170 = 80 + 80 + 10 rows), and clipvalue binds on the gradients the
+    three chunks sum in the L2 scratch image; the split launch holds out 40 positions, one held-out batch of two chunks."""
+    split, B = entry
+    M, N, E, NV = 2, 70 if B == 32 else 170, 2, 40 if split else 0
+    spec, Xs, Ys, w0s = _plan_case(km, plan, N=N + NV)
+    if B > 32:
+        # without the activity term, whose sign(a) jumps by 2 l1 where an activation lies within rounding of 0 (AdamW's second job in
+        # the two-dz plan meets one 7.7e-7 from 0 at step 4): the normalised rules carry such a jump into a step-sized difference, and
+        # there the float32 oracle stands as far from the float64 one as the kernel does
+        spec = km.FFSpec(spec.dims, spec.acts, [0.0] * len(spec.acts))
     perm = perms(M, E, N, seed=11)
-    o = fast_opt(name)
-    res = ff_run(engine, torch, spec, w0s, np.concatenate(Xs), np.concatenate(Ys), N, E, B, perm, o)
-    check_ff(oo, spec, w0s, Xs, Ys, perm, res, E, B, o)
+    o = fast_opt(name, **({"clipvalue": 0.02} if B > 32 else {}))
+    if split:
+        maps = [np.random.default_rng(50 + m).permutation(N + NV) for m in range(M)]
+        res = ff_split_run(engine, torch, spec, w0s, Xs, Ys, maps, NV, E, B, perm, optimizer=o)
+        Xs, Ys = [x[mp] for x, mp in zip(Xs, maps)], [y[mp] for y, mp in zip(Ys, maps)]  # the gathered copies
+    else:
+        res = ff_run(engine, torch, spec, w0s, np.concatenate(Xs), np.concatenate(Ys), N, E, B, perm, o)
+    check_ff(oo, spec, w0s, Xs, Ys, perm, res, E, B, o, n_val=NV)
 
 
 @pytest.mark.parametrize("name", OPTIMIZERS)
@@ -294,11 +314,12 @@ def test_null_and_plain_adam_are_the_adam_entry_points(engine, torch, km):
 
     spec = km.ff_hourglass_spec(16)
     eng = engine.FFEngine(spec.dims, spec.acts, spec.l1)
-    N = 100
-    x = dev(torch, eng, np.concatenate([waves(np.random.default_rng(m), N, 16) for m in range(2)]))
-    jobs = engine.jobs_to_device(engine.uniform_jobs(2, N), eng.device)
+    N, NV = 100, 20
+    # each job's 20 held-out positions are rows of its own after its N training rows, so no launch reads past x
+    x = dev(torch, eng, np.concatenate([waves(np.random.default_rng(m), N + NV, 16) for m in range(2)]))
+    jobs = engine.jobs_to_device(engine.make_jobs(np.arange(2), N, np.arange(2) * (N + NV)), eng.device)
     w0s = [random_net(km, spec.dims, 5 + m, spec.acts)[1] for m in range(2)]
-    split = engine.jobs_to_device(engine.make_split([20, 20]), eng.device)
+    split = engine.jobs_to_device(engine.make_split([NV, NV]), eng.device)
     stop = engine.jobs_to_device(engine.make_stop([dict(monitor="val_loss", patience=1)] * 2), eng.device)
     hp = engine._fit_hparams(3, 32, True, None, KERAS_ADAM, 7, False, 0, "huber")
     P = _cabi.ptr

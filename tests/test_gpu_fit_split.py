@@ -2,16 +2,20 @@
 gb_ffae_fit_split on the H100: training over row positions through a row map, and the validation pass at the end of every epoch.
 
 - Without a map or held-out positions it is gb_ffae_fit, bit for bit, in every memory plan.
-- With a map it is gb_ffae_fit on the gathered copy x[map], bit for bit.
+- With a map it is gb_ffae_fit on the gathered copy x[map], bit for bit, in shared memory and in both L2 plan groups.
 - Its val_loss / val_accuracy are those of the per-machine estimator's two launches per epoch (one training epoch, then an
-  lr = 0 fit of the held-out tail), bit for bit, and the float64 oracle's to 2e-4.
+  lr = 0 Adam fit of the held-out tail with the same loss), bit for bit, and the float64 oracle's to 2e-4.
+- Each of these holds for every kernel family of the fit (MSE-Adam, another loss, another optimizer: parity_helpers.FIT_KW), whose
+  split instantiations are then compared with their plain ones.
 - build_fleet(detector_shuffle=True, validation_split=0.1) replays slot by slot, and FleetModelBuilder builds the reference's
   example definition through the batched path with the metadata ModelBuilder writes.
 """
 import math
 
+import loss_oracle
 import numpy as np
 import pytest
+from parity_helpers import FIT_KW, crossed
 from sklearn.utils import shuffle as sk_shuffle
 
 pytestmark = pytest.mark.gpu
@@ -73,9 +77,9 @@ def perms(rng, lens, E, max_rows):
 
 
 # ------------------------------------------------------------------------------------------------ 1. no map, nothing held out
-@pytest.mark.parametrize("plan", list(PLANS))
+@pytest.mark.parametrize("plan,fit", crossed(PLANS, FIT_KW))
 @pytest.mark.parametrize("order", ["perm", "keyed"])
-def test_split_without_map_is_fit(engine, torch, km, plan, order):
+def test_split_without_map_is_fit(engine, torch, km, plan, order, fit):
     spec = plan_spec(km, plan)
     M, N, E, B = 2, 150, 2, 50
     rng = np.random.default_rng(5)
@@ -86,9 +90,9 @@ def test_split_without_map_is_fit(engine, torch, km, plan, order):
     jobs = engine.jobs_to_device(engine.uniform_jobs(M, N), eng.device)
     perm = dev(torch, eng, perms(rng, [N] * M, E, N)) if order == "perm" else None
     p1, p2 = eng.pack_params(w0s), eng.pack_params(w0s)
-    l1, a1, (m1, v1) = eng.fit(p1, jobs, M, N, xd, xd, epochs=E, batch_size=B, perm=perm, shuffle=True, seed=9)
+    l1, a1, (m1, v1) = eng.fit(p1, jobs, M, N, xd, xd, epochs=E, batch_size=B, perm=perm, shuffle=True, seed=9, **fit)
     split = engine.make_split(np.zeros(M, np.int32), -1)
-    l2, a2, vl, va, (m2, v2) = eng.fit_split(p2, jobs, M, N, xd, xd, split=split, epochs=E, batch_size=B, perm=perm, shuffle=True, seed=9)
+    l2, a2, vl, va, (m2, v2) = eng.fit_split(p2, jobs, M, N, xd, xd, split=split, epochs=E, batch_size=B, perm=perm, shuffle=True, seed=9, **fit)
     torch.cuda.synchronize()
     for name, g, w in (("weights", p2, p1), ("Adam m", m2, m1), ("Adam v", v2, v1), ("loss", l2, l1), ("accuracy", a2, a1)):
         assert torch.equal(g, w), name
@@ -96,10 +100,16 @@ def test_split_without_map_is_fit(engine, torch, km, plan, order):
 
 
 # ------------------------------------------------------------------------------------------------ 2. row map = gathered copy
+# shared memory, and one shape of each L2 plan group: the weight image alone, and the weight image with dz buffers
+ROW_MAP_PLANS = {"hourglass8": ("hourglass", 8), "weights_in_l2": PLANS["weights_in_l2"], "three_dz_in_l2": PLANS["three_dz_in_l2"]}
+
+
+@pytest.mark.parametrize("plan,fit", crossed(ROW_MAP_PLANS, FIT_KW))
 @pytest.mark.parametrize("shuffle", [0, 1, 2])
 @pytest.mark.parametrize("batch", [1, 32, 50, 128])
-def test_row_map_is_the_gathered_copy(engine, torch, km, shuffle, batch):
-    spec = km.ff_hourglass_spec(8)
+def test_row_map_is_the_gathered_copy(engine, torch, km, shuffle, batch, plan, fit):
+    kind, T = ROW_MAP_PLANS[plan]
+    spec = km.ff_hourglass_spec(T) if kind == "hourglass" else km.ff_symmetric_spec(T)
     rng = np.random.default_rng(100 * shuffle + batch)
     lens = np.array([200, 200, 129, 129, 7, 1, 60])
     maps = {200: sk_shuffle(np.arange(200), random_state=0), 129: sk_shuffle(np.arange(129), random_state=0), 7: rng.permutation(7)}
@@ -109,8 +119,8 @@ def test_row_map_is_the_gathered_copy(engine, torch, km, shuffle, batch):
     map_ofs = np.array([ofs.get(n, -1) if j != 6 else -1 for j, n in enumerate(lens)])  # the 60-row job reads its rows in place
     J = len(lens)
     x_row = np.concatenate([[3], 3 + np.cumsum(lens[:-1] + 5)])  # gaps between the jobs' rows
-    X = waves(rng, int(x_row[-1] + lens[-1] + 4), 8)
-    Y = waves(rng, len(X), 8)
+    X = waves(rng, int(x_row[-1] + lens[-1] + 4), T)
+    Y = waves(rng, len(X), T)
     gathered_rows = np.concatenate([x_row[j] + (row_map[map_ofs[j]:map_ofs[j] + lens[j]] if map_ofs[j] >= 0 else np.arange(lens[j])) for j in range(J)])
     g_row = np.concatenate([[0], np.cumsum(lens[:-1])])
     slots = rng.permutation(J).astype(np.int32)
@@ -118,7 +128,7 @@ def test_row_map_is_the_gathered_copy(engine, torch, km, shuffle, batch):
     E = 2
     eng = engine.FFEngine(spec.dims, spec.acts, spec.l1)
     perm = dev(torch, eng, perms(rng, lens, E, int(lens.max()))) if shuffle == 2 else None
-    kw = dict(epochs=E, batch_size=batch, shuffle=shuffle == 1, perm=perm, seed=11)
+    kw = dict(epochs=E, batch_size=batch, shuffle=shuffle == 1, perm=perm, seed=11, **fit)
     p1 = eng.pack_params(w0s)
     l1, a1, (m1, v1) = eng.fit(p1, engine.jobs_to_device(engine.make_jobs(slots, lens, g_row), eng.device), J, int(lens.max()),
                                dev(torch, eng, X[gathered_rows]), dev(torch, eng, Y[gathered_rows]), **kw)
@@ -132,8 +142,9 @@ def test_row_map_is_the_gathered_copy(engine, torch, km, shuffle, batch):
 
 
 # ------------------------------------------------------------------------------------------------ 3. validation pass
-def two_launch_witness(engine, torch, eng, w0s, xd, yd, lens, n_val, x_row, E, B, vb, perm):
-    """The per-machine estimator's method: one training launch per epoch, then an lr = 0 fit of every held-out tail."""
+def two_launch_witness(engine, torch, eng, w0s, xd, yd, lens, n_val, x_row, E, B, vb, perm, **fit):
+    """The per-machine estimator's method: one training launch per epoch, then an lr = 0 Adam fit of every held-out tail with the
+    same loss."""
     J = len(lens)
     params = eng.pack_params(w0s)
     jobs = engine.jobs_to_device(engine.make_jobs(np.arange(J), lens, x_row), eng.device)
@@ -146,7 +157,7 @@ def two_launch_witness(engine, torch, eng, w0s, xd, yd, lens, n_val, x_row, E, B
             jj = engine.jobs_to_device(engine.make_jobs([j], [lens[j]], [x_row[j]]), eng.device)
             st = None if state is None else state[j]
             l, a, s = eng.fit(params, jj, 1, int(lens[j]), xd, yd, epochs=1, batch_size=B, perm=perm[j:j + 1, e:e + 1].contiguous(), shuffle=False,
-                              state=st, step0=e * math.ceil(lens[j] / B))
+                              state=st, step0=e * math.ceil(lens[j] / B), **fit)
             l_e.append(l)
             a_e.append(a)
             if state is None:
@@ -154,7 +165,8 @@ def two_launch_witness(engine, torch, eng, w0s, xd, yd, lens, n_val, x_row, E, B
             state[j] = s
         loss.append(torch.cat(l_e))
         acc.append(torch.cat(a_e))
-        vl, va, _ = eng.fit(params.clone(), vjobs, J, int(max(n_val)), xd, yd, epochs=1, batch_size=vb, shuffle=False, adam=FROZEN)
+        vl, va, _ = eng.fit(params.clone(), vjobs, J, int(max(n_val)), xd, yd, epochs=1, batch_size=vb, shuffle=False, adam=FROZEN,
+                            loss=fit.get("loss", "mse"))
         vloss.append(vl)
         vacc.append(va)
         weights.append(eng.unpack_params(params))
@@ -162,9 +174,9 @@ def two_launch_witness(engine, torch, eng, w0s, xd, yd, lens, n_val, x_row, E, B
     return params, cat(loss), cat(acc), cat(vloss), cat(vacc), weights
 
 
-@pytest.mark.parametrize("plan", list(PLANS))
+@pytest.mark.parametrize("plan,fit", crossed(PLANS, FIT_KW))
 @pytest.mark.parametrize("vb", [1, 16, 32, 50, 128])
-def test_validation_pass_is_the_frozen_launch(engine, torch, km, plan, vb):
+def test_validation_pass_is_the_frozen_launch(engine, torch, km, plan, vb, fit):
     spec = plan_spec(km, plan)
     T = spec.dims[0]
     rng = np.random.default_rng(vb)
@@ -181,21 +193,22 @@ def test_validation_pass_is_the_frozen_launch(engine, torch, km, plan, vb):
     params = eng.pack_params(w0s)
     jobs = engine.jobs_to_device(engine.make_jobs(np.arange(len(lens)), lens, x_row), eng.device)
     loss, acc, vloss, vacc, _ = eng.fit_split(params, jobs, len(lens), int(lens.max()), xd, xd, split=engine.make_split(n_val), val_batch=vb,
-                                              epochs=E, batch_size=B, perm=perm)
-    wp, wl, wa, wvl, wva, weights = two_launch_witness(engine, torch, eng, w0s, xd, xd, lens, n_val, x_row, E, B, vb, perm)
+                                              epochs=E, batch_size=B, perm=perm, **fit)
+    wp, wl, wa, wvl, wva, weights = two_launch_witness(engine, torch, eng, w0s, xd, xd, lens, n_val, x_row, E, B, vb, perm, **fit)
     torch.cuda.synchronize()
     assert torch.equal(params, wp), "weights"
     assert torch.equal(loss, wl) and torch.equal(acc, wa), "training loss / accuracy"
     assert torch.equal(vloss, wvl), "val_loss"
     assert torch.equal(vacc, wva), "val_accuracy"
-    # the float64 oracle at the weights after each epoch: sample-weighted mean of the per-batch total losses
+    # the float64 oracle at the weights after each epoch: sample-weighted mean of the per-batch total losses (loss + activity term)
     got = vloss.cpu().numpy()
     for j in range(len(lens)):
         tail = X[x_row[j] + lens[j]: x_row[j] + lens[j] + n_val[j]]
         for e in range(E):
             num = 0.0
             for s in range(0, n_val[j], vb):
-                total, _mse, _g, _yh = km.ff_loss_and_grads(spec, weights[e][j], tail[s:s + vb], tail[s:s + vb], np.float64)
+                total, _data, _g, _yh = loss_oracle.ff_loss_and_grads(spec, weights[e][j], tail[s:s + vb], tail[s:s + vb], np.float64,
+                                                                      loss=fit.get("loss", "mse"))
                 num += float(total) * len(tail[s:s + vb])
             want = num / n_val[j]
             assert abs(got[j, e] - want) <= 2e-4 * abs(want), (j, e, got[j, e], want)

@@ -6,13 +6,16 @@ gb_ffae_fit_stop on the H100: Keras' EarlyStopping applied by every job at the e
   their snapshot's epoch), their Adam state of the last epoch run, and NaN history past their last epoch.
 - epochs run and best epoch are those of the host EarlyStopping applied to the full history, over monitors, modes, min_delta,
   baseline, start_from_epoch and restore_best_weights, NaN losses included.
-- build_fleet(early_stopping=...) replays the per-machine loop slot by slot, and FleetModelBuilder builds the reference's
-  production estimator definition in one bucket with the metadata ModelBuilder writes.
+- build_fleet(early_stopping=...) replays the per-machine loop slot by slot, with the weights in shared memory and in L2, and
+  FleetModelBuilder builds the reference's production estimator definition in one bucket with the metadata ModelBuilder writes.
+- The first three hold for every kernel family of the fit (MSE-Adam, another loss, another optimizer: parity_helpers.FIT_KW); the
+  optimizer state checked is then the optimizer's two state slots.
 """
 import math
 
 import numpy as np
 import pytest
+from parity_helpers import FIT_KW, crossed
 from sklearn.utils import shuffle as sk_shuffle
 
 pytestmark = pytest.mark.gpu
@@ -89,8 +92,8 @@ def host_rule(cfg, history, E):
 
 
 # ------------------------------------------------------------------------------------------------ 1. a rule that never fires
-@pytest.mark.parametrize("plan", list(PLANS))
-def test_rule_that_never_fires_is_fit_split(engine, torch, km, plan):
+@pytest.mark.parametrize("plan,fit", crossed(PLANS, FIT_KW))
+def test_rule_that_never_fires_is_fit_split(engine, torch, km, plan, fit):
     spec = plan_spec(km, plan)
     M, N, NV, E, B = 3, 150, 23, 3, 50
     rng = np.random.default_rng(7)
@@ -100,7 +103,7 @@ def test_rule_that_never_fires_is_fit_split(engine, torch, km, plan):
     xd = dev(torch, eng, X)
     jobs = engine.jobs_to_device(engine.make_jobs(np.arange(M), N, np.arange(M) * (N + NV)), eng.device)
     split = engine.make_split(np.full(M, NV))
-    kw = dict(split=split, epochs=E, batch_size=B, shuffle=True, seed=13)
+    kw = dict(split=split, epochs=E, batch_size=B, shuffle=True, seed=13, **fit)
     p1, p2 = eng.pack_params(w0s), eng.pack_params(w0s)
     l1, a1, vl1, va1, (m1, v1) = eng.fit_split(p1, jobs, M, N, xd, xd, **kw)
     stop = engine.make_stop([{"monitor": mon, "patience": E} for mon in ("val_loss", "loss", "val_accuracy")])
@@ -113,10 +116,10 @@ def test_rule_that_never_fires_is_fit_split(engine, torch, km, plan):
 
 
 # ------------------------------------------------------------------------------------------------ 2. ragged stops in one launch
-@pytest.mark.parametrize("plan", list(PLANS))
+@pytest.mark.parametrize("plan,fit", crossed(PLANS, FIT_KW))
 @pytest.mark.parametrize("batch", [1, 32, 128])
 @pytest.mark.parametrize("restore", [False, True])
-def test_ragged_stops(engine, torch, km, plan, batch, restore):
+def test_ragged_stops(engine, torch, km, plan, batch, restore, fit):
     spec = plan_spec(km, plan)
     lens = np.array([150, 97, 64, 33, 140])
     J, E = len(lens), 7
@@ -129,7 +132,7 @@ def test_ragged_stops(engine, torch, km, plan, batch, restore):
     eng = engine.FFEngine(spec.dims, spec.acts, spec.l1)
     xd = dev(torch, eng, X)
     jobs_h = engine.make_jobs(slots, lens, x_row)
-    kw = dict(batch_size=batch, shuffle=True, seed=5)
+    kw = dict(batch_size=batch, shuffle=True, seed=5, **fit)
     p = eng.pack_params([w0s[s] for s in range(J)])
     stop = engine.make_stop([{"monitor": "loss", "patience": int(pj), "min_delta": 1e30, "restore_best_weights": restore} for pj in patience])
     loss, acc, _, _, ran, best, (m, v) = eng.fit_split(p, engine.jobs_to_device(jobs_h, eng.device), J, int(lens.max()), xd, xd, epochs=E,
@@ -146,7 +149,7 @@ def test_ragged_stops(engine, torch, km, plan, batch, restore):
         eng.fit_split(p1, one, 1, int(lens[j]), xd, xd, epochs=1, **kw)
         torch.cuda.synchronize()
         assert torch.equal(p[s], (p1 if restore else pw)[s]), (j, "weights")
-        assert torch.equal(m[s], wm[s]) and torch.equal(v[s], wv[s]), (j, "Adam state of the last epoch run")
+        assert torch.equal(m[s], wm[s]) and torch.equal(v[s], wv[s]), (j, "optimizer state of the last epoch run")
         assert torch.equal(loss[j, :k], wl[0]) and torch.equal(acc[j, :k], wa[0]), (j, "history")
         assert bool(loss[j, k:].isnan().all()) and bool(acc[j, k:].isnan().all()), (j, "history past the stop")
 
@@ -164,8 +167,8 @@ RULES = [dict(monitor=mon, patience=pat, min_delta=md, restore_best_weights=rb, 
 ]
 
 
-@pytest.mark.parametrize("plan", ["shared", "weights_in_l2", "three_dz_in_l2"])
-def test_rule_is_the_host_early_stopping(engine, torch, km, plan):
+@pytest.mark.parametrize("plan,fit", crossed(["shared", "weights_in_l2", "three_dz_in_l2"], FIT_KW))
+def test_rule_is_the_host_early_stopping(engine, torch, km, plan, fit):
     spec = plan_spec(km, plan)
     J, N, NV, E, B = len(RULES), 120, 30, 10, 32
     rng = np.random.default_rng(31)
@@ -175,7 +178,7 @@ def test_rule_is_the_host_early_stopping(engine, torch, km, plan):
     eng = engine.FFEngine(spec.dims, spec.acts, spec.l1)
     xd = dev(torch, eng, X)
     jobs = engine.jobs_to_device(engine.make_jobs(np.arange(J), N, x_row), eng.device)
-    kw = dict(split=engine.make_split(np.full(J, NV)), batch_size=B, shuffle=True, seed=17)
+    kw = dict(split=engine.make_split(np.full(J, NV)), batch_size=B, shuffle=True, seed=17, **fit)
     # witnesses: the same launch without the rule, for every epoch count
     ref = {}
     for k in range(1, E + 1):
@@ -193,7 +196,7 @@ def test_rule_is_the_host_early_stopping(engine, torch, km, plan):
         fired += want_ran < E
         assert (int(ran[j]), int(best[j])) == (want_ran, want_best), (j, cfg)
         assert torch.equal(p[j], ref[keep][0][j]), (j, cfg, "weights")
-        assert torch.equal(m[j], ref[want_ran][1][j]) and torch.equal(v[j], ref[want_ran][2][j]), (j, cfg, "Adam state")
+        assert torch.equal(m[j], ref[want_ran][1][j]) and torch.equal(v[j], ref[want_ran][2][j]), (j, cfg, "optimizer state")
         for got, want in zip((loss, acc, vloss, vacc), ref[want_ran][3]):
             assert torch.equal(got[j, :want_ran], want[j]) and bool(got[j, want_ran:].isnan().all()), (j, cfg, "history")
     assert fired >= 3  # the grid exercises early stops, not only full runs
@@ -231,21 +234,23 @@ def test_nan_losses_never_improve(engine, torch, km, restore):
 
 
 # ------------------------------------------------------------------------------------------------ 4. build_fleet, slot by slot
-def test_build_fleet_with_early_stopping_replays(engine, torch, km):
+def replay_fleet_with_early_stopping(engine, torch, km, T, fit):
+    """build_fleet(early_stopping=...) on T-tag hourglasses against the per-machine loop, slot by slot: the fleet runs the stop kernels,
+    the loop the plain ones, one launch per epoch and the frozen Adam tail."""
     from gordo_components_b200 import fleet
     from gordo_components_b200.machine.model.models import EarlyStopping
 
-    spec = km.ff_hourglass_spec(8)
+    spec = km.ff_hourglass_spec(T)
     M, N, K, E, B, vsplit = 3, 230, 3, 10, 32, 0.1
     rng = np.random.default_rng(22)
-    X = np.concatenate([waves(rng, N, 8) for _ in range(M)])
+    X = np.concatenate([waves(rng, N, T) for _ in range(M)])
     eng = engine.FFEngine(spec.dims, spec.acts, spec.l1)
     xd = dev(torch, eng, X)
     rules = [dict(monitor="val_loss", patience=1, min_delta=1.0, restore_best_weights=False),  # stops after epoch 1
              dict(monitor="val_loss", patience=2, min_delta=2e-3, restore_best_weights=True),
              dict(monitor="val_loss", patience=E, restore_best_weights=True)]
     fb = fleet.build_fleet(eng, xd, xd, N, epochs=E, batch_size=B, n_splits=K, seed=3, adam=KERAS_ADAM, shuffle=False,
-                           detector_shuffle=True, validation_split=vsplit, early_stopping=[EarlyStopping(**r) for r in rules])
+                           detector_shuffle=True, validation_split=vsplit, early_stopping=[EarlyStopping(**r) for r in rules], **fit)
     torch.cuda.synchronize()
     assert fb.epochs == E and tuple(fb.epochs_run.shape) == (M,) and tuple(fb.fold_epochs_run.shape) == (M, K)
     test = N // (K + 1)
@@ -271,8 +276,9 @@ def test_build_fleet_with_early_stopping_replays(engine, torch, km):
             state, losses, vlosses = None, [], []
             for e in range(E):  # the per-machine loop: one epoch, the frozen tail, the callback
                 l, _, state = eng.fit(p, tj, 1, n_train, xs, xs, epochs=1, batch_size=B, shuffle=False, adam=KERAS_ADAM, state=state,
-                                      step0=e * math.ceil(n_train / B))
-                vl, _, _ = eng.fit(p.clone(), vj, 1, n - n_train, xs, xs, epochs=1, batch_size=B, shuffle=False, adam=FROZEN)
+                                      step0=e * math.ceil(n_train / B), **fit)
+                vl, _, _ = eng.fit(p.clone(), vj, 1, n - n_train, xs, xs, epochs=1, batch_size=B, shuffle=False, adam=FROZEN,
+                                   loss=fit.get("loss", "mse"))
                 losses.append(l)
                 vlosses.append(vl)
                 if cb.update(e, {"loss": float(l[0, 0]), "val_loss": float(vl[0, 0])}, lambda: p.clone()):
@@ -296,6 +302,16 @@ def test_build_fleet_with_early_stopping_replays(engine, torch, km):
     ran0 = int(fb.epochs_run[0])
     assert all(len(h[k]) == ran0 for k in ("loss", "accuracy", "val_loss", "val_accuracy"))
     assert h["params"]["epochs"] == E and det.base_estimator._history.epoch == list(range(ran0))
+
+
+def test_build_fleet_with_early_stopping_replays(engine, torch, km):
+    replay_fleet_with_early_stopping(engine, torch, km, 8, FIT_KW["mse-adam"])
+
+
+# the other stop kernels the batched build reaches: the weight image in L2 (128 tags), and another loss and optimizer (LOSS + OPT)
+@pytest.mark.parametrize("T,fit", crossed([8, 128], {k: FIT_KW[k] for k in ("mse-adam", "mae-nadam")})[1:])
+def test_build_fleet_with_early_stopping_replays_other_kernels(engine, torch, km, T, fit):
+    replay_fleet_with_early_stopping(engine, torch, km, T, fit)
 
 
 # ------------------------------------------------------------------------------------------------ 5. the production definition
