@@ -33,6 +33,7 @@ struct Args {
   const gb_job* jobs;
   const float *x, *y, *scale, *feat_thr, *agg_thr;
   float *o_model, *o_ts, *o_tu, *o_tots, *o_totu, *o_conf, *o_totconf;
+  const double *x64, *x_scale, *x_offset;  // float64 x and the slot's input scaler (X64 instantiations; x is then unused)
 };
 
 // output columns [c0, c0 + nb) of layer l as a padded [Kp][nb] image followed by their nb biases
@@ -50,8 +51,9 @@ __device__ __forceinline__ void stage_layer(float* dst, const float* P, const Ar
 // RT row groups of 32 per thread: tiles of 128 rows (RT = 4) for the usual stacks, 64 / 32 rows when wide layers (up to 256: the
 // defaults of feedforward_model / feedforward_symmetric) leave less shared memory for the activation buffers.  BLOCKED: staged
 // layers go in blocks of a.col_block output columns (only with 32-row tiles, for layers too large to stage whole); a separate
-// instantiation so that every other plan runs the single-block code.
-template <int RT, bool BLOCKED>
+// instantiation so that every other plan runs the single-block code.  X64: x is float64 and the slot's input scaler is applied as
+// it is read, x' = (float)(x * x_scale + x_offset) with two roundings in double and one to float, as gb_affine_f64 computes it.
+template <int RT, bool BLOCKED, bool X64>
 __global__ void __launch_bounds__(THREADS) ffae_infer_fma_kernel(const Args a) {
   constexpr int ROWS = 32 * RT;
   extern __shared__ __align__(16) float smem[];
@@ -76,7 +78,16 @@ __global__ void __launch_bounds__(THREADS) ffae_infer_fma_kernel(const Args a) {
   for (int tile = row_begin; tile < row_end; tile += ROWS) {
     const int nrows = min(ROWS, row_end - tile);
     // ---- X tile -> buf0[r][k], zero padded -------------------------------------------------
-    {
+    if constexpr (X64) {
+      const double* xg = a.x64 + (job.x_row + tile) * (long)n_in;
+      const double* xa = a.x_scale + (long)job.slot * n_in;
+      const double* xb = a.x_offset + (long)job.slot * n_in;
+      const int Tp = a.im.kp[0];
+      for (int idx = tid; idx < ROWS * Tp; idx += THREADS) {
+        const int r = idx / Tp, k = idx - r * Tp;
+        buf0[r * pitch + k] = (r < nrows && k < n_in) ? (float)__dadd_rn(__dmul_rn(__ldg(xg + (long)r * n_in + k), __ldg(xa + k)), __ldg(xb + k)) : 0.f;
+      }
+    } else {
       const float* xg = a.x + (job.x_row + tile) * (long)n_in;
       const int Tp = a.im.kp[0];
       if ((n_in & 3) == 0) {
@@ -311,8 +322,10 @@ extern "C" int gb_ffae_infer_plan(const gb_ffnet* net, int32_t* rows_per_tile, i
   return GB_OK;
 }
 
+// x_scale == NULL: x is float32.  Otherwise x is float64 and x_scale / x_offset [n_slots][n_in] double are the slot's input scaler.
 extern "C" int gb_ffae_infer_score_fma(const gb_ffnet* net, const float* params, const gb_job* jobs, int32_t n_jobs,
-                                       int32_t max_rows, const float* x, const float* y, const float* scale,
+                                       int32_t max_rows, const void* x, const double* x_scale, const double* x_offset,
+                                       const float* y, const float* scale,
                                        const float* feat_thr, const float* agg_thr, float* out_model,
                                        float* out_tag_scaled, float* out_tag_unscaled, float* out_total_scaled,
                                        float* out_total_unscaled, float* out_conf, float* out_total_conf,
@@ -325,9 +338,15 @@ extern "C" int gb_ffae_infer_score_fma(const gb_ffnet* net, const float* params,
   a.n_in = net->dims[0];
   a.n_out = net->dims[net->n_layers];
   a.pstride = (long)gb_ffnet_param_stride(net);
-  a.params = params; a.jobs = jobs; a.x = x; a.y = y; a.scale = scale; a.feat_thr = feat_thr; a.agg_thr = agg_thr;
+  const bool x64 = x_scale != nullptr;
+  a.params = params; a.jobs = jobs; a.y = y; a.scale = scale; a.feat_thr = feat_thr; a.agg_thr = agg_thr;
   a.o_model = out_model; a.o_ts = out_tag_scaled; a.o_tu = out_tag_unscaled; a.o_tots = out_total_scaled;
   a.o_totu = out_total_unscaled; a.o_conf = out_conf; a.o_totconf = out_total_conf;
+  if (x64) {
+    a.x64 = static_cast<const double*>(x); a.x_scale = x_scale; a.x_offset = x_offset;
+  } else {
+    a.x = static_cast<const float*>(x);
+  }
 
   int dev = 0, sms = 132;
   GB_CUDA_CHECK(cudaGetDevice(&dev));
@@ -347,8 +366,13 @@ extern "C" int gb_ffae_infer_score_fma(const gb_ffnet* net, const float* params,
     return GB_OK;
   };
   const bool blocked = a.col_block < a.im.max_np;
-  int rc = rt == 4 ? launch(ffae_infer_fma_kernel<4, false>) : rt == 2 ? launch(ffae_infer_fma_kernel<2, false>)
-           : blocked ? launch(ffae_infer_fma_kernel<1, true>) : launch(ffae_infer_fma_kernel<1, false>);
+  int rc;
+  if (!x64)
+    rc = rt == 4 ? launch(ffae_infer_fma_kernel<4, false, false>) : rt == 2 ? launch(ffae_infer_fma_kernel<2, false, false>)
+         : blocked ? launch(ffae_infer_fma_kernel<1, true, false>) : launch(ffae_infer_fma_kernel<1, false, false>);
+  else
+    rc = rt == 4 ? launch(ffae_infer_fma_kernel<4, false, true>) : rt == 2 ? launch(ffae_infer_fma_kernel<2, false, true>)
+         : blocked ? launch(ffae_infer_fma_kernel<1, true, true>) : launch(ffae_infer_fma_kernel<1, false, true>);
   if (rc != GB_OK) return rc;
   GB_CUDA_CHECK(cudaGetLastError());
   return GB_OK;

@@ -26,6 +26,7 @@ struct SmallArgs {
   const gb_job* jobs;
   const float *x, *y, *scale, *feat_thr, *agg_thr;
   float *o_model, *o_ts, *o_tu, *o_tots, *o_totu, *o_conf, *o_totconf;
+  const double *x64, *x_scale, *x_offset;  // float64 x and the slot's input scaler (X64 instantiations; x is then unused)
 };
 
 __device__ __forceinline__ float fast_tanh(float z) {
@@ -51,6 +52,14 @@ __device__ __forceinline__ void load_row(const float* __restrict__ p, int T, flo
     for (int c = 0; c < W; ++c) v[c] = c < T ? __ldg(p + c) : 0.f;
   }
 }
+// row of T doubles through the slot's input scaler a, b: (float)(x * a + b), two roundings in double and one to float as
+// gb_affine_f64 computes it; zero padded to W
+template <int W>
+__device__ __forceinline__ void load_row_x64(const double* __restrict__ p, const double* __restrict__ xa, const double* __restrict__ xb, int T,
+                                             float* v) {
+#pragma unroll
+  for (int c = 0; c < W; ++c) v[c] = c < T ? (float)__dadd_rn(__dmul_rn(__ldg(p + c), __ldg(xa + c)), __ldg(xb + c)) : 0.f;
+}
 template <int W>
 __device__ __forceinline__ void store_row(float* __restrict__ p, int T, const float* v) {
   if ((T & 3) == 0) {
@@ -64,7 +73,7 @@ __device__ __forceinline__ void store_row(float* __restrict__ p, int T, const fl
   }
 }
 
-template <int W>
+template <int W, bool X64>
 __global__ void __launch_bounds__(THREADS) ffae_infer_small_kernel(const SmallArgs a) {
   __shared__ __align__(16) float sW[GB_MAX_LAYERS][W][W];  // [layer][k][n], zero padded
   __shared__ __align__(16) float sB[GB_MAX_LAYERS][W];
@@ -97,7 +106,10 @@ __global__ void __launch_bounds__(THREADS) ffae_infer_small_kernel(const SmallAr
   const int row_end = min(job.n_rows, row0 + CHUNK);
   for (int r = row0 + tid; r < row_end; r += THREADS) {
     float act[W];
-    load_row<W>(a.x + (job.x_row + r) * (long)T_in, T_in, act);
+    if constexpr (X64)
+      load_row_x64<W>(a.x64 + (job.x_row + r) * (long)T_in, a.x_scale + (long)job.slot * T_in, a.x_offset + (long)job.slot * T_in, T_in, act);
+    else
+      load_row<W>(a.x + (job.x_row + r) * (long)T_in, T_in, act);
     for (int l = 0; l < L; ++l) {
       float z[W];
 #pragma unroll
@@ -157,8 +169,9 @@ extern "C" int gb_ffae_small_supported(const gb_ffnet* net) {
   return GB_OK;
 }
 
+// x_scale == NULL: x is float32.  Otherwise x is float64 and x_scale / x_offset [n_slots][n_in] double are the slot's input scaler.
 extern "C" int gb_ffae_infer_score_small(const gb_ffnet* net, const float* params, const gb_job* jobs, int32_t n_jobs, int32_t max_rows,
-                                         const float* x, const float* y, const float* scale, const float* feat_thr, const float* agg_thr,
+                                         const void* x, const double* x_scale, const double* x_offset, const float* y, const float* scale, const float* feat_thr, const float* agg_thr,
                                          float* out_model, float* out_tag_scaled, float* out_tag_unscaled, float* out_total_scaled,
                                          float* out_total_unscaled, float* out_conf, float* out_total_conf, void* stream) {
   int rc = gb_ffae_small_supported(net);
@@ -168,7 +181,13 @@ extern "C" int gb_ffae_infer_score_small(const gb_ffnet* net, const float* param
   a.n_in = net->dims[0];
   a.n_out = net->dims[net->n_layers];
   a.pstride = (long)gb_ffnet_param_stride(net);
-  a.params = params; a.jobs = jobs; a.x = x; a.y = y; a.scale = scale; a.feat_thr = feat_thr; a.agg_thr = agg_thr;
+  const bool x64 = x_scale != nullptr;
+  if (x64) {
+    a.x64 = static_cast<const double*>(x); a.x_scale = x_scale; a.x_offset = x_offset;
+  } else {
+    a.x = static_cast<const float*>(x);
+  }
+  a.params = params; a.jobs = jobs; a.y = y; a.scale = scale; a.feat_thr = feat_thr; a.agg_thr = agg_thr;
   a.o_model = out_model; a.o_ts = out_tag_scaled; a.o_tu = out_tag_unscaled; a.o_tots = out_total_scaled;
   a.o_totu = out_total_unscaled; a.o_conf = out_conf; a.o_totconf = out_total_conf;
   int wmax = 0;
@@ -176,9 +195,10 @@ extern "C" int gb_ffae_infer_score_small(const gb_ffnet* net, const float* param
   for (int j0 = 0; j0 < n_jobs; j0 += 65535) {  // gridDim.y carries the job index: larger fleets go out as several launches
     a.jobs = jobs + j0;
     const dim3 grid((max_rows + CHUNK - 1) / CHUNK, n_jobs - j0 < 65535 ? n_jobs - j0 : 65535);
-    if (wmax <= 4) ffae_infer_small_kernel<4><<<grid, THREADS, 0, (cudaStream_t)stream>>>(a);
-    else if (wmax <= 8) ffae_infer_small_kernel<8><<<grid, THREADS, 0, (cudaStream_t)stream>>>(a);
-    else ffae_infer_small_kernel<16><<<grid, THREADS, 0, (cudaStream_t)stream>>>(a);
+    const auto kern = wmax <= 4 ? (x64 ? ffae_infer_small_kernel<4, true> : ffae_infer_small_kernel<4, false>)
+                      : wmax <= 8 ? (x64 ? ffae_infer_small_kernel<8, true> : ffae_infer_small_kernel<8, false>)
+                                  : (x64 ? ffae_infer_small_kernel<16, true> : ffae_infer_small_kernel<16, false>);
+    kern<<<grid, THREADS, 0, (cudaStream_t)stream>>>(a);
   }
   GB_CUDA_CHECK(cudaGetLastError());
   return GB_OK;

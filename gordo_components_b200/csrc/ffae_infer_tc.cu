@@ -39,20 +39,24 @@ namespace {
 using namespace gb::sm90;
 
 constexpr int TILE = 64;  // rows per warpgroup tile (wgmma M)
-constexpr int NWG = 3;    // warpgroups per CTA
-constexpr int NTHREADS = 128 * NWG;
+constexpr int NWG_MAX = 3;  // warpgroups per CTA (float64 x tiles of a stack whose weights leave no room for three: 2)
 constexpr int MAXL = 8;
 constexpr int W = 64;  // widest feature / hidden width
-// x / y tiles in shared memory: 64 rows x 64 columns of fp32 as two TMA boxes of 32 columns (128-byte rows, SWIZZLE_128B)
+// x / y tiles in shared memory: 64 rows x 64 columns of fp32 as two TMA boxes of 32 columns (128-byte rows, SWIZZLE_128B).
+// float64 x (the input-scaler mode) is four boxes of 16 columns: the same 128-byte rows, twice the bytes per tile.
 constexpr int BOX_COLS = 32;
+constexpr int BOX_COLS_X64 = 16;
 constexpr int BOX_BYTES = TILE * BOX_COLS * 4;
 constexpr int TILE_BYTES = 2 * BOX_BYTES;
-constexpr int STAGE_BYTES = 2 * TILE_BYTES * NWG;  // per warpgroup: one x and one y tile
+// per warpgroup: one x and one y tile
+__host__ __device__ constexpr int x_tile_bytes(bool x64) { return x64 ? 2 * TILE_BYTES : TILE_BYTES; }
+__host__ __device__ constexpr int stage_bytes(bool x64, int nwg) { return (x_tile_bytes(x64) + TILE_BYTES) * nwg; }
 // output staging: a warp's 16 rows x 32 columns of one array (rows 16 wq .. of a SWIZZLE_128B box: a 1024-aligned slice)
 constexpr int OBOX_ROWS = 16;
 constexpr int OBOX_BYTES = OBOX_ROWS * BOX_COLS * 4;
-constexpr int RESTAGE_BATCH = 11;  // parameter loads per thread and layer when the weights are restaged
-static_assert(RESTAGE_BATCH * NTHREADS >= W * W + W, "a layer's kernel and bias are one batch of loads");
+// parameter loads per thread and layer when the weights are restaged: a layer's kernel and bias are one batch of loads
+__host__ __device__ constexpr int restage_batch(int nthreads) { return (W * W + W + nthreads - 1) / nthreads; }
+static_assert(restage_batch(128 * NWG_MAX) == 11, "three warpgroups restage a layer in 11 loads per thread");
 
 struct TcArgs {
   CUtensorMap tm_x, tm_y;  // x and y as [n_x_rows][T], boxes of BOX_COLS x TILE, zeros outside (tm_y unused without y)
@@ -74,6 +78,10 @@ struct TcArgs {
   const float *y, *scale, *feat_thr, *agg_thr;  // (x and y are read through tm_x / tm_y; y != nullptr says whether it is given)
   float *o_model, *o_ts, *o_tu, *o_conf, *o_tots, *o_totu, *o_totconf;
   unsigned int* work_ctr;  // global tile counter of this launch (zeroed by the launcher, stream-ordered)
+  // float64 x only: x' = (float)(x * x_scale[slot][c] + x_offset[slot][c]), the slot's pair staged at xab_ofs as double [2][W]
+  const double *x_scale, *x_offset;
+  int xab_ofs;
+  long n_x_rows;
 };
 
 // tanh(x) = 1 - 2/(1 + 2^(2x*log2 e)); absolute error ~2e-7 (ex2.approx / rcp.approx are ~1-2 ulp), exact limits at +-inf.
@@ -164,6 +172,8 @@ __device__ __forceinline__ void mma_hidden(float* d, const uint32_t (&a1)[4][4],
 // The same inside one box (col < 32); the output staging boxes use it too.
 __device__ __forceinline__ int box_ofs(int r, int col) { return r * 128 + (((col >> 2) ^ (r & 7)) << 4) + ((col & 3) << 2); }
 __device__ __forceinline__ int tile_ofs(int r, int col) { return (col >> 5) * BOX_BYTES + box_ofs(r, col & 31); }
+// ... and of the double pair (row r, columns col, col + 1) in a float64 x tile: one whole 16-byte chunk, boxes of 16 columns
+__device__ __forceinline__ int tile_ofs_x64(int r, int col) { return (col >> 4) * BOX_BYTES + r * 128 + ((((col & 15) >> 1) ^ (r & 7)) << 4); }
 
 __device__ __forceinline__ void warpgroup_sync(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(wg + 1) : "memory"); }
 
@@ -181,7 +191,11 @@ __device__ __forceinline__ void fence_frag(uint32_t (&f)[R][C]) {
 }
 
 // ------------------------------------------------------------------------------------------------ kernel
-__global__ void __launch_bounds__(NTHREADS, 1) ffae_tc_kernel(const __grid_constant__ TcArgs a) {
+// X64: x is float64 and the slot's input scaler is applied as each element is read (a.x_scale / a.x_offset).
+template <bool X64, int NWG>
+__global__ void __launch_bounds__(128 * NWG, 1) ffae_tc_kernel(const __grid_constant__ TcArgs a) {
+  constexpr int NTHREADS = 128 * NWG;
+  constexpr int RESTAGE_BATCH = restage_batch(NTHREADS);
   extern __shared__ __align__(1024) uint8_t smem[];
   const int tid = threadIdx.x, lane = tid & 31;
   const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
@@ -196,7 +210,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) ffae_tc_kernel(const __grid_const
   // this warpgroup's x and y tiles, and the mbarriers their TMA loads complete on; thread 0 of the warpgroup issues the loads
   __shared__ __align__(8) unsigned long long s_bar[2 * NWG];
   const uint32_t stage = (sbase + a.stage_ofs + 1023) & ~1023u;
-  const uint32_t xbuf = stage + wg * 2 * TILE_BYTES, ybuf = xbuf + TILE_BYTES;
+  const uint32_t xbuf = stage + wg * (x_tile_bytes(X64) + TILE_BYTES), ybuf = xbuf + x_tile_bytes(X64);
   const uint8_t* xs = smem + (xbuf - sbase);
   const uint8_t* ys = smem + (ybuf - sbase);
   const uint32_t bar_x = smem_u32(&s_bar[wg]), bar_y = smem_u32(&s_bar[NWG + wg]);
@@ -261,8 +275,18 @@ __global__ void __launch_bounds__(NTHREADS, 1) ffae_tc_kernel(const __grid_const
       tma_load_2d(buf, m, 0, row, bar);
       tma_load_2d(buf + BOX_BYTES, m, BOX_COLS, row, bar);
     };
+    // ... and a float64 x tile: four boxes of 16 columns
+    auto load_x64 = [&](int tt) {
+      const int row = (int)(job.x_row + row_begin + tt * TILE);
+      mbar_expect_tx(bar_x, x_tile_bytes(true));
+#pragma unroll
+      for (int h = 0; h < 4; ++h) tma_load_2d(xbuf + h * BOX_BYTES, &a.tm_x, BOX_COLS_X64 * h, row, bar_x);
+    };
     // the x buffer is free between items (the last tile requested no successor): the first tile loads behind the restage
-    if (leader && wg < n_tiles) load_tile(&a.tm_x, xbuf, bar_x, wg);
+    if (leader && wg < n_tiles) {
+      if constexpr (X64) load_x64(wg);
+      else load_tile(&a.tm_x, xbuf, bar_x, wg);
+    }
 
     // ---- stage this slot's weights: split (layer 0: TF32-hi + BF16 hi / lo, others: FP16 pair) as K-major wgmma B operands
     if (job.slot != cur_slot) {
@@ -323,6 +347,13 @@ __global__ void __launch_bounds__(NTHREADS, 1) ffae_tc_kernel(const __grid_const
         vec[tid] = sc;
         vec[W + tid] = vt && a.feat_thr ? 1.0f / ft : 0.f;
       }
+      if constexpr (X64) {  // zero past T: the zero-filled columns of an x tile stay exactly 0 through x * 0 + 0
+        double* xab = reinterpret_cast<double*>(smem + a.xab_ofs);
+        if (tid < W) {
+          xab[tid] = vt ? __ldg(a.x_scale + (long)job.slot * TP + tid) : 0.0;
+          xab[W + tid] = vt ? __ldg(a.x_offset + (long)job.slot * TP + tid) : 0.0;
+        }
+      }
       fence_proxy_async();  // generic-proxy writes above are read by the tensor cores (async proxy)
     }
     __syncthreads();
@@ -337,19 +368,41 @@ __global__ void __launch_bounds__(NTHREADS, 1) ffae_tc_kernel(const __grid_const
         float xr[2][16];  // this thread's x: rows g, g+8 of its warp; per 16 columns the pairs 2t, 2t+1 and 2t+8, 2t+9
         mbar_wait(bar_x, x_phase);
         x_phase ^= 1;
+        if constexpr (X64) {
+          // x' = (float)(x * a + b): two roundings in double (no fma) and one to float, as gb_affine_f64 computes it.  Rows past the
+          // end of x arrive as zeros and stay zeros, as in the float32 mode (columns past T do through a = b = 0).
+          const double* xab = reinterpret_cast<const double*>(smem + a.xab_ofs);
+          const long row0 = job.x_row + row_begin + tt * TILE + wq * 16 + g;
 #pragma unroll
-        for (int hr = 0; hr < 2; ++hr)
+          for (int hr = 0; hr < 2; ++hr) {
+            const bool live = row0 + 8 * hr < a.n_x_rows;
 #pragma unroll
-          for (int c = 0; c < 8; ++c) {
-            const float2 v = *reinterpret_cast<const float2*>(xs + tile_ofs(wq * 16 + g + 8 * hr, 8 * c + 2 * t));
-            xr[hr][2 * c] = v.x;
-            xr[hr][2 * c + 1] = v.y;
+            for (int c = 0; c < 8; ++c) {
+              const int col = 8 * c + 2 * t;
+              const double2 v = *reinterpret_cast<const double2*>(xs + tile_ofs_x64(wq * 16 + g + 8 * hr, col));
+              const double2 s = *reinterpret_cast<const double2*>(xab + col), o = *reinterpret_cast<const double2*>(xab + W + col);
+              xr[hr][2 * c] = live ? (float)__dadd_rn(__dmul_rn(v.x, s.x), o.x) : 0.f;
+              xr[hr][2 * c + 1] = live ? (float)__dadd_rn(__dmul_rn(v.y, s.y), o.y) : 0.f;
+            }
           }
+        } else {
+#pragma unroll
+          for (int hr = 0; hr < 2; ++hr)
+#pragma unroll
+            for (int c = 0; c < 8; ++c) {
+              const float2 v = *reinterpret_cast<const float2*>(xs + tile_ofs(wq * 16 + g + 8 * hr, 8 * c + 2 * t));
+              xr[hr][2 * c] = v.x;
+              xr[hr][2 * c + 1] = v.y;
+            }
+        }
         // the y tile holds the staged outputs of the previous tile: every warp's stores must have read them before y is refilled
         if (lane == 0) bulk_wait_read<0>();
         warpgroup_sync(wg);  // the whole warpgroup has read x: the buffer takes the next tile's rows, which load behind this tile's layers
         if (leader) {
-          if (tt + NWG < n_tiles) load_tile(&a.tm_x, xbuf, bar_x, tt + NWG);
+          if (tt + NWG < n_tiles) {
+            if constexpr (X64) load_x64(tt + NWG);
+            else load_tile(&a.tm_x, xbuf, bar_x, tt + NWG);
+          }
           if (has_y) load_tile(&a.tm_y, ybuf, bar_y, tt);  // behind layers 1 ..
         }
         uint32_t xhi[4][8], alo[4][4], abf[4][4];
@@ -552,8 +605,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) ffae_tc_kernel(const __grid_const
 constexpr int WORK_CTRS = 1024;
 __device__ unsigned int g_work_ctr[WORK_CTRS];
 
-// Shared-memory layout of the kernel for this architecture (fills the shape and offset fields of `a`); returns its bytes.
-int plan_smem(const gb_ffnet* net, TcArgs& a) {
+// Shared-memory layout of the kernel for this architecture, x mode and warpgroup count (fills the shape and offset fields of
+// `a`); returns its bytes.
+int plan_smem(const gb_ffnet* net, TcArgs& a, bool x64 = false, int nwg = NWG_MAX) {
   const int L = net->n_layers;
   a.L = L;
   a.T = net->dims[0];
@@ -582,8 +636,23 @@ int plan_smem(const gb_ffnet* net, TcArgs& a) {
   a.w_bytes = gb::round_up(ofs, 16);
   ofs = a.w_bytes;
   a.vec_ofs = ofs; ofs += 2 * W * 4;
-  a.stage_ofs = ofs; ofs += 1024 + STAGE_BYTES;  // (the kernel aligns the tiles up to 1024 bytes inside this slack)
+  if (x64) {
+    a.xab_ofs = ofs; ofs += 2 * W * 8;
+  }
+  a.stage_ofs = ofs; ofs += 1024 + stage_bytes(x64, nwg);  // (the kernel aligns the tiles up to 1024 bytes inside this slack)
   return ofs;
+}
+
+constexpr int SMEM_MAX = 227 * 1024;
+
+// Warpgroups of a launch with float64 x: three when their tiles fit next to this stack's weights (feedforward_hourglass(64) does
+// not: 90 KB of weights), else two, whose tiles take the bytes of three float32 ones; 0 when neither fits.
+int x64_warpgroups(const gb_ffnet* net, TcArgs& a, int* smem) {
+  for (int nwg = NWG_MAX; nwg >= 2; --nwg) {
+    *smem = plan_smem(net, a, true, nwg);
+    if (*smem <= SMEM_MAX) return nwg;
+  }
+  return 0;
 }
 
 }  // namespace
@@ -607,28 +676,52 @@ extern "C" int gb_ffae_tc_supported(const gb_ffnet* net) {
     }
   TcArgs a{};
   const int smem = plan_smem(net, a);
-  if (smem > 227 * 1024) {
+  if (smem > SMEM_MAX) {
     gb::set_error("tensor-core variant: the weights and x / y tiles of this stack need %d bytes of shared memory (227 KB per SM)", smem);
     return GB_E_SHAPE;
   }
   return GB_OK;
 }
 
+// float64 x mode: the warpgroups its launch runs with (3 or 2), GB_E_SHAPE outside the variant's range, GB_E_SMEM when the
+// stack's weights leave no room for two warpgroups' float64 x tiles.
+extern "C" int gb_ffae_tc_warpgroups_x64(const gb_ffnet* net) {
+  int rc = gb_ffae_tc_supported(net);
+  if (rc != GB_OK) return rc;
+  TcArgs a{};
+  int smem = 0;
+  const int nwg = x64_warpgroups(net, a, &smem);
+  GB_REQUIRE(nwg > 0, GB_E_SMEM, "tensor-core variant with float64 x: the weights and two warpgroups' x / y tiles of this stack need %d "
+             "bytes of shared memory (227 KB per SM)", smem);
+  return nwg;
+}
+
+// x_scale == NULL: x is float32.  Otherwise x is float64 and x_scale / x_offset [n_slots][T] double are the slot's input scaler.
 extern "C" int gb_ffae_infer_score_tc(const gb_ffnet* net, const float* params, const gb_job* jobs, int32_t n_jobs, int32_t max_rows,
-                                      int64_t n_x_rows, int64_t n_out_rows, const float* x, const float* y, const float* scale,
-                                      const float* feat_thr, const float* agg_thr, float* out_model, float* out_tag_scaled,
-                                      float* out_tag_unscaled, float* out_total_scaled, float* out_total_unscaled, float* out_conf,
-                                      float* out_total_conf, int32_t flags, void* stream) {
+                                      int64_t n_x_rows, int64_t n_out_rows, const void* x, const double* x_scale, const double* x_offset,
+                                      const float* y, const float* scale, const float* feat_thr, const float* agg_thr, float* out_model,
+                                      float* out_tag_scaled, float* out_tag_unscaled, float* out_total_scaled, float* out_total_unscaled,
+                                      float* out_conf, float* out_total_conf, int32_t flags, void* stream) {
   int rc = gb_ffae_tc_supported(net);
   if (rc != GB_OK) return rc;
   GB_REQUIRE(flags == 0, GB_E_ARG, "variant bits above the low byte must be 0");
   GB_REQUIRE(n_x_rows > 0 && n_out_rows > 0, GB_E_ARG, "the tensor-core variant needs the row counts of x and of the outputs");
+  const bool x64 = x_scale != nullptr;
   TcArgs a{};
-  const size_t smem = (size_t)plan_smem(net, a);
+  int nwg = NWG_MAX, smem_i = 0;
+  if (x64) {
+    nwg = gb_ffae_tc_warpgroups_x64(net);
+    if (nwg < 0) return nwg;
+    x64_warpgroups(net, a, &smem_i);
+  } else {
+    smem_i = plan_smem(net, a);
+  }
+  const size_t smem = (size_t)smem_i;
   GB_REQUIRE(n_x_rows < (1L << 31), GB_E_ARG, "%ld rows of x: TMA row coordinates are 32-bit", (long)n_x_rows);
   GB_REQUIRE(n_out_rows < (1L << 31), GB_E_ARG, "%ld output rows: TMA row coordinates are 32-bit", (long)n_out_rows);
   {
-    CUresult r = gb::sm90::encode_map_2d(&a.tm_x, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, x, n_x_rows, a.T, BOX_COLS, TILE);
+    CUresult r = x64 ? gb::sm90::encode_map_2d(&a.tm_x, CU_TENSOR_MAP_DATA_TYPE_FLOAT64, 8, x, n_x_rows, a.T, BOX_COLS_X64, TILE)
+                     : gb::sm90::encode_map_2d(&a.tm_x, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, x, n_x_rows, a.T, BOX_COLS, TILE);
     if (r == CUDA_SUCCESS && y) r = gb::sm90::encode_map_2d(&a.tm_y, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, y, n_x_rows, a.T, BOX_COLS, TILE);
     float* const outs[4] = {out_model, out_tag_unscaled, out_tag_scaled, out_conf};  // the order of TcArgs::tm_o
     for (int i = 0; i < 4; ++i)
@@ -647,6 +740,7 @@ extern "C" int gb_ffae_infer_score_tc(const gb_ffnet* net, const float* params, 
   a.params = params; a.jobs = jobs; a.y = y; a.scale = scale; a.feat_thr = feat_thr; a.agg_thr = agg_thr;
   a.o_model = out_model; a.o_ts = out_tag_scaled; a.o_tu = out_tag_unscaled; a.o_conf = out_conf;
   a.o_tots = out_total_scaled; a.o_totu = out_total_unscaled; a.o_totconf = out_total_conf;
+  a.x_scale = x_scale; a.x_offset = x_offset; a.n_x_rows = (long)n_x_rows;
 
   const long g_total = (long)n_jobs * tiles_per_job;
   GB_REQUIRE(g_total < (1L << 31), GB_E_ARG, "%ld tiles in one launch: split the fleet", g_total);
@@ -658,8 +752,13 @@ extern "C" int gb_ffae_infer_score_tc(const gb_ffnet* net, const float* params, 
     a.work_ctr = static_cast<unsigned int*>(base) + (next_ctr.fetch_add(1) % WORK_CTRS);
     GB_CUDA_CHECK(cudaMemsetAsync(a.work_ctr, 0, sizeof(unsigned int), (cudaStream_t)stream));
   }
-  GB_CUDA_CHECK(cudaFuncSetAttribute(ffae_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  ffae_tc_kernel<<<grid, NTHREADS, smem, (cudaStream_t)stream>>>(a);
+  auto launch = [&](auto kern, int nthreads) -> int {
+    GB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kern<<<grid, nthreads, smem, (cudaStream_t)stream>>>(a);
+    return GB_OK;
+  };
+  rc = !x64 ? launch(ffae_tc_kernel<false, 3>, 384) : nwg == 3 ? launch(ffae_tc_kernel<true, 3>, 384) : launch(ffae_tc_kernel<true, 2>, 256);
+  if (rc != GB_OK) return rc;
   GB_CUDA_CHECK(cudaGetLastError());
   return GB_OK;
 }

@@ -80,23 +80,28 @@ size_t gb_ffnet_param_count(const gb_ffnet* net) {
 
 size_t gb_ffnet_param_stride(const gb_ffnet* net) { return (gb_ffnet_param_count(net) + 3) / 4 * 4; }
 
-// kernel variants (defined in their own translation units)
-int gb_ffae_infer_score_fma(const gb_ffnet*, const float*, const gb_job*, int32_t, int32_t, const float*, const float*,
-                            const float*, const float*, const float*, float*, float*, float*, float*, float*, float*,
+// kernel variants (defined in their own translation units); x_scale == NULL: x is float32, else float64 through the input scaler
+int gb_ffae_infer_score_fma(const gb_ffnet*, const float*, const gb_job*, int32_t, int32_t, const void*, const double*, const double*,
+                            const float*, const float*, const float*, const float*, float*, float*, float*, float*, float*, float*,
                             float*, void*);
 int gb_ffae_small_supported(const gb_ffnet*);
-int gb_ffae_infer_score_small(const gb_ffnet*, const float*, const gb_job*, int32_t, int32_t, const float*, const float*, const float*,
-                              const float*, const float*, float*, float*, float*, float*, float*, float*, float*, void*);
-int gb_ffae_infer_score_tc(const gb_ffnet*, const float*, const gb_job*, int32_t, int32_t, int64_t, int64_t, const float*,
-                           const float*, const float*, const float*, const float*, float*, float*, float*, float*, float*,
+int gb_ffae_infer_score_small(const gb_ffnet*, const float*, const gb_job*, int32_t, int32_t, const void*, const double*, const double*,
+                              const float*, const float*, const float*, const float*, float*, float*, float*, float*, float*, float*,
+                              float*, void*);
+int gb_ffae_infer_score_tc(const gb_ffnet*, const float*, const gb_job*, int32_t, int32_t, int64_t, int64_t, const void*, const double*,
+                           const double*, const float*, const float*, const float*, const float*, float*, float*, float*, float*, float*,
                            float*, float*, int32_t, void*);
-int gb_ffae_tc_supported(const gb_ffnet*);
+int gb_ffae_tc_warpgroups_x64(const gb_ffnet*);
 
-int gb_ffae_infer_score(const gb_ffnet* net, const float* params, const gb_job* jobs, int32_t n_jobs, int32_t max_rows,
-                        int64_t n_x_rows, int64_t n_out_rows, const float* x, const float* y, const float* scale, const float* feat_thr,
-                        const float* agg_thr, float* out_model, float* out_tag_scaled, float* out_tag_unscaled,
-                        float* out_total_scaled, float* out_total_unscaled, float* out_conf, float* out_total_conf,
-                        int32_t variant, void* stream) {
+}  // extern "C"
+
+namespace {
+
+int infer_score(const gb_ffnet* net, const float* params, const gb_job* jobs, int32_t n_jobs, int32_t max_rows, int64_t n_x_rows,
+                int64_t n_out_rows, const void* x, const double* x_scale, const double* x_offset, const float* y, const float* scale,
+                const float* feat_thr, const float* agg_thr, float* out_model, float* out_tag_scaled, float* out_tag_unscaled,
+                float* out_total_scaled, float* out_total_unscaled, float* out_conf, float* out_total_conf, int32_t variant,
+                void* stream) {
   int rc = gb::validate_ffnet(net);
   if (rc != GB_OK) return rc;
   GB_REQUIRE(params && jobs && x && out_model, GB_E_ARG, "params/jobs/x/out_model must be non-NULL");
@@ -119,17 +124,63 @@ int gb_ffae_infer_score(const gb_ffnet* net, const float* params, const gb_job* 
   bool tc_ok = gb_ffae_tc_supported(net) == GB_OK;
   if (variant == 2 && !tc_ok) return GB_E_SHAPE;
   if (variant == 2 || (variant == 0 && tc_ok))
-    return gb_ffae_infer_score_tc(net, params, jobs, n_jobs, max_rows, n_x_rows, n_out_rows, x, y, scale, feat_thr, agg_thr,
-                                  out_model, out_tag_scaled, out_tag_unscaled, out_total_scaled, out_total_unscaled, out_conf,
+    return gb_ffae_infer_score_tc(net, params, jobs, n_jobs, max_rows, n_x_rows, n_out_rows, x, x_scale, x_offset, y, scale, feat_thr,
+                                  agg_thr, out_model, out_tag_scaled, out_tag_unscaled, out_total_scaled, out_total_unscaled, out_conf,
                                   out_total_conf, tc_flags, stream);
   const bool small_ok = gb_ffae_small_supported(net) == GB_OK;
   if (variant == 3 && !small_ok) return GB_E_SHAPE;
   if (variant == 3 || (variant == 0 && small_ok))
-    return gb_ffae_infer_score_small(net, params, jobs, n_jobs, max_rows, x, y, scale, feat_thr, agg_thr, out_model, out_tag_scaled,
-                                     out_tag_unscaled, out_total_scaled, out_total_unscaled, out_conf, out_total_conf, stream);
-  return gb_ffae_infer_score_fma(net, params, jobs, n_jobs, max_rows, x, y, scale, feat_thr, agg_thr, out_model,
-                                 out_tag_scaled, out_tag_unscaled, out_total_scaled, out_total_unscaled, out_conf,
-                                 out_total_conf, stream);
+    return gb_ffae_infer_score_small(net, params, jobs, n_jobs, max_rows, x, x_scale, x_offset, y, scale, feat_thr, agg_thr, out_model,
+                                     out_tag_scaled, out_tag_unscaled, out_total_scaled, out_total_unscaled, out_conf, out_total_conf,
+                                     stream);
+  return gb_ffae_infer_score_fma(net, params, jobs, n_jobs, max_rows, x, x_scale, x_offset, y, scale, feat_thr, agg_thr, out_model,
+                                 out_tag_scaled, out_tag_unscaled, out_total_scaled, out_total_unscaled, out_conf, out_total_conf,
+                                 stream);
+}
+
+}  // namespace
+
+extern "C" {
+
+int gb_ffae_infer_score(const gb_ffnet* net, const float* params, const gb_job* jobs, int32_t n_jobs, int32_t max_rows,
+                        int64_t n_x_rows, int64_t n_out_rows, const float* x, const float* y, const float* scale, const float* feat_thr,
+                        const float* agg_thr, float* out_model, float* out_tag_scaled, float* out_tag_unscaled,
+                        float* out_total_scaled, float* out_total_unscaled, float* out_conf, float* out_total_conf,
+                        int32_t variant, void* stream) {
+  return infer_score(net, params, jobs, n_jobs, max_rows, n_x_rows, n_out_rows, x, nullptr, nullptr, y, scale, feat_thr, agg_thr,
+                     out_model, out_tag_scaled, out_tag_unscaled, out_total_scaled, out_total_unscaled, out_conf, out_total_conf, variant,
+                     stream);
+}
+
+int gb_ffae_infer_score_x64(const gb_ffnet* net, const float* params, const gb_job* jobs, int32_t n_jobs, int32_t max_rows,
+                            int64_t n_x_rows, int64_t n_out_rows, const double* x, const double* x_scale, const double* x_offset,
+                            const float* y, const float* scale, const float* feat_thr, const float* agg_thr, float* out_model,
+                            float* out_tag_scaled, float* out_tag_unscaled, float* out_total_scaled, float* out_total_unscaled,
+                            float* out_conf, float* out_total_conf, int32_t variant, void* stream) {
+  GB_REQUIRE(x_scale && x_offset, GB_E_ARG, "x_scale/x_offset must be non-NULL");
+  return infer_score(net, params, jobs, n_jobs, max_rows, n_x_rows, n_out_rows, x, x_scale, x_offset, y, scale, feat_thr, agg_thr,
+                     out_model, out_tag_scaled, out_tag_unscaled, out_total_scaled, out_total_unscaled, out_conf, out_total_conf, variant,
+                     stream);
+}
+
+int gb_ffae_infer_plan_x64(const gb_ffnet* net, int32_t variant, int32_t* kernel, int32_t* tc_warpgroups) {
+  int rc = gb::validate_ffnet(net);
+  if (rc != GB_OK) return rc;
+  GB_REQUIRE(variant >= 0 && variant <= 3, GB_E_ARG, "variant=%d unknown (debug bits above the low byte are not part of a plan)", variant);
+  int k = variant, nwg = 0;
+  if (k == 0) k = gb_ffae_tc_supported(net) == GB_OK ? 2 : gb_ffae_small_supported(net) == GB_OK ? 3 : 1;
+  if (k == 2) {
+    nwg = gb_ffae_tc_warpgroups_x64(net);
+    if (nwg < 0) return nwg;
+  } else if (k == 3) {
+    if (gb_ffae_small_supported(net) != GB_OK) return GB_E_SHAPE;
+  } else {
+    rc = gb_ffae_infer_plan(net, nullptr, nullptr);
+    if (rc != GB_OK) return rc;
+  }
+  if (kernel) *kernel = k;
+  if (tc_warpgroups) *tc_warpgroups = nwg;
+  return GB_OK;
 }
 
 }  // extern "C"

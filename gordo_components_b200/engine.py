@@ -121,10 +121,14 @@ class FFEngine:
 
     # ------------------------------------------------------------------ K1 + K4
     def infer_score(self, params, jobs_dev, n_jobs: int, max_rows: int, x, y=None, scale=None, feat_thr=None, agg_thr=None,
-                    out_rows: Optional[int] = None, want: Sequence[str] = SCORE_KEYS, variant: int = 0, out: Optional[Dict] = None):
+                    out_rows: Optional[int] = None, want: Sequence[str] = SCORE_KEYS, variant: int = 0, out: Optional[Dict] = None,
+                    x_affine=None):
         """
         One fused launch: model output (+ the requested anomaly columns) for every job.
         ``want`` selects score outputs (names as in the anomaly frame); outputs are float32 device tensors.
+        ``x_affine``: None, or (a, b) float64 device tensors [n_slots, n_in], the per-slot input scaler of a Pipeline.  ``x`` is then
+        float64 and the kernel applies ``(float)(x * a + b)`` as it reads it (gb_ffae_infer_score_x64): bit for bit ``affine_f64``
+        followed by this call with the float32 result, on the same variant, in one launch.
         """
         torch = _torch()
         total = int(out_rows if out_rows is not None else x.shape[0])
@@ -152,10 +156,26 @@ class FFEngine:
         o_conf = g("anomaly-confidence", (total, self.n_out))
         o_totc = g("total-anomaly-confidence", (total,))
         p = _cabi.ptr
-        _cabi.check(self.lib.gb_ffae_infer_score(
-            C.byref(self.net), p(params), p(jobs_dev), int(n_jobs), int(max_rows), int(x.shape[0]), total, p(x), p(y), p(scale), p(feat_thr), p(agg_thr),
-            p(o_model), p(o_ts), p(o_tu), p(o_tots), p(o_totu), p(o_conf), p(o_totc), int(variant), _stream_ptr()))
+        outs = (p(o_model), p(o_ts), p(o_tu), p(o_tots), p(o_totu), p(o_conf), p(o_totc), int(variant), _stream_ptr())
+        if x_affine is None:
+            _cabi.check(self.lib.gb_ffae_infer_score(
+                C.byref(self.net), p(params), p(jobs_dev), int(n_jobs), int(max_rows), int(x.shape[0]), total, p(x), p(y), p(scale), p(feat_thr),
+                p(agg_thr), *outs))
+        else:
+            a, b = x_affine
+            if x.dtype != torch.float64 or a.dtype != torch.float64 or b.dtype != torch.float64:
+                raise ValueError(f"x_affine takes float64 x, scale and offset, got {x.dtype}, {a.dtype}, {b.dtype}")
+            _cabi.check(self.lib.gb_ffae_infer_score_x64(
+                C.byref(self.net), p(params), p(jobs_dev), int(n_jobs), int(max_rows), int(x.shape[0]), total, p(x), p(a), p(b), p(y), p(scale),
+                p(feat_thr), p(agg_thr), *outs))
         return res
+
+    def infer_plan_x64(self, variant: int = 0):
+        """(kernel, tensor-core warpgroups) ``infer_score(..., x_affine=...)`` runs on ``variant`` (gb_ffae_infer_plan_x64; no device
+        work), or None when it refuses this architecture there."""
+        kernel, nwg = C.c_int32(0), C.c_int32(0)
+        rc = self.lib.gb_ffae_infer_plan_x64(C.byref(self.net), int(variant), C.byref(kernel), C.byref(nwg))
+        return (kernel.value, nwg.value) if rc == 0 else None
 
     # ------------------------------------------------------------------ K2
     def fit(self, params, jobs_dev, n_jobs: int, max_rows: int, x, y, epochs: int = 1, batch_size: int = 32, shuffle=True,

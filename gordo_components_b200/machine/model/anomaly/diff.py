@@ -295,15 +295,20 @@ class DiffBasedAnomalyDetector(AnomalyDetectorBase):
             pre, ae = fused
             eng = ae._engine()
             affine = _compose_affine(pre, eng.n_in)
-            variant = 0
+            variant, x_affine = 0, None
             if pre and affine is not None:
-                # per-feature scalers in front of the network: one f64 pass on the device (gb_affine_f64) instead of sklearn on the host
+                # per-feature scalers in front of the network, in float64 on the device instead of sklearn on the host: applied by the
+                # fused kernel as it reads x (gb_ffae_infer_score_x64), or, for a stack that mode does not hold, as a separate pass
+                # (gb_affine_f64) -- the same float32 x' either way, so the same bits out
                 Xv = np.ascontiguousarray(_values(X), dtype=np.float64)
                 _refuse_infinity(Xv)  # what the sklearn steps would have raised
                 n = len(Xv)
                 jobs = engine.jobs_to_device(engine.make_jobs([0], [n], [0]), dev)
                 a_d, b_d = (torch.from_numpy(v.reshape(1, -1)).to(dev) for v in affine)
-                xd = engine.affine_f64(jobs, 1, n, torch.from_numpy(Xv).to(dev), a_d, b_d) if n else torch.empty((0, eng.n_in), dtype=torch.float32, device=dev)
+                if n and eng.infer_plan_x64(variant) is not None:
+                    xd, x_affine = torch.from_numpy(Xv).to(dev), (a_d, b_d)
+                else:
+                    xd = engine.affine_f64(jobs, 1, n, torch.from_numpy(Xv).to(dev), a_d, b_d) if n else torch.empty((0, eng.n_in), dtype=torch.float32, device=dev)
             else:
                 Xt = X
                 for step in pre:
@@ -317,7 +322,7 @@ class DiffBasedAnomalyDetector(AnomalyDetectorBase):
                     # turns ±inf into NaN, so an input holding ±inf is not given to it
                     variant = 1
             yd = engine.to_device_f32(yv, dev)
-            res = eng.infer_score(ae._device_params(), jobs, 1, n, xd, yd, scale_d, ft_d, at_d, want=want, variant=variant)
+            res = eng.infer_score(ae._device_params(), jobs, 1, n, xd, yd, scale_d, ft_d, at_d, want=want, variant=variant, x_affine=x_affine)
         else:
             # diff.py:350-385: pandas arithmetic on float64 y and the (float32- or float64-valued) predictions widened to float64
             pred = np.asarray(estimator_owner.predict(X) if hasattr(estimator_owner, "predict") else estimator_owner.transform(X))

@@ -246,47 +246,64 @@ class ResidentBucket:
     models -- become one fused launch.  Eligible: this package's ``DiffBasedAnomalyDetector`` around a bare ``KerasAutoEncoder``
     (no smoothing window, an affine error scaler); pass ``bucket=`` to ``anomaly_prediction`` and every eligible model is answered
     through it, the rest as before.  The replies are the same bytes either way (rows are independent in the kernel).
+
+    ``input_scalers=True`` also admits the definition the reference's examples deploy, a ``Pipeline`` of per-feature scalers
+    (MinMaxScaler, StandardScaler, RobustScaler, MaxAbsScaler) ending in a ``KerasAutoEncoder``: the composed float64 scaler of
+    each model rides with its weights, and the launch applies it as it reads X (``serving.AnomalyCoalescer(x_scale=, x_offset=)``).
+    Bare and Pipeline models never share a bucket.
     """
 
-    def __init__(self, store: "ModelStore", names: Optional[List[str]] = None, **coalescer_kwargs):
+    input_scalers = False  # the bucket holds Pipeline models (set by the constructor)
+
+    def __init__(self, store: "ModelStore", names: Optional[List[str]] = None, input_scalers: bool = False, **coalescer_kwargs):
         from . import engine
-        from .machine.model.anomaly.diff import _scaler_multiplier
+        from .machine.model.anomaly.diff import _compose_affine, _scaler_multiplier
         from .serving import AnomalyCoalescer
 
         groups: Dict[Any, List[str]] = {}
         for name in names if names is not None else store.names():
             model = store.model(name)
-            if self.eligible(model):
-                spec = model.base_estimator.model.spec
+            if self.eligible(model, input_scalers):
+                pre, ae = _served_parts(model)
+                spec = ae.model.spec
                 has_thr = tuple(t is not None for t in model._thresholds())
-                groups.setdefault((tuple(spec.dims), tuple(spec.acts), tuple(spec.l1), has_thr), []).append(name)
+                groups.setdefault((tuple(spec.dims), tuple(spec.acts), tuple(spec.l1), has_thr, bool(pre)), []).append(name)
         if not groups:
             raise ValueError("no model in the store can be served through a coalescer")
         self.names = max(groups.values(), key=len)  # the largest architecture group
         self.slot = {name: i for i, name in enumerate(self.names)}
         models = [store.model(n) for n in self.names]
-        spec = models[0].base_estimator.model.spec
+        parts = [_served_parts(m) for m in models]
+        spec = parts[0][1].model.spec
         eng = engine.ff_engine_for(spec)
         torch = engine._torch()
-        params = eng.pack_params([m.base_estimator.model.weights for m in models])
-        to_dev = lambda rows: torch.from_numpy(np.ascontiguousarray(np.stack(rows), dtype=np.float32)).to(eng.device)  # noqa: E731
+        params = eng.pack_params([ae.model.weights for _, ae in parts])
+        to_dev = lambda rows, dt=np.float32: torch.from_numpy(np.ascontiguousarray(np.stack(rows), dtype=dt)).to(eng.device)  # noqa: E731
         scale = to_dev([_scaler_multiplier(m.scaler, eng.n_out) for m in models])
         feat, agg = zip(*(m._thresholds() for m in models))
         feat_thr = to_dev([np.asarray(f, dtype=np.float32) for f in feat]) if feat[0] is not None else None
         agg_thr = to_dev([np.float32(a) for a in agg]) if agg[0] is not None else None
+        self.input_scalers = bool(parts[0][0])
+        if self.input_scalers:
+            a, b = zip(*(_compose_affine(pre, eng.n_in) for pre, _ in parts))
+            coalescer_kwargs.update(x_scale=to_dev(a, np.float64), x_offset=to_dev(b, np.float64))
         self.coalescer = AnomalyCoalescer(eng, params, scale, feat_thr, agg_thr, **coalescer_kwargs)
 
     @staticmethod
-    def eligible(model) -> bool:
-        from .machine.model.models import KerasAutoEncoder
-
-        if not (_frame_is_from_blocks(model) and type(model.base_estimator) is KerasAutoEncoder and model.base_estimator.model is not None
-                and model.window is None and not (model.require_thresholds and all(t is None for t in model._thresholds()))):
+    def eligible(model, input_scalers: bool = False) -> bool:
+        if not (_frame_is_from_blocks(model) and model.window is None
+                and not (model.require_thresholds and all(t is None for t in model._thresholds()))):
             return False
-        from .machine.model.anomaly.diff import _scaler_multiplier
+        parts = _served_parts(model)
+        if parts is None or parts[1].model is None or (parts[0] and not input_scalers):
+            return False
+        pre, ae = parts
+        from .machine.model.anomaly.diff import _compose_affine, _scaler_multiplier
 
+        if pre and (_compose_affine(pre, ae.model.spec.dims[0]) is None or not _x64_launch_holds(ae.model.spec)):
+            return False  # served per request: sklearn's own transform, or the separate gb_affine_f64 pass
         try:  # a non-affine error scaler (clip=True, QuantileTransformer, ...) is served on the per-request path, not refused for the whole store
-            _scaler_multiplier(model.scaler, model.base_estimator.model.spec.dims[-1])
+            _scaler_multiplier(model.scaler, ae.model.spec.dims[-1])
         except (ValueError, AttributeError):
             return False
         return True
@@ -296,7 +313,10 @@ class ResidentBucket:
 
         model = store.model(name)
         _refuse_infinity(_values(y))
-        if _has_inf(_values(X)):
+        if self.input_scalers:
+            # what the Pipeline's sklearn steps raise, as the per-request route does before any launch
+            _refuse_infinity(np.ascontiguousarray(_values(X), dtype=np.float64))
+        elif _has_inf(_values(X)):
             # the coalescer's launch may run the tensor-core kernel, which does not take ±inf inputs: this request goes on its own
             return model.anomaly_blocks(X, y, frequency=frequency)
         scores = self.coalescer.anomaly(self.slot[name], X, y)
@@ -327,6 +347,31 @@ def _extract_X_y(store: ModelStore, name: str, json: Optional[dict], files: Opti
         if isinstance(y, Reply):
             return y
     return X, y
+
+
+def _served_parts(model):
+    """(input scaler steps, ``KerasAutoEncoder``) of a detector whose base estimator is a bare autoencoder ([] for the steps) or a
+    ``Pipeline`` ending in one, else None."""
+    from sklearn.pipeline import Pipeline
+
+    from .machine.model.models import KerasAutoEncoder
+
+    est = model.base_estimator
+    if type(est) is KerasAutoEncoder:
+        return [], est
+    if type(est) is Pipeline and len(est.steps) > 1 and type(est.steps[-1][1]) is KerasAutoEncoder:
+        return [step for _, step in est.steps[:-1]], est.steps[-1][1]
+    return None
+
+
+def _x64_launch_holds(spec) -> bool:
+    """True when the fused launch with float64 x holds this stack on the kernel the per-request route picks (no device needed)."""
+    import ctypes as C
+
+    from . import _cabi
+
+    lib = _cabi.load_library()
+    return lib.gb_ffae_infer_plan_x64(C.byref(_cabi.make_ffnet(spec.dims, spec.acts, spec.l1)), 0, None, None) == 0
 
 
 def _frame_is_from_blocks(model) -> bool:

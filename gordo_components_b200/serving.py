@@ -12,6 +12,10 @@ requests are waiting into ONE ``gb_ffae_infer_score`` launch (a request is just 
     fut = co.submit(machine_index, X, y)          # any thread; X, y: [rows, tags] arrays
     cols = fut.result()                           # dict of host arrays named like the anomaly frame's blocks
 
+With ``x_scale`` / ``x_offset`` (float64 [n_slots, n_in] device tensors: the composed per-feature input scalers of Pipeline models)
+requests' X is staged as float64 and the launch applies each slot's scaler as it reads x (gb_ffae_infer_score_x64), exactly the
+float32 batch ``gb_affine_f64`` would have produced.
+
 Thread-safe, re-entrant, no shared mutable scratch outside the worker thread (the reference's threading convention,
 SURVEY §8b).  The per-request results are bit-identical to a per-request launch: rows are independent in the kernel.
 """
@@ -31,17 +35,22 @@ from .fleet import PER_ROW, PER_TAG
 
 class AnomalyCoalescer:
     def __init__(self, eng: "engine.FFEngine", params, scale, feat_thr=None, agg_thr=None, max_batch_rows: int = 1 << 18,
-                 max_wait_ms: float = 1.0, want: Optional[Sequence[str]] = None):
+                 max_wait_ms: float = 1.0, want: Optional[Sequence[str]] = None, x_scale=None, x_offset=None):
         torch = engine._torch()
         self.eng, self.params, self.scale, self.feat_thr, self.agg_thr = eng, params, scale, feat_thr, agg_thr
+        if (x_scale is None) != (x_offset is None):
+            raise ValueError("x_scale and x_offset go together")
+        self.x_affine = (x_scale, x_offset) if x_scale is not None else None
+        x_dtype = torch.float64 if self.x_affine is not None else torch.float32
+        self._x_np = np.float64 if self.x_affine is not None else np.float32
         self.max_rows, self.max_wait = int(max_batch_rows), float(max_wait_ms) * 1e-3
         self.want = tuple(want) if want is not None else tuple(
             k for k in PER_TAG + PER_ROW if not ((feat_thr is None and k == "anomaly-confidence") or (agg_thr is None and k == "total-anomaly-confidence")))
         dev = eng.device
         self._stream = torch.cuda.Stream(device=dev)
-        self._xh = torch.empty((self.max_rows, eng.n_in), dtype=torch.float32).pin_memory()
+        self._xh = torch.empty((self.max_rows, eng.n_in), dtype=x_dtype).pin_memory()
         self._yh = torch.empty((self.max_rows, eng.n_out), dtype=torch.float32).pin_memory()
-        self._xd = torch.empty((self.max_rows, eng.n_in), dtype=torch.float32, device=dev)
+        self._xd = torch.empty((self.max_rows, eng.n_in), dtype=x_dtype, device=dev)
         self._yd = torch.empty((self.max_rows, eng.n_out), dtype=torch.float32, device=dev)
         self._out_d = {k: torch.empty((self.max_rows, eng.n_out) if k in PER_TAG else (self.max_rows,), dtype=torch.float32, device=dev) for k in self.want}
         self._out_h = {k: torch.empty(v.shape, dtype=torch.float32).pin_memory() for k, v in self._out_d.items()}
@@ -58,7 +67,7 @@ class AnomalyCoalescer:
         """Queue one request; the Future resolves to {column block: host array} for exactly these rows."""
         if self._closed:
             raise RuntimeError("coalescer is closed")
-        Xv = np.ascontiguousarray(getattr(X, "values", X), dtype=np.float32)
+        Xv = np.ascontiguousarray(getattr(X, "values", X), dtype=self._x_np)
         yv = np.ascontiguousarray(getattr(y, "values", y), dtype=np.float32)
         if Xv.ndim != 2 or Xv.shape[1] != self.eng.n_in or yv.shape != (len(Xv), self.eng.n_out):
             raise ValueError(f"request of shape X {Xv.shape} / y {yv.shape} does not fit a {self.eng.n_in}->{self.eng.n_out} model")
@@ -128,7 +137,8 @@ class AnomalyCoalescer:
             self._yd[:rows].copy_(self._yh[:rows], non_blocking=True)
             if rows:
                 self.eng.infer_score(self.params, jobs_d, len(batch), max_rows, self._xd[:rows], self._yd[:rows], self.scale, self.feat_thr,
-                                     self.agg_thr, out_rows=rows, want=self.want, out={k: v[:rows] for k, v in self._out_d.items()})
+                                     self.agg_thr, out_rows=rows, want=self.want, out={k: v[:rows] for k, v in self._out_d.items()},
+                                     x_affine=self.x_affine)
             for k in self.want:
                 self._out_h[k][:rows].copy_(self._out_d[k][:rows], non_blocking=True)
         self._stream.synchronize()

@@ -135,6 +135,26 @@ int gb_ffae_tc_supported(const gb_ffnet* net);
  * would refuse the architecture on variant 1 for shared memory; either output may be NULL. */
 int gb_ffae_infer_plan(const gb_ffnet* net, int32_t* rows_per_tile, int32_t* resident);
 
+/* gb_ffae_infer_score behind a Pipeline's per-feature input scalers (sklearn MinMaxScaler / StandardScaler / RobustScaler /
+ * MaxAbsScaler .transform in front of the network, composed into one affine map): x is float64 [n_x_rows][n_in], and the kernel
+ * applies x' = (float)((x * x_scale[slot][c]) + x_offset[slot][c]) as it loads each element -- two roundings in double, no fma,
+ * one rounding to float, exactly what gb_affine_f64 writes.  x_scale, x_offset: [n_slots][n_in] double, both non-NULL (GB_E_ARG).
+ * Everything else -- arguments, variants, outputs, the handling of NaN and ±inf in x' -- is that of gb_ffae_infer_score, and the
+ * result is bit for bit gb_affine_f64 followed by gb_ffae_infer_score with the same variant on the same device.  It reads x once
+ * instead of reading it, writing x' and reading x' back.  Variant 2 stages twice the bytes per x tile: a stack whose weights
+ * leave no room for them is GB_E_SMEM (see gb_ffae_infer_plan_x64), never a silent change of kernel. */
+int gb_ffae_infer_score_x64(const gb_ffnet* net, const float* params, const gb_job* jobs, int32_t n_jobs, int32_t max_rows,
+                            int64_t n_x_rows, int64_t n_out_rows, const double* x, const double* x_scale, const double* x_offset,
+                            const float* y, const float* scale, const float* feat_thr, const float* agg_thr, float* out_model,
+                            float* out_tag_scaled, float* out_tag_unscaled, float* out_total_scaled, float* out_total_unscaled,
+                            float* out_conf, float* out_total_conf, int32_t variant, void* stream);
+
+/* The kernel gb_ffae_infer_score_x64 runs for this architecture and variant (0..3, no debug bits), without launching and without
+ * a device: *kernel = 1, 2 or 3 (0 resolved as gb_ffae_infer_score resolves it), *tc_warpgroups = warpgroups per CTA of the
+ * tensor-core launch (3, or 2 when three warpgroups' float64 x tiles do not fit next to the weights; 0 for kernels 1 and 3).
+ * GB_E_SHAPE / GB_E_SMEM exactly when gb_ffae_infer_score_x64 refuses the architecture on that variant; either output may be NULL. */
+int gb_ffae_infer_plan_x64(const gb_ffnet* net, int32_t variant, int32_t* kernel, int32_t* tc_warpgroups);
+
 /* ---- K4 alone: anomaly score of predictions that already exist ----------------------------
  * Same outputs as gb_ffae_infer_score, for a `yhat` produced elsewhere (a base estimator that is not
  * one of ours, e.g. the sklearn regressors the reference's detector tests use; an LSTM prediction from
