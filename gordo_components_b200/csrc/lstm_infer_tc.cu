@@ -44,11 +44,11 @@ constexpr int NTHREADS = 128 * CONSUMERS + 32;       // + one producer warp
 struct TcLayerArgs {
   int u, kc_below, kc_own;           // units; K chunks coming from the layer below / from this layer's own h
   int act;
-  int tiles_per_job, t, n_items;     // n_items counts (window tile, unit block)
-  const gb_job* jobs;
+  int t, n_items;                    // n_items counts (window tile, unit block)
+  const int4* tiles;                 // per flat window tile: {slot, windows of the job from this tile on, job, tile within the job}
   const float* bias;                 // [n_slots][4u] reordered (layers >= 1; layer 0's bias lives in xk)
-  const float* xk;                   // layer 0: input projection of each job's own x rows, [job][row in job / 128][4u reordered][128]
-  int xk_blocks;                     // 128-row blocks per job in xk
+  const float* xk;                   // layer 0: input projection of each job's own x rows, [128-row block][4u reordered][128]
+  int xk_pad;                        // job j's xk blocks begin at tile_base[j] + j * xk_pad (its tiles, plus the lookback's rows)
   float* c;                          // [tile][u][128 windows]
   __half *h_out_hi, *h_out_lo;       // [rows][u]
 };
@@ -110,17 +110,16 @@ lstm_tc_step_kernel(const __grid_constant__ TcLayerArgs a, const __grid_constant
   const int n_chunks = a.kc_below + a.kc_own;
   const int nub = u / UB;
   // item -> (tile, ub): the unit blocks of one window tile are neighbours, so CTAs running side by side read the same A operand from L2
-  struct Item { int tile, tj, ub, slot, n_rows, job; bool real; };
+  struct Item { int tile, ub, slot, rem, job; bool real; };
   auto item_of = [&](int item) -> Item {
     Item it;
     const int grp = item / nub;
     it.ub = item - grp * nub;
-    it.job = grp / a.tiles_per_job;
-    it.tj = grp - it.job * a.tiles_per_job;
     it.tile = grp;
-    const int2 sn = __ldg(reinterpret_cast<const int2*>(a.jobs + it.job));  // slot, n_rows
-    it.slot = sn.x; it.n_rows = sn.y;
-    it.real = it.tj * TILE < it.n_rows;
+    const int2 sr = __ldg(reinterpret_cast<const int2*>(a.tiles + grp));  // slot, windows of the job from this tile on
+    it.slot = sr.x; it.rem = sr.y;
+    it.job = FIRST ? __ldg(reinterpret_cast<const int*>(a.tiles + grp) + 2) : 0;
+    it.real = it.rem > 0;
     return it;
   };
 
@@ -181,16 +180,17 @@ lstm_tc_step_kernel(const __grid_constant__ TcLayerArgs a, const __grid_constant
       if ((tid & 127) == 0) mbar_arrive(bar_empty + 8 * ((cc - 1) % STAGES));
 #pragma unroll
       for (int i = 0; i < 128; ++i) fence_reg(d[i]);
-
 #pragma unroll
       for (int hr = 0; hr < 2; ++hr) {
         const int r = r0 + 8 * hr;
-        const int w = it.tj * TILE + r;  // window index inside the job (may exceed n_rows in the last tile)
         const long row = (long)it.tile * TILE + r;
         const float* xk = nullptr;
-        if (FIRST) {  // xk is stored per job and row-blocked, [job][row / 128][4u reordered][128]
-          const int xr = min(w, it.n_rows - 1) + a.t;  // x row relative to the job's x_row
-          xk = a.xk + (((long)it.job * a.xk_blocks + (xr >> 7)) * (4 * u) + it.ub * NCOL) * TILE + (xr & (TILE - 1));
+        if (FIRST) {
+          // xk is stored per job and row-blocked, the job's blocks from tile_base[job] + job * xk_pad: window tj * 128 + r reads x row
+          // tj * 128 + min(r, rem - 1) + t of the job (the last tile's padding rows repeat its last window), i.e. row xr of block
+          // tile + job * xk_pad
+          const int xr = min(r, it.rem - 1) + a.t;
+          xk = a.xk + (((long)it.tile + (long)it.job * a.xk_pad + (xr >> 7)) * (4 * u) + it.ub * NCOL) * TILE + (xr & (TILE - 1));
         }
         const float* bias = FIRST ? nullptr : a.bias + (long)it.slot * 4 * u + it.ub * NCOL;
         float* ccol = a.c + ((long)it.tile * u + it.ub * UB) * TILE + r;  // unit j of this window: ccol[j * TILE]
@@ -264,14 +264,36 @@ __global__ void lstm_tc_weights_kernel(const float* __restrict__ params, long ps
     }
 }
 
-// layer 0 input projection per x row of a job: xk[job][r][n'] = x[x_row + r] . K0[:, col(n')] + b0[col(n')] with the job's slot;
-// grid (ceil(rows/32), 4u/64, jobs from job0)
-__global__ void __launch_bounds__(256) lstm_tc_xk_kernel(const gb_job* __restrict__ jobs, int job0, const float* __restrict__ x, int F, int u, int up,
-                                                         int lookback, const float* __restrict__ params, long pstride, int xk_blocks,
-                                                         float* __restrict__ xk) {
-  const long job_id = job0 + blockIdx.z;
+// Window tiles are flat: job j owns tiles [tile_base[j], tile_base[j + 1]), ceil(n_rows / 128) of them (the uniform entry gives
+// every job max_windows' count).  The record of each tile lets the step and head kernels find an item's job with one load.
+__global__ void lstm_tc_uniform_tiles_kernel(int n_jobs, int tiles_per_job, int32_t* __restrict__ tile_base) {
+  for (int j = blockIdx.x * blockDim.x + threadIdx.x; j <= n_jobs; j += gridDim.x * blockDim.x) tile_base[j] = j * tiles_per_job;
+}
+
+__global__ void lstm_tc_tiles_kernel(const gb_job* __restrict__ jobs, int n_jobs, const int32_t* __restrict__ tile_base, int n_tiles, int4* __restrict__ tiles) {
+  for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < n_tiles; t += gridDim.x * blockDim.x) {
+    int lo = 0, hi = n_jobs - 1;  // the last job whose first tile is <= t: a job without windows shares its first tile with the next job
+    while (lo < hi) {
+      const int mid = (lo + hi + 1) >> 1;
+      if (__ldg(tile_base + mid) <= t) lo = mid; else hi = mid - 1;
+    }
+    const int tj = t - __ldg(tile_base + lo);
+    const int2 sn = __ldg(reinterpret_cast<const int2*>(jobs + lo));  // slot, n_rows
+    tiles[t] = tj < 0 ? make_int4(sn.x, 0, lo, 0) : make_int4(sn.x, (int)max(0L, sn.y - (long)tj * TILE), lo, tj);  // a tile before job 0's first holds no window
+  }
+}
+
+// layer 0 input projection per x row of a job: xk[block][n'][r] = x[x_row + r] . K0[:, col(n')] + b0[col(n')] with the job's slot;
+// grid (ceil(rows/32), 4u/64, jobs from job0).  Job j writes its n_rows + lookback - 1 rows into the blocks from tile_base[j] + j * xk_pad
+// (never past the next job's first block).
+__global__ void __launch_bounds__(256) lstm_tc_xk_kernel(const gb_job* __restrict__ jobs, int job0, const int32_t* __restrict__ tile_base, int n_tiles,
+                                                         const float* __restrict__ x, int F, int u, int up, int lookback, const float* __restrict__ params,
+                                                         long pstride, int xk_pad, float* __restrict__ xk) {
+  const int job_id = job0 + blockIdx.z;
   const gb_job job = jobs[job_id];
-  const int n_x = job.n_rows + lookback - 1;  // x rows this job's windows touch
+  const int tb0 = __ldg(tile_base + job_id), tb1 = __ldg(tile_base + job_id + 1);
+  if (tb0 < 0 || tb1 < tb0 || tb1 > n_tiles) return;
+  const int n_x = (int)min((long)job.n_rows + lookback - 1, (long)(tb1 - tb0 + xk_pad) * TILE);  // x rows this job's windows touch
   const int r0 = blockIdx.x * 32;
   if (r0 >= n_x) return;
   const float* P = params + (long)job.slot * pstride;  // layer 0: kernel [F][4u] first
@@ -307,28 +329,28 @@ __global__ void __launch_bounds__(256) lstm_tc_xk_kernel(const gb_job* __restric
 #pragma unroll
   for (int i = 0; i < 8; ++i) sW[rg + 4 * i][col] = acc[i] + b;  // sW reused as [32 rows][64 columns]
   __syncthreads();
-  float* xj = xk + job_id * xk_blocks * (4L * up) * TILE;
+  float* xj = xk + ((long)tb0 + (long)job_id * xk_pad) * (4L * up) * TILE;
   for (int i = tid; i < 64 * 32; i += 256) {
     const int c = i >> 5, rr = i & 31, r = r0 + rr;
     if (r < n_x) xj[((r >> 7) * (long)(4 * up) + c0 + c) * TILE + (r & (TILE - 1))] = sW[rr][c];
   }
 }
 
-// Dense head on the last layer's final h: out[w][o] = act(sum_k h[w][k] Wd[k][o] + bd[o]); grid (tiles, jobs from job0)
-__global__ void __launch_bounds__(128) lstm_tc_head_kernel(const gb_job* __restrict__ jobs, int job0, int tiles_per_job, const __half* __restrict__ h_hi,
+// Dense head on the last layer's final h: out[w][o] = act(sum_k h[w][k] Wd[k][o] + bd[o]); one CTA per flat window tile
+__global__ void __launch_bounds__(128) lstm_tc_head_kernel(const gb_job* __restrict__ jobs, const int4* __restrict__ tiles, const __half* __restrict__ h_hi,
                                                            const __half* __restrict__ h_lo, int u, int up, int n_out, int out_act,
                                                            const float* __restrict__ params, long pstride, long dofs, float* __restrict__ out) {
-  const long job_id = job0 + blockIdx.y;
-  const gb_job job = jobs[job_id];
-  const int w = blockIdx.x * TILE + threadIdx.x;
-  if (w >= job.n_rows) return;
-  const long row = (job_id * tiles_per_job + blockIdx.x) * TILE + threadIdx.x;
-  const float* Wd = params + (long)job.slot * pstride + dofs;
+  const int4 rec = tiles[blockIdx.x];  // slot, windows of the job from this tile on, job, tile within the job
+  if ((int)threadIdx.x >= rec.y) return;
+  const int w = rec.w * TILE + threadIdx.x;
+  const long row = (long)blockIdx.x * TILE + threadIdx.x;
+  const long out_row = jobs[rec.z].out_row;
+  const float* Wd = params + (long)rec.x * pstride + dofs;
   const float* bd = Wd + (long)u * n_out;
   for (int o = 0; o < n_out; ++o) {
     float acc = __ldg(bd + o);
     for (int k = 0; k < u; ++k) acc = fmaf(__half2float(h_hi[row * up + k]) + __half2float(h_lo[row * up + k]), __ldg(Wd + (long)k * n_out + o), acc);
-    out[(job.out_row + w) * (long)n_out + o] = gb::apply_act(out_act, acc);
+    out[(out_row + w) * (long)n_out + o] = gb::apply_act(out_act, acc);
   }
 }
 
@@ -344,19 +366,20 @@ struct Plan {
   int nl, F, n_out, L;
   int u[GB_MAX_LAYERS], ur[GB_MAX_LAYERS], in[GB_MAX_LAYERS], kp_below[GB_MAX_LAYERS], kp[GB_MAX_LAYERS];  // u: padded to 64, ur / in: real widths
   long kofs[GB_MAX_LAYERS], dofs;
-  int xk_blocks;  // 128-row blocks of each job's input projection: its windows touch max_windows + lookback - 1 x rows
+  int xk_pad;  // 128-row xk blocks each job has beyond its window tiles: its windows touch n_rows + lookback - 1 x rows
   // workspace offsets (bytes)
   size_t w_hi[GB_MAX_LAYERS], w_lo[GB_MAX_LAYERS], bias[GB_MAX_LAYERS], h_hi[GB_MAX_LAYERS][2], h_lo[GB_MAX_LAYERS][2], c[GB_MAX_LAYERS], xk, total;
+  size_t tile_base, tiles;  // the uniform entry's tile table [n_jobs + 1] and the tile records [n_tiles]
   size_t state_begin, state_end;
 };
 
 size_t align256(size_t v) { return (v + 255) / 256 * 256; }
 
-void make_plan(const gb_lstmnet* net, int n_slots, int n_jobs, int max_windows, Plan* p) {
+// Sizes follow the flat tiles: the recurrent state holds n_tiles * 128 rows, xk n_tiles + n_jobs * xk_pad blocks.
+void make_plan(const gb_lstmnet* net, int n_slots, int n_jobs, long n_tiles, Plan* p) {
   p->nl = net->n_layers; p->F = net->n_features; p->n_out = net->n_features_out; p->L = net->lookback;
-  const long tiles_per_job = (max_windows + TILE - 1) / TILE;
-  const long rows_pad = (long)n_jobs * tiles_per_job * TILE;
-  p->xk_blocks = (int)(((long)max_windows + p->L - 1 + TILE - 1) / TILE);
+  const long rows = n_tiles * TILE;
+  p->xk_pad = (p->L - 1 + TILE - 1) / TILE;  // ceil((n + L - 1) / 128) <= ceil(n / 128) + ceil((L - 1) / 128)
   long pofs = 0;
   int in = net->n_features;
   size_t ofs = 0;
@@ -373,59 +396,56 @@ void make_plan(const gb_lstmnet* net, int n_slots, int n_jobs, int max_windows, 
     in = ur;
   }
   p->dofs = pofs;
-  p->xk = ofs; ofs = align256(ofs + (size_t)n_jobs * p->xk_blocks * TILE * 4 * p->u[0] * sizeof(float));
+  p->tile_base = ofs; ofs = align256(ofs + (size_t)(n_jobs + 1) * sizeof(int32_t));
+  p->tiles = ofs; ofs = align256(ofs + (size_t)n_tiles * sizeof(int4));
+  p->xk = ofs; ofs = align256(ofs + (size_t)(n_tiles + (long)n_jobs * p->xk_pad) * TILE * 4 * p->u[0] * sizeof(float));
   p->state_begin = ofs;
   for (int l = 0; l < p->nl; ++l) {
-    const size_t hb = (size_t)rows_pad * p->u[l] * sizeof(__half);
+    const size_t hb = (size_t)rows * p->u[l] * sizeof(__half);
     for (int b = 0; b < 2; ++b) {
       p->h_hi[l][b] = ofs; ofs = align256(ofs + hb);
       p->h_lo[l][b] = ofs; ofs = align256(ofs + hb);
     }
-    p->c[l] = ofs; ofs = align256(ofs + (size_t)rows_pad * p->u[l] * sizeof(float));
+    p->c[l] = ofs; ofs = align256(ofs + (size_t)rows * p->u[l] * sizeof(float));
   }
   p->state_end = ofs;
   p->total = ofs;
 }
 
-}  // namespace
+constexpr long MAX_TILES = (1L << 31) / (512 / UB) - 1;  // work items (tile, unit block) are counted in int
 
-extern "C" int gb_lstm_tc_supported(const gb_lstmnet* net) {
-  GB_REQUIRE(net != nullptr, GB_E_ARG, "net is NULL");
-  GB_REQUIRE(net->n_layers >= 1 && net->n_layers <= GB_MAX_LAYERS, GB_E_SHAPE, "n_layers=%d outside [1,%d]", net->n_layers, GB_MAX_LAYERS);
-  for (int l = 0; l < net->n_layers; ++l)
-    GB_REQUIRE(net->units[l] >= 1 && net->units[l] <= 512, GB_E_SHAPE, "tensor-core LSTM variant covers layer widths 1..512, units[%d]=%d", l, net->units[l]);
-  GB_REQUIRE(net->n_features >= 1 && net->n_features <= 512 && net->n_features_out >= 1 && net->n_features_out <= 512, GB_E_SHAPE, "bad feature counts");
-  GB_REQUIRE(net->lookback >= 1, GB_E_ARG, "lookback=%d must be >= 1", net->lookback);
-  for (int l = 0; l < net->n_layers; ++l)  // h is carried as an FP16 pair: only cells with |h| < 1
-    GB_REQUIRE(net->act[l] == GB_ACT_TANH || net->act[l] == GB_ACT_SIGMOID, GB_E_SHAPE,
-               "tensor-core LSTM variant covers tanh and sigmoid cells (a relu or linear cell's h overflows FP16), act[%d]=%d", l, net->act[l]);
+// Host-side checks shared by both entries; n_tiles as a long so that a uniform layout too large to count is refused, not wrapped.
+int check_sizes(int32_t n_slots, int32_t n_jobs, long n_tiles, int32_t max_windows) {
+  GB_REQUIRE(n_jobs >= 0 && max_windows >= 0 && n_slots >= 1 && n_tiles >= 0, GB_E_ARG, "bad n_jobs=%d / max_windows=%d / n_slots=%d / n_tiles=%ld",
+             n_jobs, max_windows, n_slots, n_tiles);
+  const long tiles_per_job = ((long)max_windows + TILE - 1) / TILE;
+  GB_REQUIRE(n_tiles <= (long)n_jobs * tiles_per_job, GB_E_SHAPE, "n_tiles=%ld exceeds n_jobs * ceil(max_windows / 128) = %ld", n_tiles,
+             (long)n_jobs * tiles_per_job);
+  GB_REQUIRE(n_tiles <= MAX_TILES, GB_E_SHAPE, "n_tiles=%ld exceeds %ld window tiles per launch", n_tiles, MAX_TILES);
   return GB_OK;
 }
 
-// x_rows: rows of the x array (not needed for the size: each job's input projection covers its own max_windows + lookback - 1 rows)
-extern "C" size_t gb_lstm_tc_workspace_bytes(const gb_lstmnet* net, int32_t n_slots, int32_t n_jobs, int32_t max_windows, int64_t /*x_rows*/) {
-  if (gb_lstm_tc_supported(net) != GB_OK || n_jobs < 0 || max_windows < 0 || n_slots < 0) return 0;
-  Plan p;
-  make_plan(net, n_slots, n_jobs, max_windows, &p);
-  return p.total;
-}
-
-extern "C" int gb_lstm_infer_tc(const gb_lstmnet* net, const float* params, int32_t n_slots, const gb_job* jobs, int32_t n_jobs, int32_t max_windows,
-                                const float* x, int64_t x_rows, float* out_model, void* workspace, void* stream) {
-  int rc = gb_lstm_tc_supported(net);
-  if (rc != GB_OK) return rc;
-  GB_REQUIRE(params && jobs && x && out_model && workspace, GB_E_ARG, "params/jobs/x/out_model/workspace must be non-NULL");
-  GB_REQUIRE(n_jobs >= 0 && max_windows >= 0 && n_slots >= 1 && x_rows >= 1, GB_E_ARG, "bad n_jobs/max_windows/n_slots/x_rows");
+// tile_base == nullptr: the uniform layout, every job ceil(max_windows / 128) tiles, its table written into the workspace
+int infer_tc(const gb_lstmnet* net, const float* params, int32_t n_slots, const gb_job* jobs, int32_t n_jobs, const int32_t* tile_base, int n_tiles,
+             int32_t max_windows, const float* x, float* out_model, void* workspace, cudaStream_t st) {
+  int rc;
   GB_REQUIRE(gb::aligned16(workspace), GB_E_ALIGN, "workspace must be 16-byte aligned");
-  if (n_jobs == 0 || max_windows == 0) return GB_OK;
-  cudaStream_t st = (cudaStream_t)stream;
-  const int tiles_per_job = (max_windows + TILE - 1) / TILE;
-  const long rows_pad = (long)n_jobs * tiles_per_job * TILE;
+  if (n_jobs == 0 || n_tiles == 0 || max_windows == 0) return GB_OK;
+  const long rows = (long)n_tiles * TILE;
   Plan p;
-  make_plan(net, n_slots, n_jobs, max_windows, &p);
+  make_plan(net, n_slots, n_jobs, n_tiles, &p);
   uint8_t* ws = static_cast<uint8_t*>(workspace);
   const long pstride = (long)gb_lstm_param_stride(net);
   constexpr int GRID_YZ = 65535;  // gridDim.y / z carry slots and jobs: larger fleets go out as several launches
+
+  // ---- the tile table and the per-tile records
+  if (tile_base == nullptr) {
+    int32_t* tb = reinterpret_cast<int32_t*>(ws + p.tile_base);
+    lstm_tc_uniform_tiles_kernel<<<(n_jobs + 256) / 256, 256, 0, st>>>(n_jobs, (max_windows + TILE - 1) / TILE, tb);
+    tile_base = tb;
+  }
+  int4* tiles = reinterpret_cast<int4*>(ws + p.tiles);
+  lstm_tc_tiles_kernel<<<min((n_tiles + 255) / 256, 4096), 256, 0, st>>>(jobs, n_jobs, tile_base, n_tiles, tiles);
 
   // ---- operands that do not depend on the timestep
   for (int l = 0; l < p.nl; ++l)
@@ -435,16 +455,16 @@ extern "C" int gb_lstm_infer_tc(const gb_lstmnet* net, const float* params, int3
                                                                                   reinterpret_cast<__half*>(ws + p.w_lo[l]), reinterpret_cast<float*>(ws + p.bias[l]));
   const int xr_max = max_windows + p.L - 1;
   for (int j0 = 0; j0 < n_jobs; j0 += GRID_YZ)
-    lstm_tc_xk_kernel<<<dim3((xr_max + 31) / 32, 4 * p.u[0] / 64, min(n_jobs - j0, GRID_YZ)), 256, 0, st>>>(jobs, j0, x, p.F, p.ur[0], p.u[0], p.L, params,
-                                                                                                        pstride, p.xk_blocks, reinterpret_cast<float*>(ws + p.xk));
+    lstm_tc_xk_kernel<<<dim3((xr_max + 31) / 32, 4 * p.u[0] / 64, min(n_jobs - j0, GRID_YZ)), 256, 0, st>>>(
+        jobs, j0, tile_base, n_tiles, x, p.F, p.ur[0], p.u[0], p.L, params, pstride, p.xk_pad, reinterpret_cast<float*>(ws + p.xk));
   GB_CUDA_CHECK(cudaMemsetAsync(ws + p.state_begin, 0, p.state_end - p.state_begin, st));
   GB_CUDA_CHECK(cudaGetLastError());
 
   CUtensorMap m_h[GB_MAX_LAYERS][2][2], m_w[GB_MAX_LAYERS][2];
   for (int l = 0; l < p.nl; ++l) {
     for (int b = 0; b < 2; ++b) {
-      if ((rc = make_map_f16(&m_h[l][b][0], ws + p.h_hi[l][b], rows_pad, p.u[l], TILE)) != GB_OK) return rc;
-      if ((rc = make_map_f16(&m_h[l][b][1], ws + p.h_lo[l][b], rows_pad, p.u[l], TILE)) != GB_OK) return rc;
+      if ((rc = make_map_f16(&m_h[l][b][0], ws + p.h_hi[l][b], rows, p.u[l], TILE)) != GB_OK) return rc;
+      if ((rc = make_map_f16(&m_h[l][b][1], ws + p.h_lo[l][b], rows, p.u[l], TILE)) != GB_OK) return rc;
     }
     if ((rc = make_map_f16(&m_w[l][0], ws + p.w_hi[l], (long)n_slots * 4 * p.u[l], p.kp[l], NCOL)) != GB_OK) return rc;
     if ((rc = make_map_f16(&m_w[l][1], ws + p.w_lo[l], (long)n_slots * 4 * p.u[l], p.kp[l], NCOL)) != GB_OK) return rc;
@@ -465,14 +485,14 @@ extern "C" int gb_lstm_infer_tc(const gb_lstmnet* net, const float* params, int3
     for (int l = 0; l < p.nl; ++l) {
       TcLayerArgs a{};
       a.u = p.u[l]; a.kc_below = p.kp_below[l] / KC; a.kc_own = p.u[l] / KC; a.act = net->act[l];
-      a.tiles_per_job = tiles_per_job; a.t = t; a.jobs = jobs;
+      a.t = t; a.tiles = tiles;
       a.bias = reinterpret_cast<const float*>(ws + p.bias[l]);
-      a.xk = reinterpret_cast<const float*>(ws + p.xk); a.xk_blocks = p.xk_blocks;
+      a.xk = reinterpret_cast<const float*>(ws + p.xk); a.xk_pad = p.xk_pad;
       a.c = reinterpret_cast<float*>(ws + p.c[l]);
       a.h_out_hi = reinterpret_cast<__half*>(ws + p.h_hi[l][wr]);
       a.h_out_lo = reinterpret_cast<__half*>(ws + p.h_lo[l][wr]);
       const int lb = l > 0 ? l - 1 : 0;
-      a.n_items = n_jobs * tiles_per_job * (p.u[l] / UB);
+      a.n_items = n_tiles * (p.u[l] / UB);
       const int grid = a.n_items < sms ? a.n_items : sms;
       kernels[l == 0][net->act[l] == GB_ACT_TANH]<<<grid, NTHREADS, smem, st>>>(a, m_h[lb][wr][0], m_h[lb][wr][1], m_h[l][rd][0], m_h[l][rd][1],
                                                                               m_w[l][0], m_w[l][1]);
@@ -480,10 +500,64 @@ extern "C" int gb_lstm_infer_tc(const gb_lstmnet* net, const float* params, int3
     }
   }
   const int top = p.nl - 1, fin = (p.L - 1) & 1;
-  for (int j0 = 0; j0 < n_jobs; j0 += GRID_YZ)
-    lstm_tc_head_kernel<<<dim3(tiles_per_job, min(n_jobs - j0, GRID_YZ)), TILE, 0, st>>>(jobs, j0, tiles_per_job, reinterpret_cast<const __half*>(ws + p.h_hi[top][fin]),
-                                                                                          reinterpret_cast<const __half*>(ws + p.h_lo[top][fin]), p.ur[top], p.u[top],
-                                                                                          p.n_out, net->out_act, params, pstride, p.dofs, out_model);
+  lstm_tc_head_kernel<<<n_tiles, TILE, 0, st>>>(jobs, tiles, reinterpret_cast<const __half*>(ws + p.h_hi[top][fin]),
+                                                reinterpret_cast<const __half*>(ws + p.h_lo[top][fin]), p.ur[top], p.u[top], p.n_out, net->out_act, params,
+                                                pstride, p.dofs, out_model);
   GB_CUDA_CHECK(cudaGetLastError());
   return GB_OK;
+}
+
+}  // namespace
+
+extern "C" int gb_lstm_tc_supported(const gb_lstmnet* net) {
+  GB_REQUIRE(net != nullptr, GB_E_ARG, "net is NULL");
+  GB_REQUIRE(net->n_layers >= 1 && net->n_layers <= GB_MAX_LAYERS, GB_E_SHAPE, "n_layers=%d outside [1,%d]", net->n_layers, GB_MAX_LAYERS);
+  for (int l = 0; l < net->n_layers; ++l)
+    GB_REQUIRE(net->units[l] >= 1 && net->units[l] <= 512, GB_E_SHAPE, "tensor-core LSTM variant covers layer widths 1..512, units[%d]=%d", l, net->units[l]);
+  GB_REQUIRE(net->n_features >= 1 && net->n_features <= 512 && net->n_features_out >= 1 && net->n_features_out <= 512, GB_E_SHAPE, "bad feature counts");
+  GB_REQUIRE(net->lookback >= 1, GB_E_ARG, "lookback=%d must be >= 1", net->lookback);
+  for (int l = 0; l < net->n_layers; ++l)  // h is carried as an FP16 pair: only cells with |h| < 1
+    GB_REQUIRE(net->act[l] == GB_ACT_TANH || net->act[l] == GB_ACT_SIGMOID, GB_E_SHAPE,
+               "tensor-core LSTM variant covers tanh and sigmoid cells (a relu or linear cell's h overflows FP16), act[%d]=%d", l, net->act[l]);
+  return GB_OK;
+}
+
+// x_rows: rows of the x array (not needed for the size: each job's input projection covers its own n_rows + lookback - 1 rows)
+extern "C" size_t gb_lstm_tc_workspace_bytes(const gb_lstmnet* net, int32_t n_slots, int32_t n_jobs, int32_t max_windows, int64_t /*x_rows*/) {
+  if (gb_lstm_tc_supported(net) != GB_OK || n_jobs < 0 || max_windows < 0 || n_slots < 0) return 0;
+  Plan p;
+  make_plan(net, n_slots, n_jobs, (long)n_jobs * ((max_windows + TILE - 1) / TILE), &p);
+  return p.total;
+}
+
+extern "C" size_t gb_lstm_tc_ragged_workspace_bytes(const gb_lstmnet* net, int32_t n_slots, int32_t n_jobs, int32_t n_tiles, int32_t max_windows) {
+  const long tiles_per_job = ((long)max_windows + TILE - 1) / TILE;
+  if (gb_lstm_tc_supported(net) != GB_OK || n_slots < 0 || n_jobs < 0 || max_windows < 0 || n_tiles < 0 || n_tiles > n_jobs * tiles_per_job ||
+      n_tiles > MAX_TILES)
+    return 0;
+  Plan p;
+  make_plan(net, n_slots, n_jobs, n_tiles, &p);
+  return p.total;
+}
+
+extern "C" int gb_lstm_infer_tc(const gb_lstmnet* net, const float* params, int32_t n_slots, const gb_job* jobs, int32_t n_jobs, int32_t max_windows,
+                                const float* x, int64_t x_rows, float* out_model, void* workspace, void* stream) {
+  int rc = gb_lstm_tc_supported(net);
+  if (rc != GB_OK) return rc;
+  GB_REQUIRE(params && jobs && x && out_model && workspace, GB_E_ARG, "params/jobs/x/out_model/workspace must be non-NULL");
+  GB_REQUIRE(n_jobs >= 0 && max_windows >= 0 && n_slots >= 1 && x_rows >= 1, GB_E_ARG, "bad n_jobs/max_windows/n_slots/x_rows");
+  const long n_tiles = (long)n_jobs * ((max_windows + TILE - 1) / TILE);
+  if ((rc = check_sizes(n_slots, n_jobs, n_tiles, max_windows)) != GB_OK) return rc;
+  return infer_tc(net, params, n_slots, jobs, n_jobs, nullptr, (int)n_tiles, max_windows, x, out_model, workspace, (cudaStream_t)stream);
+}
+
+extern "C" int gb_lstm_infer_tc_ragged(const gb_lstmnet* net, const float* params, int32_t n_slots, const gb_job* jobs, int32_t n_jobs,
+                                       const int32_t* tile_base, int32_t n_tiles, int32_t max_windows, const float* x, int64_t x_rows,
+                                       float* out_model, void* workspace, void* stream) {
+  int rc = gb_lstm_tc_supported(net);
+  if (rc != GB_OK) return rc;
+  GB_REQUIRE(params && jobs && tile_base && x && out_model && workspace, GB_E_ARG, "params/jobs/tile_base/x/out_model/workspace must be non-NULL");
+  GB_REQUIRE(x_rows >= 1, GB_E_ARG, "x_rows=%lld must be >= 1", (long long)x_rows);
+  if ((rc = check_sizes(n_slots, n_jobs, n_tiles, max_windows)) != GB_OK) return rc;
+  return infer_tc(net, params, n_slots, jobs, n_jobs, tile_base, n_tiles, max_windows, x, out_model, workspace, (cudaStream_t)stream);
 }

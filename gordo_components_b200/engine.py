@@ -707,14 +707,39 @@ class LSTMEngine:
     def tc_supported(self) -> bool:
         return self.lib.gb_lstm_tc_supported(C.byref(self.net)) == 0
 
-    def infer(self, params, jobs_dev, n_jobs, max_windows, x, out_rows, variant: int = 0):
+    TILE = 128  # windows per tile of the tensor-core inference kernels
+
+    @classmethod
+    def tile_base(cls, n_windows) -> np.ndarray:
+        """int32 [n_jobs + 1] prefix sums of ceil(n_windows_j / 128): the ragged tile layout of ``infer(tile_base=)``."""
+        tiles = (np.asarray(n_windows, dtype=np.int64) + cls.TILE - 1) // cls.TILE
+        return np.concatenate([[0], np.cumsum(tiles)]).astype(np.int32)
+
+    def tc_workspace_bytes(self, n_slots: int, n_jobs: int, max_windows: int, n_tiles: Optional[int] = None) -> int:
+        """Device scratch of one tensor-core ``infer`` launch: every job max_windows' tiles, or with ``n_tiles`` the ragged layout (0: refused)."""
+        if n_tiles is None:
+            return int(self.lib.gb_lstm_tc_workspace_bytes(C.byref(self.net), int(n_slots), int(n_jobs), int(max_windows), 1))
+        return int(self.lib.gb_lstm_tc_ragged_workspace_bytes(C.byref(self.net), int(n_slots), int(n_jobs), int(n_tiles), int(max_windows)))
+
+    def infer(self, params, jobs_dev, n_jobs, max_windows, x, out_rows, variant: int = 0, tile_base=None, n_tiles: Optional[int] = None):
         """
         out[j] = net(x[j : j + lookback]) for every job's windows (jobs' n_rows counts windows).
         variant 0 = tensor-core (wgmma) kernel when the layer widths allow it, 1 = fp32 CUDA-core kernel, 2 = tensor-core kernel (error if unsupported).
+        ``tile_base`` (int32 device tensor of ``tile_base(n_rows)``) with ``n_tiles`` = its last entry: the ragged tile layout
+        (gb_lstm_infer_tc_ragged), where a batch costs its jobs' own windows; tensor-core kernel only, the same bits per window.
         """
         torch = _torch()
         out = torch.empty((int(out_rows), self.n_out), dtype=torch.float32, device=self.device)
         p = _cabi.ptr
+        if tile_base is not None:
+            if n_tiles is None or variant == 1:
+                raise ValueError("a ragged tile layout takes n_tiles and runs on the tensor-core kernel only")
+            _cabi.check(self.lib.gb_lstm_tc_supported(C.byref(self.net)))
+            ws_bytes = self.tc_workspace_bytes(params.shape[0], n_jobs, max_windows, n_tiles)
+            ws = torch.empty((ws_bytes + 255,), dtype=torch.uint8, device=self.device)
+            _cabi.check(self.lib.gb_lstm_infer_tc_ragged(C.byref(self.net), p(params), int(params.shape[0]), p(jobs_dev), int(n_jobs), p(tile_base),
+                                                         int(n_tiles), int(max_windows), p(x), int(x.shape[0]), p(out), p(ws), _stream_ptr()))
+            return out
         if variant == 2 or (variant == 0 and self.tc_supported):
             ws_bytes = int(self.lib.gb_lstm_tc_workspace_bytes(C.byref(self.net), int(params.shape[0]), int(n_jobs), int(max_windows), int(x.shape[0])))
             if ws_bytes == 0:

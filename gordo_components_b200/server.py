@@ -20,7 +20,7 @@ import os
 import threading
 import timeit
 from collections import OrderedDict
-from typing import Any, Dict, List, Optional, Union
+from typing import Any, Dict, List, Optional, Sequence, Union
 
 import dateutil.parser
 import numpy as np
@@ -251,15 +251,25 @@ class ResidentBucket:
     (MinMaxScaler, StandardScaler, RobustScaler, MaxAbsScaler) ending in a ``KerasAutoEncoder``: the composed float64 scaler of
     each model rides with its weights, and the launch applies it as it reads X (``serving.AnomalyCoalescer(x_scale=, x_offset=)``).
     Bare and Pipeline models never share a bucket.
+
+    ``lstm=True`` builds a bucket of LSTM detectors instead, served through ``serving.LSTMAnomalyCoalescer``: a
+    ``KerasLSTMAutoEncoder`` or ``KerasLSTMForecast``, bare or as the last step of a ``Pipeline``, on a stack the tensor-core LSTM
+    kernel runs (tanh and sigmoid cells).  The Pipeline's leading steps run on the host as ``Pipeline.predict`` runs them; autoencoder
+    and forecast models of one architecture share a bucket (the lookahead only decides which rows of y a request stages).
     """
 
     input_scalers = False  # the bucket holds Pipeline models (set by the constructor)
+    lstm = False  # the bucket holds LSTM models (set by the constructor)
 
-    def __init__(self, store: "ModelStore", names: Optional[List[str]] = None, input_scalers: bool = False, **coalescer_kwargs):
+    def __init__(self, store: "ModelStore", names: Optional[List[str]] = None, input_scalers: bool = False, lstm: bool = False,
+                 **coalescer_kwargs):
         from . import engine
         from .machine.model.anomaly.diff import _compose_affine, _scaler_multiplier
         from .serving import AnomalyCoalescer
 
+        if lstm:
+            self._init_lstm(store, names, coalescer_kwargs)
+            return
         groups: Dict[Any, List[str]] = {}
         for name in names if names is not None else store.names():
             model = store.model(name)
@@ -289,6 +299,63 @@ class ResidentBucket:
             coalescer_kwargs.update(x_scale=to_dev(a, np.float64), x_offset=to_dev(b, np.float64))
         self.coalescer = AnomalyCoalescer(eng, params, scale, feat_thr, agg_thr, **coalescer_kwargs)
 
+    def _init_lstm(self, store: "ModelStore", names: Optional[List[str]], coalescer_kwargs):
+        from . import engine
+        from .machine.model.anomaly.diff import _scaler_multiplier
+        from .serving import LSTMAnomalyCoalescer
+
+        groups = self.lstm_groups({name: store.model(name) for name in (names if names is not None else store.names())})
+        if not groups:
+            raise ValueError("no LSTM model in the store can be served through a coalescer")
+        self.lstm = True
+        self.names = max(groups.values(), key=len)  # the largest architecture group
+        self.slot = {name: i for i, name in enumerate(self.names)}
+        models = [store.model(n) for n in self.names]
+        nets = [_served_lstm_parts(m)[1] for m in models]
+        eng = engine.lstm_engine_for(nets[0].model.spec)
+        torch = engine._torch()
+        to_dev = lambda rows: torch.from_numpy(np.ascontiguousarray(np.stack(rows), dtype=np.float64)).to(eng.device)  # noqa: E731
+        params = eng.pack_params([net.model.weights for net in nets])
+        scale = to_dev([_scaler_multiplier(m.scaler, eng.n_out) for m in models])
+        feat, agg = zip(*(m._thresholds() for m in models))
+        feat_thr = to_dev([np.asarray(f, dtype=np.float64) for f in feat]) if feat[0] is not None else None
+        agg_thr = to_dev([np.float64(a) for a in agg]) if agg[0] is not None else None
+        self.coalescer = LSTMAnomalyCoalescer(eng, params, scale, feat_thr, agg_thr, **coalescer_kwargs)
+
+    @classmethod
+    def lstm_groups(cls, models: Dict[str, Any]) -> Dict[Any, List[str]]:
+        """The eligible LSTM detectors of ``models`` (name -> model) by (architecture, which thresholds are present)."""
+        groups: Dict[Any, List[str]] = {}
+        for name, model in models.items():
+            if cls.eligible_lstm(model):
+                spec = _served_lstm_parts(model)[1].model.spec
+                groups.setdefault((spec.key(), tuple(t is not None for t in model._thresholds())), []).append(name)
+        return groups
+
+    @staticmethod
+    def eligible_lstm(model) -> bool:
+        """True for a detector ``ResidentBucket(lstm=True)`` serves (no device needed)."""
+        import ctypes as C
+
+        from . import _cabi
+        from .machine.model.anomaly.diff import _scaler_multiplier
+
+        if not (_frame_is_from_blocks(model) and model.window is None
+                and not (model.require_thresholds and all(t is None for t in model._thresholds()))):
+            return False
+        parts = _served_lstm_parts(model)
+        if parts is None or parts[1].model is None:
+            return False
+        spec = parts[1].model.spec
+        net = _cabi.make_lstmnet(spec.n_features, spec.lstm_units, spec.acts, spec.n_features_out, spec.out_func, spec.lookback_window)
+        if _cabi.load_library().gb_lstm_tc_supported(C.byref(net)) != 0:
+            return False  # relu / linear cells: the fp32 kernel, on the per-request route
+        try:
+            _scaler_multiplier(model.scaler, spec.n_features_out)
+        except (ValueError, AttributeError):
+            return False
+        return True
+
     @staticmethod
     def eligible(model, input_scalers: bool = False) -> bool:
         if not (_frame_is_from_blocks(model) and model.window is None
@@ -313,6 +380,8 @@ class ResidentBucket:
 
         model = store.model(name)
         _refuse_infinity(_values(y))
+        if self.lstm:
+            return self._lstm_anomaly_blocks(name, model, X, y, frequency)
         if self.input_scalers:
             # what the Pipeline's sklearn steps raise, as the per-request route does before any launch
             _refuse_infinity(np.ascontiguousarray(_values(X), dtype=np.float64))
@@ -320,6 +389,23 @@ class ResidentBucket:
             # the coalescer's launch may run the tensor-core kernel, which does not take ±inf inputs: this request goes on its own
             return model.anomaly_blocks(X, y, frequency=frequency)
         scores = self.coalescer.anomaly(self.slot[name], X, y)
+        _refuse_infinity(scores["model-output"])
+        return model.blocks_from_scores(scores, X, y, frequency)
+
+    def _lstm_anomaly_blocks(self, name: str, model, X: pd.DataFrame, y: pd.DataFrame, frequency):
+        """What ``model.anomaly_blocks`` computes, in the order the per-request route raises: the leading steps' transform (which
+        refuses ±inf in X), the lookback check; a transformed X holding ±inf goes on its own (the fp32 kernel saturates the gates)."""
+        from .machine.model.anomaly.diff import _has_inf, _refuse_infinity, _values
+
+        pre, net = _served_lstm_parts(model)
+        Xt = X
+        for step in pre:
+            Xt = step.transform(Xt)
+        Xv = net._validate_and_fix_size_of_X(np.asarray(_values(Xt)))
+        if _has_inf(Xv):
+            return model.anomaly_blocks(X, y, frequency=frequency)
+        n = len(Xv) - net.lookback_window + 1 - net.lookahead
+        scores = self.coalescer.anomaly(self.slot[name], Xv, _values(y)[-n:])
         _refuse_infinity(scores["model-output"])
         return model.blocks_from_scores(scores, X, y, frequency)
 
@@ -364,6 +450,22 @@ def _served_parts(model):
     return None
 
 
+def _served_lstm_parts(model):
+    """(leading Pipeline steps, ``KerasLSTMAutoEncoder`` / ``KerasLSTMForecast``) of a detector whose base estimator is a bare LSTM
+    network ([] for the steps) or a ``Pipeline`` ending in one, else None.  Skipped steps (None, "passthrough") are left out, as
+    ``Pipeline.predict`` leaves them out."""
+    from sklearn.pipeline import Pipeline
+
+    from .machine.model.models import KerasLSTMAutoEncoder, KerasLSTMForecast
+
+    est = model.base_estimator
+    if type(est) in (KerasLSTMAutoEncoder, KerasLSTMForecast):
+        return [], est
+    if type(est) is Pipeline and len(est.steps) > 1 and type(est.steps[-1][1]) in (KerasLSTMAutoEncoder, KerasLSTMForecast):
+        return [step for _, step in est.steps[:-1] if step is not None and step != "passthrough"], est.steps[-1][1]
+    return None
+
+
 def _x64_launch_holds(spec) -> bool:
     """True when the fused launch with float64 x holds this stack on the kernel the per-request route picks (no device needed)."""
     import ctypes as C
@@ -389,10 +491,12 @@ def _respond(frame: pd.DataFrame, fmt: Optional[str], start: float) -> Reply:
 
 
 def anomaly_prediction(store: ModelStore, name: str, json: Optional[dict] = None, files: Optional[Dict[str, bytes]] = None,
-                       all_columns: bool = False, fmt: Optional[str] = None, bucket: Optional[ResidentBucket] = None) -> Reply:
+                       all_columns: bool = False, fmt: Optional[str] = None,
+                       bucket: Union[ResidentBucket, Sequence[ResidentBucket], None] = None) -> Reply:
     """
     ``POST .../<name>/anomaly/prediction`` (anomaly.py:28-122): the anomaly frame of the request's X against its y.  With ``bucket``
-    the models it holds are scored through its request coalescer (one launch for everything that is waiting).
+    the models it holds are scored through its request coalescer (one launch for everything that is waiting); a sequence of buckets
+    (say a feed-forward and an LSTM one over the same store) is asked in order, and the first that holds the model answers.
     """
     start = timeit.default_timer()
     try:
@@ -410,10 +514,12 @@ def anomaly_prediction(store: ModelStore, name: str, json: Optional[dict] = None
         return not_a_detector
     skip = () if all_columns else DELETED_FROM_RESPONSE_COLUMNS
     try:
-        coalesced = bucket is not None and name in bucket.slot
-        if coalesced or (fmt != "parquet" and _frame_is_from_blocks(model)):
+        buckets = () if bucket is None else (bucket,) if isinstance(bucket, ResidentBucket) else tuple(bucket)
+        holder = next((b for b in buckets if name in b.slot), None)
+        if holder is not None or (fmt != "parquet" and _frame_is_from_blocks(model)):
             # this package's detectors: straight from the column blocks, no DataFrame in between for JSON
-            blocks = bucket.anomaly_blocks(store, name, X, y, store.frequency(name)) if coalesced else model.anomaly_blocks(X, y, frequency=store.frequency(name))
+            blocks = (holder.anomaly_blocks(store, name, X, y, store.frequency(name)) if holder is not None
+                      else model.anomaly_blocks(X, y, frequency=store.frequency(name)))
             if fmt != "parquet":
                 return Reply(200, {"data": blocks_to_dict(*blocks, skip=skip), "time-seconds": f"{timeit.default_timer() - start:.4f}"})
             frame = model_utils.frame_from_blocks(*blocks)

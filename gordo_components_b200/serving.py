@@ -18,6 +18,9 @@ float32 batch ``gb_affine_f64`` would have produced.
 
 Thread-safe, re-entrant, no shared mutable scratch outside the worker thread (the reference's threading convention,
 SURVEY §8b).  The per-request results are bit-identical to a per-request launch: rows are independent in the kernel.
+
+``LSTMAnomalyCoalescer`` does the same for LSTM detectors: the waiting requests become one ragged tensor-core LSTM launch
+sequence (gb_lstm_infer_tc_ragged, each request a job of its own windows) and one float64 scoring launch (gb_anomaly_score_f64).
 """
 from __future__ import annotations
 
@@ -54,7 +57,13 @@ class AnomalyCoalescer:
         self._yd = torch.empty((self.max_rows, eng.n_out), dtype=torch.float32, device=dev)
         self._out_d = {k: torch.empty((self.max_rows, eng.n_out) if k in PER_TAG else (self.max_rows,), dtype=torch.float32, device=dev) for k in self.want}
         self._out_h = {k: torch.empty(v.shape, dtype=torch.float32).pin_memory() for k, v in self._out_d.items()}
-        self._jobs_h = torch.empty((4096 * engine._cabi.JOB_DTYPE.itemsize,), dtype=torch.uint8).pin_memory()
+        self._jobs_h = torch.empty((self.max_jobs * engine._cabi.JOB_DTYPE.itemsize,), dtype=torch.uint8).pin_memory()
+        self.max_cost = self.max_rows
+        self._start()
+
+    max_jobs = 4096  # requests per batch: the pinned buffer the job records are staged through holds this many
+
+    def _start(self):
         self._q: "queue.Queue" = queue.Queue()
         self._closed = False
         self.batches = 0
@@ -67,17 +76,25 @@ class AnomalyCoalescer:
         """Queue one request; the Future resolves to {column block: host array} for exactly these rows."""
         if self._closed:
             raise RuntimeError("coalescer is closed")
+        if not (0 <= int(slot) < self.params.shape[0]):
+            raise ValueError(f"unknown machine slot {slot}")
+        fut: Future = Future()
+        self._q.put((int(slot), *self._request(X, y), fut))
+        return fut
+
+    def _request(self, X, y):
+        """The request's staged (X, y) host arrays, or ValueError when they do not fit the bucket."""
         Xv = np.ascontiguousarray(getattr(X, "values", X), dtype=self._x_np)
         yv = np.ascontiguousarray(getattr(y, "values", y), dtype=np.float32)
         if Xv.ndim != 2 or Xv.shape[1] != self.eng.n_in or yv.shape != (len(Xv), self.eng.n_out):
             raise ValueError(f"request of shape X {Xv.shape} / y {yv.shape} does not fit a {self.eng.n_in}->{self.eng.n_out} model")
         if len(Xv) > self.max_rows:
             raise ValueError(f"a request of {len(Xv)} rows exceeds max_batch_rows={self.max_rows}")
-        if not (0 <= int(slot) < self.params.shape[0]):
-            raise ValueError(f"unknown machine slot {slot}")
-        fut: Future = Future()
-        self._q.put((int(slot), Xv, yv, fut))
-        return fut
+        return Xv, yv
+
+    def _cost(self, item) -> int:
+        """What a request adds to a batch, against ``max_cost``: its rows."""
+        return len(item[1])
 
     def anomaly(self, slot: int, X, y) -> Dict[str, np.ndarray]:
         return self.submit(slot, X, y).result()
@@ -96,9 +113,9 @@ class AnomalyCoalescer:
             pending = None
             if first is None:
                 return
-            batch, rows = [first], len(first[1])
+            batch, cost = [first], self._cost(first)
             deadline = time.perf_counter() + self.max_wait
-            while rows < self.max_rows and len(batch) < 4096:
+            while cost < self.max_cost and len(batch) < self.max_jobs:
                 try:
                     item = self._q.get(timeout=max(0.0, deadline - time.perf_counter())) if self._q.empty() else self._q.get_nowait()
                 except queue.Empty:
@@ -106,17 +123,17 @@ class AnomalyCoalescer:
                 if item is None:
                     self._q.put(None)
                     break
-                if rows + len(item[1]) > self.max_rows:
+                if cost + self._cost(item) > self.max_cost:
                     pending = item
                     break
                 batch.append(item)
-                rows += len(item[1])
+                cost += self._cost(item)
             try:
-                self._launch(torch, batch, rows)
+                self._launch(torch, batch, cost)
             except BaseException as exc:  # noqa: BLE001 - every waiting caller must hear about it
-                for _, _, _, fut in batch:
-                    if not fut.done():
-                        fut.set_exception(exc)
+                for item in batch:
+                    if not item[-1].done():
+                        item[-1].set_exception(exc)
 
     def _launch(self, torch, batch, rows):
         jobs = np.empty(len(batch), dtype=engine._cabi.JOB_DTYPE)
@@ -149,3 +166,101 @@ class AnomalyCoalescer:
             n = len(Xv)
             fut.set_result({k: self._out_h[k][ofs:ofs + n].numpy().copy() for k in self.want})
             ofs += n
+
+
+class LSTMAnomalyCoalescer(AnomalyCoalescer):
+    """
+    ``AnomalyCoalescer`` for the LSTM detectors of one architecture: ``params`` [n_slots, param_stride] float32, ``scale`` /
+    ``feat_thr`` [n_slots, n_out] and ``agg_thr`` [n_slots] float64 device tensors.  A request is the model input ``X`` (float32, the
+    Pipeline's leading steps already applied) and the float64 targets of its windows, ``y[-n_windows:]``; ``X`` must hold at least
+    ``n_windows + lookback - 1`` rows (a forecast's last row is not read).  Per batch: X packed back to back, the batch's distinct
+    models gathered into compact tensors (the launch stages the FP16 images of the slots it is given), one ragged tensor-core launch
+    sequence, the prediction widened to float64 on the device and scored there, one synchronisation.  A batch closes at
+    ``max_batch_tiles`` 128-window tiles or ``max_jobs`` requests.  Results: float32 ``model-output``, float64 scores, as the
+    per-request route returns them.
+    """
+
+    def __init__(self, eng: "engine.LSTMEngine", params, scale, feat_thr=None, agg_thr=None, max_batch_tiles: int = 1024,
+                 max_wait_ms: float = 1.0):
+        torch = engine._torch()
+        self.eng, self.params, self.scale, self.feat_thr, self.agg_thr = eng, params, scale, feat_thr, agg_thr
+        self.max_cost, self.max_wait = int(max_batch_tiles), float(max_wait_ms) * 1e-3
+        self.want = tuple(k for k in PER_TAG + PER_ROW if not ((feat_thr is None and k == "anomaly-confidence")
+                                                                or (agg_thr is None and k == "total-anomaly-confidence")))
+        self._stream = torch.cuda.Stream(device=eng.device)
+        # staged per batch in one copy: the infer jobs, the score jobs, tile_base, the distinct slots and the gather job
+        jb = engine._cabi.JOB_DTYPE.itemsize
+        self._stage_h = torch.empty((2 * self.max_jobs * jb + 2 * (self.max_jobs + 1) * 4 + jb,), dtype=torch.uint8).pin_memory()
+        self._start()
+
+    def _request(self, X, y):
+        Xv = np.ascontiguousarray(getattr(X, "values", X), dtype=np.float32)
+        yv = np.ascontiguousarray(getattr(y, "values", y), dtype=np.float64)
+        n = len(yv)
+        if Xv.ndim != 2 or Xv.shape[1] != self.eng.n_features or yv.ndim != 2 or yv.shape[1] != self.eng.n_out:
+            raise ValueError(f"request of shape X {Xv.shape} / y {yv.shape} does not fit a {self.eng.n_features}->{self.eng.n_out} LSTM model")
+        if not 1 <= n <= len(Xv) - self.eng.lookback + 1:
+            raise ValueError(f"{n} target rows for {len(Xv)} input rows: a lookback of {self.eng.lookback} gives 1 to "
+                             f"{len(Xv) - self.eng.lookback + 1} windows")
+        if self._tiles(n) > self.max_cost:
+            raise ValueError(f"a request of {n} windows exceeds max_batch_tiles={self.max_cost} tiles of {self.eng.TILE}")
+        return Xv, yv
+
+    def _tiles(self, n_windows: int) -> int:
+        return -(-int(n_windows) // self.eng.TILE)
+
+    def _cost(self, item) -> int:
+        return self._tiles(len(item[2]))
+
+    def _launch(self, torch, batch, n_tiles):
+        _cabi = engine._cabi
+        k = len(batch)
+        slots = np.fromiter((item[0] for item in batch), dtype=np.int64, count=k)
+        uniq, compact = np.unique(slots, return_inverse=True)
+        x_rows = np.fromiter((len(item[1]) for item in batch), dtype=np.int64, count=k)
+        windows = np.fromiter((len(item[2]) for item in batch), dtype=np.int64, count=k)
+        x_ofs = np.concatenate([[0], np.cumsum(x_rows)])
+        w_ofs = np.concatenate([[0], np.cumsum(windows)])
+        rows, total = int(x_ofs[-1]), int(w_ofs[-1])
+        infer_jobs = engine.make_jobs(compact, windows, x_ofs[:-1], w_ofs[:-1])
+        score_jobs = engine.make_jobs(compact, windows, w_ofs[:-1])  # y and the prediction both at the windows' rows
+        tile_base = self.eng.tile_base(windows)
+        gather_job = engine.make_jobs([0], [len(uniq)], [0])
+        # job records first: they hold int64 fields and stay 8-byte aligned in the staged buffer
+        parts = [infer_jobs.view(np.uint8), score_jobs.view(np.uint8), gather_job.view(np.uint8), tile_base.view(np.uint8),
+                 uniq.astype(np.int32).view(np.uint8)]
+        sizes = [p.nbytes for p in parts]
+        stage = self._stage_h.numpy()
+        ofs = np.concatenate([[0], np.cumsum(sizes)])
+        for p, o in zip(parts, ofs[:-1]):
+            stage[o:o + p.nbytes] = p
+        xh = torch.empty((rows, self.eng.n_features), dtype=torch.float32, pin_memory=True)
+        yh = torch.empty((total, self.eng.n_out), dtype=torch.float64, pin_memory=True)
+        xn, yn = xh.numpy(), yh.numpy()
+        for i, (_, Xv, yv, _) in enumerate(batch):
+            xn[x_ofs[i]:x_ofs[i + 1]] = Xv
+            yn[w_ofs[i]:w_ofs[i + 1]] = yv
+        dev = self.eng.device
+        with torch.cuda.stream(self._stream):
+            staged = self._stage_h[: int(ofs[-1])].to(dev, non_blocking=True)
+            view = [staged[int(ofs[i]):int(ofs[i + 1])] for i in range(len(parts))]
+            jobs_d, score_d, gjob_d, tb_d, map_d = view[0], view[1], view[2], view[3].view(torch.int32), view[4].view(torch.int32)
+            xd = xh.to(dev, non_blocking=True)
+            yd = yh.to(dev, non_blocking=True)
+            gather = lambda t: engine.gather_rows(gjob_d, 1, len(uniq), map_d, t, len(uniq))  # noqa: E731 - the batch's models, compact
+            params = gather(self.params)
+            scale = gather(self.scale)
+            feat_thr = gather(self.feat_thr) if self.feat_thr is not None else None
+            agg_thr = gather(self.agg_thr) if self.agg_thr is not None else None
+            pred = self.eng.infer(params, jobs_d, k, int(windows.max()), xd, total, tile_base=tb_d, n_tiles=int(tile_base[-1]))
+            res = engine.anomaly_score(score_d, k, int(windows.max()), pred.to(torch.float64), yd, self.eng.n_out, scale, feat_thr, agg_thr,
+                                       want=self.want)
+            res["model-output"] = pred
+            host = {key: torch.empty(v.shape, dtype=v.dtype, pin_memory=True) for key, v in res.items()}
+            for key, v in res.items():
+                host[key].copy_(v, non_blocking=True)
+        self._stream.synchronize()
+        self.batches += 1
+        self.requests += k
+        for i, item in enumerate(batch):
+            item[-1].set_result({key: v[w_ofs[i]:w_ofs[i + 1]].numpy().copy() for key, v in host.items()})

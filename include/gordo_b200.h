@@ -416,6 +416,16 @@ int gb_lstm_tc_supported(const gb_lstmnet* net);
 size_t gb_lstm_tc_workspace_bytes(const gb_lstmnet* net, int32_t n_slots, int32_t n_jobs, int32_t max_windows, int64_t x_rows);
 int gb_lstm_infer_tc(const gb_lstmnet* net, const float* params, int32_t n_slots, const gb_job* jobs, int32_t n_jobs,
                      int32_t max_windows, const float* x, int64_t x_rows, float* out_model, void* workspace, void* stream);
+/* The same kernels over a ragged tile layout, for jobs of very different lengths (a request coalescer's batch): job j's windows
+ * occupy the flat 128-window tiles [tile_base[j], tile_base[j + 1]), so the recurrent state, the input projection and the work
+ * grow with the jobs' own windows, not with n_jobs x the longest job.  tile_base: DEVICE array of n_jobs + 1 int32, the prefix sums
+ * of ceil(n_rows_j / 128) (tile_base[0] = 0, tile_base[n_jobs] = n_tiles); max_windows >= every job's n_rows, and n_tiles <=
+ * n_jobs * ceil(max_windows / 128).  Each window's arithmetic is that of gb_lstm_infer_tc, so its output is the same bits in
+ * either entry and any batch.  workspace: gb_lstm_tc_ragged_workspace_bytes() bytes (0 for arguments it refuses). */
+size_t gb_lstm_tc_ragged_workspace_bytes(const gb_lstmnet* net, int32_t n_slots, int32_t n_jobs, int32_t n_tiles, int32_t max_windows);
+int gb_lstm_infer_tc_ragged(const gb_lstmnet* net, const float* params, int32_t n_slots, const gb_job* jobs, int32_t n_jobs,
+                            const int32_t* tile_base, int32_t n_tiles, int32_t max_windows, const float* x, int64_t x_rows,
+                            float* out_model, void* workspace, void* stream);
 
 /* ---- K3-fit: LSTM training (back-propagation through time) ---------------------------------
  * Replaces KerasLSTMBaseEstimator.fit (models.py:557-616): if `primer`, one Adam step on the single
