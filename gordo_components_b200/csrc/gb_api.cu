@@ -28,6 +28,26 @@ int validate_ffnet(const gb_ffnet* net) {
   return GB_OK;
 }
 
+// the LSTM stacks every inference and fit kernel takes
+constexpr int LSTM_MAX_UNITS = 512;
+constexpr int LSTM_MAX_FEATURES = 512;
+
+int validate_lstmnet(const gb_lstmnet* net) {
+  GB_REQUIRE(net != nullptr, GB_E_ARG, "net is NULL");
+  GB_REQUIRE(net->n_layers >= 1 && net->n_layers <= GB_MAX_LAYERS, GB_E_SHAPE, "n_layers=%d outside [1,%d]",
+             net->n_layers, GB_MAX_LAYERS);
+  GB_REQUIRE(net->n_features >= 1 && net->n_features <= LSTM_MAX_FEATURES && net->n_features_out >= 1 &&
+                 net->n_features_out <= LSTM_MAX_FEATURES,
+             GB_E_SHAPE, "n_features/n_features_out outside [1,%d]", LSTM_MAX_FEATURES);
+  GB_REQUIRE(net->lookback >= 1, GB_E_ARG, "lookback=%d must be >= 1", net->lookback);
+  for (int l = 0; l < net->n_layers; ++l) {
+    GB_REQUIRE(net->units[l] >= 1 && net->units[l] <= LSTM_MAX_UNITS, GB_E_SHAPE, "units[%d]=%d outside [1,%d]", l,
+               net->units[l], LSTM_MAX_UNITS);
+    GB_REQUIRE(net->act[l] >= GB_ACT_LINEAR && net->act[l] <= GB_ACT_SIGMOID, GB_E_ARG, "act[%d] unknown", l);
+  }
+  return GB_OK;
+}
+
 FFImage make_ff_image(const gb_ffnet* net, int pad) {
   FFImage im{};
   int ofs = 0, pofs = 0, max_np = round_up(net->dims[0], pad);

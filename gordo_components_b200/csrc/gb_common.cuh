@@ -31,6 +31,7 @@ inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 
 inline int round_up(int v, int m) { return (v + m - 1) / m * m; }
 
 int validate_ffnet(const gb_ffnet* net);
+int validate_lstmnet(const gb_lstmnet* net);
 
 // padded shared-memory image of one slot's Dense stack: W_l as [Kp][Np] (zero padded), then biases [Np]
 struct FFImage {

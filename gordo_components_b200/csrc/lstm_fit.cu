@@ -17,44 +17,11 @@
 //   Adam      m += (g-m)(1-b1); v += (g^2-v)(1-b2); w -= lr sqrt(1-b2^t)/(1-b1^t) m/(sqrt(v)+eps)   [3P keras]
 // fp32 CUDA cores throughout (a tensor-core path for these GEMMs is the next step for this kernel family).
 #include "gb_common.cuh"
-#include "lstm_fit_stop.cuh"
+#include "lstm_fit_common.cuh"
 
 namespace {
 
 constexpr int MAXB = 32;  // windows per batch handled by one row tile
-constexpr int LSTM_MAX_UNITS = 512;
-constexpr int LSTM_MAX_FEATURES = 512;
-
-struct Lay {
-  int in, u;       // input width, units
-  int act;
-  long kofs;       // offset of [K; U] (rows in + u, 4u columns) in the parameter vector; bias follows
-  long zofs, cofs, hofs, dhofs, nxofs;  // workspace offsets (floats, per job): gates [L][B][4u], c / h [L][B][u], dh_seq [L][B][u], (dh_next, dc_next) [2][B][u]
-};
-
-struct FitArgs {
-  int n_layers, L, F, T_out, out_act, lookahead;
-  Lay lay[GB_MAX_LAYERS];
-  long dofs;        // Dense kernel offset in the parameter vector
-  long pstride, ws_stride;  // floats per slot / per job
-  long gofs;        // gradient vector offset in the job workspace
-  long topdh;       // [B][u_top] dh of the last LSTM layer at t = L-1
-  float* params;
-  float *adam_m, *adam_v;
-  int* adam_t;
-  const gb_job* jobs;
-  const float *x, *y;
-  float* ws;
-  float *loss_sum, *hit_sum;  // [n_jobs]
-  const int* step;            // device: {first window, nominal batch size} of the optimizer step being replayed (the launch
-                              // sequence of one step is captured once as a CUDA graph; only these two numbers change)
-  float lr, b1, b2, eps;
-  int loss;                   // gb_loss of the head
-  gb_optimizer opt;            // gb_lstm_fit_opt with another optimizer than plain Adam (lstm_opt_kernel)
-};
-
-__device__ __forceinline__ float sigm(float z) { return 1.f / (1.f + expf(-z)); }
-__device__ __forceinline__ int job_batch(const gb_job& job, int win0, int bsz) { return max(0, min(bsz, job.n_rows - win0)); }
 
 // ---------------------------------------------------------------------------------------------- forward cell
 // grid (ceil(u/16), n_jobs), 256 threads: 16 units x 4 gates = 64 gate columns x up to 32 batch rows.
@@ -210,39 +177,6 @@ __global__ void __launch_bounds__(256) lstm_head_kernel(const FitArgs a) {
   }
 }
 
-// ---------------------------------------------------------------------------------------------- backward: gate gradients
-// grid (ceil(MAXB*u/256), n_jobs).  Overwrites the saved gates of (l, t) with dz, updates dc_next.
-__global__ void __launch_bounds__(256) lstm_bwd_gates_kernel(const FitArgs a, int l, int t) {
-  const gb_job job = a.jobs[blockIdx.y];
-  const int nb = job_batch(job, a.step[0], a.step[1]);
-  if (nb == 0) return;
-  const Lay ly = a.lay[l];
-  const int u = ly.u, u4 = 4 * u;
-  const int i = blockIdx.x * 256 + threadIdx.x;
-  const int b = i / u, un = i - b * u;
-  if (b >= nb) return;
-  float* ws = a.ws + (long)blockIdx.y * a.ws_stride;
-  float* Z = ws + ly.zofs + (long)t * MAXB * u4 + (long)b * u4;
-  const float ig = Z[un], fg = Z[u + un], gg = Z[2 * u + un], og = Z[3 * u + un];
-  const float c = ws[ly.cofs + (long)t * MAXB * u + b * u + un];
-  const float cp = t > 0 ? ws[ly.cofs + (long)(t - 1) * MAXB * u + b * u + un] : 0.f;
-  float* nx = ws + ly.nxofs;  // dh_next [B][u], dc_next [B][u]
-  const bool last_t = t == a.L - 1;
-  float dh = last_t ? 0.f : nx[b * u + un];
-  if (l == a.n_layers - 1) {
-    if (last_t) dh += ws[a.topdh + b * u + un];
-  } else {
-    dh += ws[ly.dhofs + (long)t * MAXB * u + b * u + un];
-  }
-  const float ac = gb::apply_act(ly.act, c);
-  const float dc = dh * og * gb::act_grad_from_output(ly.act, ac) + (last_t ? 0.f : nx[MAXB * u + b * u + un]);
-  Z[un] = dc * gg * ig * (1.f - ig);
-  Z[u + un] = dc * cp * fg * (1.f - fg);
-  Z[2 * u + un] = dc * ig * gb::act_grad_from_output(ly.act, gg);
-  Z[3 * u + un] = dh * ac * og * (1.f - og);
-  nx[MAXB * u + b * u + un] = dc * fg;
-}
-
 // ---------------------------------------------------------------------------------------------- backward: [dx_t | dh_{t-1}] = dz_t [K; U]^T
 // grid (ceil(cols/64), n_jobs) over the columns that are needed (layer 0 has no dx), 256 threads.
 __global__ void __launch_bounds__(256) lstm_bwd_input_kernel(const FitArgs a, int l, int t) {
@@ -345,67 +279,6 @@ __global__ void __launch_bounds__(256) lstm_wgrad_kernel(const FitArgs a, int l)
   if (blockIdx.y == 0 && rg == 0) G[(long)KK * u4 + c] = bsum;
 }
 
-// ---------------------------------------------------------------------------------------------- Adam
-__global__ void __launch_bounds__(256) lstm_adam_kernel(const FitArgs a, long n_params) {
-  const gb_job job = a.jobs[blockIdx.y];
-  if (job_batch(job, a.step[0], a.step[1]) == 0) return;
-  const int t = a.adam_t[job.slot] + 1;
-  const float alpha = (float)((double)a.lr * sqrt(1.0 - pow((double)a.b2, (double)t)) / (1.0 - pow((double)a.b1, (double)t)));
-  const float* G = a.ws + (long)blockIdx.y * a.ws_stride + a.gofs;
-  float* P = a.params + (long)job.slot * a.pstride;
-  float* M = a.adam_m + (long)job.slot * a.pstride;
-  float* V = a.adam_v + (long)job.slot * a.pstride;
-  for (long i = (long)blockIdx.x * 256 + threadIdx.x; i < n_params; i += (long)gridDim.x * 256) {
-    const float g = G[i];
-    const float m = M[i] + (g - M[i]) * (1.f - a.b1);
-    const float v = V[i] + (g * g - V[i]) * (1.f - a.b2);
-    M[i] = m;
-    V[i] = v;
-    P[i] -= alpha * m / (sqrtf(v) + a.eps);
-  }
-}
-// Every other optimizer than plain Adam (gb::opt_update; state slots 0 / 1 = adam_m / adam_v), captured in place of lstm_adam_kernel.
-// The per-step scalars come from the slot's step count, once per CTA (for Nadam a product over the slot's steps, a few cycles each).
-__global__ void __launch_bounds__(256) lstm_opt_kernel(const FitArgs a, long n_params) {
-  const gb_job job = a.jobs[blockIdx.y];
-  if (job_batch(job, a.step[0], a.step[1]) == 0) return;
-  __shared__ gb::OptStep s_st;
-  if (threadIdx.x == 0) s_st = gb::opt_step_at(a.opt, a.adam_t[job.slot] + 1);
-  __syncthreads();
-  const gb::OptStep st = s_st;
-  const float* G = a.ws + (long)blockIdx.y * a.ws_stride + a.gofs;
-  float* P = a.params + (long)job.slot * a.pstride;
-  float* S0 = a.adam_m + (long)job.slot * a.pstride;
-  float* S1 = a.adam_v + (long)job.slot * a.pstride;
-  for (long i = (long)blockIdx.x * 256 + threadIdx.x; i < n_params; i += (long)gridDim.x * 256) {
-    float w = P[i], s0 = S0[i], s1 = S1[i];
-    gb::opt_update(a.opt, st, w, G[i], s0, s1);
-    P[i] = w;
-    S0[i] = s0;
-    S1[i] = s1;
-  }
-}
-__global__ void lstm_bump_kernel(const FitArgs a, int n_jobs) {
-  const int j = blockIdx.x * blockDim.x + threadIdx.x;
-  if (j < n_jobs && job_batch(a.jobs[j], a.step[0], a.step[1]) > 0) a.adam_t[a.jobs[j].slot] += 1;
-}
-__global__ void lstm_set_step_kernel(int* step, int win0, int bsz) {
-  step[0] = win0;
-  step[1] = bsz;
-}
-// epoch bookkeeping: history[job][epoch] = sums / n_windows; sums reset
-__global__ void lstm_epoch_kernel(const gb_job* jobs, int n_jobs, float* loss_sum, float* hit_sum, float* out_loss, float* out_acc, int epoch, int epochs) {
-  const int j = blockIdx.x * blockDim.x + threadIdx.x;
-  if (j >= n_jobs) return;
-  if (epoch >= 0) {
-    const float n = (float)max(jobs[j].n_rows, 1);
-    out_loss[(long)j * epochs + epoch] = loss_sum[j] / n;
-    out_acc[(long)j * epochs + epoch] = hit_sum[j] / n;
-  }
-  loss_sum[j] = 0.f;
-  hit_sum[j] = 0.f;
-}
-
 // ---------------------------------------------------------------------------------------------- orthogonal initialiser
 // Keras' Orthogonal for a recurrent kernel [u, 4u] [3P]: QR of a [4u, u] standard-normal draw, Q's columns sign-corrected so that
 // diag(R) > 0, transposed.  That Q is what Gram-Schmidt gives, so: one CTA per matrix orthonormalises the rows of its own
@@ -443,51 +316,47 @@ __global__ void __launch_bounds__(256) orthonormal_rows_kernel(double* g, int ro
   }
 }
 
-int validate(const gb_lstmnet* net) {
-  GB_REQUIRE(net != nullptr, GB_E_ARG, "net is NULL");
-  GB_REQUIRE(net->n_layers >= 1 && net->n_layers <= GB_MAX_LAYERS, GB_E_SHAPE, "n_layers=%d outside [1,%d]", net->n_layers, GB_MAX_LAYERS);
-  GB_REQUIRE(net->n_features >= 1 && net->n_features <= LSTM_MAX_FEATURES && net->n_features_out >= 1 && net->n_features_out <= LSTM_MAX_FEATURES,
-             GB_E_SHAPE, "n_features/n_features_out outside [1,%d]", LSTM_MAX_FEATURES);
-  GB_REQUIRE(net->lookback >= 1, GB_E_ARG, "lookback=%d must be >= 1", net->lookback);
-  for (int l = 0; l < net->n_layers; ++l) {
-    GB_REQUIRE(net->units[l] >= 1 && net->units[l] <= LSTM_MAX_UNITS, GB_E_SHAPE, "units[%d]=%d outside [1,%d]", l, net->units[l], LSTM_MAX_UNITS);
-    GB_REQUIRE(net->act[l] >= GB_ACT_LINEAR && net->act[l] <= GB_ACT_SIGMOID, GB_E_ARG, "act[%d] unknown", l);
-  }
-  return GB_OK;
-}
+// fit_driver's policy for this family: one MAXB-row tile per batch, the head of a job in one CTA
+struct Fp32Fit {
+  static constexpr int max_batch = MAXB;
+  static constexpr const char* who = "this kernel family";
+  static constexpr int head_rows = 0;
+  static int rows(int) { return MAXB; }
+  size_t head_smem = 0;
 
-// workspace layout of one job (floats); returns the total
-long layout(const gb_lstmnet* net, FitArgs* a) {
-  long ofs = 0, pofs = 0;
-  int in = net->n_features;
-  const long L = net->lookback;
-  for (int l = 0; l < net->n_layers; ++l) {
-    const int u = net->units[l];
-    Lay& ly = a->lay[l];
-    ly.in = in; ly.u = u; ly.act = net->act[l];
-    ly.kofs = pofs;
-    pofs += 4L * u * (in + u + 1);
-    ly.zofs = ofs; ofs += L * MAXB * 4 * u;
-    ly.cofs = ofs; ofs += L * MAXB * u;
-    ly.hofs = ofs; ofs += L * MAXB * u;
-    ly.dhofs = ofs; ofs += (l + 1 < net->n_layers) ? L * MAXB * u : 0;
-    ly.nxofs = ofs; ofs += 2L * MAXB * u;
-    in = u;
+  int prepare(const FitArgs& a) {
+    head_smem = (size_t)(MAXB * a.lay[a.n_layers - 1].u + 2 * MAXB * a.T_out) * sizeof(float);
+    GB_REQUIRE(head_smem <= 200 * 1024, GB_E_SMEM, "Dense head needs %zu bytes of shared memory", head_smem);
+    GB_CUDA_CHECK(cudaFuncSetAttribute(lstm_head_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)head_smem));
+    return GB_OK;
   }
-  a->dofs = pofs;
-  a->topdh = ofs; ofs += (long)MAXB * in;
-  a->gofs = ofs; ofs += (long)gb_lstm_param_stride(net);
-  return (ofs + 3) / 4 * 4;
-}
+
+  void record(const FitArgs& a, int n_jobs, cudaStream_t st) const {
+    for (int t = 0; t < a.L; ++t)
+      for (int l = 0; l < a.n_layers; ++l) lstm_fwd_kernel<<<dim3((a.lay[l].u + 15) / 16, n_jobs), 256, 0, st>>>(a, l, t);
+    lstm_head_kernel<<<n_jobs, 256, head_smem, st>>>(a);
+    for (int t = a.L - 1; t >= 0; --t)
+      for (int l = a.n_layers - 1; l >= 0; --l) {
+        const Lay& ly = a.lay[l];
+        lstm_bwd_gates_kernel<<<dim3((MAXB * ly.u + 255) / 256, n_jobs), 256, 0, st>>>(a, l, t);
+        const int cols = l == 0 ? ly.u : ly.in + ly.u;
+        if (t > 0 || l > 0) lstm_bwd_input_kernel<<<dim3((cols + 63) / 64, n_jobs), 256, 0, st>>>(a, l, t);
+      }
+    for (int l = 0; l < a.n_layers; ++l) {
+      const Lay& ly = a.lay[l];
+      lstm_wgrad_kernel<<<dim3((4 * ly.u + 63) / 64, (ly.in + ly.u + 31) / 32, n_jobs), 256, 0, st>>>(a, l);
+    }
+  }
+};
 
 }  // namespace
 
 extern "C" {
 
 size_t gb_lstm_fit_workspace_bytes(const gb_lstmnet* net, int32_t n_jobs) {
-  if (validate(net) != GB_OK || n_jobs < 0) return 0;
+  if (gb::validate_lstmnet(net) != GB_OK || n_jobs < 0) return 0;
   FitArgs a{};
-  return (size_t)(layout(net, &a) * (long)n_jobs + 2L * n_jobs + 4) * sizeof(float);
+  return workspace_bytes(layout(net, MAXB, 0, &a), n_jobs);
 }
 
 int gb_lstm_fit(const gb_lstmnet* net, float* params, float* adam_m, float* adam_v, int32_t* adam_t, const gb_job* jobs, int32_t n_jobs,
@@ -504,121 +373,19 @@ int gb_lstm_fit_loss(const gb_lstmnet* net, float* params, float* adam_m, float*
                          nullptr, stream);
 }
 
-// gb_lstm_fit_opt (stop NULL: the step graph and launches as they have always been) and gb_lstm_fit_stop
-static int launch_fit(const gb_lstmnet* net, float* params, float* adam_m, float* adam_v, int32_t* adam_t, const gb_job* jobs,
-                      int32_t n_jobs, int32_t max_windows, const float* x, const float* y, const gb_lstm_fit_hparams* hp, void* workspace,
-                      float* out_loss, float* out_acc, int32_t loss, const gb_optimizer* opt, const gb_fit_stop* stop, float* best_params,
-                      int32_t* out_epochs, int32_t* out_best_epoch, void* stream) {
-  int rc = validate(net);
-  if (rc != GB_OK) return rc;
-  if ((rc = gb::validate_optimizer(opt)) != GB_OK) return rc;
-  GB_REQUIRE(loss >= GB_LOSS_MSE && loss <= GB_LOSS_LOG_COSH, GB_E_ARG, "loss=%d unknown (gb_loss: 0..5)", loss);
-  GB_REQUIRE(params && adam_m && adam_v && adam_t && jobs && x && y && hp && workspace && out_loss && out_acc, GB_E_ARG, "NULL argument");
-  GB_REQUIRE(n_jobs >= 0 && n_jobs <= 65535 && max_windows >= 0, GB_E_ARG, "bad n_jobs/max_windows");
-  GB_REQUIRE(hp->epochs >= 0 && hp->batch_size >= 1, GB_E_ARG, "epochs=%d batch_size=%d", hp->epochs, hp->batch_size);
-  GB_REQUIRE(hp->batch_size <= MAXB, GB_E_SHAPE, "batch_size=%d: this kernel family handles batches of at most %d windows", hp->batch_size, MAXB);
-  GB_REQUIRE(hp->lookahead >= 0, GB_E_ARG, "Value of `lookahead` can not be negative, is %d", hp->lookahead);
-  if (stop != nullptr) {
-    GB_REQUIRE(best_params && out_epochs && out_best_epoch, GB_E_ARG, "stop needs best_params, out_epochs and out_best_epoch");
-    GB_REQUIRE(gb::aligned16(best_params), GB_E_ARG, "best_params must be 16-byte aligned");
-    if ((rc = lstm_stop::validate(stop, n_jobs)) != GB_OK) return rc;
-  }
-  if (n_jobs == 0) return GB_OK;
-  cudaStream_t st = (cudaStream_t)stream;
-  FitArgs a{};
-  a.n_layers = net->n_layers; a.L = net->lookback; a.F = net->n_features; a.T_out = net->n_features_out; a.out_act = net->out_act;
-  a.lookahead = hp->lookahead;
-  a.ws_stride = layout(net, &a);
-  a.pstride = (long)gb_lstm_param_stride(net);
-  a.params = params; a.adam_m = adam_m; a.adam_v = adam_v; a.adam_t = adam_t; a.jobs = jobs; a.x = x; a.y = y;
-  a.ws = static_cast<float*>(workspace);
-  a.loss_sum = a.ws + a.ws_stride * n_jobs;
-  a.hit_sum = a.loss_sum + n_jobs;
-  a.lr = hp->lr; a.b1 = hp->beta1; a.b2 = hp->beta2; a.eps = hp->eps;
-  const bool use_opt = !gb::plain_adam(opt);
-  if (opt != nullptr && !use_opt) { a.lr = opt->lr; a.b1 = opt->beta1; a.b2 = opt->beta2; a.eps = opt->eps; }  // plain Adam: the Adam kernel
-  if (use_opt) a.opt = *opt;
-  a.loss = loss;
-  const long n_params = (long)gb_lstm_param_count(net);
-  const int u_top = net->units[net->n_layers - 1];
-  const size_t head_smem = (size_t)(MAXB * u_top + 2 * MAXB * net->n_features_out) * sizeof(float);
-  GB_REQUIRE(head_smem <= 200 * 1024, GB_E_SMEM, "Dense head needs %zu bytes of shared memory", head_smem);
-  GB_CUDA_CHECK(cudaFuncSetAttribute(lstm_head_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)head_smem));
-  const int jb = (n_jobs + 127) / 128;
-
-  int* d_step = reinterpret_cast<int*>(a.hit_sum + n_jobs);
-  a.step = d_step;
-  const lstm_stop::Run run(workspace, gb_lstm_fit_workspace_bytes(net, n_jobs), jobs, n_jobs, hp->epochs, out_epochs, out_best_epoch,
-                           params, best_params, a.pstride, n_params);
-  if (stop != nullptr) {
-    run.init(stop, st);
-    a.jobs = run.job_copy;  // a job that stops gets n_rows 0 here, so job_batch gives it no windows
-  }
-  // One optimizer step is ~2 600 small launches (18 per timestep): captured once as a CUDA graph and replayed per step, the
-  // step's (first window, batch size) being read from device memory -- launch overhead was >90 % of a step for few machines.
-  cudaGraphExec_t gexec = nullptr;
-  rc = capture_step(&gexec, stop != nullptr ? run.live : nullptr, [&](cudaStream_t st) {
-    for (int t = 0; t < a.L; ++t)
-      for (int l = 0; l < a.n_layers; ++l) lstm_fwd_kernel<<<dim3((a.lay[l].u + 15) / 16, n_jobs), 256, 0, st>>>(a, l, t);
-    lstm_head_kernel<<<n_jobs, 256, head_smem, st>>>(a);
-    for (int t = a.L - 1; t >= 0; --t)
-      for (int l = a.n_layers - 1; l >= 0; --l) {
-        const Lay& ly = a.lay[l];
-        lstm_bwd_gates_kernel<<<dim3((MAXB * ly.u + 255) / 256, n_jobs), 256, 0, st>>>(a, l, t);
-        const int cols = l == 0 ? ly.u : ly.in + ly.u;
-        if (t > 0 || l > 0) lstm_bwd_input_kernel<<<dim3((cols + 63) / 64, n_jobs), 256, 0, st>>>(a, l, t);
-      }
-    for (int l = 0; l < a.n_layers; ++l) {
-      const Lay& ly = a.lay[l];
-      lstm_wgrad_kernel<<<dim3((4 * ly.u + 63) / 64, (ly.in + ly.u + 31) / 32, n_jobs), 256, 0, st>>>(a, l);
-    }
-    if (use_opt)
-      lstm_opt_kernel<<<dim3((unsigned)((n_params + 256 * 8 - 1) / (256 * 8)), n_jobs), 256, 0, st>>>(a, n_params);
-    else
-      lstm_adam_kernel<<<dim3((unsigned)((n_params + 256 * 8 - 1) / (256 * 8)), n_jobs), 256, 0, st>>>(a, n_params);
-    lstm_bump_kernel<<<jb, 128, 0, st>>>(a, n_jobs);
-  });
-  if (rc != GB_OK) return rc;
-  auto step = [&](int win0, int bsz) -> int {
-    lstm_set_step_kernel<<<1, 1, 0, st>>>(d_step, win0, bsz);
-    const cudaError_t ce = cudaGraphLaunch(gexec, st);
-    if (ce != cudaSuccess) {
-      gb::set_error("cudaGraphLaunch failed: %s", cudaGetErrorString(ce));
-      return GB_E_CUDA;
-    }
-    return GB_OK;
-  };
-
-  lstm_epoch_kernel<<<jb, 128, 0, st>>>(jobs, n_jobs, a.loss_sum, a.hit_sum, out_loss, out_acc, -1, hp->epochs);
-  if (hp->primer) {
-    if ((rc = step(0, 1)) != GB_OK) return rc;
-    lstm_epoch_kernel<<<jb, 128, 0, st>>>(jobs, n_jobs, a.loss_sum, a.hit_sum, out_loss, out_acc, -1, hp->epochs);
-  }
-  for (int e = 0; e < hp->epochs; ++e) {
-    for (int w = 0; w < max_windows; w += hp->batch_size)
-      if ((rc = step(w, hp->batch_size)) != GB_OK) return rc;
-    if (stop != nullptr) run.end_epoch(e, a.loss_sum, a.hit_sum, out_loss, out_acc, st);
-    else lstm_epoch_kernel<<<jb, 128, 0, st>>>(jobs, n_jobs, a.loss_sum, a.hit_sum, out_loss, out_acc, e, hp->epochs);
-  }
-  if (stop != nullptr) run.finish(st);
-  cudaGraphExecDestroy(gexec);  // the enqueued replays keep what they need
-  GB_CUDA_CHECK(cudaGetLastError());
-  return GB_OK;
-}
-
 int gb_lstm_fit_opt(const gb_lstmnet* net, float* params, float* adam_m, float* adam_v, int32_t* adam_t, const gb_job* jobs,
                     int32_t n_jobs, int32_t max_windows, const float* x, const float* y, const gb_lstm_fit_hparams* hp, void* workspace,
                     float* out_loss, float* out_acc, int32_t loss, const gb_optimizer* opt, void* stream) {
-  return launch_fit(net, params, adam_m, adam_v, adam_t, jobs, n_jobs, max_windows, x, y, hp, workspace, out_loss, out_acc, loss, opt,
-                    nullptr, nullptr, nullptr, nullptr, stream);
+  return fit_driver(Fp32Fit{}, net, params, adam_m, adam_v, adam_t, jobs, n_jobs, max_windows, x, y, hp, workspace, out_loss, out_acc,
+                    loss, opt, nullptr, nullptr, nullptr, nullptr, stream);
 }
 
 int gb_lstm_fit_stop(const gb_lstmnet* net, float* params, float* adam_m, float* adam_v, int32_t* adam_t, const gb_job* jobs,
                      int32_t n_jobs, int32_t max_windows, const float* x, const float* y, const gb_lstm_fit_hparams* hp, void* workspace,
                      float* out_loss, float* out_acc, int32_t loss, const gb_optimizer* opt, const gb_fit_stop* stop, float* best_params,
                      int32_t* out_epochs, int32_t* out_best_epoch, void* stream) {
-  return launch_fit(net, params, adam_m, adam_v, adam_t, jobs, n_jobs, max_windows, x, y, hp, workspace, out_loss, out_acc, loss, opt,
-                    stop, best_params, out_epochs, out_best_epoch, stream);
+  return fit_driver(Fp32Fit{}, net, params, adam_m, adam_v, adam_t, jobs, n_jobs, max_windows, x, y, hp, workspace, out_loss, out_acc,
+                    loss, opt, stop, best_params, out_epochs, out_best_epoch, stream);
 }
 
 size_t gb_lstm_fit_stop_state_bytes(int32_t n_jobs) { return n_jobs < 0 ? 0 : lstm_stop::state_bytes(n_jobs); }

@@ -21,7 +21,7 @@
 // row order, and the slice sums added in slice order.  No atomics: every launch is deterministic.
 #include "gb_common.cuh"
 #include "gb_sm90.cuh"
-#include "lstm_fit_stop.cuh"
+#include "lstm_fit_common.cuh"
 
 namespace {
 
@@ -32,41 +32,6 @@ constexpr int TN = 64;           // output columns per tile (wgmma N)
 constexpr int TK = 32;           // reduction rows staged per mma_step
 constexpr int MAX_BATCH = 256;   // largest batch_size accepted
 constexpr int HEAD_ROWS = 16;    // batch rows per CTA of the head
-constexpr int LSTM_MAX_UNITS = 512;
-constexpr int LSTM_MAX_FEATURES = 512;
-
-struct Lay {
-  int in, u;       // input width, units
-  int act;
-  long kofs;       // offset of [K; U] (rows in + u, 4u columns) in the parameter vector; bias follows
-  long zofs, cofs, hofs, dhofs, nxofs;  // workspace offsets (floats, per job): gates [L][Bp][4u], c / h [L][Bp][u], dh_seq [L][Bp][u], (dh_next, dc_next) [2][Bp][u]
-};
-
-struct FitArgs {
-  int n_layers, L, F, T_out, out_act, lookahead;
-  int Bp;           // batch rows the workspace holds per timestep: batch_size rounded up to TM
-  Lay lay[GB_MAX_LAYERS];
-  long dofs;        // Dense kernel offset in the parameter vector
-  long pstride, ws_stride;  // floats per slot / per job
-  long gofs;        // gradient vector offset in the job workspace
-  long topdh;       // [Bp][u_top] dh of the last LSTM layer at t = L-1
-  long doutofs;     // [Bp][T_out] d(loss)/d(Dense pre-activation)
-  long partofs;     // [Bp / HEAD_ROWS][2] loss and hit sums per head slice
-  float* params;
-  float *adam_m, *adam_v;
-  int* adam_t;
-  const gb_job* jobs;
-  const float *x, *y;
-  float* ws;
-  float *loss_sum, *hit_sum;  // [n_jobs]
-  const int* step;            // device: {first window, batch size} of the optimizer step being replayed
-  float lr, b1, b2, eps;
-  int loss;
-  gb_optimizer opt;  // another optimizer than plain Adam (tc_opt_kernel)
-};
-
-__device__ __forceinline__ float sigm(float z) { return 1.f / (1.f + expf(-z)); }
-__device__ __forceinline__ int job_batch(const gb_job& job, int win0, int bsz) { return max(0, min(bsz, job.n_rows - win0)); }
 
 __device__ __forceinline__ float tf32_hi(float v) {
   uint32_t r;
@@ -314,40 +279,6 @@ __global__ void __launch_bounds__(256) tc_head_grad_kernel(const FitArgs a) {
   }
 }
 
-// ---------------------------------------------------------------------------------------------- backward: gate gradients
-// grid (ceil(Bp*u/256), n_jobs).  Overwrites the saved gates of (l, t) with dz, updates dc_next.
-__global__ void __launch_bounds__(256) tc_bwd_gates_kernel(const FitArgs a, int l, int t) {
-  const gb_job job = a.jobs[blockIdx.y];
-  const int nb = job_batch(job, a.step[0], a.step[1]);
-  if (nb == 0) return;
-  const Lay ly = a.lay[l];
-  const int u = ly.u, u4 = 4 * u, Bp = a.Bp;
-  const int i = blockIdx.x * 256 + threadIdx.x;
-  const int b = i / u, un = i - b * u;
-  if (b >= nb) return;
-  float* ws = a.ws + (long)blockIdx.y * a.ws_stride;
-  float* Z = ws + ly.zofs + (long)t * Bp * u4 + (long)b * u4;
-  const float ig = Z[un], fg = Z[u + un], gg = Z[2 * u + un], og = Z[3 * u + un];
-  const long bu = (long)b * u + un;
-  const float c = ws[ly.cofs + (long)t * Bp * u + bu];
-  const float cp = t > 0 ? ws[ly.cofs + (long)(t - 1) * Bp * u + bu] : 0.f;
-  float* nx = ws + ly.nxofs;  // dh_next [Bp][u], dc_next [Bp][u]
-  const bool last_t = t == a.L - 1;
-  float dh = last_t ? 0.f : nx[bu];
-  if (l == a.n_layers - 1) {
-    if (last_t) dh += ws[a.topdh + bu];
-  } else {
-    dh += ws[ly.dhofs + (long)t * Bp * u + bu];
-  }
-  const float ac = gb::apply_act(ly.act, c);
-  const float dc = dh * og * gb::act_grad_from_output(ly.act, ac) + (last_t ? 0.f : nx[(long)Bp * u + bu]);
-  Z[un] = dc * gg * ig * (1.f - ig);
-  Z[u + un] = dc * cp * fg * (1.f - fg);
-  Z[2 * u + un] = dc * ig * gb::act_grad_from_output(ly.act, gg);
-  Z[3 * u + un] = dh * ac * og * (1.f - og);
-  nx[(long)Bp * u + bu] = dc * fg;
-}
-
 // ---------------------------------------------------------------------------------------------- backward: [dx_t | dh_{t-1}] = dz_t [K; U]^T
 // grid (ceil(cols/64), Bp/64, n_jobs) over the columns that are needed (layer 0 has no dx), 128 threads.
 __global__ void __launch_bounds__(128) tc_bwd_input_kernel(const FitArgs a, int l, int t) {
@@ -445,116 +376,50 @@ __global__ void __launch_bounds__(128) tc_wgrad_kernel(const FitArgs a, int l) {
   }
 }
 
-// ---------------------------------------------------------------------------------------------- Adam and step bookkeeping (as lstm_fit.cu)
-__global__ void __launch_bounds__(256) tc_adam_kernel(const FitArgs a, long n_params) {
-  const gb_job job = a.jobs[blockIdx.y];
-  if (job_batch(job, a.step[0], a.step[1]) == 0) return;
-  const int t = a.adam_t[job.slot] + 1;
-  const float alpha = (float)((double)a.lr * sqrt(1.0 - pow((double)a.b2, (double)t)) / (1.0 - pow((double)a.b1, (double)t)));
-  const float* G = a.ws + (long)blockIdx.y * a.ws_stride + a.gofs;
-  float* P = a.params + (long)job.slot * a.pstride;
-  float* M = a.adam_m + (long)job.slot * a.pstride;
-  float* V = a.adam_v + (long)job.slot * a.pstride;
-  for (long i = (long)blockIdx.x * 256 + threadIdx.x; i < n_params; i += (long)gridDim.x * 256) {
-    const float g = G[i];
-    const float m = M[i] + (g - M[i]) * (1.f - a.b1);
-    const float v = V[i] + (g * g - V[i]) * (1.f - a.b2);
-    M[i] = m;
-    V[i] = v;
-    P[i] -= alpha * m / (sqrtf(v) + a.eps);
-  }
-}
-// Every other optimizer than plain Adam (gb::opt_update; state slots 0 / 1 = adam_m / adam_v), captured in place of tc_adam_kernel.
-// The per-step scalars come from the slot's step count, once per CTA (for Nadam a product over the slot's steps, a few cycles each).
-__global__ void __launch_bounds__(256) tc_opt_kernel(const FitArgs a, long n_params) {
-  const gb_job job = a.jobs[blockIdx.y];
-  if (job_batch(job, a.step[0], a.step[1]) == 0) return;
-  __shared__ gb::OptStep s_st;
-  if (threadIdx.x == 0) s_st = gb::opt_step_at(a.opt, a.adam_t[job.slot] + 1);
-  __syncthreads();
-  const gb::OptStep st = s_st;
-  const float* G = a.ws + (long)blockIdx.y * a.ws_stride + a.gofs;
-  float* P = a.params + (long)job.slot * a.pstride;
-  float* S0 = a.adam_m + (long)job.slot * a.pstride;
-  float* S1 = a.adam_v + (long)job.slot * a.pstride;
-  for (long i = (long)blockIdx.x * 256 + threadIdx.x; i < n_params; i += (long)gridDim.x * 256) {
-    float w = P[i], s0 = S0[i], s1 = S1[i];
-    gb::opt_update(a.opt, st, w, G[i], s0, s1);
-    P[i] = w;
-    S0[i] = s0;
-    S1[i] = s1;
-  }
-}
-__global__ void tc_bump_kernel(const FitArgs a, int n_jobs) {
-  const int j = blockIdx.x * blockDim.x + threadIdx.x;
-  if (j < n_jobs && job_batch(a.jobs[j], a.step[0], a.step[1]) > 0) a.adam_t[a.jobs[j].slot] += 1;
-}
-__global__ void tc_set_step_kernel(int* step, int win0, int bsz) {
-  step[0] = win0;
-  step[1] = bsz;
-}
-__global__ void tc_epoch_kernel(const gb_job* jobs, int n_jobs, float* loss_sum, float* hit_sum, float* out_loss, float* out_acc, int epoch, int epochs) {
-  const int j = blockIdx.x * blockDim.x + threadIdx.x;
-  if (j >= n_jobs) return;
-  if (epoch >= 0) {
-    const float n = (float)max(jobs[j].n_rows, 1);
-    out_loss[(long)j * epochs + epoch] = loss_sum[j] / n;
-    out_acc[(long)j * epochs + epoch] = hit_sum[j] / n;
-  }
-  loss_sum[j] = 0.f;
-  hit_sum[j] = 0.f;
-}
-
-int validate(const gb_lstmnet* net) {
-  GB_REQUIRE(net != nullptr, GB_E_ARG, "net is NULL");
-  GB_REQUIRE(net->n_layers >= 1 && net->n_layers <= GB_MAX_LAYERS, GB_E_SHAPE, "n_layers=%d outside [1,%d]", net->n_layers, GB_MAX_LAYERS);
-  GB_REQUIRE(net->n_features >= 1 && net->n_features <= LSTM_MAX_FEATURES && net->n_features_out >= 1 && net->n_features_out <= LSTM_MAX_FEATURES,
-             GB_E_SHAPE, "n_features/n_features_out outside [1,%d]", LSTM_MAX_FEATURES);
-  GB_REQUIRE(net->lookback >= 1, GB_E_ARG, "lookback=%d must be >= 1", net->lookback);
-  for (int l = 0; l < net->n_layers; ++l) {
-    GB_REQUIRE(net->units[l] >= 1 && net->units[l] <= LSTM_MAX_UNITS, GB_E_SHAPE, "units[%d]=%d outside [1,%d]", l, net->units[l], LSTM_MAX_UNITS);
-    GB_REQUIRE(net->act[l] >= GB_ACT_LINEAR && net->act[l] <= GB_ACT_SIGMOID, GB_E_ARG, "act[%d] unknown", l);
-  }
-  return GB_OK;
-}
-
 int padded_batch(int batch_size) { return (batch_size + TM - 1) / TM * TM; }
 
-// workspace layout of one job (floats) for batches of up to Bp windows; returns the total
-long layout(const gb_lstmnet* net, int Bp, FitArgs* a) {
-  long ofs = 0, pofs = 0;
-  int in = net->n_features;
-  const long L = net->lookback;
-  a->Bp = Bp;
-  for (int l = 0; l < net->n_layers; ++l) {
-    const int u = net->units[l];
-    Lay& ly = a->lay[l];
-    ly.in = in; ly.u = u; ly.act = net->act[l];
-    ly.kofs = pofs;
-    pofs += 4L * u * (in + u + 1);
-    ly.zofs = ofs; ofs += L * Bp * 4 * u;
-    ly.cofs = ofs; ofs += L * Bp * u;
-    ly.hofs = ofs; ofs += L * Bp * u;
-    ly.dhofs = ofs; ofs += (l + 1 < net->n_layers) ? L * Bp * u : 0;
-    ly.nxofs = ofs; ofs += 2L * Bp * u;
-    in = u;
+// fit_driver's policy for this family: the batch in TM-row tiles, the head in HEAD_ROWS-row slices
+struct TcFit {
+  static constexpr int max_batch = MAX_BATCH;
+  static constexpr const char* who = "the tensor-core LSTM fit";
+  static constexpr int head_rows = HEAD_ROWS;
+  static int rows(int batch_size) { return padded_batch(batch_size); }
+  size_t head_smem = 0;
+
+  int prepare(const FitArgs& a) {
+    head_smem = (size_t)(HEAD_ROWS * a.lay[a.n_layers - 1].u + 2 * HEAD_ROWS * a.T_out) * sizeof(float);
+    GB_CUDA_CHECK(cudaFuncSetAttribute(tc_head_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)head_smem));
+    return GB_OK;
   }
-  a->dofs = pofs;
-  a->topdh = ofs; ofs += (long)Bp * in;
-  a->doutofs = ofs; ofs += (long)Bp * net->n_features_out;
-  a->partofs = ofs; ofs += 2L * (Bp / HEAD_ROWS);
-  a->gofs = ofs; ofs += (long)gb_lstm_param_stride(net);
-  return (ofs + 3) / 4 * 4;
-}
+
+  void record(const FitArgs& a, int n_jobs, cudaStream_t st) const {
+    const int nbt = a.Bp / TM, u_top = a.lay[a.n_layers - 1].u, T = a.T_out;
+    for (int t = 0; t < a.L; ++t)
+      for (int l = 0; l < a.n_layers; ++l) tc_fwd_kernel<<<dim3((a.lay[l].u + 15) / 16, nbt, n_jobs), 128, 0, st>>>(a, l, t);
+    tc_head_rows_kernel<<<dim3(a.Bp / HEAD_ROWS, n_jobs), 256, head_smem, st>>>(a);
+    tc_head_grad_kernel<<<dim3(((u_top + 1) * T + 255) / 256, n_jobs), 256, 0, st>>>(a);
+    for (int t = a.L - 1; t >= 0; --t)
+      for (int l = a.n_layers - 1; l >= 0; --l) {
+        const Lay& ly = a.lay[l];
+        lstm_bwd_gates_kernel<<<dim3((a.Bp * ly.u + 255) / 256, n_jobs), 256, 0, st>>>(a, l, t);
+        const int cols = l == 0 ? ly.u : ly.in + ly.u;
+        if (t > 0 || l > 0) tc_bwd_input_kernel<<<dim3((cols + TN - 1) / TN, nbt, n_jobs), 128, 0, st>>>(a, l, t);
+      }
+    for (int l = 0; l < a.n_layers; ++l) {
+      const Lay& ly = a.lay[l];
+      tc_wgrad_kernel<<<dim3((4 * ly.u + TN - 1) / TN, (ly.in + ly.u + 1 + TM - 1) / TM, n_jobs), 128, 0, st>>>(a, l);
+    }
+  }
+};
 
 }  // namespace
 
 extern "C" {
 
 size_t gb_lstm_fit_tc_workspace_bytes(const gb_lstmnet* net, int32_t n_jobs, int32_t batch_size) {
-  if (validate(net) != GB_OK || n_jobs < 0 || batch_size < 1 || batch_size > MAX_BATCH) return 0;
+  if (gb::validate_lstmnet(net) != GB_OK || n_jobs < 0 || batch_size < 1 || batch_size > MAX_BATCH) return 0;
   FitArgs a{};
-  return (size_t)(layout(net, padded_batch(batch_size), &a) * (long)n_jobs + 2L * n_jobs + 4) * sizeof(float);
+  return workspace_bytes(layout(net, padded_batch(batch_size), HEAD_ROWS, &a), n_jobs);
 }
 
 int gb_lstm_fit_tc(const gb_lstmnet* net, float* params, float* adam_m, float* adam_v, int32_t* adam_t, const gb_job* jobs,
@@ -564,123 +429,19 @@ int gb_lstm_fit_tc(const gb_lstmnet* net, float* params, float* adam_m, float* a
                             nullptr, stream);
 }
 
-// gb_lstm_fit_tc_opt (stop NULL: the step graph and launches as they have always been) and gb_lstm_fit_tc_stop
-static int launch_fit(const gb_lstmnet* net, float* params, float* adam_m, float* adam_v, int32_t* adam_t, const gb_job* jobs,
-                      int32_t n_jobs, int32_t max_windows, const float* x, const float* y, const gb_lstm_fit_hparams* hp, void* workspace,
-                      float* out_loss, float* out_acc, int32_t loss, const gb_optimizer* opt, const gb_fit_stop* stop, float* best_params,
-                      int32_t* out_epochs, int32_t* out_best_epoch, void* stream) {
-  int rc = validate(net);
-  if (rc != GB_OK) return rc;
-  if ((rc = gb::validate_optimizer(opt)) != GB_OK) return rc;
-  GB_REQUIRE(loss >= GB_LOSS_MSE && loss <= GB_LOSS_LOG_COSH, GB_E_ARG, "loss=%d unknown (gb_loss: 0..5)", loss);
-  GB_REQUIRE(params && adam_m && adam_v && adam_t && jobs && x && y && hp && workspace && out_loss && out_acc, GB_E_ARG, "NULL argument");
-  GB_REQUIRE(n_jobs >= 0 && n_jobs <= 65535 && max_windows >= 0, GB_E_ARG, "bad n_jobs/max_windows");
-  GB_REQUIRE(hp->epochs >= 0 && hp->batch_size >= 1, GB_E_ARG, "epochs=%d batch_size=%d", hp->epochs, hp->batch_size);
-  GB_REQUIRE(hp->batch_size <= MAX_BATCH, GB_E_SHAPE, "batch_size=%d: the tensor-core LSTM fit handles batches of at most %d windows",
-             hp->batch_size, MAX_BATCH);
-  GB_REQUIRE(hp->lookahead >= 0, GB_E_ARG, "Value of `lookahead` can not be negative, is %d", hp->lookahead);
-  if (stop != nullptr) {
-    GB_REQUIRE(best_params && out_epochs && out_best_epoch, GB_E_ARG, "stop needs best_params, out_epochs and out_best_epoch");
-    GB_REQUIRE(gb::aligned16(best_params), GB_E_ARG, "best_params must be 16-byte aligned");
-    if ((rc = lstm_stop::validate(stop, n_jobs)) != GB_OK) return rc;
-  }
-  if (n_jobs == 0) return GB_OK;
-  cudaStream_t st = (cudaStream_t)stream;
-  FitArgs a{};
-  a.n_layers = net->n_layers; a.L = net->lookback; a.F = net->n_features; a.T_out = net->n_features_out; a.out_act = net->out_act;
-  a.lookahead = hp->lookahead;
-  a.ws_stride = layout(net, padded_batch(hp->batch_size), &a);
-  a.pstride = (long)gb_lstm_param_stride(net);
-  a.params = params; a.adam_m = adam_m; a.adam_v = adam_v; a.adam_t = adam_t; a.jobs = jobs; a.x = x; a.y = y;
-  a.ws = static_cast<float*>(workspace);
-  a.loss_sum = a.ws + a.ws_stride * n_jobs;
-  a.hit_sum = a.loss_sum + n_jobs;
-  a.lr = hp->lr; a.b1 = hp->beta1; a.b2 = hp->beta2; a.eps = hp->eps;
-  const bool use_opt = !gb::plain_adam(opt);
-  if (opt != nullptr && !use_opt) { a.lr = opt->lr; a.b1 = opt->beta1; a.b2 = opt->beta2; a.eps = opt->eps; }  // plain Adam: the Adam kernel
-  if (use_opt) a.opt = *opt;
-  a.loss = loss;
-  const long n_params = (long)gb_lstm_param_count(net);
-  const int u_top = net->units[net->n_layers - 1], T = net->n_features_out;
-  const size_t head_smem = (size_t)(HEAD_ROWS * u_top + 2 * HEAD_ROWS * T) * sizeof(float);
-  GB_CUDA_CHECK(cudaFuncSetAttribute(tc_head_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)head_smem));
-  const int jb = (n_jobs + 127) / 128;
-  const int nbt = a.Bp / TM;
-
-  int* d_step = reinterpret_cast<int*>(a.hit_sum + n_jobs);
-  a.step = d_step;
-  const lstm_stop::Run run(workspace, gb_lstm_fit_tc_workspace_bytes(net, n_jobs, hp->batch_size), jobs, n_jobs, hp->epochs, out_epochs,
-                           out_best_epoch, params, best_params, a.pstride, n_params);
-  if (stop != nullptr) {
-    run.init(stop, st);
-    a.jobs = run.job_copy;  // a job that stops gets n_rows 0 here, so job_batch gives it no windows
-  }
-  // the launch sequence of one optimizer step, captured once and replayed per step as in gb_lstm_fit_loss
-  cudaGraphExec_t gexec = nullptr;
-  rc = capture_step(&gexec, stop != nullptr ? run.live : nullptr, [&](cudaStream_t st) {
-    for (int t = 0; t < a.L; ++t)
-      for (int l = 0; l < a.n_layers; ++l) tc_fwd_kernel<<<dim3((a.lay[l].u + 15) / 16, nbt, n_jobs), 128, 0, st>>>(a, l, t);
-    tc_head_rows_kernel<<<dim3(a.Bp / HEAD_ROWS, n_jobs), 256, head_smem, st>>>(a);
-    tc_head_grad_kernel<<<dim3(((u_top + 1) * T + 255) / 256, n_jobs), 256, 0, st>>>(a);
-    for (int t = a.L - 1; t >= 0; --t)
-      for (int l = a.n_layers - 1; l >= 0; --l) {
-        const Lay& ly = a.lay[l];
-        tc_bwd_gates_kernel<<<dim3((a.Bp * ly.u + 255) / 256, n_jobs), 256, 0, st>>>(a, l, t);
-        const int cols = l == 0 ? ly.u : ly.in + ly.u;
-        if (t > 0 || l > 0) tc_bwd_input_kernel<<<dim3((cols + TN - 1) / TN, nbt, n_jobs), 128, 0, st>>>(a, l, t);
-      }
-    for (int l = 0; l < a.n_layers; ++l) {
-      const Lay& ly = a.lay[l];
-      tc_wgrad_kernel<<<dim3((4 * ly.u + TN - 1) / TN, (ly.in + ly.u + 1 + TM - 1) / TM, n_jobs), 128, 0, st>>>(a, l);
-    }
-    if (use_opt)
-      tc_opt_kernel<<<dim3((unsigned)((n_params + 256 * 8 - 1) / (256 * 8)), n_jobs), 256, 0, st>>>(a, n_params);
-    else
-      tc_adam_kernel<<<dim3((unsigned)((n_params + 256 * 8 - 1) / (256 * 8)), n_jobs), 256, 0, st>>>(a, n_params);
-    tc_bump_kernel<<<jb, 128, 0, st>>>(a, n_jobs);
-  });
-  if (rc != GB_OK) return rc;
-  auto step = [&](int win0, int bsz) -> int {
-    tc_set_step_kernel<<<1, 1, 0, st>>>(d_step, win0, bsz);
-    const cudaError_t ce = cudaGraphLaunch(gexec, st);
-    if (ce != cudaSuccess) {
-      cudaGraphExecDestroy(gexec);
-      gb::set_error("cudaGraphLaunch failed: %s", cudaGetErrorString(ce));
-      return GB_E_CUDA;
-    }
-    return GB_OK;
-  };
-
-  tc_epoch_kernel<<<jb, 128, 0, st>>>(jobs, n_jobs, a.loss_sum, a.hit_sum, out_loss, out_acc, -1, hp->epochs);
-  if (hp->primer) {
-    if ((rc = step(0, 1)) != GB_OK) return rc;
-    tc_epoch_kernel<<<jb, 128, 0, st>>>(jobs, n_jobs, a.loss_sum, a.hit_sum, out_loss, out_acc, -1, hp->epochs);
-  }
-  for (int e = 0; e < hp->epochs; ++e) {
-    for (int w = 0; w < max_windows; w += hp->batch_size)
-      if ((rc = step(w, hp->batch_size)) != GB_OK) return rc;
-    if (stop != nullptr) run.end_epoch(e, a.loss_sum, a.hit_sum, out_loss, out_acc, st);
-    else tc_epoch_kernel<<<jb, 128, 0, st>>>(jobs, n_jobs, a.loss_sum, a.hit_sum, out_loss, out_acc, e, hp->epochs);
-  }
-  if (stop != nullptr) run.finish(st);
-  cudaGraphExecDestroy(gexec);  // the enqueued replays keep what they need
-  GB_CUDA_CHECK(cudaGetLastError());
-  return GB_OK;
-}
-
 int gb_lstm_fit_tc_opt(const gb_lstmnet* net, float* params, float* adam_m, float* adam_v, int32_t* adam_t, const gb_job* jobs,
                        int32_t n_jobs, int32_t max_windows, const float* x, const float* y, const gb_lstm_fit_hparams* hp, void* workspace,
                        float* out_loss, float* out_acc, int32_t loss, const gb_optimizer* opt, void* stream) {
-  return launch_fit(net, params, adam_m, adam_v, adam_t, jobs, n_jobs, max_windows, x, y, hp, workspace, out_loss, out_acc, loss, opt,
-                    nullptr, nullptr, nullptr, nullptr, stream);
+  return fit_driver(TcFit{}, net, params, adam_m, adam_v, adam_t, jobs, n_jobs, max_windows, x, y, hp, workspace, out_loss, out_acc,
+                    loss, opt, nullptr, nullptr, nullptr, nullptr, stream);
 }
 
 int gb_lstm_fit_tc_stop(const gb_lstmnet* net, float* params, float* adam_m, float* adam_v, int32_t* adam_t, const gb_job* jobs,
                         int32_t n_jobs, int32_t max_windows, const float* x, const float* y, const gb_lstm_fit_hparams* hp, void* workspace,
                         float* out_loss, float* out_acc, int32_t loss, const gb_optimizer* opt, const gb_fit_stop* stop, float* best_params,
                         int32_t* out_epochs, int32_t* out_best_epoch, void* stream) {
-  return launch_fit(net, params, adam_m, adam_v, adam_t, jobs, n_jobs, max_windows, x, y, hp, workspace, out_loss, out_acc, loss, opt,
-                    stop, best_params, out_epochs, out_best_epoch, stream);
+  return fit_driver(TcFit{}, net, params, adam_m, adam_v, adam_t, jobs, n_jobs, max_windows, x, y, hp, workspace, out_loss, out_acc,
+                    loss, opt, stop, best_params, out_epochs, out_best_epoch, stream);
 }
 
 }  // extern "C"

@@ -15,8 +15,6 @@ namespace {
 constexpr int THREADS = 256;
 constexpr int NWARPS = THREADS / 32;
 constexpr int BW = 16;  // windows per CTA
-constexpr int LSTM_MAX_UNITS = 512;
-constexpr int LSTM_MAX_FEATURES = 512;
 
 struct LstmArgs {
   gb_lstmnet net;
@@ -176,22 +174,6 @@ __global__ void __launch_bounds__(THREADS) lstm_infer_kernel(const LstmArgs a) {
   }
 }
 
-int validate_lstm(const gb_lstmnet* net) {
-  GB_REQUIRE(net != nullptr, GB_E_ARG, "net is NULL");
-  GB_REQUIRE(net->n_layers >= 1 && net->n_layers <= GB_MAX_LAYERS, GB_E_SHAPE, "n_layers=%d outside [1,%d]",
-             net->n_layers, GB_MAX_LAYERS);
-  GB_REQUIRE(net->n_features >= 1 && net->n_features <= LSTM_MAX_FEATURES && net->n_features_out >= 1 &&
-                 net->n_features_out <= LSTM_MAX_FEATURES,
-             GB_E_SHAPE, "n_features/n_features_out outside [1,%d]", LSTM_MAX_FEATURES);
-  GB_REQUIRE(net->lookback >= 1, GB_E_ARG, "lookback=%d must be >= 1", net->lookback);
-  for (int l = 0; l < net->n_layers; ++l) {
-    GB_REQUIRE(net->units[l] >= 1 && net->units[l] <= LSTM_MAX_UNITS, GB_E_SHAPE, "units[%d]=%d outside [1,%d]", l,
-               net->units[l], LSTM_MAX_UNITS);
-    GB_REQUIRE(net->act[l] >= GB_ACT_LINEAR && net->act[l] <= GB_ACT_SIGMOID, GB_E_ARG, "act[%d] unknown", l);
-  }
-  return GB_OK;
-}
-
 int pitch4(int w) {
   int p4 = (w + 3) / 4;
   if ((p4 & 1) == 0) ++p4;
@@ -203,7 +185,7 @@ int pitch4(int w) {
 extern "C" {
 
 size_t gb_lstm_param_count(const gb_lstmnet* net) {
-  if (validate_lstm(net) != GB_OK) return 0;
+  if (gb::validate_lstmnet(net) != GB_OK) return 0;
   size_t p = 0;
   int in = net->n_features;
   for (int l = 0; l < net->n_layers; ++l) {
@@ -220,7 +202,7 @@ size_t gb_lstm_workspace_bytes(const gb_lstmnet*, int32_t, int32_t) { return 0; 
 
 int gb_lstm_infer(const gb_lstmnet* net, const float* params, const gb_job* jobs, int32_t n_jobs, int32_t max_rows,
                   const float* x, float* out_model, void* /*workspace*/, void* stream) {
-  int rc = validate_lstm(net);
+  int rc = gb::validate_lstmnet(net);
   if (rc != GB_OK) return rc;
   GB_REQUIRE(params && jobs && x && out_model, GB_E_ARG, "params/jobs/x/out_model must be non-NULL");
   GB_REQUIRE(n_jobs >= 0 && max_rows >= 0, GB_E_ARG, "bad n_jobs/max_rows");

@@ -187,27 +187,15 @@ class FFEngine:
         (``_cabi.LOSS_CODES``) the fit minimises and reports.  ``optimizer``: None (Adam from ``adam``) or the (name, record) pair of
         ``factories.specs.resolve_optimizer`` (gb_ffae_fit_opt); (m, v) are then its state slots 0 and 1.
         """
-        torch = _torch()
         hp = _fit_hparams(epochs, batch_size, shuffle, perm, adam, seed, l1_div_batch, step0, loss)
-        m, v = self._fit_state(params, state)
-        hist = torch.empty((n_jobs, epochs), dtype=torch.float32, device=self.device)
-        acc = torch.empty((n_jobs, epochs), dtype=torch.float32, device=self.device)
-        p = _cabi.ptr
-        if optimizer is not None:
-            opt = _cabi.make_optimizer(*optimizer)
-            _cabi.check(self.lib.gb_ffae_fit_opt(C.byref(self.net), p(params), p(m), p(v), p(jobs_dev), None, int(n_jobs), int(max_rows), p(x),
-                                                 p(y), None, p(perm), C.byref(hp), 1, p(hist), p(acc), None, None, None, None, None, None,
-                                                 C.byref(opt), _stream_ptr()))
-            return hist, acc, (m, v)
-        _cabi.check(self.lib.gb_ffae_fit(C.byref(self.net), p(params), p(m), p(v), p(jobs_dev), int(n_jobs), int(max_rows), p(x), p(y),
-                                         p(perm), C.byref(hp), p(hist), p(acc), _stream_ptr()))
-        return hist, acc, (m, v)
+        hist, acc, *_, mv = self._fit_launch(params, jobs_dev, n_jobs, max_rows, x, y, perm, hp, state, optimizer)
+        return hist, acc, mv
 
     def fit_split(self, params, jobs_dev, n_jobs: int, max_rows: int, x, y, split=None, row_map=None, val_batch: Optional[int] = None,
                   epochs: int = 1, batch_size: int = 32, shuffle=True, perm=None, adam: Optional[Dict[str, float]] = None, seed: int = 0,
                   l1_div_batch: bool = False, state=None, step0: int = 0, stop=None, loss: str = "mse", optimizer=None):
         """
-        ``fit`` over row *positions* with Keras' ``validation_split``, in one launch (gb_ffae_fit_split).  Job i trains on its
+        ``fit`` over row *positions* with Keras' ``validation_split``, in one launch (gb_ffae_fit_opt with a split).  Job i trains on its
         positions [0, n_rows) exactly as ``fit`` trains on its rows, and after every epoch runs the network forward over the held-out
         positions [n_rows, n_rows + split[i].n_val) in batches of ``val_batch`` (default ``batch_size``) rows -- what Keras reports as
         ``val_loss`` / ``val_accuracy``.  Position p reads row x_row + row_map[map_ofs + p] (x_row + p where map_ofs is -1).
@@ -218,46 +206,46 @@ class FFEngine:
         positions are NaN.
 
         ``stop``: ``make_stop`` records [n_jobs] (host array or device bytes): every job applies its Keras EarlyStopping rule at the
-        end of each epoch inside the launch (gb_ffae_fit_stop) and leaves the kernel when it fires; with ``restore_best_weights``
+        end of each epoch inside the launch (gb_ffae_fit_opt with a stop array) and leaves the kernel when it fires; with ``restore_best_weights``
         its slot of ``params`` ends with the weights of its best epoch.  Returns (loss, accuracy, val_loss, val_accuracy,
         epochs_run, best_epoch, (m, v)): epochs_run / best_epoch are int32 [n_jobs] (best_epoch -1 when no epoch improved and no
         snapshot was taken), and every history entry past a job's epochs_run is NaN.
 
         ``loss``, ``optimizer``: as in ``fit``; the held-out statistics report the same loss.
         """
-        torch = _torch()
         hp = _fit_hparams(epochs, batch_size, shuffle, perm, adam, seed, l1_div_batch, step0, loss)
+        vb = int(val_batch if val_batch is not None else batch_size)
+        *out, epochs_run, best_epoch, mv = self._fit_launch(params, jobs_dev, n_jobs, max_rows, x, y, perm, hp, state, optimizer, val=True,
+                                                            split=split, row_map=row_map, val_batch=vb, stop=stop)
+        return (*out, mv) if stop is None else (*out, epochs_run, best_epoch, mv)
+
+    def _fit_launch(self, params, jobs_dev, n_jobs, max_rows, x, y, perm, hp, state, optimizer, val=False, split=None, row_map=None,
+                    val_batch=1, stop=None):
+        """
+        The one gb_ffae_fit_opt launch of ``fit`` and ``fit_split``, with NULL where there is no split, stop rule or optimizer.
+        Returns (loss, accuracy, val_loss, val_accuracy, epochs_run, best_epoch, (m, v)): val_* (NaN where no held-out pass writes)
+        only with ``val``; epochs_run / best_epoch only with ``stop``, which also fills loss / accuracy with NaN first.
+        """
+        torch = _torch()
         m, v = self._fit_state(params, state)
         if split is not None and isinstance(split, np.ndarray):
             split = jobs_to_device(split, self.device)
+        shape = (n_jobs, hp.epochs)
         make = torch.empty if stop is None else (lambda shape, **kw: torch.full(shape, float("nan"), **kw))  # noqa: E731
-        out = [make((n_jobs, epochs), dtype=torch.float32, device=self.device) for _ in range(2)]
-        out += [torch.full((n_jobs, epochs), float("nan"), dtype=torch.float32, device=self.device) for _ in range(2)]
-        vb = int(val_batch if val_batch is not None else batch_size)
-        p = _cabi.ptr
+        out = [make(shape, dtype=torch.float32, device=self.device) for _ in range(2)]
+        out += [torch.full(shape, float("nan"), dtype=torch.float32, device=self.device) if val else None for _ in range(2)]
+        best = epochs_run = best_epoch = None
+        if stop is not None:
+            if isinstance(stop, np.ndarray):
+                stop = jobs_to_device(stop, self.device)
+            best = torch.empty_like(params)  # snapshot area
+            epochs_run = torch.zeros((n_jobs,), dtype=torch.int32, device=self.device)
+            best_epoch = torch.full((n_jobs,), -1, dtype=torch.int32, device=self.device)
         opt = None if optimizer is None else _cabi.make_optimizer(*optimizer)
-        if stop is None and opt is not None:
-            _cabi.check(self.lib.gb_ffae_fit_opt(C.byref(self.net), p(params), p(m), p(v), p(jobs_dev), p(split), int(n_jobs), int(max_rows),
-                                                 p(x), p(y), p(row_map), p(perm), C.byref(hp), vb, *(p(t) for t in out), None, None, None, None,
-                                                 C.byref(opt), _stream_ptr()))
-            return (*out, (m, v))
-        if stop is None:
-            _cabi.check(self.lib.gb_ffae_fit_split(C.byref(self.net), p(params), p(m), p(v), p(jobs_dev), p(split), int(n_jobs), int(max_rows),
-                                                   p(x), p(y), p(row_map), p(perm), C.byref(hp), vb, *(p(t) for t in out), _stream_ptr()))
-            return (*out, (m, v))
-        if isinstance(stop, np.ndarray):
-            stop = jobs_to_device(stop, self.device)
-        best = torch.empty_like(params)  # snapshot area
-        epochs_run = torch.zeros((n_jobs,), dtype=torch.int32, device=self.device)
-        best_epoch = torch.full((n_jobs,), -1, dtype=torch.int32, device=self.device)
-        if opt is not None:
-            _cabi.check(self.lib.gb_ffae_fit_opt(C.byref(self.net), p(params), p(m), p(v), p(jobs_dev), p(split), int(n_jobs), int(max_rows),
-                                                 p(x), p(y), p(row_map), p(perm), C.byref(hp), vb, *(p(t) for t in out), p(stop), p(best),
-                                                 p(epochs_run), p(best_epoch), C.byref(opt), _stream_ptr()))
-            return (*out, epochs_run, best_epoch, (m, v))
-        _cabi.check(self.lib.gb_ffae_fit_stop(C.byref(self.net), p(params), p(m), p(v), p(jobs_dev), p(split), int(n_jobs), int(max_rows),
-                                              p(x), p(y), p(row_map), p(perm), C.byref(hp), vb, *(p(t) for t in out), p(stop), p(best),
-                                              p(epochs_run), p(best_epoch), _stream_ptr()))
+        p = _cabi.ptr
+        _cabi.check(self.lib.gb_ffae_fit_opt(C.byref(self.net), p(params), p(m), p(v), p(jobs_dev), p(split), int(n_jobs), int(max_rows), p(x),
+                                             p(y), p(row_map), p(perm), C.byref(hp), int(val_batch), *(p(t) for t in out), p(stop), p(best),
+                                             p(epochs_run), p(best_epoch), None if opt is None else C.byref(opt), _stream_ptr()))
         return (*out, epochs_run, best_epoch, (m, v))
 
     def _fit_state(self, params, state):
@@ -628,10 +616,9 @@ class LSTMEngine:
         Keras loss name (``_cabi.LOSS_CODES``), for the primer step too (gb_lstm_fit_loss).  ``optimizer``: None (Adam from
         ``adam``) or the (name, record) pair of ``factories.specs.resolve_optimizer`` (gb_lstm_fit_opt); m and v are its state slots.
         """
-        ws_bytes = int(self.lib.gb_lstm_fit_workspace_bytes(C.byref(self.net), int(n_jobs)))
-        entry = self.lib.gb_lstm_fit_loss if optimizer is None else self.lib.gb_lstm_fit_opt
-        return self._fit_launch(entry, ws_bytes, params, jobs_dev, n_jobs, max_windows, x, y, epochs, batch_size,
-                                lookahead, primer, adam, state, loss, optimizer)
+        hist, acc, _, _, st = self._fit_launch(False, params, jobs_dev, n_jobs, max_windows, x, y, epochs, batch_size, lookahead, primer,
+                                               adam, state, loss, optimizer)
+        return hist, acc, st
 
     def fit_tc(self, params, jobs_dev, n_jobs, max_windows, x, y, epochs: int = 1, batch_size: int = 32, lookahead: int = 0,
                primer: bool = True, adam: Optional[Dict[str, float]] = None, state=None, loss: str = "mse", optimizer=None):
@@ -642,10 +629,9 @@ class LSTMEngine:
         """
         if not 1 <= int(batch_size) <= self.TC_MAX_BATCH:
             raise ValueError(f"batch_size={int(batch_size)}: the LSTM fit handles batches of 1 to {self.TC_MAX_BATCH} windows")
-        ws_bytes = self.fit_tc_workspace_bytes(n_jobs, batch_size)
-        entry = self.lib.gb_lstm_fit_tc if optimizer is None else self.lib.gb_lstm_fit_tc_opt
-        return self._fit_launch(entry, ws_bytes, params, jobs_dev, n_jobs, max_windows, x, y, epochs, batch_size,
-                                lookahead, primer, adam, state, loss, optimizer)
+        hist, acc, _, _, st = self._fit_launch(True, params, jobs_dev, n_jobs, max_windows, x, y, epochs, batch_size, lookahead, primer,
+                                               adam, state, loss, optimizer)
+        return hist, acc, st
 
     def fit_stop(self, params, jobs_dev, n_jobs, max_windows, x, y, stop, epochs: int = 1, batch_size: int = 32, lookahead: int = 0,
                  primer: bool = True, adam: Optional[Dict[str, float]] = None, state=None, loss: str = "mse", optimizer=None):
@@ -657,30 +643,31 @@ class LSTMEngine:
         are int32 [n_jobs] (best_epoch -1 when no epoch improved and no snapshot was taken), and every history entry past a job's
         epochs_run is NaN.  The other arguments and (m, v, t) are ``fit``'s.
         """
-        torch = _torch()
         if not 1 <= int(batch_size) <= self.TC_MAX_BATCH:
             raise ValueError(f"batch_size={int(batch_size)}: the LSTM fit handles batches of 1 to {self.TC_MAX_BATCH} windows")
         stop = np.ascontiguousarray(stop, dtype=_cabi.STOP_DTYPE)
         if stop.shape != (int(n_jobs),):
             raise ValueError(f"stop holds {stop.shape} records for {int(n_jobs)} jobs")
-        tc = int(batch_size) > self.FP32_MAX_BATCH
-        ws_bytes = self.fit_workspace_bytes_for_batch(n_jobs, batch_size) + int(self.lib.gb_lstm_fit_stop_state_bytes(int(n_jobs)))
-        entry = self.lib.gb_lstm_fit_tc_stop if tc else self.lib.gb_lstm_fit_stop
-        epochs_run = torch.zeros((int(n_jobs),), dtype=torch.int32, device=self.device)
-        best_epoch = torch.full((int(n_jobs),), -1, dtype=torch.int32, device=self.device)
-        best = torch.empty_like(params)  # snapshot area
-        hist, acc, st = self._fit_launch(entry, ws_bytes, params, jobs_dev, n_jobs, max_windows, x, y, epochs, batch_size, lookahead, primer,
-                                         adam, state, loss, optimizer, stop=(stop, best, epochs_run, best_epoch))
-        return hist, acc, epochs_run, best_epoch, st
+        return self._fit_launch(int(batch_size) > self.FP32_MAX_BATCH, params, jobs_dev, n_jobs, max_windows, x, y, epochs, batch_size,
+                                lookahead, primer, adam, state, loss, optimizer, stop=stop)
 
-    def _fit_launch(self, entry, ws_bytes, params, jobs_dev, n_jobs, max_windows, x, y, epochs, batch_size, lookahead, primer, adam, state,
-                    loss, optimizer=None, stop=None):
-        code = _cabi.loss_code(loss)
-        opt = () if optimizer is None else (C.byref(_cabi.make_optimizer(*optimizer)),)
-        if stop is not None:  # the _stop entry points always take the optimizer argument, then the rule's arrays
-            records, best, epochs_run, best_epoch = stop
-            opt = (opt[0] if opt else None, records.ctypes.data_as(C.c_void_p), _cabi.ptr(best), _cabi.ptr(epochs_run), _cabi.ptr(best_epoch))
+    def _fit_launch(self, tc, params, jobs_dev, n_jobs, max_windows, x, y, epochs, batch_size, lookahead, primer, adam, state, loss,
+                    optimizer=None, stop=None):
+        """
+        The one launch of ``fit`` / ``fit_tc`` / ``fit_stop``: the family's _stop entry (gb_lstm_fit_tc_stop if ``tc``, else
+        gb_lstm_fit_stop), with NULL for a missing optimizer and, without ``stop`` records, for the rule and its outputs.  Returns
+        (loss, accuracy, epochs_run, best_epoch, (m, v, t)); epochs_run / best_epoch None without ``stop``.
+        """
         torch = _torch()
+        entry = self.lib.gb_lstm_fit_tc_stop if tc else self.lib.gb_lstm_fit_stop
+        ws_bytes = self.fit_tc_workspace_bytes(n_jobs, batch_size) if tc else self.fit_workspace_bytes(n_jobs)
+        best = epochs_run = best_epoch = None
+        if stop is not None:
+            ws_bytes += int(self.lib.gb_lstm_fit_stop_state_bytes(int(n_jobs)))
+            epochs_run = torch.zeros((int(n_jobs),), dtype=torch.int32, device=self.device)
+            best_epoch = torch.full((int(n_jobs),), -1, dtype=torch.int32, device=self.device)
+            best = torch.empty_like(params)  # snapshot area
+        opt = None if optimizer is None else _cabi.make_optimizer(*optimizer)
         adam = adam or {}
         hp = _cabi.GbLstmFitHParams()
         hp.epochs, hp.batch_size, hp.lookahead, hp.primer = int(epochs), int(batch_size), int(lookahead), int(bool(primer))
@@ -700,8 +687,9 @@ class LSTMEngine:
         acc = torch.full((n_jobs, max(epochs, 1)), fill, dtype=torch.float32, device=self.device)
         p = _cabi.ptr
         _cabi.check(entry(C.byref(self.net), p(params), p(m), p(v), p(t), p(jobs_dev), int(n_jobs), int(max_windows), p(x), p(y), C.byref(hp),
-                          p(ws), p(hist), p(acc), code, *opt, _stream_ptr()))
-        return hist[:, :epochs], acc[:, :epochs], (m, v, t)
+                          p(ws), p(hist), p(acc), _cabi.loss_code(loss), None if opt is None else C.byref(opt),
+                          None if stop is None else stop.ctypes.data_as(C.c_void_p), p(best), p(epochs_run), p(best_epoch), _stream_ptr()))
+        return hist[:, :epochs], acc[:, :epochs], epochs_run, best_epoch, (m, v, t)
 
     @property
     def tc_supported(self) -> bool:

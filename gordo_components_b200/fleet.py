@@ -305,27 +305,21 @@ def _keras_initial_params(eng: "engine.FFEngine", n_slots: int, generator):
 def _fit_slots(eng, params, fit_jobs, n_jobs, max_rows, x, y, split, row_map, n_machines, epochs, batch_size, shuffle, adam, seed,
                validation_batch_size, early_stopping, loss="mse", optimizer=None):
     """
-    The one fit launch of a bucket (job j trains a slot of machine j mod n_machines): gb_ffae_fit without held-out positions or a
-    row map, gb_ffae_fit_split with them, gb_ffae_fit_stop with an EarlyStopping callback (one for all machines or one per machine).
-    Returns (loss, acc, val_loss, val_acc, epochs_run, best_epoch); the last four None where the launch has none.
+    The one fit launch of a bucket (job j trains a slot of machine j mod n_machines), with held-out positions and a row map where
+    ``split`` is given and an EarlyStopping callback (one for all machines or one per machine) where ``early_stopping`` is.
+    Returns (loss, acc, val_loss, val_acc, epochs_run, best_epoch): val_* rows NaN for jobs without held-out positions,
+    epochs_run / best_epoch None without a callback.
     """
-    val_loss = val_acc = epochs_run = best_epoch = None
-    vb = validation_batch_size or batch_size
+    stop = None
     if early_stopping is not None:
         per_machine = list(early_stopping) if isinstance(early_stopping, (list, tuple)) else [early_stopping] * n_machines
         if len(per_machine) != n_machines:
             raise ValueError(f"early_stopping: {len(per_machine)} callbacks for {n_machines} machines")
         stop = engine.make_stop([per_machine[j % n_machines] for j in range(n_jobs)])
-        hist, acc, val_loss, val_acc, epochs_run, best_epoch, _ = eng.fit_split(
-            params, fit_jobs, n_jobs, max_rows, x, y, split=split, row_map=row_map, val_batch=vb, epochs=epochs, batch_size=batch_size,
-            shuffle=shuffle, adam=adam, seed=seed, stop=stop, loss=loss, optimizer=optimizer)
-    elif split is None:
-        hist, acc, _ = eng.fit(params, fit_jobs, n_jobs, max_rows, x, y, epochs=epochs, batch_size=batch_size, shuffle=shuffle, adam=adam, seed=seed,
-                               loss=loss, optimizer=optimizer)
-    else:
-        hist, acc, val_loss, val_acc, _ = eng.fit_split(params, fit_jobs, n_jobs, max_rows, x, y, split=split, row_map=row_map, val_batch=vb,
-                                                        epochs=epochs, batch_size=batch_size, shuffle=shuffle, adam=adam, seed=seed, loss=loss,
-                                                        optimizer=optimizer)
+    hist, acc, val_loss, val_acc, *ran, _ = eng.fit_split(
+        params, fit_jobs, n_jobs, max_rows, x, y, split=split, row_map=row_map, val_batch=validation_batch_size or batch_size, epochs=epochs,
+        batch_size=batch_size, shuffle=shuffle, adam=adam, seed=seed, stop=stop, loss=loss, optimizer=optimizer)
+    epochs_run, best_epoch = ran or (None, None)
     return hist, acc, val_loss, val_acc, epochs_run, best_epoch
 
 
