@@ -16,43 +16,40 @@ namespace {
 constexpr int SM_THREADS = 64;
 constexpr int SM_CHUNK = 128;  // rows per work item of the rolling kernels
 
-__global__ void __launch_bounds__(SM_THREADS) smooth_sma_kernel(const gb_job* jobs, int job0, const float* arr, int n_cols, int window, float* out) {
-  const gb_job job = jobs[job0 + blockIdx.y];
-  const int j = blockIdx.x * SM_THREADS + threadIdx.x;
-  const int t0 = blockIdx.z * SM_CHUNK;
-  if (j >= n_cols || t0 >= job.n_rows) return;
-  const int t1 = min(job.n_rows, t0 + SM_CHUNK);
-  const float* src = arr + job.out_row * (long)n_cols + j;
-  float* dst = out + job.out_row * (long)n_cols + j;
+// One column of one job, rows [t0, t1) (the rolling methods) or all of them (ewma): src / dst point at the job's first row of the
+// column, element t at src[t * stride].  The kernels below only decide which column a thread owns; gb_smooth and gb_smooth_scores
+// share these bodies, so a column comes out with the same bits from either.  In is float or double; a double is rounded to float
+// as it is read, exactly the float32 array the host would have passed.
+template <typename In>
+__device__ __forceinline__ float load_f32(const In* p) { return (float)*p; }
+
+template <typename In>
+__device__ __forceinline__ void sma_column(const In* src, long stride, float* dst, long dstride, int t0, int t1, int window) {
   double sum = 0.0;
   int bad = 0;  // NaNs currently inside the window
   for (int t = max(0, t0 - window); t < t0; ++t) {  // window state as the row before the chunk left it: rows [t0 - window, t0)
-    const float v = src[(long)t * n_cols];
+    const float v = load_f32(src + t * stride);
     if (v == v) sum += (double)v; else ++bad;
   }
   for (int t = t0; t < t1; ++t) {
-    const float v = src[(long)t * n_cols];
+    const float v = load_f32(src + t * stride);
     if (v == v) sum += (double)v; else ++bad;
     if (t >= window) {
-      const float old = src[(long)(t - window) * n_cols];
+      const float old = load_f32(src + (t - window) * stride);
       if (old == old) sum -= (double)old; else --bad;
     }
-    dst[(long)t * n_cols] = (t >= window - 1 && bad == 0) ? (float)(sum / (double)window) : CUDART_NAN_F;
+    dst[t * dstride] = (t >= window - 1 && bad == 0) ? (float)(sum / (double)window) : CUDART_NAN_F;
   }
 }
 
 // pandas/_libs/window/aggregations.pyx ewm() [3P, pandas 1.5.3 pinned by the reference], adjust=True, ignore_na=False, minp=1
-__global__ void __launch_bounds__(SM_THREADS) smooth_ewma_kernel(const gb_job* jobs, int job0, const float* arr, int n_cols, int window, float* out) {
-  const gb_job job = jobs[job0 + blockIdx.y];
-  const int j = blockIdx.x * SM_THREADS + threadIdx.x;
-  if (j >= n_cols || job.n_rows <= 0) return;
-  const float* src = arr + job.out_row * (long)n_cols + j;
-  float* dst = out + job.out_row * (long)n_cols + j;
+template <typename In>
+__device__ __forceinline__ void ewma_column(const In* src, long stride, float* dst, long dstride, int n_rows, int window) {
   const double alpha = 2.0 / ((double)window + 1.0), old_wt_factor = 1.0 - alpha, new_wt = 1.0;
-  double weighted = (double)src[0], old_wt = 1.0;
+  double weighted = (double)load_f32(src), old_wt = 1.0;
   dst[0] = (float)weighted;  // NaN when the first value is NaN
-  for (int t = 1; t < job.n_rows; ++t) {
-    const double cur = (double)src[(long)t * n_cols];
+  for (int t = 1; t < n_rows; ++t) {
+    const double cur = (double)load_f32(src + t * stride);
     const bool is_obs = cur == cur;
     if (weighted == weighted) {
       old_wt *= old_wt_factor;  // ignore_na=False: a missing value still ages the weights
@@ -63,22 +60,15 @@ __global__ void __launch_bounds__(SM_THREADS) smooth_ewma_kernel(const gb_job* j
     } else if (is_obs) {
       weighted = cur;
     }
-    dst[(long)t * n_cols] = (float)weighted;
+    dst[t * dstride] = (float)weighted;
   }
 }
 
-// rolling median: sorted window of the non-NaN values per thread in shared memory, [window][nthreads] so lanes hit different banks
-__global__ void __launch_bounds__(SM_THREADS) smooth_median_kernel(const gb_job* jobs, int job0, const float* arr, int n_cols, int window, float* out) {
-  extern __shared__ float s_win[];
-  const int nthr = blockDim.x;
-  const gb_job job = jobs[job0 + blockIdx.y];
-  const int j = blockIdx.x * nthr + threadIdx.x;
-  const int t0 = blockIdx.z * SM_CHUNK;
-  if (j >= n_cols || t0 >= job.n_rows) return;
-  const int t1 = min(job.n_rows, t0 + SM_CHUNK);
-  float* win = s_win + threadIdx.x;  // element i at win[i * nthr]
-  const float* src = arr + job.out_row * (long)n_cols + j;
-  float* dst = out + job.out_row * (long)n_cols + j;
+// rolling median: sorted window of the non-NaN values, element i at win[i * nthr] (a [window][nthreads] shared array, so the lanes
+// of a warp hit different banks)
+template <typename In>
+__device__ __forceinline__ void median_column(const In* src, long stride, float* dst, long dstride, int t0, int t1, int window, float* win,
+                                              int nthr) {
   int count = 0, bad = 0;  // sorted values held / NaNs currently inside the window
   auto insert = [&](float v) {
     if (!(v == v)) { ++bad; return; }
@@ -100,17 +90,80 @@ __global__ void __launch_bounds__(SM_THREADS) smooth_median_kernel(const gb_job*
     for (int i = lo; i + 1 < count; ++i) win[i * nthr] = win[(i + 1) * nthr];
     --count;
   };
-  for (int t = max(0, t0 - window); t < t0; ++t) insert(src[(long)t * n_cols]);  // window state as the row before the chunk left it
+  for (int t = max(0, t0 - window); t < t0; ++t) insert(load_f32(src + t * stride));  // window state as the row before the chunk left it
   for (int t = t0; t < t1; ++t) {
-    if (t >= window) remove(src[(long)(t - window) * n_cols]);
-    insert(src[(long)t * n_cols]);
+    if (t >= window) remove(load_f32(src + (t - window) * stride));
+    insert(load_f32(src + t * stride));
     float m = CUDART_NAN_F;
     if (t >= window - 1 && bad == 0) {  // count == window
       const int h = window >> 1;
       m = (window & 1) ? win[h * nthr] : 0.5f * (win[(h - 1) * nthr] + win[h * nthr]);
     }
-    dst[(long)t * n_cols] = m;
+    dst[t * dstride] = m;
   }
+}
+
+__global__ void __launch_bounds__(SM_THREADS) smooth_sma_kernel(const gb_job* jobs, int job0, const float* arr, int n_cols, int window, float* out) {
+  const gb_job job = jobs[job0 + blockIdx.y];
+  const int j = blockIdx.x * SM_THREADS + threadIdx.x;
+  const int t0 = blockIdx.z * SM_CHUNK;
+  if (j >= n_cols || t0 >= job.n_rows) return;
+  sma_column(arr + job.out_row * (long)n_cols + j, n_cols, out + job.out_row * (long)n_cols + j, n_cols, t0, min(job.n_rows, t0 + SM_CHUNK),
+             window);
+}
+
+__global__ void __launch_bounds__(SM_THREADS) smooth_ewma_kernel(const gb_job* jobs, int job0, const float* arr, int n_cols, int window, float* out) {
+  const gb_job job = jobs[job0 + blockIdx.y];
+  const int j = blockIdx.x * SM_THREADS + threadIdx.x;
+  if (j >= n_cols || job.n_rows <= 0) return;
+  ewma_column(arr + job.out_row * (long)n_cols + j, n_cols, out + job.out_row * (long)n_cols + j, n_cols, job.n_rows, window);
+}
+
+__global__ void __launch_bounds__(SM_THREADS) smooth_median_kernel(const gb_job* jobs, int job0, const float* arr, int n_cols, int window, float* out) {
+  extern __shared__ float s_win[];
+  const gb_job job = jobs[job0 + blockIdx.y];
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  const int t0 = blockIdx.z * SM_CHUNK;
+  if (j >= n_cols || t0 >= job.n_rows) return;
+  median_column(arr + job.out_row * (long)n_cols + j, n_cols, out + job.out_row * (long)n_cols + j, n_cols, t0, min(job.n_rows, t0 + SM_CHUNK),
+                window, s_win + threadIdx.x, (int)blockDim.x);
+}
+
+// The four anomaly arrays of a batch as one grid of 2T + 2 columns: [0, T) the columns of tag-anomaly-scaled, [T, 2T) those of
+// tag-anomaly-unscaled, 2T total-anomaly-scaled, 2T + 1 total-anomaly-unscaled.  A thread finds its array and stride and runs the
+// same column body gb_smooth runs, so the per-row arrays fill lanes of the tag arrays' CTAs instead of CTAs of their own.
+struct ScoreArrays {
+  const void* in[4];  // tag scaled, total scaled, tag unscaled, total unscaled
+  float* out[4];
+};
+
+template <typename In>
+__device__ __forceinline__ bool score_column(const ScoreArrays& a, int c, int T, const gb_job& job, const In*& src, float*& dst, long& stride) {
+  if (c >= 2 * T + 2) return false;
+  // selects, not a[i] with a runtime i: an indexed kernel parameter would be copied to local memory first
+  const bool tag = c < 2 * T, scaled = tag ? c < T : c == 2 * T;
+  const void* in = tag ? (scaled ? a.in[0] : a.in[2]) : (scaled ? a.in[1] : a.in[3]);
+  float* out = tag ? (scaled ? a.out[0] : a.out[2]) : (scaled ? a.out[1] : a.out[3]);
+  stride = tag ? T : 1;
+  const long ofs = job.out_row * stride + (tag ? (scaled ? c : c - T) : 0);
+  src = static_cast<const In*>(in) + ofs;
+  dst = out + ofs;
+  return true;
+}
+
+template <typename In, int METHOD>
+__global__ void __launch_bounds__(SM_THREADS) smooth_scores_kernel(const gb_job* jobs, int job0, ScoreArrays a, int T, int window) {
+  extern __shared__ float s_win[];
+  const gb_job job = jobs[job0 + blockIdx.y];
+  const int t0 = blockIdx.z * SM_CHUNK;
+  const In* src;
+  float* dst;
+  long stride;
+  if (t0 >= job.n_rows || !score_column<In>(a, blockIdx.x * blockDim.x + threadIdx.x, T, job, src, dst, stride)) return;
+  const int t1 = min(job.n_rows, t0 + SM_CHUNK);
+  if (METHOD == 0) median_column(src, stride, dst, stride, t0, t1, window, s_win + threadIdx.x, (int)blockDim.x);
+  else if (METHOD == 1) sma_column(src, stride, dst, stride, t0, t1, window);
+  else ewma_column(src, stride, dst, stride, job.n_rows, window);
 }
 
 // x'[r][c] = x[r][c] * a[slot][c] + b[slot][c] in double, rounded once to float: what sklearn's per-feature scalers compute
@@ -249,6 +302,7 @@ constexpr int MAX_GRID_Y = 65535;  // gridDim.y carries the job index: larger fl
 
 }  // namespace
 
+
 extern "C" int gb_quantile(const gb_job* jobs, int32_t n_jobs, int32_t max_rows, const float* arr, int32_t n_cols, float q, float* out,
                            void* stream) {
   GB_REQUIRE(jobs && arr && out, GB_E_ARG, "jobs/arr/out must be non-NULL");
@@ -286,6 +340,40 @@ extern "C" int gb_affine_f64(const gb_job* jobs, int32_t n_jobs, int32_t max_row
   return GB_OK;
 }
 
+namespace {
+
+// Threads per CTA of the rolling median and the shared memory they need: one sorted window per thread, so wide windows run
+// fewer columns per CTA.  false when even one thread's window does not fit.
+constexpr size_t MEDIAN_SMEM_MAX = 200 * 1024;
+bool median_block(int window, int& nthr, size_t& smem) {
+  nthr = SM_THREADS;
+  while (nthr > 1 && (size_t)window * nthr * sizeof(float) > MEDIAN_SMEM_MAX) nthr >>= 1;
+  smem = (size_t)window * nthr * sizeof(float);
+  return smem <= MEDIAN_SMEM_MAX;
+}
+
+template <typename In>
+int launch_smooth_scores(const gb_job* jobs, int n_jobs, int max_rows, const ScoreArrays& a, int T, int window, int method, cudaStream_t st) {
+  const int chunks = (max_rows + SM_CHUNK - 1) / SM_CHUNK;
+  const int n_cols = 2 * T + 2;
+  int nthr = SM_THREADS;
+  size_t smem = 0;
+  if (method == 0) {
+    median_block(window, nthr, smem);
+    GB_CUDA_CHECK(cudaFuncSetAttribute(smooth_scores_kernel<In, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  }
+  for (int j0 = 0; j0 < n_jobs; j0 += MAX_GRID_Y) {
+    const int nj = n_jobs - j0 < MAX_GRID_Y ? n_jobs - j0 : MAX_GRID_Y;
+    if (method == 0) smooth_scores_kernel<In, 0><<<dim3((n_cols + nthr - 1) / nthr, nj, chunks), nthr, smem, st>>>(jobs, j0, a, T, window);
+    else if (method == 1) smooth_scores_kernel<In, 1><<<dim3((n_cols + SM_THREADS - 1) / SM_THREADS, nj, chunks), SM_THREADS, 0, st>>>(jobs, j0, a, T, window);
+    else smooth_scores_kernel<In, 2><<<dim3((n_cols + SM_THREADS - 1) / SM_THREADS, nj), SM_THREADS, 0, st>>>(jobs, j0, a, T, window);
+  }
+  GB_CUDA_CHECK(cudaGetLastError());
+  return GB_OK;
+}
+
+}  // namespace
+
 extern "C" int gb_smooth(const gb_job* jobs, int32_t n_jobs, int32_t max_rows, const float* arr, int32_t n_cols, int32_t window, int32_t method,
                          float* out, void* stream) {
   GB_REQUIRE(jobs && arr && out, GB_E_ARG, "jobs/arr/out must be non-NULL");
@@ -299,9 +387,8 @@ extern "C" int gb_smooth(const gb_job* jobs, int32_t n_jobs, int32_t max_rows, c
   int nthr = SM_THREADS;
   size_t smem = 0;
   if (method == 0) {
-    while (nthr > 1 && (size_t)window * nthr * sizeof(float) > 200 * 1024) nthr >>= 1;  // wide windows: fewer columns per CTA
-    smem = (size_t)window * nthr * sizeof(float);
-    GB_REQUIRE(smem <= 200 * 1024, GB_E_SMEM, "rolling-median window %d exceeds the %d values one thread's sorted window may hold", window, 200 * 1024 / 4);
+    GB_REQUIRE(median_block(window, nthr, smem), GB_E_SMEM, "rolling-median window %d exceeds the %d values one thread's sorted window may hold",
+               window, (int)(MEDIAN_SMEM_MAX / sizeof(float)));
     GB_CUDA_CHECK(cudaFuncSetAttribute(smooth_median_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   }
   for (int j0 = 0; j0 < n_jobs; j0 += MAX_GRID_Y) {
@@ -312,4 +399,29 @@ extern "C" int gb_smooth(const gb_job* jobs, int32_t n_jobs, int32_t max_rows, c
   }
   GB_CUDA_CHECK(cudaGetLastError());
   return GB_OK;
+}
+
+extern "C" int gb_smooth_scores(const gb_job* jobs, int32_t n_jobs, int32_t max_rows, const void* tag_scaled, const void* total_scaled,
+                                const void* tag_unscaled, const void* total_unscaled, int32_t in_f64, int32_t n_tags, int32_t window, int32_t method,
+                                float* smooth_tag_scaled, float* smooth_total_scaled, float* smooth_tag_unscaled, float* smooth_total_unscaled,
+                                void* stream) {
+  GB_REQUIRE(jobs && tag_scaled && total_scaled && tag_unscaled && total_unscaled, GB_E_ARG, "jobs and the four score arrays must be non-NULL");
+  GB_REQUIRE(smooth_tag_scaled && smooth_total_scaled && smooth_tag_unscaled && smooth_total_unscaled, GB_E_ARG,
+             "the four smoothed outputs must be non-NULL");
+  GB_REQUIRE(in_f64 == 0 || in_f64 == 1, GB_E_ARG, "in_f64=%d must be 0 (float32 scores) or 1 (float64)", in_f64);
+  GB_REQUIRE(n_tags >= 1 && n_tags <= (1 << 24), GB_E_ARG, "n_tags=%d must be in [1, %d]", n_tags, 1 << 24);
+  GB_REQUIRE(window >= 1, GB_E_ARG, "window=%d must be >= 1", window);
+  GB_REQUIRE(method >= 0 && method <= 2, GB_E_ARG, "method=%d unknown (0 smm, 1 sma, 2 ewma)", method);
+  GB_REQUIRE(n_jobs >= 0 && max_rows >= 0, GB_E_ARG, "bad n_jobs / max_rows");
+  GB_REQUIRE((max_rows + SM_CHUNK - 1) / SM_CHUNK <= 65535, GB_E_ARG, "smoothing handles at most %d rows per job", 65535 * SM_CHUNK);
+  int nthr;
+  size_t smem;
+  GB_REQUIRE(method != 0 || median_block(window, nthr, smem), GB_E_SMEM,
+             "rolling-median window %d exceeds the %d values one thread's sorted window may hold", window, (int)(MEDIAN_SMEM_MAX / sizeof(float)));
+  if (n_jobs == 0 || max_rows == 0) return GB_OK;
+  const ScoreArrays a{{tag_scaled, total_scaled, tag_unscaled, total_unscaled},
+                      {smooth_tag_scaled, smooth_total_scaled, smooth_tag_unscaled, smooth_total_unscaled}};
+  cudaStream_t st = (cudaStream_t)stream;
+  return in_f64 ? launch_smooth_scores<double>(jobs, n_jobs, max_rows, a, n_tags, window, method, st)
+                : launch_smooth_scores<float>(jobs, n_jobs, max_rows, a, n_tags, window, method, st);
 }

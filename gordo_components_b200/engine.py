@@ -516,6 +516,33 @@ def smooth(jobs_dev, n_jobs, arr, window: int, method: str, max_rows: Optional[i
     return out
 
 
+SMOOTH_SCORE_KEYS = ("tag-anomaly-scaled", "total-anomaly-scaled", "tag-anomaly-unscaled", "total-anomaly-unscaled")
+
+
+def smooth_scores(jobs_dev, n_jobs, max_rows, scores, window: int, method: str):
+    """
+    ``smooth`` of the four anomaly arrays of every job in one launch (gb_smooth_scores): ``scores`` holds the SMOOTH_SCORE_KEYS
+    arrays ([rows, tags] / [rows], all float32 or all float64; float64 is rounded to float32 as it is read).  Returns
+    ``{"smooth-<key>": float32 tensor of the same shape}``; rows outside every job are NaN.
+    """
+    torch = _torch()
+    lib = _cabi.load_library()
+    if method not in SMOOTH_METHODS:
+        raise ValueError(f"smoothing_method {method!r} must be one of {sorted(SMOOTH_METHODS)}")
+    ins = [scores[k] for k in SMOOTH_SCORE_KEYS]
+    dtype = ins[0].dtype
+    if dtype not in (torch.float32, torch.float64) or any(t.dtype != dtype for t in ins):
+        raise ValueError(f"smooth_scores takes four float32 or four float64 arrays, got {[t.dtype for t in ins]}")
+    rows, n_tags = ins[0].shape
+    if ins[2].shape != (rows, n_tags) or ins[1].shape != (rows,) or ins[3].shape != (rows,):
+        raise ValueError(f"smooth_scores: score arrays of shapes {[tuple(t.shape) for t in ins]} are not [rows, tags] / [rows]")
+    out = {"smooth-" + k: torch.full(t.shape, float("nan"), dtype=torch.float32, device=t.device) for k, t in zip(SMOOTH_SCORE_KEYS, ins)}
+    p = _cabi.ptr
+    _cabi.check(lib.gb_smooth_scores(p(jobs_dev), int(n_jobs), int(max_rows), *(p(t) for t in ins), int(dtype == torch.float64), int(n_tags),
+                                     int(window), SMOOTH_METHODS[method], *(p(out["smooth-" + k]) for k in SMOOTH_SCORE_KEYS), _stream_ptr()))
+    return out
+
+
 class LSTMEngine:
     """All machines of one LSTM-stack architecture."""
 

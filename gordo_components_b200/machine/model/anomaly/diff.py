@@ -411,10 +411,11 @@ class DiffBasedAnomalyDetector(AnomalyDetectorBase):
         """
         return model_utils.frame_from_blocks(*self.anomaly_blocks(X, y, frequency))
 
-    def anomaly_blocks(self, X: pd.DataFrame, y: pd.DataFrame, frequency: Optional[timedelta] = None):
+    def anomaly_blocks(self, X: pd.DataFrame, y: pd.DataFrame, frequency: Optional[timedelta] = None, smooth: bool = True):
         """
         The anomaly frame before it becomes a DataFrame: ``(row index, [column blocks], [(top, sub) column names])``.  A caller that
-        only serialises the result (``server.anomaly_prediction``) reads the blocks directly and skips the frame.
+        only serialises the result (``server.anomaly_prediction``) reads the blocks directly and skips the frame.  ``smooth=False``
+        leaves out the ``smooth-*`` blocks (and the work behind them), for a reply that drops them anyway.
         """
         if not hasattr(X, "values"):
             raise ValueError("Unable to find X.values property")
@@ -424,15 +425,19 @@ class DiffBasedAnomalyDetector(AnomalyDetectorBase):
                 f"to calculate these thresholds before calling `.anomaly`"
             )
         feat_thr, agg_thr = self._thresholds()
-        return self.blocks_from_scores(self._score(self, X, y, self.scaler, feat_thr, agg_thr), X, y, frequency)
+        return self.blocks_from_scores(self._score(self, X, y, self.scaler, feat_thr, agg_thr), X, y, frequency, smooth=smooth)
 
     def _thresholds(self):
         feat_thr = self.feature_thresholds_.values if getattr(self, "feature_thresholds_", None) is not None else None
         agg_thr = self.aggregate_threshold_ if getattr(self, "aggregate_threshold_", None) is not None else None
         return feat_thr, agg_thr
 
-    def blocks_from_scores(self, res: Dict[str, np.ndarray], X, y, frequency: Optional[timedelta] = None):
-        """``anomaly_blocks`` for score arrays that already exist (``res`` as ``_score`` returns it, e.g. out of a request coalescer)."""
+    def blocks_from_scores(self, res: Dict[str, np.ndarray], X, y, frequency: Optional[timedelta] = None, smooth: bool = True):
+        """
+        ``anomaly_blocks`` for score arrays that already exist (``res`` as ``_score`` returns it, e.g. out of a request coalescer).
+        ``smooth-*`` arrays already in ``res`` (a coalescer's smoothing launch) are used as they are; the caller makes sure they were
+        smoothed from the same totals, i.e. that no row's total is recomputed here (a target holding NaN).
+        """
         feat_thr, agg_thr = self._thresholds()
         res = dict(res)
         # rows with a missing target tag: pandas' totals, and the total confidence from them, before anything is smoothed
@@ -470,10 +475,11 @@ class DiffBasedAnomalyDetector(AnomalyDetectorBase):
         add("total-anomaly-scaled", False)
         add("tag-anomaly-unscaled", True)
         add("total-anomaly-unscaled", False)
-        if self.window is not None and self.smoothing_method is not None:
+        if smooth and self.window is not None and self.smoothing_method is not None:
             for name, per_tag in (("tag-anomaly-scaled", True), ("total-anomaly-scaled", False), ("tag-anomaly-unscaled", True),
                                   ("total-anomaly-unscaled", False)):
-                res["smooth-" + name] = self._smoothing(res[name])
+                if "smooth-" + name not in res:
+                    res["smooth-" + name] = self._smoothing(res[name])
                 add("smooth-" + name, per_tag)
         if feat_thr is not None:
             add("anomaly-confidence", True)

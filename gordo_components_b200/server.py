@@ -244,7 +244,7 @@ class ResidentBucket:
     The models of a store that share one feed-forward architecture, served through ONE ``serving.AnomalyCoalescer``: their weights,
     scaler slopes and thresholds sit packed on the device, and whatever requests are waiting -- from any thread, for any of the
     models -- become one fused launch.  Eligible: this package's ``DiffBasedAnomalyDetector`` around a bare ``KerasAutoEncoder``
-    (no smoothing window, an affine error scaler); pass ``bucket=`` to ``anomaly_prediction`` and every eligible model is answered
+    (an affine error scaler, no smoothing window unless ``smoothing=True``); pass ``bucket=`` to ``anomaly_prediction`` and every eligible model is answered
     through it, the rest as before.  The replies are the same bytes either way (rows are independent in the kernel).
 
     ``input_scalers=True`` also admits the definition the reference's examples deploy, a ``Pipeline`` of per-feature scalers
@@ -256,28 +256,30 @@ class ResidentBucket:
     ``KerasLSTMAutoEncoder`` or ``KerasLSTMForecast``, bare or as the last step of a ``Pipeline``, on a stack the tensor-core LSTM
     kernel runs (tanh and sigmoid cells).  The Pipeline's leading steps run on the host as ``Pipeline.predict`` runs them; autoencoder
     and forecast models of one architecture share a bucket (the lookahead only decides which rows of y a request stages).
+
+    ``smoothing=True`` (with either of the above) also admits detectors with a smoothing window -- ``DiffBasedAnomalyDetector`` with
+    ``window`` and ``DiffBasedKFCVAnomalyDetector``, the reference's production definition (``window=144``, smm) -- whose ``window``
+    is a positive int and whose ``smoothing_method`` is smm, sma or ewma (a median window of at most ``serving.SMM_MAX_WINDOW``).
+    Models are grouped by window and method as well, and windowed and unwindowed models never share a bucket.  A reply that carries
+    the ``smooth-*`` columns (``all_columns=True``) gets them from one smoothing launch over the batch's requests that asked; a
+    request whose y holds a NaN and that asks for them is answered per request, where pandas' totals of those rows are recomputed
+    on the host before they are smoothed.
     """
 
     input_scalers = False  # the bucket holds Pipeline models (set by the constructor)
     lstm = False  # the bucket holds LSTM models (set by the constructor)
+    smoothing = None  # (window, method) of the bucket's windowed detectors (set by the constructor)
 
     def __init__(self, store: "ModelStore", names: Optional[List[str]] = None, input_scalers: bool = False, lstm: bool = False,
-                 **coalescer_kwargs):
+                 smoothing: bool = False, **coalescer_kwargs):
         from . import engine
         from .machine.model.anomaly.diff import _compose_affine, _scaler_multiplier
         from .serving import AnomalyCoalescer
 
         if lstm:
-            self._init_lstm(store, names, coalescer_kwargs)
+            self._init_lstm(store, names, smoothing, coalescer_kwargs)
             return
-        groups: Dict[Any, List[str]] = {}
-        for name in names if names is not None else store.names():
-            model = store.model(name)
-            if self.eligible(model, input_scalers):
-                pre, ae = _served_parts(model)
-                spec = ae.model.spec
-                has_thr = tuple(t is not None for t in model._thresholds())
-                groups.setdefault((tuple(spec.dims), tuple(spec.acts), tuple(spec.l1), has_thr, bool(pre)), []).append(name)
+        groups = self.ff_groups({name: store.model(name) for name in (names if names is not None else store.names())}, input_scalers, smoothing)
         if not groups:
             raise ValueError("no model in the store can be served through a coalescer")
         self.names = max(groups.values(), key=len)  # the largest architecture group
@@ -297,14 +299,15 @@ class ResidentBucket:
         if self.input_scalers:
             a, b = zip(*(_compose_affine(pre, eng.n_in) for pre, _ in parts))
             coalescer_kwargs.update(x_scale=to_dev(a, np.float64), x_offset=to_dev(b, np.float64))
-        self.coalescer = AnomalyCoalescer(eng, params, scale, feat_thr, agg_thr, **coalescer_kwargs)
+        self.smoothing = _smoothing_of(models[0])
+        self.coalescer = AnomalyCoalescer(eng, params, scale, feat_thr, agg_thr, smoothing=self.smoothing, **coalescer_kwargs)
 
-    def _init_lstm(self, store: "ModelStore", names: Optional[List[str]], coalescer_kwargs):
+    def _init_lstm(self, store: "ModelStore", names: Optional[List[str]], smoothing: bool, coalescer_kwargs):
         from . import engine
         from .machine.model.anomaly.diff import _scaler_multiplier
         from .serving import LSTMAnomalyCoalescer
 
-        groups = self.lstm_groups({name: store.model(name) for name in (names if names is not None else store.names())})
+        groups = self.lstm_groups({name: store.model(name) for name in (names if names is not None else store.names())}, smoothing)
         if not groups:
             raise ValueError("no LSTM model in the store can be served through a coalescer")
         self.lstm = True
@@ -320,27 +323,41 @@ class ResidentBucket:
         feat, agg = zip(*(m._thresholds() for m in models))
         feat_thr = to_dev([np.asarray(f, dtype=np.float64) for f in feat]) if feat[0] is not None else None
         agg_thr = to_dev([np.float64(a) for a in agg]) if agg[0] is not None else None
-        self.coalescer = LSTMAnomalyCoalescer(eng, params, scale, feat_thr, agg_thr, **coalescer_kwargs)
+        self.smoothing = _smoothing_of(models[0])
+        self.coalescer = LSTMAnomalyCoalescer(eng, params, scale, feat_thr, agg_thr, smoothing=self.smoothing, **coalescer_kwargs)
 
     @classmethod
-    def lstm_groups(cls, models: Dict[str, Any]) -> Dict[Any, List[str]]:
-        """The eligible LSTM detectors of ``models`` (name -> model) by (architecture, which thresholds are present)."""
+    def ff_groups(cls, models: Dict[str, Any], input_scalers: bool = False, smoothing: bool = False) -> Dict[Any, List[str]]:
+        """The eligible feed-forward detectors of ``models`` (name -> model) by (architecture, which thresholds are present, bare or
+        Pipeline, smoothing)."""
         groups: Dict[Any, List[str]] = {}
         for name, model in models.items():
-            if cls.eligible_lstm(model):
+            if cls.eligible(model, input_scalers, smoothing):
+                pre, ae = _served_parts(model)
+                spec = ae.model.spec
+                has_thr = tuple(t is not None for t in model._thresholds())
+                groups.setdefault((tuple(spec.dims), tuple(spec.acts), tuple(spec.l1), has_thr, bool(pre), _smoothing_of(model)), []).append(name)
+        return groups
+
+    @classmethod
+    def lstm_groups(cls, models: Dict[str, Any], smoothing: bool = False) -> Dict[Any, List[str]]:
+        """The eligible LSTM detectors of ``models`` (name -> model) by (architecture, which thresholds are present, smoothing)."""
+        groups: Dict[Any, List[str]] = {}
+        for name, model in models.items():
+            if cls.eligible_lstm(model, smoothing):
                 spec = _served_lstm_parts(model)[1].model.spec
-                groups.setdefault((spec.key(), tuple(t is not None for t in model._thresholds())), []).append(name)
+                groups.setdefault((spec.key(), tuple(t is not None for t in model._thresholds()), _smoothing_of(model)), []).append(name)
         return groups
 
     @staticmethod
-    def eligible_lstm(model) -> bool:
-        """True for a detector ``ResidentBucket(lstm=True)`` serves (no device needed)."""
+    def eligible_lstm(model, smoothing: bool = False) -> bool:
+        """True for a detector ``ResidentBucket(lstm=True, smoothing=smoothing)`` serves (no device needed)."""
         import ctypes as C
 
         from . import _cabi
         from .machine.model.anomaly.diff import _scaler_multiplier
 
-        if not (_frame_is_from_blocks(model) and model.window is None
+        if not (_frame_is_from_blocks(model) and _window_served(model, smoothing)
                 and not (model.require_thresholds and all(t is None for t in model._thresholds()))):
             return False
         parts = _served_lstm_parts(model)
@@ -357,8 +374,8 @@ class ResidentBucket:
         return True
 
     @staticmethod
-    def eligible(model, input_scalers: bool = False) -> bool:
-        if not (_frame_is_from_blocks(model) and model.window is None
+    def eligible(model, input_scalers: bool = False, smoothing: bool = False) -> bool:
+        if not (_frame_is_from_blocks(model) and _window_served(model, smoothing)
                 and not (model.require_thresholds and all(t is None for t in model._thresholds()))):
             return False
         parts = _served_parts(model)
@@ -375,24 +392,34 @@ class ResidentBucket:
             return False
         return True
 
-    def anomaly_blocks(self, store: "ModelStore", name: str, X: pd.DataFrame, y: pd.DataFrame, frequency=None):
+    def anomaly_blocks(self, store: "ModelStore", name: str, X: pd.DataFrame, y: pd.DataFrame, frequency=None, smooth: bool = True):
+        """``model.anomaly_blocks(X, y, frequency, smooth)`` of the bucket's model ``name``, through the coalescer."""
         from .machine.model.anomaly.diff import _has_inf, _refuse_infinity, _values
 
         model = store.model(name)
         _refuse_infinity(_values(y))
+        smooth = smooth and self.smoothing is not None
+        if smooth and np.isnan(np.asarray(_values(y), dtype=np.float64)).any():
+            # the rows of a missing target get pandas' totals on the host, and those are what is smoothed: this request goes on its own
+            return model.anomaly_blocks(X, y, frequency=frequency, smooth=True)
         if self.lstm:
-            return self._lstm_anomaly_blocks(name, model, X, y, frequency)
+            return self._lstm_anomaly_blocks(name, model, X, y, frequency, smooth)
         if self.input_scalers:
             # what the Pipeline's sklearn steps raise, as the per-request route does before any launch
             _refuse_infinity(np.ascontiguousarray(_values(X), dtype=np.float64))
         elif _has_inf(_values(X)):
             # the coalescer's launch may run the tensor-core kernel, which does not take ±inf inputs: this request goes on its own
-            return model.anomaly_blocks(X, y, frequency=frequency)
-        scores = self.coalescer.anomaly(self.slot[name], X, y)
+            return model.anomaly_blocks(X, y, frequency=frequency, smooth=smooth)
+        scores = self._scores(name, X, y, smooth)
         _refuse_infinity(scores["model-output"])
-        return model.blocks_from_scores(scores, X, y, frequency)
+        return model.blocks_from_scores(scores, X, y, frequency, smooth=smooth)
 
-    def _lstm_anomaly_blocks(self, name: str, model, X: pd.DataFrame, y: pd.DataFrame, frequency):
+    def _scores(self, name: str, X, y, smooth: bool):
+        """The coalescer's result for one request; ``smooth`` is only passed when set, the call of a bucket without smoothing stays
+        ``anomaly(slot, X, y)``."""
+        return self.coalescer.anomaly(self.slot[name], X, y, smooth=True) if smooth else self.coalescer.anomaly(self.slot[name], X, y)
+
+    def _lstm_anomaly_blocks(self, name: str, model, X: pd.DataFrame, y: pd.DataFrame, frequency, smooth: bool):
         """What ``model.anomaly_blocks`` computes, in the order the per-request route raises: the leading steps' transform (which
         refuses ±inf in X), the lookback check; a transformed X holding ±inf goes on its own (the fp32 kernel saturates the gates)."""
         from .machine.model.anomaly.diff import _has_inf, _refuse_infinity, _values
@@ -403,11 +430,11 @@ class ResidentBucket:
             Xt = step.transform(Xt)
         Xv = net._validate_and_fix_size_of_X(np.asarray(_values(Xt)))
         if _has_inf(Xv):
-            return model.anomaly_blocks(X, y, frequency=frequency)
+            return model.anomaly_blocks(X, y, frequency=frequency, smooth=smooth)
         n = len(Xv) - net.lookback_window + 1 - net.lookahead
-        scores = self.coalescer.anomaly(self.slot[name], Xv, _values(y)[-n:])
+        scores = self._scores(name, Xv, _values(y)[-n:], smooth)
         _refuse_infinity(scores["model-output"])
-        return model.blocks_from_scores(scores, X, y, frequency)
+        return model.blocks_from_scores(scores, X, y, frequency, smooth=smooth)
 
     def close(self):
         self.coalescer.close()
@@ -466,6 +493,27 @@ def _served_lstm_parts(model):
     return None
 
 
+def _smoothing_of(model):
+    """None for a detector without a smoothing window; (window, method) for one whose smoothing the coalescers run (a positive int
+    window, smm / sma / ewma, a median window the kernel holds); False for any other."""
+    from .engine import SMOOTH_METHODS
+    from .serving import SMM_MAX_WINDOW
+
+    window, method = model.window, model.smoothing_method
+    if window is None:
+        return None
+    if isinstance(window, bool) or not isinstance(window, (int, np.integer)) or window < 1 or method not in SMOOTH_METHODS \
+            or (method == "smm" and window > SMM_MAX_WINDOW):
+        return False
+    return int(window), method
+
+
+def _window_served(model, smoothing: bool) -> bool:
+    """True when a bucket built with ``smoothing`` takes the detector's smoothing window (or it has none)."""
+    s = _smoothing_of(model)
+    return s is None or (smoothing and s is not False)
+
+
 def _x64_launch_holds(spec) -> bool:
     """True when the fused launch with float64 x holds this stack on the kernel the per-request route picks (no device needed)."""
     import ctypes as C
@@ -516,10 +564,11 @@ def anomaly_prediction(store: ModelStore, name: str, json: Optional[dict] = None
     try:
         buckets = () if bucket is None else (bucket,) if isinstance(bucket, ResidentBucket) else tuple(bucket)
         holder = next((b for b in buckets if name in b.slot), None)
-        if holder is not None or (fmt != "parquet" and _frame_is_from_blocks(model)):
-            # this package's detectors: straight from the column blocks, no DataFrame in between for JSON
-            blocks = (holder.anomaly_blocks(store, name, X, y, store.frequency(name)) if holder is not None
-                      else model.anomaly_blocks(X, y, frequency=store.frequency(name)))
+        if holder is not None or _frame_is_from_blocks(model):
+            # this package's detectors: straight from the column blocks (no DataFrame in between for JSON), the smoothed ones only
+            # when the reply carries them
+            blocks = (holder.anomaly_blocks(store, name, X, y, store.frequency(name), smooth=all_columns) if holder is not None
+                      else model.anomaly_blocks(X, y, frequency=store.frequency(name), smooth=all_columns))
             if fmt != "parquet":
                 return Reply(200, {"data": blocks_to_dict(*blocks, skip=skip), "time-seconds": f"{timeit.default_timer() - start:.4f}"})
             frame = model_utils.frame_from_blocks(*blocks)

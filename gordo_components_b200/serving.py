@@ -21,6 +21,12 @@ SURVEY §8b).  The per-request results are bit-identical to a per-request launch
 
 ``LSTMAnomalyCoalescer`` does the same for LSTM detectors: the waiting requests become one ragged tensor-core LSTM launch
 sequence (gb_lstm_infer_tc_ragged, each request a job of its own windows) and one float64 scoring launch (gb_anomaly_score_f64).
+
+Either coalescer built with ``smoothing=(window, method)`` (the detectors' ``window`` / ``smoothing_method``) also answers the
+smoothed columns: ``submit(slot, X, y, smooth=True)`` marks a request whose reply carries them, and a batch holding such requests
+runs one more launch (gb_smooth_scores) over exactly their jobs, reading the score arrays the batch's launch left on the device.
+Its results come back with the rest of the batch, before the batch's one synchronisation.  Each request is smoothed on its own
+rows (its windows start at its first row), as ``DiffBasedAnomalyDetector._smoothing`` smooths it on the per-request route.
 """
 from __future__ import annotations
 
@@ -35,10 +41,12 @@ import numpy as np
 from . import engine
 from .fleet import PER_ROW, PER_TAG
 
+SMM_MAX_WINDOW = 200 * 1024 // 4  # the rolling median keeps one thread's sorted window in shared memory (gb_smooth / gb_smooth_scores)
+
 
 class AnomalyCoalescer:
     def __init__(self, eng: "engine.FFEngine", params, scale, feat_thr=None, agg_thr=None, max_batch_rows: int = 1 << 18,
-                 max_wait_ms: float = 1.0, want: Optional[Sequence[str]] = None, x_scale=None, x_offset=None):
+                 max_wait_ms: float = 1.0, want: Optional[Sequence[str]] = None, x_scale=None, x_offset=None, smoothing=None):
         torch = engine._torch()
         self.eng, self.params, self.scale, self.feat_thr, self.agg_thr = eng, params, scale, feat_thr, agg_thr
         if (x_scale is None) != (x_offset is None):
@@ -49,6 +57,7 @@ class AnomalyCoalescer:
         self.max_rows, self.max_wait = int(max_batch_rows), float(max_wait_ms) * 1e-3
         self.want = tuple(want) if want is not None else tuple(
             k for k in PER_TAG + PER_ROW if not ((feat_thr is None and k == "anomaly-confidence") or (agg_thr is None and k == "total-anomaly-confidence")))
+        self.smoothing = self._check_smoothing(smoothing)
         dev = eng.device
         self._stream = torch.cuda.Stream(device=dev)
         self._xh = torch.empty((self.max_rows, eng.n_in), dtype=x_dtype).pin_memory()
@@ -57,11 +66,28 @@ class AnomalyCoalescer:
         self._yd = torch.empty((self.max_rows, eng.n_out), dtype=torch.float32, device=dev)
         self._out_d = {k: torch.empty((self.max_rows, eng.n_out) if k in PER_TAG else (self.max_rows,), dtype=torch.float32, device=dev) for k in self.want}
         self._out_h = {k: torch.empty(v.shape, dtype=torch.float32).pin_memory() for k, v in self._out_d.items()}
-        self._jobs_h = torch.empty((self.max_jobs * engine._cabi.JOB_DTYPE.itemsize,), dtype=torch.uint8).pin_memory()
+        # the batch's jobs, then those of its requests that want the smoothed columns
+        self._jobs_h = torch.empty((2 * self.max_jobs * engine._cabi.JOB_DTYPE.itemsize,), dtype=torch.uint8).pin_memory()
         self.max_cost = self.max_rows
         self._start()
 
     max_jobs = 4096  # requests per batch: the pinned buffer the job records are staged through holds this many
+
+    def _check_smoothing(self, smoothing):
+        """``smoothing`` as (int window, method name), or None; ValueError for anything the smoothing launch does not take."""
+        if smoothing is None:
+            return None
+        window, method = smoothing
+        if isinstance(window, bool) or not isinstance(window, (int, np.integer)) or window < 1:
+            raise ValueError(f"smoothing window {window!r} must be a positive int")
+        if method not in engine.SMOOTH_METHODS:
+            raise ValueError(f"smoothing_method {method!r} must be one of {sorted(engine.SMOOTH_METHODS)}")
+        if method == "smm" and window > SMM_MAX_WINDOW:
+            raise ValueError(f"a rolling-median window of {window} exceeds the {SMM_MAX_WINDOW} values the kernel holds")
+        missing = [k for k in engine.SMOOTH_SCORE_KEYS if k not in self.want]
+        if missing:
+            raise ValueError(f"smoothing needs the score arrays {missing}, which this coalescer does not compute")
+        return int(window), method
 
     def _start(self):
         self._q: "queue.Queue" = queue.Queue()
@@ -72,14 +98,17 @@ class AnomalyCoalescer:
         self._worker.start()
 
     # ------------------------------------------------------------------ client side
-    def submit(self, slot: int, X, y) -> Future:
-        """Queue one request; the Future resolves to {column block: host array} for exactly these rows."""
+    def submit(self, slot: int, X, y, smooth: bool = False) -> Future:
+        """Queue one request; the Future resolves to {column block: host array} for exactly these rows.  ``smooth=True`` adds the
+        four ``smooth-*`` arrays (float32) of a coalescer built with ``smoothing``."""
         if self._closed:
             raise RuntimeError("coalescer is closed")
         if not (0 <= int(slot) < self.params.shape[0]):
             raise ValueError(f"unknown machine slot {slot}")
+        if smooth and self.smoothing is None:
+            raise ValueError("smoothed columns asked of a coalescer built without smoothing")
         fut: Future = Future()
-        self._q.put((int(slot), *self._request(X, y), fut))
+        self._q.put((int(slot), *self._request(X, y), bool(smooth), fut))
         return fut
 
     def _request(self, X, y):
@@ -96,8 +125,8 @@ class AnomalyCoalescer:
         """What a request adds to a batch, against ``max_cost``: its rows."""
         return len(item[1])
 
-    def anomaly(self, slot: int, X, y) -> Dict[str, np.ndarray]:
-        return self.submit(slot, X, y).result()
+    def anomaly(self, slot: int, X, y, smooth: bool = False) -> Dict[str, np.ndarray]:
+        return self.submit(slot, X, y, smooth).result()
 
     def close(self):
         self._closed = True
@@ -135,36 +164,73 @@ class AnomalyCoalescer:
                     if not item[-1].done():
                         item[-1].set_exception(exc)
 
+    def _smoothing_jobs(self, batch, starts, counts):
+        """The job records of the batch's requests that want the smoothed columns, on rows ``[starts[i] - lo, + counts[i])`` of the
+        score arrays' rows ``[lo, hi)``, the span those requests cover; (jobs, lo, hi), or None when no request asked."""
+        sel = np.fromiter((item[-2] for item in batch), dtype=bool, count=len(batch))
+        if not sel.any():
+            return None
+        starts, counts = np.asarray(starts, dtype=np.int64)[sel], np.asarray(counts, dtype=np.int64)[sel]
+        lo, hi = int(starts[0]), int(starts[-1] + counts[-1])
+        return engine.make_jobs(np.zeros(len(starts), dtype=np.int64), counts, starts - lo), lo, hi
+
+    def _smooth(self, torch, jobs_d, jobs, lo, hi, scores):
+        """One gb_smooth_scores launch over ``jobs`` on rows [lo, hi) of the batch's device ``scores``, on the current stream, and
+        the copy of its results into pinned host memory: {"smooth-<key>": host tensor of rows [lo, hi)}."""
+        window, method = self.smoothing
+        if hi == lo:  # only empty requests asked: nothing to launch
+            return {"smooth-" + k: torch.empty((0,) + tuple(scores[k].shape[1:]), dtype=torch.float32) for k in engine.SMOOTH_SCORE_KEYS}
+        res = engine.smooth_scores(jobs_d, len(jobs), int(jobs["n_rows"].max()), {k: scores[k][lo:hi] for k in engine.SMOOTH_SCORE_KEYS},
+                                   window, method)
+        host = {k: torch.empty(v.shape, dtype=v.dtype, pin_memory=True) for k, v in res.items()}
+        for k, v in res.items():
+            host[k].copy_(v, non_blocking=True)
+        return host
+
+    @staticmethod
+    def _with_smoothed(result, item, smoothed, start, n):
+        """``result`` plus the request's rows of the smoothed arrays when it asked for them."""
+        if item[-2]:
+            lo = smoothed[1]
+            result.update({k: v[start - lo:start - lo + n].numpy().copy() for k, v in smoothed[0].items()})
+        return result
+
     def _launch(self, torch, batch, rows):
         jobs = np.empty(len(batch), dtype=engine._cabi.JOB_DTYPE)
         ofs = 0
         xh, yh = self._xh.numpy(), self._yh.numpy()
-        for i, (slot, Xv, yv, _) in enumerate(batch):
+        for i, (slot, Xv, yv, _, _) in enumerate(batch):
             n = len(Xv)
             xh[ofs:ofs + n] = Xv
             yh[ofs:ofs + n] = yv
             jobs[i] = (slot, n, ofs, ofs)
             ofs += n
         max_rows = int(jobs["n_rows"].max()) if len(jobs) else 0
-        jb = self._jobs_h[: jobs.nbytes]
-        jb.numpy()[:] = jobs.view(np.uint8)
+        smooth = self._smoothing_jobs(batch, jobs["out_row"], jobs["n_rows"]) if rows else None
+        staged = jobs if smooth is None else np.concatenate([jobs, smooth[0]])
+        jb = self._jobs_h[: staged.nbytes]
+        jb.numpy()[:] = staged.view(np.uint8)
+        smoothed = None
         with torch.cuda.stream(self._stream):
-            jobs_d = jb.to(self.eng.device, non_blocking=True)
+            jobs_all = jb.to(self.eng.device, non_blocking=True)
+            jobs_d = jobs_all[: jobs.nbytes]
             self._xd[:rows].copy_(self._xh[:rows], non_blocking=True)
             self._yd[:rows].copy_(self._yh[:rows], non_blocking=True)
             if rows:
                 self.eng.infer_score(self.params, jobs_d, len(batch), max_rows, self._xd[:rows], self._yd[:rows], self.scale, self.feat_thr,
                                      self.agg_thr, out_rows=rows, want=self.want, out={k: v[:rows] for k, v in self._out_d.items()},
                                      x_affine=self.x_affine)
+            if smooth is not None:
+                smoothed = (self._smooth(torch, jobs_all[jobs.nbytes:], *smooth, self._out_d), smooth[1])
             for k in self.want:
                 self._out_h[k][:rows].copy_(self._out_d[k][:rows], non_blocking=True)
         self._stream.synchronize()
         self.batches += 1
         self.requests += len(batch)
         ofs = 0
-        for slot, Xv, _, fut in batch:
-            n = len(Xv)
-            fut.set_result({k: self._out_h[k][ofs:ofs + n].numpy().copy() for k in self.want})
+        for item in batch:
+            n = len(item[1])
+            item[-1].set_result(self._with_smoothed({k: self._out_h[k][ofs:ofs + n].numpy().copy() for k in self.want}, item, smoothed, ofs, n))
             ofs += n
 
 
@@ -181,16 +247,18 @@ class LSTMAnomalyCoalescer(AnomalyCoalescer):
     """
 
     def __init__(self, eng: "engine.LSTMEngine", params, scale, feat_thr=None, agg_thr=None, max_batch_tiles: int = 1024,
-                 max_wait_ms: float = 1.0):
+                 max_wait_ms: float = 1.0, smoothing=None):
         torch = engine._torch()
         self.eng, self.params, self.scale, self.feat_thr, self.agg_thr = eng, params, scale, feat_thr, agg_thr
         self.max_cost, self.max_wait = int(max_batch_tiles), float(max_wait_ms) * 1e-3
         self.want = tuple(k for k in PER_TAG + PER_ROW if not ((feat_thr is None and k == "anomaly-confidence")
                                                                 or (agg_thr is None and k == "total-anomaly-confidence")))
+        self.smoothing = self._check_smoothing(smoothing)
         self._stream = torch.cuda.Stream(device=eng.device)
-        # staged per batch in one copy: the infer jobs, the score jobs, tile_base, the distinct slots and the gather job
+        # staged per batch in one copy: the infer jobs, the score jobs, the gather job, the smoothing jobs, tile_base and the
+        # distinct slots
         jb = engine._cabi.JOB_DTYPE.itemsize
-        self._stage_h = torch.empty((2 * self.max_jobs * jb + 2 * (self.max_jobs + 1) * 4 + jb,), dtype=torch.uint8).pin_memory()
+        self._stage_h = torch.empty((3 * self.max_jobs * jb + 2 * (self.max_jobs + 1) * 4 + jb,), dtype=torch.uint8).pin_memory()
         self._start()
 
     def _request(self, X, y):
@@ -226,9 +294,11 @@ class LSTMAnomalyCoalescer(AnomalyCoalescer):
         score_jobs = engine.make_jobs(compact, windows, w_ofs[:-1])  # y and the prediction both at the windows' rows
         tile_base = self.eng.tile_base(windows)
         gather_job = engine.make_jobs([0], [len(uniq)], [0])
+        smooth = self._smoothing_jobs(batch, w_ofs[:-1], windows)
+        smooth_jobs = smooth[0] if smooth is not None else engine.make_jobs([], [], [])
         # job records first: they hold int64 fields and stay 8-byte aligned in the staged buffer
-        parts = [infer_jobs.view(np.uint8), score_jobs.view(np.uint8), gather_job.view(np.uint8), tile_base.view(np.uint8),
-                 uniq.astype(np.int32).view(np.uint8)]
+        parts = [infer_jobs.view(np.uint8), score_jobs.view(np.uint8), gather_job.view(np.uint8), smooth_jobs.view(np.uint8),
+                 tile_base.view(np.uint8), uniq.astype(np.int32).view(np.uint8)]
         sizes = [p.nbytes for p in parts]
         stage = self._stage_h.numpy()
         ofs = np.concatenate([[0], np.cumsum(sizes)])
@@ -237,14 +307,14 @@ class LSTMAnomalyCoalescer(AnomalyCoalescer):
         xh = torch.empty((rows, self.eng.n_features), dtype=torch.float32, pin_memory=True)
         yh = torch.empty((total, self.eng.n_out), dtype=torch.float64, pin_memory=True)
         xn, yn = xh.numpy(), yh.numpy()
-        for i, (_, Xv, yv, _) in enumerate(batch):
+        for i, (_, Xv, yv, _, _) in enumerate(batch):
             xn[x_ofs[i]:x_ofs[i + 1]] = Xv
             yn[w_ofs[i]:w_ofs[i + 1]] = yv
         dev = self.eng.device
         with torch.cuda.stream(self._stream):
             staged = self._stage_h[: int(ofs[-1])].to(dev, non_blocking=True)
             view = [staged[int(ofs[i]):int(ofs[i + 1])] for i in range(len(parts))]
-            jobs_d, score_d, gjob_d, tb_d, map_d = view[0], view[1], view[2], view[3].view(torch.int32), view[4].view(torch.int32)
+            jobs_d, score_d, gjob_d, sjobs_d, tb_d, map_d = view[0], view[1], view[2], view[3], view[4].view(torch.int32), view[5].view(torch.int32)
             xd = xh.to(dev, non_blocking=True)
             yd = yh.to(dev, non_blocking=True)
             gather = lambda t: engine.gather_rows(gjob_d, 1, len(uniq), map_d, t, len(uniq))  # noqa: E731 - the batch's models, compact
@@ -256,6 +326,7 @@ class LSTMAnomalyCoalescer(AnomalyCoalescer):
             res = engine.anomaly_score(score_d, k, int(windows.max()), pred.to(torch.float64), yd, self.eng.n_out, scale, feat_thr, agg_thr,
                                        want=self.want)
             res["model-output"] = pred
+            smoothed = (self._smooth(torch, sjobs_d, *smooth, res), smooth[1]) if smooth is not None else None
             host = {key: torch.empty(v.shape, dtype=v.dtype, pin_memory=True) for key, v in res.items()}
             for key, v in res.items():
                 host[key].copy_(v, non_blocking=True)
@@ -263,4 +334,5 @@ class LSTMAnomalyCoalescer(AnomalyCoalescer):
         self.batches += 1
         self.requests += k
         for i, item in enumerate(batch):
-            item[-1].set_result({key: v[w_ofs[i]:w_ofs[i + 1]].numpy().copy() for key, v in host.items()})
+            result = {key: v[w_ofs[i]:w_ofs[i + 1]].numpy().copy() for key, v in host.items()}
+            item[-1].set_result(self._with_smoothed(result, item, smoothed, int(w_ofs[i]), int(windows[i])))

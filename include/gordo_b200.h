@@ -217,6 +217,16 @@ int gb_cv_moments(const gb_job* jobs, int32_t n_jobs, const float* yhat, const f
 int gb_smooth(const gb_job* jobs, int32_t n_jobs, int32_t max_rows, const float* arr, int32_t n_cols, int32_t window, int32_t method,
               float* out, void* stream);
 
+/* The four smoothed anomaly arrays of a ragged batch of requests in one launch (one per 65 535 jobs): tag_scaled / tag_unscaled
+ * [rows][n_tags] and total_scaled / total_unscaled [rows], float32 (in_f64 = 0) or float64 (in_f64 = 1, each value rounded to
+ * float32 as it is read).  Job i smooths rows [out_row, out_row+n_rows) of each array into the same rows of the float32 output of
+ * the same shape; its windows start at its own first row.  method / window as gb_smooth, the same for every job.  Every column
+ * comes out bit for bit what gb_smooth gives for that array (as float32) alone: both run the same per-column code. */
+int gb_smooth_scores(const gb_job* jobs, int32_t n_jobs, int32_t max_rows, const void* tag_scaled, const void* total_scaled,
+                     const void* tag_unscaled, const void* total_unscaled, int32_t in_f64, int32_t n_tags, int32_t window, int32_t method,
+                     float* smooth_tag_scaled, float* smooth_total_scaled, float* smooth_tag_unscaled, float* smooth_total_unscaled,
+                     void* stream);
+
 /* ---- K9: percentile thresholds of DiffBasedKFCVAnomalyDetector (diff.py:623-635: smoothed validation metric
  * .quantile(threshold_percentile)).  out[job][c] = q-quantile (linear interpolation, NaNs skipped -- pandas
  * semantics) of column c of rows [out_row, out_row+n_rows) of arr [rows][n_cols].  Jobs of up to 32768 rows are sorted in shared
