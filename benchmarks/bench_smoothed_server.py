@@ -10,7 +10,14 @@ in the reference).  Four arms: each route with ``all_columns`` off (the default 
 bytes.  A separate pass times, with CUDA events, the fused launch and the gb_smooth_scores launch of a batch of the size the bucket
 formed in its all-columns arm.
 
-    python benchmarks/bench_smoothed_server.py [--machines 1000] [--requests 400]
+``--ttr`` serves the reference's real production definition instead: the estimator is ``TransformedTargetRegressor(transformer=
+MinMaxScaler, regressor=Pipeline([MinMaxScaler, KerasAutoEncoder]))``, through ``ResidentBucket(store, input_scalers=True,
+smoothing=True, target_scaler=True)`` (prediction-only fused launch, then gb_minmax_inverse_score_f64 and float64 smoothing input).
+Its kernel pass times, with CUDA events, gb_minmax_inverse_score_f64 against gb_minmax_inverse_f32 + gb_anomaly_score_f64 at the
+fold-scoring shape of ``bench_fleet_builder.py --kfcv`` (125 machines x 10 000 rows x 64 tags, 5 folds), for the two outputs the
+builder asks for; algorithmic bytes per 64-tag row are 2 568 for the pair and 1 544 for the single pass.
+
+    python benchmarks/bench_smoothed_server.py [--machines 1000] [--requests 400] [--ttr]
 
 Prints one JSON line (progress goes to stderr).
 """
@@ -28,7 +35,19 @@ def card():
     return {"device": torch.cuda.get_device_name(), "nvidia_smi": q.stdout.strip().splitlines()[:1]}
 
 
-def make_store(root, machines):
+def _production_estimator(ae, rng):
+    """The production definition's fitted TransformedTargetRegressor around ``ae``, without the training."""
+    from sklearn.compose import TransformedTargetRegressor
+    from sklearn.pipeline import Pipeline
+    from sklearn.preprocessing import MinMaxScaler
+
+    reg = Pipeline([("s", MinMaxScaler().fit(rng.random((50, TAGS)) * 10)), ("m", ae)])
+    ttr = TransformedTargetRegressor(transformer=MinMaxScaler(), regressor=reg)
+    ttr._training_dim, ttr.transformer_, ttr.regressor_ = 2, MinMaxScaler().fit(rng.random((50, TAGS)) * 10), reg
+    return ttr
+
+
+def make_store(root, machines, ttr=False):
     import pandas as pd
 
     from gordo_components_b200 import serializer, server
@@ -42,7 +61,7 @@ def make_store(root, machines):
         ae = KerasAutoEncoder(kind="feedforward_hourglass")
         ae.kwargs.update({"n_features": TAGS, "n_features_out": TAGS})
         ae._prepare_model()  # Glorot-initialised weights: the arithmetic of a trained model, without the training
-        det = DiffBasedKFCVAnomalyDetector(base_estimator=ae, window=WINDOW, smoothing_method="smm")
+        det = DiffBasedKFCVAnomalyDetector(base_estimator=_production_estimator(ae, rng) if ttr else ae, window=WINDOW, smoothing_method="smm")
         det.scaler.fit(rng.random((50, TAGS)) * 10)
         det.feature_thresholds_ = pd.Series(rng.random(TAGS) + 0.5, index=tags)
         det.aggregate_threshold_ = float(rng.random() + 0.5)
@@ -132,6 +151,58 @@ def launch_times(torch, bucket, k, rows, reps):
     return res
 
 
+def ttr_kernel_times(torch, reps, machines=125, rows=10_000, folds=5):
+    """Median CUDA-event times (ms) of the K-fold fold scoring of TTR buckets: gb_minmax_inverse_f32 + gb_anomaly_score_f64 against
+    gb_minmax_inverse_score_f64, both asked for tag-anomaly-unscaled and total-anomaly-scaled (what build_kfold_fleet asks for).
+    Outputs are checked bit for bit before timing."""
+    from gordo_components_b200 import engine
+
+    dev = engine.cuda_device()
+    rng = np.random.default_rng(3)
+    n_test = rows // folds
+    km, total = machines * folds, machines * rows
+    jobs = engine.jobs_to_device(engine.make_jobs(np.arange(km), n_test, np.arange(km) * n_test), dev)
+    pred = torch.rand((total, TAGS), device=dev)
+    y = torch.rand((total, TAGS), device=dev, dtype=torch.float64) * 100
+    y_scale = torch.rand((km, TAGS), device=dev, dtype=torch.float64) * 0.1 + 0.01
+    y_min = -torch.rand((km, TAGS), device=dev, dtype=torch.float64)
+    mult = torch.rand((km, TAGS), device=dev, dtype=torch.float64)
+    want = ("tag-anomaly-unscaled", "total-anomaly-scaled")
+
+    def pair():
+        back = engine.minmax_inverse_f32(jobs, km, n_test, pred, y_scale, y_min)
+        res = engine.anomaly_score(jobs, km, n_test, back["f64"], y, TAGS, scale=mult, want=want)
+        res["model-output"] = back["f32"]
+        return res
+
+    def fused():
+        return engine.minmax_inverse_score_f64(jobs, km, n_test, pred, y, y_scale, y_min, scale=mult, want=want)
+
+    a, b = pair(), fused()
+    identical = all(torch.equal(a[k].view(torch.uint8) if a[k].dtype == torch.float32 else a[k].view(torch.int64),
+                                b[k].view(torch.uint8) if b[k].dtype == torch.float32 else b[k].view(torch.int64)) for k in a)
+    del a, b
+    res = {"shape": {"machines": machines, "rows": rows, "folds": folds, "tags": TAGS}, "bit_identical": bool(identical),
+           "bytes_per_row": {"inverse_f32_plus_score_f64": 2568, "inverse_score_f64": 1544}}
+    for name, fn in (("inverse_f32_plus_score_f64", pair), ("inverse_score_f64", fused)):
+        for _ in range(3):
+            fn()
+        torch.cuda.synchronize()
+        ms = []
+        for _ in range(reps):
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            fn()
+            e1.record()
+            torch.cuda.synchronize()
+            ms.append(e0.elapsed_time(e1))
+        med = float(np.median(ms))
+        res[name] = {"ms_median": med, "ms_min": float(np.min(ms)), "ms_max": float(np.max(ms)),
+                     "GB_per_s": res["bytes_per_row"][name] * total / (med * 1e-3) / 1e9}
+    res["speedup"] = res["inverse_f32_plus_score_f64"]["ms_median"] / res["inverse_score_f64"]["ms_median"]
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--machines", type=int, default=1000)
@@ -139,6 +210,7 @@ def main():
     ap.add_argument("--rows", type=int, default=100 + WINDOW)
     ap.add_argument("--threads", type=int, default=8)
     ap.add_argument("--reps", type=int, default=200)
+    ap.add_argument("--ttr", action="store_true", help="the production definition's TransformedTargetRegressor estimator")
     a = ap.parse_args()
     import torch
     import __graft_entry__ as ge
@@ -148,12 +220,14 @@ def main():
 
     with tempfile.TemporaryDirectory() as root:
         t0 = time.perf_counter()
-        store = make_store(root, a.machines)
+        store = make_store(root, a.machines, a.ttr)
         for n in store.names():
-            store.model(n).base_estimator._device_params()  # every model's weights on the device before any arm, for both routes
+            est = store.model(n).base_estimator
+            (est.regressor_.steps[-1][1] if a.ttr else est)._device_params()  # every model's weights on the device before any arm, for both routes
         setup_s = time.perf_counter() - t0
         print(f"{a.machines} models resident in {setup_s:.1f} s", file=sys.stderr, flush=True)
-        bucket = server.ResidentBucket(store, smoothing=True)
+        bucket = (server.ResidentBucket(store, input_scalers=True, smoothing=True, target_scaler=True) if a.ttr
+                  else server.ResidentBucket(store, smoothing=True))
         assert len(bucket.names) == a.machines and bucket.smoothing == (WINDOW, "smm")
         warm = payloads(store, 3 * a.threads, a.rows, 1)
         reqs = payloads(store, a.requests, a.rows, 2)
@@ -173,9 +247,9 @@ def main():
         same = {c: replies[f"per_request_{c}"] == replies[f"bucket_{c}"] for c in ("default", "all_columns")}
         on = arms["bucket_all_columns"]
         k = max(1, round(on["requests"] / max(on["batches"], 1)))
-        launches = launch_times(torch, bucket, k, a.rows, a.reps)
+        launches = ttr_kernel_times(torch, min(a.reps, 50)) if a.ttr else launch_times(torch, bucket, k, a.rows, a.reps)
         bucket.close()
-    print(json.dumps({"card": card(), "machines": a.machines, "tags": TAGS, "window": WINDOW, "method": "smm", "rows_per_request": a.rows,
+    print(json.dumps({"card": card(), "estimator": "ttr" if a.ttr else "autoencoder", "machines": a.machines, "tags": TAGS, "window": WINDOW, "method": "smm", "rows_per_request": a.rows,
                       "requests": a.requests, "threads": a.threads, "setup_s": setup_s, "arms": arms, "replies_identical": same,
                       "per_batch_launches": {"requests_per_batch": k, **launches}}))
 

@@ -1,11 +1,14 @@
-// K5 + K7: the two small column reductions of the anomaly path.
+// K5 + K7: the two small column reductions of the anomaly path, and the scoring of existing predictions.
 //   gb_minmax_fit : sklearn MinMaxScaler.fit on the targets (reference diff.py:173)
 //   gb_thresholds : rolling(window).min().max() per tag and for the aggregate series (diff.py:222-233)
+//   gb_anomaly_score[_f64], gb_minmax_inverse_score_f64 : the anomaly columns of a prediction, the latter after the
+//                   TransformedTargetRegressor's MinMax inverse in the same pass
 // Both are HBM-bound single passes over [rows][n_out] arrays: lanes run along the tag axis so every warp
 // request is one contiguous segment, partial results meet in shared memory and one atomic per (CTA, column)
 // publishes them.
 #include <math_constants.h>
 #include "gb_common.cuh"
+#include "postprocess.cuh"
 
 namespace {
 
@@ -188,28 +191,38 @@ __global__ void __launch_bounds__(THREADS) anomaly_score_kernel(const gb_job* jo
   const T inv = (T)1 / (T)n_out;
   for (int r = r0 + warp; r < r1; r += NWARPS) {
     const long go = (job.out_row + r) * (long)n_out, gy = (job.x_row + r) * (long)n_out;
-    T ss = 0, su = 0;
-    for (int j = lane; j < n_out; j += 32) {
-      const T diff = __ldg(yhat + go + j) - __ldg(y + gy + j);
-      const T d = fabs(diff);  // +0.0 for yhat = -0.0, y = +0.0, as np.abs
-      if (o_tu) o_tu[go + j] = d;
-      su += d * d;
-      if (sc) {
-        const T e = d * __ldg(sc + j);
-        if (o_ts) o_ts[go + j] = e;
-        ss += e * e;
-      }
-      if (o_conf) o_conf[go + j] = d / __ldg(ft + j);
-    }
-    for (int o = 16; o > 0; o >>= 1) {
-      ss += __shfl_xor_sync(0xffffffffu, ss, o);
-      su += __shfl_xor_sync(0xffffffffu, su, o);
-    }
-    if (lane == 0) {
-      if (o_tots) o_tots[job.out_row + r] = ss * inv;
-      if (o_totu) o_totu[job.out_row + r] = su * inv;
-      if (o_totconf) o_totconf[job.out_row + r] = ss * inv / __ldg(agg_thr + job.slot);
-    }
+    GB_SCORE_ROW(T, __ldg(yhat + go + j));
+  }
+}
+
+// The TransformedTargetRegressor's prediction scored in one pass: every element of the network's float32 output p goes through
+// the slot's MinMax inverse (y_scale / y_min), is stored to out_model and is scored as a double against the float64 y, exactly
+// as minmax_inverse_kernel followed by anomaly_score_kernel<double> on its widened output compute it.  p and out_model may be
+// the same array (each element is read before the same thread overwrites it), so neither goes through the read-only path.
+__global__ void __launch_bounds__(THREADS) minmax_inverse_score_kernel(const gb_job* jobs, int job0, const float* p, const double* y, int n_out,
+                                                                        const double* y_scale, const double* y_min,
+                                                                        const double* scale, const double* feat_thr,
+                                                                        const double* agg_thr, float* out_model, double* o_ts,
+                                                                        double* o_tu, double* o_tots, double* o_totu,
+                                                                        double* o_conf, double* o_totconf) {
+  const gb_job job = jobs[job0 + blockIdx.y];
+  const int r0 = blockIdx.x * ROWS_PER_CTA;
+  if (r0 >= job.n_rows) return;
+  const int r1 = min(job.n_rows, r0 + ROWS_PER_CTA);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const double* sc = scale ? scale + (long)job.slot * n_out : nullptr;
+  const double* ft = feat_thr ? feat_thr + (long)job.slot * n_out : nullptr;
+  const double* ys = y_scale + (long)job.slot * n_out;
+  const double* ym = y_min + (long)job.slot * n_out;
+  const double inv = 1.0 / (double)n_out;
+  for (int r = r0 + warp; r < r1; r += NWARPS) {
+    const long go = (job.out_row + r) * (long)n_out, gy = (job.x_row + r) * (long)n_out;
+    const auto yhat = [&](int j) {
+      const float v = gb_post::minmax_inverse(p[go + j], ym + j, ys + j);
+      out_model[go + j] = v;
+      return (double)v;
+    };
+    GB_SCORE_ROW(double, yhat(j));
   }
 }
 
@@ -323,6 +336,27 @@ int gb_anomaly_score_f64(const gb_job* jobs, int32_t n_jobs, int32_t max_rows, c
                          double* out_total_unscaled, double* out_conf, double* out_total_conf, void* stream) {
   return anomaly_score_launch<double>(jobs, n_jobs, max_rows, yhat, y, n_out, scale, feat_thr, agg_thr, out_tag_scaled,
                                       out_tag_unscaled, out_total_scaled, out_total_unscaled, out_conf, out_total_conf, stream);
+}
+
+int gb_minmax_inverse_score_f64(const gb_job* jobs, int32_t n_jobs, int32_t max_rows, const float* p, const double* y,
+                                int32_t n_out, const double* y_scale, const double* y_min, const double* scale,
+                                const double* feat_thr, const double* agg_thr, float* out_model,
+                                double* out_tag_scaled, double* out_tag_unscaled, double* out_total_scaled,
+                                double* out_total_unscaled, double* out_conf, double* out_total_conf, void* stream) {
+  GB_REQUIRE(jobs && p && y && y_scale && y_min && out_model, GB_E_ARG, "jobs/p/y/y_scale/y_min/out_model must be non-NULL");
+  GB_REQUIRE(n_out >= 1, GB_E_SHAPE, "n_out=%d must be >= 1", n_out);
+  GB_REQUIRE(scale || (!out_tag_scaled && !out_total_scaled && !out_total_conf), GB_E_ARG, "scaled outputs requested without scale");
+  GB_REQUIRE(!out_conf || feat_thr, GB_E_ARG, "out_conf requested without feat_thr");
+  GB_REQUIRE(!out_total_conf || agg_thr, GB_E_ARG, "out_total_conf requested without agg_thr");
+  GB_REQUIRE(n_jobs >= 0, GB_E_ARG, "bad n_jobs");
+  if (n_jobs == 0 || max_rows <= 0) return GB_OK;
+  const int chunks = (max_rows + ROWS_PER_CTA - 1) / ROWS_PER_CTA;
+  for (int j0 = 0; j0 < n_jobs; j0 += MAX_GRID_Y)
+    minmax_inverse_score_kernel<<<dim3(chunks, min(MAX_GRID_Y, n_jobs - j0)), THREADS, 0, (cudaStream_t)stream>>>(
+        jobs, j0, p, y, n_out, y_scale, y_min, scale, feat_thr, agg_thr, out_model, out_tag_scaled, out_tag_unscaled, out_total_scaled,
+        out_total_unscaled, out_conf, out_total_conf);
+  GB_CUDA_CHECK(cudaGetLastError());
+  return GB_OK;
 }
 
 int gb_minmax_fit(const gb_job* jobs, int32_t n_jobs, int32_t max_rows, const float* y, int32_t n_out, float* scale,

@@ -4,6 +4,7 @@
 //   gb_minmax_inverse_f32  : sklearn's MinMaxScaler.inverse_transform of a float32 prediction (TransformedTargetRegressor.predict)
 // Both are HBM-bound single passes: a grid-stride loop over the job's (row, unit) pairs, the job index on gridDim.y.
 #include "gb_common.cuh"
+#include "postprocess.cuh"
 
 namespace {
 
@@ -47,7 +48,7 @@ __global__ void __launch_bounds__(THREADS) gather_narrow_kernel(const gb_job* __
   }
 }
 
-// X -= min_; X /= scale_ on a float32 array with float64 attributes: numpy computes each in-place step in float64 and stores float32.
+// X -= min_; X /= scale_ on a float32 array with float64 attributes (gb_post::minmax_inverse).
 __global__ void __launch_bounds__(THREADS) minmax_inverse_kernel(const gb_job* __restrict__ jobs, int job0, const float* __restrict__ p, int n_cols,
                                                                  const double* __restrict__ scale, const double* __restrict__ mn,
                                                                  float* __restrict__ out32, double* __restrict__ out64) {
@@ -59,8 +60,7 @@ __global__ void __launch_bounds__(THREADS) minmax_inverse_kernel(const gb_job* _
   const double* jm = mn + (long)job.slot * n_cols;
   for (long i = (long)blockIdx.x * THREADS + threadIdx.x; i < total; i += (long)gridDim.x * THREADS) {
     const int c = (int)(i % n_cols);
-    const float t = __double2float_rn(__dsub_rn((double)__ldg(src + i), __ldg(jm + c)));
-    const float v = __double2float_rn(__ddiv_rn((double)t, __ldg(js + c)));
+    const float v = gb_post::minmax_inverse(__ldg(src + i), jm + c, js + c);
     if (out32) out32[o + i] = v;
     if (out64) out64[o + i] = (double)v;
   }

@@ -481,6 +481,57 @@ def minmax_inverse_f32(jobs_dev, n_jobs, max_rows, pred, scale, min_, out_rows=N
     return res
 
 
+def minmax_inverse_score_f64(jobs_dev, n_jobs, max_rows, pred, y, y_scale, y_min, scale=None, feat_thr=None, agg_thr=None,
+                             want=SCORE_KEYS, out_rows=None, out=None):
+    """
+    The anomaly columns of a ``TransformedTargetRegressor(transformer=MinMaxScaler)`` prediction in one launch
+    (gb_minmax_inverse_score_f64): the float32 network output ``pred`` goes through sklearn's float32 ``inverse_transform`` with the
+    slot's float64 ``y_scale`` / ``y_min`` ([n_slots, n_out]) and is scored in float64 against the float64 ``y``, bit for bit
+    ``minmax_inverse_f32`` followed by ``anomaly_score`` on its float64 form.  ``pred`` and the outputs at out_row, ``y`` at x_row.
+    Returns ``{"model-output": float32, <want>: float64}`` keyed as ``anomaly_score`` keys them; ``out`` may hold preallocated
+    tensors under those keys (``out["model-output"]`` may be ``pred`` itself: the inverse is then written in place).
+    """
+    torch = _torch()
+    lib = _cabi.load_library()
+    n_out = int(pred.shape[1])
+    total = int(out_rows if out_rows is not None else pred.shape[0])
+    if pred.dtype != torch.float32:
+        raise ValueError(f"minmax_inverse_score_f64 takes a float32 prediction, got {pred.dtype}")
+    for name, t in (("y", y), ("y_scale", y_scale), ("y_min", y_min), ("scale", scale), ("feat_thr", feat_thr), ("agg_thr", agg_thr)):
+        if t is not None and t.dtype != torch.float64:
+            raise ValueError(f"minmax_inverse_score_f64: {name} is {t.dtype}, not float64")
+    sel = set(want)
+    if scale is None:
+        sel -= {"tag-anomaly-scaled", "total-anomaly-scaled", "total-anomaly-confidence"}
+    if feat_thr is None:
+        sel.discard("anomaly-confidence")
+    if agg_thr is None:
+        sel.discard("total-anomaly-confidence")
+    res = {}
+
+    def g(name, shape, dtype=torch.float64):
+        if name != "model-output" and name not in sel:
+            return None
+        if out is not None and name in out:
+            res[name] = out[name]
+        else:
+            res[name] = torch.empty(shape, dtype=dtype, device=pred.device)
+        return res[name]
+
+    o_model = g("model-output", (total, n_out), torch.float32)
+    o_ts = g("tag-anomaly-scaled", (total, n_out))
+    o_tu = g("tag-anomaly-unscaled", (total, n_out))
+    o_tots = g("total-anomaly-scaled", (total,))
+    o_totu = g("total-anomaly-unscaled", (total,))
+    o_conf = g("anomaly-confidence", (total, n_out))
+    o_totc = g("total-anomaly-confidence", (total,))
+    p = _cabi.ptr
+    _cabi.check(lib.gb_minmax_inverse_score_f64(p(jobs_dev), int(n_jobs), int(max_rows), p(pred), p(y), n_out, p(y_scale), p(y_min), p(scale),
+                                                p(feat_thr), p(agg_thr), p(o_model), p(o_ts), p(o_tu), p(o_tots), p(o_totu), p(o_conf), p(o_totc),
+                                                _stream_ptr()))
+    return res
+
+
 def orthonormal_rows(g, out, out_offset: int, out_stride: int):
     """
     Keras' Orthogonal initialiser for every float64 standard-normal draw ``g`` [n, rows, cols] (overwritten): the rows

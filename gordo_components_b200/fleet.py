@@ -836,8 +836,8 @@ def build_kfold_fleet(eng: "engine.FFEngine", x, y, rows: int, cv, epochs: int =
     contiguous block; the fits read their rows through K + 1 shared maps.  ``input_scaler``: the network is behind a MinMaxScaler
     (``Pipeline([MinMaxScaler(), KerasAutoEncoder])``); ``target_scaler``: the estimator is ``TransformedTargetRegressor(transformer=
     MinMaxScaler(), regressor=...)``, so every slot trains on its own MinMax-scaled targets and the fold models' predictions are
-    mapped back by sklearn's float32 inverse (gb_minmax_inverse_f32) and scored in float64, as the per-machine detector scores a
-    foreign estimator.  Every scaler's extrema come from gb_minmax_f64 over the test blocks (a slot's rows are a union of blocks)
+    mapped back by sklearn's float32 inverse and scored in float64 in one pass (gb_minmax_inverse_score_f64), as the per-machine
+    detector scores a foreign estimator.  Every scaler's extrema come from gb_minmax_f64 over the test blocks (a slot's rows are a union of blocks)
     with sklearn's float64 attribute arithmetic.  ``detector_shuffle``, ``validation_split``, ``early_stopping``, ``loss`` as in
     ``build_fleet``.
     """
@@ -933,13 +933,12 @@ def build_kfold_fleet(eng: "engine.FFEngine", x, y, rows: int, cv, epochs: int =
         res = eng.infer_score(params, sc_jobs, KM, max_test, xf, yf, torch.from_numpy(mult.astype(np.float32)).to(dev), out_rows=M * N, want=want)
         pred32, tag_err, tot_err = res["model-output"], res["tag-anomaly-unscaled"], res["total-anomaly-scaled"]
         mom_jobs, y32 = sc_jobs, yf
-    else:  # predict, sklearn's float32 inverse of the slot's transformer, float64 scoring against the float64 targets
+    else:  # predict, then in one pass sklearn's float32 inverse of the slot's transformer and float64 scoring against the float64 targets
         pred = eng.infer_score(params, sc_jobs, KM, max_test, xf, out_rows=M * N)["model-output"]
         mom_jobs = jobs(sc_slots, n_test[fk], out0, out0)
-        back = engine.minmax_inverse_f32(mom_jobs, KM, max_test, pred, f64(y_scale), f64(y_offset), out_rows=M * N)
-        pred32 = back["f32"]
-        res = engine.anomaly_score(mom_jobs, KM, max_test, back["f64"], yq, T, scale=f64(mult), want=want)
-        tag_err, tot_err = res["tag-anomaly-unscaled"], res["total-anomaly-scaled"]
+        res = engine.minmax_inverse_score_f64(mom_jobs, KM, max_test, pred, yq, f64(y_scale), f64(y_offset), scale=f64(mult), want=want,
+                                              out_rows=M * N)
+        pred32, tag_err, tot_err = res["model-output"], res["tag-anomaly-unscaled"], res["total-anomaly-scaled"]
         y32 = engine.gather_rows(whole, M, N, to_fold, y, M * N, to_f32=True)
 
     # 5. K-fold thresholds: errors back in time order (float32, as the detector stores them), smoothed, the percentile

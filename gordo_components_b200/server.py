@@ -264,14 +264,24 @@ class ResidentBucket:
     the ``smooth-*`` columns (``all_columns=True``) gets them from one smoothing launch over the batch's requests that asked; a
     request whose y holds a NaN and that asks for them is answered per request, where pandas' totals of those rows are recomputed
     on the host before they are smoothed.
+
+    ``target_scaler=True`` (with any of the feed-forward flags) also admits detectors whose base estimator is a fitted
+    ``TransformedTargetRegressor(transformer=MinMaxScaler(), regressor=...)`` without ``func`` / ``inverse_func`` -- the reference's
+    production definition -- around a bare ``KerasAutoEncoder`` or, with ``input_scalers=True``, a ``Pipeline([MinMaxScaler(),
+    KerasAutoEncoder])``.  The coalescer predicts, then applies each model's target inverse and scores in float64 in one launch
+    (``serving.AnomalyCoalescer(y_inverse=)``), as the per-request route does with sklearn's ``inverse_transform`` and
+    gb_anomaly_score_f64.  Other input scalers stay on the per-request route inside a TransformedTargetRegressor: sklearn's
+    ``Pipeline.predict`` runs their subtract-and-divide transform there, which the composed affine scaler of the launch does not
+    round the same way.  Models with and without a target transformer never share a bucket.
     """
 
     input_scalers = False  # the bucket holds Pipeline models (set by the constructor)
     lstm = False  # the bucket holds LSTM models (set by the constructor)
     smoothing = None  # (window, method) of the bucket's windowed detectors (set by the constructor)
+    target_scaler = False  # the bucket holds TransformedTargetRegressor models (set by the constructor)
 
     def __init__(self, store: "ModelStore", names: Optional[List[str]] = None, input_scalers: bool = False, lstm: bool = False,
-                 smoothing: bool = False, **coalescer_kwargs):
+                 smoothing: bool = False, target_scaler: bool = False, **coalescer_kwargs):
         from . import engine
         from .machine.model.anomaly.diff import _compose_affine, _scaler_multiplier
         from .serving import AnomalyCoalescer
@@ -279,7 +289,8 @@ class ResidentBucket:
         if lstm:
             self._init_lstm(store, names, smoothing, coalescer_kwargs)
             return
-        groups = self.ff_groups({name: store.model(name) for name in (names if names is not None else store.names())}, input_scalers, smoothing)
+        groups = self.ff_groups({name: store.model(name) for name in (names if names is not None else store.names())}, input_scalers, smoothing,
+                                target_scaler)
         if not groups:
             raise ValueError("no model in the store can be served through a coalescer")
         self.names = max(groups.values(), key=len)  # the largest architecture group
@@ -291,10 +302,15 @@ class ResidentBucket:
         torch = engine._torch()
         params = eng.pack_params([ae.model.weights for _, ae in parts])
         to_dev = lambda rows, dt=np.float32: torch.from_numpy(np.ascontiguousarray(np.stack(rows), dtype=dt)).to(eng.device)  # noqa: E731
-        scale = to_dev([_scaler_multiplier(m.scaler, eng.n_out) for m in models])
+        self.target_scaler = _target_minmax(models[0]) is not None
+        dt = np.float64 if self.target_scaler else np.float32  # the scores of a target inverse are float64, as on the per-request route
+        scale = to_dev([_scaler_multiplier(m.scaler, eng.n_out) for m in models], dt)
         feat, agg = zip(*(m._thresholds() for m in models))
-        feat_thr = to_dev([np.asarray(f, dtype=np.float32) for f in feat]) if feat[0] is not None else None
-        agg_thr = to_dev([np.float32(a) for a in agg]) if agg[0] is not None else None
+        feat_thr = to_dev([np.asarray(f, dtype=dt) for f in feat], dt) if feat[0] is not None else None
+        agg_thr = to_dev([dt(a) for a in agg], dt) if agg[0] is not None else None
+        if self.target_scaler:
+            y_scale, y_min = zip(*(_target_minmax(m) for m in models))
+            coalescer_kwargs.update(y_inverse=(to_dev(y_scale, np.float64), to_dev(y_min, np.float64)))
         self.input_scalers = bool(parts[0][0])
         if self.input_scalers:
             a, b = zip(*(_compose_affine(pre, eng.n_in) for pre, _ in parts))
@@ -327,16 +343,18 @@ class ResidentBucket:
         self.coalescer = LSTMAnomalyCoalescer(eng, params, scale, feat_thr, agg_thr, smoothing=self.smoothing, **coalescer_kwargs)
 
     @classmethod
-    def ff_groups(cls, models: Dict[str, Any], input_scalers: bool = False, smoothing: bool = False) -> Dict[Any, List[str]]:
+    def ff_groups(cls, models: Dict[str, Any], input_scalers: bool = False, smoothing: bool = False,
+                  target_scaler: bool = False) -> Dict[Any, List[str]]:
         """The eligible feed-forward detectors of ``models`` (name -> model) by (architecture, which thresholds are present, bare or
-        Pipeline, smoothing)."""
+        Pipeline, with or without a target transformer, smoothing)."""
         groups: Dict[Any, List[str]] = {}
         for name, model in models.items():
-            if cls.eligible(model, input_scalers, smoothing):
+            if cls.eligible(model, input_scalers, smoothing, target_scaler):
                 pre, ae = _served_parts(model)
                 spec = ae.model.spec
                 has_thr = tuple(t is not None for t in model._thresholds())
-                groups.setdefault((tuple(spec.dims), tuple(spec.acts), tuple(spec.l1), has_thr, bool(pre), _smoothing_of(model)), []).append(name)
+                key = (tuple(spec.dims), tuple(spec.acts), tuple(spec.l1), has_thr, bool(pre), _target_minmax(model) is not None, _smoothing_of(model))
+                groups.setdefault(key, []).append(name)
         return groups
 
     @classmethod
@@ -374,7 +392,7 @@ class ResidentBucket:
         return True
 
     @staticmethod
-    def eligible(model, input_scalers: bool = False, smoothing: bool = False) -> bool:
+    def eligible(model, input_scalers: bool = False, smoothing: bool = False, target_scaler: bool = False) -> bool:
         if not (_frame_is_from_blocks(model) and _window_served(model, smoothing)
                 and not (model.require_thresholds and all(t is None for t in model._thresholds()))):
             return False
@@ -382,10 +400,19 @@ class ResidentBucket:
         if parts is None or parts[1].model is None or (parts[0] and not input_scalers):
             return False
         pre, ae = parts
+        from sklearn.compose import TransformedTargetRegressor
+        from sklearn.preprocessing import MinMaxScaler
+
         from .machine.model.anomaly.diff import _compose_affine, _scaler_multiplier
 
         if pre and (_compose_affine(pre, ae.model.spec.dims[0]) is None or not _x64_launch_holds(ae.model.spec)):
             return False  # served per request: sklearn's own transform, or the separate gb_affine_f64 pass
+        if type(model.base_estimator) is TransformedTargetRegressor:
+            target = _target_minmax(model)
+            if not target_scaler or target is None or target[0].shape != (ae.model.spec.dims[-1],):
+                return False
+            if pre and not (len(pre) == 1 and type(pre[0]) is MinMaxScaler):
+                return False  # other scalers subtract and divide in sklearn's Pipeline.predict, which the composed affine does not round alike
         try:  # a non-affine error scaler (clip=True, QuantileTransformer, ...) is served on the per-request path, not refused for the whole store
             _scaler_multiplier(model.scaler, ae.model.spec.dims[-1])
         except (ValueError, AttributeError):
@@ -411,6 +438,10 @@ class ResidentBucket:
             # the coalescer's launch may run the tensor-core kernel, which does not take ±inf inputs: this request goes on its own
             return model.anomaly_blocks(X, y, frequency=frequency, smooth=smooth)
         scores = self._scores(name, X, y, smooth)
+        raw = scores.pop("raw-model-output", None)
+        if raw is not None and _has_inf(raw):
+            # what sklearn's inverse_transform raises on the regressor's prediction, before the per-request route's own check
+            raise ValueError(f"Input contains infinity or a value too large for {raw.dtype!r}.")
         _refuse_infinity(scores["model-output"])
         return model.blocks_from_scores(scores, X, y, frequency, smooth=smooth)
 
@@ -464,17 +495,40 @@ def _extract_X_y(store: ModelStore, name: str, json: Optional[dict], files: Opti
 
 def _served_parts(model):
     """(input scaler steps, ``KerasAutoEncoder``) of a detector whose base estimator is a bare autoencoder ([] for the steps) or a
-    ``Pipeline`` ending in one, else None."""
+    ``Pipeline`` ending in one, else None.  For a fitted ``TransformedTargetRegressor`` these are the parts of its ``regressor_``
+    (its target transformer: ``_target_minmax``)."""
+    from sklearn.compose import TransformedTargetRegressor
     from sklearn.pipeline import Pipeline
 
     from .machine.model.models import KerasAutoEncoder
 
     est = model.base_estimator
+    if type(est) is TransformedTargetRegressor:
+        est = getattr(est, "regressor_", None)
     if type(est) is KerasAutoEncoder:
         return [], est
     if type(est) is Pipeline and len(est.steps) > 1 and type(est.steps[-1][1]) is KerasAutoEncoder:
         return [step for _, step in est.steps[:-1]], est.steps[-1][1]
     return None
+
+
+def _target_minmax(model):
+    """(scale_, min_) as float64 arrays of the target transformer of a detector whose base estimator is a fitted
+    ``TransformedTargetRegressor`` without ``func`` / ``inverse_func`` whose ``transformer_`` is exactly a ``MinMaxScaler`` (what
+    gb_minmax_inverse_score_f64 applies), else None."""
+    from sklearn.compose import TransformedTargetRegressor
+    from sklearn.preprocessing import MinMaxScaler
+
+    est = model.base_estimator
+    if type(est) is not TransformedTargetRegressor or est.func is not None or est.inverse_func is not None:
+        return None
+    tr = getattr(est, "transformer_", None)
+    if type(tr) is not MinMaxScaler or getattr(est, "_training_dim", None) != 2:
+        return None  # a 1-D target comes back squeezed from predict
+    scale, mn = getattr(tr, "scale_", None), getattr(tr, "min_", None)
+    if scale is None or mn is None or np.ndim(scale) != 1 or np.shape(scale) != np.shape(mn):
+        return None
+    return np.ascontiguousarray(scale, dtype=np.float64), np.ascontiguousarray(mn, dtype=np.float64)
 
 
 def _served_lstm_parts(model):

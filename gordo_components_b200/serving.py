@@ -16,6 +16,13 @@ With ``x_scale`` / ``x_offset`` (float64 [n_slots, n_in] device tensors: the com
 requests' X is staged as float64 and the launch applies each slot's scaler as it reads x (gb_ffae_infer_score_x64), exactly the
 float32 batch ``gb_affine_f64`` would have produced.
 
+With ``y_inverse=(y_scale, y_min)`` (float64 [n_slots, n_out] device tensors: the MinMax ``transformer_`` of detectors around a
+``TransformedTargetRegressor``) the batch runs the fused launch for the prediction only, then one gb_minmax_inverse_score_f64
+launch that applies sklearn's float32 ``inverse_transform`` and scores in float64 against the float64 y, as the per-request route
+does on the host and in gb_anomaly_score_f64.  ``scale`` / thresholds are then float64 and so are the score arrays; a request
+whose model output holds ±inf also gets the network's raw prediction of its rows under ``raw-model-output``, so the caller can
+tell an infinite prediction from an inverse that overflows float32.
+
 Thread-safe, re-entrant, no shared mutable scratch outside the worker thread (the reference's threading convention,
 SURVEY §8b).  The per-request results are bit-identical to a per-request launch: rows are independent in the kernel.
 
@@ -46,7 +53,7 @@ SMM_MAX_WINDOW = 200 * 1024 // 4  # the rolling median keeps one thread's sorted
 
 class AnomalyCoalescer:
     def __init__(self, eng: "engine.FFEngine", params, scale, feat_thr=None, agg_thr=None, max_batch_rows: int = 1 << 18,
-                 max_wait_ms: float = 1.0, want: Optional[Sequence[str]] = None, x_scale=None, x_offset=None, smoothing=None):
+                 max_wait_ms: float = 1.0, want: Optional[Sequence[str]] = None, x_scale=None, x_offset=None, smoothing=None, y_inverse=None):
         torch = engine._torch()
         self.eng, self.params, self.scale, self.feat_thr, self.agg_thr = eng, params, scale, feat_thr, agg_thr
         if (x_scale is None) != (x_offset is None):
@@ -54,6 +61,9 @@ class AnomalyCoalescer:
         self.x_affine = (x_scale, x_offset) if x_scale is not None else None
         x_dtype = torch.float64 if self.x_affine is not None else torch.float32
         self._x_np = np.float64 if self.x_affine is not None else np.float32
+        self.y_inverse = tuple(y_inverse) if y_inverse is not None else None
+        y_dtype, score_dtype = (torch.float64, torch.float64) if self.y_inverse is not None else (torch.float32, torch.float32)
+        self._y_np = np.float64 if self.y_inverse is not None else np.float32
         self.max_rows, self.max_wait = int(max_batch_rows), float(max_wait_ms) * 1e-3
         self.want = tuple(want) if want is not None else tuple(
             k for k in PER_TAG + PER_ROW if not ((feat_thr is None and k == "anomaly-confidence") or (agg_thr is None and k == "total-anomaly-confidence")))
@@ -61,11 +71,14 @@ class AnomalyCoalescer:
         dev = eng.device
         self._stream = torch.cuda.Stream(device=dev)
         self._xh = torch.empty((self.max_rows, eng.n_in), dtype=x_dtype).pin_memory()
-        self._yh = torch.empty((self.max_rows, eng.n_out), dtype=torch.float32).pin_memory()
+        self._yh = torch.empty((self.max_rows, eng.n_out), dtype=y_dtype).pin_memory()
         self._xd = torch.empty((self.max_rows, eng.n_in), dtype=x_dtype, device=dev)
-        self._yd = torch.empty((self.max_rows, eng.n_out), dtype=torch.float32, device=dev)
-        self._out_d = {k: torch.empty((self.max_rows, eng.n_out) if k in PER_TAG else (self.max_rows,), dtype=torch.float32, device=dev) for k in self.want}
-        self._out_h = {k: torch.empty(v.shape, dtype=torch.float32).pin_memory() for k, v in self._out_d.items()}
+        self._yd = torch.empty((self.max_rows, eng.n_out), dtype=y_dtype, device=dev)
+        self._out_d = {k: torch.empty((self.max_rows, eng.n_out) if k in PER_TAG else (self.max_rows,),
+                                      dtype=torch.float32 if k == "model-output" else score_dtype, device=dev) for k in self.want}
+        if self.y_inverse is not None:  # the network's raw prediction, kept apart from its inverse
+            self._out_d["raw-model-output"] = torch.empty((self.max_rows, eng.n_out), dtype=torch.float32, device=dev)
+        self._out_h = {k: torch.empty(v.shape, dtype=v.dtype).pin_memory() for k, v in self._out_d.items()}
         # the batch's jobs, then those of its requests that want the smoothed columns
         self._jobs_h = torch.empty((2 * self.max_jobs * engine._cabi.JOB_DTYPE.itemsize,), dtype=torch.uint8).pin_memory()
         self.max_cost = self.max_rows
@@ -114,7 +127,7 @@ class AnomalyCoalescer:
     def _request(self, X, y):
         """The request's staged (X, y) host arrays, or ValueError when they do not fit the bucket."""
         Xv = np.ascontiguousarray(getattr(X, "values", X), dtype=self._x_np)
-        yv = np.ascontiguousarray(getattr(y, "values", y), dtype=np.float32)
+        yv = np.ascontiguousarray(getattr(y, "values", y), dtype=self._y_np)
         if Xv.ndim != 2 or Xv.shape[1] != self.eng.n_in or yv.shape != (len(Xv), self.eng.n_out):
             raise ValueError(f"request of shape X {Xv.shape} / y {yv.shape} does not fit a {self.eng.n_in}->{self.eng.n_out} model")
         if len(Xv) > self.max_rows:
@@ -216,13 +229,19 @@ class AnomalyCoalescer:
             jobs_d = jobs_all[: jobs.nbytes]
             self._xd[:rows].copy_(self._xh[:rows], non_blocking=True)
             self._yd[:rows].copy_(self._yh[:rows], non_blocking=True)
-            if rows:
+            out = {k: v[:rows] for k, v in self._out_d.items()}
+            if rows and self.y_inverse is None:
                 self.eng.infer_score(self.params, jobs_d, len(batch), max_rows, self._xd[:rows], self._yd[:rows], self.scale, self.feat_thr,
-                                     self.agg_thr, out_rows=rows, want=self.want, out={k: v[:rows] for k, v in self._out_d.items()},
+                                     self.agg_thr, out_rows=rows, want=self.want, out=out, x_affine=self.x_affine)
+            elif rows:  # prediction only, then the target inverse and float64 scoring in one pass
+                raw = out.pop("raw-model-output")
+                self.eng.infer_score(self.params, jobs_d, len(batch), max_rows, self._xd[:rows], out_rows=rows, out={"model-output": raw},
                                      x_affine=self.x_affine)
+                engine.minmax_inverse_score_f64(jobs_d, len(batch), max_rows, raw, self._yd[:rows], *self.y_inverse, self.scale, self.feat_thr,
+                                                self.agg_thr, want=self.want, out_rows=rows, out=out)
             if smooth is not None:
                 smoothed = (self._smooth(torch, jobs_all[jobs.nbytes:], *smooth, self._out_d), smooth[1])
-            for k in self.want:
+            for k in self._out_d:
                 self._out_h[k][:rows].copy_(self._out_d[k][:rows], non_blocking=True)
         self._stream.synchronize()
         self.batches += 1
@@ -230,7 +249,10 @@ class AnomalyCoalescer:
         ofs = 0
         for item in batch:
             n = len(item[1])
-            item[-1].set_result(self._with_smoothed({k: self._out_h[k][ofs:ofs + n].numpy().copy() for k in self.want}, item, smoothed, ofs, n))
+            result = {k: self._out_h[k][ofs:ofs + n].numpy().copy() for k in self.want}
+            if self.y_inverse is not None and np.isinf(result.get("model-output", 0.0)).any():
+                result["raw-model-output"] = self._out_h["raw-model-output"][ofs:ofs + n].numpy().copy()
+            item[-1].set_result(self._with_smoothed(result, item, smoothed, ofs, n))
             ofs += n
 
 

@@ -174,6 +174,19 @@ int gb_anomaly_score_f64(const gb_job* jobs, int32_t n_jobs, int32_t max_rows, c
                          double* out_tag_scaled, double* out_tag_unscaled, double* out_total_scaled,
                          double* out_total_unscaled, double* out_conf, double* out_total_conf, void* stream);
 
+/* A TransformedTargetRegressor(transformer=MinMaxScaler) prediction, inverse-transformed and scored in float64 in one pass: for
+ * every element, v = (float)((double)(float)((double)p - y_min) / y_scale) (sklearn's MinMaxScaler.inverse_transform on the float32
+ * prediction, as gb_minmax_inverse_f32) goes to out_model, and (double)v is scored against y exactly as gb_anomaly_score_f64 scores
+ * it, in the same order.  Every output is bit for bit gb_minmax_inverse_f32 followed by gb_anomaly_score_f64 on the widened
+ * result, without the float64 copy of the prediction in between.  p (the network's raw float32 output), out_model and the score
+ * outputs are indexed by out_row, y by x_row; p and out_model may be the same array.  y_scale / y_min: [n_slots][n_out], the
+ * transformer's scale_ / min_.  scale / feat_thr / agg_thr and every score output as gb_anomaly_score_f64 (any output may be NULL). */
+int gb_minmax_inverse_score_f64(const gb_job* jobs, int32_t n_jobs, int32_t max_rows, const float* p, const double* y,
+                                int32_t n_out, const double* y_scale, const double* y_min, const double* scale,
+                                const double* feat_thr, const double* agg_thr, float* out_model,
+                                double* out_tag_scaled, double* out_tag_unscaled, double* out_total_scaled,
+                                double* out_total_unscaled, double* out_conf, double* out_total_conf, void* stream);
+
 /* ---- K7: MinMaxScaler.fit on the targets (diff.py:173; sklearn MinMaxScaler [3P]) -------
  * per job: scale[slot][j] = 1/(max_j - min_j) (zero range -> 1), offset[slot][j] = -min_j*scale.
  * minmax_ws: workspace [n_slots][2][n_out] floats (overwritten). */
