@@ -10,6 +10,7 @@ number a `gordo build` user sees.
     python benchmarks/bench_fleet_builder.py --example-config --machines 125 --rows 10000 --tags 64 --epochs 10 --single 3
     python benchmarks/bench_fleet_builder.py --early-stopping --machines 125 --rows 10000 --tags 64 --epochs 100 --single 1
     python benchmarks/bench_fleet_builder.py --kfcv --machines 125 --rows 10000 --tags 64 --epochs 20 --single 1
+    python benchmarks/bench_fleet_builder.py --ragged 5000:15000 --machines 125 --tags 64 --epochs 10 --single 1 [--kfcv | --lstm | --example-config]
 
 ``--lstm`` builds DiffBasedAnomalyDetector(KerasLSTMAutoEncoder(lstm_hourglass)) machines instead (batched by
 fleet.build_lstm_fleet).  ``--example-config`` builds the model of gordo's examples/model-configuration.yaml:
@@ -24,6 +25,10 @@ compression_factor 0.5, 1 encoding layer, batch 128, validation_split 0.1, Early
 under KFold(5, shuffle=True, random_state=0), with FleetModelBuilder(early_stopping=True, kfcv=True); it also reports the device
 time of the K-fold threshold stage (errors back to time order, smoothing, percentile, metric moments: the launches
 fleet.build_kfold_fleet makes after the fold scoring, on arrays of the bucket's shape), CUDA events, after a warm-up.
+``--ragged LO:HI`` draws every machine's length uniformly from [LO, HI] (seeded) and builds the project with
+FleetModelBuilder(ragged=True) and with the default, alternating, ``--runs`` times each: wall time, the number of buckets and of
+fit launches, and the device time of the fit launches (CUDA events around each, summed per build).  Without the flag every
+length is its own bucket.
 Measured numbers and the card they were measured on are in DESIGN.md §5b and §7.
 """
 import argparse, json, os, sys, tempfile, time
@@ -56,6 +61,8 @@ def main():
     ap.add_argument("--launch-runs", type=int, default=3, help="--early-stopping: timed fit launches of each kind")
     ap.add_argument("--min-delta", type=float, default=0.0, help="--early-stopping: the callback's min_delta (the reference's definition has none)")
     ap.add_argument("--kfcv", action="store_true", help="the reference's production definition: a K-fold detector under KFold(5, shuffle, random_state=0)")
+    ap.add_argument("--ragged", default=None, metavar="LO:HI", help="per-machine lengths drawn uniformly from [LO, HI]; ragged=True against the default")
+    ap.add_argument("--runs", type=int, default=2, help="--ragged: builds of each kind, alternating")
     a = ap.parse_args()
     import numpy as np
     import pandas as pd
@@ -94,13 +101,22 @@ def main():
         evaluation, n_splits = {"cv": {"sklearn.model_selection.KFold": {"n_splits": 5, "shuffle": True, "random_state": 0}}}, 5
     flags = dict(early_stopping=a.early_stopping or a.kfcv, kfcv=a.kfcv)
     rng = np.random.default_rng(0)
-    idx = pd.date_range("2019-01-01", periods=a.rows, freq="10min", tz="UTC")
-    t = np.linspace(0, 60, a.rows)[:, None]
+    if a.ragged:
+        lo, hi = (int(v) for v in a.ragged.split(":"))
+        lengths = np.random.default_rng(1).integers(lo, hi + 1, size=a.machines)
+    else:
+        lengths = np.full(a.machines, a.rows)
     machines = []
     for m in range(a.machines):
-        values = 0.5 + 0.4 * np.sin(t * rng.uniform(0.5, 2, a.tags) + rng.uniform(0, 6, a.tags)) + rng.normal(0, 0.02, (a.rows, a.tags))
+        rows = int(lengths[m])
+        idx = pd.date_range("2019-01-01", periods=rows, freq="10min", tz="UTC")
+        t = np.linspace(0, 60 * rows / a.rows, rows)[:, None]
+        values = 0.5 + 0.4 * np.sin(t * rng.uniform(0.5, 2, a.tags) + rng.uniform(0, 6, a.tags)) + rng.normal(0, 0.02, (rows, a.tags))
         frame = pd.DataFrame(values.astype(np.float32), index=idx, columns=[f"tag-{i}" for i in range(a.tags)])
         machines.append({"name": f"machine-{m}", "model": model, "dataset": {"X": frame, "y": frame}, "evaluation": evaluation})
+    if a.ragged:
+        print(json.dumps(_ragged_builds(a, machines, flags, n_splits, lengths)))
+        return
 
     builder.FleetModelBuilder(machines[:2], **flags).build()  # warm-up: library load, first launches
     torch.cuda.synchronize()
@@ -141,6 +157,73 @@ def main():
         out.update({"final_fit_epochs_run_min": int(ran.min()), "final_fit_epochs_run_median": float(np.median(ran)), "final_fit_epochs_run_max": int(ran.max())})
         out.update(_kfold_threshold_stage(a))
     print(json.dumps(out))
+
+
+def _ragged_builds(a, machines, flags, n_splits, lengths):
+    """
+    The project built with FleetModelBuilder(ragged=True) and with the default, alternating: wall time of each build (host work and
+    the written files included), buckets, and the fit launches' device time (CUDA events around every fit launch of the build,
+    read after the build's final synchronise).  One warm-up of each kind first.
+    """
+    import numpy as np
+    import torch
+
+    from gordo_components_b200 import builder, engine
+
+    launches, buckets = [], []
+
+    def timed(fn):
+        def run(*args, **kw):
+            ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
+            ev[0].record()
+            res = fn(*args, **kw)
+            ev[1].record()
+            launches.append(ev)
+            return res
+        return run
+
+    def counted(fn):
+        def run(members):
+            buckets.append(len(members))
+            return fn(members)
+        return run
+
+    engine.FFEngine._fit_launch = timed(engine.FFEngine._fit_launch)
+    engine.LSTMEngine._fit_launch = timed(engine.LSTMEngine._fit_launch)
+    builder.FleetModelBuilder._build_bucket = staticmethod(counted(builder.FleetModelBuilder._build_bucket))
+
+    def build(ragged, project):
+        launches.clear()
+        buckets.clear()
+        with tempfile.TemporaryDirectory() as out:
+            t0 = time.perf_counter()
+            builder.FleetModelBuilder(project, ragged=ragged, **flags).build(out)
+            torch.cuda.synchronize()
+            wall = time.perf_counter() - t0
+        return {"wall_s": wall, "buckets": len(buckets), "fit_launches": len(launches),
+                "fit_launch_ms": sum(e[0].elapsed_time(e[1]) for e in launches)}
+
+    build(True, machines[:2]), build(False, machines[:2])  # warm-up
+    runs = {"ragged": [], "default": []}
+    for _ in range(a.runs):
+        runs["ragged"].append(build(True, machines))
+        runs["default"].append(build(False, machines))
+    single_s = None
+    if a.single:
+        t0 = time.perf_counter()
+        for m in machines[: a.single]:
+            builder.ModelBuilder(m).build()
+        torch.cuda.synchronize()
+        single_s = (time.perf_counter() - t0) / a.single
+    kind = "K-fold detector (--kfcv)" if a.kfcv else ("LSTM hourglass" if a.lstm else ("example-config hourglass" if a.example_config else "hourglass"))
+    out = {"gpu": torch.cuda.get_device_name(0), "power_limit_w": _power_limit(),
+           "workload": f"{a.machines} machines x {a.tags}-tag {kind}, lengths uniform in [{a.ragged}] (seed 1; total {int(lengths.sum())} rows), "
+                       f"{a.epochs} epochs, {n_splits}-fold CV, written to disk",
+           "model_builder_s_per_machine": single_s}
+    for kind, rs in runs.items():
+        out[kind] = {key: [r[key] for r in rs] for key in rs[0]}
+    out["wall_speedup_median"] = float(np.median(out["default"]["wall_s"]) / np.median(out["ragged"]["wall_s"]))
+    return out
 
 
 def _kfold_threshold_stage(a, runs: int = 5):

@@ -6,7 +6,7 @@ definition -> cross validation with the evaluation metrics -> final fit -> offse
 
 ``FleetModelBuilder`` is where the batched kernels pay off: machines whose definition is the canonical
 ``DiffBasedAnomalyDetector(base_estimator=KerasAutoEncoder(<feed-forward kind>), scaler=MinMaxScaler())`` -- the network bare or
-behind one ``MinMaxScaler`` in a Pipeline, as in gordo's example configs -- are bucketed by architecture and training length, and every bucket is built by ``fleet.build_fleet`` -- all final fits and all CV folds
+behind one ``MinMaxScaler`` in a Pipeline, as in gordo's example configs -- are bucketed by architecture and training length (with ``FleetModelBuilder(ragged=True)`` by architecture alone), and every bucket is built by ``fleet.build_fleet`` -- all final fits and all CV folds
 in one ``gb_ffae_fit`` launch, fold scoring / thresholds / scaler statistics / metric moments one launch each.  With
 ``FleetModelBuilder(early_stopping=True)`` an estimator with one Keras ``EarlyStopping`` callback on a metric its fit reports
 (loss, accuracy, and their ``val_*`` forms with a ``validation_split``) is batched as well: every fit applies the rule inside the
@@ -337,10 +337,11 @@ class _Canonical:
         self.X, self.y, self.dataset_meta, self.query_sec = X, y, dataset_meta, query_sec
         self.fit, self.n_splits, self.evaluation = fit, n_splits, evaluation
 
-    def bucket(self):
+    def bucket(self, ragged: bool = False):
+        """The fields machines of one batched build share; ``ragged`` leaves out the row count (``FleetModelBuilder(ragged=True)``)."""
         s = self.spec
         return (tuple(s.dims), tuple(s.acts), tuple(float(v) for v in s.l1), tuple(sorted(s.adam.items())), tuple(s.metrics), s.loss,
-                len(self.X), self.fit["epochs"], self.fit["batch_size"], self.fit["shuffle"], self.n_splits, int(self.evaluation.get("seed", 0)),
+                None if ragged else len(self.X), self.fit["epochs"], self.fit["batch_size"], self.fit["shuffle"], self.n_splits, int(self.evaluation.get("seed", 0)),
                 self.split, self.early_stopping is not None, self.input_scaler) + optimizer_key(s)  # EarlyStopping's parameters are per-job records
 
 
@@ -473,9 +474,9 @@ class _CanonicalLSTM(_Canonical):
         super().__init__(*args)
         self.lookahead = lookahead
 
-    def bucket(self):
+    def bucket(self, ragged: bool = False):
         s = self.spec
-        return (s.key(), tuple(sorted(s.adam.items())), tuple(s.metrics), s.loss, self.lookahead, len(self.X), self.fit["epochs"], self.fit["batch_size"],
+        return (s.key(), tuple(sorted(s.adam.items())), tuple(s.metrics), s.loss, self.lookahead, None if ragged else len(self.X), self.fit["epochs"], self.fit["batch_size"],
                 self.n_splits, int(self.evaluation.get("seed", 0)), self.input_scaler, self.early_stopping is not None) + optimizer_key(s)  # EarlyStopping's parameters are per-job records
 
 
@@ -576,9 +577,9 @@ class _CanonicalKFold(_Canonical):
         super().__init__(*args)
         self.cv, self.target_scaler = cv, target_scaler
 
-    def bucket(self):
+    def bucket(self, ragged: bool = False):
         m = self.model  # every field below is a scalar of the shared row maps or of the gb_smooth / gb_quantile launches
-        return super().bucket() + ((self.cv.n_splits, bool(self.cv.shuffle), self.cv.random_state), m.window, m.smoothing_method,
+        return super().bucket(ragged) + ((self.cv.n_splits, bool(self.cv.shuffle), self.cv.random_state), m.window, m.smoothing_method,
                                    float(m.threshold_percentile), bool(m.shuffle), self.target_scaler)
 
 
@@ -680,10 +681,17 @@ class FleetModelBuilder:
     ``accuracy`` (``_canonical_lstm``).  Every fit applies the rule inside its launch (``fleet.build_lstm_fleet(early_stopping=...)``)
     and a fit that stops does no further work.  Off by default for the same reason as ``kfcv``: without it such machines build
     through ``ModelBuilder``, one epoch launch at a time.  It combines with ``lstm_wide_batches``.
+
+    ``ragged``: let machines of different lengths share a bucket (the bucket keys leave out the row count; every other field
+    still separates buckets).  Each machine keeps its own CV split, fold blocks, scalers and metadata; the batched builds take
+    one row count per machine.  Off by default for the same reason as ``kfcv``: the batched fits draw their initial weights per
+    bucket, so merging lengths changes which weights a machine starts from.  Without it buckets, builds and artefacts are
+    those of equal-length buckets.
     """
 
     def __init__(self, machines: Sequence, early_stopping: bool = False, kfcv: bool = False, lstm_wide_batches: bool = False,
-                 lstm_early_stopping: bool = False):
+                 lstm_early_stopping: bool = False, ragged: bool = False):
+        self.ragged = bool(ragged)
         self.early_stopping = bool(early_stopping)
         self.kfcv = bool(kfcv)
         self.lstm_wide_batches = bool(lstm_wide_batches)
@@ -701,7 +709,8 @@ class FleetModelBuilder:
         from . import fleet
 
         return FleetModelBuilder([self.machines[i] for i in fleet.partition(len(self.machines), world)[rank]], early_stopping=self.early_stopping,
-                                 kfcv=self.kfcv, lstm_wide_batches=self.lstm_wide_batches, lstm_early_stopping=self.lstm_early_stopping)
+                                 kfcv=self.kfcv, lstm_wide_batches=self.lstm_wide_batches, lstm_early_stopping=self.lstm_early_stopping,
+                                 ragged=self.ragged)
 
     def build(self, output_dir: Optional[str] = None) -> List[Tuple[Any, dict]]:
         results: List[Optional[Tuple[Any, dict]]] = [None] * len(self.machines)
@@ -716,7 +725,7 @@ class FleetModelBuilder:
             if c is None:
                 results[i] = ModelBuilder(machine).build()
             else:
-                buckets.setdefault(c.bucket(), []).append(c)
+                buckets.setdefault(c.bucket(self.ragged), []).append(c)
         for members in buckets.values():
             try:
                 built_bucket = self._build_bucket(members)
@@ -740,7 +749,7 @@ class FleetModelBuilder:
 
         first = members[0]
         eng = engine.ff_engine_for(first.spec)
-        rows, K = len(first.X), first.n_splits
+        rows, K = [len(c.X) for c in members], first.n_splits
         t0 = time.time()
         x_host = np.concatenate([np.ascontiguousarray(c.X.values, dtype=np.float32) for c in members])
         same_y = all(c.y is c.X for c in members)
@@ -755,7 +764,6 @@ class FleetModelBuilder:
         scale = fb.scale.cpu().numpy().astype(np.float64)
         engine._torch().cuda.synchronize()
         share = (time.time() - t0) / len(members)  # the bucket's wall time, spread evenly: there is no per-machine time any more
-        test = rows // (K + 1)
         split_obj = TimeSeriesSplit(n_splits=K)
         out = []
         for m, c in enumerate(members):
@@ -763,7 +771,7 @@ class FleetModelBuilder:
             model = fb.detector(m, tags=tags, template=c.model, input_tags=list(c.X.columns))
             names = [s.rpartition(".")[2] for s in c.evaluation["metrics"]]
             scoring_scale = scale[m] if c.evaluation.get("scoring_scaler") else None
-            scores = scores_block(scores_from_moments(moments[m], test, scoring_scale, names), tags)
+            scores = scores_block(scores_from_moments(moments[m], int(fb.n_test[m]), scoring_scale, names), tags)
             model_block = {
                 "model_offset": 0,  # a Dense stack answers every row
                 "model_creation_date": _now(),
@@ -782,7 +790,7 @@ class FleetModelBuilder:
 
         first = members[0]
         eng = engine.lstm_engine_for(first.spec)
-        rows, K = len(first.X), first.n_splits
+        rows, K = [len(c.X) for c in members], first.n_splits
         t0 = time.time()
         xd = engine._torch().from_numpy(np.concatenate([np.ascontiguousarray(c.X.values, dtype=np.float64) for c in members])).to(eng.device)
         same_y = all(c.y is c.X for c in members)
@@ -800,7 +808,7 @@ class FleetModelBuilder:
             model = fb.detector(m, tags=tags, template=c.model, input_tags=list(c.X.columns))
             names = [s.rpartition(".")[2] for s in c.evaluation["metrics"]]
             scoring_scale = model.scaler.scale_ if c.evaluation.get("scoring_scaler") else None  # the scoring scaler sees all targets too
-            scores = scores_block(scores_from_moments(fb.cv_moments[m], fb.n_test, scoring_scale, names), tags)
+            scores = scores_block(scores_from_moments(fb.cv_moments[m], int(fb.machine_n_test[m]), scoring_scale, names), tags)
             model_block = {
                 "model_offset": eng.lookback - 1 + c.lookahead,  # the first prediction answers row lookback_window - 1 + lookahead
                 "model_creation_date": _now(),
@@ -820,7 +828,7 @@ class FleetModelBuilder:
 
         first = members[0]
         eng = engine.ff_engine_for(first.spec)
-        rows, K = len(first.X), first.n_splits
+        rows, K = [len(c.X) for c in members], first.n_splits
         torch = engine._torch()
         t0 = time.time()
         xd = torch.from_numpy(np.concatenate([np.ascontiguousarray(c.X.values, dtype=np.float64) for c in members])).to(eng.device)
@@ -842,7 +850,7 @@ class FleetModelBuilder:
             model = fb.detector(m, c.model, tags=tags, input_tags=list(c.X.columns))
             names = [s.rpartition(".")[2] for s in c.evaluation["metrics"]]
             scoring_scale = model.scaler.scale_ if c.evaluation.get("scoring_scaler") else None  # the scoring scaler sees all targets too
-            scores = scores_block(scores_from_moments(fb.cv_moments[m], fb.n_test, scoring_scale, names), tags)
+            scores = scores_block(scores_from_moments(fb.cv_moments[m], fb.n_test[m], scoring_scale, names), tags)
             model_block = {
                 "model_offset": 0,  # a Dense stack answers every row
                 "model_creation_date": _now(),

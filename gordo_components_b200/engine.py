@@ -437,11 +437,12 @@ def affine_f64(jobs_dev, n_jobs, max_rows, x64, a, b, out_rows=None):
     return out
 
 
-def gather_rows(jobs_dev, n_jobs, max_rows, row_map, src, out_rows: int, to_f32: bool = False, out=None):
+def gather_rows(jobs_dev, n_jobs, max_rows, row_map, src, out_rows: int, to_f32: bool = False, out=None, map_ofs=None):
     """
     Row permutation per job (gb_gather_rows): out[out_row + p] = src[x_row + row_map[p]] for p < n_rows.  ``src``: [rows, cols]
     or [rows] tensor of 4- or 8-byte elements; ``to_f32`` narrows float64 to float32 in the same pass.  ``row_map``: int32 device
-    tensor shared by every job.  Returns ``out`` ([out_rows, ...], allocated when not given).
+    tensor shared by every job.  ``map_ofs``: int64 device tensor [n_jobs] giving each job its own map, row_map[map_ofs[i] + p]
+    (gb_gather_rows_ragged).  Returns ``out`` ([out_rows, ...], allocated when not given).
     """
     torch = _torch()
     lib = _cabi.load_library()
@@ -456,6 +457,12 @@ def gather_rows(jobs_dev, n_jobs, max_rows, row_map, src, out_rows: int, to_f32:
     if out.dtype != dtype:
         raise ValueError(f"gather_rows: out is {out.dtype}, expected {dtype}")
     p = _cabi.ptr
+    if map_ofs is not None:
+        if map_ofs.dtype != torch.int64:
+            raise ValueError(f"gather_rows takes int64 map offsets, got {map_ofs.dtype}")
+        _cabi.check(lib.gb_gather_rows_ragged(p(jobs_dev), int(n_jobs), int(max_rows), p(row_map), p(map_ofs), p(src), n_cols, int(src.element_size()),
+                                              int(bool(to_f32)), p(out), _stream_ptr()))
+        return out
     _cabi.check(lib.gb_gather_rows(p(jobs_dev), int(n_jobs), int(max_rows), p(row_map), p(src), n_cols, int(src.element_size()), int(bool(to_f32)),
                                    p(out), _stream_ptr()))
     return out

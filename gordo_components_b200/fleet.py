@@ -167,14 +167,19 @@ class FleetBuild:
     def __init__(self, eng, n_machines, n_splits, params, scale, offset, feat_thr, agg_thr, loss, acc, fold_loss, fold_feat_thr, fold_agg_thr,
                  fold_params=None, cv_moments=None, in_scale=None, in_offset=None, fold_in_scale=None, fold_in_offset=None, steps_per_epoch=None,
                  val_loss=None, val_acc=None, fold_val_loss=None, fold_val_acc=None, epochs=None, epochs_run=None, best_epoch=None,
-                 fold_epochs_run=None, fold_best_epoch=None):
+                 fold_epochs_run=None, fold_best_epoch=None, rows=None, n_test=None, starts=None, init_params=None):
         # EarlyStopping: epochs each fit ran and its best epoch (-1: none) ([M]; per CV fold [M, K]); None without the callback.
         # History entries past a fit's epochs_run are NaN.  `epochs` is the configured count (keras History.params["epochs"]).
         self.epochs = epochs
+        # per machine: rows [M], test rows of every fold [M], first test row of fold k [M, K] (its TimeSeriesSplit)
+        self.rows, self.n_test, self.starts = rows, n_test, starts
+        self.init_params = init_params                                         # [S, stride] initial parameters (keep_init_params), or None
         self.epochs_run, self.best_epoch, self.fold_epochs_run, self.fold_best_epoch = epochs_run, best_epoch, fold_epochs_run, fold_best_epoch
         # Keras validation_split: per-epoch loss / accuracy on the held-out tail ([M, epochs]; per CV fold [M, K, epochs]); None without one
         self.val_loss, self.val_acc, self.fold_val_loss, self.fold_val_acc = val_loss, val_acc, fold_val_loss, fold_val_acc
-        self.steps_per_epoch = steps_per_epoch                                 # optimizer steps per epoch of the final fit (keras History.params["steps"])
+        # optimizer steps per epoch of every machine's final fit (keras History.params["steps"]) [M]; steps_per_epoch: machine 0's
+        self.machine_steps = None if steps_per_epoch is None else np.atleast_1d(np.asarray(steps_per_epoch, dtype=np.int64))
+        self.steps_per_epoch = None if steps_per_epoch is None else int(self.machine_steps[0])
         # float64 scale_ / min_ of the MinMaxScaler in front of the network ([M, T]; per CV fold [M, K, T]); None without one
         self.in_scale, self.in_offset, self.fold_in_scale, self.fold_in_offset = in_scale, in_offset, fold_in_scale, fold_in_offset
         self.eng, self.n_machines, self.n_splits = eng, n_machines, n_splits
@@ -235,12 +240,13 @@ class FleetBuild:
         if self.val_loss is not None:  # the keys and their order of the per-machine History
             hist["val_loss"] = [float(v) for v in self.val_loss[m].cpu().numpy()]
             hist["val_accuracy"] = [float(v) for v in self.val_acc[m].cpu().numpy()]
+        steps = None if self.machine_steps is None else int(self.machine_steps[m])
         if self.epochs_run is None:
-            ae._history = History(hist, {"verbose": 0, "epochs": len(hist["loss"]), "steps": self.steps_per_epoch}, list(range(len(hist["loss"]))))
+            ae._history = History(hist, {"verbose": 0, "epochs": len(hist["loss"]), "steps": steps}, list(range(len(hist["loss"]))))
         else:  # as the per-machine fit loop leaves it: the epochs run, against the configured count
             ran = int(self.epochs_run[m])
             hist = {k: v[:ran] for k, v in hist.items()}
-            ae._history = History(hist, {"verbose": 0, "epochs": int(self.epochs), "steps": self.steps_per_epoch}, list(range(ran)))
+            ae._history = History(hist, {"verbose": 0, "epochs": int(self.epochs), "steps": steps}, list(range(ran)))
         sc = self._fill_minmax(MinMaxScaler(), self.scale[m].cpu().numpy().astype(np.float64), self.offset[m].cpu().numpy().astype(np.float64), None)
         if template is not None:
             det = template
@@ -323,17 +329,61 @@ def _fit_slots(eng, params, fit_jobs, n_jobs, max_rows, x, y, split, row_map, n_
     return hist, acc, val_loss, val_acc, epochs_run, best_epoch
 
 
-def build_fleet(eng: "engine.FFEngine", x, y, rows: int, epochs: int = 1, batch_size: int = 32, n_splits: int = 3, seed: int = 0,
+def _machine_rows(x, rows):
+    """
+    (row counts [M], first rows [M]) of the machines stacked in ``x``: ``rows`` is an int, M = len(x) // rows machines of that
+    many rows each, or one count per machine.  Machine m owns rows [row0[m], row0[m] + rows[m]), row0 the prefix sum.
+    """
+    if np.ndim(rows) == 0:
+        n = np.full(x.shape[0] // int(rows), int(rows), dtype=np.int64)
+    else:
+        n = np.asarray(rows, dtype=np.int64)
+        if n.ndim != 1 or len(n) == 0 or (n < 1).any() or int(n.sum()) > x.shape[0]:
+            raise ValueError(f"rows: {n.size} per-machine counts (sum {int(n.sum())}) for {x.shape[0]} stacked rows")
+    return n, _prefix(n)
+
+
+def _prefix(counts) -> np.ndarray:
+    """Exclusive prefix sums (int64): the first row of every block laid out back to back."""
+    return np.concatenate([[0], np.cumsum(counts)[:-1]]).astype(np.int64)
+
+
+def tss_layout(rows, n_splits: int):
+    """
+    Every machine's sklearn ``TimeSeriesSplit(n_splits)`` over its own ``rows[m]`` rows: (test rows [M], starts [M, K]), fold k of
+    machine m training on [0, starts[m, k]) and testing the next test[m] rows.
+    """
+    n, K = np.asarray(rows, dtype=np.int64), int(n_splits)
+    test = n // (K + 1)
+    if (test == 0).any():
+        raise ValueError("Too many splits for number of samples")
+    return test, n[:, None] - (K - np.arange(K))[None, :] * test[:, None]
+
+
+def shuffle_maps(slot_rows):
+    """
+    The row maps of ``DiffBasedAnomalyDetector(shuffle=True)`` for slots of ``slot_rows`` rows: ``sklearn.utils.shuffle(arange(n),
+    random_state=0)`` once per distinct length, back to back (int32), and every slot's offset into them (int64).
+    """
+    lengths = list(dict.fromkeys(int(v) for v in slot_rows))  # in slot order
+    first = dict(zip(lengths, _prefix(lengths)))
+    maps = np.concatenate([sk_shuffle(np.arange(v), random_state=0) for v in lengths]).astype(np.int32)
+    return maps, np.asarray([first[int(v)] for v in slot_rows], dtype=np.int64)
+
+
+def build_fleet(eng: "engine.FFEngine", x, y, rows, epochs: int = 1, batch_size: int = 32, n_splits: int = 3, seed: int = 0,
                 adam: Optional[Dict[str, float]] = None, shuffle: bool = True, generator=None, input_scaler: bool = False,
                 detector_shuffle: bool = False, validation_split: float = 0.0, validation_batch_size: Optional[int] = None,
-                early_stopping=None, loss: str = "mse", optimizer=None) -> FleetBuild:
+                early_stopping=None, loss: str = "mse", optimizer=None, keep_init_params: bool = False) -> FleetBuild:
     """
     The batched form of ``gordo build`` for one architecture bucket: for every machine the 3-fold TimeSeriesSplit
     cross-validation (fit on each prefix, thresholds from the following test block: diff.py:176-266) and the final fit on
     all rows (build_model.py:257-321) -- ``(n_splits + 1) * n_machines`` fits in ONE gb_ffae_fit launch (one CTA per fit),
     then fold scoring, threshold reduction and scaler statistics, each a single launch.
 
-    x, y: device tensors [n_machines * rows, T]; machine m owns rows [m*rows, (m+1)*rows).
+    x, y: device tensors of the machines' rows stacked.  ``rows``: an int, machine m owning rows [m*rows, (m+1)*rows), or one
+    count per machine, machine m owning rows [row0[m], row0[m] + rows[m]) with row0 the prefix sum.  Every machine gets its own
+    TimeSeriesSplit (``test = rows[m] // (n_splits + 1)``), and each fit, scoring and reduction job covers its own slot's rows.
 
     ``input_scaler``: the network sits behind a MinMaxScaler (``Pipeline([MinMaxScaler(), KerasAutoEncoder])``, the shape of
     gordo's example configs, examples/config.yaml:74-81).  Inside cross validation every fold clone fits that scaler on its
@@ -342,7 +392,8 @@ def build_fleet(eng: "engine.FFEngine", x, y, rows: int, epochs: int = 1, batch_
 
     ``detector_shuffle``: ``DiffBasedAnomalyDetector(shuffle=True)``, which hands its estimator its rows in the order of
     ``sklearn.utils.shuffle(X, y, random_state=0)`` (the final fit on all rows, every CV clone on its own prefix).  The fits read
-    the rows through that order (a row map; one per slot length, shared by every machine) instead of a shuffled copy.
+    the rows through that order (a row map; one per distinct slot length, shared by every slot of that length) instead of a
+    shuffled copy.
     ``validation_split``: Keras' hold-out of the estimator: of a slot's ``n`` (shuffled) rows it trains on the first
     ``floor(n * (1 - validation_split))`` and reports the loss and accuracy of the rest after every epoch (``val_loss``,
     ``val_accuracy``; in batches of ``validation_batch_size``, default ``batch_size``), computed inside the same fit launch.
@@ -353,70 +404,68 @@ def build_fleet(eng: "engine.FFEngine", x, y, rows: int, epochs: int = 1, batch_
     result then carries ``epochs_run`` / ``best_epoch``; history entries past a fit's ``epochs_run`` are NaN.
     ``loss``: the estimator's canonical Keras loss name (``FFNetSpec.loss``), trained on and reported by every fit.
     ``optimizer``: None (Adam from ``adam``) or the estimator's (name, record) (``factories.specs.fit_optimizer``), for every fit.
+    ``keep_init_params``: keep the initial parameters of every slot on the result (``init_params``).
     """
     torch = engine._torch()
     dev = eng.device
-    M, K, N = x.shape[0] // rows, n_splits, rows
-    test = N // (K + 1)
-    if test == 0:
-        raise ValueError("Too many splits for number of samples")
-    starts = [N - (K - k) * test for k in range(K)]  # sklearn TimeSeriesSplit: fold k trains on [0, starts[k]), tests the next `test` rows
+    n, row0 = _machine_rows(x, rows)
+    M, K = len(n), n_splits
+    test, starts = tss_layout(n, K)
     g = generator or torch.Generator(device=dev).manual_seed(seed)
     # slots: [0, M) final models, then fold k of machine m at M + k*M + m
-    params = _keras_initial_params(eng, M * (K + 1), g)
-    base = np.arange(M, dtype=np.int64) * N
-    slot_n = [N] + starts  # rows of the final fit, then of fold k
+    S = M * (K + 1)
+    params = _keras_initial_params(eng, S, g)
+    init_params = params.clone() if keep_init_params else None
+    N = int(n.max())                                             # the longest slot
+    slot_n = np.concatenate([n] + [starts[:, k] for k in range(K)])  # every row of a slot: what its scalers see
     vsplit = float(validation_split or 0.0)
-    n_train = [int(math.floor(n * (1.0 - vsplit))) if 0.0 < vsplit < 1.0 else n for n in slot_n]  # keras' split (models.py)
-    if min(n_train) < 1:
-        raise ValueError(f"validation_split {vsplit} leaves the {min(slot_n)}-row slot without a training row")
-    fit_slots = np.concatenate([np.arange(M)] + [M + k * M + np.arange(M) for k in range(K)])
-    all_rows = np.repeat(slot_n, M)     # every row of a slot: what its scalers see
-    fit_rows = np.repeat(n_train, M)    # the positions its optimizer steps visit
-    fit_x = np.concatenate([base] * (K + 1))
+    n_train = np.asarray([int(math.floor(v * (1.0 - vsplit))) if 0.0 < vsplit < 1.0 else int(v) for v in slot_n], dtype=np.int64)  # keras' split
+    if n_train.min() < 1:
+        raise ValueError(f"validation_split {vsplit} leaves the {int(slot_n.min())}-row slot without a training row")
+    held_out = bool((n_train != slot_n).any())
+    fit_x = np.tile(row0, K + 1)                                 # first row of every slot's machine
     split = row_map = None
-    if detector_shuffle or n_train != slot_n:
-        maps = [sk_shuffle(np.arange(n), random_state=0) if detector_shuffle else None for n in slot_n]
-        map_ofs = np.cumsum([0] + slot_n[:-1]) if detector_shuffle else np.full(K + 1, -1)
-        split = engine.make_split(all_rows - fit_rows, np.repeat(map_ofs, M))
+    if detector_shuffle or held_out:
+        map_ofs = np.full(S, -1, dtype=np.int64)
         if detector_shuffle:
-            row_map = torch.from_numpy(np.concatenate(maps).astype(np.int32)).to(dev)
+            maps, map_ofs = shuffle_maps(slot_n)
+            row_map = torch.from_numpy(maps).to(dev)
+        split = engine.make_split(slot_n - n_train, map_ofs)
     in_scale = in_offset = None
     if input_scaler:
-        S = M * (K + 1)
-        prefix_jobs = engine.jobs_to_device(engine.make_jobs(fit_slots, all_rows, fit_x), dev)
+        prefix_jobs = engine.jobs_to_device(engine.make_jobs(np.arange(S), slot_n, fit_x), dev)
         _, _, lo, hi = engine.minmax_fit(prefix_jobs, S, N, x, eng.n_in, S, dev, return_minmax=True)
         lo, span = lo.double(), hi.double() - lo.double()
         span[~(span >= 10 * np.finfo(np.float64).eps)] = 1.0  # sklearn _handle_zeros_in_scale (also catches all-NaN columns)
         in_scale = 1.0 / span
         in_offset = -lo * in_scale
-        # slot s works on its own copy of machine (s mod M)'s rows, at rows [s*N, (s+1)*N) of the replicated arrays
-        copy_jobs = engine.jobs_to_device(engine.make_jobs(np.arange(S), N, fit_x, np.arange(S, dtype=np.int64) * N), dev)
-        x = engine.affine_f64(copy_jobs, S, N, x.double(), in_scale.contiguous(), in_offset.contiguous(), out_rows=S * N)
-        y = y.view(M, N, -1).repeat(K + 1, 1, 1).view(S * N, -1)
-        base_of = lambda k: (M + k * M + np.arange(M, dtype=np.int64)) * N  # noqa: E731
-        fit_x = np.arange(S, dtype=np.int64) * N
-    else:
-        base_of = lambda k: base  # noqa: E731
-    fit_jobs = engine.jobs_to_device(engine.make_jobs(fit_slots, fit_rows, fit_x), dev)
+        # slot s works on its own copy of its machine's rows: the stacked machines repeated K + 1 times, slot s at copy0[s]
+        total = int(n.sum())
+        copy0 = np.arange(K + 1, dtype=np.int64).repeat(M) * total + fit_x
+        copy_jobs = engine.jobs_to_device(engine.make_jobs(np.arange(S), np.tile(n, K + 1), fit_x, copy0), dev)
+        x = engine.affine_f64(copy_jobs, S, N, x.double(), in_scale.contiguous(), in_offset.contiguous(), out_rows=(K + 1) * total)
+        y = y[:total].repeat(K + 1, 1)
+        fit_x = copy0
+    fit_jobs = engine.jobs_to_device(engine.make_jobs(np.arange(S), n_train, fit_x), dev)
     hist, acc, val_loss, val_acc, epochs_run, best_epoch = _fit_slots(
-        eng, params, fit_jobs, len(fit_slots), N, x, y, split, row_map, M, epochs, batch_size, shuffle, adam, seed, validation_batch_size, early_stopping,
+        eng, params, fit_jobs, S, N, x, y, split, row_map, M, epochs, batch_size, shuffle, adam, seed, validation_batch_size, early_stopping,
         loss, optimizer)
-    if n_train == slot_n:  # nothing held out
+    if not held_out:
         val_loss = val_acc = None
     # scalers: final on all rows, fold k on its training prefix (diff.py:173 inside each CV clone), held-out rows included
-    all_jobs = fit_jobs if n_train == slot_n else engine.jobs_to_device(engine.make_jobs(fit_slots, all_rows, fit_x), dev)
-    scale, offset = eng.minmax_fit(all_jobs, len(fit_slots), N, y, M * (K + 1))
-    # fold scoring on the test blocks: compact output rows [(k*M + m)*test, ...)
-    sc_slots = np.concatenate([M + k * M + np.arange(M) for k in range(K)])
-    sc_x = np.concatenate([base_of(k) + starts[k] for k in range(K)])
-    sc_out = np.arange(K * M, dtype=np.int64) * test
-    sc_jobs = engine.jobs_to_device(engine.make_jobs(sc_slots, test, sc_x, sc_out), dev)
-    res = eng.infer_score(params, sc_jobs, K * M, test, x, y, scale, out_rows=K * M * test, want=("tag-anomaly-unscaled", "total-anomaly-scaled"))
-    feat, agg = eng.thresholds(sc_jobs, K * M, test, res["tag-anomaly-unscaled"], res["total-anomaly-scaled"], M * (K + 1), window=6)
+    all_jobs = engine.jobs_to_device(engine.make_jobs(np.arange(S), slot_n, fit_x), dev) if held_out else fit_jobs
+    scale, offset = eng.minmax_fit(all_jobs, S, N, y, S)
+    # fold scoring on the test blocks: job k*M + m scores fold k of machine m, outputs back to back
+    KM = K * M
+    fk, fm = np.repeat(np.arange(K), M), np.tile(np.arange(M), K)
+    sc_n = test[fm]
+    sc_jobs = engine.jobs_to_device(engine.make_jobs(M + np.arange(KM), sc_n, fit_x[M:] + starts[fm, fk], _prefix(sc_n)), dev)
+    max_test = int(test.max())
+    res = eng.infer_score(params, sc_jobs, KM, max_test, x, y, scale, out_rows=int(sc_n.sum()), want=("tag-anomaly-unscaled", "total-anomaly-scaled"))
+    feat, agg = eng.thresholds(sc_jobs, KM, max_test, res["tag-anomaly-unscaled"], res["total-anomaly-scaled"], S, window=6)
     T = eng.n_out
     # the evaluation metrics of ModelBuilder's cross validation (build_model.py:250-289) reduce to five sums per (fold, tag)
-    moments = engine.cv_moments(sc_jobs, K * M, res["model-output"], y, T).view(K, M, 5, T).permute(1, 0, 2, 3).contiguous()
+    moments = engine.cv_moments(sc_jobs, KM, res["model-output"], y, T).view(K, M, 5, T).permute(1, 0, 2, 3).contiguous()
     fold_params = params[M:].view(K, M, -1).permute(1, 0, 2).contiguous()
     fold_feat = feat[M:].view(K, M, T).permute(1, 0, 2).contiguous()
     fold_agg = agg[M:].view(K, M).t().contiguous()
@@ -429,11 +478,12 @@ def build_fleet(eng: "engine.FFEngine", x, y, rows: int, epochs: int = 1, batch_
                       in_scale=None if in_scale is None else in_scale[:M].contiguous(), in_offset=None if in_offset is None else in_offset[:M].contiguous(),
                       fold_in_scale=None if in_scale is None else in_scale[M:].view(K, M, -1).permute(1, 0, 2).contiguous(),
                       fold_in_offset=None if in_offset is None else in_offset[M:].view(K, M, -1).permute(1, 0, 2).contiguous(),
-                      steps_per_epoch=(n_train[0] + int(batch_size) - 1) // int(batch_size),
+                      steps_per_epoch=(n_train[:M] + int(batch_size) - 1) // int(batch_size),
                       val_loss=None if val_loss is None else val_loss[:M], val_acc=None if val_acc is None else val_acc[:M],
                       fold_val_loss=folds(val_loss), fold_val_acc=folds(val_acc), epochs=int(epochs),
                       epochs_run=None if epochs_run is None else epochs_run[:M], best_epoch=None if best_epoch is None else best_epoch[:M],
-                      fold_epochs_run=fold_jobs(epochs_run), fold_best_epoch=fold_jobs(best_epoch))
+                      fold_epochs_run=fold_jobs(epochs_run), fold_best_epoch=fold_jobs(best_epoch), rows=n, n_test=test, starts=starts,
+                      init_params=init_params)
 
 
 # ------------------------------------------------------------------------------------------------ fleet build of LSTM detectors
@@ -470,10 +520,15 @@ class LSTMFleetBuild:
         # the callback.  History entries past a fit's epochs_run are NaN.  `epochs` is the configured count (History.params["epochs"]).
         self.epochs = epochs
         self.epochs_run, self.best_epoch, self.fold_epochs_run, self.fold_best_epoch = epochs_run, best_epoch, fold_epochs_run, fold_best_epoch
-        self.eng, self.n_machines, self.n_splits, self.rows = eng, n_machines, n_splits, rows
+        self.eng, self.n_machines, self.n_splits = eng, n_machines, n_splits
+        self.rows = np.asarray(rows, dtype=np.int64)          # [M] rows of every machine
         self.lookahead, self.batch_size = lookahead, batch_size
-        self.steps_per_epoch = math.ceil((rows - eng.lookback + 1 - lookahead) / batch_size)  # of the final fit (History.params["steps"])
-        self.starts, self.n_test = starts, n_test            # first test row of every fold; predictions per test block
+        # optimizer steps per epoch of every machine's final fit (History.params["steps"]) [M]; steps_per_epoch: machine 0's
+        self.machine_steps = -(-(self.rows - eng.lookback + 1 - lookahead) // batch_size)
+        self.steps_per_epoch = int(self.machine_steps[0])
+        # per machine: first test row of every fold [M, K] and predictions per test block [M]; starts / n_test: machine 0's
+        self.machine_starts, self.machine_n_test = np.asarray(starts, dtype=np.int64), np.asarray(n_test, dtype=np.int64)
+        self.starts, self.n_test = [int(v) for v in self.machine_starts[0]], int(self.machine_n_test[0])
         self.params, self.fold_params, self.init_params = params, fold_params, init_params  # device float32 ([S, stride] or None)
         self.loss, self.acc, self.fold_loss, self.fold_acc = loss, acc, fold_loss, fold_acc   # [M, epochs], [M, K, epochs]
         # float64 column extrema of the targets (final fit on all rows, fold k on its training prefix): the detector scalers
@@ -483,7 +538,7 @@ class LSTMFleetBuild:
         self.feat_thr, self.agg_thr = feat_thr, agg_thr                                # [M, T], [M] float64 (last fold)
         self.fold_feat_thr, self.fold_agg_thr = fold_feat_thr, fold_agg_thr            # [M, K, T], [M, K] float64
         self.cv_moments = cv_moments                                                   # [M, K, 5, T] float64
-        self.fold_predictions = fold_predictions                                       # [M, K, n_test, T] float32 (device)
+        self.fold_predictions = fold_predictions          # fold_predictions[m, k]: [machine_n_test[m], T] float32 (device)
 
     def detector(self, m: int, tags=None, template=None, input_tags=None):
         """
@@ -514,7 +569,7 @@ class LSTMFleetBuild:
             if spec.key() != ("lstm", eng.n_features, tuple(eng.units), tuple(eng.acts), T, eng.out_func, eng.lookback):
                 raise ValueError("template architecture differs from the fleet's")
             if isinstance(est, Pipeline):
-                _fill_minmax_from_extrema(est.steps[0][1], self.in_min[m], self.in_max[m], self.rows, input_tags)
+                _fill_minmax_from_extrema(est.steps[0][1], self.in_min[m], self.in_max[m], self.rows[m], input_tags)
         else:
             cls = KerasLSTMForecast if self.lookahead else KerasLSTMAutoEncoder
             lstm = cls(kind="lstm_model", lookback_window=eng.lookback, batch_size=self.batch_size, encoding_dim=tuple(eng.units),
@@ -527,13 +582,13 @@ class LSTMFleetBuild:
         if "accuracy" in spec.metrics:
             hist["accuracy"] = [float(v) for v in self.acc[m]]
         if self.epochs_run is None:
-            lstm._history = History(hist, {"verbose": 0, "epochs": len(hist["loss"]), "steps": self.steps_per_epoch}, list(range(len(hist["loss"]))))
+            lstm._history = History(hist, {"verbose": 0, "epochs": len(hist["loss"]), "steps": int(self.machine_steps[m])}, list(range(len(hist["loss"]))))
         else:  # as the per-machine fit loop leaves it: the epochs run, against the configured count
             ran = int(self.epochs_run[m])
             hist = {k: v[:ran] for k, v in hist.items()}
-            lstm._history = History(hist, {"verbose": 0, "epochs": int(self.epochs), "steps": self.steps_per_epoch}, list(range(ran)))
+            lstm._history = History(hist, {"verbose": 0, "epochs": int(self.epochs), "steps": int(self.machine_steps[m])}, list(range(ran)))
         lstm.model.history = lstm._history
-        _fill_minmax_from_extrema(det.scaler, self.y_min[m], self.y_max[m], self.rows, tags)
+        _fill_minmax_from_extrema(det.scaler, self.y_min[m], self.y_max[m], self.rows[m], tags)
         det.feature_thresholds_ = pd.Series(self.feat_thr[m].copy(), index=tags, name=f"fold-{K - 1}")
         det.aggregate_threshold_ = float(self.agg_thr[m])
         det.feature_thresholds_per_fold_ = pd.DataFrame(self.fold_feat_thr[m].copy(), columns=tags, index=[f"fold-{k}" for k in range(K)])
@@ -545,7 +600,19 @@ class LSTMFleetBuild:
         return det
 
 
-def build_lstm_fleet(eng: "engine.LSTMEngine", x, y, rows: int, lookahead: int = 0, epochs: int = 1, batch_size: int = 32, n_splits: int = 3,
+class _FoldBlocks:
+    """``blocks[m, k]``: the rows of fold k of machine m in an array of per-job blocks laid out back to back (job k*M + m)."""
+
+    def __init__(self, arr, first, count, n_machines):
+        self.arr, self.first, self.count, self.M = arr, first, count, n_machines
+
+    def __getitem__(self, mk):
+        m, k = mk
+        j = k * self.M + m
+        return self.arr[int(self.first[j]) : int(self.first[j] + self.count[j])]
+
+
+def build_lstm_fleet(eng: "engine.LSTMEngine", x, y, rows, lookahead: int = 0, epochs: int = 1, batch_size: int = 32, n_splits: int = 3,
                      seed: int = 0, adam: Optional[Dict[str, float]] = None, input_scaler: bool = False, memory_budget: int = 8 << 30,
                      keep_init_params: bool = False, generator=None, loss: str = "mse", optimizer=None, early_stopping=None) -> LSTMFleetBuild:
     """
@@ -554,13 +621,16 @@ def build_lstm_fleet(eng: "engine.LSTMEngine", x, y, rows: int, lookahead: int =
     ``(n_splits + 1) * n_machines`` jobs of gb_lstm_fit (primer step, ordered batches), then one gb_lstm_infer(_tc) launch for
     every fold model's test block and float64 scoring, thresholds, scaler extrema and metric moments, one launch each.
 
-    x, y: float64 device tensors [n_machines * rows, T]; machine m owns rows [m*rows, (m+1)*rows).  ``y`` may be ``x``.
+    x, y: float64 device tensors of the machines' rows stacked; ``rows`` an int (machine m owns rows [m*rows, (m+1)*rows)) or one
+    count per machine (machine m owns rows [row0[m], row0[m] + rows[m]), row0 the prefix sum).  ``y`` may be ``x``.  Every machine
+    gets its own TimeSeriesSplit, windows and test blocks; a fit launch steps its jobs in lockstep up to its longest one.
 
     ``batch_size``: up to 32 windows on gb_lstm_fit, up to 256 on gb_lstm_fit_tc (``LSTMEngine.fit_for_batch``).
     ``memory_budget``: bytes of fit workspace (gb_lstm_fit_workspace_bytes, or gb_lstm_fit_tc_workspace_bytes at the batch size)
     one fit launch may take.  Machines are
     trained in chunks that fit it -- all ``n_splits + 1`` fits of a machine in the same chunk; every job's result is the same
-    whatever the chunking.  ``keep_init_params``: keep the initial parameters of every slot on the result (``init_params``).
+    whatever the chunking.  Chunks take the machines shortest first, so each chunk's lockstep loop runs close to its own
+    longest machine.  ``keep_init_params``: keep the initial parameters of every slot on the result (``init_params``).
     ``loss``: the estimator's canonical Keras loss name (``LSTMNetSpec.loss``).  ``optimizer``: as in ``build_fleet``.
     ``early_stopping``: the estimator's Keras ``EarlyStopping`` callback -- one for every machine, or a sequence of one per machine
     (``engine.make_stop`` takes any form).  Every slot of machine m, the final fit and each CV fold, applies m's rule at the end of
@@ -572,24 +642,24 @@ def build_lstm_fleet(eng: "engine.LSTMEngine", x, y, rows: int, lookahead: int =
     dev = eng.device
     if x.dtype != torch.float64 or y.dtype != torch.float64:
         raise ValueError(f"build_lstm_fleet takes float64 x and y, got {x.dtype} / {y.dtype}")
-    M, K, N, T = x.shape[0] // rows, int(n_splits), int(rows), eng.n_out
+    n, row0 = _machine_rows(x, rows)
+    M, K, T = len(n), int(n_splits), eng.n_out
+    N = int(n.max())                                 # the longest machine
     L, la = eng.lookback, int(lookahead)
-    test = N // (K + 1)
-    if test == 0:
-        raise ValueError("Too many splits for number of samples")
-    starts = [N - (K - k) * test for k in range(K)]  # sklearn TimeSeriesSplit: fold k trains on [0, starts[k]), tests the next `test` rows
-    train_rows = [N] + starts                        # final fit, then fold k
-    windows = [n - L + 1 - la for n in train_rows]   # the estimator's window count
-    n_test = test - L + 1 - la                       # predictions per test block
-    if min(windows) < 1 or starts[0] <= L or n_test < 1:
-        raise ValueError(f"{N} rows leave fold 0 without a training window or a test block without a prediction at lookback_window {L}, lookahead {la}")
+    test, starts = tss_layout(n, K)
+    n_test = test - L + 1 - la                       # predictions per test block, per machine
+    for m in range(M):
+        if starts[m, 0] - L + 1 - la < 1 or starts[m, 0] <= L or n_test[m] < 1:
+            raise ValueError(f"{int(n[m])} rows leave fold 0 without a training window or a test block without a prediction at lookback_window {L}, "
+                             f"lookahead {la}")
     S = M * (K + 1)
     g = generator or torch.Generator(device=dev).manual_seed(int(seed))
     params = eng.initial_params(S, g)
     init_params = params.clone() if keep_init_params else None
-    # per slot: training rows / windows and the first row of its machine
-    slot_rows, slot_windows = np.repeat(train_rows, M).astype(np.int64), np.repeat(windows, M).astype(np.int64)
-    base = np.tile(np.arange(M, dtype=np.int64) * N, K + 1)
+    # per slot (final fits, then fold k of machine m at M + k*M + m): training rows / windows and the first row of its machine
+    slot_rows = np.concatenate([n] + [starts[:, k] for k in range(K)])
+    slot_windows = slot_rows - L + 1 - la            # the estimator's window count
+    base = np.tile(row0, K + 1)
 
     def host(t):
         return t.cpu().numpy()
@@ -607,13 +677,15 @@ def build_lstm_fleet(eng: "engine.LSTMEngine", x, y, rows: int, lookahead: int =
     in_lo = in_hi = None
     if input_scaler:
         # every fold clone fits the Pipeline's MinMaxScaler on its own prefix: slot s trains on its own float64-scaled copy of its
-        # machine's rows, at rows [s*N, (s+1)*N) of the replicated arrays (gb_affine_f64: sklearn's transform, rounded once)
+        # machine's rows -- the stacked machines repeated K + 1 times, slot s at x_row[s] (gb_affine_f64: sklearn's transform,
+        # rounded once)
         in_lo, in_hi = (y_lo, y_hi) if y is x else extrema(x)
         a, b = (torch.from_numpy(np.ascontiguousarray(v)).to(dev) for v in _minmax_attributes(in_lo, in_hi))
-        copy_jobs = engine.jobs_to_device(engine.make_jobs(np.arange(S), N, base, np.arange(S, dtype=np.int64) * N), dev)
-        xf = engine.affine_f64(copy_jobs, S, N, x, a, b, out_rows=S * N)
-        yf = y32.view(M, N, T).repeat(K + 1, 1, 1).view(S * N, T)
-        x_row = np.arange(S, dtype=np.int64) * N
+        total = int(n.sum())
+        x_row = np.arange(K + 1, dtype=np.int64).repeat(M) * total + base
+        copy_jobs = engine.jobs_to_device(engine.make_jobs(np.arange(S), np.tile(n, K + 1), base, x_row), dev)
+        xf = engine.affine_f64(copy_jobs, S, N, x, a, b, out_rows=(K + 1) * total)
+        yf = y32[:total].repeat(K + 1, 1)
     else:
         xf = y32 if y is x else x.to(torch.float32)
         yf, x_row = y32, base
@@ -635,8 +707,9 @@ def build_lstm_fleet(eng: "engine.LSTMEngine", x, y, rows: int, lookahead: int =
     chunk = max(1, min(M, int(memory_budget) // max(per_machine_bytes, 1), 65535 // (K + 1)))
     hist = torch.empty((S, epochs), dtype=torch.float32, device=dev)
     acc = torch.empty_like(hist)
+    by_length = np.argsort(n, kind="stable")
     for m0 in range(0, M, chunk):
-        ms = np.arange(m0, min(M, m0 + chunk))
+        ms = by_length[m0:m0 + chunk]
         slots = np.concatenate([j * M + ms for j in range(K + 1)])
         idx = torch.from_numpy(slots).to(dev)
         p = params.index_select(0, idx)
@@ -652,19 +725,25 @@ def build_lstm_fleet(eng: "engine.LSTMEngine", x, y, rows: int, lookahead: int =
         hist.index_copy_(0, idx, cl)
         acc.index_copy_(0, idx, ca)
 
-    # fold scoring: fold k of machine m (job k*M + m) predicts the windows inside its test block, in one launch
+    # fold scoring: fold k of machine m (job k*M + m) predicts the windows inside its test block, in one launch, outputs back to back
     KM = K * M
     fk, fm = np.repeat(np.arange(K), M), np.tile(np.arange(M), K)
-    test_start = np.asarray(starts, dtype=np.int64)[fk]
-    out0 = np.arange(KM, dtype=np.int64) * n_test
-    infer_jobs = engine.jobs_to_device(engine.make_jobs(M + np.arange(KM), n_test, x_row[M:] + test_start, out0), dev)
-    pred = eng.infer(params, infer_jobs, KM, n_test, xf, KM * n_test)
+    test_start = starts[fm, fk]
+    job_n = n_test[fm]
+    out0 = _prefix(job_n)
+    max_n = int(n_test.max())
+    infer_jobs = engine.jobs_to_device(engine.make_jobs(M + np.arange(KM), job_n, x_row[M:] + test_start, out0), dev)
+    if eng.tc_supported:  # the ragged tile layout: each job costs its own windows (the same bits per window as gb_lstm_infer_tc)
+        tiles = eng.tile_base(job_n)
+        pred = eng.infer(params, infer_jobs, KM, max_n, xf, int(job_n.sum()), tile_base=torch.from_numpy(tiles).to(dev), n_tiles=int(tiles[-1]))
+    else:
+        pred = eng.infer(params, infer_jobs, KM, max_n, xf, int(job_n.sum()))
     # targets tail-aligned to the predictions, scored in float64 as the per-machine detector scores LSTM output (diff.py:350-385)
-    score_jobs = engine.jobs_to_device(engine.make_jobs(np.arange(KM), n_test, fm * N + test_start + L - 1 + la, out0), dev)
+    score_jobs = engine.jobs_to_device(engine.make_jobs(np.arange(KM), job_n, row0[fm] + test_start + L - 1 + la, out0), dev)
     y_scale, _ = _minmax_attributes(y_lo, y_hi)
     fold_scale = torch.from_numpy(np.ascontiguousarray(y_scale[M:])).to(dev)
-    res = engine.anomaly_score(score_jobs, KM, n_test, pred.to(torch.float64), y, T, scale=fold_scale, want=("tag-anomaly-unscaled", "total-anomaly-scaled"))
-    feat, agg = engine.thresholds(score_jobs, KM, n_test, res["tag-anomaly-unscaled"], res["total-anomaly-scaled"], T, KM, 6, dev)
+    res = engine.anomaly_score(score_jobs, KM, max_n, pred.to(torch.float64), y, T, scale=fold_scale, want=("tag-anomaly-unscaled", "total-anomaly-scaled"))
+    feat, agg = engine.thresholds(score_jobs, KM, max_n, res["tag-anomaly-unscaled"], res["total-anomaly-scaled"], T, KM, 6, dev)
     # the evaluation metrics of ModelBuilder's cross validation reduce to five sums per (fold, tag)
     moments = host(engine.cv_moments(score_jobs, KM, pred, y32, T)).reshape(K, M, 5, T).transpose(1, 0, 2, 3)
     fold_feat = host(feat).reshape(K, M, T).transpose(1, 0, 2)
@@ -675,10 +754,10 @@ def build_lstm_fleet(eng: "engine.LSTMEngine", x, y, rows: int, lookahead: int =
         return np.ascontiguousarray(np.swapaxes(a[M:].reshape((K, M) + a.shape[1:]), 0, 1))
 
     return LSTMFleetBuild(
-        eng, M, K, N, la, int(batch_size), starts, n_test, params[:M].contiguous(), params[M:].view(K, M, -1).permute(1, 0, 2).contiguous(),
+        eng, M, K, n, la, int(batch_size), starts, n_test, params[:M].contiguous(), params[M:].view(K, M, -1).permute(1, 0, 2).contiguous(),
         init_params, loss_h[:M], acc_h[:M], folds(loss_h), folds(acc_h), y_lo[:M], y_hi[:M], folds(y_lo), folds(y_hi),
         np.ascontiguousarray(fold_feat[:, K - 1]), np.ascontiguousarray(fold_agg[:, K - 1]), np.ascontiguousarray(fold_feat),
-        np.ascontiguousarray(fold_agg), np.ascontiguousarray(moments), pred.view(K, M, n_test, T).permute(1, 0, 2, 3),
+        np.ascontiguousarray(fold_agg), np.ascontiguousarray(moments), _FoldBlocks(pred, out0, job_n, M),
         in_min=None if in_lo is None else in_lo[:M], in_max=None if in_hi is None else in_hi[:M],
         fold_in_min=None if in_lo is None else folds(in_lo), fold_in_max=None if in_hi is None else folds(in_hi), epochs=int(epochs),
         epochs_run=None if stop is None else epochs_run[:M], best_epoch=None if stop is None else best_epoch[:M],
@@ -697,8 +776,9 @@ class KFoldFleetBuild:
 
     def __init__(self, eng, n_machines, n_splits, rows, n_test, params, init_params, loss, acc, val_loss, val_acc, epochs, epochs_run,
                  best_epoch, slot_steps, y_min, y_max, in_min, in_max, target_scaler, feat_thr, agg_thr, cv_moments):
-        self.eng, self.n_machines, self.n_splits, self.rows = eng, n_machines, n_splits, rows
-        self.n_test = n_test                                  # [K] test rows of every fold (KFold folds differ by one row at most)
+        self.eng, self.n_machines, self.n_splits = eng, n_machines, n_splits
+        self.rows = rows                                      # [M] rows of every machine
+        self.n_test = n_test                                  # [M, K] test rows of every fold (a machine's KFold folds differ by one row at most)
         self.params, self.init_params = params, init_params
         # per slot [S, epochs] (val_* None without a validation_split; NaN past a fit's epochs_run with EarlyStopping)
         self.loss, self.acc, self.val_loss, self.val_acc = loss, acc, val_loss, val_acc
@@ -737,7 +817,8 @@ class KFoldFleetBuild:
         from .machine.model.models import History
 
         eng, M = self.eng, self.n_machines
-        n_rows = self.rows if s < M else self.rows - int(self.n_test[(s - M) // M])  # the rows the slot's scalers saw
+        m = s % M
+        n_rows = int(self.rows[m]) if s < M else int(self.rows[m] - self.n_test[m, (s - M) // M])  # the rows the slot's scalers saw
         T = eng.n_out
         tags = list(tags) if tags is not None else list(range(T))
         det = template
@@ -800,6 +881,26 @@ def kfold_row_maps(trains, inverse, rows: int, detector_shuffle: bool):
     return [inverse[t] for t in orders]
 
 
+def kfold_bucket_maps(cv, rows, detector_shuffle: bool):
+    """
+    The row maps of a K-fold bucket whose machines have ``rows[m]`` rows, made once per distinct length (a KFold split depends only
+    on the length and ``cv``) and laid out back to back.  Returns (n_test [M, K], to_fold, to_time, machine_ofs [M], fit_maps,
+    slot_ofs [S]): machine m's fold-order map (``kfold_layout``'s order) and time-order map (its inverse) start at machine_ofs[m]
+    of to_fold / to_time; slot s (finals, then fold k of machine m at M + k*M + m) reads map j of ``kfold_row_maps`` for its
+    machine's length (j = 0 for the final fit, k + 1 for fold k) at slot_ofs[s] of fit_maps.  Maps are int32, offsets int64.
+    """
+    n = np.asarray(rows, dtype=np.int64)
+    lengths = list(dict.fromkeys(int(v) for v in n))
+    layouts = [kfold_layout(cv, v) for v in lengths]
+    of_length = np.asarray([lengths.index(int(v)) for v in n], dtype=np.int64)
+    n_test = np.asarray([[len(t) for t in layouts[i][0]] for i in of_length], dtype=np.int64).reshape(len(n), -1)
+    maps = [kfold_row_maps(lay[1], lay[3], v, detector_shuffle) for lay, v in zip(layouts, lengths)]
+    fit_ofs = _prefix([len(mp) for per_length in maps for mp in per_length]).reshape(len(lengths), -1)
+    i32 = lambda parts: np.concatenate(parts).astype(np.int32)  # noqa: E731
+    return (n_test, i32([lay[2] for lay in layouts]), i32([lay[3] for lay in layouts]), _prefix(lengths)[of_length],
+            i32([mp for per_length in maps for mp in per_length]), fit_ofs[of_length].T.reshape(-1))
+
+
 def combine_fold_extrema(lo, hi):
     """
     Column extrema per slot from those of the K test blocks (``lo`` / ``hi``: [K, M, T]): the final slot's over all blocks, fold
@@ -817,7 +918,7 @@ def combine_fold_extrema(lo, hi):
     return s_lo, s_hi
 
 
-def build_kfold_fleet(eng: "engine.FFEngine", x, y, rows: int, cv, epochs: int = 1, batch_size: int = 32, seed: int = 0,
+def build_kfold_fleet(eng: "engine.FFEngine", x, y, rows, cv, epochs: int = 1, batch_size: int = 32, seed: int = 0,
                       adam: Optional[Dict[str, float]] = None, shuffle: bool = True, generator=None, input_scaler: bool = False,
                       target_scaler: bool = False, detector_shuffle: bool = False, validation_split: float = 0.0,
                       validation_batch_size: Optional[int] = None, early_stopping=None, window: Optional[int] = None,
@@ -829,11 +930,13 @@ def build_kfold_fleet(eng: "engine.FFEngine", x, y, rows: int, cv, epochs: int =
     fit launch -- then every fold model's test block scored in one launch, the errors brought back to time order, smoothed and
     reduced to the ``threshold_percentile`` quantile, and the CV metric moments.
 
-    x, y: float64 device tensors [n_machines * rows, T]; machine m owns rows [m*rows, (m+1)*rows).  ``y`` may be ``x``.
+    x, y: float64 device tensors of the machines' rows stacked; ``rows`` an int (machine m owns rows [m*rows, (m+1)*rows)) or one
+    count per machine (machine m owns rows [row0[m], row0[m] + rows[m]), row0 the prefix sum).  ``y`` may be ``x``.
 
-    Every machine of a bucket has the same rows, so the KFold split and every row map are the same for all of them.  x and y are
-    laid out once in fold order (the folds' test rows one after the other, gb_gather_rows), where fold k's test rows are one
-    contiguous block; the fits read their rows through K + 1 shared maps.  ``input_scaler``: the network is behind a MinMaxScaler
+    A KFold split depends only on the row count and ``cv``, so the split and its row maps are made once per distinct length and
+    shared by every machine of that length.  x and y are laid out once in fold order (each machine's folds' test rows one after
+    the other, gb_gather_rows_ragged with each job pointing at its machine's map), where fold k's test rows are one contiguous
+    block; the fits read their rows through the K + 1 maps of their machine's length.  ``input_scaler``: the network is behind a MinMaxScaler
     (``Pipeline([MinMaxScaler(), KerasAutoEncoder])``); ``target_scaler``: the estimator is ``TransformedTargetRegressor(transformer=
     MinMaxScaler(), regressor=...)``, so every slot trains on its own MinMax-scaled targets and the fold models' predictions are
     mapped back by sklearn's float32 inverse and scored in float64 in one pass (gb_minmax_inverse_score_f64), as the per-machine
@@ -847,32 +950,38 @@ def build_kfold_fleet(eng: "engine.FFEngine", x, y, rows: int, cv, epochs: int =
         raise ValueError(f"build_kfold_fleet takes float64 x and y, got {x.dtype} / {y.dtype}")
     x, y = x.contiguous(), (None if y is x else y.contiguous())
     y = x if y is None else y
-    M, N, T = x.shape[0] // rows, int(rows), eng.n_out
-    tests, trains, order, inverse = kfold_layout(cv, N)
-    K, S, KM = len(tests), M * (len(tests) + 1), M * len(tests)
-    n_test = np.asarray([len(t) for t in tests], dtype=np.int64)
-    o = np.concatenate([[0], np.cumsum(n_test)[:-1]])           # first fold-order row of fold k's test block
+    n, row0 = _machine_rows(x, rows)
+    M, N, T = len(n), int(n.max()), eng.n_out
+    total = int(n.sum())
+    n_test, to_fold, to_time, machine_ofs, fit_maps, slot_map = kfold_bucket_maps(cv, n, detector_shuffle)
+    K = n_test.shape[1]
+    S, KM = M * (K + 1), M * K
+    o = np.cumsum(n_test, axis=1) - n_test                      # first fold-order row of fold k's test block in machine m's rows
     max_test = int(n_test.max())
-    base = np.arange(M, dtype=np.int64) * N
 
     def i32(a):
         return torch.from_numpy(np.ascontiguousarray(a, dtype=np.int32)).to(dev)
 
-    def jobs(slots, n, x_row, out_row=None):
-        return engine.jobs_to_device(engine.make_jobs(slots, n, x_row, out_row), dev)
+    def i64(a):
+        return torch.from_numpy(np.ascontiguousarray(a, dtype=np.int64)).to(dev)
+
+    def jobs(slots, rows_, x_row, out_row=None):
+        return engine.jobs_to_device(engine.make_jobs(slots, rows_, x_row, out_row), dev)
 
     def f64(a):
         return torch.from_numpy(np.ascontiguousarray(a, dtype=np.float64)).to(dev)
 
+    to_fold, to_time = i32(to_fold), i32(to_time)
+
     # 1. fold order: one gather per array
-    whole = jobs(np.arange(M), N, base)
-    to_fold = i32(order)
-    xq = engine.gather_rows(whole, M, N, to_fold, x, M * N)
-    yq = xq if y is x else engine.gather_rows(whole, M, N, to_fold, y, M * N)
+    whole = jobs(np.arange(M), n, row0)
+    per_machine = i64(machine_ofs)
+    xq = engine.gather_rows(whole, M, N, to_fold, x, total, map_ofs=per_machine)
+    yq = xq if y is x else engine.gather_rows(whole, M, N, to_fold, y, total, map_ofs=per_machine)
 
     # 2. scaler extrema: one reduction over the K*M test blocks (job k*M + m), combined per slot on the host
     fk, fm = np.repeat(np.arange(K), M), np.tile(np.arange(M), K)
-    blocks = jobs(np.arange(KM), n_test[fk], fm * N + o[fk])
+    blocks = jobs(np.arange(KM), n_test[fm, fk], row0[fm] + o[fm, fk])
 
     def slot_extrema(a):
         lo, hi = (t.cpu().numpy().reshape(K, M, -1) for t in engine.minmax_f64(blocks, KM, max_test, a, KM))
@@ -887,65 +996,68 @@ def build_kfold_fleet(eng: "engine.FFEngine", x, y, rows: int, cv, epochs: int =
     if input_scaler:
         in_lo, in_hi = (y_lo, y_hi) if y is x else slot_extrema(xq)
 
-    # 3. the fits' inputs: with a scaler in front of the network or on the targets, slot s owns rows [s*N, (s+1)*N) of x and y
+    # 3. the fits' inputs: with a scaler in front of the network or on the targets, slot s owns its own copy of its machine's rows
+    # (the stacked machines repeated K + 1 times, slot s at slot_x[s])
     per_slot = input_scaler or target_scaler
-    slot_x = np.arange(S, dtype=np.int64) * N if per_slot else np.tile(base, K + 1)  # first row of slot s in x / y
-    machine_of = np.tile(base, K + 1)
-    copy_jobs = jobs(np.arange(S), N, machine_of, slot_x)
+    machine_of = np.tile(row0, K + 1)
+    slot_x = np.arange(K + 1, dtype=np.int64).repeat(M) * total + machine_of if per_slot else machine_of  # first row of slot s in x / y
+    slot_rows = np.tile(n, K + 1)
+    copy_jobs = jobs(np.arange(S), slot_rows, machine_of, slot_x)
+    per_slot_ofs = i64(np.tile(machine_ofs, K + 1))
     if input_scaler:
         a, b = _minmax_attributes(in_lo, in_hi)
-        xf = engine.affine_f64(copy_jobs, S, N, xq, f64(a), f64(b), out_rows=S * N)
-    else:
-        xf = engine.gather_rows(copy_jobs if per_slot else whole, S if per_slot else M, N, to_fold, x, S * N if per_slot else M * N, to_f32=True)
-    if target_scaler:
-        yf = xf if (input_scaler and y is x) else engine.affine_f64(copy_jobs, S, N, yq, f64(y_scale), f64(y_offset), out_rows=S * N)
+        xf = engine.affine_f64(copy_jobs, S, N, xq, f64(a), f64(b), out_rows=(K + 1) * total)
     elif per_slot:
-        yf = engine.gather_rows(copy_jobs, S, N, to_fold, y, S * N, to_f32=True)
+        xf = engine.gather_rows(copy_jobs, S, N, to_fold, x, (K + 1) * total, to_f32=True, map_ofs=per_slot_ofs)
     else:
-        yf = xf if y is x else engine.gather_rows(whole, M, N, to_fold, y, M * N, to_f32=True)
+        xf = engine.gather_rows(whole, M, N, to_fold, x, total, to_f32=True, map_ofs=per_machine)
+    if target_scaler:
+        yf = xf if (input_scaler and y is x) else engine.affine_f64(copy_jobs, S, N, yq, f64(y_scale), f64(y_offset), out_rows=(K + 1) * total)
+    elif per_slot:
+        yf = engine.gather_rows(copy_jobs, S, N, to_fold, y, (K + 1) * total, to_f32=True, map_ofs=per_slot_ofs)
+    else:
+        yf = xf if y is x else engine.gather_rows(whole, M, N, to_fold, y, total, to_f32=True, map_ofs=per_machine)
 
-    maps = kfold_row_maps(trains, inverse, N, detector_shuffle)
-    slot_n = [N] + [N - int(n) for n in n_test]                    # rows each slot's estimator receives
+    slot_n = np.concatenate([n] + [n - n_test[:, k] for k in range(K)])  # rows each slot's estimator receives
     vsplit = float(validation_split or 0.0)
-    n_train = [int(math.floor(n * (1.0 - vsplit))) if 0.0 < vsplit < 1.0 else n for n in slot_n]  # keras' split (models.py)
-    if min(n_train) < 1:
-        raise ValueError(f"validation_split {vsplit} leaves the {min(slot_n)}-row slot without a training row")
-    map_ofs = np.cumsum([0] + slot_n[:-1])
-    split = engine.make_split(np.repeat(slot_n, M) - np.repeat(n_train, M), np.repeat(map_ofs, M))
-    row_map = i32(np.concatenate(maps))
+    n_train = np.asarray([int(math.floor(v * (1.0 - vsplit))) if 0.0 < vsplit < 1.0 else int(v) for v in slot_n], dtype=np.int64)  # keras' split
+    if n_train.min() < 1:
+        raise ValueError(f"validation_split {vsplit} leaves the {int(slot_n.min())}-row slot without a training row")
+    split = engine.make_split(slot_n - n_train, slot_map)
+    row_map = i32(fit_maps)
     g = generator or torch.Generator(device=dev).manual_seed(seed)
     params = _keras_initial_params(eng, S, g)
     init_params = params.clone() if keep_init_params else None
-    fit_jobs = jobs(np.arange(S), np.repeat(n_train, M), slot_x)
+    fit_jobs = jobs(np.arange(S), n_train, slot_x)
     hist, acc, val_loss, val_acc, epochs_run, best_epoch = _fit_slots(
         eng, params, fit_jobs, S, N, xf, yf, split, row_map, M, epochs, batch_size, shuffle, adam, seed, validation_batch_size, early_stopping,
         loss, optimizer)
-    if n_train == slot_n:  # nothing held out
+    if (n_train == slot_n).all():  # nothing held out
         val_loss = val_acc = None
 
     # 4. fold errors in fold order, by the route the per-machine detector takes (DiffBasedAnomalyDetector._score)
     sc_slots = M + np.arange(KM)
-    out0 = fm * N + o[fk]                                           # fold-order rows of the test block in machine layout
-    sc_jobs = jobs(sc_slots, n_test[fk], slot_x[sc_slots] + o[fk], out0)
+    sc_n = n_test[fm, fk]
+    out0 = row0[fm] + o[fm, fk]                                     # fold-order rows of the test block in machine layout
+    sc_jobs = jobs(sc_slots, sc_n, slot_x[sc_slots] + o[fm, fk], out0)
     mult = (y_scale + y_offset) - y_offset                          # _scaler_multiplier: transform(1) - transform(0)
     want = ("tag-anomaly-unscaled", "total-anomaly-scaled")
     if not target_scaler:  # fused predict + score, fp32, with the fold detector's multiplier
-        res = eng.infer_score(params, sc_jobs, KM, max_test, xf, yf, torch.from_numpy(mult.astype(np.float32)).to(dev), out_rows=M * N, want=want)
+        res = eng.infer_score(params, sc_jobs, KM, max_test, xf, yf, torch.from_numpy(mult.astype(np.float32)).to(dev), out_rows=total, want=want)
         pred32, tag_err, tot_err = res["model-output"], res["tag-anomaly-unscaled"], res["total-anomaly-scaled"]
         mom_jobs, y32 = sc_jobs, yf
     else:  # predict, then in one pass sklearn's float32 inverse of the slot's transformer and float64 scoring against the float64 targets
-        pred = eng.infer_score(params, sc_jobs, KM, max_test, xf, out_rows=M * N)["model-output"]
-        mom_jobs = jobs(sc_slots, n_test[fk], out0, out0)
+        pred = eng.infer_score(params, sc_jobs, KM, max_test, xf, out_rows=total)["model-output"]
+        mom_jobs = jobs(sc_slots, sc_n, out0, out0)
         res = engine.minmax_inverse_score_f64(mom_jobs, KM, max_test, pred, yq, f64(y_scale), f64(y_offset), scale=f64(mult), want=want,
-                                              out_rows=M * N)
+                                              out_rows=total)
         pred32, tag_err, tot_err = res["model-output"], res["tag-anomaly-unscaled"], res["total-anomaly-scaled"]
-        y32 = engine.gather_rows(whole, M, N, to_fold, y, M * N, to_f32=True)
+        y32 = engine.gather_rows(whole, M, N, to_fold, y, total, to_f32=True, map_ofs=per_machine)
 
     # 5. K-fold thresholds: errors back in time order (float32, as the detector stores them), smoothed, the percentile
-    to_time = i32(inverse)
     narrow = tag_err.dtype == torch.float64
-    tag_t = engine.gather_rows(whole, M, N, to_time, tag_err, M * N, to_f32=narrow)
-    tot_t = engine.gather_rows(whole, M, N, to_time, tot_err, M * N, to_f32=narrow)
+    tag_t = engine.gather_rows(whole, M, N, to_time, tag_err, total, to_f32=narrow, map_ofs=per_machine)
+    tot_t = engine.gather_rows(whole, M, N, to_time, tot_err, total, to_f32=narrow, map_ofs=per_machine)
     if window is not None and smoothing_method is not None:
         tag_t = engine.smooth(whole, M, tag_t, int(window), smoothing_method, max_rows=N)
         tot_t = engine.smooth(whole, M, tot_t, int(window), smoothing_method, max_rows=N)
@@ -960,6 +1072,6 @@ def build_kfold_fleet(eng: "engine.FFEngine", x, y, rows: int, cv, epochs: int =
         return None if t is None else t.cpu().numpy()
 
     return KFoldFleetBuild(
-        eng, M, K, N, n_test, params, init_params, host(hist), host(acc), host(val_loss), host(val_acc), int(epochs), host(epochs_run),
-        host(best_epoch), (np.repeat(n_train, M) + int(batch_size) - 1) // int(batch_size), y_lo, y_hi, in_lo, in_hi, bool(target_scaler),
+        eng, M, K, n, n_test, params, init_params, host(hist), host(acc), host(val_loss), host(val_acc), int(epochs), host(epochs_run),
+        host(best_epoch), (n_train + int(batch_size) - 1) // int(batch_size), y_lo, y_hi, in_lo, in_hi, bool(target_scaler),
         host(feat).astype(np.float64), host(agg).astype(np.float64), host(moments).reshape(K, M, 5, T).transpose(1, 0, 2, 3).copy())

@@ -262,6 +262,13 @@ int gb_affine_f64(const gb_job* jobs, int32_t n_jobs, int32_t max_rows, const do
 int gb_gather_rows(const gb_job* jobs, int32_t n_jobs, int32_t max_rows, const int32_t* row_map, const void* src, int32_t n_cols,
                    int32_t elem_bytes, int32_t to_f32, void* dst, void* stream);
 
+/* gb_gather_rows with a map per job, for buckets whose machines differ in length (each length has its own KFold split):
+ * dst row out_row + p = src row x_row + row_map[map_ofs[i] + p] for job i and p < n_rows.  map_ofs: DEVICE array [n_jobs] of
+ * offsets into row_map; jobs may share a map.  Element sizes, to_f32, the 16-byte path and the launches per 65 535 jobs as
+ * gb_gather_rows; the same argument checks, and map_ofs must be non-NULL (GB_E_ARG), all before any launch. */
+int gb_gather_rows_ragged(const gb_job* jobs, int32_t n_jobs, int32_t max_rows, const int32_t* row_map, const int64_t* map_ofs,
+                          const void* src, int32_t n_cols, int32_t elem_bytes, int32_t to_f32, void* dst, void* stream);
+
 /* MinMaxScaler.inverse_transform of float32 predictions, as sklearn does it inside TransformedTargetRegressor.predict: the
  * array stays float32 and each in-place step rounds to it, t = (float)((double)p - min_), v = (float)((double)t / scale_).
  * p indexed by x_row, outputs by out_row; scale / min_: [n_slots][n_cols] double.  out_f32 gets v, out_f64 gets (double)v;
