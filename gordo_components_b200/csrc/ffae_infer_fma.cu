@@ -180,11 +180,13 @@ __global__ void __launch_bounds__(THREADS) ffae_infer_fma_kernel(const Args a) {
     const float* sc = a.scale ? a.scale + (long)job.slot * n_out : nullptr;
     const float* ft = a.feat_thr ? a.feat_thr + (long)job.slot * n_out : nullptr;
     const bool totals = score && (a.o_tots || a.o_totu || a.o_totconf);
-    if (totals && tid < 2 * ROWS) rowsum[tid] = 0.f;
-    if (totals) __syncthreads();
     const int g4 = n_out >> 2;
     const bool vec = (n_out & 3) == 0;
     const bool pow2 = vec && g4 <= 32 && (g4 & (g4 - 1)) == 0;
+    // Per-row totals.  pow2: a row's groups of 4 are one aligned segment of a warp, summed by shuffles.  Otherwise each |yhat - y|
+    // is parked in the free activation buffer and the row's thread sums them in column order after the barrier: a row's totals do
+    // not depend on where in a tile, or in which launch, it lands (a request alone and in a coalesced batch score the same bits).
+    float* const dpark = out;
     if (vec) {
       const int limit = nrows * g4;
       const int limit_up = (limit + THREADS - 1) / THREADS * THREADS;
@@ -201,6 +203,7 @@ __global__ void __launch_bounds__(THREADS) ffae_infer_fma_kernel(const Args a) {
             float4 d;
             d.x = fabsf(yh.x - yt.x); d.y = fabsf(yh.y - yt.y); d.z = fabsf(yh.z - yt.z); d.w = fabsf(yh.w - yt.w);
             if (a.o_tu) *reinterpret_cast<float4*>(a.o_tu + g) = d;
+            if (totals && !pow2) *reinterpret_cast<float4*>(dpark + r * pitch + 4 * j4) = d;
             su = d.x * d.x + d.y * d.y + d.z * d.z + d.w * d.w;
             if (sc) {
               const float4 s4 = __ldg(reinterpret_cast<const float4*>(sc) + j4);
@@ -217,17 +220,12 @@ __global__ void __launch_bounds__(THREADS) ffae_infer_fma_kernel(const Args a) {
             }
           }
         }
-        if (totals) {
-          if (pow2) {
-            for (int o = g4 >> 1; o > 0; o >>= 1) {
-              ss += __shfl_xor_sync(0xffffffffu, ss, o);
-              su += __shfl_xor_sync(0xffffffffu, su, o);
-            }
-            if (live && j4 == 0) { rowsum[r] = ss; rowsum[ROWS + r] = su; }
-          } else if (live) {
-            atomicAdd(&rowsum[r], ss);
-            atomicAdd(&rowsum[ROWS + r], su);
+        if (totals && pow2) {
+          for (int o = g4 >> 1; o > 0; o >>= 1) {
+            ss += __shfl_xor_sync(0xffffffffu, ss, o);
+            su += __shfl_xor_sync(0xffffffffu, su, o);
           }
+          if (live && j4 == 0) { rowsum[r] = ss; rowsum[ROWS + r] = su; }
         }
       }
     } else {
@@ -242,9 +240,8 @@ __global__ void __launch_bounds__(THREADS) ffae_infer_fma_kernel(const Args a) {
           if (sc) {
             const float e = d * __ldg(sc + j);
             if (a.o_ts) a.o_ts[g] = e;
-            if (totals) atomicAdd(&rowsum[r], e * e);
           }
-          if (totals) atomicAdd(&rowsum[ROWS + r], d * d);
+          if (totals) dpark[r * pitch + j] = d;
           if (a.o_conf) a.o_conf[g] = d / __ldg(ft + j);
         }
       }
@@ -252,7 +249,20 @@ __global__ void __launch_bounds__(THREADS) ffae_infer_fma_kernel(const Args a) {
     __syncthreads();
     if (totals && tid < nrows) {
       const float inv = 1.f / (float)n_out;
-      const float ts = rowsum[tid] * inv, tu = rowsum[ROWS + tid] * inv;
+      float ss = 0.f, su = 0.f;
+      if (pow2) {
+        ss = rowsum[tid];
+        su = rowsum[ROWS + tid];
+      } else {
+        const float* dr = dpark + tid * pitch;
+        for (int j = 0; j < n_out; ++j) su = fmaf(dr[j], dr[j], su);
+        if (sc)
+          for (int j = 0; j < n_out; ++j) {
+            const float e = dr[j] * __ldg(sc + j);
+            ss = fmaf(e, e, ss);
+          }
+      }
+      const float ts = ss * inv, tu = su * inv;
       if (a.o_tots) a.o_tots[orow + tid] = ts;
       if (a.o_totu) a.o_totu[orow + tid] = tu;
       if (a.o_totconf) a.o_totconf[orow + tid] = ts / __ldg(a.agg_thr + job.slot);

@@ -159,16 +159,20 @@ def test_nan_targets_never_improve_and_val_monitors_never_stop(engine, torch, B)
 
 @pytest.mark.parametrize("B", [16, 64])
 def test_no_step_kernel_runs_once_every_job_has_stopped(engine, torch, B):
-    from torch.profiler import ProfilerActivity, profile
+    from torch.profiler import ProfilerActivity, profile, schedule
 
     eng, params, jobs, nwin, x, y = _setup(engine, torch, [90, 90], seed=4)
     rules = [{"monitor": "loss", "patience": 1, "min_delta": HUGE}] * 2  # both stop after epoch 1
 
     def forward_kernels(run):
+        # one warm-up step traced and discarded, then the counted one: the first CUDA trace of a process can come back without
+        # kernel records while the activity tracer starts up
         torch.cuda.synchronize()
-        with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            run()
-            torch.cuda.synchronize()
+        with profile(activities=[ProfilerActivity.CUDA], schedule=schedule(wait=0, warmup=1, active=1, repeat=1)) as prof:
+            for _ in range(2):
+                run()
+                torch.cuda.synchronize()
+                prof.step()
         return sum(e.count for e in prof.key_averages() if "fwd_kernel" in e.key)
 
     stopped = forward_kernels(lambda: _stop(engine, eng, params, jobs, nwin, x, y, rules, 12, B))
