@@ -59,9 +59,29 @@ def make_optimizer(name: str, cfg) -> GbOptimizer:
     return o
 
 
+class GbDenseReg(C.Structure):
+    _fields_ = [("kernel_l1", C.c_float * GB_MAX_LAYERS), ("kernel_l2", C.c_float * GB_MAX_LAYERS), ("bias_l1", C.c_float * GB_MAX_LAYERS),
+                ("bias_l2", C.c_float * GB_MAX_LAYERS)]
+
+
+REG_FIELDS = ("kernel_l1", "kernel_l2", "bias_l1", "bias_l2")
+
+
+def make_dense_reg(kernel_l1=None, kernel_l2=None, bias_l1=None, bias_l2=None) -> GbDenseReg:
+    """gb_dense_reg of per-layer Keras kernel / bias regularizer coefficients (None or a list per field, zeros where absent)."""
+    r = GbDenseReg()
+    for name, vals in zip(REG_FIELDS, (kernel_l1, kernel_l2, bias_l1, bias_l2)):
+        vals = list(vals or ())
+        if len(vals) > GB_MAX_LAYERS:
+            raise ValueError(f"{name}: {len(vals)} layers is more than {GB_MAX_LAYERS}")
+        for i, v in enumerate(vals):
+            getattr(r, name)[i] = float(v)
+    return r
+
+
 EXPORTS = (
     "gb_abi_version", "gb_last_error", "gb_device_check", "gb_ffnet_param_count", "gb_ffnet_param_stride",
-    "gb_ffae_infer_score", "gb_ffae_tc_supported", "gb_ffae_infer_plan", "gb_ffae_infer_score_x64", "gb_ffae_infer_plan_x64", "gb_anomaly_score", "gb_anomaly_score_f64", "gb_minmax_fit", "gb_minmax_f64", "gb_thresholds", "gb_thresholds_f64", "gb_cv_moments", "gb_smooth", "gb_smooth_scores", "gb_quantile", "gb_affine_f64", "gb_gather_rows", "gb_gather_rows_ragged", "gb_minmax_inverse_f32", "gb_minmax_inverse_score_f64", "gb_ffae_fit_state_stride", "gb_ffae_fit", "gb_ffae_fit_split", "gb_ffae_fit_stop", "gb_ffae_fit_plan", "gb_ffae_fit_opt",
+    "gb_ffae_infer_score", "gb_ffae_tc_supported", "gb_ffae_infer_plan", "gb_ffae_infer_score_x64", "gb_ffae_infer_plan_x64", "gb_anomaly_score", "gb_anomaly_score_f64", "gb_minmax_fit", "gb_minmax_f64", "gb_thresholds", "gb_thresholds_f64", "gb_cv_moments", "gb_smooth", "gb_smooth_scores", "gb_quantile", "gb_affine_f64", "gb_gather_rows", "gb_gather_rows_ragged", "gb_minmax_inverse_f32", "gb_minmax_inverse_score_f64", "gb_ffae_fit_state_stride", "gb_ffae_fit", "gb_ffae_fit_split", "gb_ffae_fit_stop", "gb_ffae_fit_plan", "gb_ffae_fit_opt", "gb_ffae_fit_reg",
     "gb_lstm_param_count", "gb_lstm_param_stride", "gb_lstm_workspace_bytes", "gb_lstm_infer", "gb_lstm_tc_supported", "gb_lstm_tc_workspace_bytes", "gb_lstm_infer_tc", "gb_lstm_tc_ragged_workspace_bytes", "gb_lstm_infer_tc_ragged", "gb_lstm_fit_workspace_bytes", "gb_lstm_fit", "gb_lstm_fit_loss", "gb_lstm_fit_tc_workspace_bytes", "gb_lstm_fit_tc", "gb_lstm_fit_opt", "gb_lstm_fit_tc_opt",
     "gb_lstm_fit_stop_state_bytes", "gb_lstm_fit_stop", "gb_lstm_fit_tc_stop",
     "gb_orthonormal_rows",
@@ -205,6 +225,8 @@ def _declare(lib):
     lib.gb_lstm_fit_tc.restype = C.c_int
     lib.gb_ffae_fit_opt.argtypes = lib.gb_ffae_fit_stop.argtypes[:-1] + [C.POINTER(GbOptimizer), _P]
     lib.gb_ffae_fit_opt.restype = C.c_int
+    lib.gb_ffae_fit_reg.argtypes = lib.gb_ffae_fit_opt.argtypes[:-1] + [C.POINTER(GbDenseReg), _P]
+    lib.gb_ffae_fit_reg.restype = C.c_int
     for name in ("gb_lstm_fit_opt", "gb_lstm_fit_tc_opt"):
         getattr(lib, name).argtypes = lib.gb_lstm_fit_loss.argtypes[:-1] + [C.POINTER(GbOptimizer), _P]
         getattr(lib, name).restype = C.c_int

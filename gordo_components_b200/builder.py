@@ -48,7 +48,7 @@ from sklearn.preprocessing import MinMaxScaler
 
 from . import __version__, serializer
 from .machine.model.base import GordoBase
-from .machine.model.factories.specs import fit_optimizer, optimizer_key
+from .machine.model.factories.specs import fit_optimizer, fit_reg, optimizer_key, reg_key
 from .machine.model.utils import metric_wrapper
 
 logger = logging.getLogger(__name__)
@@ -342,7 +342,7 @@ class _Canonical:
         s = self.spec
         return (tuple(s.dims), tuple(s.acts), tuple(float(v) for v in s.l1), tuple(sorted(s.adam.items())), tuple(s.metrics), s.loss,
                 None if ragged else len(self.X), self.fit["epochs"], self.fit["batch_size"], self.fit["shuffle"], self.n_splits, int(self.evaluation.get("seed", 0)),
-                self.split, self.early_stopping is not None, self.input_scaler) + optimizer_key(s)  # EarlyStopping's parameters are per-job records
+                self.split, self.early_stopping is not None, self.input_scaler) + optimizer_key(s) + reg_key(s)  # EarlyStopping's parameters are per-job records
 
 
 def _default_minmax(scaler) -> bool:
@@ -418,13 +418,14 @@ def _evaluation_refusal(evaluation: dict) -> Optional[str]:
 
 
 def _ff_network(est):
-    """(the KerasAutoEncoder, whether a default MinMaxScaler is in front of it) of a bare AE or ``Pipeline([MinMaxScaler(), AE])``; (None, False) otherwise."""
-    from .machine.model.models import KerasAutoEncoder
+    """(the KerasAutoEncoder or KerasRawModelRegressor, whether a default MinMaxScaler is in front of it) of a bare network or
+    ``Pipeline([MinMaxScaler(), network])``; (None, False) otherwise."""
+    from .machine.model.models import KerasAutoEncoder, KerasRawModelRegressor
 
     input_scaler = False
     if type(est) is Pipeline and len(est.steps) == 2 and _default_minmax(est.steps[0][1]):
         est, input_scaler = est.steps[1][1], True  # Pipeline([MinMaxScaler(), KerasAutoEncoder]): gordo's example config
-    return (est, input_scaler) if type(est) is KerasAutoEncoder else (None, False)
+    return (est, input_scaler) if type(est) in (KerasAutoEncoder, KerasRawModelRegressor) else (None, False)
 
 
 def _early_stopping(fit_args, early_stopping: bool, flag: str):
@@ -759,7 +760,8 @@ class FleetModelBuilder:
                                seed=int(first.evaluation.get("seed", 0)), adam=first.spec.adam, shuffle=first.fit["shuffle"],
                                input_scaler=first.input_scaler, detector_shuffle=first.split[0], validation_split=first.split[1],
                                validation_batch_size=first.split[2],
-                               early_stopping=None if first.early_stopping is None else [c.early_stopping for c in members], loss=first.spec.loss, optimizer=fit_optimizer(first.spec))
+                               early_stopping=None if first.early_stopping is None else [c.early_stopping for c in members], loss=first.spec.loss, optimizer=fit_optimizer(first.spec),
+                               reg=fit_reg(first.spec))
         moments = fb.cv_moments.cpu().numpy()
         scale = fb.scale.cpu().numpy().astype(np.float64)
         engine._torch().cuda.synchronize()
@@ -841,7 +843,7 @@ class FleetModelBuilder:
                                      validation_split=first.split[1], validation_batch_size=first.split[2],
                                      early_stopping=None if first.early_stopping is None else [c.early_stopping for c in members],
                                      window=det.window, smoothing_method=det.smoothing_method, threshold_percentile=det.threshold_percentile,
-                                     loss=first.spec.loss, optimizer=fit_optimizer(first.spec))
+                                     loss=first.spec.loss, optimizer=fit_optimizer(first.spec), reg=fit_reg(first.spec))
         torch.cuda.synchronize()
         share = (time.time() - t0) / len(members)  # the bucket's wall time, spread evenly: there is no per-machine time any more
         out = []

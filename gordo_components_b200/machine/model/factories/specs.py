@@ -143,9 +143,28 @@ def optimizer_key(spec) -> tuple:
     return () if cfg is None else (("optimizer", spec.optimizer, tuple(sorted(cfg.items()))),)
 
 
+REG_FIELDS = ("kernel_l1", "kernel_l2", "bias_l1", "bias_l2")
+
+
+def fit_reg(spec):
+    """What the engine's Dense fits take as ``reg``: None when the spec has no non-zero weight regularizer, else the per-layer
+    coefficients of every field of ``REG_FIELDS`` (zeros where a layer has none)."""
+    n = len(spec.dims) - 1
+    reg = {k: [float(v) for v in (getattr(spec, k, None) or [0.0] * n)] for k in REG_FIELDS}
+    return reg if any(v for vals in reg.values() for v in vals) else None
+
+
+def reg_key(spec) -> tuple:
+    """A bucket-key suffix that separates machines by weight regularizers: empty when there are none, so that other keys are what
+    they were."""
+    reg = fit_reg(spec)
+    return () if reg is None else (("reg", *(tuple(reg[k]) for k in REG_FIELDS)),)
+
+
 @dataclass
 class FFNetSpec:
-    """Dense stack: ``dims[0]`` inputs, ``dims[l+1]`` units / ``acts[l]`` / ``l1[l]`` activity-L1 of layer l."""
+    """Dense stack: ``dims[0]`` inputs, ``dims[l+1]`` units / ``acts[l]`` / ``l1[l]`` activity-L1 of layer l.  ``kernel_l1`` ..
+    ``bias_l2``: per-layer weight regularizer coefficients (Keras ``kernel_regularizer`` / ``bias_regularizer``), None = none."""
 
     dims: List[int]
     acts: List[str]
@@ -157,6 +176,11 @@ class FFNetSpec:
     # fields existed loads as the Adam fit of ``adam``
     optimizer: str = "adam"
     optimizer_config: Optional[Dict[str, Any]] = None
+    # plain None defaults, so that a spec pickled before these fields existed loads without regularizers
+    kernel_l1: Optional[List[float]] = None
+    kernel_l2: Optional[List[float]] = None
+    bias_l1: Optional[List[float]] = None
+    bias_l2: Optional[List[float]] = None
 
     @property
     def n_layers(self):

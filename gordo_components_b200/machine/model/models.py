@@ -1,6 +1,6 @@
 """
 sklearn-style model wrappers with the public surface of gordo/machine/model/models.py
-(KerasBaseEstimator :36-357, KerasAutoEncoder :360-398, KerasLSTMBaseEstimator :463-698,
+(KerasBaseEstimator :36-357, KerasAutoEncoder :360-398, KerasRawModelRegressor :401-460, KerasLSTMBaseEstimator :463-698,
 KerasLSTMForecast :701-704, KerasLSTMAutoEncoder :707-710, create_keras_timeseriesgenerator :713-793)
 -- same class names, constructor arguments, methods, return types and exceptions -- whose fit and
 predict run as CUDA kernels on an H100 through ``gordo_components_b200.engine``.
@@ -17,6 +17,7 @@ import logging
 import math
 from copy import copy, deepcopy
 from importlib.util import find_spec
+from pprint import pformat
 from typing import Any, Callable, Dict, Optional, Tuple, Union
 
 import numpy as np
@@ -27,7 +28,8 @@ from sklearn.metrics import explained_variance_score
 
 from .base import GordoBase
 from .factories import *  # noqa: F401,F403  -- executes the @register_model_builder decorators
-from .factories.specs import FFNetSpec, LSTMNetSpec, fit_optimizer
+from .factories.raw import raw_spec
+from .factories.specs import FFNetSpec, LSTMNetSpec, fit_optimizer, fit_reg
 from .register import register_model_builder
 
 logger = logging.getLogger(__name__)
@@ -326,6 +328,7 @@ class KerasBaseEstimator(BaseEstimator, GordoBase):
             self._prepare_model()
         spec = self.model.spec
         optimizer = fit_optimizer(spec)  # None: Adam from spec.adam
+        reg = fit_reg(spec)  # None: no weight regularizers
         if spec.dims[0] != X.shape[1] or spec.dims[-1] != y.shape[1]:
             raise ValueError(f"model was built for {spec.dims[0]}->{spec.dims[-1]} features, got X {X.shape} y {y.shape}")
         fit_args = {**self.extract_supported_fit_args(self.kwargs), **kwargs}
@@ -365,15 +368,17 @@ class KerasBaseEstimator(BaseEstimator, GordoBase):
             frozen = dict(spec.adam, lr=0.0)  # an Adam pass at lr 0 whatever the fit's optimizer: it moves nothing
             for e in range(epochs):
                 loss, acc, state = eng.fit(params, jobs, 1, n_train, xd, yd, epochs=1, batch_size=batch_size, shuffle=shuffle,
-                                           adam=spec.adam, seed=seed + e, state=state, step0=step0, loss=spec.loss, optimizer=optimizer)
+                                           adam=spec.adam, seed=seed + e, state=state, step0=step0, loss=spec.loss, optimizer=optimizer,
+                                           reg=reg)
                 step0 += steps
                 logs = {"loss": float(loss[0, 0])}
                 if "accuracy" in history:
                     logs["accuracy"] = float(acc[0, 0])
                 if n_val:
-                    # keras evaluates the *total* loss (the compiled loss + activity regularisation) on the held-out tail in batches: the fit
-                    # kernel with a zero learning rate on a throw-away optimizer state computes exactly that and moves nothing
-                    vl, va, _ = eng.fit(params, vjobs, 1, n_val, xd, yd, epochs=1, batch_size=vbatch, shuffle=False, adam=frozen, loss=spec.loss)
+                    # keras evaluates the *total* loss (the compiled loss + activity and weight regularisation) on the held-out tail in
+                    # batches: the fit kernel with a zero learning rate on a throw-away optimizer state computes exactly that and moves nothing
+                    vl, va, _ = eng.fit(params, vjobs, 1, n_val, xd, yd, epochs=1, batch_size=vbatch, shuffle=False, adam=frozen, loss=spec.loss,
+                                        reg=reg)
                     logs["val_loss"] = float(vl[0, 0])
                     if "accuracy" in history:
                         logs["val_accuracy"] = float(va[0, 0])
@@ -387,7 +392,7 @@ class KerasBaseEstimator(BaseEstimator, GordoBase):
             epochs_run = len(history["loss"])
         else:
             loss, acc, _ = eng.fit(params, jobs, 1, n_train, xd, yd, epochs=epochs, batch_size=batch_size, shuffle=shuffle,
-                                   adam=spec.adam, seed=seed, loss=spec.loss, optimizer=optimizer)
+                                   adam=spec.adam, seed=seed, loss=spec.loss, optimizer=optimizer, reg=reg)
             history["loss"] = [float(v) for v in loss[0].cpu().numpy()]
             if "accuracy" in history:
                 history["accuracy"] = [float(v) for v in acc[0].cpu().numpy()]
@@ -431,6 +436,39 @@ class KerasAutoEncoder(KerasBaseEstimator, TransformerMixin):
         if self.model is None:
             raise NotFittedError(f"This {self.__class__.__name__} has not been fitted yet.")
         return explained_variance_score(_as_2d_values(y), self.predict(X, **kwargs))
+
+
+class KerasRawModelRegressor(KerasAutoEncoder):
+    """
+    A Dense network from a raw model definition: ``kind`` is the dict itself, ``{"spec": {...models.Sequential: {"layers": [...]}},
+    "compile": {"loss": ..., "optimizer": ..., "metrics": ...}}``, as gordo project YAML gives it.  The ``Sequential`` must be a stack
+    of ``Dense`` layers (``factories.raw``); it trains and predicts on the Dense kernels, its L1 / L2 kernel and bias regularizers
+    inside the fit kernel.  Any other graph is refused with a ValueError.  ``score`` is the explained variance, as for
+    ``KerasAutoEncoder``.
+
+    >>> model = KerasRawModelRegressor(kind={"compile": {"loss": "mse", "optimizer": "adam"},
+    ...     "spec": {"tensorflow.keras.models.Sequential": {"layers": [{"tensorflow.keras.layers.Dense": {"units": 4, "input_shape": [4]}},
+    ...                                                                {"tensorflow.keras.layers.Dense": {"units": 1}}]}}})
+    >>> model.kwargs.update(n_features=4, n_features_out=1)
+    >>> model._build_spec().dims
+    [4, 4, 1]
+    """
+
+    _expected_keys = ("spec", "compile")
+
+    def load_kind(self, kind):
+        return kind
+
+    def __repr__(self):
+        return f"{self.__class__.__name__}(kind: {pformat(self.kind)})"
+
+    def __sklearn_clone__(self):
+        return self.__class__(deepcopy(self.kind), **deepcopy(self.kwargs))
+
+    def _build_spec(self):
+        if not all(k in self.kind for k in self._expected_keys):
+            raise ValueError(f"Expected spec to have keys: {self._expected_keys}, but found {self.kind.keys()}")
+        return raw_spec(self.kind, self.kwargs.get("n_features"), self.kwargs.get("n_features_out"))
 
 
 class KerasLSTMBaseEstimator(KerasBaseEstimator, TransformerMixin, metaclass=abc.ABCMeta):

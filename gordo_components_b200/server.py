@@ -496,18 +496,20 @@ def _extract_X_y(store: ModelStore, name: str, json: Optional[dict], files: Opti
 def _served_parts(model):
     """(input scaler steps, ``KerasAutoEncoder``) of a detector whose base estimator is a bare autoencoder ([] for the steps) or a
     ``Pipeline`` ending in one, else None.  For a fitted ``TransformedTargetRegressor`` these are the parts of its ``regressor_``
-    (its target transformer: ``_target_minmax``)."""
+    (its target transformer: ``_target_minmax``).  A ``KerasRawModelRegressor`` is served as an autoencoder is: it is a Dense
+    stack too, and inference does not see its weight regularizers."""
     from sklearn.compose import TransformedTargetRegressor
     from sklearn.pipeline import Pipeline
 
-    from .machine.model.models import KerasAutoEncoder
+    from .machine.model.models import KerasAutoEncoder, KerasRawModelRegressor
 
+    served = (KerasAutoEncoder, KerasRawModelRegressor)
     est = model.base_estimator
     if type(est) is TransformedTargetRegressor:
         est = getattr(est, "regressor_", None)
-    if type(est) is KerasAutoEncoder:
+    if type(est) in served:
         return [], est
-    if type(est) is Pipeline and len(est.steps) > 1 and type(est.steps[-1][1]) is KerasAutoEncoder:
+    if type(est) is Pipeline and len(est.steps) > 1 and type(est.steps[-1][1]) in served:
         return [step for _, step in est.steps[:-1]], est.steps[-1][1]
     return None
 

@@ -406,6 +406,26 @@ int gb_ffae_fit_opt(const gb_ffnet* net, float* params, float* adam_m, float* ad
                     float* out_loss, float* out_acc, float* out_val_loss, float* out_val_acc, const gb_fit_stop* stop,
                     float* best_params, int32_t* out_epochs, int32_t* out_best_epoch, const gb_optimizer* opt, void* stream);
 
+/* Keras kernel_regularizer / bias_regularizer of Dense layer l (keras 3.3.3 regularizers.L1 / L2 / L1L2 [3P], restated, not verified
+ * against TF).  The fit minimises loss + R, R = sum_l kernel_l1[l] sum|W_l| + kernel_l2[l] sum W_l^2 + bias_l1[l] sum|b_l| + bias_l2[l] sum b_l^2,
+ * with R evaluated on the weights the step's forward pass uses.  R is part of every mini-batch's total loss, beside the activity
+ * term and weighted as it is in the epoch means, so the history, the held-out statistics (R of the current weights) and the
+ * EarlyStopping monitor all carry it.  Its gradient l1 sign(w) + 2 l2 w (sign(0) = 0) is added once per optimizer step to the summed
+ * mini-batch gradient, before clipvalue and the optimizer's rule; weight decay stays the optimizer's own term. */
+typedef struct gb_dense_reg {
+  float kernel_l1[GB_MAX_LAYERS], kernel_l2[GB_MAX_LAYERS];
+  float bias_l1[GB_MAX_LAYERS], bias_l2[GB_MAX_LAYERS];
+} gb_dense_reg;
+
+/* gb_ffae_fit_opt with the weight regularizers `reg`.  reg NULL, or every coefficient 0: exactly gb_ffae_fit_opt (same kernel,
+ * bit-identical results).  A negative or non-finite coefficient of a layer of the net is GB_E_ARG, nothing enqueued. */
+int gb_ffae_fit_reg(const gb_ffnet* net, float* params, float* adam_m, float* adam_v, const gb_job* jobs,
+                    const gb_fit_split* split, int32_t n_jobs, int32_t max_rows, const float* x, const float* y,
+                    const int32_t* row_map, const int32_t* perm, const gb_fit_hparams* hp, int32_t val_batch,
+                    float* out_loss, float* out_acc, float* out_val_loss, float* out_val_acc, const gb_fit_stop* stop,
+                    float* best_params, int32_t* out_epochs, int32_t* out_best_epoch, const gb_optimizer* opt,
+                    const gb_dense_reg* reg, void* stream);
+
 /* The memory plan gb_ffae_fit uses for this architecture (host only, no device needed).  The first of five that fits in
  * 227 KB of shared memory: everything in shared memory; the weight image in the slot's L2-resident state area
  * (*weights_in_l2 = 1); then one, two or three of the three dz buffers there as well (*dz_in_l2).  GB_E_SMEM if none fits
