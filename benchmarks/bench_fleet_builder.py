@@ -29,6 +29,8 @@ fleet.build_kfold_fleet makes after the fold scoring, on arrays of the bucket's 
 FleetModelBuilder(ragged=True) and with the default, alternating, ``--runs`` times each: wall time, the number of buckets and of
 fit launches, and the device time of the fit launches (CUDA events around each, summed per build).  Without the flag every
 length is its own bucket.
+``--window W`` gives the plain detectors a smoothing window W (smm) and builds them with FleetModelBuilder(smoothing=True), whose
+fold thresholds at 6 rows and at W come from one gb_thresholds_pair launch.
 Measured numbers and the card they were measured on are in DESIGN.md §5b and §7.
 """
 import argparse, json, os, sys, tempfile, time
@@ -63,6 +65,7 @@ def main():
     ap.add_argument("--kfcv", action="store_true", help="the reference's production definition: a K-fold detector under KFold(5, shuffle, random_state=0)")
     ap.add_argument("--ragged", default=None, metavar="LO:HI", help="per-machine lengths drawn uniformly from [LO, HI]; ragged=True against the default")
     ap.add_argument("--runs", type=int, default=2, help="--ragged: builds of each kind, alternating")
+    ap.add_argument("--window", type=int, default=None, help="plain detectors with this smoothing window (smm), batched by FleetModelBuilder(smoothing=True)")
     a = ap.parse_args()
     import numpy as np
     import pandas as pd
@@ -100,6 +103,9 @@ def main():
             "scaler": "sklearn.preprocessing.MinMaxScaler", "window": 144, "shuffle": True, "threshold_percentile": 0.975}}
         evaluation, n_splits = {"cv": {"sklearn.model_selection.KFold": {"n_splits": 5, "shuffle": True, "random_state": 0}}}, 5
     flags = dict(early_stopping=a.early_stopping or a.kfcv, kfcv=a.kfcv)
+    if a.window is not None and not a.kfcv:
+        next(iter(model.values())).update({"window": a.window, "smoothing_method": "smm"})
+        flags["smoothing"] = True
     rng = np.random.default_rng(0)
     if a.ragged:
         lo, hi = (int(v) for v in a.ragged.split(":"))
@@ -140,6 +146,8 @@ def main():
     if a.kfcv:
         net = ("K-fold detector (window 144, percentile 0.975) around TransformedTargetRegressor(MinMaxScaler) of a hourglass (compression 0.5, "
                "1 encoding layer, batch 128, validation_split 0.1), KFold(5, shuffle, random_state=0)")
+    if a.window is not None and not a.kfcv:
+        net += f", smoothing window {a.window}"
     if a.early_stopping or a.kfcv:
         net += f", EarlyStopping(val_loss, patience 10, min_delta {a.min_delta:g}, restore_best_weights)"
     out = {

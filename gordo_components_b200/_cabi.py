@@ -81,7 +81,7 @@ def make_dense_reg(kernel_l1=None, kernel_l2=None, bias_l1=None, bias_l2=None) -
 
 EXPORTS = (
     "gb_abi_version", "gb_last_error", "gb_device_check", "gb_ffnet_param_count", "gb_ffnet_param_stride",
-    "gb_ffae_infer_score", "gb_ffae_tc_supported", "gb_ffae_infer_plan", "gb_ffae_infer_score_x64", "gb_ffae_infer_plan_x64", "gb_anomaly_score", "gb_anomaly_score_f64", "gb_minmax_fit", "gb_minmax_f64", "gb_thresholds", "gb_thresholds_f64", "gb_cv_moments", "gb_smooth", "gb_smooth_scores", "gb_quantile", "gb_affine_f64", "gb_gather_rows", "gb_gather_rows_ragged", "gb_minmax_inverse_f32", "gb_minmax_inverse_score_f64", "gb_ffae_fit_state_stride", "gb_ffae_fit", "gb_ffae_fit_split", "gb_ffae_fit_stop", "gb_ffae_fit_plan", "gb_ffae_fit_opt", "gb_ffae_fit_reg",
+    "gb_ffae_infer_score", "gb_ffae_tc_supported", "gb_ffae_infer_plan", "gb_ffae_infer_score_x64", "gb_ffae_infer_plan_x64", "gb_anomaly_score", "gb_anomaly_score_f64", "gb_minmax_fit", "gb_minmax_f64", "gb_thresholds", "gb_thresholds_f64", "gb_thresholds_pair", "gb_thresholds_pair_f64", "gb_cv_moments", "gb_smooth", "gb_smooth_scores", "gb_quantile", "gb_affine_f64", "gb_gather_rows", "gb_gather_rows_ragged", "gb_minmax_inverse_f32", "gb_minmax_inverse_score_f64", "gb_ffae_fit_state_stride", "gb_ffae_fit", "gb_ffae_fit_split", "gb_ffae_fit_stop", "gb_ffae_fit_plan", "gb_ffae_fit_opt", "gb_ffae_fit_reg",
     "gb_lstm_param_count", "gb_lstm_param_stride", "gb_lstm_workspace_bytes", "gb_lstm_infer", "gb_lstm_tc_supported", "gb_lstm_tc_workspace_bytes", "gb_lstm_infer_tc", "gb_lstm_tc_ragged_workspace_bytes", "gb_lstm_infer_tc_ragged", "gb_lstm_fit_workspace_bytes", "gb_lstm_fit", "gb_lstm_fit_loss", "gb_lstm_fit_tc_workspace_bytes", "gb_lstm_fit_tc", "gb_lstm_fit_opt", "gb_lstm_fit_tc_opt",
     "gb_lstm_fit_stop_state_bytes", "gb_lstm_fit_stop", "gb_lstm_fit_tc_stop",
     "gb_orthonormal_rows",
@@ -175,6 +175,10 @@ def _declare(lib):
     lib.gb_thresholds.argtypes = [_P, C.c_int32, C.c_int32, _P, _P, C.c_int32, C.c_int32, _P, _P, C.c_int32, _P]
     lib.gb_thresholds_f64.argtypes = lib.gb_thresholds.argtypes
     lib.gb_thresholds_f64.restype = C.c_int
+    lib.gb_thresholds_pair.argtypes = [_P, C.c_int32, C.c_int32, _P, _P, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P, _P, C.c_int32, _P]
+    lib.gb_thresholds_pair.restype = C.c_int
+    lib.gb_thresholds_pair_f64.argtypes = lib.gb_thresholds_pair.argtypes
+    lib.gb_thresholds_pair_f64.restype = C.c_int
     lib.gb_cv_moments.argtypes = [_P, C.c_int32, _P, _P, C.c_int32, _P, _P]
     lib.gb_cv_moments.restype = C.c_int
     lib.gb_smooth.argtypes = [_P, C.c_int32, C.c_int32, _P, C.c_int32, C.c_int32, C.c_int32, _P, _P]

@@ -336,24 +336,43 @@ class _Canonical:
         self.early_stopping = early_stopping  # the estimator's one EarlyStopping callback, or None
         self.X, self.y, self.dataset_meta, self.query_sec = X, y, dataset_meta, query_sec
         self.fit, self.n_splits, self.evaluation = fit, n_splits, evaluation
+        self.window = None  # the plain detector's smoothing window (FleetModelBuilder(smoothing=True)), or None
+
+    def _window_key(self) -> tuple:
+        """The smoothing window as a bucket field, only when there is one: keys of machines without a window stay as they were.
+        The smoothing method does not enter the thresholds, so it does not split buckets."""
+        return () if self.window is None else (("window", self.window),)
 
     def bucket(self, ragged: bool = False):
         """The fields machines of one batched build share; ``ragged`` leaves out the row count (``FleetModelBuilder(ragged=True)``)."""
         s = self.spec
         return (tuple(s.dims), tuple(s.acts), tuple(float(v) for v in s.l1), tuple(sorted(s.adam.items())), tuple(s.metrics), s.loss,
                 None if ragged else len(self.X), self.fit["epochs"], self.fit["batch_size"], self.fit["shuffle"], self.n_splits, int(self.evaluation.get("seed", 0)),
-                self.split, self.early_stopping is not None, self.input_scaler) + optimizer_key(s) + reg_key(s)  # EarlyStopping's parameters are per-job records
+                self.split, self.early_stopping is not None, self.input_scaler) + optimizer_key(s) + reg_key(s) + self._window_key()  # EarlyStopping's parameters are per-job records
 
 
 def _default_minmax(scaler) -> bool:
     return type(scaler) is MinMaxScaler and tuple(scaler.feature_range) == (0, 1) and not getattr(scaler, "clip", False)
 
 
-def _canonical(index, machine, early_stopping: bool = False) -> Optional[_Canonical]:
+def _window_refusal(model) -> Optional[str]:
+    """Why the batched builds cannot take this detector's smoothing window (not a positive int, or an unknown method), or None."""
+    import numbers
+
+    if model.window is not None and (not isinstance(model.window, numbers.Integral) or isinstance(model.window, bool) or model.window < 1):
+        return f"window {model.window!r} is not a positive int"
+    if model.window is not None and model.smoothing_method not in ("smm", "sma", "ewma"):
+        return f"smoothing_method {model.smoothing_method!r}"
+    return None
+
+
+def _canonical(index, machine, early_stopping: bool = False, smoothing: bool = False) -> Optional[_Canonical]:
     """
     The machine as a candidate for the batched path, or ``None`` with the reason logged.  ``early_stopping``: also take an
     estimator with one Keras ``EarlyStopping`` callback on a metric its fit reports (``FleetModelBuilder(early_stopping=True)``);
-    without it any callback sends the machine to ``ModelBuilder``.
+    without it any callback sends the machine to ``ModelBuilder``.  ``smoothing``: also take a detector with a smoothing
+    ``window`` (a positive int, smm / sma / ewma; ``FleetModelBuilder(smoothing=True)``); without it such a detector goes to
+    ``ModelBuilder``.
     """
     from .machine.model.anomaly.diff import DiffBasedAnomalyDetector
     from .machine.model.factories.specs import FFNetSpec
@@ -371,8 +390,11 @@ def _canonical(index, machine, early_stopping: bool = False) -> Optional[_Canoni
         return no("cv is not a plain TimeSeriesSplit")
 
     model = serializer.from_definition(machine["model"])
-    if type(model) is not DiffBasedAnomalyDetector or model.window is not None:
+    if type(model) is not DiffBasedAnomalyDetector or (model.window is not None and not smoothing):
         return no("model is not a plain DiffBasedAnomalyDetector")
+    reason = _window_refusal(model)
+    if reason:
+        return no(reason)
     if not _default_minmax(model.scaler):
         return no("detector scaler is not a default MinMaxScaler")
     ae, input_scaler = _ff_network(model.base_estimator)
@@ -399,8 +421,9 @@ def _canonical(index, machine, early_stopping: bool = False) -> Optional[_Canoni
         return no(reason)
     fit = {"epochs": int(fit_args.get("epochs", 1)), "batch_size": int(fit_args.get("batch_size") or 32), "shuffle": bool(fit_args.get("shuffle", True))}
     split = (bool(model.shuffle), vsplit, int(fit_args.get("validation_batch_size") or fit["batch_size"]) if vsplit else None)
-    return _Canonical(index, machine, model, spec, X, y, dataset_meta, query_sec, fit, split_obj.n_splits, evaluation, input_scaler, split,
-                      stopping)
+    c = _Canonical(index, machine, model, spec, X, y, dataset_meta, query_sec, fit, split_obj.n_splits, evaluation, input_scaler, split, stopping)
+    c.window = None if model.window is None else int(model.window)
+    return c
 
 
 def _evaluation_refusal(evaluation: dict) -> Optional[str]:
@@ -478,7 +501,7 @@ class _CanonicalLSTM(_Canonical):
     def bucket(self, ragged: bool = False):
         s = self.spec
         return (s.key(), tuple(sorted(s.adam.items())), tuple(s.metrics), s.loss, self.lookahead, None if ragged else len(self.X), self.fit["epochs"], self.fit["batch_size"],
-                self.n_splits, int(self.evaluation.get("seed", 0)), self.input_scaler, self.early_stopping is not None) + optimizer_key(s)  # EarlyStopping's parameters are per-job records
+                self.n_splits, int(self.evaluation.get("seed", 0)), self.input_scaler, self.early_stopping is not None) + optimizer_key(s) + self._window_key()  # EarlyStopping's parameters are per-job records
 
 
 def _is_lstm_definition(machine) -> bool:
@@ -496,7 +519,7 @@ def _is_lstm_definition(machine) -> bool:
     return isinstance(est, KerasLSTMBaseEstimator)
 
 
-def _canonical_lstm(index, machine, wide_batches: bool = False, early_stopping: bool = False) -> Optional[_CanonicalLSTM]:
+def _canonical_lstm(index, machine, wide_batches: bool = False, early_stopping: bool = False, smoothing: bool = False) -> Optional[_CanonicalLSTM]:
     """
     The LSTM form of the canonical definition -- ``DiffBasedAnomalyDetector(KerasLSTMAutoEncoder | KerasLSTMForecast)``, the network bare
     or behind one default ``MinMaxScaler``, under the evaluation ``_canonical`` accepts -- as a candidate for the batched path, or
@@ -504,6 +527,7 @@ def _canonical_lstm(index, machine, wide_batches: bool = False, early_stopping: 
     ``wide_batches``: also take batch sizes above 32, up to ``LSTMEngine.TC_MAX_BATCH`` (the tensor-core fit family;
     ``FleetModelBuilder(lstm_wide_batches=True)``).  ``early_stopping``: also take an estimator with one Keras ``EarlyStopping``
     callback on a metric its fit reports, ``loss`` or (with the accuracy metric) ``accuracy`` (``FleetModelBuilder(lstm_early_stopping=True)``).
+    ``smoothing``: also take a detector with a smoothing ``window``, as ``_canonical`` does (``FleetModelBuilder(smoothing=True)``).
     """
     from .machine.model.anomaly.diff import DiffBasedAnomalyDetector
     from .engine import LSTMEngine
@@ -529,8 +553,11 @@ def _canonical_lstm(index, machine, wide_batches: bool = False, early_stopping: 
         return no("cv is not a plain TimeSeriesSplit")
 
     model = serializer.from_definition(machine["model"])
-    if type(model) is not DiffBasedAnomalyDetector or model.window is not None or model.shuffle:
+    if type(model) is not DiffBasedAnomalyDetector or (model.window is not None and not smoothing) or model.shuffle:
         return no("model is not a plain DiffBasedAnomalyDetector")
+    reason = _window_refusal(model)
+    if reason:
+        return no(reason)
     if not _default_minmax(model.scaler):
         return no("detector scaler is not a default MinMaxScaler")
     est, input_scaler = model.base_estimator, False
@@ -567,8 +594,10 @@ def _canonical_lstm(index, machine, wide_batches: bool = False, early_stopping: 
     if reason:
         return no(reason)
     fit = {"epochs": int(fit_args.get("epochs", 1)), "batch_size": batch_size, "shuffle": False}
-    return _CanonicalLSTM(index, machine, model, spec, X, y, dataset_meta, query_sec, fit, K, evaluation, input_scaler, (False, 0.0, None), stopping,
-                          lookahead=la)
+    c = _CanonicalLSTM(index, machine, model, spec, X, y, dataset_meta, query_sec, fit, K, evaluation, input_scaler, (False, 0.0, None), stopping,
+                       lookahead=la)
+    c.window = None if model.window is None else int(model.window)
+    return c
 
 
 class _CanonicalKFold(_Canonical):
@@ -688,11 +717,18 @@ class FleetModelBuilder:
     one row count per machine.  Off by default for the same reason as ``kfcv``: the batched fits draw their initial weights per
     bucket, so merging lengths changes which weights a machine starts from.  Without it buckets, builds and artefacts are
     those of equal-length buckets.
+
+    ``smoothing``: also batch plain feed-forward and LSTM detectors with a smoothing ``window`` (a positive int) and smm / sma / ewma
+    ``smoothing_method``.  Every fold's 6-row and window thresholds come from one pass over its scores (``gb_thresholds_pair``),
+    and the detectors carry the ``smooth_*`` thresholds and metadata ``ModelBuilder`` gives them.  The window is a bucket field;
+    the method is not (it does not enter the thresholds).  Off by default for the same reason as ``kfcv``: without it such
+    machines build through ``ModelBuilder`` as before.
     """
 
     def __init__(self, machines: Sequence, early_stopping: bool = False, kfcv: bool = False, lstm_wide_batches: bool = False,
-                 lstm_early_stopping: bool = False, ragged: bool = False):
+                 lstm_early_stopping: bool = False, ragged: bool = False, smoothing: bool = False):
         self.ragged = bool(ragged)
+        self.smoothing = bool(smoothing)
         self.early_stopping = bool(early_stopping)
         self.kfcv = bool(kfcv)
         self.lstm_wide_batches = bool(lstm_wide_batches)
@@ -711,18 +747,18 @@ class FleetModelBuilder:
 
         return FleetModelBuilder([self.machines[i] for i in fleet.partition(len(self.machines), world)[rank]], early_stopping=self.early_stopping,
                                  kfcv=self.kfcv, lstm_wide_batches=self.lstm_wide_batches, lstm_early_stopping=self.lstm_early_stopping,
-                                 ragged=self.ragged)
+                                 ragged=self.ragged, smoothing=self.smoothing)
 
     def build(self, output_dir: Optional[str] = None) -> List[Tuple[Any, dict]]:
         results: List[Optional[Tuple[Any, dict]]] = [None] * len(self.machines)
         buckets: Dict[tuple, List[_Canonical]] = {}
         for i, machine in enumerate(self.machines):
             if _is_lstm_definition(machine):
-                c = _canonical_lstm(i, machine, wide_batches=self.lstm_wide_batches, early_stopping=self.lstm_early_stopping)
+                c = _canonical_lstm(i, machine, wide_batches=self.lstm_wide_batches, early_stopping=self.lstm_early_stopping, smoothing=self.smoothing)
             elif self.kfcv and _is_kfcv_definition(machine):
                 c = _canonical_kfcv(i, machine, early_stopping=self.early_stopping)
             else:
-                c = _canonical(i, machine, early_stopping=self.early_stopping)
+                c = _canonical(i, machine, early_stopping=self.early_stopping, smoothing=self.smoothing)
             if c is None:
                 results[i] = ModelBuilder(machine).build()
             else:
@@ -761,7 +797,7 @@ class FleetModelBuilder:
                                input_scaler=first.input_scaler, detector_shuffle=first.split[0], validation_split=first.split[1],
                                validation_batch_size=first.split[2],
                                early_stopping=None if first.early_stopping is None else [c.early_stopping for c in members], loss=first.spec.loss, optimizer=fit_optimizer(first.spec),
-                               reg=fit_reg(first.spec))
+                               reg=fit_reg(first.spec), window=first.window)
         moments = fb.cv_moments.cpu().numpy()
         scale = fb.scale.cpu().numpy().astype(np.float64)
         engine._torch().cuda.synchronize()
@@ -800,7 +836,8 @@ class FleetModelBuilder:
         fb = fleet.build_lstm_fleet(eng, xd, yd, rows, lookahead=first.lookahead, epochs=first.fit["epochs"], batch_size=first.fit["batch_size"],
                                     n_splits=K, seed=int(first.evaluation.get("seed", 0)), adam=first.spec.adam, input_scaler=first.input_scaler,
                                     loss=first.spec.loss, optimizer=fit_optimizer(first.spec),
-                                    early_stopping=None if first.early_stopping is None else [c.early_stopping for c in members])
+                                    early_stopping=None if first.early_stopping is None else [c.early_stopping for c in members],
+                                    window=first.window)
         engine._torch().cuda.synchronize()
         share = (time.time() - t0) / len(members)  # the bucket's wall time, spread evenly: there is no per-machine time any more
         split_obj = TimeSeriesSplit(n_splits=K)

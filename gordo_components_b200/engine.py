@@ -271,6 +271,9 @@ class FFEngine:
     def thresholds(self, jobs_dev, n_jobs, max_rows, tag_unscaled, total_scaled, n_slots, window=6):
         return thresholds(jobs_dev, n_jobs, max_rows, tag_unscaled, total_scaled, self.n_out, n_slots, window, self.device)
 
+    def thresholds_pair(self, jobs_dev, n_jobs, max_rows, tag_unscaled, total_scaled, n_slots, w0, w1):
+        return thresholds_pair(jobs_dev, n_jobs, max_rows, tag_unscaled, total_scaled, self.n_out, n_slots, w0, w1, self.device)
+
 
 def _fit_hparams(epochs, batch_size, shuffle, perm, adam, seed, l1_div_batch, step0, loss="mse") -> "_cabi.GbFitHParams":
     adam = adam or {}
@@ -366,6 +369,24 @@ def thresholds(jobs_dev, n_jobs, max_rows, tag_unscaled, total_scaled, n_out, n_
     _cabi.check(fn(p(jobs_dev), int(n_jobs), int(max_rows), p(tag_unscaled), p(total_scaled), int(n_out), int(window),
                                   p(feat), p(agg), int(n_slots), _stream_ptr()))
     return feat, agg
+
+
+def thresholds_pair(jobs_dev, n_jobs, max_rows, tag_unscaled, total_scaled, n_out, n_slots, w0, w1, device):
+    """
+    ``thresholds`` at two windows from one pass over the score arrays (gb_thresholds_pair): (feat_thr0, agg_thr0, feat_thr1,
+    agg_thr1), the first pair at ``w0`` and the second at ``w1``, each bit for bit what ``thresholds`` gives at that window.
+    """
+    torch = _torch()
+    lib = _cabi.load_library()
+    dtype = tag_unscaled.dtype
+    if total_scaled.dtype != dtype or dtype not in (torch.float32, torch.float64):
+        raise ValueError(f"thresholds need two float32 or two float64 arrays, got {dtype} / {total_scaled.dtype}")
+    out = [torch.full(shape, float("nan"), dtype=dtype, device=device) for shape in ((n_slots, n_out), (n_slots,)) * 2]
+    p = _cabi.ptr
+    fn = lib.gb_thresholds_pair if dtype == torch.float32 else lib.gb_thresholds_pair_f64
+    _cabi.check(fn(p(jobs_dev), int(n_jobs), int(max_rows), p(tag_unscaled), p(total_scaled), int(n_out), int(w0), int(w1),
+                   *(p(t) for t in out), int(n_slots), _stream_ptr()))
+    return tuple(out)
 
 
 def cv_moments(jobs_dev, n_jobs, yhat, y, n_out):

@@ -158,6 +158,28 @@ def time_e2e(eng, params, jobs_h, x_dev, y_dev, scale, feat_thr, agg_thr, steps:
 
 
 # ------------------------------------------------------------------------------------------------ fleet build (train + thresholds)
+def _fill_smooth_thresholds(det, window, fold_feat, fold_agg, tags):
+    """
+    The four smooth-threshold attributes ``DiffBasedAnomalyDetector.cross_validate`` leaves (diff.py:384-391): from the per-fold
+    window-``window`` thresholds ``fold_feat`` [K, T] / ``fold_agg`` [K] when the detector has a window, else the empty values.
+    """
+    import pandas as pd
+
+    if window is None:
+        det.smooth_feature_thresholds_per_fold_ = pd.DataFrame()
+        det.smooth_aggregate_thresholds_per_fold_ = {}
+        det.smooth_aggregate_threshold_ = None
+        det.smooth_feature_thresholds_ = None
+        return det
+    K = len(fold_agg)
+    ff = np.asarray(fold_feat, dtype=np.float64)
+    det.smooth_feature_thresholds_per_fold_ = pd.DataFrame(ff.copy(), columns=tags, index=[f"fold-{k}" for k in range(K)])
+    det.smooth_aggregate_thresholds_per_fold_ = {f"fold-{k}": float(fold_agg[k]) for k in range(K)}
+    det.smooth_feature_thresholds_ = pd.Series(ff[K - 1].copy(), index=tags, name=f"fold-{K - 1}")
+    det.smooth_aggregate_threshold_ = float(fold_agg[K - 1])
+    return det
+
+
 class FleetBuild:
     """
     Result of ``build_fleet``: everything ``ModelBuilder._build`` (gordo/builder/build_model.py:192-339) produces for one
@@ -167,7 +189,10 @@ class FleetBuild:
     def __init__(self, eng, n_machines, n_splits, params, scale, offset, feat_thr, agg_thr, loss, acc, fold_loss, fold_feat_thr, fold_agg_thr,
                  fold_params=None, cv_moments=None, in_scale=None, in_offset=None, fold_in_scale=None, fold_in_offset=None, steps_per_epoch=None,
                  val_loss=None, val_acc=None, fold_val_loss=None, fold_val_acc=None, epochs=None, epochs_run=None, best_epoch=None,
-                 fold_epochs_run=None, fold_best_epoch=None, rows=None, n_test=None, starts=None, init_params=None):
+                 fold_epochs_run=None, fold_best_epoch=None, rows=None, n_test=None, starts=None, init_params=None, window=None,
+                 fold_smooth_feat_thr=None, fold_smooth_agg_thr=None):
+        # the detector's smoothing window and every fold's thresholds at it ([M, K, T], [M, K]); None without a window
+        self.window, self.fold_smooth_feat_thr, self.fold_smooth_agg_thr = window, fold_smooth_feat_thr, fold_smooth_agg_thr
         # EarlyStopping: epochs each fit ran and its best epoch (-1: none) ([M]; per CV fold [M, K]); None without the callback.
         # History entries past a fit's epochs_run are NaN.  `epochs` is the configured count (keras History.params["epochs"]).
         self.epochs = epochs
@@ -254,17 +279,15 @@ class FleetBuild:
             det = template
             det.scaler = sc
         else:
-            det = DiffBasedAnomalyDetector(base_estimator=ae, scaler=sc)
+            det = DiffBasedAnomalyDetector(base_estimator=ae, scaler=sc, **({} if self.window is None else {"window": self.window}))
         det.feature_thresholds_ = pd.Series(self.feat_thr[m].cpu().numpy().astype(np.float64), index=tags, name=f"fold-{self.n_splits - 1}")
         det.aggregate_threshold_ = float(self.agg_thr[m])
         ff = self.fold_feat_thr[m].cpu().numpy().astype(np.float64)
         det.feature_thresholds_per_fold_ = pd.DataFrame(ff, columns=tags, index=[f"fold-{k}" for k in range(self.n_splits)])
         det.aggregate_thresholds_per_fold_ = {f"fold-{k}": float(self.fold_agg_thr[m, k]) for k in range(self.n_splits)}
-        det.smooth_feature_thresholds_per_fold_ = pd.DataFrame()
-        det.smooth_aggregate_thresholds_per_fold_ = {}
-        det.smooth_aggregate_threshold_ = None
-        det.smooth_feature_thresholds_ = None
-        return det
+        if self.window is None:
+            return _fill_smooth_thresholds(det, None, None, None, tags)
+        return _fill_smooth_thresholds(det, self.window, self.fold_smooth_feat_thr[m].cpu().numpy(), self.fold_smooth_agg_thr[m].cpu().numpy(), tags)
 
 
 def dump_fleet(fb: "FleetBuild", root: str, names: Sequence[str], tags: Optional[Sequence[Sequence[str]]] = None,
@@ -376,7 +399,8 @@ def shuffle_maps(slot_rows):
 def build_fleet(eng: "engine.FFEngine", x, y, rows, epochs: int = 1, batch_size: int = 32, n_splits: int = 3, seed: int = 0,
                 adam: Optional[Dict[str, float]] = None, shuffle: bool = True, generator=None, input_scaler: bool = False,
                 detector_shuffle: bool = False, validation_split: float = 0.0, validation_batch_size: Optional[int] = None,
-                early_stopping=None, loss: str = "mse", optimizer=None, keep_init_params: bool = False, reg=None) -> FleetBuild:
+                early_stopping=None, loss: str = "mse", optimizer=None, keep_init_params: bool = False, reg=None,
+                window: Optional[int] = None) -> FleetBuild:
     """
     The batched form of ``gordo build`` for one architecture bucket: for every machine the 3-fold TimeSeriesSplit
     cross-validation (fit on each prefix, thresholds from the following test block: diff.py:176-266) and the final fit on
@@ -408,6 +432,8 @@ def build_fleet(eng: "engine.FFEngine", x, y, rows, epochs: int = 1, batch_size:
     ``optimizer``: None (Adam from ``adam``) or the estimator's (name, record) (``factories.specs.fit_optimizer``), for every fit.
     ``reg``: None or the estimator's weight regularizers (``factories.specs.fit_reg``), for every fit.
     ``keep_init_params``: keep the initial parameters of every slot on the result (``init_params``).
+    ``window``: the detector's smoothing window.  Every fold then also gets its thresholds at that window (the detector's
+    ``smooth_*`` attributes), from the same pass over the fold scores as its 6-row thresholds (gb_thresholds_pair).
     """
     torch = engine._torch()
     dev = eng.device
@@ -465,7 +491,13 @@ def build_fleet(eng: "engine.FFEngine", x, y, rows, epochs: int = 1, batch_size:
     sc_jobs = engine.jobs_to_device(engine.make_jobs(M + np.arange(KM), sc_n, fit_x[M:] + starts[fm, fk], _prefix(sc_n)), dev)
     max_test = int(test.max())
     res = eng.infer_score(params, sc_jobs, KM, max_test, x, y, scale, out_rows=int(sc_n.sum()), want=("tag-anomaly-unscaled", "total-anomaly-scaled"))
-    feat, agg = eng.thresholds(sc_jobs, KM, max_test, res["tag-anomaly-unscaled"], res["total-anomaly-scaled"], S, window=6)
+    fold_sfeat = fold_sagg = None
+    if window is None:
+        feat, agg = eng.thresholds(sc_jobs, KM, max_test, res["tag-anomaly-unscaled"], res["total-anomaly-scaled"], S, window=6)
+    else:
+        feat, agg, sfeat, sagg = eng.thresholds_pair(sc_jobs, KM, max_test, res["tag-anomaly-unscaled"], res["total-anomaly-scaled"], S, 6, int(window))
+        fold_sfeat = sfeat[M:].view(K, M, eng.n_out).permute(1, 0, 2).contiguous()
+        fold_sagg = sagg[M:].view(K, M).t().contiguous()
     T = eng.n_out
     # the evaluation metrics of ModelBuilder's cross validation (build_model.py:250-289) reduce to five sums per (fold, tag)
     moments = engine.cv_moments(sc_jobs, KM, res["model-output"], y, T).view(K, M, 5, T).permute(1, 0, 2, 3).contiguous()
@@ -486,7 +518,8 @@ def build_fleet(eng: "engine.FFEngine", x, y, rows, epochs: int = 1, batch_size:
                       fold_val_loss=folds(val_loss), fold_val_acc=folds(val_acc), epochs=int(epochs),
                       epochs_run=None if epochs_run is None else epochs_run[:M], best_epoch=None if best_epoch is None else best_epoch[:M],
                       fold_epochs_run=fold_jobs(epochs_run), fold_best_epoch=fold_jobs(best_epoch), rows=n, n_test=test, starts=starts,
-                      init_params=init_params)
+                      init_params=init_params, window=None if window is None else int(window), fold_smooth_feat_thr=fold_sfeat,
+                      fold_smooth_agg_thr=fold_sagg)
 
 
 # ------------------------------------------------------------------------------------------------ fleet build of LSTM detectors
@@ -518,7 +551,9 @@ class LSTMFleetBuild:
     def __init__(self, eng, n_machines, n_splits, rows, lookahead, batch_size, starts, n_test, params, fold_params, init_params, loss, acc,
                  fold_loss, fold_acc, y_min, y_max, fold_y_min, fold_y_max, feat_thr, agg_thr, fold_feat_thr, fold_agg_thr, cv_moments,
                  fold_predictions, in_min=None, in_max=None, fold_in_min=None, fold_in_max=None, epochs=None, epochs_run=None, best_epoch=None,
-                 fold_epochs_run=None, fold_best_epoch=None):
+                 fold_epochs_run=None, fold_best_epoch=None, window=None, fold_smooth_feat_thr=None, fold_smooth_agg_thr=None):
+        # the detector's smoothing window and every fold's thresholds at it ([M, K, T], [M, K] float64); None without a window
+        self.window, self.fold_smooth_feat_thr, self.fold_smooth_agg_thr = window, fold_smooth_feat_thr, fold_smooth_agg_thr
         # EarlyStopping: epochs each fit ran and its best epoch (-1: none) ([M]; per CV fold [M, K]) as int32 host arrays; None without
         # the callback.  History entries past a fit's epochs_run are NaN.  `epochs` is the configured count (History.params["epochs"]).
         self.epochs = epochs
@@ -579,7 +614,7 @@ class LSTMFleetBuild:
                        encoding_func=tuple(eng.acts), decoding_dim=(), decoding_func=(), out_func=eng.out_func, n_features=eng.n_features,
                        n_features_out=T)
             spec = lstm._build_spec()
-            det = DiffBasedAnomalyDetector(base_estimator=lstm, scaler=MinMaxScaler())
+            det = DiffBasedAnomalyDetector(base_estimator=lstm, scaler=MinMaxScaler(), **({} if self.window is None else {"window": self.window}))
         lstm.model = FittedNet(spec, eng.unpack_params(self.params[m : m + 1])[0])
         hist = {"loss": [float(v) for v in self.loss[m]]}
         if "accuracy" in spec.metrics:
@@ -596,11 +631,9 @@ class LSTMFleetBuild:
         det.aggregate_threshold_ = float(self.agg_thr[m])
         det.feature_thresholds_per_fold_ = pd.DataFrame(self.fold_feat_thr[m].copy(), columns=tags, index=[f"fold-{k}" for k in range(K)])
         det.aggregate_thresholds_per_fold_ = {f"fold-{k}": float(self.fold_agg_thr[m, k]) for k in range(K)}
-        det.smooth_feature_thresholds_per_fold_ = pd.DataFrame()
-        det.smooth_aggregate_thresholds_per_fold_ = {}
-        det.smooth_aggregate_threshold_ = None
-        det.smooth_feature_thresholds_ = None
-        return det
+        if self.window is None:
+            return _fill_smooth_thresholds(det, None, None, None, tags)
+        return _fill_smooth_thresholds(det, self.window, self.fold_smooth_feat_thr[m], self.fold_smooth_agg_thr[m], tags)
 
 
 class _FoldBlocks:
@@ -617,7 +650,8 @@ class _FoldBlocks:
 
 def build_lstm_fleet(eng: "engine.LSTMEngine", x, y, rows, lookahead: int = 0, epochs: int = 1, batch_size: int = 32, n_splits: int = 3,
                      seed: int = 0, adam: Optional[Dict[str, float]] = None, input_scaler: bool = False, memory_budget: int = 8 << 30,
-                     keep_init_params: bool = False, generator=None, loss: str = "mse", optimizer=None, early_stopping=None) -> LSTMFleetBuild:
+                     keep_init_params: bool = False, generator=None, loss: str = "mse", optimizer=None, early_stopping=None,
+                     window: Optional[int] = None) -> LSTMFleetBuild:
     """
     The batched ``gordo build`` of one bucket of LSTM machines (``DiffBasedAnomalyDetector(KerasLSTMAutoEncoder | KerasLSTMForecast)``,
     the network bare or behind one MinMaxScaler): for every machine the TimeSeriesSplit cross validation and the final fit, as
@@ -640,6 +674,8 @@ def build_lstm_fleet(eng: "engine.LSTMEngine", x, y, rows, lookahead: int = 0, e
     each of its epochs inside the fit launch (``LSTMEngine.fit_stop``), as sklearn's clone hands every fold the same callbacks.  The
     result then carries ``epochs_run`` / ``best_epoch``; history entries past a fit's ``epochs_run`` are NaN.  With
     ``restore_best_weights`` the launch also holds a snapshot of every slot, which ``memory_budget`` counts.
+    ``window``: the detector's smoothing window, as in ``build_fleet``: every fold also gets its thresholds at that window, from
+    the same pass over its float64 fold scores (gb_thresholds_pair_f64).
     """
     torch = engine._torch()
     dev = eng.device
@@ -746,7 +782,14 @@ def build_lstm_fleet(eng: "engine.LSTMEngine", x, y, rows, lookahead: int = 0, e
     y_scale, _ = _minmax_attributes(y_lo, y_hi)
     fold_scale = torch.from_numpy(np.ascontiguousarray(y_scale[M:])).to(dev)
     res = engine.anomaly_score(score_jobs, KM, max_n, pred.to(torch.float64), y, T, scale=fold_scale, want=("tag-anomaly-unscaled", "total-anomaly-scaled"))
-    feat, agg = engine.thresholds(score_jobs, KM, max_n, res["tag-anomaly-unscaled"], res["total-anomaly-scaled"], T, KM, 6, dev)
+    fold_sfeat = fold_sagg = None
+    if window is None:
+        feat, agg = engine.thresholds(score_jobs, KM, max_n, res["tag-anomaly-unscaled"], res["total-anomaly-scaled"], T, KM, 6, dev)
+    else:
+        feat, agg, sfeat, sagg = engine.thresholds_pair(score_jobs, KM, max_n, res["tag-anomaly-unscaled"], res["total-anomaly-scaled"], T, KM, 6,
+                                                        int(window), dev)
+        fold_sfeat = np.ascontiguousarray(host(sfeat).reshape(K, M, T).transpose(1, 0, 2))
+        fold_sagg = np.ascontiguousarray(host(sagg).reshape(K, M).T)
     # the evaluation metrics of ModelBuilder's cross validation reduce to five sums per (fold, tag)
     moments = host(engine.cv_moments(score_jobs, KM, pred, y32, T)).reshape(K, M, 5, T).transpose(1, 0, 2, 3)
     fold_feat = host(feat).reshape(K, M, T).transpose(1, 0, 2)
@@ -765,7 +808,8 @@ def build_lstm_fleet(eng: "engine.LSTMEngine", x, y, rows, lookahead: int = 0, e
         fold_in_min=None if in_lo is None else folds(in_lo), fold_in_max=None if in_hi is None else folds(in_hi), epochs=int(epochs),
         epochs_run=None if stop is None else epochs_run[:M], best_epoch=None if stop is None else best_epoch[:M],
         fold_epochs_run=None if stop is None else epochs_run[M:].reshape(K, M).T.copy(),
-        fold_best_epoch=None if stop is None else best_epoch[M:].reshape(K, M).T.copy())
+        fold_best_epoch=None if stop is None else best_epoch[M:].reshape(K, M).T.copy(), window=None if window is None else int(window),
+        fold_smooth_feat_thr=fold_sfeat, fold_smooth_agg_thr=fold_sagg)
 
 
 # ------------------------------------------------------------------------------------------------ fleet build of K-fold detectors

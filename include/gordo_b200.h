@@ -213,6 +213,19 @@ int gb_thresholds_f64(const gb_job* jobs, int32_t n_jobs, int32_t max_rows, cons
                       const double* total_scaled, int32_t n_out, int32_t window, double* feat_thr,
                       double* agg_thr, int32_t n_slots, void* stream);
 
+/* Both fold thresholds of a detector with a smoothing window in one pass over the score arrays: feat_thr0 / agg_thr0 are
+ * gb_thresholds at window w0 (the 6-row thresholds), feat_thr1 / agg_thr1 at window w1 (the smooth ones), bit for bit.  The
+ * rolling minimum costs the same per row whatever the windows (van Herk / Gil-Werman blocks).  tag_unscaled, feat_thr0 and
+ * feat_thr1 are all NULL or all set, and so are total_scaled, agg_thr0 and agg_thr1.  n_out in [1, GB_MAX_WIDTH], w0, w1 >= 1,
+ * max_rows, n_jobs, n_slots >= 0; any other value is GB_E_ARG / GB_E_SHAPE naming the field, before any launch.  When a warp's
+ * w0 + w1 buffer values do not fit in shared memory, the launch allocates a scratch area of at most 64 MB on the stream. */
+int gb_thresholds_pair(const gb_job* jobs, int32_t n_jobs, int32_t max_rows, const float* tag_unscaled,
+                       const float* total_scaled, int32_t n_out, int32_t w0, int32_t w1, float* feat_thr0,
+                       float* agg_thr0, float* feat_thr1, float* agg_thr1, int32_t n_slots, void* stream);
+int gb_thresholds_pair_f64(const gb_job* jobs, int32_t n_jobs, int32_t max_rows, const double* tag_unscaled,
+                           const double* total_scaled, int32_t n_out, int32_t w0, int32_t w1, double* feat_thr0,
+                           double* agg_thr0, double* feat_thr1, double* agg_thr1, int32_t n_slots, void* stream);
+
 /* ---- K8: column moments behind the builder's cross-validation metrics (build_model.py:250-289, 378-446) ----
  * For job i, over rows yhat[out_row .. out_row+n_rows) and y[x_row .. x_row+n_rows), with e = yhat - y and
  * y0 = the job's first target row:  out[i][q][j] (double) = q0: sum e, q1: sum e^2, q2: sum |e|,
