@@ -175,6 +175,13 @@ int odd_pitch(int width) {
   return p4 * 4;
 }
 
+// A block may opt into 227 KB of shared memory, static and dynamic together: cudaFuncSetAttribute refuses a dynamic size that
+// leaves less than the kernel's static arrays (s_red, s_alpha, s_opt, s_idx, s_phase of ffae_fit_body.cuh: 752 bytes, 808 with
+// OPT; cuobjdump -res-usage reports 1776 / 1824, adding the 1 KB sm_90 reserves for every block).  The plans keep 2 KB for them,
+// which covers either count; tests/test_fit_widths_host.py checks the reported sizes against it.
+constexpr size_t FIT_STATIC_SMEM = 2048;
+constexpr size_t FIT_DYNAMIC_SMEM = 227 * 1024 - FIT_STATIC_SMEM;
+
 // Memory plan of a fit: the first of five layouts that fits.  Everything in shared memory; else the weight image in the slot's
 // L2-resident state area; then, one by one, the dz buffers in L2 as well (at most as many as the two spare thirds of the Adam-v
 // area hold).  Fills the layout fields of `a` (net, image, widths, offsets, pitches, d_global) and the dynamic shared memory.
@@ -204,10 +211,11 @@ int plan_fit(const gb_ffnet* net, FitArgs& a, bool& w_global, size_t& smem) {
     for (int b = 0; b < 3 - a.d_global; ++b) { a.dofs[b] = ofs; ofs += BR * a.dpitch; }
     a.smem_floats = ofs;
     smem = (size_t)ofs * sizeof(float);
-    if (smem <= 227 * 1024 && (long)a.d_global * BR * a.dpitch <= 2L * a.wfloats) break;
+    if (smem <= FIT_DYNAMIC_SMEM && (long)a.d_global * BR * a.dpitch <= 2L * a.wfloats) break;
   }
-  GB_REQUIRE(smem <= 227 * 1024 && (long)a.d_global * BR * a.dpitch <= 2L * a.wfloats, GB_E_SMEM,
-             "architecture needs %zu bytes of shared memory for the activations of one mini-batch chunk", smem);
+  GB_REQUIRE(smem <= FIT_DYNAMIC_SMEM && (long)a.d_global * BR * a.dpitch <= 2L * a.wfloats, GB_E_SMEM,
+             "architecture needs %zu bytes of shared memory for the activations of one mini-batch chunk (at most %zu)", smem,
+             FIT_DYNAMIC_SMEM);
   return GB_OK;
 }
 

@@ -440,7 +440,7 @@ int gb_ffae_fit_reg(const gb_ffnet* net, float* params, float* adam_m, float* ad
                     const gb_dense_reg* reg, void* stream);
 
 /* The memory plan gb_ffae_fit uses for this architecture (host only, no device needed).  The first of five that fits in
- * 227 KB of shared memory: everything in shared memory; the weight image in the slot's L2-resident state area
+ * 227 KB of shared memory less 2 KB for the fit kernels' static arrays: everything in shared memory; the weight image in the slot's L2-resident state area
  * (*weights_in_l2 = 1); then one, two or three of the three dz buffers there as well (*dz_in_l2).  GB_E_SMEM if none fits
  * (gb_ffae_fit refuses the architecture with the same status); either output may be NULL. */
 int gb_ffae_fit_plan(const gb_ffnet* net, int32_t* weights_in_l2, int32_t* dz_in_l2);
