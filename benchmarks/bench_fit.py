@@ -3,6 +3,12 @@ BASELINE configs[2] (scaled): batched training of 64-tag feedforward_hourglass a
 Reports row-epochs/s, microseconds per optimizer step and the CPU oracle (NumPy Keras-style loop) on a small sample.
 
     python benchmarks/bench_fit.py [--machines 296] [--rows 10000] [--epochs 3] [--batch 32] [--loss mse] [--optimizer Nadam]
+                                   [--dropout 0.2 [--repeats 3]]
+
+With --dropout RATE, Keras Dropout(RATE) on every hidden boundary but the output of the encoder's activity-regularized first
+layer (dropout after an activity L1 is not supported): the same fit is
+timed with and without dropout, alternating the two --repeats times in the one process, and the result carries both timings
+(the GPU's name and power limit beside them).
 """
 import argparse, json, os, sys, time
 import numpy as np
@@ -20,6 +26,9 @@ def main():
     ap.add_argument("--loss", default="mse", help="training loss (a canonical name: mse, mae, mape, msle, huber, log_cosh)")
     ap.add_argument("--optimizer", default=None, help="a Keras optimizer name (RMSprop, Adagrad, Adadelta, Adamax, Nadam, AdamW, Adam) "
                     "with its default hyperparameters; without it, Adam through the Adam kernels")
+    ap.add_argument("--dropout", type=float, default=None, help="time the fit with Dropout(RATE) on the hidden boundaries against the same "
+                    "fit without it, alternating")
+    ap.add_argument("--repeats", type=int, default=3, help="with --dropout: timed rounds of each variant")
     a = ap.parse_args()
     import torch
     import __graft_entry__ as ge
@@ -58,6 +67,25 @@ def main():
         "algorithmic_tflops": M * N * E * 90708 / (ms * 1e-3) / 1e12,
         "extrapolated_s_1000_machines_100_epochs": ms * 1e-3 * (100 / E) * (((1000 + sms - 1) // sms) / waves) if N == 10000 else None,
     }
+    if a.dropout is not None:
+        rates = [0.0] + [0.0 if spec.l1[l - 1] else a.dropout for l in range(1, spec.n_layers)]  # not after an activity L1 (refused)
+        eng.fit(p0.clone(), jobs, M, N, x, x, epochs=1, batch_size=B, loss=a.loss, optimizer=opt, dropout=rates)  # warm-up
+        times = {"without": [], "with": []}
+        for _ in range(a.repeats):
+            for name, d in (("without", None), ("with", rates)):
+                p = p0.clone()
+                torch.cuda.synchronize()
+                ev0.record()
+                eng.fit(p, jobs, M, N, x, x, epochs=E, batch_size=B, loss=a.loss, optimizer=opt, dropout=d)
+                ev1.record()
+                torch.cuda.synchronize()
+                times[name].append(ev0.elapsed_time(ev1))
+        per_step = {k: [t * 1e3 / (steps * waves) for t in v] for k, v in times.items()}
+        out["dropout"] = {
+            "rates": rates, "repeats": a.repeats, "ms": times, "us_per_step_per_cta": per_step,
+            "median_cost": float(np.median(per_step["with"]) / np.median(per_step["without"]) - 1.0),
+            "gpu": torch.cuda.get_device_name(dev), "power_limit": _power_limit(),
+        }
     if a.cpu:
         w0 = km.init_ff_weights(spec, np.random.default_rng(0))
         Xc = np.random.default_rng(1).random((2000, a.tags)).astype(np.float32)
@@ -67,6 +95,18 @@ def main():
         out["cpu_oracle_row_epochs_per_s_1core"] = 2000 / dt
         out["cpu_oracle_us_per_step"] = dt * 1e6 / ((2000 + B - 1) // B)
     print(json.dumps(out))
+
+
+def _power_limit():
+    """The card's power limit and maximum SM clock, as nvidia-smi reports them (None where it cannot be read)."""
+    import subprocess
+
+    try:
+        r = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True,
+                           timeout=30)
+        return r.stdout.strip().splitlines()[0] if r.returncode == 0 and r.stdout.strip() else None
+    except (OSError, subprocess.SubprocessError):
+        return None
 
 
 if __name__ == "__main__":

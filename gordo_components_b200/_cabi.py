@@ -79,9 +79,24 @@ def make_dense_reg(kernel_l1=None, kernel_l2=None, bias_l1=None, bias_l2=None) -
     return r
 
 
+class GbDenseDropout(C.Structure):
+    _fields_ = [("rate", C.c_float * GB_MAX_LAYERS)]
+
+
+def make_dense_dropout(rate=None) -> GbDenseDropout:
+    """gb_dense_dropout of per-layer Keras Dropout rates (``rate[l]`` on the input of Dense layer l; zeros where absent)."""
+    r = GbDenseDropout()
+    vals = list(rate or ())
+    if len(vals) > GB_MAX_LAYERS:
+        raise ValueError(f"dropout: {len(vals)} layers is more than {GB_MAX_LAYERS}")
+    for i, v in enumerate(vals):
+        r.rate[i] = float(v)
+    return r
+
+
 EXPORTS = (
     "gb_abi_version", "gb_last_error", "gb_device_check", "gb_ffnet_param_count", "gb_ffnet_param_stride",
-    "gb_ffae_infer_score", "gb_ffae_tc_supported", "gb_ffae_infer_plan", "gb_ffae_infer_score_x64", "gb_ffae_infer_plan_x64", "gb_anomaly_score", "gb_anomaly_score_f64", "gb_minmax_fit", "gb_minmax_f64", "gb_thresholds", "gb_thresholds_f64", "gb_thresholds_pair", "gb_thresholds_pair_f64", "gb_cv_moments", "gb_smooth", "gb_smooth_scores", "gb_quantile", "gb_affine_f64", "gb_gather_rows", "gb_gather_rows_ragged", "gb_minmax_inverse_f32", "gb_minmax_inverse_score_f64", "gb_ffae_fit_state_stride", "gb_ffae_fit", "gb_ffae_fit_split", "gb_ffae_fit_stop", "gb_ffae_fit_plan", "gb_ffae_fit_opt", "gb_ffae_fit_reg",
+    "gb_ffae_infer_score", "gb_ffae_tc_supported", "gb_ffae_infer_plan", "gb_ffae_infer_score_x64", "gb_ffae_infer_plan_x64", "gb_anomaly_score", "gb_anomaly_score_f64", "gb_minmax_fit", "gb_minmax_f64", "gb_thresholds", "gb_thresholds_f64", "gb_thresholds_pair", "gb_thresholds_pair_f64", "gb_cv_moments", "gb_smooth", "gb_smooth_scores", "gb_quantile", "gb_affine_f64", "gb_gather_rows", "gb_gather_rows_ragged", "gb_minmax_inverse_f32", "gb_minmax_inverse_score_f64", "gb_ffae_fit_state_stride", "gb_ffae_fit", "gb_ffae_fit_split", "gb_ffae_fit_stop", "gb_ffae_fit_plan", "gb_ffae_fit_opt", "gb_ffae_fit_reg", "gb_ffae_fit_drop",
     "gb_lstm_param_count", "gb_lstm_param_stride", "gb_lstm_workspace_bytes", "gb_lstm_infer", "gb_lstm_tc_supported", "gb_lstm_tc_workspace_bytes", "gb_lstm_infer_tc", "gb_lstm_tc_ragged_workspace_bytes", "gb_lstm_infer_tc_ragged", "gb_lstm_fit_workspace_bytes", "gb_lstm_fit", "gb_lstm_fit_loss", "gb_lstm_fit_tc_workspace_bytes", "gb_lstm_fit_tc", "gb_lstm_fit_opt", "gb_lstm_fit_tc_opt",
     "gb_lstm_fit_stop_state_bytes", "gb_lstm_fit_stop", "gb_lstm_fit_tc_stop",
     "gb_orthonormal_rows",
@@ -231,6 +246,8 @@ def _declare(lib):
     lib.gb_ffae_fit_opt.restype = C.c_int
     lib.gb_ffae_fit_reg.argtypes = lib.gb_ffae_fit_opt.argtypes[:-1] + [C.POINTER(GbDenseReg), _P]
     lib.gb_ffae_fit_reg.restype = C.c_int
+    lib.gb_ffae_fit_drop.argtypes = lib.gb_ffae_fit_reg.argtypes[:-1] + [C.POINTER(GbDenseDropout), _P]
+    lib.gb_ffae_fit_drop.restype = C.c_int
     for name in ("gb_lstm_fit_opt", "gb_lstm_fit_tc_opt"):
         getattr(lib, name).argtypes = lib.gb_lstm_fit_loss.argtypes[:-1] + [C.POINTER(GbOptimizer), _P]
         getattr(lib, name).restype = C.c_int

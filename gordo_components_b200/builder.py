@@ -48,7 +48,7 @@ from sklearn.preprocessing import MinMaxScaler
 
 from . import __version__, serializer
 from .machine.model.base import GordoBase
-from .machine.model.factories.specs import fit_optimizer, fit_reg, optimizer_key, reg_key
+from .machine.model.factories.specs import dropout_key, fit_dropout, fit_optimizer, fit_reg, optimizer_key, reg_key
 from .machine.model.utils import metric_wrapper
 
 logger = logging.getLogger(__name__)
@@ -348,7 +348,7 @@ class _Canonical:
         s = self.spec
         return (tuple(s.dims), tuple(s.acts), tuple(float(v) for v in s.l1), tuple(sorted(s.adam.items())), tuple(s.metrics), s.loss,
                 None if ragged else len(self.X), self.fit["epochs"], self.fit["batch_size"], self.fit["shuffle"], self.n_splits, int(self.evaluation.get("seed", 0)),
-                self.split, self.early_stopping is not None, self.input_scaler) + optimizer_key(s) + reg_key(s) + self._window_key()  # EarlyStopping's parameters are per-job records
+                self.split, self.early_stopping is not None, self.input_scaler) + optimizer_key(s) + reg_key(s) + dropout_key(s) + self._window_key()  # EarlyStopping's parameters are per-job records
 
 
 def _default_minmax(scaler) -> bool:
@@ -797,7 +797,7 @@ class FleetModelBuilder:
                                input_scaler=first.input_scaler, detector_shuffle=first.split[0], validation_split=first.split[1],
                                validation_batch_size=first.split[2],
                                early_stopping=None if first.early_stopping is None else [c.early_stopping for c in members], loss=first.spec.loss, optimizer=fit_optimizer(first.spec),
-                               reg=fit_reg(first.spec), window=first.window)
+                               reg=fit_reg(first.spec), window=first.window, dropout=fit_dropout(first.spec))
         moments = fb.cv_moments.cpu().numpy()
         scale = fb.scale.cpu().numpy().astype(np.float64)
         engine._torch().cuda.synchronize()
@@ -880,7 +880,8 @@ class FleetModelBuilder:
                                      validation_split=first.split[1], validation_batch_size=first.split[2],
                                      early_stopping=None if first.early_stopping is None else [c.early_stopping for c in members],
                                      window=det.window, smoothing_method=det.smoothing_method, threshold_percentile=det.threshold_percentile,
-                                     loss=first.spec.loss, optimizer=fit_optimizer(first.spec), reg=fit_reg(first.spec))
+                                     loss=first.spec.loss, optimizer=fit_optimizer(first.spec), reg=fit_reg(first.spec),
+                                     dropout=fit_dropout(first.spec))
         torch.cuda.synchronize()
         share = (time.time() - t0) / len(members)  # the bucket's wall time, spread evenly: there is no per-machine time any more
         out = []

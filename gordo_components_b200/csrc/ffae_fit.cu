@@ -16,151 +16,17 @@
 // an L2-resident scratch image (second half of the opaque Adam-m state) and the optimizer runs with the last chunk.
 // The two products with the batch rows as the outer dimension (a.W and dz.W^T) give a lane four rows and a quarter of the reduction
 // index (4x4 register tile, reduce-scatter over the four quarters); the weight gradient gives a thread a 4x2 block of W.
-#include <cuda_pipeline.h>
-#include <math_constants.h>
-#include <type_traits>
-#include "gb_common.cuh"
+#include "ffae_fit_kernels.cuh"
 
 namespace {
 
-constexpr int THREADS = 512;
-constexpr int NWARPS = THREADS / 32;
-constexpr int BR = 32;  // rows of a mini-batch chunk: one row per lane
+using gb_fit::FIT_PLAIN;
+using gb_fit::FIT_SPLIT;
+using gb_fit::FIT_STOP;
+using gb_fit::FitEntry;
 
-struct FitArgs {
-  gb_ffnet net;
-  gb::FFImage im;
-  gb_fit_hparams hp;
-  int apitch[GB_MAX_LAYERS + 1];  // pitch of activation buffer l (l = 0: x staging)
-  int aofs[GB_MAX_LAYERS + 1];    // offset of activation buffer l (l >= 1) in smem floats
-  int xofs[2], yofs[2], dofs[3];
-  int gather_layer, gather_layer2;  // the two forward layers with the fewest tiles (the same layer twice in a one-layer stack): their idle warps issue the cp.async gather of the next chunk
-  int d_global;  // how many of the three dz buffers (from the last one) live in the slot's L2-resident state area instead of shared memory
-  int ypitch, dpitch;
-  int wfloats, smem_floats;
-  int n_in, n_out, max_rows;
-  long pstride, sstride;
-  float* params;
-  float* adam_m;
-  float* adam_v;
-  const gb_job* jobs;
-  const float *x, *y;
-  const int32_t* perm;
-  float *out_loss, *out_acc;
-  long long* trace;  // debug (gb_debug_set_fit_trace): cycles of CTA 0 per phase, summed over the fit; NULL in production
-  // gb_ffae_fit_split only (appended, so that the fields above keep their offsets in the parameter block of every kernel)
-  const gb_fit_split* split;  // per job: held-out positions and row map; NULL = none
-  const int32_t* row_map;
-  int val_batch;
-  float *out_val_loss, *out_val_acc;
-  // gb_ffae_fit_stop only (appended too)
-  const gb_fit_stop* stop;  // per job: the EarlyStopping rule; NULL = none
-  float* best_params;       // [n_slots][pstride]: the snapshots
-  int32_t *out_epochs, *out_best_epoch;
-  // gb_ffae_fit_opt only (appended too): the optimizer of the OPT kernels
-  gb_optimizer opt;
-  // gb_ffae_fit_reg only (appended too): the weight regularizers of the REG kernels
-  gb_dense_reg reg;
-};
-
-__device__ __forceinline__ uint32_t mix32(uint32_t h) {
-  h ^= h >> 16; h *= 0x7feb352dU; h ^= h >> 15; h *= 0x846ca68bU; h ^= h >> 16;
-  return h;
-}
-
-// keyed bijection on [0, n): 4-round Feistel network on the enclosing power of four, cycle-walked into range
-__device__ __forceinline__ uint32_t permute_index(uint32_t i, uint32_t n, uint32_t key) {
-  if (n <= 2) return (n == 2) ? (i ^ (key & 1u)) : 0u;
-  int bits = 32 - __clz(n - 1);
-  if (bits & 1) ++bits;
-  const int half = bits >> 1;
-  const uint32_t mask = (1u << half) - 1u;
-  do {
-    uint32_t l = i >> half, r = i & mask;
-#pragma unroll
-    for (int round = 0; round < 4; ++round) {
-      const uint32_t t = l ^ (mix32(r * 0x9e3779b9U + key + round * 0x85ebca6bU) & mask);
-      l = r;
-      r = t;
-    }
-    i = (l << half) | r;
-  } while (i >= n);
-  return i;
-}
-
-// float -> unsigned with the same ordering (negative values below positive ones)
-__device__ __forceinline__ unsigned order_key(float x) {
-  const unsigned u = __float_as_uint(x);
-  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-
-__device__ __forceinline__ void adam_update(float& w, float g, float& m, float& v, float alpha, float omb1, float omb2,
-                                            float eps) {
-  m += (g - m) * omb1;
-  v += (g * g - v) * omb2;
-  float sq;
-  asm("sqrt.approx.ftz.f32 %0, %1;" : "=f"(sq) : "f"(v));  // ~1 ulp, exact 0 at v = 0
-  w -= __fdividef(alpha * m, sq + eps);
-}
-
-// acc[j][c]: partial sums of rows p + 8 j (j = 0..3) x 4 columns held by lane (p = lane & 7, kq = lane >> 3), to be summed over the four kq.
-// Reduce-scatter in two rounds: the lanes 16 apart split rows {0,1} / {2,3}, then the lanes 8 apart split the remaining pair, so lane
-// (p, kq) ends with the complete sums of row p + 8 kq (12 shuffles instead of 32 for an all-reduce).
-__device__ __forceinline__ void quarter_reduce(const float (&acc)[4][4], int lane, float (&out)[4]) {
-  const bool hi16 = (lane & 16) != 0, hi8 = (lane & 8) != 0;
-  float h[2][4];
-#pragma unroll
-  for (int c = 0; c < 4; ++c) {
-#pragma unroll
-    for (int jj = 0; jj < 2; ++jj) {
-      const float keep = hi16 ? acc[2 + jj][c] : acc[jj][c], send = hi16 ? acc[jj][c] : acc[2 + jj][c];
-      h[jj][c] = keep + __shfl_xor_sync(0xffffffffu, send, 16);
-    }
-  }
-#pragma unroll
-  for (int c = 0; c < 4; ++c) {
-    const float keep = hi8 ? h[1][c] : h[0][c], send = hi8 ? h[0][c] : h[1][c];
-    out[c] = keep + __shfl_xor_sync(0xffffffffu, send, 8);
-  }
-}
-
-// WG = false: the slot's padded weight image lives in shared memory for the whole fit (every 64-tag stack).  WG = true: the image does
-// not fit beside the activations (e.g. the 128-tag hourglass, 245 KB) and lives in the slot's L2-resident state area instead; the
-// code is the same, the loads become global.
-// SPLIT (gb_ffae_fit_split): a job's rows are positions.  Training visits positions [0, n_rows); every epoch then ends with
-// forward-only mini-batches of val_batch rows over the held-out positions [n_rows, n_rows + n_val), in order, whose loss and
-// accuracy are the epoch's validation statistics.  Position p reads row x_row + row_map[map_ofs + p] (x_row + p without a map).
-// The held-out batches are more chunks of the same visiting order, so the cp.async prefetch runs across them as well.
-// STOP (gb_ffae_fit_stop, with SPLIT): Keras' EarlyStopping at the end of every epoch.  Thread 0 applies the job's rule to the
-// monitored history entry it has just written and posts the decision (snapshot, stop) in s_red, free between two epoch_stats;
-// one barrier shares it.  A snapshot is the weight image written to best_params in canonical layout; a job that stops drains
-// its cp.async prefetch and leaves, so its SM takes the next job of the launch.
-// LOSS (a fit whose hp.loss is not MSE): the output layer takes f / f' from gb::loss_value / gb::loss_grad.  Kept apart so that
-// the MSE fits keep the exact code of the kernels without it.
-// OPT (an optimizer other than plain Adam, gb_ffae_fit_opt; instantiated with LOSS only): the weight and bias updates are
-// gb::opt_update on the two state slots (the Adam m / v loads and stores), with the per-step scalars gb::OptStep in place of
-// the Adam step size, computed one step ahead as that is.
-// REG (gb_ffae_fit_reg; instantiated with LOSS and OPT only, as ffae_fit_reg_kernel): Keras kernel / bias regularizers.  Their
-// gradient joins the summed mini-batch gradient in the update loop, which also sums the penalty of the weights it writes, per thread and over real entries
-// only: the next step's penalty is then ready without another pass (a pass over the canonical weights at the start of the launch
-// seeds it).  Every thread adds rows * (its share of the penalty) to its acc_reg once per mini-batch, training or held-out, so the
-// reduction of epoch_stats sums the penalty into the epoch's loss exactly as it sums the activity term.
-// The kernel body, shared by the two kernel templates below (every flag is a compile-time constant where it is included).  The
-// REG kernels are a template of their own, so that the other kernels keep their six-flag names and their exact code.
-// DG: some dz buffers live in global memory too (kept apart so that the usual case addresses them as shared memory)
-template <bool WG, bool DG, bool SPLIT = false, bool STOP = false, bool LOSS = false, bool OPT = false>
-__global__ void __launch_bounds__(THREADS, 1) ffae_fit_kernel(const FitArgs a) {
-  constexpr bool REG = false;
-#include "ffae_fit_body.cuh"
-}
-
-template <bool WG, bool DG, bool SPLIT, bool STOP>
-__global__ void __launch_bounds__(THREADS, 1) ffae_fit_reg_kernel(const FitArgs a) {
-  constexpr bool LOSS = true, OPT = true, REG = true;
-#include "ffae_fit_body.cuh"
-}
-
-// the kernel of one dispatch cell: REG takes the regularized kernels (LOSS and OPT implied)
+// the kernel of one dispatch cell: REG takes the regularized kernels (LOSS and OPT implied); the dropout kernels are launched by
+// gb_fit::launch_drop (ffae_fit_drop.cu)
 template <bool WG, bool DG, bool SPLIT, bool STOP, bool LOSS, bool OPT, bool REG>
 constexpr auto fit_kernel() {
   if constexpr (REG) return &ffae_fit_reg_kernel<WG, DG, SPLIT, STOP>;
@@ -219,14 +85,12 @@ int plan_fit(const gb_ffnet* net, FitArgs& a, bool& w_global, size_t& smem) {
   return GB_OK;
 }
 
-enum FitEntry { FIT_PLAIN, FIT_SPLIT, FIT_STOP };
-
 // gb_ffae_fit (FIT_PLAIN: the kernels without the held-out pass), gb_ffae_fit_split and gb_ffae_fit_stop
 int launch_fit(const gb_ffnet* net, float* params, float* adam_m, float* adam_v, const gb_job* jobs, const gb_fit_split* split,
                int32_t n_jobs, int32_t max_rows, const float* x, const float* y, const int32_t* row_map, const int32_t* perm,
                const gb_fit_hparams* hp, int32_t val_batch, float* out_loss, float* out_acc, float* out_val_loss, float* out_val_acc,
                const gb_fit_stop* stop, float* best_params, int32_t* out_epochs, int32_t* out_best_epoch, FitEntry entry,
-               const gb_optimizer* opt, const gb_dense_reg* reg, void* stream) {
+               const gb_optimizer* opt, const gb_dense_reg* reg, const gb_dense_dropout* drop, void* stream) {
   int rc = gb::validate_ffnet(net);
   if (rc != GB_OK) return rc;
   rc = gb::validate_optimizer(opt);
@@ -254,13 +118,22 @@ int launch_fit(const gb_ffnet* net, float* params, float* adam_m, float* adam_v,
     a.hp.lr = opt->lr; a.hp.beta1 = opt->beta1; a.hp.beta2 = opt->beta2; a.hp.eps = opt->eps;
   }
   if (use_opt) a.opt = *opt;
-  if (reg != nullptr) {  // the REG kernels are OPT kernels: plain Adam, too, runs through gb::opt_update there
-    a.reg = *reg;
+  if (reg != nullptr || drop != nullptr) {  // the REG and DROP kernels are OPT kernels: plain Adam, too, runs through gb::opt_update there
+    if (reg != nullptr) a.reg = *reg;  // else zeros: the DROP kernels add a penalty of 0
     if (opt != nullptr) {
       a.opt = *opt;
     } else {
       a.opt = gb_optimizer{};
       a.opt.kind = GB_OPT_ADAM; a.opt.lr = hp->lr; a.opt.beta1 = hp->beta1; a.opt.beta2 = hp->beta2; a.opt.eps = hp->eps;
+    }
+  }
+  if (drop != nullptr) {
+    for (int l = 0; l < GB_MAX_LAYERS; ++l) {
+      if (drop->rate[l] == 0.f) continue;
+      const double r = (double)drop->rate[l];
+      a.drop_layers |= 1u << l;
+      a.drop_thr[l] = (uint32_t)floor(r * 4294967296.0);
+      a.drop_scale[l] = (float)(1.0 / (1.0 - r));
     }
   }
   const int L = net->n_layers;
@@ -300,10 +173,11 @@ int launch_fit(const gb_ffnet* net, float* params, float* adam_m, float* adam_v,
     return launch(fit_kernel<false, false, false, false, LS, OP, RG>());
   };
   // another optimizer than plain Adam takes the LOSS kernels (their loss switch covers MSE), so it adds 9 instantiations, not 18;
-  // weight regularizers take the 9 ffae_fit_reg_kernel instantiations
+  // weight regularizers take the 9 ffae_fit_reg_kernel instantiations, dropout the 9 ffae_fit_drop_kernel ones (ffae_fit_drop.cu)
   const std::false_type no{};
   const std::true_type yes{};
-  if (reg != nullptr) rc = dispatch(yes, yes, yes);
+  if (drop != nullptr) rc = gb_fit::launch_drop(a, entry, w_global, smem, n_jobs, (cudaStream_t)stream);
+  else if (reg != nullptr) rc = dispatch(yes, yes, yes);
   else if (use_opt) rc = dispatch(yes, yes, no);
   else rc = hp->loss == GB_LOSS_MSE ? dispatch(no, no, no) : dispatch(yes, no, no);
   if (rc != GB_OK) return rc;
@@ -343,7 +217,7 @@ int gb_ffae_fit(const gb_ffnet* net, float* params, float* adam_m, float* adam_v
                 int32_t max_rows, const float* x, const float* y, const int32_t* perm, const gb_fit_hparams* hp,
                 float* out_loss, float* out_acc, void* stream) {
   return launch_fit(net, params, adam_m, adam_v, jobs, nullptr, n_jobs, max_rows, x, y, nullptr, perm, hp, 1, out_loss, out_acc,
-                    nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, FIT_PLAIN, nullptr, nullptr, stream);
+                    nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, FIT_PLAIN, nullptr, nullptr, nullptr, stream);
 }
 
 int gb_ffae_fit_split(const gb_ffnet* net, float* params, float* adam_m, float* adam_v, const gb_job* jobs,
@@ -353,7 +227,7 @@ int gb_ffae_fit_split(const gb_ffnet* net, float* params, float* adam_m, float* 
   GB_REQUIRE(!split || out_val_loss, GB_E_ARG, "split needs out_val_loss");
   GB_REQUIRE(!split || val_batch >= 1, GB_E_ARG, "val_batch=%d must be >= 1", val_batch);
   return launch_fit(net, params, adam_m, adam_v, jobs, split, n_jobs, max_rows, x, y, row_map, perm, hp, split ? val_batch : 1,
-                    out_loss, out_acc, out_val_loss, out_val_acc, nullptr, nullptr, nullptr, nullptr, FIT_SPLIT, nullptr, nullptr, stream);
+                    out_loss, out_acc, out_val_loss, out_val_acc, nullptr, nullptr, nullptr, nullptr, FIT_SPLIT, nullptr, nullptr, nullptr, stream);
 }
 
 int gb_ffae_fit_stop(const gb_ffnet* net, float* params, float* adam_m, float* adam_v, const gb_job* jobs,
@@ -367,15 +241,15 @@ int gb_ffae_fit_stop(const gb_ffnet* net, float* params, float* adam_m, float* a
              "stop needs best_params, out_epochs and out_best_epoch");
   GB_REQUIRE(!stop || gb::aligned16(best_params), GB_E_ARG, "best_params must be 16-byte aligned");
   return launch_fit(net, params, adam_m, adam_v, jobs, split, n_jobs, max_rows, x, y, row_map, perm, hp, split ? val_batch : 1,
-                    out_loss, out_acc, out_val_loss, out_val_acc, stop, best_params, out_epochs, out_best_epoch, FIT_STOP, nullptr, nullptr, stream);
+                    out_loss, out_acc, out_val_loss, out_val_acc, stop, best_params, out_epochs, out_best_epoch, FIT_STOP, nullptr, nullptr, nullptr, stream);
 }
 
-int gb_ffae_fit_reg(const gb_ffnet* net, float* params, float* adam_m, float* adam_v, const gb_job* jobs,
-                    const gb_fit_split* split, int32_t n_jobs, int32_t max_rows, const float* x, const float* y,
-                    const int32_t* row_map, const int32_t* perm, const gb_fit_hparams* hp, int32_t val_batch,
-                    float* out_loss, float* out_acc, float* out_val_loss, float* out_val_acc, const gb_fit_stop* stop,
-                    float* best_params, int32_t* out_epochs, int32_t* out_best_epoch, const gb_optimizer* opt,
-                    const gb_dense_reg* reg, void* stream) {
+int gb_ffae_fit_drop(const gb_ffnet* net, float* params, float* adam_m, float* adam_v, const gb_job* jobs,
+                     const gb_fit_split* split, int32_t n_jobs, int32_t max_rows, const float* x, const float* y,
+                     const int32_t* row_map, const int32_t* perm, const gb_fit_hparams* hp, int32_t val_batch,
+                     float* out_loss, float* out_acc, float* out_val_loss, float* out_val_acc, const gb_fit_stop* stop,
+                     float* best_params, int32_t* out_epochs, int32_t* out_best_epoch, const gb_optimizer* opt,
+                     const gb_dense_reg* reg, const gb_dense_dropout* drop, void* stream) {
   GB_REQUIRE(!split || out_val_loss, GB_E_ARG, "split needs out_val_loss");
   GB_REQUIRE(!split || val_batch >= 1, GB_E_ARG, "val_batch=%d must be >= 1", val_batch);
   GB_REQUIRE(!stop || (best_params && out_epochs && out_best_epoch), GB_E_ARG,
@@ -394,10 +268,34 @@ int gb_ffae_fit_reg(const gb_ffnet* net, float* params, float* adam_m, float* ad
         any = any || f.c[l] != 0.f;
       }
   }
+  bool any_drop = false;  // likewise: all-zero rates run the kernels of gb_ffae_fit_reg
+  if (drop != nullptr) {
+    const int rc = gb::validate_ffnet(net);
+    if (rc != GB_OK) return rc;
+    for (int l = 0; l < GB_MAX_LAYERS; ++l) {
+      const float r = drop->rate[l];
+      GB_REQUIRE(r >= 0.f && r < 1.f, GB_E_ARG, "dropout rate[%d]=%g must be finite, >= 0 and < 1", l, (double)r);  // false for NaN
+      GB_REQUIRE(r == 0.f || l < net->n_layers, GB_E_ARG, "dropout rate[%d]=%g: the net has %d layers (rate[l] is on the input of layer l)",
+                 l, (double)r, net->n_layers);
+      GB_REQUIRE(r == 0.f || l == 0 || net->l1[l - 1] == 0.f, GB_E_ARG,
+                 "dropout rate[%d]=%g on the output of layer %d, which has an activity L1: not supported", l, (double)r, l - 1);
+      any_drop = any_drop || r != 0.f;
+    }
+  }
   const FitEntry entry = stop ? FIT_STOP : split ? FIT_SPLIT : FIT_PLAIN;
   return launch_fit(net, params, adam_m, adam_v, jobs, split, n_jobs, max_rows, x, y, row_map, perm, hp, split ? val_batch : 1,
                     out_loss, out_acc, out_val_loss, out_val_acc, stop, best_params, out_epochs, out_best_epoch, entry, opt,
-                    any ? reg : nullptr, stream);
+                    any ? reg : nullptr, any_drop ? drop : nullptr, stream);
+}
+
+int gb_ffae_fit_reg(const gb_ffnet* net, float* params, float* adam_m, float* adam_v, const gb_job* jobs,
+                    const gb_fit_split* split, int32_t n_jobs, int32_t max_rows, const float* x, const float* y,
+                    const int32_t* row_map, const int32_t* perm, const gb_fit_hparams* hp, int32_t val_batch,
+                    float* out_loss, float* out_acc, float* out_val_loss, float* out_val_acc, const gb_fit_stop* stop,
+                    float* best_params, int32_t* out_epochs, int32_t* out_best_epoch, const gb_optimizer* opt,
+                    const gb_dense_reg* reg, void* stream) {
+  return gb_ffae_fit_drop(net, params, adam_m, adam_v, jobs, split, n_jobs, max_rows, x, y, row_map, perm, hp, val_batch, out_loss,
+                          out_acc, out_val_loss, out_val_acc, stop, best_params, out_epochs, out_best_epoch, opt, reg, nullptr, stream);
 }
 
 int gb_ffae_fit_opt(const gb_ffnet* net, float* params, float* adam_m, float* adam_v, const gb_job* jobs,

@@ -1,6 +1,6 @@
-// Body of the Dense fit kernels (ffae_fit.cu): included inside ffae_fit_kernel and ffae_fit_reg_kernel, where the template flags
-// WG, DG, SPLIT, STOP, LOSS, OPT and REG, THREADS / NWARPS / BR, FitArgs a and the helpers of ffae_fit.cu are in scope.  Not a
-// header of its own: see the description of the flags above the two kernels.
+// Body of the Dense fit kernels (ffae_fit.cu): included inside ffae_fit_kernel, ffae_fit_reg_kernel and ffae_fit_drop_kernel, where
+// the template flags WG, DG, SPLIT, STOP, LOSS, OPT, REG and DROP, THREADS / NWARPS / BR, FitArgs a and the helpers of ffae_fit.cu
+// are in scope.  Not a header of its own: see the description of the flags above the three kernels.
   extern __shared__ __align__(16) float smem[];
   __shared__ float s_red[3][NWARPS];
   __shared__ float s_alpha[2];  // Adam step size of optimizer step t at [t & 1]: written one step ahead, off the critical path
@@ -68,6 +68,7 @@
   auto held_out = [&](int s) -> bool { return SPLIT && s >= steps; };
   auto batch_rows = [&](int s) -> int { return held_out(s) ? min(VB, nv - (s - steps) * VB) : min(B, n - s * B); };
   const uint32_t key_base = mix32((uint32_t)a.hp.seed ^ mix32((uint32_t)(a.hp.seed >> 32) + 0x632be5abU * (uint32_t)(job.slot + 1)));
+  const uint32_t drop_key = DROP ? mix32(key_base ^ 0x2545f491U) : 0u;  // DROP: the job's dropout key (gb_dense_dropout)
 
   auto row_index = [&](int e, int i) -> int {
     if (a.hp.shuffle == 0) return i;
@@ -205,6 +206,26 @@
       __syncthreads();
       stamp(0);
       const bool more2 = more && advance(ne, ns, nc);  // (ne, ns, nc): the chunk after next
+      const int pos0 = c * BR;                          // position of the chunk's first row in its mini-batch
+      uint32_t drop_ks = 0u;                            // DROP: the key of optimizer step t_step
+      if constexpr (DROP) {
+        if (!val) {
+          drop_ks = mix32(drop_key + (uint32_t)t_step * 0x9e3779b9U);
+          if (a.drop_layers & 1u) {  // input dropout, in place on the staged rows (weight_step(0) reads them too)
+            float* xs = smem + a.xofs[cur];
+            const uint32_t thr = a.drop_thr[0];
+            const float sc = a.drop_scale[0];
+            for (int r = warp; r < nb; r += NWARPS) {  // live rows only: a padding row keeps its finite stale values
+              const uint32_t kr = drop_row(drop_ks, pos0 + r, 0);
+              for (int k = lane; k < n_in; k += 32) {
+                const float v = xs[r * a.apitch[0] + k];
+                xs[r * a.apitch[0] + k] = drop_keep(kr, k, thr) ? v * sc : 0.f;
+              }
+            }
+            __syncthreads();
+          }
+        }
+      }
 
       // ---- forward ---------------------------------------------------------------------------
       for (int l = 0; l < L; ++l) {
@@ -215,6 +236,17 @@
         const float* Wl = sW + a.im.wofs[l];
         const float* bl = sW + a.im.bofs[l];
         const float l1c = a.net.l1[l] * (a.hp.l1_div_batch ? 1.f : (float)nbt);
+        bool drop_out = false;  // DROP: this layer's activation is the input of a dropped layer
+        uint32_t out_kr = 0u, out_thr = 0u;
+        float out_sc = 1.f;
+        if constexpr (DROP) {
+          drop_out = !val && ((a.drop_layers >> (l + 1)) & 1u);
+          if (drop_out) {
+            out_kr = drop_row(drop_ks, pos0 + (lane & 7) + 8 * (lane >> 3), l + 1);  // the row this lane stores
+            out_thr = a.drop_thr[l + 1];
+            out_sc = a.drop_scale[l + 1];
+          }
+        }
         // cp.async of the next chunk: off the step's critical path (at the head of a chunk it cost 2 k cycles), half of the rows in each of
         // the two narrowest layers, by the warps without a tile there (a row costs its warp ~700 cycles of dependent address work)
         if (more && (l == a.gather_layer || l == a.gather_layer2)) {
@@ -267,6 +299,14 @@
           o.y = (n0 + 1 < N) ? gb::apply_act(act, s4[1] + bv.y) : 0.f;
           o.z = (n0 + 2 < N) ? gb::apply_act(act, s4[2] + bv.z) : 0.f;
           o.w = (n0 + 3 < N) ? gb::apply_act(act, s4[3] + bv.w) : 0.f;
+          if constexpr (DROP) {
+            if (drop_out) {
+              o.x = drop_keep(out_kr, n0 + 0, out_thr) ? o.x * out_sc : 0.f;
+              o.y = drop_keep(out_kr, n0 + 1, out_thr) ? o.y * out_sc : 0.f;
+              o.z = drop_keep(out_kr, n0 + 2, out_thr) ? o.z * out_sc : 0.f;
+              o.w = drop_keep(out_kr, n0 + 3, out_thr) ? o.w * out_sc : 0.f;
+            }
+          }
           *reinterpret_cast<float4*>(out + row * op + n0) = o;
           if (l1c != 0.f && row < nb) acc_reg += l1c * (fabsf(o.x) + fabsf(o.y) + fabsf(o.z) + fabsf(o.w));
         }
@@ -340,6 +380,17 @@
         const float* aprev = smem + a.aofs[l];  // output of layer l-1
         const float cp = a.net.l1[l - 1] / (a.hp.l1_div_batch ? (float)nbt : 1.f);
         const int p8 = lane & 7, kq = lane >> 3, Nb = Np >> 2;  // lane = (row group, quarter of the n blocks): as in the forward pass
+        bool drop_in = false;  // DROP: layer l's input was dropped in the forward pass
+        uint32_t in_kr = 0u, in_thr = 0u;
+        float in_sc = 1.f;
+        if constexpr (DROP) {
+          drop_in = (a.drop_layers >> l) & 1u;
+          if (drop_in) {
+            in_kr = drop_row(drop_ks, pos0 + p8 + 8 * kq, l);
+            in_thr = a.drop_thr[l];
+            in_sc = a.drop_scale[l];
+          }
+        }
         for (int task = NWARPS - 1 - warp; task < (Kp >> 2); task += NWARPS) {
           const int k0 = task << 2;
           float acc[4][4];
@@ -373,6 +424,13 @@
           const float4 ao = *reinterpret_cast<const float4*>(aprev + row * a.apitch[l] + k0);
           auto dz = [&](float g, float o, int j) -> float {
             if (!live || j >= K) return 0.f;
+            if constexpr (DROP) {
+              if (drop_in) {  // dropped: no gradient; kept: g s act'(a), a = stored value / s
+                if (!drop_keep(in_kr, j, in_thr)) return 0.f;
+                g *= in_sc;
+                o = o / in_sc;
+              }
+            }
             if (cp != 0.f) g += cp * ((o > 0.f) ? 1.f : ((o < 0.f) ? -1.f : 0.f));
             return g * gb::act_grad_from_output(actp, o);
           };

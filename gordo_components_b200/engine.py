@@ -180,22 +180,26 @@ class FFEngine:
     # ------------------------------------------------------------------ K2
     def fit(self, params, jobs_dev, n_jobs: int, max_rows: int, x, y, epochs: int = 1, batch_size: int = 32, shuffle=True,
             perm=None, adam: Optional[Dict[str, float]] = None, seed: int = 0, l1_div_batch: bool = False, state=None,
-            step0: int = 0, loss: str = "mse", optimizer=None, reg=None):
+            step0: int = 0, loss: str = "mse", optimizer=None, reg=None, dropout=None):
         """
         Trains every job's slot in place (``params`` is updated).  Returns (loss [n_jobs, epochs], accuracy, (m, v)).
         ``perm`` (int32 [n_jobs, epochs, max_rows]) pins the visiting order (parity tests).  ``loss``: canonical Keras loss name
         (``_cabi.LOSS_CODES``) the fit minimises and reports.  ``optimizer``: None (Adam from ``adam``) or the (name, record) pair of
         ``factories.specs.resolve_optimizer`` (gb_ffae_fit_opt); (m, v) are then its state slots 0 and 1.  ``reg``: None or the
         per-layer weight regularizer coefficients ``factories.specs.fit_reg`` gives (gb_ffae_fit_reg), added to the loss the fit
-        minimises and reports.
+        minimises and reports.  ``dropout``: None or the per-layer Dropout rates ``factories.specs.fit_dropout`` gives
+        (gb_ffae_fit_drop): ``dropout[l]`` on the input of layer l, in training mini-batches only, masks keyed by ``seed``, the
+        slot and the absolute optimizer step (``step0`` counts), so E one-epoch fits that carry ``step0`` draw the masks of one
+        E-epoch fit.
         """
         hp = _fit_hparams(epochs, batch_size, shuffle, perm, adam, seed, l1_div_batch, step0, loss)
-        hist, acc, *_, mv = self._fit_launch(params, jobs_dev, n_jobs, max_rows, x, y, perm, hp, state, optimizer, reg=reg)
+        hist, acc, *_, mv = self._fit_launch(params, jobs_dev, n_jobs, max_rows, x, y, perm, hp, state, optimizer, reg=reg, dropout=dropout)
         return hist, acc, mv
 
     def fit_split(self, params, jobs_dev, n_jobs: int, max_rows: int, x, y, split=None, row_map=None, val_batch: Optional[int] = None,
                   epochs: int = 1, batch_size: int = 32, shuffle=True, perm=None, adam: Optional[Dict[str, float]] = None, seed: int = 0,
-                  l1_div_batch: bool = False, state=None, step0: int = 0, stop=None, loss: str = "mse", optimizer=None, reg=None):
+                  l1_div_batch: bool = False, state=None, step0: int = 0, stop=None, loss: str = "mse", optimizer=None, reg=None,
+                  dropout=None):
         """
         ``fit`` over row *positions* with Keras' ``validation_split``, in one launch (gb_ffae_fit_opt with a split).  Job i trains on its
         positions [0, n_rows) exactly as ``fit`` trains on its rows, and after every epoch runs the network forward over the held-out
@@ -213,19 +217,21 @@ class FFEngine:
         epochs_run, best_epoch, (m, v)): epochs_run / best_epoch are int32 [n_jobs] (best_epoch -1 when no epoch improved and no
         snapshot was taken), and every history entry past a job's epochs_run is NaN.
 
-        ``loss``, ``optimizer``, ``reg``: as in ``fit``; the held-out statistics report the same loss.
+        ``loss``, ``optimizer``, ``reg``, ``dropout``: as in ``fit``; the held-out statistics report the same loss, without dropout.
         """
         hp = _fit_hparams(epochs, batch_size, shuffle, perm, adam, seed, l1_div_batch, step0, loss)
         vb = int(val_batch if val_batch is not None else batch_size)
         *out, epochs_run, best_epoch, mv = self._fit_launch(params, jobs_dev, n_jobs, max_rows, x, y, perm, hp, state, optimizer, val=True,
-                                                            split=split, row_map=row_map, val_batch=vb, stop=stop, reg=reg)
+                                                            split=split, row_map=row_map, val_batch=vb, stop=stop, reg=reg,
+                                                            dropout=dropout)
         return (*out, mv) if stop is None else (*out, epochs_run, best_epoch, mv)
 
     def _fit_launch(self, params, jobs_dev, n_jobs, max_rows, x, y, perm, hp, state, optimizer, val=False, split=None, row_map=None,
-                    val_batch=1, stop=None, reg=None):
+                    val_batch=1, stop=None, reg=None, dropout=None):
         """
         The one gb_ffae_fit_opt launch of ``fit`` and ``fit_split``, with NULL where there is no split, stop rule or optimizer; with a
-        ``reg`` that has a non-zero coefficient, the gb_ffae_fit_reg launch instead.
+        ``reg`` that has a non-zero coefficient, the gb_ffae_fit_reg launch instead, and with a ``dropout`` that has a non-zero rate,
+        the gb_ffae_fit_drop launch (NULL ``reg`` where it has none).
         Returns (loss, accuracy, val_loss, val_accuracy, epochs_run, best_epoch, (m, v)): val_* (NaN where no held-out pass writes)
         only with ``val``; epochs_run / best_epoch only with ``stop``, which also fills loss / accuracy with NaN first.
         """
@@ -249,7 +255,12 @@ class FFEngine:
         args = (C.byref(self.net), p(params), p(m), p(v), p(jobs_dev), p(split), int(n_jobs), int(max_rows), p(x), p(y), p(row_map), p(perm),
                 C.byref(hp), int(val_batch), *(p(t) for t in out), p(stop), p(best), p(epochs_run), p(best_epoch),
                 None if opt is None else C.byref(opt))
-        if reg is not None and any(v for vals in reg.values() for v in vals):
+        has_reg = reg is not None and any(v for vals in reg.values() for v in vals)
+        if dropout is not None and any(dropout):
+            rec = _cabi.make_dense_reg(**reg) if has_reg else None
+            drop = _cabi.make_dense_dropout(dropout)
+            _cabi.check(self.lib.gb_ffae_fit_drop(*args, None if rec is None else C.byref(rec), C.byref(drop), _stream_ptr()))
+        elif has_reg:
             rec = _cabi.make_dense_reg(**reg)
             _cabi.check(self.lib.gb_ffae_fit_reg(*args, C.byref(rec), _stream_ptr()))
         else:

@@ -334,7 +334,7 @@ def _keras_initial_params(eng: "engine.FFEngine", n_slots: int, generator):
 
 
 def _fit_slots(eng, params, fit_jobs, n_jobs, max_rows, x, y, split, row_map, n_machines, epochs, batch_size, shuffle, adam, seed,
-               validation_batch_size, early_stopping, loss="mse", optimizer=None, reg=None):
+               validation_batch_size, early_stopping, loss="mse", optimizer=None, reg=None, dropout=None):
     """
     The one fit launch of a bucket (job j trains a slot of machine j mod n_machines), with held-out positions and a row map where
     ``split`` is given and an EarlyStopping callback (one for all machines or one per machine) where ``early_stopping`` is.
@@ -349,7 +349,7 @@ def _fit_slots(eng, params, fit_jobs, n_jobs, max_rows, x, y, split, row_map, n_
         stop = engine.make_stop([per_machine[j % n_machines] for j in range(n_jobs)])
     hist, acc, val_loss, val_acc, *ran, _ = eng.fit_split(
         params, fit_jobs, n_jobs, max_rows, x, y, split=split, row_map=row_map, val_batch=validation_batch_size or batch_size, epochs=epochs,
-        batch_size=batch_size, shuffle=shuffle, adam=adam, seed=seed, stop=stop, loss=loss, optimizer=optimizer, reg=reg)
+        batch_size=batch_size, shuffle=shuffle, adam=adam, seed=seed, stop=stop, loss=loss, optimizer=optimizer, reg=reg, dropout=dropout)
     epochs_run, best_epoch = ran or (None, None)
     return hist, acc, val_loss, val_acc, epochs_run, best_epoch
 
@@ -400,7 +400,7 @@ def build_fleet(eng: "engine.FFEngine", x, y, rows, epochs: int = 1, batch_size:
                 adam: Optional[Dict[str, float]] = None, shuffle: bool = True, generator=None, input_scaler: bool = False,
                 detector_shuffle: bool = False, validation_split: float = 0.0, validation_batch_size: Optional[int] = None,
                 early_stopping=None, loss: str = "mse", optimizer=None, keep_init_params: bool = False, reg=None,
-                window: Optional[int] = None) -> FleetBuild:
+                window: Optional[int] = None, dropout=None) -> FleetBuild:
     """
     The batched form of ``gordo build`` for one architecture bucket: for every machine the 3-fold TimeSeriesSplit
     cross-validation (fit on each prefix, thresholds from the following test block: diff.py:176-266) and the final fit on
@@ -431,6 +431,8 @@ def build_fleet(eng: "engine.FFEngine", x, y, rows, epochs: int = 1, batch_size:
     ``loss``: the estimator's canonical Keras loss name (``FFNetSpec.loss``), trained on and reported by every fit.
     ``optimizer``: None (Adam from ``adam``) or the estimator's (name, record) (``factories.specs.fit_optimizer``), for every fit.
     ``reg``: None or the estimator's weight regularizers (``factories.specs.fit_reg``), for every fit.
+    ``dropout``: None or the estimator's Dropout rates (``factories.specs.fit_dropout``), for every fit; each slot draws its masks
+    under its own key (gb_dense_dropout).
     ``keep_init_params``: keep the initial parameters of every slot on the result (``init_params``).
     ``window``: the detector's smoothing window.  Every fold then also gets its thresholds at that window (the detector's
     ``smooth_*`` attributes), from the same pass over the fold scores as its 6-row thresholds (gb_thresholds_pair).
@@ -478,7 +480,7 @@ def build_fleet(eng: "engine.FFEngine", x, y, rows, epochs: int = 1, batch_size:
     fit_jobs = engine.jobs_to_device(engine.make_jobs(np.arange(S), n_train, fit_x), dev)
     hist, acc, val_loss, val_acc, epochs_run, best_epoch = _fit_slots(
         eng, params, fit_jobs, S, N, x, y, split, row_map, M, epochs, batch_size, shuffle, adam, seed, validation_batch_size, early_stopping,
-        loss, optimizer, reg)
+        loss, optimizer, reg, dropout)
     if not held_out:
         val_loss = val_acc = None
     # scalers: final on all rows, fold k on its training prefix (diff.py:173 inside each CV clone), held-out rows included
@@ -970,7 +972,7 @@ def build_kfold_fleet(eng: "engine.FFEngine", x, y, rows, cv, epochs: int = 1, b
                       target_scaler: bool = False, detector_shuffle: bool = False, validation_split: float = 0.0,
                       validation_batch_size: Optional[int] = None, early_stopping=None, window: Optional[int] = None,
                       smoothing_method: Optional[str] = None, threshold_percentile: float = 0.99,
-                      keep_init_params: bool = False, loss: str = "mse", optimizer=None, reg=None) -> KFoldFleetBuild:
+                      keep_init_params: bool = False, loss: str = "mse", optimizer=None, reg=None, dropout=None) -> KFoldFleetBuild:
     """
     The batched ``gordo build`` of one bucket of ``DiffBasedKFCVAnomalyDetector`` machines (diff.py:566-635 in the reference):
     for every machine the K-fold cross validation under ``cv`` (a KFold) and the final fit -- ``(K + 1) * n_machines`` fits in one
@@ -989,7 +991,7 @@ def build_kfold_fleet(eng: "engine.FFEngine", x, y, rows, cv, epochs: int = 1, b
     mapped back by sklearn's float32 inverse and scored in float64 in one pass (gb_minmax_inverse_score_f64), as the per-machine
     detector scores a foreign estimator.  Every scaler's extrema come from gb_minmax_f64 over the test blocks (a slot's rows are a union of blocks)
     with sklearn's float64 attribute arithmetic.  ``detector_shuffle``, ``validation_split``, ``early_stopping``, ``loss``, ``optimizer``,
-    ``reg`` as in ``build_fleet``.
+    ``reg``, ``dropout`` as in ``build_fleet``.
     """
     torch = engine._torch()
     dev = eng.device
@@ -1078,7 +1080,7 @@ def build_kfold_fleet(eng: "engine.FFEngine", x, y, rows, cv, epochs: int = 1, b
     fit_jobs = jobs(np.arange(S), n_train, slot_x)
     hist, acc, val_loss, val_acc, epochs_run, best_epoch = _fit_slots(
         eng, params, fit_jobs, S, N, xf, yf, split, row_map, M, epochs, batch_size, shuffle, adam, seed, validation_batch_size, early_stopping,
-        loss, optimizer, reg)
+        loss, optimizer, reg, dropout)
     if (n_train == slot_n).all():  # nothing held out
         val_loss = val_acc = None
 

@@ -4,8 +4,13 @@ reference hands to ``serializer.from_definition`` and ``model.compile``), transl
 
 Only what the Dense fit and inference kernels run is accepted: a ``Sequential`` of ``Dense`` layers (optionally after one
 ``Input`` / ``InputLayer``) with bias, the default initialisers, the kernel activations of ``SUPPORTED_ACTIVATIONS``, L1 / L2 / L1L2
-kernel and bias regularizers and an L1 activity regularizer.  Everything else is refused with a ValueError naming what is supported.
+kernel and bias regularizers and an L1 activity regularizer, with ``Dropout`` layers between two Dense layers or in front of the
+first one.  Everything else is refused with a ValueError naming what is supported.
 Regularizer defaults are keras 3.3.3's [3P], restated: ``L1(l1=0.01)``, ``L2(l2=0.01)``, ``L1L2(l1=0.0, l2=0.0)``.
+
+A Dropout's rate becomes ``FFNetSpec.dropout[l]``, the rate on the input of the Dense layer l that follows it; the fit kernel
+draws its masks from its own seeded generator (include/gordo_b200.h, gb_dense_dropout), so a Dropout's ``seed`` is taken but
+selects nothing.  Prediction runs without dropout, as Keras' does.
 """
 import math
 from typing import Any, Dict, Optional, Tuple
@@ -21,9 +26,11 @@ _REGULARIZER_DEFAULTS = {"L1": {"l1": 0.01}, "L2": {"l2": 0.01}, "L1L2": {"l1": 
 _REGULARIZER_NAMES = {"l1": "L1", "l2": "L2", "l1_l2": "L1L2", "L1": "L1", "L2": "L2", "L1L2": "L1L2"}
 _DENSE_KEYS = ("units", "activation", "kernel_regularizer", "bias_regularizer", "activity_regularizer", "name", "input_shape",
                "input_dim", "use_bias", "kernel_initializer", "bias_initializer", "kernel_constraint", "bias_constraint")
+_DROPOUT_KEYS = ("rate", "noise_shape", "seed", "name", "input_shape")
 _COMPILE_IGNORED = ("run_eagerly", "jit_compile", "steps_per_execution")
 SUPPORTED = ("a models.Sequential of layers.Dense (units, activation, kernel_regularizer, bias_regularizer, activity_regularizer "
              "with L1 only, name, input_shape / input_dim on the first layer), optionally after one layers.Input / InputLayer; "
+             "layers.Dropout (rate, seed, name, input_shape as the first layer) between two Dense layers or before the first one; "
              "regularizers L1, L2, L1L2")
 
 
@@ -134,6 +141,28 @@ def _dense(kw: dict, first: bool, index: int):
     return units, act, kernel, bias, activity[0], width
 
 
+def _dropout(kw: dict, first: bool, index: int):
+    """(rate, input width or None) of a Dropout layer's arguments."""
+    what = f"layer {index} (Dropout)"
+    unknown = sorted(set(kw) - set(_DROPOUT_KEYS))
+    if unknown:
+        raise ValueError(f"{what}: unsupported arguments {unknown}; supported: {SUPPORTED}")
+    rate = kw.get("rate")
+    if isinstance(rate, bool) or not isinstance(rate, (int, float)) or not math.isfinite(rate) or not 0.0 <= rate < 1.0:
+        raise ValueError(f"{what}: rate={rate!r} must be a finite float in [0, 1)")
+    if kw.get("noise_shape") is not None:
+        raise ValueError(f"{what}: noise_shape is not supported (the fit kernel drops every element independently)")
+    seed = kw.get("seed")
+    if seed is not None and (isinstance(seed, bool) or not isinstance(seed, int)):
+        raise ValueError(f"{what}: seed={seed!r} must be an int or None")
+    width = None
+    if kw.get("input_shape") is not None:
+        if not first:
+            raise ValueError(f"{what}: input_shape is only taken on the first layer")
+        width = _input_width(kw["input_shape"], f"{what} input_shape")
+    return float(rate), width
+
+
 def raw_spec(kind: dict, n_features: Optional[int], n_features_out: Optional[int] = None) -> FFNetSpec:
     """
     The ``FFNetSpec`` of a raw model definition (``kind["spec"]``, ``kind["compile"]``) for rows of ``n_features`` inputs and
@@ -147,8 +176,9 @@ def raw_spec(kind: dict, n_features: Optional[int], n_features_out: Optional[int
     if unknown:
         raise ValueError(f"models.Sequential: unsupported arguments {unknown} (it takes layers and name)")
     layers = kw.get("layers") or []
-    width, dims, acts, l1 = None, [], [], []
+    width, dims, acts, l1, dropout = None, [], [], [], []
     reg = {"kernel_l1": [], "kernel_l2": [], "bias_l1": [], "bias_l2": []}
+    pending = None  # (index, path, rate) of a Dropout that waits for the Dense layer whose input it drops
     for i, item in enumerate(layers):
         lpath, lkw = _entry(item, f"layer {i}")
         name = _name(lpath, "layers")
@@ -157,6 +187,17 @@ def raw_spec(kind: dict, n_features: Optional[int], n_features_out: Optional[int
                 raise ValueError(f"layer {i}: layers.{name} must come first")
             width = _input_layer(name, lkw)
             continue
+        if name == "Dropout":
+            if pending is not None:
+                raise ValueError(f"layer {i} {lpath!r} right after the Dropout of layer {pending[0]} is not supported: two Dropout "
+                                 f"layers in a row; supported: {SUPPORTED}")
+            rate, w = _dropout(lkw, i == 0, i)
+            width = w if w is not None else width
+            if dims and l1[-1] != 0.0 and rate != 0.0:
+                raise ValueError(f"layer {i} {lpath!r} after a Dense layer with an activity_regularizer is not supported: the fit "
+                                 f"kernel keeps only the dropped activation; supported: {SUPPORTED}")
+            pending = (i, lpath, rate)
+            continue
         if name != "Dense":
             raise ValueError(f"layer {i} {lpath!r} is not supported: {SUPPORTED}")
         units, act, kernel, bias, activity, w = _dense(lkw, not dims and width is None, i)
@@ -164,10 +205,15 @@ def raw_spec(kind: dict, n_features: Optional[int], n_features_out: Optional[int
         dims.append(units)
         acts.append(act)
         l1.append(activity)
+        dropout.append(0.0 if pending is None else pending[2])
+        pending = None
         for k, v in zip(reg, (*kernel, *bias)):
             reg[k].append(v)
     if not dims:
         raise ValueError(f"models.Sequential has no Dense layer: {SUPPORTED}")
+    if pending is not None:
+        raise ValueError(f"layer {pending[0]} {pending[1]!r} after the last Dense layer is not supported: it would drop the model's "
+                         f"output; supported: {SUPPORTED}")
     if width is not None and n_features is not None and width != int(n_features):
         raise ValueError(f"the spec's input shape [{width}] does not match the {int(n_features)} features of X")
     if width is None:
@@ -195,4 +241,4 @@ def raw_spec(kind: dict, n_features: Optional[int], n_features_out: Optional[int
     metrics = [metrics] if isinstance(metrics, str) else list(metrics)
     if metrics not in ([], ["accuracy"]):
         raise ValueError(f"compile metrics {metrics!r}: the fit kernels report accuracy only (metrics: none or ['accuracy'])")
-    return FFNetSpec([width, *dims], acts, l1, adam, metrics, loss, opt, opt_cfg, **reg)
+    return FFNetSpec([width, *dims], acts, l1, adam, metrics, loss, opt, opt_cfg, **reg, dropout=dropout if any(dropout) else None)

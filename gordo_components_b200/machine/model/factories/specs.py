@@ -161,10 +161,25 @@ def reg_key(spec) -> tuple:
     return () if reg is None else (("reg", *(tuple(reg[k]) for k in REG_FIELDS)),)
 
 
+def fit_dropout(spec):
+    """What the engine's Dense fits take as ``dropout``: None when the spec has no non-zero Dropout rate, else the per-layer rates
+    (``dropout[l]`` on the input of Dense layer l, 0.0 where there is none)."""
+    rates = [float(v) for v in (getattr(spec, "dropout", None) or [0.0] * (len(spec.dims) - 1))]
+    return rates if any(rates) else None
+
+
+def dropout_key(spec) -> tuple:
+    """A bucket-key suffix that separates machines by Dropout rates: empty when there are none, so that other keys are what they
+    were."""
+    rates = fit_dropout(spec)
+    return () if rates is None else (("dropout", tuple(rates)),)
+
+
 @dataclass
 class FFNetSpec:
     """Dense stack: ``dims[0]`` inputs, ``dims[l+1]`` units / ``acts[l]`` / ``l1[l]`` activity-L1 of layer l.  ``kernel_l1`` ..
-    ``bias_l2``: per-layer weight regularizer coefficients (Keras ``kernel_regularizer`` / ``bias_regularizer``), None = none."""
+    ``bias_l2``: per-layer weight regularizer coefficients (Keras ``kernel_regularizer`` / ``bias_regularizer``), None = none.
+    ``dropout``: per-layer Keras Dropout rates, ``dropout[l]`` on the input of layer l (``dropout[0]``: input dropout), None = none."""
 
     dims: List[int]
     acts: List[str]
@@ -181,6 +196,8 @@ class FFNetSpec:
     kernel_l2: Optional[List[float]] = None
     bias_l1: Optional[List[float]] = None
     bias_l2: Optional[List[float]] = None
+    # likewise: a spec pickled before this field existed loads without dropout
+    dropout: Optional[List[float]] = None
 
     @property
     def n_layers(self):

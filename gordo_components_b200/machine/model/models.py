@@ -29,7 +29,7 @@ from sklearn.metrics import explained_variance_score
 from .base import GordoBase
 from .factories import *  # noqa: F401,F403  -- executes the @register_model_builder decorators
 from .factories.raw import raw_spec
-from .factories.specs import FFNetSpec, LSTMNetSpec, fit_optimizer, fit_reg
+from .factories.specs import FFNetSpec, LSTMNetSpec, fit_dropout, fit_optimizer, fit_reg
 from .register import register_model_builder
 
 logger = logging.getLogger(__name__)
@@ -329,6 +329,7 @@ class KerasBaseEstimator(BaseEstimator, GordoBase):
         spec = self.model.spec
         optimizer = fit_optimizer(spec)  # None: Adam from spec.adam
         reg = fit_reg(spec)  # None: no weight regularizers
+        dropout = fit_dropout(spec)  # None: no Dropout layers
         if spec.dims[0] != X.shape[1] or spec.dims[-1] != y.shape[1]:
             raise ValueError(f"model was built for {spec.dims[0]}->{spec.dims[-1]} features, got X {X.shape} y {y.shape}")
         fit_args = {**self.extract_supported_fit_args(self.kwargs), **kwargs}
@@ -369,7 +370,7 @@ class KerasBaseEstimator(BaseEstimator, GordoBase):
             for e in range(epochs):
                 loss, acc, state = eng.fit(params, jobs, 1, n_train, xd, yd, epochs=1, batch_size=batch_size, shuffle=shuffle,
                                            adam=spec.adam, seed=seed + e, state=state, step0=step0, loss=spec.loss, optimizer=optimizer,
-                                           reg=reg)
+                                           reg=reg, dropout=dropout)
                 step0 += steps
                 logs = {"loss": float(loss[0, 0])}
                 if "accuracy" in history:
@@ -377,6 +378,7 @@ class KerasBaseEstimator(BaseEstimator, GordoBase):
                 if n_val:
                     # keras evaluates the *total* loss (the compiled loss + activity and weight regularisation) on the held-out tail in
                     # batches: the fit kernel with a zero learning rate on a throw-away optimizer state computes exactly that and moves nothing
+                    # (and, without ``dropout``, runs the network as Keras' evaluation does, undropped)
                     vl, va, _ = eng.fit(params, vjobs, 1, n_val, xd, yd, epochs=1, batch_size=vbatch, shuffle=False, adam=frozen, loss=spec.loss,
                                         reg=reg)
                     logs["val_loss"] = float(vl[0, 0])
@@ -392,7 +394,7 @@ class KerasBaseEstimator(BaseEstimator, GordoBase):
             epochs_run = len(history["loss"])
         else:
             loss, acc, _ = eng.fit(params, jobs, 1, n_train, xd, yd, epochs=epochs, batch_size=batch_size, shuffle=shuffle,
-                                   adam=spec.adam, seed=seed, loss=spec.loss, optimizer=optimizer, reg=reg)
+                                   adam=spec.adam, seed=seed, loss=spec.loss, optimizer=optimizer, reg=reg, dropout=dropout)
             history["loss"] = [float(v) for v in loss[0].cpu().numpy()]
             if "accuracy" in history:
                 history["accuracy"] = [float(v) for v in acc[0].cpu().numpy()]
@@ -442,8 +444,9 @@ class KerasRawModelRegressor(KerasAutoEncoder):
     """
     A Dense network from a raw model definition: ``kind`` is the dict itself, ``{"spec": {...models.Sequential: {"layers": [...]}},
     "compile": {"loss": ..., "optimizer": ..., "metrics": ...}}``, as gordo project YAML gives it.  The ``Sequential`` must be a stack
-    of ``Dense`` layers (``factories.raw``); it trains and predicts on the Dense kernels, its L1 / L2 kernel and bias regularizers
-    inside the fit kernel.  Any other graph is refused with a ValueError.  ``score`` is the explained variance, as for
+    of ``Dense`` layers, with ``Dropout`` layers between them or in front of the first one (``factories.raw``); it trains and
+    predicts on the Dense kernels, its L1 / L2 kernel and bias regularizers and its dropout inside the fit kernel (``predict`` runs
+    without dropout, as Keras' does).  Any other graph is refused with a ValueError.  ``score`` is the explained variance, as for
     ``KerasAutoEncoder``.
 
     >>> model = KerasRawModelRegressor(kind={"compile": {"loss": "mse", "optimizer": "adam"},

@@ -439,6 +439,39 @@ int gb_ffae_fit_reg(const gb_ffnet* net, float* params, float* adam_m, float* ad
                     float* best_params, int32_t* out_epochs, int32_t* out_best_epoch, const gb_optimizer* opt,
                     const gb_dense_reg* reg, void* stream);
 
+/* Keras Dropout(rate) on the input of Dense layer l (keras 3.3.3 layers.Dropout -> tf.nn.dropout [3P], restated, not verified against
+ * TF); rate[l] = 0 is the identity, so rate[0] is input dropout and rate[l], l >= 1, drops the activation of layer l-1.  In a training
+ * mini-batch, element k of row i of that input becomes keep ? v * s : 0 with s = (float)(1.0 / (1.0 - (double)rate[l])).  The next
+ * layer's forward pass, its weight gradient and the reported training loss (and so an EarlyStopping monitor on "loss") read the
+ * dropped values; the gradient that flows back through the layer is g * keep * s.  Held-out mini-batches (validation_split) run
+ * without dropout, as Keras' evaluation does.  A fresh mask is drawn for every optimizer step.
+ * The mask is a stateless counter-based hash, in uint32 arithmetic that wraps, with
+ *   mix32(h): h ^= h >> 16; h *= 0x7feb352d; h ^= h >> 15; h *= 0x846ca68b; h ^= h >> 16
+ *   key = mix32(lo ^ mix32(hi + 0x632be5ab * (slot + 1)))   lo / hi: low / high 32 bits of hp->seed; slot: the job's gb_job.slot
+ *                                                           (the key of the shuffle == 1 permutation)
+ *   kd  = mix32(key ^ 0x2545f491)                           the job's dropout key
+ *   ks  = mix32(kd + t * 0x9e3779b9)                        t: the absolute 1-based optimizer step of the mini-batch
+ *                                                           (hp->step0 + 1 for the first mini-batch of the launch)
+ *   kr  = mix32(ks + (p * GB_MAX_LAYERS + l) * 0x85ebca6b)  p: the row's position in its mini-batch, 32 c + r for row r of chunk c
+ *   u   = mix32(kr + k * 0x27d4eb2f)                        k: the unit of the input of layer l
+ * and the element is kept iff u >= floor(rate[l] * 2^32), computed in double.  Because t counts hp->step0, E one-epoch launches
+ * with step0 carried from one to the next draw the masks of one E-epoch launch.  The masks are not Keras' (nor are its initial
+ * weights): a Dropout's own seed does not select them. */
+typedef struct gb_dense_dropout {
+  float rate[GB_MAX_LAYERS];  /* rate on the input of Dense layer l; 0 = none */
+} gb_dense_dropout;
+
+/* gb_ffae_fit_reg with dropout `drop`.  drop NULL, or every rate 0: exactly gb_ffae_fit_reg (same kernel, bit-identical results).
+ * Invalid (GB_E_ARG, nothing enqueued; the message names the layer): a rate that is negative, >= 1 or not finite; a non-zero rate
+ * at l >= net->n_layers; a non-zero rate[l] on the output of a layer with an activity L1 (net->l1[l-1] != 0), whose gradient would
+ * need the undropped activation.  The memory plan (gb_ffae_fit_plan) is the same with or without dropout. */
+int gb_ffae_fit_drop(const gb_ffnet* net, float* params, float* adam_m, float* adam_v, const gb_job* jobs,
+                     const gb_fit_split* split, int32_t n_jobs, int32_t max_rows, const float* x, const float* y,
+                     const int32_t* row_map, const int32_t* perm, const gb_fit_hparams* hp, int32_t val_batch,
+                     float* out_loss, float* out_acc, float* out_val_loss, float* out_val_acc, const gb_fit_stop* stop,
+                     float* best_params, int32_t* out_epochs, int32_t* out_best_epoch, const gb_optimizer* opt,
+                     const gb_dense_reg* reg, const gb_dense_dropout* drop, void* stream);
+
 /* The memory plan gb_ffae_fit uses for this architecture (host only, no device needed).  The first of five that fits in
  * 227 KB of shared memory less 2 KB for the fit kernels' static arrays: everything in shared memory; the weight image in the slot's L2-resident state area
  * (*weights_in_l2 = 1); then one, two or three of the three dz buffers there as well (*dz_in_l2).  GB_E_SMEM if none fits
