@@ -11,6 +11,7 @@ number a `gordo build` user sees.
     python benchmarks/bench_fleet_builder.py --early-stopping --machines 125 --rows 10000 --tags 64 --epochs 100 --single 1
     python benchmarks/bench_fleet_builder.py --kfcv --machines 125 --rows 10000 --tags 64 --epochs 20 --single 1
     python benchmarks/bench_fleet_builder.py --ragged 5000:15000 --machines 125 --tags 64 --epochs 10 --single 1 [--kfcv | --lstm | --example-config]
+    python benchmarks/bench_fleet_builder.py --ttr --scaled --machines 125 --rows 10000 --tags 64 --epochs 10 --single 1 [--lstm]
 
 ``--lstm`` builds DiffBasedAnomalyDetector(KerasLSTMAutoEncoder(lstm_hourglass)) machines instead (batched by
 fleet.build_lstm_fleet).  ``--example-config`` builds the model of gordo's examples/model-configuration.yaml:
@@ -31,6 +32,9 @@ fit launches, and the device time of the fit launches (CUDA events around each, 
 length is its own bucket.
 ``--window W`` gives the plain detectors a smoothing window W (smm) and builds them with FleetModelBuilder(smoothing=True), whose
 fold thresholds at 6 rows and at W come from one gb_thresholds_pair launch.
+``--ttr`` wraps the plain detector's estimator (feed-forward, ``--scaled`` or ``--lstm``) in TransformedTargetRegressor(transformer=
+MinMaxScaler()), the reference's production base estimator under the default TimeSeriesSplit(3), and builds it with
+FleetModelBuilder(target_scaler=True).
 Measured numbers and the card they were measured on are in DESIGN.md §5b and §7.
 """
 import argparse, json, os, sys, tempfile, time
@@ -66,6 +70,8 @@ def main():
     ap.add_argument("--ragged", default=None, metavar="LO:HI", help="per-machine lengths drawn uniformly from [LO, HI]; ragged=True against the default")
     ap.add_argument("--runs", type=int, default=2, help="--ragged: builds of each kind, alternating")
     ap.add_argument("--window", type=int, default=None, help="plain detectors with this smoothing window (smm), batched by FleetModelBuilder(smoothing=True)")
+    ap.add_argument("--ttr", action="store_true", help="the plain detector's estimator inside TransformedTargetRegressor(MinMaxScaler), "
+                                                        "batched by FleetModelBuilder(target_scaler=True)")
     a = ap.parse_args()
     import numpy as np
     import pandas as pd
@@ -106,6 +112,11 @@ def main():
     if a.window is not None and not a.kfcv:
         next(iter(model.values())).update({"window": a.window, "smoothing_method": "smm"})
         flags["smoothing"] = True
+    if a.ttr and not a.kfcv:
+        detector = next(iter(model.values()))
+        detector["base_estimator"] = {"sklearn.compose.TransformedTargetRegressor": {
+            "transformer": "sklearn.preprocessing.MinMaxScaler", "regressor": detector["base_estimator"]}}
+        flags["target_scaler"] = True
     rng = np.random.default_rng(0)
     if a.ragged:
         lo, hi = (int(v) for v in a.ragged.split(":"))
@@ -148,6 +159,8 @@ def main():
                "1 encoding layer, batch 128, validation_split 0.1), KFold(5, shuffle, random_state=0)")
     if a.window is not None and not a.kfcv:
         net += f", smoothing window {a.window}"
+    if a.ttr and not a.kfcv:
+        net = f"TransformedTargetRegressor(MinMaxScaler) of a {net}"
     if a.early_stopping or a.kfcv:
         net += f", EarlyStopping(val_loss, patience 10, min_delta {a.min_delta:g}, restore_best_weights)"
     out = {

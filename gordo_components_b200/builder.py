@@ -19,7 +19,7 @@ With ``FleetModelBuilder(lstm_early_stopping=True)`` an LSTM estimator with one 
 cross-validation ``scores`` block of the metadata is then assembled on the host from ``gb_cv_moments``' five sums per
 (fold, tag).  Any other definition (other transformers in a Pipeline, callbacks unless batched as above, LSTM fits with
 ``validation_split``, K-fold detectors unless ``FleetModelBuilder(kfcv=True)`` batches them under a KFold cv through ``fleet.build_kfold_fleet``,
-custom metrics ...) goes through ``ModelBuilder``: one machine at a time, still on the GPU through the estimators' own fit / predict.
+``TransformedTargetRegressor`` estimators unless ``FleetModelBuilder(target_scaler=True)`` batches them, custom metrics ...) goes through ``ModelBuilder``: one machine at a time, still on the GPU through the estimators' own fit / predict.
 
 Machines are plain dicts in the layout of ``Machine.to_dict()`` (gordo/machine/machine.py:226-246): ``name``, ``model`` (a
 definition), ``dataset``, and optionally ``project_name``, ``evaluation``, ``metadata``, ``runtime``.  ``dataset`` is
@@ -337,18 +337,23 @@ class _Canonical:
         self.X, self.y, self.dataset_meta, self.query_sec = X, y, dataset_meta, query_sec
         self.fit, self.n_splits, self.evaluation = fit, n_splits, evaluation
         self.window = None  # the plain detector's smoothing window (FleetModelBuilder(smoothing=True)), or None
+        self.target_scaler = False  # the estimator is a TransformedTargetRegressor(MinMaxScaler()) (FleetModelBuilder(target_scaler=True))
 
     def _window_key(self) -> tuple:
         """The smoothing window as a bucket field, only when there is one: keys of machines without a window stay as they were.
         The smoothing method does not enter the thresholds, so it does not split buckets."""
         return () if self.window is None else (("window", self.window),)
 
+    def _target_key(self) -> tuple:
+        """The target transformer as a bucket field, only when there is one: keys of machines without one stay as they were."""
+        return (("target_scaler", True),) if self.target_scaler else ()
+
     def bucket(self, ragged: bool = False):
         """The fields machines of one batched build share; ``ragged`` leaves out the row count (``FleetModelBuilder(ragged=True)``)."""
         s = self.spec
         return (tuple(s.dims), tuple(s.acts), tuple(float(v) for v in s.l1), tuple(sorted(s.adam.items())), tuple(s.metrics), s.loss,
                 None if ragged else len(self.X), self.fit["epochs"], self.fit["batch_size"], self.fit["shuffle"], self.n_splits, int(self.evaluation.get("seed", 0)),
-                self.split, self.early_stopping is not None, self.input_scaler) + optimizer_key(s) + reg_key(s) + dropout_key(s) + self._window_key()  # EarlyStopping's parameters are per-job records
+                self.split, self.early_stopping is not None, self.input_scaler) + optimizer_key(s) + reg_key(s) + dropout_key(s) + self._window_key() + self._target_key()  # EarlyStopping's parameters are per-job records
 
 
 def _default_minmax(scaler) -> bool:
@@ -366,13 +371,29 @@ def _window_refusal(model) -> Optional[str]:
     return None
 
 
-def _canonical(index, machine, early_stopping: bool = False, smoothing: bool = False) -> Optional[_Canonical]:
+def _target_regressor(est, target_scaler: bool = True):
+    """
+    (refusal or None, the regressor, whether it sits in a TransformedTargetRegressor) of a detector's base estimator.  A
+    TransformedTargetRegressor is taken only with ``target_scaler`` and a default MinMaxScaler transformer, without ``func`` /
+    ``inverse_func``; any other estimator is its own regressor.
+    """
+    if type(est) is not TransformedTargetRegressor:
+        return None, est, False
+    if est.func is not None or est.inverse_func is not None or est.transformer is None or not _default_minmax(est.transformer):
+        return "TransformedTargetRegressor without a default MinMaxScaler transformer", est, True
+    if not target_scaler:
+        return "a TransformedTargetRegressor is batched with FleetModelBuilder(target_scaler=True)", est, True
+    return None, est.regressor, True
+
+
+def _canonical(index, machine, early_stopping: bool = False, smoothing: bool = False, target_scaler: bool = False) -> Optional[_Canonical]:
     """
     The machine as a candidate for the batched path, or ``None`` with the reason logged.  ``early_stopping``: also take an
     estimator with one Keras ``EarlyStopping`` callback on a metric its fit reports (``FleetModelBuilder(early_stopping=True)``);
     without it any callback sends the machine to ``ModelBuilder``.  ``smoothing``: also take a detector with a smoothing
     ``window`` (a positive int, smm / sma / ewma; ``FleetModelBuilder(smoothing=True)``); without it such a detector goes to
-    ``ModelBuilder``.
+    ``ModelBuilder``.  ``target_scaler``: also take the estimator inside a ``TransformedTargetRegressor`` with a default MinMaxScaler
+    transformer (``FleetModelBuilder(target_scaler=True)``); without it such a detector goes to ``ModelBuilder``.
     """
     from .machine.model.anomaly.diff import DiffBasedAnomalyDetector
     from .machine.model.factories.specs import FFNetSpec
@@ -397,7 +418,10 @@ def _canonical(index, machine, early_stopping: bool = False, smoothing: bool = F
         return no(reason)
     if not _default_minmax(model.scaler):
         return no("detector scaler is not a default MinMaxScaler")
-    ae, input_scaler = _ff_network(model.base_estimator)
+    reason, est, in_ttr = _target_regressor(model.base_estimator, target_scaler)
+    if reason:
+        return no(reason)
+    ae, input_scaler = _ff_network(est)
     if ae is None:
         return no("base_estimator is not a KerasAutoEncoder, bare or behind one default MinMaxScaler")
     reason, fit_args, stopping, vsplit = _ff_fit_arguments(ae, early_stopping)
@@ -423,6 +447,7 @@ def _canonical(index, machine, early_stopping: bool = False, smoothing: bool = F
     split = (bool(model.shuffle), vsplit, int(fit_args.get("validation_batch_size") or fit["batch_size"]) if vsplit else None)
     c = _Canonical(index, machine, model, spec, X, y, dataset_meta, query_sec, fit, split_obj.n_splits, evaluation, input_scaler, split, stopping)
     c.window = None if model.window is None else int(model.window)
+    c.target_scaler = in_ttr
     return c
 
 
@@ -501,11 +526,12 @@ class _CanonicalLSTM(_Canonical):
     def bucket(self, ragged: bool = False):
         s = self.spec
         return (s.key(), tuple(sorted(s.adam.items())), tuple(s.metrics), s.loss, self.lookahead, None if ragged else len(self.X), self.fit["epochs"], self.fit["batch_size"],
-                self.n_splits, int(self.evaluation.get("seed", 0)), self.input_scaler, self.early_stopping is not None) + optimizer_key(s) + self._window_key()  # EarlyStopping's parameters are per-job records
+                self.n_splits, int(self.evaluation.get("seed", 0)), self.input_scaler, self.early_stopping is not None) + optimizer_key(s) + self._window_key() + self._target_key()  # EarlyStopping's parameters are per-job records
 
 
 def _is_lstm_definition(machine) -> bool:
-    """True when the machine's model is a DiffBasedAnomalyDetector around an LSTM estimator (bare or last Pipeline step)."""
+    """True when the machine's model is a DiffBasedAnomalyDetector around an LSTM estimator (bare or last Pipeline step, either of
+    them optionally inside a TransformedTargetRegressor)."""
     from .machine.model.anomaly.diff import DiffBasedAnomalyDetector
     from .machine.model.models import KerasLSTMBaseEstimator
 
@@ -514,12 +540,15 @@ def _is_lstm_definition(machine) -> bool:
     except Exception:  # ModelBuilder raises the definition's own error
         return False
     est = getattr(model, "base_estimator", None) if isinstance(model, DiffBasedAnomalyDetector) else None
+    if isinstance(est, TransformedTargetRegressor):
+        est = est.regressor
     if isinstance(est, Pipeline) and est.steps:
         est = est.steps[-1][1]
     return isinstance(est, KerasLSTMBaseEstimator)
 
 
-def _canonical_lstm(index, machine, wide_batches: bool = False, early_stopping: bool = False, smoothing: bool = False) -> Optional[_CanonicalLSTM]:
+def _canonical_lstm(index, machine, wide_batches: bool = False, early_stopping: bool = False, smoothing: bool = False,
+                    target_scaler: bool = False) -> Optional[_CanonicalLSTM]:
     """
     The LSTM form of the canonical definition -- ``DiffBasedAnomalyDetector(KerasLSTMAutoEncoder | KerasLSTMForecast)``, the network bare
     or behind one default ``MinMaxScaler``, under the evaluation ``_canonical`` accepts -- as a candidate for the batched path, or
@@ -528,6 +557,8 @@ def _canonical_lstm(index, machine, wide_batches: bool = False, early_stopping: 
     ``FleetModelBuilder(lstm_wide_batches=True)``).  ``early_stopping``: also take an estimator with one Keras ``EarlyStopping``
     callback on a metric its fit reports, ``loss`` or (with the accuracy metric) ``accuracy`` (``FleetModelBuilder(lstm_early_stopping=True)``).
     ``smoothing``: also take a detector with a smoothing ``window``, as ``_canonical`` does (``FleetModelBuilder(smoothing=True)``).
+    ``target_scaler``: also take the estimator inside a ``TransformedTargetRegressor`` with a default MinMaxScaler transformer, as
+    ``_canonical`` does (``FleetModelBuilder(target_scaler=True)``).
     """
     from .machine.model.anomaly.diff import DiffBasedAnomalyDetector
     from .engine import LSTMEngine
@@ -560,7 +591,10 @@ def _canonical_lstm(index, machine, wide_batches: bool = False, early_stopping: 
         return no(reason)
     if not _default_minmax(model.scaler):
         return no("detector scaler is not a default MinMaxScaler")
-    est, input_scaler = model.base_estimator, False
+    reason, est, in_ttr = _target_regressor(model.base_estimator, target_scaler)
+    if reason:
+        return no(reason)
+    input_scaler = False
     if type(est) is Pipeline and len(est.steps) == 2 and _default_minmax(est.steps[0][1]):
         est, input_scaler = est.steps[1][1], True
     if type(est) not in (KerasLSTMAutoEncoder, KerasLSTMForecast):
@@ -597,6 +631,7 @@ def _canonical_lstm(index, machine, wide_batches: bool = False, early_stopping: 
     c = _CanonicalLSTM(index, machine, model, spec, X, y, dataset_meta, query_sec, fit, K, evaluation, input_scaler, (False, 0.0, None), stopping,
                        lookahead=la)
     c.window = None if model.window is None else int(model.window)
+    c.target_scaler = in_ttr
     return c
 
 
@@ -611,6 +646,9 @@ class _CanonicalKFold(_Canonical):
         m = self.model  # every field below is a scalar of the shared row maps or of the gb_smooth / gb_quantile launches
         return super().bucket(ragged) + ((self.cv.n_splits, bool(self.cv.shuffle), self.cv.random_state), m.window, m.smoothing_method,
                                    float(m.threshold_percentile), bool(m.shuffle), self.target_scaler)
+
+    def _target_key(self) -> tuple:
+        return ()  # the K-fold key carries the target transformer in a field of its own
 
 
 def _is_kfcv_definition(machine) -> bool:
@@ -655,11 +693,9 @@ def _canonical_kfcv(index, machine, early_stopping: bool = False) -> Optional[_C
         return no(f"window {model.window!r} is not a positive int")
     if model.window is not None and model.smoothing_method not in ("smm", "sma", "ewma"):
         return no(f"smoothing_method {model.smoothing_method!r}")
-    est, target_scaler = model.base_estimator, False
-    if type(est) is TransformedTargetRegressor:
-        if est.func is not None or est.inverse_func is not None or est.transformer is None or not _default_minmax(est.transformer):
-            return no("TransformedTargetRegressor without a default MinMaxScaler transformer")
-        est, target_scaler = est.regressor, True
+    reason, est, target_scaler = _target_regressor(model.base_estimator)
+    if reason:
+        return no(reason)
     ae, input_scaler = _ff_network(est)
     if ae is None:
         return no("the estimator is not a KerasAutoEncoder, bare or behind one default MinMaxScaler")
@@ -723,11 +759,19 @@ class FleetModelBuilder:
     and the detectors carry the ``smooth_*`` thresholds and metadata ``ModelBuilder`` gives them.  The window is a bucket field;
     the method is not (it does not enter the thresholds).  Off by default for the same reason as ``kfcv``: without it such
     machines build through ``ModelBuilder`` as before.
+
+    ``target_scaler``: also batch plain feed-forward and LSTM detectors whose estimator is a ``TransformedTargetRegressor`` with a
+    default MinMaxScaler transformer and no ``func`` / ``inverse_func`` around a network those paths take (bare or behind one default
+    MinMaxScaler) -- the reference's production base estimator under the default ``TimeSeriesSplit`` cv.  Every slot trains on its
+    own scaled targets, and the fold models' predictions go through sklearn's float32 inverse and float64 scoring in one launch
+    (``gb_minmax_inverse_score_f64``).  The target transformer is a bucket field.  Off by default for the same reason as ``kfcv``: without it such
+    machines build through ``ModelBuilder`` as before.  K-fold detectors with a TransformedTargetRegressor are ``kfcv``'s.
     """
 
     def __init__(self, machines: Sequence, early_stopping: bool = False, kfcv: bool = False, lstm_wide_batches: bool = False,
-                 lstm_early_stopping: bool = False, ragged: bool = False, smoothing: bool = False):
+                 lstm_early_stopping: bool = False, ragged: bool = False, smoothing: bool = False, target_scaler: bool = False):
         self.ragged = bool(ragged)
+        self.target_scaler = bool(target_scaler)
         self.smoothing = bool(smoothing)
         self.early_stopping = bool(early_stopping)
         self.kfcv = bool(kfcv)
@@ -747,18 +791,19 @@ class FleetModelBuilder:
 
         return FleetModelBuilder([self.machines[i] for i in fleet.partition(len(self.machines), world)[rank]], early_stopping=self.early_stopping,
                                  kfcv=self.kfcv, lstm_wide_batches=self.lstm_wide_batches, lstm_early_stopping=self.lstm_early_stopping,
-                                 ragged=self.ragged, smoothing=self.smoothing)
+                                 ragged=self.ragged, smoothing=self.smoothing, target_scaler=self.target_scaler)
 
     def build(self, output_dir: Optional[str] = None) -> List[Tuple[Any, dict]]:
         results: List[Optional[Tuple[Any, dict]]] = [None] * len(self.machines)
         buckets: Dict[tuple, List[_Canonical]] = {}
         for i, machine in enumerate(self.machines):
             if _is_lstm_definition(machine):
-                c = _canonical_lstm(i, machine, wide_batches=self.lstm_wide_batches, early_stopping=self.lstm_early_stopping, smoothing=self.smoothing)
+                c = _canonical_lstm(i, machine, wide_batches=self.lstm_wide_batches, early_stopping=self.lstm_early_stopping, smoothing=self.smoothing,
+                                    target_scaler=self.target_scaler)
             elif self.kfcv and _is_kfcv_definition(machine):
                 c = _canonical_kfcv(i, machine, early_stopping=self.early_stopping)
             else:
-                c = _canonical(i, machine, early_stopping=self.early_stopping, smoothing=self.smoothing)
+                c = _canonical(i, machine, early_stopping=self.early_stopping, smoothing=self.smoothing, target_scaler=self.target_scaler)
             if c is None:
                 results[i] = ModelBuilder(machine).build()
             else:
@@ -788,16 +833,21 @@ class FleetModelBuilder:
         eng = engine.ff_engine_for(first.spec)
         rows, K = [len(c.X) for c in members], first.n_splits
         t0 = time.time()
-        x_host = np.concatenate([np.ascontiguousarray(c.X.values, dtype=np.float32) for c in members])
         same_y = all(c.y is c.X for c in members)
-        xd = engine.to_device_f32(x_host, eng.device)
-        yd = xd if same_y else engine.to_device_f32(np.concatenate([np.ascontiguousarray(c.y.values, dtype=np.float32) for c in members]), eng.device)
+        if first.target_scaler:  # TransformedTargetRegressor.fit hands its transformer the float64 targets
+            torch = engine._torch()
+            xd = torch.from_numpy(np.concatenate([np.ascontiguousarray(c.X.values, dtype=np.float64) for c in members])).to(eng.device)
+            yd = xd if same_y else torch.from_numpy(np.concatenate([np.ascontiguousarray(c.y.values, dtype=np.float64) for c in members])).to(eng.device)
+        else:
+            x_host = np.concatenate([np.ascontiguousarray(c.X.values, dtype=np.float32) for c in members])
+            xd = engine.to_device_f32(x_host, eng.device)
+            yd = xd if same_y else engine.to_device_f32(np.concatenate([np.ascontiguousarray(c.y.values, dtype=np.float32) for c in members]), eng.device)
         fb = fleet.build_fleet(eng, xd, yd, rows, epochs=first.fit["epochs"], batch_size=first.fit["batch_size"], n_splits=K,
                                seed=int(first.evaluation.get("seed", 0)), adam=first.spec.adam, shuffle=first.fit["shuffle"],
                                input_scaler=first.input_scaler, detector_shuffle=first.split[0], validation_split=first.split[1],
                                validation_batch_size=first.split[2],
                                early_stopping=None if first.early_stopping is None else [c.early_stopping for c in members], loss=first.spec.loss, optimizer=fit_optimizer(first.spec),
-                               reg=fit_reg(first.spec), window=first.window, dropout=fit_dropout(first.spec))
+                               reg=fit_reg(first.spec), window=first.window, dropout=fit_dropout(first.spec), target_scaler=first.target_scaler)
         moments = fb.cv_moments.cpu().numpy()
         scale = fb.scale.cpu().numpy().astype(np.float64)
         engine._torch().cuda.synchronize()
@@ -837,7 +887,7 @@ class FleetModelBuilder:
                                     n_splits=K, seed=int(first.evaluation.get("seed", 0)), adam=first.spec.adam, input_scaler=first.input_scaler,
                                     loss=first.spec.loss, optimizer=fit_optimizer(first.spec),
                                     early_stopping=None if first.early_stopping is None else [c.early_stopping for c in members],
-                                    window=first.window)
+                                    window=first.window, target_scaler=first.target_scaler)
         engine._torch().cuda.synchronize()
         share = (time.time() - t0) / len(members)  # the bucket's wall time, spread evenly: there is no per-machine time any more
         split_obj = TimeSeriesSplit(n_splits=K)

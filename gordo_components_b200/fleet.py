@@ -190,7 +190,10 @@ class FleetBuild:
                  fold_params=None, cv_moments=None, in_scale=None, in_offset=None, fold_in_scale=None, fold_in_offset=None, steps_per_epoch=None,
                  val_loss=None, val_acc=None, fold_val_loss=None, fold_val_acc=None, epochs=None, epochs_run=None, best_epoch=None,
                  fold_epochs_run=None, fold_best_epoch=None, rows=None, n_test=None, starts=None, init_params=None, window=None,
-                 fold_smooth_feat_thr=None, fold_smooth_agg_thr=None):
+                 fold_smooth_feat_thr=None, fold_smooth_agg_thr=None, y_min=None, y_max=None, fold_y_min=None, fold_y_max=None):
+        # TransformedTargetRegressor(MinMaxScaler()): float64 column extrema of the targets ([M, T]; per CV fold [M, K, T]), which the
+        # transformer and the detector's scaler both saw; None without one (scale / offset are then float32)
+        self.y_min, self.y_max, self.fold_y_min, self.fold_y_max = y_min, y_max, fold_y_min, fold_y_max
         # the detector's smoothing window and every fold's thresholds at it ([M, K, T], [M, K]); None without a window
         self.window, self.fold_smooth_feat_thr, self.fold_smooth_agg_thr = window, fold_smooth_feat_thr, fold_smooth_agg_thr
         # EarlyStopping: epochs each fit ran and its best epoch (-1: none) ([M]; per CV fold [M, K]); None without the callback.
@@ -245,8 +248,9 @@ class FleetBuild:
         tags = list(tags) if tags is not None else list(range(T))
         from sklearn.pipeline import Pipeline
 
+        ttr = None
         if template is not None:
-            est = template.base_estimator
+            ttr, est = _target_regressor_of(template.base_estimator, self.y_min is not None)
             ae = est.steps[-1][1] if isinstance(est, Pipeline) else est
             if isinstance(est, Pipeline) != (self.in_scale is not None):
                 raise ValueError("the template's input scaler and the fleet's do not match")
@@ -257,6 +261,8 @@ class FleetBuild:
             if list(ae.model.spec.dims) != list(eng.dims) or list(ae.model.spec.acts) != list(eng.acts):
                 raise ValueError("template architecture differs from the fleet's")
             ae.model.weights = eng.unpack_params(self.params[m : m + 1])[0]
+        elif self.y_min is not None:
+            raise ValueError("a fleet with a target transformer materialises its detectors from a template")
         else:
             ae = KerasAutoEncoder(kind="feedforward_model", n_features=eng.n_in, n_features_out=T)
             spec = FFNetSpec(list(eng.dims), list(eng.acts), list(eng.l1))
@@ -274,7 +280,11 @@ class FleetBuild:
             ran = int(self.epochs_run[m])
             hist = {k: v[:ran] for k, v in hist.items()}
             ae._history = History(hist, {"verbose": 0, "epochs": int(self.epochs), "steps": steps}, list(range(ran)))
-        sc = self._fill_minmax(MinMaxScaler(), self.scale[m].cpu().numpy().astype(np.float64), self.offset[m].cpu().numpy().astype(np.float64), None)
+        if ttr is not None:
+            _fill_target_regressor(ttr, est, self.y_min[m], self.y_max[m], self.rows[m])
+            sc = _fill_minmax_from_extrema(MinMaxScaler(), self.y_min[m], self.y_max[m], self.rows[m], tags)
+        else:
+            sc = self._fill_minmax(MinMaxScaler(), self.scale[m].cpu().numpy().astype(np.float64), self.offset[m].cpu().numpy().astype(np.float64), None)
         if template is not None:
             det = template
             det.scaler = sc
@@ -400,7 +410,7 @@ def build_fleet(eng: "engine.FFEngine", x, y, rows, epochs: int = 1, batch_size:
                 adam: Optional[Dict[str, float]] = None, shuffle: bool = True, generator=None, input_scaler: bool = False,
                 detector_shuffle: bool = False, validation_split: float = 0.0, validation_batch_size: Optional[int] = None,
                 early_stopping=None, loss: str = "mse", optimizer=None, keep_init_params: bool = False, reg=None,
-                window: Optional[int] = None, dropout=None) -> FleetBuild:
+                window: Optional[int] = None, dropout=None, target_scaler: bool = False) -> FleetBuild:
     """
     The batched form of ``gordo build`` for one architecture bucket: for every machine the 3-fold TimeSeriesSplit
     cross-validation (fit on each prefix, thresholds from the following test block: diff.py:176-266) and the final fit on
@@ -436,9 +446,18 @@ def build_fleet(eng: "engine.FFEngine", x, y, rows, epochs: int = 1, batch_size:
     ``keep_init_params``: keep the initial parameters of every slot on the result (``init_params``).
     ``window``: the detector's smoothing window.  Every fold then also gets its thresholds at that window (the detector's
     ``smooth_*`` attributes), from the same pass over the fold scores as its 6-row thresholds (gb_thresholds_pair).
+    ``target_scaler``: the estimator is ``TransformedTargetRegressor(transformer=MinMaxScaler(), regressor=...)``; x and y are then
+    float64, as the estimator receives them.  Every slot's transformer and the detector's scaler take the float64 extrema of that
+    slot's targets (gb_minmax_f64; held-out rows included), and the slot trains on its own float32 copy of its scaled targets
+    (gb_affine_f64; one copy serves both scalers when y is x and the network is behind an input scaler).  The fold models'
+    predictions go through sklearn's float32 inverse of the fold's transformer and are scored in float64 against the float64
+    targets in one launch (gb_minmax_inverse_score_f64), as the per-machine detector scores a foreign estimator, so the fold
+    thresholds and the result's ``fold_*_thr`` are float64; the metric moments are in target units.
     """
     torch = engine._torch()
     dev = eng.device
+    if target_scaler and (x.dtype != torch.float64 or y.dtype != torch.float64):
+        raise ValueError(f"build_fleet(target_scaler=True) takes float64 x and y, got {x.dtype} / {y.dtype}")
     n, row0 = _machine_rows(x, rows)
     M, K = len(n), n_splits
     test, starts = tss_layout(n, K)
@@ -463,7 +482,26 @@ def build_fleet(eng: "engine.FFEngine", x, y, rows, epochs: int = 1, batch_size:
             row_map = torch.from_numpy(maps).to(dev)
         split = engine.make_split(slot_n - n_train, map_ofs)
     in_scale = in_offset = None
-    if input_scaler:
+    y64 = y_lo = y_hi = None
+    if target_scaler:
+        y64, same_y, total = y, y is x, int(n.sum())
+        prefix_jobs = engine.jobs_to_device(engine.make_jobs(np.arange(S), slot_n, fit_x), dev)
+        y_lo, y_hi = _slot_extrema(prefix_jobs, S, N, y)
+        t_scale_h, t_offset_h = _minmax_attributes(y_lo, y_hi)
+        t_scale, t_offset = _f64(t_scale_h, dev), _f64(t_offset_h, dev)
+        # slot s works on its own copies of its machine's rows: the stacked machines repeated K + 1 times, slot s at copy0[s]
+        copy0 = np.arange(K + 1, dtype=np.int64).repeat(M) * total + fit_x
+        copy_jobs = engine.jobs_to_device(engine.make_jobs(np.arange(S), np.tile(n, K + 1), fit_x, copy0), dev)
+        if input_scaler:
+            in_lo, in_hi = (y_lo, y_hi) if same_y else _slot_extrema(prefix_jobs, S, N, x)
+            in_scale, in_offset = (_f64(v, dev) for v in _minmax_attributes(in_lo, in_hi))
+            x = engine.affine_f64(copy_jobs, S, N, x, in_scale, in_offset, out_rows=(K + 1) * total)
+        else:
+            x = x[:total].to(torch.float32).repeat(K + 1, 1)
+        # the same extrema and the same arithmetic give the same copy when the input scaler and the transformer see one array
+        y = x if (input_scaler and same_y) else engine.affine_f64(copy_jobs, S, N, y64, t_scale, t_offset, out_rows=(K + 1) * total)
+        fit_x = copy0
+    elif input_scaler:
         prefix_jobs = engine.jobs_to_device(engine.make_jobs(np.arange(S), slot_n, fit_x), dev)
         _, _, lo, hi = engine.minmax_fit(prefix_jobs, S, N, x, eng.n_in, S, dev, return_minmax=True)
         lo, span = lo.double(), hi.double() - lo.double()
@@ -484,15 +522,29 @@ def build_fleet(eng: "engine.FFEngine", x, y, rows, epochs: int = 1, batch_size:
     if not held_out:
         val_loss = val_acc = None
     # scalers: final on all rows, fold k on its training prefix (diff.py:173 inside each CV clone), held-out rows included
-    all_jobs = engine.jobs_to_device(engine.make_jobs(np.arange(S), slot_n, fit_x), dev) if held_out else fit_jobs
-    scale, offset = eng.minmax_fit(all_jobs, S, N, y, S)
+    if target_scaler:  # the detector's scaler saw the float64 targets too
+        scale, offset = t_scale, t_offset
+    else:
+        all_jobs = engine.jobs_to_device(engine.make_jobs(np.arange(S), slot_n, fit_x), dev) if held_out else fit_jobs
+        scale, offset = eng.minmax_fit(all_jobs, S, N, y, S)
     # fold scoring on the test blocks: job k*M + m scores fold k of machine m, outputs back to back
     KM = K * M
     fk, fm = np.repeat(np.arange(K), M), np.tile(np.arange(M), K)
     sc_n = test[fm]
     sc_jobs = engine.jobs_to_device(engine.make_jobs(M + np.arange(KM), sc_n, fit_x[M:] + starts[fm, fk], _prefix(sc_n)), dev)
     max_test = int(test.max())
-    res = eng.infer_score(params, sc_jobs, KM, max_test, x, y, scale, out_rows=int(sc_n.sum()), want=("tag-anomaly-unscaled", "total-anomaly-scaled"))
+    want = ("tag-anomaly-unscaled", "total-anomaly-scaled")
+    if target_scaler:
+        # the fold models' outputs, then sklearn's float32 inverse of the fold's transformer and float64 scoring against the float64
+        # targets (at their own rows, x_row) with the fold detector's multiplier, transform(1) - transform(0)
+        pred = eng.infer_score(params, sc_jobs, KM, max_test, x, out_rows=int(sc_n.sum()))["model-output"]
+        mom_jobs = engine.jobs_to_device(engine.make_jobs(M + np.arange(KM), sc_n, row0[fm] + starts[fm, fk], _prefix(sc_n)), dev)
+        res = engine.minmax_inverse_score_f64(mom_jobs, KM, max_test, pred, y64, t_scale, t_offset, scale=_f64((t_scale_h + t_offset_h) - t_offset_h, dev),
+                                              want=want, out_rows=int(sc_n.sum()), out={"model-output": pred})
+        y_true = y64.to(torch.float32)
+    else:
+        res = eng.infer_score(params, sc_jobs, KM, max_test, x, y, scale, out_rows=int(sc_n.sum()), want=want)
+        mom_jobs, y_true = sc_jobs, y
     fold_sfeat = fold_sagg = None
     if window is None:
         feat, agg = eng.thresholds(sc_jobs, KM, max_test, res["tag-anomaly-unscaled"], res["total-anomaly-scaled"], S, window=6)
@@ -502,7 +554,7 @@ def build_fleet(eng: "engine.FFEngine", x, y, rows, epochs: int = 1, batch_size:
         fold_sagg = sagg[M:].view(K, M).t().contiguous()
     T = eng.n_out
     # the evaluation metrics of ModelBuilder's cross validation (build_model.py:250-289) reduce to five sums per (fold, tag)
-    moments = engine.cv_moments(sc_jobs, KM, res["model-output"], y, T).view(K, M, 5, T).permute(1, 0, 2, 3).contiguous()
+    moments = engine.cv_moments(mom_jobs, KM, res["model-output"], y_true, T).view(K, M, 5, T).permute(1, 0, 2, 3).contiguous()
     fold_params = params[M:].view(K, M, -1).permute(1, 0, 2).contiguous()
     fold_feat = feat[M:].view(K, M, T).permute(1, 0, 2).contiguous()
     fold_agg = agg[M:].view(K, M).t().contiguous()
@@ -521,7 +573,28 @@ def build_fleet(eng: "engine.FFEngine", x, y, rows, epochs: int = 1, batch_size:
                       epochs_run=None if epochs_run is None else epochs_run[:M], best_epoch=None if best_epoch is None else best_epoch[:M],
                       fold_epochs_run=fold_jobs(epochs_run), fold_best_epoch=fold_jobs(best_epoch), rows=n, n_test=test, starts=starts,
                       init_params=init_params, window=None if window is None else int(window), fold_smooth_feat_thr=fold_sfeat,
-                      fold_smooth_agg_thr=fold_sagg)
+                      fold_smooth_agg_thr=fold_sagg, **({} if y_lo is None else dict(y_min=y_lo[:M], y_max=y_hi[:M], fold_y_min=_folds(y_lo, M, K),
+                                                                                      fold_y_max=_folds(y_hi, M, K))))
+
+
+def _f64(a, device):
+    """A host array as a float64 device tensor."""
+    return engine._torch().from_numpy(np.ascontiguousarray(a, dtype=np.float64)).to(device)
+
+
+def _slot_extrema(jobs_dev, n_jobs, max_rows, a64):
+    """Float64 column (min, max) of every job's rows as host arrays [n_jobs, cols] (gb_minmax_f64); ValueError when a column has no
+    finite value."""
+    lo, hi = (t.cpu().numpy() for t in engine.minmax_f64(jobs_dev, n_jobs, max_rows, a64, n_jobs))
+    if not (np.isfinite(lo).all() and np.isfinite(hi).all()):
+        raise ValueError("a column without finite values in a training block")
+    return lo, hi
+
+
+def _folds(a, n_machines: int, n_splits: int):
+    """Slot-ordered host rows [S, ...] (finals, then fold k of machine m at M + k*M + m) -> every machine's folds [M, K, ...]."""
+    M, K = n_machines, n_splits
+    return np.ascontiguousarray(np.swapaxes(a[M:].reshape((K, M) + a.shape[1:]), 0, 1))
 
 
 # ------------------------------------------------------------------------------------------------ fleet build of LSTM detectors
@@ -543,6 +616,31 @@ def _fill_minmax_from_extrema(sc, lo, hi, n_samples, names):
     return sc
 
 
+def _target_regressor_of(est, target_scaler: bool):
+    """(the TransformedTargetRegressor or None, the estimator to fill: a clone of its regressor, or ``est`` itself) of a template's
+    base estimator; ValueError when the template and the fleet disagree on the target transformer."""
+    from sklearn.base import clone
+    from sklearn.compose import TransformedTargetRegressor
+
+    ttr = est if isinstance(est, TransformedTargetRegressor) else None
+    if (ttr is not None) != bool(target_scaler):
+        raise ValueError("the template's target transformer and the fleet's do not match")
+    return ttr, (clone(ttr.regressor) if ttr is not None else est)
+
+
+def _fill_target_regressor(ttr, reg, lo, hi, n_samples):
+    """What ``TransformedTargetRegressor.fit`` leaves: the transformer fitted on the target array (extrema ``lo`` / ``hi``), the
+    fitted regressor clone ``reg``, and the regressor's input names."""
+    from sklearn.base import clone
+
+    ttr._training_dim = 2
+    ttr.transformer_ = _fill_minmax_from_extrema(clone(ttr.transformer), lo, hi, n_samples, None)
+    ttr.regressor_ = reg
+    if hasattr(reg, "feature_names_in_"):
+        ttr.feature_names_in_ = reg.feature_names_in_
+    return ttr
+
+
 class LSTMFleetBuild:
     """
     Result of ``build_lstm_fleet``: what ``ModelBuilder._build`` produces for one LSTM machine -- final weights, target scaler,
@@ -553,7 +651,11 @@ class LSTMFleetBuild:
     def __init__(self, eng, n_machines, n_splits, rows, lookahead, batch_size, starts, n_test, params, fold_params, init_params, loss, acc,
                  fold_loss, fold_acc, y_min, y_max, fold_y_min, fold_y_max, feat_thr, agg_thr, fold_feat_thr, fold_agg_thr, cv_moments,
                  fold_predictions, in_min=None, in_max=None, fold_in_min=None, fold_in_max=None, epochs=None, epochs_run=None, best_epoch=None,
-                 fold_epochs_run=None, fold_best_epoch=None, window=None, fold_smooth_feat_thr=None, fold_smooth_agg_thr=None):
+                 fold_epochs_run=None, fold_best_epoch=None, window=None, fold_smooth_feat_thr=None, fold_smooth_agg_thr=None,
+                 target_scaler=False):
+        # the estimator is a TransformedTargetRegressor(MinMaxScaler()), whose transformer saw the same targets as the detector's
+        # scaler (y_min / y_max); fold_predictions are then in target units
+        self.target_scaler = bool(target_scaler)
         # the detector's smoothing window and every fold's thresholds at it ([M, K, T], [M, K] float64); None without a window
         self.window, self.fold_smooth_feat_thr, self.fold_smooth_agg_thr = window, fold_smooth_feat_thr, fold_smooth_agg_thr
         # EarlyStopping: epochs each fit ran and its best epoch (-1: none) ([M]; per CV fold [M, K]) as int32 host arrays; None without
@@ -596,9 +698,10 @@ class LSTMFleetBuild:
         eng = self.eng
         T, K = eng.n_out, self.n_splits
         tags = list(tags) if tags is not None else list(range(T))
+        ttr = None
         if template is not None:
             det = template
-            est = det.base_estimator
+            ttr, est = _target_regressor_of(det.base_estimator, self.target_scaler)
             lstm = est.steps[-1][1] if isinstance(est, Pipeline) else est
             if isinstance(est, Pipeline) != (self.in_min is not None):
                 raise ValueError("the template's input scaler and the fleet's do not match")
@@ -610,6 +713,8 @@ class LSTMFleetBuild:
                 raise ValueError("template architecture differs from the fleet's")
             if isinstance(est, Pipeline):
                 _fill_minmax_from_extrema(est.steps[0][1], self.in_min[m], self.in_max[m], self.rows[m], input_tags)
+        elif self.target_scaler:
+            raise ValueError("a fleet with a target transformer materialises its detectors from a template")
         else:
             cls = KerasLSTMForecast if self.lookahead else KerasLSTMAutoEncoder
             lstm = cls(kind="lstm_model", lookback_window=eng.lookback, batch_size=self.batch_size, encoding_dim=tuple(eng.units),
@@ -628,7 +733,10 @@ class LSTMFleetBuild:
             hist = {k: v[:ran] for k, v in hist.items()}
             lstm._history = History(hist, {"verbose": 0, "epochs": int(self.epochs), "steps": int(self.machine_steps[m])}, list(range(ran)))
         lstm.model.history = lstm._history
-        _fill_minmax_from_extrema(det.scaler, self.y_min[m], self.y_max[m], self.rows[m], tags)
+        if ttr is not None:
+            _fill_target_regressor(ttr, est, self.y_min[m], self.y_max[m], self.rows[m])
+        # a fresh scaler: detectors made from definitions without a scaler share the constructor's default MinMaxScaler object
+        det.scaler = _fill_minmax_from_extrema(MinMaxScaler(), self.y_min[m], self.y_max[m], self.rows[m], tags)
         det.feature_thresholds_ = pd.Series(self.feat_thr[m].copy(), index=tags, name=f"fold-{K - 1}")
         det.aggregate_threshold_ = float(self.agg_thr[m])
         det.feature_thresholds_per_fold_ = pd.DataFrame(self.fold_feat_thr[m].copy(), columns=tags, index=[f"fold-{k}" for k in range(K)])
@@ -653,7 +761,7 @@ class _FoldBlocks:
 def build_lstm_fleet(eng: "engine.LSTMEngine", x, y, rows, lookahead: int = 0, epochs: int = 1, batch_size: int = 32, n_splits: int = 3,
                      seed: int = 0, adam: Optional[Dict[str, float]] = None, input_scaler: bool = False, memory_budget: int = 8 << 30,
                      keep_init_params: bool = False, generator=None, loss: str = "mse", optimizer=None, early_stopping=None,
-                     window: Optional[int] = None) -> LSTMFleetBuild:
+                     window: Optional[int] = None, target_scaler: bool = False) -> LSTMFleetBuild:
     """
     The batched ``gordo build`` of one bucket of LSTM machines (``DiffBasedAnomalyDetector(KerasLSTMAutoEncoder | KerasLSTMForecast)``,
     the network bare or behind one MinMaxScaler): for every machine the TimeSeriesSplit cross validation and the final fit, as
@@ -678,6 +786,10 @@ def build_lstm_fleet(eng: "engine.LSTMEngine", x, y, rows, lookahead: int = 0, e
     ``restore_best_weights`` the launch also holds a snapshot of every slot, which ``memory_budget`` counts.
     ``window``: the detector's smoothing window, as in ``build_fleet``: every fold also gets its thresholds at that window, from
     the same pass over its float64 fold scores (gb_thresholds_pair_f64).
+    ``target_scaler``: the estimator is ``TransformedTargetRegressor(transformer=MinMaxScaler(), regressor=...)``.  Its transformer
+    sees all of a slot's rows of y (the detector scaler's extrema), and every slot trains on its own float32 copy of its scaled
+    targets (gb_affine_f64).  The fold predictions go through sklearn's float32 inverse of the fold's transformer and are scored in
+    float64 in one launch (gb_minmax_inverse_score_f64), so ``fold_predictions`` and the metric moments are in target units.
     """
     torch = engine._torch()
     dev = eng.device
@@ -730,6 +842,16 @@ def build_lstm_fleet(eng: "engine.LSTMEngine", x, y, rows, lookahead: int = 0, e
     else:
         xf = y32 if y is x else x.to(torch.float32)
         yf, x_row = y32, base
+    if target_scaler:
+        # TransformedTargetRegressor(MinMaxScaler()): the transformer saw the extrema above, and slot s trains on its own float32 copy of
+        # its scaled targets at x_row[s], laid out as the input scaler's copies are (one copy for both when they see the same array)
+        total = int(n.sum())
+        if not input_scaler:
+            x_row = np.arange(K + 1, dtype=np.int64).repeat(M) * total + base
+            xf = xf[:total].repeat(K + 1, 1)
+        copy_jobs = engine.jobs_to_device(engine.make_jobs(np.arange(S), np.tile(n, K + 1), base, x_row), dev)
+        t_scale, t_offset = _minmax_attributes(y_lo, y_hi)
+        yf = xf if (input_scaler and y is x) else engine.affine_f64(copy_jobs, S, N, y, _f64(t_scale, dev), _f64(t_offset, dev), out_rows=(K + 1) * total)
 
     # fits: chunks of whole machines (final + K folds) whose workspace fits the budget
     # (batches above 32 windows train on the tensor-core family, whose workspace grows with the batch)
@@ -781,9 +903,14 @@ def build_lstm_fleet(eng: "engine.LSTMEngine", x, y, rows, lookahead: int = 0, e
         pred = eng.infer(params, infer_jobs, KM, max_n, xf, int(job_n.sum()))
     # targets tail-aligned to the predictions, scored in float64 as the per-machine detector scores LSTM output (diff.py:350-385)
     score_jobs = engine.jobs_to_device(engine.make_jobs(np.arange(KM), job_n, row0[fm] + test_start + L - 1 + la, out0), dev)
-    y_scale, _ = _minmax_attributes(y_lo, y_hi)
-    fold_scale = torch.from_numpy(np.ascontiguousarray(y_scale[M:])).to(dev)
-    res = engine.anomaly_score(score_jobs, KM, max_n, pred.to(torch.float64), y, T, scale=fold_scale, want=("tag-anomaly-unscaled", "total-anomaly-scaled"))
+    y_scale, y_offset = _minmax_attributes(y_lo, y_hi)
+    want = ("tag-anomaly-unscaled", "total-anomaly-scaled")
+    if target_scaler:  # sklearn's float32 inverse of the fold's transformer, in place, and float64 scoring with transform(1) - transform(0)
+        res = engine.minmax_inverse_score_f64(score_jobs, KM, max_n, pred, y, _f64(y_scale[M:], dev), _f64(y_offset[M:], dev),
+                                              scale=_f64(((y_scale + y_offset) - y_offset)[M:], dev), want=want, out={"model-output": pred})
+    else:
+        fold_scale = torch.from_numpy(np.ascontiguousarray(y_scale[M:])).to(dev)
+        res = engine.anomaly_score(score_jobs, KM, max_n, pred.to(torch.float64), y, T, scale=fold_scale, want=want)
     fold_sfeat = fold_sagg = None
     if window is None:
         feat, agg = engine.thresholds(score_jobs, KM, max_n, res["tag-anomaly-unscaled"], res["total-anomaly-scaled"], T, KM, 6, dev)
@@ -811,7 +938,7 @@ def build_lstm_fleet(eng: "engine.LSTMEngine", x, y, rows, lookahead: int = 0, e
         epochs_run=None if stop is None else epochs_run[:M], best_epoch=None if stop is None else best_epoch[:M],
         fold_epochs_run=None if stop is None else epochs_run[M:].reshape(K, M).T.copy(),
         fold_best_epoch=None if stop is None else best_epoch[M:].reshape(K, M).T.copy(), window=None if window is None else int(window),
-        fold_smooth_feat_thr=fold_sfeat, fold_smooth_agg_thr=fold_sagg)
+        fold_smooth_feat_thr=fold_sfeat, fold_smooth_agg_thr=fold_sagg, target_scaler=target_scaler)
 
 
 # ------------------------------------------------------------------------------------------------ fleet build of K-fold detectors
@@ -859,9 +986,8 @@ class KFoldFleetBuild:
 
     def _fill(self, s: int, template, tags, input_tags):
         """``template`` with the fitted state of slot ``s``: scalers, weights, History, the target transformer."""
-        from sklearn.base import clone
-        from sklearn.compose import TransformedTargetRegressor
         from sklearn.pipeline import Pipeline
+        from sklearn.preprocessing import MinMaxScaler
 
         from .machine.model.models import History
 
@@ -871,11 +997,7 @@ class KFoldFleetBuild:
         T = eng.n_out
         tags = list(tags) if tags is not None else list(range(T))
         det = template
-        est = det.base_estimator
-        ttr = est if isinstance(est, TransformedTargetRegressor) else None
-        if (ttr is not None) != self.target_scaler:
-            raise ValueError("the template's target transformer and the fleet's do not match")
-        reg = clone(ttr.regressor) if ttr is not None else est
+        ttr, reg = _target_regressor_of(det.base_estimator, self.target_scaler)
         ae = reg.steps[-1][1] if isinstance(reg, Pipeline) else reg
         if isinstance(reg, Pipeline) != (self.in_min is not None):
             raise ValueError("the template's input scaler and the fleet's do not match")
@@ -893,13 +1015,10 @@ class KFoldFleetBuild:
             hist["val_accuracy"] = [float(v) for v in self.val_acc[s, :ran]]
         ae._history = History(hist, {"verbose": 0, "epochs": int(self.epochs), "steps": int(self.slot_steps[s])}, list(range(ran)))
         ae.model.history = ae._history
-        if ttr is not None:  # what TransformedTargetRegressor.fit leaves: the transformer fitted on the target array, a fitted clone
-            ttr._training_dim = 2
-            ttr.transformer_ = _fill_minmax_from_extrema(clone(ttr.transformer), self.y_min[s], self.y_max[s], n_rows, None)
-            ttr.regressor_ = reg
-            if hasattr(reg, "feature_names_in_"):
-                ttr.feature_names_in_ = reg.feature_names_in_
-        _fill_minmax_from_extrema(det.scaler, self.y_min[s], self.y_max[s], n_rows, tags)
+        if ttr is not None:
+            _fill_target_regressor(ttr, reg, self.y_min[s], self.y_max[s], n_rows)
+        # a fresh scaler: detectors made from definitions without a scaler share the constructor's default MinMaxScaler object
+        det.scaler = _fill_minmax_from_extrema(MinMaxScaler(), self.y_min[s], self.y_max[s], n_rows, tags)
         return det
 
 
