@@ -2,14 +2,23 @@
 LSTM anomaly requests through ``server.anomaly_prediction``: one request at a time (the per-request route, one tensor-core launch
 sequence of lookback x n_layers step launches each) against ``ResidentBucket(store, lstm=True)`` (the waiting requests of all
 threads as one ragged launch sequence).  BASELINE configs[3] architecture (128 tags, lstm_symmetric 256/128/64, lookback 144),
-32 models, 8 client threads (gunicorn threads per worker in the reference), parquet in and out.  Two workloads:
+32 models, 8 client threads (gunicorn threads per worker in the reference), parquet in and out.  Three workloads:
 
   (a) uniform: every request 100 windows;
-  (b) mixed:   one request in 64 has 10 000 windows (the uniform layout would give every job of its batch 79 tiles).
+  (b) mixed:   one request in 64 has 10 000 windows (the uniform layout would give every job of its batch 79 tiles);
+  (c) overlap: every request 100 windows from ``--overlap-threads`` threads (32), served by a bucket that waits
+      ``--overlap-wait-ms`` (5 ms) for a batch to fill, so that requests actually share launches.  At 8 threads and the default
+      1 ms the host work around each request leaves few requests waiting at once.
 
-The two arms run alternately in one process and their replies must be the same bytes.
+``--ttr`` wraps every model as the production base estimator in LSTM form, ``TransformedTargetRegressor(MinMaxScaler(),
+Pipeline([MinMaxScaler(), KerasLSTMAutoEncoder]))``, served through ``ResidentBucket(lstm=True, target_scaler=True)``; the per-request
+route then adds sklearn's host inverse and a copy back to the device per request.
 
-    python benchmarks/bench_lstm_server.py [--requests 256] [--reps 2]
+The two arms run alternately in one process.  The result records the card (name, power limit and max SM clock from
+nvidia-smi, read in the same run), batches per request and whether the two arms' replies were the same bytes; the run exits
+non-zero when they were not.
+
+    python benchmarks/bench_lstm_server.py [--requests 256] [--reps 2] [--ttr]
 """
 import argparse, json, os, subprocess, sys, tempfile, threading, time
 import numpy as np
@@ -25,8 +34,10 @@ def card():
     return {"device": torch.cuda.get_device_name(), "nvidia_smi": q.stdout.strip().splitlines()[:1]}
 
 
-def make_store(root):
+def make_store(root, ttr=False):
     import pandas as pd
+    from sklearn.compose import TransformedTargetRegressor
+    from sklearn.pipeline import Pipeline
     from sklearn.preprocessing import MinMaxScaler
 
     from gordo_components_b200 import serializer, server
@@ -37,6 +48,12 @@ def make_store(root):
     tags = [f"TAG {i}" for i in range(TAGS)]
     for m in range(MODELS):
         net = KerasLSTMAutoEncoder(kind="lstm_symmetric", lookback_window=LOOKBACK).initialize(TAGS, TAGS)
+        if ttr:  # the state TransformedTargetRegressor.fit leaves, with statistics of the payloads' range
+            est = TransformedTargetRegressor(transformer=MinMaxScaler(), regressor=Pipeline([("s", MinMaxScaler()), ("m", net)]))
+            est._training_dim = 2
+            est.transformer_ = MinMaxScaler().fit(rng.random((50, TAGS)) * 10)
+            est.regressor_ = Pipeline([("s", MinMaxScaler().fit(rng.random((50, TAGS)) * 10)), ("m", net)])
+            net = est
         det = DiffBasedAnomalyDetector(base_estimator=net, scaler=MinMaxScaler().fit(rng.random((50, TAGS)) * 10))
         det.feature_thresholds_ = pd.Series(rng.random(TAGS) + 0.5, index=tags)
         det.aggregate_threshold_ = float(rng.random() + 0.5)
@@ -94,6 +111,9 @@ def main():
     ap.add_argument("--requests", type=int, default=256)
     ap.add_argument("--reps", type=int, default=2)
     ap.add_argument("--threads", type=int, default=8)
+    ap.add_argument("--overlap-threads", type=int, default=32)
+    ap.add_argument("--overlap-wait-ms", type=float, default=5.0)
+    ap.add_argument("--ttr", action="store_true", help="serve TransformedTargetRegressor models (ResidentBucket(target_scaler=True))")
     a = ap.parse_args()
     import torch
     from torch.profiler import ProfilerActivity, profile
@@ -105,39 +125,52 @@ def main():
 
     info = card()
     with tempfile.TemporaryDirectory() as root:
-        store = make_store(root)
-        bucket = server.ResidentBucket(store, lstm=True)
+        store = make_store(root, a.ttr)
+        bucket = server.ResidentBucket(store, lstm=True, target_scaler=a.ttr)
+        overlap_bucket = server.ResidentBucket(store, lstm=True, target_scaler=a.ttr, max_wait_ms=a.overlap_wait_ms)
+        assert bucket.target_scaler == a.ttr and len(bucket.names) == MODELS
         co = bucket.coalescer
-        formed = []  # (windows per request) of every batch the coalescer launched
-        launch = co._launch
+        formed = []  # (windows per request) of every batch either coalescer launched
 
-        def recording_launch(torch_, batch, cost):
-            formed.append([len(item[2]) for item in batch])
-            return launch(torch_, batch, cost)
+        def record(c):
+            launch = c._launch
 
-        co._launch = recording_launch
-        results = {"card": info, "models": MODELS, "threads": a.threads, "lookback": LOOKBACK, "tags": TAGS}
+            def recording_launch(torch_, batch, cost):
+                formed.append([len(item[2]) for item in batch])
+                return launch(torch_, batch, cost)
+
+            c._launch = recording_launch
+
+        record(co)
+        record(overlap_bucket.coalescer)
+        results = {"card": info, "models": MODELS, "threads": a.threads, "lookback": LOOKBACK, "tags": TAGS,
+                   "base_estimator": "TTR(MinMaxScaler, Pipeline([MinMaxScaler, KerasLSTMAutoEncoder]))" if a.ttr else "KerasLSTMAutoEncoder"}
+        identical = True
         try:
-            for wl, mixed in (("uniform", False), ("mixed", True)):
+            for wl, mixed, b_wl, threads in (("uniform", False, bucket, a.threads), ("mixed", True, bucket, a.threads),
+                                              ("overlap", False, overlap_bucket, a.overlap_threads)):
                 reqs = payloads(a.requests, mixed, 1 if mixed else 0)
                 windows = sum(w for _, _, w in reqs)
-                drive(store, reqs[:16], None, a.threads)  # warm-up: modules, allocator pools, the models' device copies
-                drive(store, reqs[:16], bucket, a.threads)
+                drive(store, reqs[:16], None, threads)  # warm-up: modules, allocator pools, the models' device copies
+                drive(store, reqs[:16], b_wl, threads)
                 arms = {"per_request": [], "coalesced": []}
                 replies = {}
-                batches0, formed0 = co.batches, len(formed)
+                batches0, requests0, formed0 = b_wl.coalescer.batches, b_wl.coalescer.requests, len(formed)
                 for _ in range(a.reps):
-                    for arm, b in (("per_request", None), ("coalesced", bucket)):
-                        wall, lat, bodies = drive(store, reqs, b, a.threads)
+                    for arm, b in (("per_request", None), ("coalesced", b_wl)):
+                        wall, lat, bodies = drive(store, reqs, b, threads)
                         arms[arm].append({"requests_per_s": len(reqs) / wall, "windows_per_s": windows / wall,
                                           "p50_ms": float(np.percentile(lat, 50) * 1e3), "p99_ms": float(np.percentile(lat, 99) * 1e3)})
                         if arm in replies:
                             assert replies[arm] == bodies, f"{arm}: replies changed between repetitions"
                         replies[arm] = bodies
-                assert replies["per_request"] == replies["coalesced"], "the coalesced replies differ from the per-request ones"
+                same = replies["per_request"] == replies["coalesced"]
+                identical &= same
                 batches = formed[formed0:]
-                res = {"requests": len(reqs), "windows": windows, "arms": arms, "batches_formed": co.batches - batches0,
-                       "requests_per_batch": float(np.mean([len(b) for b in batches]))}
+                n_batches, n_requests = b_wl.coalescer.batches - batches0, b_wl.coalescer.requests - requests0
+                res = {"requests": len(reqs), "windows": windows, "threads": threads, "max_wait_ms": b_wl.coalescer.max_wait * 1e3,
+                       "arms": arms, "replies_identical": same, "batches_formed": n_batches,
+                       "requests_per_batch": float(np.mean([len(b) for b in batches])), "batches_per_request": n_batches / max(1, n_requests)}
                 if mixed:
                     eng = co.eng
                     ws_u = [eng.tc_workspace_bytes(min(len(b), MODELS), len(b), max(b)) for b in batches]
@@ -159,7 +192,11 @@ def main():
                                   "step_launches_per_batch": steps / max(1, co.batches - before), "lookback_x_layers": LOOKBACK * 6}
         finally:
             bucket.close()
+            overlap_bucket.close()
+    results["replies_identical"] = identical
     print(json.dumps(results))
+    if not identical:
+        sys.exit("the coalesced replies differ from the per-request ones")
 
 
 if __name__ == "__main__":

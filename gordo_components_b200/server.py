@@ -256,6 +256,9 @@ class ResidentBucket:
     ``KerasLSTMAutoEncoder`` or ``KerasLSTMForecast``, bare or as the last step of a ``Pipeline``, on a stack the tensor-core LSTM
     kernel runs (tanh and sigmoid cells).  The Pipeline's leading steps run on the host as ``Pipeline.predict`` runs them; autoencoder
     and forecast models of one architecture share a bucket (the lookahead only decides which rows of y a request stages).
+    With ``target_scaler=True`` it also admits those networks as the ``regressor_`` of a fitted ``TransformedTargetRegressor`` (the
+    same MinMax transformer condition as below); any leading Pipeline steps are admitted, since they run on the host either way.  The
+    batch applies each model's target inverse and scores in float64 in one launch (``serving.LSTMAnomalyCoalescer(y_inverse=)``).
 
     ``smoothing=True`` (with either of the above) also admits detectors with a smoothing window -- ``DiffBasedAnomalyDetector`` with
     ``window`` and ``DiffBasedKFCVAnomalyDetector``, the reference's production definition (``window=144``, smm) -- whose ``window``
@@ -287,7 +290,7 @@ class ResidentBucket:
         from .serving import AnomalyCoalescer
 
         if lstm:
-            self._init_lstm(store, names, smoothing, coalescer_kwargs)
+            self._init_lstm(store, names, smoothing, target_scaler, coalescer_kwargs)
             return
         groups = self.ff_groups({name: store.model(name) for name in (names if names is not None else store.names())}, input_scalers, smoothing,
                                 target_scaler)
@@ -318,12 +321,13 @@ class ResidentBucket:
         self.smoothing = _smoothing_of(models[0])
         self.coalescer = AnomalyCoalescer(eng, params, scale, feat_thr, agg_thr, smoothing=self.smoothing, **coalescer_kwargs)
 
-    def _init_lstm(self, store: "ModelStore", names: Optional[List[str]], smoothing: bool, coalescer_kwargs):
+    def _init_lstm(self, store: "ModelStore", names: Optional[List[str]], smoothing: bool, target_scaler: bool, coalescer_kwargs):
         from . import engine
         from .machine.model.anomaly.diff import _scaler_multiplier
         from .serving import LSTMAnomalyCoalescer
 
-        groups = self.lstm_groups({name: store.model(name) for name in (names if names is not None else store.names())}, smoothing)
+        groups = self.lstm_groups({name: store.model(name) for name in (names if names is not None else store.names())}, smoothing,
+                                  target_scaler)
         if not groups:
             raise ValueError("no LSTM model in the store can be served through a coalescer")
         self.lstm = True
@@ -340,6 +344,10 @@ class ResidentBucket:
         feat_thr = to_dev([np.asarray(f, dtype=np.float64) for f in feat]) if feat[0] is not None else None
         agg_thr = to_dev([np.float64(a) for a in agg]) if agg[0] is not None else None
         self.smoothing = _smoothing_of(models[0])
+        self.target_scaler = _target_minmax(models[0]) is not None
+        if self.target_scaler:
+            y_scale, y_min = zip(*(_target_minmax(m) for m in models))
+            coalescer_kwargs.update(y_inverse=(to_dev(y_scale), to_dev(y_min)))
         self.coalescer = LSTMAnomalyCoalescer(eng, params, scale, feat_thr, agg_thr, smoothing=self.smoothing, **coalescer_kwargs)
 
     @classmethod
@@ -358,19 +366,24 @@ class ResidentBucket:
         return groups
 
     @classmethod
-    def lstm_groups(cls, models: Dict[str, Any], smoothing: bool = False) -> Dict[Any, List[str]]:
-        """The eligible LSTM detectors of ``models`` (name -> model) by (architecture, which thresholds are present, smoothing)."""
+    def lstm_groups(cls, models: Dict[str, Any], smoothing: bool = False, target_scaler: bool = False) -> Dict[Any, List[str]]:
+        """The eligible LSTM detectors of ``models`` (name -> model) by (architecture, which thresholds are present, with or without
+        a target transformer, smoothing)."""
         groups: Dict[Any, List[str]] = {}
         for name, model in models.items():
-            if cls.eligible_lstm(model, smoothing):
+            if cls.eligible_lstm(model, smoothing, target_scaler):
                 spec = _served_lstm_parts(model)[1].model.spec
-                groups.setdefault((spec.key(), tuple(t is not None for t in model._thresholds()), _smoothing_of(model)), []).append(name)
+                key = (spec.key(), tuple(t is not None for t in model._thresholds()), _target_minmax(model) is not None, _smoothing_of(model))
+                groups.setdefault(key, []).append(name)
         return groups
 
     @staticmethod
-    def eligible_lstm(model, smoothing: bool = False) -> bool:
-        """True for a detector ``ResidentBucket(lstm=True, smoothing=smoothing)`` serves (no device needed)."""
+    def eligible_lstm(model, smoothing: bool = False, target_scaler: bool = False) -> bool:
+        """True for a detector ``ResidentBucket(lstm=True, smoothing=smoothing, target_scaler=target_scaler)`` serves (no device
+        needed)."""
         import ctypes as C
+
+        from sklearn.compose import TransformedTargetRegressor
 
         from . import _cabi
         from .machine.model.anomaly.diff import _scaler_multiplier
@@ -382,6 +395,10 @@ class ResidentBucket:
         if parts is None or parts[1].model is None:
             return False
         spec = parts[1].model.spec
+        if type(model.base_estimator) is TransformedTargetRegressor:
+            target = _target_minmax(model)
+            if not target_scaler or target is None or target[0].shape != (spec.n_features_out,):
+                return False
         net = _cabi.make_lstmnet(spec.n_features, spec.lstm_units, spec.acts, spec.n_features_out, spec.out_func, spec.lookback_window)
         if _cabi.load_library().gb_lstm_tc_supported(C.byref(net)) != 0:
             return False  # relu / linear cells: the fp32 kernel, on the per-request route
@@ -438,22 +455,26 @@ class ResidentBucket:
             # the coalescer's launch may run the tensor-core kernel, which does not take ±inf inputs: this request goes on its own
             return model.anomaly_blocks(X, y, frequency=frequency, smooth=smooth)
         scores = self._scores(name, X, y, smooth)
+        return model.blocks_from_scores(scores, X, y, frequency, smooth=smooth)
+
+    def _scores(self, name: str, X, y, smooth: bool):
+        """The coalescer's result for one request, refused as the per-request route refuses its model output; ``smooth`` is only
+        passed when set, the call of a bucket without smoothing stays ``anomaly(slot, X, y)``."""
+        from .machine.model.anomaly.diff import _has_inf, _refuse_infinity
+
+        scores = self.coalescer.anomaly(self.slot[name], X, y, smooth=True) if smooth else self.coalescer.anomaly(self.slot[name], X, y)
         raw = scores.pop("raw-model-output", None)
         if raw is not None and _has_inf(raw):
             # what sklearn's inverse_transform raises on the regressor's prediction, before the per-request route's own check
             raise ValueError(f"Input contains infinity or a value too large for {raw.dtype!r}.")
         _refuse_infinity(scores["model-output"])
-        return model.blocks_from_scores(scores, X, y, frequency, smooth=smooth)
-
-    def _scores(self, name: str, X, y, smooth: bool):
-        """The coalescer's result for one request; ``smooth`` is only passed when set, the call of a bucket without smoothing stays
-        ``anomaly(slot, X, y)``."""
-        return self.coalescer.anomaly(self.slot[name], X, y, smooth=True) if smooth else self.coalescer.anomaly(self.slot[name], X, y)
+        return scores
 
     def _lstm_anomaly_blocks(self, name: str, model, X: pd.DataFrame, y: pd.DataFrame, frequency, smooth: bool):
         """What ``model.anomaly_blocks`` computes, in the order the per-request route raises: the leading steps' transform (which
-        refuses ±inf in X), the lookback check; a transformed X holding ±inf goes on its own (the fp32 kernel saturates the gates)."""
-        from .machine.model.anomaly.diff import _has_inf, _refuse_infinity, _values
+        refuses ±inf in X), the lookback check; a transformed X holding ±inf goes on its own (the fp32 kernel saturates the gates).
+        Around a TransformedTargetRegressor, the inverse's refusals follow the launch (``_scores``)."""
+        from .machine.model.anomaly.diff import _has_inf, _values
 
         pre, net = _served_lstm_parts(model)
         Xt = X
@@ -464,7 +485,6 @@ class ResidentBucket:
             return model.anomaly_blocks(X, y, frequency=frequency, smooth=smooth)
         n = len(Xv) - net.lookback_window + 1 - net.lookahead
         scores = self._scores(name, Xv, _values(y)[-n:], smooth)
-        _refuse_infinity(scores["model-output"])
         return model.blocks_from_scores(scores, X, y, frequency, smooth=smooth)
 
     def close(self):
@@ -536,12 +556,16 @@ def _target_minmax(model):
 def _served_lstm_parts(model):
     """(leading Pipeline steps, ``KerasLSTMAutoEncoder`` / ``KerasLSTMForecast``) of a detector whose base estimator is a bare LSTM
     network ([] for the steps) or a ``Pipeline`` ending in one, else None.  Skipped steps (None, "passthrough") are left out, as
-    ``Pipeline.predict`` leaves them out."""
+    ``Pipeline.predict`` leaves them out.  For a fitted ``TransformedTargetRegressor`` these are the parts of its ``regressor_``
+    (its target transformer: ``_target_minmax``)."""
+    from sklearn.compose import TransformedTargetRegressor
     from sklearn.pipeline import Pipeline
 
     from .machine.model.models import KerasLSTMAutoEncoder, KerasLSTMForecast
 
     est = model.base_estimator
+    if type(est) is TransformedTargetRegressor:
+        est = getattr(est, "regressor_", None)
     if type(est) in (KerasLSTMAutoEncoder, KerasLSTMForecast):
         return [], est
     if type(est) is Pipeline and len(est.steps) > 1 and type(est.steps[-1][1]) in (KerasLSTMAutoEncoder, KerasLSTMForecast):

@@ -27,7 +27,8 @@ Thread-safe, re-entrant, no shared mutable scratch outside the worker thread (th
 SURVEY §8b).  The per-request results are bit-identical to a per-request launch: rows are independent in the kernel.
 
 ``LSTMAnomalyCoalescer`` does the same for LSTM detectors: the waiting requests become one ragged tensor-core LSTM launch
-sequence (gb_lstm_infer_tc_ragged, each request a job of its own windows) and one float64 scoring launch (gb_anomaly_score_f64).
+sequence (gb_lstm_infer_tc_ragged, each request a job of its own windows) and one float64 scoring launch (gb_anomaly_score_f64, or
+with ``y_inverse`` gb_minmax_inverse_score_f64, as above).
 
 Either coalescer built with ``smoothing=(window, method)`` (the detectors' ``window`` / ``smoothing_method``) also answers the
 smoothed columns: ``submit(slot, X, y, smooth=True)`` marks a request whose reply carries them, and a batch holding such requests
@@ -266,12 +267,18 @@ class LSTMAnomalyCoalescer(AnomalyCoalescer):
     sequence, the prediction widened to float64 on the device and scored there, one synchronisation.  A batch closes at
     ``max_batch_tiles`` 128-window tiles or ``max_jobs`` requests.  Results: float32 ``model-output``, float64 scores, as the
     per-request route returns them.
+
+    With ``y_inverse=(y_scale, y_min)`` (float64 [n_slots, n_out] device tensors, the MinMax ``transformer_`` of detectors around a
+    ``TransformedTargetRegressor``) the prediction is not widened and scored: one gb_minmax_inverse_score_f64 launch writes its float32
+    inverse as ``model-output`` and the float64 scores, and a request whose inverse holds ±inf also gets its raw prediction under
+    ``raw-model-output``, as ``AnomalyCoalescer`` does.
     """
 
     def __init__(self, eng: "engine.LSTMEngine", params, scale, feat_thr=None, agg_thr=None, max_batch_tiles: int = 1024,
-                 max_wait_ms: float = 1.0, smoothing=None):
+                 max_wait_ms: float = 1.0, smoothing=None, y_inverse=None):
         torch = engine._torch()
         self.eng, self.params, self.scale, self.feat_thr, self.agg_thr = eng, params, scale, feat_thr, agg_thr
+        self.y_inverse = tuple(y_inverse) if y_inverse is not None else None
         self.max_cost, self.max_wait = int(max_batch_tiles), float(max_wait_ms) * 1e-3
         self.want = tuple(k for k in PER_TAG + PER_ROW if not ((feat_thr is None and k == "anomaly-confidence")
                                                                 or (agg_thr is None and k == "total-anomaly-confidence")))
@@ -345,9 +352,15 @@ class LSTMAnomalyCoalescer(AnomalyCoalescer):
             feat_thr = gather(self.feat_thr) if self.feat_thr is not None else None
             agg_thr = gather(self.agg_thr) if self.agg_thr is not None else None
             pred = self.eng.infer(params, jobs_d, k, int(windows.max()), xd, total, tile_base=tb_d, n_tiles=int(tile_base[-1]))
-            res = engine.anomaly_score(score_d, k, int(windows.max()), pred.to(torch.float64), yd, self.eng.n_out, scale, feat_thr, agg_thr,
-                                       want=self.want)
-            res["model-output"] = pred
+            if self.y_inverse is None:
+                res = engine.anomaly_score(score_d, k, int(windows.max()), pred.to(torch.float64), yd, self.eng.n_out, scale, feat_thr,
+                                           agg_thr, want=self.want)
+                res["model-output"] = pred
+            else:
+                y_scale, y_min = (gather(t) for t in self.y_inverse)
+                res = engine.minmax_inverse_score_f64(score_d, k, int(windows.max()), pred, yd, y_scale, y_min, scale, feat_thr, agg_thr,
+                                                      want=self.want)
+                res["raw-model-output"] = pred
             smoothed = (self._smooth(torch, sjobs_d, *smooth, res), smooth[1]) if smooth is not None else None
             host = {key: torch.empty(v.shape, dtype=v.dtype, pin_memory=True) for key, v in res.items()}
             for key, v in res.items():
@@ -355,6 +368,9 @@ class LSTMAnomalyCoalescer(AnomalyCoalescer):
         self._stream.synchronize()
         self.batches += 1
         self.requests += k
+        raw = host.pop("raw-model-output", None)
         for i, item in enumerate(batch):
             result = {key: v[w_ofs[i]:w_ofs[i + 1]].numpy().copy() for key, v in host.items()}
+            if raw is not None and np.isinf(result["model-output"]).any():
+                result["raw-model-output"] = raw[w_ofs[i]:w_ofs[i + 1]].numpy().copy()
             item[-1].set_result(self._with_smoothed(result, item, smoothed, int(w_ofs[i]), int(windows[i])))
