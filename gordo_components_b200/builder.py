@@ -386,6 +386,26 @@ def _target_regressor(est, target_scaler: bool = True):
     return None, est.regressor, True
 
 
+def _refuse(machine, reason: str) -> None:
+    """Log why ``machine`` takes the per-machine path; the classifiers return this None."""
+    logger.info("machine %s takes the per-machine path: %s", machine["name"], reason)
+    return None
+
+
+def _tss_refusal(split_obj) -> Optional[str]:
+    """Why the batched builds cannot take this cv (anything but a plain TimeSeriesSplit), or None."""
+    if type(split_obj) is not TimeSeriesSplit or split_obj.max_train_size is not None or split_obj.test_size is not None or split_obj.gap:
+        return "cv is not a plain TimeSeriesSplit"
+    return None
+
+
+def _fetch(machine):
+    """(X, y, dataset metadata, query seconds) of the machine's dataset."""
+    t0 = time.time()
+    X, y, dataset_meta = _get_data(machine["dataset"])
+    return X, y, dataset_meta, time.time() - t0
+
+
 def _canonical(index, machine, early_stopping: bool = False, smoothing: bool = False, target_scaler: bool = False) -> Optional[_Canonical]:
     """
     The machine as a candidate for the batched path, or ``None`` with the reason logged.  ``early_stopping``: also take an
@@ -397,54 +417,49 @@ def _canonical(index, machine, early_stopping: bool = False, smoothing: bool = F
     """
     from .machine.model.anomaly.diff import DiffBasedAnomalyDetector
     from .machine.model.factories.specs import FFNetSpec
-
-    def no(reason):
-        logger.info("machine %s takes the per-machine path: %s", machine["name"], reason)
-        return None
+    from .machine.model.models import KerasAutoEncoder, KerasRawModelRegressor
 
     evaluation = {**DEFAULT_EVALUATION, **(machine.get("evaluation") or {})}
     reason = _evaluation_refusal(evaluation)
     if reason:
-        return no(reason)
+        return _refuse(machine, reason)
     split_obj = serializer.from_definition(evaluation.get("cv", DEFAULT_CV))
-    if type(split_obj) is not TimeSeriesSplit or split_obj.max_train_size is not None or split_obj.test_size is not None or split_obj.gap:
-        return no("cv is not a plain TimeSeriesSplit")
+    reason = _tss_refusal(split_obj)
+    if reason:
+        return _refuse(machine, reason)
 
     model = serializer.from_definition(machine["model"])
     if type(model) is not DiffBasedAnomalyDetector or (model.window is not None and not smoothing):
-        return no("model is not a plain DiffBasedAnomalyDetector")
+        return _refuse(machine, "model is not a plain DiffBasedAnomalyDetector")
     reason = _window_refusal(model)
     if reason:
-        return no(reason)
+        return _refuse(machine, reason)
     if not _default_minmax(model.scaler):
-        return no("detector scaler is not a default MinMaxScaler")
+        return _refuse(machine, "detector scaler is not a default MinMaxScaler")
     reason, est, in_ttr = _target_regressor(model.base_estimator, target_scaler)
     if reason:
-        return no(reason)
-    ae, input_scaler = _ff_network(est)
+        return _refuse(machine, reason)
+    ae, input_scaler = _network(est, (KerasAutoEncoder, KerasRawModelRegressor))
     if ae is None:
-        return no("base_estimator is not a KerasAutoEncoder, bare or behind one default MinMaxScaler")
+        return _refuse(machine, "base_estimator is not a KerasAutoEncoder, bare or behind one default MinMaxScaler")
     reason, fit_args, stopping, vsplit = _ff_fit_arguments(ae, early_stopping)
     if reason:
-        return no(reason)
+        return _refuse(machine, reason)
 
-    t0 = time.time()
-    X, y, dataset_meta = _get_data(machine["dataset"])
-    query_sec = time.time() - t0
+    X, y, dataset_meta, query_sec = _fetch(machine)
     ae.kwargs.update({"n_features": X.shape[1], "n_features_out": y.shape[1]})
     spec = ae._build_spec()
     if not isinstance(spec, FFNetSpec):
-        return no("not a feed-forward network")
+        return _refuse(machine, "not a feed-forward network")
     test = len(X) // (split_obj.n_splits + 1)
     if len(X) != len(y) or test == 0:
-        return no("too few rows for the CV folds")
+        return _refuse(machine, "too few rows for the CV folds")
     if vsplit and math.floor((len(X) - split_obj.n_splits * test) * (1.0 - vsplit)) < 1:  # the smallest fold: keras' split (models.py)
-        return no(f"validation_split {vsplit} leaves the first CV fold without a training row")
+        return _refuse(machine, f"validation_split {vsplit} leaves the first CV fold without a training row")
     reason = _monitor_refusal(stopping, spec, vsplit)
     if reason:
-        return no(reason)
-    fit = {"epochs": int(fit_args.get("epochs", 1)), "batch_size": int(fit_args.get("batch_size") or 32), "shuffle": bool(fit_args.get("shuffle", True))}
-    split = (bool(model.shuffle), vsplit, int(fit_args.get("validation_batch_size") or fit["batch_size"]) if vsplit else None)
+        return _refuse(machine, reason)
+    fit, split = _ff_fit(fit_args, model.shuffle, vsplit)
     c = _Canonical(index, machine, model, spec, X, y, dataset_meta, query_sec, fit, split_obj.n_splits, evaluation, input_scaler, split, stopping)
     c.window = None if model.window is None else int(model.window)
     c.target_scaler = in_ttr
@@ -465,15 +480,20 @@ def _evaluation_refusal(evaluation: dict) -> Optional[str]:
     return None
 
 
-def _ff_network(est):
-    """(the KerasAutoEncoder or KerasRawModelRegressor, whether a default MinMaxScaler is in front of it) of a bare network or
+def _network(est, types: tuple):
+    """(the network, whether a default MinMaxScaler is in front of it) of a bare network of one of ``types`` or
     ``Pipeline([MinMaxScaler(), network])``; (None, False) otherwise."""
-    from .machine.model.models import KerasAutoEncoder, KerasRawModelRegressor
-
     input_scaler = False
     if type(est) is Pipeline and len(est.steps) == 2 and _default_minmax(est.steps[0][1]):
         est, input_scaler = est.steps[1][1], True  # Pipeline([MinMaxScaler(), KerasAutoEncoder]): gordo's example config
-    return (est, input_scaler) if type(est) in (KerasAutoEncoder, KerasRawModelRegressor) else (None, False)
+    return (est, input_scaler) if type(est) in types else (None, False)
+
+
+def _ff_fit(fit_args, detector_shuffle, vsplit: float):
+    """The ``fit`` dict (epochs, batch size, shuffle) and ``split`` tuple (detector shuffle, validation_split, validation batch
+    size or None without a split) of a feed-forward estimator's fit arguments."""
+    fit = {"epochs": int(fit_args.get("epochs", 1)), "batch_size": int(fit_args.get("batch_size") or 32), "shuffle": bool(fit_args.get("shuffle", True))}
+    return fit, (bool(detector_shuffle), vsplit, int(fit_args.get("validation_batch_size") or fit["batch_size"]) if vsplit else None)
 
 
 def _early_stopping(fit_args, early_stopping: bool, flag: str):
@@ -565,68 +585,55 @@ def _canonical_lstm(index, machine, wide_batches: bool = False, early_stopping: 
     from .machine.model.factories.specs import LSTMNetSpec
     from .machine.model.models import KerasLSTMAutoEncoder, KerasLSTMForecast
 
-    def no(reason):
-        logger.info("machine %s takes the per-machine path: %s", machine["name"], reason)
-        return None
-
     evaluation = {**DEFAULT_EVALUATION, **(machine.get("evaluation") or {})}
-    if str(evaluation["cv_mode"]).lower() != "full_build":
-        return no(f"cv_mode {evaluation['cv_mode']}")
-    if any(m.rpartition(".")[2] not in MOMENT_METRICS or ("." in m and not m.startswith("sklearn.metrics.")) for m in evaluation["metrics"]):
-        return no("evaluation metrics beyond the four moment metrics")
-    scoring = evaluation.get("scoring_scaler")
-    if scoring:
-        scoring = serializer.from_definition(scoring) if isinstance(scoring, (str, dict)) else scoring
-        if not _default_minmax(scoring):
-            return no("scoring_scaler is not a default MinMaxScaler")
+    reason = _evaluation_refusal(evaluation)
+    if reason:
+        return _refuse(machine, reason)
     split_obj = serializer.from_definition(evaluation.get("cv", DEFAULT_CV))
-    if type(split_obj) is not TimeSeriesSplit or split_obj.max_train_size is not None or split_obj.test_size is not None or split_obj.gap:
-        return no("cv is not a plain TimeSeriesSplit")
+    reason = _tss_refusal(split_obj)
+    if reason:
+        return _refuse(machine, reason)
 
     model = serializer.from_definition(machine["model"])
     if type(model) is not DiffBasedAnomalyDetector or (model.window is not None and not smoothing) or model.shuffle:
-        return no("model is not a plain DiffBasedAnomalyDetector")
+        return _refuse(machine, "model is not a plain DiffBasedAnomalyDetector")
     reason = _window_refusal(model)
     if reason:
-        return no(reason)
+        return _refuse(machine, reason)
     if not _default_minmax(model.scaler):
-        return no("detector scaler is not a default MinMaxScaler")
+        return _refuse(machine, "detector scaler is not a default MinMaxScaler")
     reason, est, in_ttr = _target_regressor(model.base_estimator, target_scaler)
     if reason:
-        return no(reason)
-    input_scaler = False
-    if type(est) is Pipeline and len(est.steps) == 2 and _default_minmax(est.steps[0][1]):
-        est, input_scaler = est.steps[1][1], True
-    if type(est) not in (KerasLSTMAutoEncoder, KerasLSTMForecast):
-        return no("base_estimator is not a KerasLSTMAutoEncoder / KerasLSTMForecast, bare or behind one default MinMaxScaler")
+        return _refuse(machine, reason)
+    est, input_scaler = _network(est, (KerasLSTMAutoEncoder, KerasLSTMForecast))
+    if est is None:
+        return _refuse(machine, "base_estimator is not a KerasLSTMAutoEncoder / KerasLSTMForecast, bare or behind one default MinMaxScaler")
     fit_args = est.extract_supported_fit_args(est.kwargs)
     if fit_args.get("validation_split"):
-        return no("validation_split needs the per-machine fit")
+        return _refuse(machine, "validation_split needs the per-machine fit")
     reason, stopping = _early_stopping(fit_args, early_stopping, "lstm_early_stopping")
     if reason:
-        return no(reason)
+        return _refuse(machine, reason)
     batch_size = int(est.batch_size)
     if not 1 <= batch_size <= LSTMEngine.FP32_MAX_BATCH and not (wide_batches and 1 <= batch_size <= LSTMEngine.TC_MAX_BATCH):
         if wide_batches:
-            return no(f"batch_size {batch_size}: the batched LSTM fit takes at most {LSTMEngine.TC_MAX_BATCH} windows per batch")
-        return no(f"batch_size {batch_size}: the batched LSTM fit takes at most {LSTMEngine.FP32_MAX_BATCH} windows per batch "
+            return _refuse(machine, f"batch_size {batch_size}: the batched LSTM fit takes at most {LSTMEngine.TC_MAX_BATCH} windows per batch")
+        return _refuse(machine, f"batch_size {batch_size}: the batched LSTM fit takes at most {LSTMEngine.FP32_MAX_BATCH} windows per batch "
                   "(FleetModelBuilder(lstm_wide_batches=True) batches up to 256)")
 
-    t0 = time.time()
-    X, y, dataset_meta = _get_data(machine["dataset"])
-    query_sec = time.time() - t0
+    X, y, dataset_meta, query_sec = _fetch(machine)
     est.kwargs.update({"n_features": X.shape[1], "n_features_out": y.shape[1]})
     spec = est._build_spec()
     if not isinstance(spec, LSTMNetSpec):
-        return no("not an LSTM network")
+        return _refuse(machine, "not an LSTM network")
     L, la, K = int(est.lookback_window), int(est.lookahead), split_obj.n_splits
     test = len(X) // (K + 1)
     first_train = len(X) - K * test
     if len(X) != len(y) or test <= L + la or first_train <= L or first_train - L + 1 - la < 1:
-        return no("too few rows for the CV folds at this lookback_window")
+        return _refuse(machine, "too few rows for the CV folds at this lookback_window")
     reason = _monitor_refusal(stopping, spec, 0.0)  # the generator fit has no validation data
     if reason:
-        return no(reason)
+        return _refuse(machine, reason)
     fit = {"epochs": int(fit_args.get("epochs", 1)), "batch_size": batch_size, "shuffle": False}
     c = _CanonicalLSTM(index, machine, model, spec, X, y, dataset_meta, query_sec, fit, K, evaluation, input_scaler, (False, 0.0, None), stopping,
                        lookahead=la)
@@ -671,55 +678,48 @@ def _canonical_kfcv(index, machine, early_stopping: bool = False) -> Optional[_C
     import numbers
 
     from .machine.model.factories.specs import FFNetSpec
-
-    def no(reason):
-        logger.info("machine %s takes the per-machine path: %s", machine["name"], reason)
-        return None
+    from .machine.model.models import KerasAutoEncoder, KerasRawModelRegressor
 
     evaluation = {**DEFAULT_EVALUATION, **(machine.get("evaluation") or {})}
     reason = _evaluation_refusal(evaluation)
     if reason:
-        return no(reason)
+        return _refuse(machine, reason)
     cv = serializer.from_definition(evaluation.get("cv", DEFAULT_CV))
     if type(cv) is not KFold:
-        return no("a K-fold detector is batched under a KFold cv only")
+        return _refuse(machine, "a K-fold detector is batched under a KFold cv only")
     if cv.shuffle and (not isinstance(cv.random_state, numbers.Integral) or isinstance(cv.random_state, bool)):
-        return no("a shuffled KFold without an int random_state gives every machine other folds")
+        return _refuse(machine, "a shuffled KFold without an int random_state gives every machine other folds")
 
     model = serializer.from_definition(machine["model"])
     if not _default_minmax(model.scaler):
-        return no("detector scaler is not a default MinMaxScaler")
-    if model.window is not None and (not isinstance(model.window, numbers.Integral) or isinstance(model.window, bool) or model.window < 1):
-        return no(f"window {model.window!r} is not a positive int")
-    if model.window is not None and model.smoothing_method not in ("smm", "sma", "ewma"):
-        return no(f"smoothing_method {model.smoothing_method!r}")
+        return _refuse(machine, "detector scaler is not a default MinMaxScaler")
+    reason = _window_refusal(model)
+    if reason:
+        return _refuse(machine, reason)
     reason, est, target_scaler = _target_regressor(model.base_estimator)
     if reason:
-        return no(reason)
-    ae, input_scaler = _ff_network(est)
+        return _refuse(machine, reason)
+    ae, input_scaler = _network(est, (KerasAutoEncoder, KerasRawModelRegressor))
     if ae is None:
-        return no("the estimator is not a KerasAutoEncoder, bare or behind one default MinMaxScaler")
+        return _refuse(machine, "the estimator is not a KerasAutoEncoder, bare or behind one default MinMaxScaler")
     reason, fit_args, stopping, vsplit = _ff_fit_arguments(ae, early_stopping)
     if reason:
-        return no(reason)
+        return _refuse(machine, reason)
 
-    t0 = time.time()
-    X, y, dataset_meta = _get_data(machine["dataset"])
-    query_sec = time.time() - t0
+    X, y, dataset_meta, query_sec = _fetch(machine)
     ae.kwargs.update({"n_features": X.shape[1], "n_features_out": y.shape[1]})
     spec = ae._build_spec()
     if not isinstance(spec, FFNetSpec):
-        return no("not a feed-forward network")
+        return _refuse(machine, "not a feed-forward network")
     if len(X) != len(y) or len(X) < cv.n_splits:
-        return no("too few rows for the CV folds")
+        return _refuse(machine, "too few rows for the CV folds")
     smallest = len(X) - math.ceil(len(X) / cv.n_splits)  # the training rows of the largest test fold
     if vsplit and math.floor(smallest * (1.0 - vsplit)) < 1:
-        return no(f"validation_split {vsplit} leaves a CV fold without a training row")
+        return _refuse(machine, f"validation_split {vsplit} leaves a CV fold without a training row")
     reason = _monitor_refusal(stopping, spec, vsplit)
     if reason:
-        return no(reason)
-    fit = {"epochs": int(fit_args.get("epochs", 1)), "batch_size": int(fit_args.get("batch_size") or 32), "shuffle": bool(fit_args.get("shuffle", True))}
-    split = (bool(model.shuffle), vsplit, int(fit_args.get("validation_batch_size") or fit["batch_size"]) if vsplit else None)
+        return _refuse(machine, reason)
+    fit, split = _ff_fit(fit_args, model.shuffle, vsplit)
     return _CanonicalKFold(index, machine, model, spec, X, y, dataset_meta, query_sec, fit, cv.n_splits, evaluation, input_scaler, split, stopping,
                            cv=cv, target_scaler=target_scaler)
 
@@ -831,46 +831,15 @@ class FleetModelBuilder:
 
         first = members[0]
         eng = engine.ff_engine_for(first.spec)
-        rows, K = [len(c.X) for c in members], first.n_splits
         t0 = time.time()
-        same_y = all(c.y is c.X for c in members)
-        if first.target_scaler:  # TransformedTargetRegressor.fit hands its transformer the float64 targets
-            torch = engine._torch()
-            xd = torch.from_numpy(np.concatenate([np.ascontiguousarray(c.X.values, dtype=np.float64) for c in members])).to(eng.device)
-            yd = xd if same_y else torch.from_numpy(np.concatenate([np.ascontiguousarray(c.y.values, dtype=np.float64) for c in members])).to(eng.device)
-        else:
-            x_host = np.concatenate([np.ascontiguousarray(c.X.values, dtype=np.float32) for c in members])
-            xd = engine.to_device_f32(x_host, eng.device)
-            yd = xd if same_y else engine.to_device_f32(np.concatenate([np.ascontiguousarray(c.y.values, dtype=np.float32) for c in members]), eng.device)
-        fb = fleet.build_fleet(eng, xd, yd, rows, epochs=first.fit["epochs"], batch_size=first.fit["batch_size"], n_splits=K,
-                               seed=int(first.evaluation.get("seed", 0)), adam=first.spec.adam, shuffle=first.fit["shuffle"],
+        xd, yd = _upload(members, eng.device, float64=first.target_scaler)  # TransformedTargetRegressor.fit hands its transformer float64 targets
+        fb = fleet.build_fleet(eng, xd, yd, [len(c.X) for c in members], epochs=first.fit["epochs"], batch_size=first.fit["batch_size"],
+                               n_splits=first.n_splits, seed=int(first.evaluation.get("seed", 0)), adam=first.spec.adam, shuffle=first.fit["shuffle"],
                                input_scaler=first.input_scaler, detector_shuffle=first.split[0], validation_split=first.split[1],
-                               validation_batch_size=first.split[2],
-                               early_stopping=None if first.early_stopping is None else [c.early_stopping for c in members], loss=first.spec.loss, optimizer=fit_optimizer(first.spec),
-                               reg=fit_reg(first.spec), window=first.window, dropout=fit_dropout(first.spec), target_scaler=first.target_scaler)
-        moments = fb.cv_moments.cpu().numpy()
-        scale = fb.scale.cpu().numpy().astype(np.float64)
-        engine._torch().cuda.synchronize()
-        share = (time.time() - t0) / len(members)  # the bucket's wall time, spread evenly: there is no per-machine time any more
-        split_obj = TimeSeriesSplit(n_splits=K)
-        out = []
-        for m, c in enumerate(members):
-            tags = list(c.y.columns)
-            model = fb.detector(m, tags=tags, template=c.model, input_tags=list(c.X.columns))
-            names = [s.rpartition(".")[2] for s in c.evaluation["metrics"]]
-            scoring_scale = scale[m] if c.evaluation.get("scoring_scaler") else None
-            scores = scores_block(scores_from_moments(moments[m], int(fb.n_test[m]), scoring_scale, names), tags)
-            model_block = {
-                "model_offset": 0,  # a Dense stack answers every row
-                "model_creation_date": _now(),
-                "model_builder_version": __version__,
-                "model_training_duration_sec": share * 1.0 / (K + 1),
-                "cross_validation": {"scores": scores, "cv_duration_sec": share * K / (K + 1), "splits": build_split_dict(c.X, split_obj)},
-                "model_meta": extract_metadata_from_model(model),
-            }
-            dataset_block = {"query_duration_sec": c.query_sec, "dataset_meta": c.dataset_meta}
-            out.append((model, _machine_out(c.machine, {"model": model_block, "dataset": dataset_block})))
-        return out
+                               validation_batch_size=first.split[2], early_stopping=_stops(members), loss=first.spec.loss,
+                               optimizer=fit_optimizer(first.spec), reg=fit_reg(first.spec), window=first.window, dropout=fit_dropout(first.spec),
+                               target_scaler=first.target_scaler)
+        return _assemble(members, fb, fb.cv_moments.cpu().numpy(), fb.n_test, 0, TimeSeriesSplit(n_splits=first.n_splits), t0)  # a Dense stack answers every row
 
     @staticmethod
     def _build_lstm_bucket(members: List[_CanonicalLSTM]) -> List[Tuple[Any, dict]]:
@@ -878,36 +847,14 @@ class FleetModelBuilder:
 
         first = members[0]
         eng = engine.lstm_engine_for(first.spec)
-        rows, K = [len(c.X) for c in members], first.n_splits
         t0 = time.time()
-        xd = engine._torch().from_numpy(np.concatenate([np.ascontiguousarray(c.X.values, dtype=np.float64) for c in members])).to(eng.device)
-        same_y = all(c.y is c.X for c in members)
-        yd = xd if same_y else engine._torch().from_numpy(np.concatenate([np.ascontiguousarray(c.y.values, dtype=np.float64) for c in members])).to(eng.device)
-        fb = fleet.build_lstm_fleet(eng, xd, yd, rows, lookahead=first.lookahead, epochs=first.fit["epochs"], batch_size=first.fit["batch_size"],
-                                    n_splits=K, seed=int(first.evaluation.get("seed", 0)), adam=first.spec.adam, input_scaler=first.input_scaler,
-                                    loss=first.spec.loss, optimizer=fit_optimizer(first.spec),
-                                    early_stopping=None if first.early_stopping is None else [c.early_stopping for c in members],
-                                    window=first.window, target_scaler=first.target_scaler)
-        engine._torch().cuda.synchronize()
-        share = (time.time() - t0) / len(members)  # the bucket's wall time, spread evenly: there is no per-machine time any more
-        split_obj = TimeSeriesSplit(n_splits=K)
-        out = []
-        for m, c in enumerate(members):
-            tags = list(c.y.columns)
-            model = fb.detector(m, tags=tags, template=c.model, input_tags=list(c.X.columns))
-            names = [s.rpartition(".")[2] for s in c.evaluation["metrics"]]
-            scoring_scale = model.scaler.scale_ if c.evaluation.get("scoring_scaler") else None  # the scoring scaler sees all targets too
-            scores = scores_block(scores_from_moments(fb.cv_moments[m], int(fb.machine_n_test[m]), scoring_scale, names), tags)
-            model_block = {
-                "model_offset": eng.lookback - 1 + c.lookahead,  # the first prediction answers row lookback_window - 1 + lookahead
-                "model_creation_date": _now(),
-                "model_builder_version": __version__,
-                "model_training_duration_sec": share * 1.0 / (K + 1),
-                "cross_validation": {"scores": scores, "cv_duration_sec": share * K / (K + 1), "splits": build_split_dict(c.X, split_obj)},
-                "model_meta": extract_metadata_from_model(model),
-            }
-            dataset_block = {"query_duration_sec": c.query_sec, "dataset_meta": c.dataset_meta}
-            out.append((model, _machine_out(c.machine, {"model": model_block, "dataset": dataset_block})))
+        xd, yd = _upload(members, eng.device, float64=True)
+        fb = fleet.build_lstm_fleet(eng, xd, yd, [len(c.X) for c in members], lookahead=first.lookahead, epochs=first.fit["epochs"],
+                                    batch_size=first.fit["batch_size"], n_splits=first.n_splits, seed=int(first.evaluation.get("seed", 0)),
+                                    adam=first.spec.adam, input_scaler=first.input_scaler, loss=first.spec.loss, optimizer=fit_optimizer(first.spec),
+                                    early_stopping=_stops(members), window=first.window, target_scaler=first.target_scaler)
+        # the first prediction answers row lookback_window - 1 + lookahead
+        out = _assemble(members, fb, fb.cv_moments, fb.machine_n_test, eng.lookback - 1 + first.lookahead, TimeSeriesSplit(n_splits=first.n_splits), t0)
         logger.info("built %d LSTM machines in one batched bucket", len(members))
         return out
 
@@ -917,42 +864,68 @@ class FleetModelBuilder:
 
         first = members[0]
         eng = engine.ff_engine_for(first.spec)
-        rows, K = [len(c.X) for c in members], first.n_splits
-        torch = engine._torch()
         t0 = time.time()
-        xd = torch.from_numpy(np.concatenate([np.ascontiguousarray(c.X.values, dtype=np.float64) for c in members])).to(eng.device)
-        same_y = all(c.y is c.X for c in members)
-        yd = xd if same_y else torch.from_numpy(np.concatenate([np.ascontiguousarray(c.y.values, dtype=np.float64) for c in members])).to(eng.device)
+        xd, yd = _upload(members, eng.device, float64=True)
         det = first.model
-        fb = fleet.build_kfold_fleet(eng, xd, yd, rows, first.cv, epochs=first.fit["epochs"], batch_size=first.fit["batch_size"],
+        fb = fleet.build_kfold_fleet(eng, xd, yd, [len(c.X) for c in members], first.cv, epochs=first.fit["epochs"], batch_size=first.fit["batch_size"],
                                      seed=int(first.evaluation.get("seed", 0)), adam=first.spec.adam, shuffle=first.fit["shuffle"],
                                      input_scaler=first.input_scaler, target_scaler=first.target_scaler, detector_shuffle=first.split[0],
-                                     validation_split=first.split[1], validation_batch_size=first.split[2],
-                                     early_stopping=None if first.early_stopping is None else [c.early_stopping for c in members],
+                                     validation_split=first.split[1], validation_batch_size=first.split[2], early_stopping=_stops(members),
                                      window=det.window, smoothing_method=det.smoothing_method, threshold_percentile=det.threshold_percentile,
                                      loss=first.spec.loss, optimizer=fit_optimizer(first.spec), reg=fit_reg(first.spec),
                                      dropout=fit_dropout(first.spec))
-        torch.cuda.synchronize()
-        share = (time.time() - t0) / len(members)  # the bucket's wall time, spread evenly: there is no per-machine time any more
-        out = []
-        for m, c in enumerate(members):
-            tags = list(c.y.columns)
-            model = fb.detector(m, c.model, tags=tags, input_tags=list(c.X.columns))
-            names = [s.rpartition(".")[2] for s in c.evaluation["metrics"]]
-            scoring_scale = model.scaler.scale_ if c.evaluation.get("scoring_scaler") else None  # the scoring scaler sees all targets too
-            scores = scores_block(scores_from_moments(fb.cv_moments[m], fb.n_test[m], scoring_scale, names), tags)
-            model_block = {
-                "model_offset": 0,  # a Dense stack answers every row
-                "model_creation_date": _now(),
-                "model_builder_version": __version__,
-                "model_training_duration_sec": share * 1.0 / (K + 1),
-                "cross_validation": {"scores": scores, "cv_duration_sec": share * K / (K + 1), "splits": build_split_dict(c.X, c.cv)},
-                "model_meta": extract_metadata_from_model(model),
-            }
-            dataset_block = {"query_duration_sec": c.query_sec, "dataset_meta": c.dataset_meta}
-            out.append((model, _machine_out(c.machine, {"model": model_block, "dataset": dataset_block})))
+        out = _assemble(members, fb, fb.cv_moments, fb.n_test, 0, first.cv, t0)  # a Dense stack answers every row
         logger.info("built %d K-fold machines in one batched bucket", len(members))
         return out
+
+
+def _upload(members: List[_Canonical], device, float64: bool):
+    """The machines' X and y stacked on the device, float64 or float32; y is X when every machine's y is its X."""
+    from . import engine
+
+    def stacked(frames):
+        if float64:
+            return engine._torch().from_numpy(np.concatenate([np.ascontiguousarray(f.values, dtype=np.float64) for f in frames])).to(device)
+        return engine.to_device_f32(np.concatenate([np.ascontiguousarray(f.values, dtype=np.float32) for f in frames]), device)
+
+    xd = stacked([c.X for c in members])
+    return xd, (xd if all(c.y is c.X for c in members) else stacked([c.y for c in members]))
+
+
+def _stops(members: List[_Canonical]):
+    """The bucket's EarlyStopping callbacks, one per machine, or None without them."""
+    return None if members[0].early_stopping is None else [c.early_stopping for c in members]
+
+
+def _assemble(members: List[_Canonical], fb, moments, n_test, model_offset: int, split_obj, t0: float) -> List[Tuple[Any, dict]]:
+    """
+    Every machine of a built bucket as ``ModelBuilder`` returns it: the detector from ``fb.detector`` and its metadata, the CV
+    scores from the host ``moments`` [M, K, 5, T] over ``n_test[m]`` test rows per fold.  The bucket's wall time since ``t0`` is
+    spread evenly: there is no per-machine time any more.
+    """
+    from . import engine
+
+    engine._torch().cuda.synchronize()
+    share = (time.time() - t0) / len(members)
+    K = members[0].n_splits
+    out = []
+    for m, c in enumerate(members):
+        tags = list(c.y.columns)
+        model = fb.detector(m, tags=tags, template=c.model, input_tags=list(c.X.columns))
+        names = [s.rpartition(".")[2] for s in c.evaluation["metrics"]]
+        scoring_scale = model.scaler.scale_ if c.evaluation.get("scoring_scaler") else None  # the scoring scaler sees all targets too
+        scores = scores_block(scores_from_moments(moments[m], n_test[m], scoring_scale, names), tags)
+        model_block = {
+            "model_offset": model_offset,
+            "model_creation_date": _now(),
+            "model_builder_version": __version__,
+            "model_training_duration_sec": share * 1.0 / (K + 1),
+            "cross_validation": {"scores": scores, "cv_duration_sec": share * K / (K + 1), "splits": build_split_dict(c.X, split_obj)},
+            "model_meta": extract_metadata_from_model(model),
+        }
+        dataset_block = {"query_duration_sec": c.query_sec, "dataset_meta": c.dataset_meta}
+        out.append((model, _machine_out(c.machine, {"model": model_block, "dataset": dataset_block})))
+    return out
 
 
 # ------------------------------------------------------------------------------------------------ from a project config

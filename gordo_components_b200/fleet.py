@@ -158,26 +158,72 @@ def time_e2e(eng, params, jobs_h, x_dev, y_dev, scale, feat_thr, agg_thr, steps:
 
 
 # ------------------------------------------------------------------------------------------------ fleet build (train + thresholds)
-def _fill_smooth_thresholds(det, window, fold_feat, fold_agg, tags):
+def _fill_history(est, metrics, epochs: int, steps, loss, acc, val_loss=None, val_acc=None, epochs_run=None):
     """
-    The four smooth-threshold attributes ``DiffBasedAnomalyDetector.cross_validate`` leaves (diff.py:384-391): from the per-fold
-    window-``window`` thresholds ``fold_feat`` [K, T] / ``fold_agg`` [K] when the detector has a window, else the empty values.
+    The Keras ``History`` a fit leaves, as ``est._history`` and ``est.model.history``, from one fit's host per-epoch rows: loss,
+    accuracy when ``metrics`` has it, and their ``val_*`` forms with a validation split, in the per-machine History's key order.
+    ``epochs_run``: the epochs an EarlyStopping fit ran (None: every row); ``epochs`` / ``steps`` are History.params'.
+    """
+    from .machine.model.models import History
+
+    ran = len(loss) if epochs_run is None else int(epochs_run)
+    rows = {"loss": loss, "accuracy": acc, "val_loss": val_loss, "val_accuracy": val_acc}
+    hist = {k: [float(v) for v in r[:ran]] for k, r in rows.items() if r is not None and ("accuracy" in metrics or not k.endswith("accuracy"))}
+    est._history = History(hist, {"verbose": 0, "epochs": int(epochs), "steps": steps}, list(range(ran)))
+    est.model.history = est._history
+    return est
+
+
+def _fill_thresholds(det, tags, feat, agg, fold_feat=None, fold_agg=None, window=None, fold_smooth_feat=None, fold_smooth_agg=None):
+    """
+    The thresholds a detector's ``cross_validate`` leaves, from host arrays: ``feature_thresholds_`` / ``aggregate_threshold_``
+    (``feat`` [T], ``agg``), and with ``fold_feat`` [K, T] / ``fold_agg`` [K] the per-fold ones (diff.py:257-264) and the four
+    smooth-threshold attributes (diff.py:384-391) -- from the per-fold window-``window`` thresholds ``fold_smooth_feat`` [K, T] /
+    ``fold_smooth_agg`` [K] when the detector has a window, else the empty values.  Without ``fold_feat`` (a K-fold detector)
+    only the first two, the Series unnamed.
     """
     import pandas as pd
 
+    K = None if fold_agg is None else len(fold_agg)
+    det.feature_thresholds_ = pd.Series(np.array(feat, dtype=np.float64), index=tags, name=None if K is None else f"fold-{K - 1}")
+    det.aggregate_threshold_ = float(agg)
+    if K is None:
+        return det
+    det.feature_thresholds_per_fold_ = pd.DataFrame(np.array(fold_feat, dtype=np.float64), columns=tags, index=[f"fold-{k}" for k in range(K)])
+    det.aggregate_thresholds_per_fold_ = {f"fold-{k}": float(fold_agg[k]) for k in range(K)}
     if window is None:
         det.smooth_feature_thresholds_per_fold_ = pd.DataFrame()
         det.smooth_aggregate_thresholds_per_fold_ = {}
         det.smooth_aggregate_threshold_ = None
         det.smooth_feature_thresholds_ = None
         return det
-    K = len(fold_agg)
-    ff = np.asarray(fold_feat, dtype=np.float64)
+    ff = np.asarray(fold_smooth_feat, dtype=np.float64)
     det.smooth_feature_thresholds_per_fold_ = pd.DataFrame(ff.copy(), columns=tags, index=[f"fold-{k}" for k in range(K)])
-    det.smooth_aggregate_thresholds_per_fold_ = {f"fold-{k}": float(fold_agg[k]) for k in range(K)}
+    det.smooth_aggregate_thresholds_per_fold_ = {f"fold-{k}": float(fold_smooth_agg[k]) for k in range(K)}
     det.smooth_feature_thresholds_ = pd.Series(ff[K - 1].copy(), index=tags, name=f"fold-{K - 1}")
-    det.smooth_aggregate_threshold_ = float(fold_agg[K - 1])
+    det.smooth_aggregate_threshold_ = float(fold_smooth_agg[K - 1])
     return det
+
+
+def _ff_template(eng, template, target_scaler: bool, input_scaler: bool, params):
+    """
+    Fill the feed-forward network of ``template`` (an unfitted detector from the machine's own definition) with the fleet's
+    architecture and the weights ``params`` [1, stride].  Returns (the TransformedTargetRegressor or None, the estimator inside
+    it -- the Pipeline, whose MinMaxScaler the caller fills, or the network -- and the network); ValueError when the template's
+    target transformer, input scaler or architecture differ from the fleet's.
+    """
+    from sklearn.pipeline import Pipeline
+
+    ttr, est = _target_regressor_of(template.base_estimator, target_scaler)
+    ae = est.steps[-1][1] if isinstance(est, Pipeline) else est
+    if isinstance(est, Pipeline) != bool(input_scaler):
+        raise ValueError("the template's input scaler and the fleet's do not match")
+    ae.kwargs.update({"n_features": eng.n_in, "n_features_out": eng.n_out})
+    ae._prepare_model()
+    if list(ae.model.spec.dims) != list(eng.dims) or list(ae.model.spec.acts) != list(eng.acts):
+        raise ValueError("template architecture differs from the fleet's")
+    ae.model.weights = eng.unpack_params(params)[0]
+    return ttr, est, ae
 
 
 class FleetBuild:
@@ -236,68 +282,41 @@ class FleetBuild:
         unfitted detector built from the machine's own definition (same architecture) to fill in, so that ``kind`` and the
         other constructor arguments survive into ``get_params`` / ``into_definition``.
         """
-        import pandas as pd
         from sklearn.preprocessing import MinMaxScaler
 
         from .machine.model.anomaly.diff import DiffBasedAnomalyDetector
         from .machine.model.factories.specs import FFNetSpec
-        from .machine.model.models import FittedNet, History, KerasAutoEncoder
+        from .machine.model.models import FittedNet, KerasAutoEncoder
 
         eng = self.eng
         T = eng.n_out
         tags = list(tags) if tags is not None else list(range(T))
-        from sklearn.pipeline import Pipeline
-
+        host = lambda t: None if t is None else t[m].cpu().numpy()  # noqa: E731
         ttr = None
         if template is not None:
-            ttr, est = _target_regressor_of(template.base_estimator, self.y_min is not None)
-            ae = est.steps[-1][1] if isinstance(est, Pipeline) else est
-            if isinstance(est, Pipeline) != (self.in_scale is not None):
-                raise ValueError("the template's input scaler and the fleet's do not match")
-            if isinstance(est, Pipeline):
-                self._fill_minmax(est.steps[0][1], self.in_scale[m].cpu().numpy(), self.in_offset[m].cpu().numpy(), input_tags)
-            ae.kwargs.update({"n_features": eng.n_in, "n_features_out": T})
-            ae._prepare_model()
-            if list(ae.model.spec.dims) != list(eng.dims) or list(ae.model.spec.acts) != list(eng.acts):
-                raise ValueError("template architecture differs from the fleet's")
-            ae.model.weights = eng.unpack_params(self.params[m : m + 1])[0]
+            ttr, est, ae = _ff_template(eng, template, self.y_min is not None, self.in_scale is not None, self.params[m : m + 1])
+            if self.in_scale is not None:
+                self._fill_minmax(est.steps[0][1], host(self.in_scale), host(self.in_offset), input_tags)
         elif self.y_min is not None:
             raise ValueError("a fleet with a target transformer materialises its detectors from a template")
         else:
             ae = KerasAutoEncoder(kind="feedforward_model", n_features=eng.n_in, n_features_out=T)
             spec = FFNetSpec(list(eng.dims), list(eng.acts), list(eng.l1))
             ae.model = FittedNet(spec, eng.unpack_params(self.params[m : m + 1])[0])
-        hist = {"loss": [float(v) for v in self.loss[m].cpu().numpy()], "accuracy": [float(v) for v in self.acc[m].cpu().numpy()]}
-        if self.val_loss is not None:  # the keys and their order of the per-machine History
-            hist["val_loss"] = [float(v) for v in self.val_loss[m].cpu().numpy()]
-            hist["val_accuracy"] = [float(v) for v in self.val_acc[m].cpu().numpy()]
-        if "accuracy" not in ae.model.spec.metrics:  # e.g. a raw Sequential spec compiled without metrics: keras reports the loss only
-            hist = {k: v for k, v in hist.items() if not k.endswith("accuracy")}
-        steps = None if self.machine_steps is None else int(self.machine_steps[m])
-        if self.epochs_run is None:
-            ae._history = History(hist, {"verbose": 0, "epochs": len(hist["loss"]), "steps": steps}, list(range(len(hist["loss"]))))
-        else:  # as the per-machine fit loop leaves it: the epochs run, against the configured count
-            ran = int(self.epochs_run[m])
-            hist = {k: v[:ran] for k, v in hist.items()}
-            ae._history = History(hist, {"verbose": 0, "epochs": int(self.epochs), "steps": steps}, list(range(ran)))
+        _fill_history(ae, ae.model.spec.metrics, self.epochs, int(self.machine_steps[m]), host(self.loss), host(self.acc), host(self.val_loss),
+                      host(self.val_acc), host(self.epochs_run))
         if ttr is not None:
             _fill_target_regressor(ttr, est, self.y_min[m], self.y_max[m], self.rows[m])
             sc = _fill_minmax_from_extrema(MinMaxScaler(), self.y_min[m], self.y_max[m], self.rows[m], tags)
         else:
-            sc = self._fill_minmax(MinMaxScaler(), self.scale[m].cpu().numpy().astype(np.float64), self.offset[m].cpu().numpy().astype(np.float64), None)
+            sc = self._fill_minmax(MinMaxScaler(), host(self.scale).astype(np.float64), host(self.offset).astype(np.float64), None)
         if template is not None:
             det = template
             det.scaler = sc
         else:
             det = DiffBasedAnomalyDetector(base_estimator=ae, scaler=sc, **({} if self.window is None else {"window": self.window}))
-        det.feature_thresholds_ = pd.Series(self.feat_thr[m].cpu().numpy().astype(np.float64), index=tags, name=f"fold-{self.n_splits - 1}")
-        det.aggregate_threshold_ = float(self.agg_thr[m])
-        ff = self.fold_feat_thr[m].cpu().numpy().astype(np.float64)
-        det.feature_thresholds_per_fold_ = pd.DataFrame(ff, columns=tags, index=[f"fold-{k}" for k in range(self.n_splits)])
-        det.aggregate_thresholds_per_fold_ = {f"fold-{k}": float(self.fold_agg_thr[m, k]) for k in range(self.n_splits)}
-        if self.window is None:
-            return _fill_smooth_thresholds(det, None, None, None, tags)
-        return _fill_smooth_thresholds(det, self.window, self.fold_smooth_feat_thr[m].cpu().numpy(), self.fold_smooth_agg_thr[m].cpu().numpy(), tags)
+        return _fill_thresholds(det, tags, host(self.feat_thr), host(self.agg_thr), host(self.fold_feat_thr), host(self.fold_agg_thr), self.window,
+                                host(self.fold_smooth_feat_thr), host(self.fold_smooth_agg_thr))
 
 
 def dump_fleet(fb: "FleetBuild", root: str, names: Sequence[str], tags: Optional[Sequence[Sequence[str]]] = None,
@@ -351,17 +370,43 @@ def _fit_slots(eng, params, fit_jobs, n_jobs, max_rows, x, y, split, row_map, n_
     Returns (loss, acc, val_loss, val_acc, epochs_run, best_epoch): val_* rows NaN for jobs without held-out positions,
     epochs_run / best_epoch None without a callback.
     """
-    stop = None
-    if early_stopping is not None:
-        per_machine = list(early_stopping) if isinstance(early_stopping, (list, tuple)) else [early_stopping] * n_machines
-        if len(per_machine) != n_machines:
-            raise ValueError(f"early_stopping: {len(per_machine)} callbacks for {n_machines} machines")
-        stop = engine.make_stop([per_machine[j % n_machines] for j in range(n_jobs)])
+    stop = _slot_stops(early_stopping, n_machines, n_jobs)
     hist, acc, val_loss, val_acc, *ran, _ = eng.fit_split(
         params, fit_jobs, n_jobs, max_rows, x, y, split=split, row_map=row_map, val_batch=validation_batch_size or batch_size, epochs=epochs,
         batch_size=batch_size, shuffle=shuffle, adam=adam, seed=seed, stop=stop, loss=loss, optimizer=optimizer, reg=reg, dropout=dropout)
     epochs_run, best_epoch = ran or (None, None)
     return hist, acc, val_loss, val_acc, epochs_run, best_epoch
+
+
+def _slot_stops(early_stopping, n_machines: int, n_slots: int):
+    """The stop records of ``n_slots`` fits, slot s applying machine s mod M's EarlyStopping callback (``early_stopping``: one for
+    every machine or one per machine), or None without a callback."""
+    if early_stopping is None:
+        return None
+    per_machine = list(early_stopping) if isinstance(early_stopping, (list, tuple)) else [early_stopping] * n_machines
+    if len(per_machine) != n_machines:
+        raise ValueError(f"early_stopping: {len(per_machine)} callbacks for {n_machines} machines")
+    return engine.make_stop([per_machine[s % n_machines] for s in range(n_slots)])
+
+
+def _keras_train_rows(slot_n, validation_split):
+    """Keras' ``validation_split``: the rows each slot of ``slot_n`` rows trains on (int64), the rest held out."""
+    vsplit = float(validation_split or 0.0)
+    n_train = np.asarray([int(math.floor(v * (1.0 - vsplit))) if 0.0 < vsplit < 1.0 else int(v) for v in slot_n], dtype=np.int64)
+    if n_train.min() < 1:
+        raise ValueError(f"validation_split {vsplit} leaves the {int(slot_n.min())}-row slot without a training row")
+    return n_train
+
+
+def _slot_copies(n, row0, n_splits: int, device):
+    """
+    Every slot's own copy of its machine's rows, for slots that scale them on their own: the stacked machines (rows ``n``, first
+    rows ``row0``) repeated K + 1 times, slot s (finals, then fold k of machine m at M + k*M + m) at copy0[s].  Returns (copy0,
+    the device jobs that copy slot s's machine rows to copy0[s]).
+    """
+    base = np.tile(row0, n_splits + 1)
+    copy0 = np.arange(n_splits + 1, dtype=np.int64).repeat(len(n)) * int(n.sum()) + base
+    return copy0, engine.jobs_to_device(engine.make_jobs(np.arange(len(base)), np.tile(n, n_splits + 1), base, copy0), device)
 
 
 def _machine_rows(x, rows):
@@ -468,10 +513,7 @@ def build_fleet(eng: "engine.FFEngine", x, y, rows, epochs: int = 1, batch_size:
     init_params = params.clone() if keep_init_params else None
     N = int(n.max())                                             # the longest slot
     slot_n = np.concatenate([n] + [starts[:, k] for k in range(K)])  # every row of a slot: what its scalers see
-    vsplit = float(validation_split or 0.0)
-    n_train = np.asarray([int(math.floor(v * (1.0 - vsplit))) if 0.0 < vsplit < 1.0 else int(v) for v in slot_n], dtype=np.int64)  # keras' split
-    if n_train.min() < 1:
-        raise ValueError(f"validation_split {vsplit} leaves the {int(slot_n.min())}-row slot without a training row")
+    n_train = _keras_train_rows(slot_n, validation_split)
     held_out = bool((n_train != slot_n).any())
     fit_x = np.tile(row0, K + 1)                                 # first row of every slot's machine
     split = row_map = None
@@ -489,9 +531,7 @@ def build_fleet(eng: "engine.FFEngine", x, y, rows, epochs: int = 1, batch_size:
         y_lo, y_hi = _slot_extrema(prefix_jobs, S, N, y)
         t_scale_h, t_offset_h = _minmax_attributes(y_lo, y_hi)
         t_scale, t_offset = _f64(t_scale_h, dev), _f64(t_offset_h, dev)
-        # slot s works on its own copies of its machine's rows: the stacked machines repeated K + 1 times, slot s at copy0[s]
-        copy0 = np.arange(K + 1, dtype=np.int64).repeat(M) * total + fit_x
-        copy_jobs = engine.jobs_to_device(engine.make_jobs(np.arange(S), np.tile(n, K + 1), fit_x, copy0), dev)
+        copy0, copy_jobs = _slot_copies(n, row0, K, dev)  # slot s works on its own copies of its machine's rows
         if input_scaler:
             in_lo, in_hi = (y_lo, y_hi) if same_y else _slot_extrema(prefix_jobs, S, N, x)
             in_scale, in_offset = (_f64(v, dev) for v in _minmax_attributes(in_lo, in_hi))
@@ -508,10 +548,8 @@ def build_fleet(eng: "engine.FFEngine", x, y, rows, epochs: int = 1, batch_size:
         span[~(span >= 10 * np.finfo(np.float64).eps)] = 1.0  # sklearn _handle_zeros_in_scale (also catches all-NaN columns)
         in_scale = 1.0 / span
         in_offset = -lo * in_scale
-        # slot s works on its own copy of its machine's rows: the stacked machines repeated K + 1 times, slot s at copy0[s]
         total = int(n.sum())
-        copy0 = np.arange(K + 1, dtype=np.int64).repeat(M) * total + fit_x
-        copy_jobs = engine.jobs_to_device(engine.make_jobs(np.arange(S), np.tile(n, K + 1), fit_x, copy0), dev)
+        copy0, copy_jobs = _slot_copies(n, row0, K, dev)  # slot s works on its own copy of its machine's rows
         x = engine.affine_f64(copy_jobs, S, N, x.double(), in_scale.contiguous(), in_offset.contiguous(), out_rows=(K + 1) * total)
         y = y[:total].repeat(K + 1, 1)
         fit_x = copy0
@@ -550,31 +588,25 @@ def build_fleet(eng: "engine.FFEngine", x, y, rows, epochs: int = 1, batch_size:
         feat, agg = eng.thresholds(sc_jobs, KM, max_test, res["tag-anomaly-unscaled"], res["total-anomaly-scaled"], S, window=6)
     else:
         feat, agg, sfeat, sagg = eng.thresholds_pair(sc_jobs, KM, max_test, res["tag-anomaly-unscaled"], res["total-anomaly-scaled"], S, 6, int(window))
-        fold_sfeat = sfeat[M:].view(K, M, eng.n_out).permute(1, 0, 2).contiguous()
-        fold_sagg = sagg[M:].view(K, M).t().contiguous()
-    T = eng.n_out
+        fold_sfeat = _device_folds(sfeat[M:], M).contiguous()
+        fold_sagg = _device_folds(sagg[M:], M).contiguous()
     # the evaluation metrics of ModelBuilder's cross validation (build_model.py:250-289) reduce to five sums per (fold, tag)
-    moments = engine.cv_moments(mom_jobs, KM, res["model-output"], y_true, T).view(K, M, 5, T).permute(1, 0, 2, 3).contiguous()
-    fold_params = params[M:].view(K, M, -1).permute(1, 0, 2).contiguous()
-    fold_feat = feat[M:].view(K, M, T).permute(1, 0, 2).contiguous()
-    fold_agg = agg[M:].view(K, M).t().contiguous()
-    E = hist.shape[1]
-    folds = lambda t: None if t is None else t[M:].view(K, M, E).permute(1, 0, 2)  # noqa: E731
-    fold_jobs = lambda t: None if t is None else t[M:].view(K, M).t()  # noqa: E731
+    moments = _device_folds(engine.cv_moments(mom_jobs, KM, res["model-output"], y_true, eng.n_out), M).contiguous()
+    finals = lambda t: None if t is None else t[:M]  # noqa: E731
+    folds = lambda t: None if t is None else _device_folds(t[M:], M)  # noqa: E731
+    finals_c = lambda t: None if t is None else t[:M].contiguous()  # noqa: E731
+    folds_c = lambda t: None if t is None else folds(t).contiguous()  # noqa: E731
+    fold_params, fold_feat, fold_agg = folds_c(params), folds_c(feat), folds_c(agg)
     return FleetBuild(eng, M, K, params[:M].contiguous(), scale[:M].contiguous(), offset[:M].contiguous(), fold_feat[:, K - 1].contiguous(),
-                      fold_agg[:, K - 1].contiguous(), hist[:M], acc[:M], hist[M:].view(K, M, E).permute(1, 0, 2), fold_feat, fold_agg,
-                      fold_params=fold_params, cv_moments=moments,
-                      in_scale=None if in_scale is None else in_scale[:M].contiguous(), in_offset=None if in_offset is None else in_offset[:M].contiguous(),
-                      fold_in_scale=None if in_scale is None else in_scale[M:].view(K, M, -1).permute(1, 0, 2).contiguous(),
-                      fold_in_offset=None if in_offset is None else in_offset[M:].view(K, M, -1).permute(1, 0, 2).contiguous(),
+                      fold_agg[:, K - 1].contiguous(), hist[:M], acc[:M], folds(hist), fold_feat, fold_agg,
+                      fold_params=fold_params, cv_moments=moments, in_scale=finals_c(in_scale), in_offset=finals_c(in_offset),
+                      fold_in_scale=folds_c(in_scale), fold_in_offset=folds_c(in_offset),
                       steps_per_epoch=(n_train[:M] + int(batch_size) - 1) // int(batch_size),
-                      val_loss=None if val_loss is None else val_loss[:M], val_acc=None if val_acc is None else val_acc[:M],
-                      fold_val_loss=folds(val_loss), fold_val_acc=folds(val_acc), epochs=int(epochs),
-                      epochs_run=None if epochs_run is None else epochs_run[:M], best_epoch=None if best_epoch is None else best_epoch[:M],
-                      fold_epochs_run=fold_jobs(epochs_run), fold_best_epoch=fold_jobs(best_epoch), rows=n, n_test=test, starts=starts,
-                      init_params=init_params, window=None if window is None else int(window), fold_smooth_feat_thr=fold_sfeat,
-                      fold_smooth_agg_thr=fold_sagg, **({} if y_lo is None else dict(y_min=y_lo[:M], y_max=y_hi[:M], fold_y_min=_folds(y_lo, M, K),
-                                                                                      fold_y_max=_folds(y_hi, M, K))))
+                      val_loss=finals(val_loss), val_acc=finals(val_acc), fold_val_loss=folds(val_loss), fold_val_acc=folds(val_acc), epochs=int(epochs),
+                      epochs_run=finals(epochs_run), best_epoch=finals(best_epoch), fold_epochs_run=folds(epochs_run), fold_best_epoch=folds(best_epoch),
+                      rows=n, n_test=test, starts=starts, init_params=init_params, window=None if window is None else int(window),
+                      fold_smooth_feat_thr=fold_sfeat, fold_smooth_agg_thr=fold_sagg,
+                      **({} if y_lo is None else dict(y_min=y_lo[:M], y_max=y_hi[:M], fold_y_min=_folds(y_lo[M:], M), fold_y_max=_folds(y_hi[M:], M))))
 
 
 def _f64(a, device):
@@ -591,10 +623,15 @@ def _slot_extrema(jobs_dev, n_jobs, max_rows, a64):
     return lo, hi
 
 
-def _folds(a, n_machines: int, n_splits: int):
-    """Slot-ordered host rows [S, ...] (finals, then fold k of machine m at M + k*M + m) -> every machine's folds [M, K, ...]."""
-    M, K = n_machines, n_splits
-    return np.ascontiguousarray(np.swapaxes(a[M:].reshape((K, M) + a.shape[1:]), 0, 1))
+def _folds(a, n_machines: int):
+    """Fold-ordered host rows [K*M, ...] (fold k of machine m at k*M + m: the rows of a slot-ordered array from M on, or one per
+    fold job) -> every machine's folds [M, K, ...], contiguous."""
+    return np.ascontiguousarray(np.swapaxes(a.reshape((-1, n_machines) + a.shape[1:]), 0, 1))
+
+
+def _device_folds(t, n_machines: int):
+    """``_folds`` of a device tensor, as a view."""
+    return t.view((-1, n_machines) + tuple(t.shape[1:])).transpose(0, 1)
 
 
 # ------------------------------------------------------------------------------------------------ fleet build of LSTM detectors
@@ -688,15 +725,14 @@ class LSTMFleetBuild:
         attributes the per-machine build leaves.  ``template``: an unfitted detector from the machine's own definition, filled in
         so that the estimator class, ``kind`` and the other constructor arguments survive.
         """
-        import pandas as pd
         from sklearn.pipeline import Pipeline
         from sklearn.preprocessing import MinMaxScaler
 
         from .machine.model.anomaly.diff import DiffBasedAnomalyDetector
-        from .machine.model.models import FittedNet, History, KerasLSTMAutoEncoder, KerasLSTMForecast
+        from .machine.model.models import FittedNet, KerasLSTMAutoEncoder, KerasLSTMForecast
 
         eng = self.eng
-        T, K = eng.n_out, self.n_splits
+        T = eng.n_out
         tags = list(tags) if tags is not None else list(range(T))
         ttr = None
         if template is not None:
@@ -723,27 +759,15 @@ class LSTMFleetBuild:
             spec = lstm._build_spec()
             det = DiffBasedAnomalyDetector(base_estimator=lstm, scaler=MinMaxScaler(), **({} if self.window is None else {"window": self.window}))
         lstm.model = FittedNet(spec, eng.unpack_params(self.params[m : m + 1])[0])
-        hist = {"loss": [float(v) for v in self.loss[m]]}
-        if "accuracy" in spec.metrics:
-            hist["accuracy"] = [float(v) for v in self.acc[m]]
-        if self.epochs_run is None:
-            lstm._history = History(hist, {"verbose": 0, "epochs": len(hist["loss"]), "steps": int(self.machine_steps[m])}, list(range(len(hist["loss"]))))
-        else:  # as the per-machine fit loop leaves it: the epochs run, against the configured count
-            ran = int(self.epochs_run[m])
-            hist = {k: v[:ran] for k, v in hist.items()}
-            lstm._history = History(hist, {"verbose": 0, "epochs": int(self.epochs), "steps": int(self.machine_steps[m])}, list(range(ran)))
-        lstm.model.history = lstm._history
+        _fill_history(lstm, spec.metrics, self.epochs, int(self.machine_steps[m]), self.loss[m], self.acc[m],
+                      epochs_run=None if self.epochs_run is None else self.epochs_run[m])
         if ttr is not None:
             _fill_target_regressor(ttr, est, self.y_min[m], self.y_max[m], self.rows[m])
         # a fresh scaler: detectors made from definitions without a scaler share the constructor's default MinMaxScaler object
         det.scaler = _fill_minmax_from_extrema(MinMaxScaler(), self.y_min[m], self.y_max[m], self.rows[m], tags)
-        det.feature_thresholds_ = pd.Series(self.feat_thr[m].copy(), index=tags, name=f"fold-{K - 1}")
-        det.aggregate_threshold_ = float(self.agg_thr[m])
-        det.feature_thresholds_per_fold_ = pd.DataFrame(self.fold_feat_thr[m].copy(), columns=tags, index=[f"fold-{k}" for k in range(K)])
-        det.aggregate_thresholds_per_fold_ = {f"fold-{k}": float(self.fold_agg_thr[m, k]) for k in range(K)}
-        if self.window is None:
-            return _fill_smooth_thresholds(det, None, None, None, tags)
-        return _fill_smooth_thresholds(det, self.window, self.fold_smooth_feat_thr[m], self.fold_smooth_agg_thr[m], tags)
+        windowed = self.window is not None
+        return _fill_thresholds(det, tags, self.feat_thr[m], self.agg_thr[m], self.fold_feat_thr[m], self.fold_agg_thr[m], self.window,
+                                self.fold_smooth_feat_thr[m] if windowed else None, self.fold_smooth_agg_thr[m] if windowed else None)
 
 
 class _FoldBlocks:
@@ -812,44 +836,34 @@ def build_lstm_fleet(eng: "engine.LSTMEngine", x, y, rows, lookahead: int = 0, e
     # per slot (final fits, then fold k of machine m at M + k*M + m): training rows / windows and the first row of its machine
     slot_rows = np.concatenate([n] + [starts[:, k] for k in range(K)])
     slot_windows = slot_rows - L + 1 - la            # the estimator's window count
-    base = np.tile(row0, K + 1)
+    x_row = np.tile(row0, K + 1)
 
     def host(t):
         return t.cpu().numpy()
 
-    def extrema(a):
-        jobs = engine.jobs_to_device(engine.make_jobs(np.arange(S), slot_rows, base), dev)
-        lo, hi = (host(t) for t in engine.minmax_f64(jobs, S, N, a, S))
-        if not (np.isfinite(lo).all() and np.isfinite(hi).all()):
-            raise ValueError("a column without finite values in a training block")
-        return lo, hi
-
     # target scalers: final on all rows, fold k on its training prefix (diff.py:173 inside each CV clone), float64 like _fit_scaler
-    y_lo, y_hi = extrema(y)
+    prefix_jobs = engine.jobs_to_device(engine.make_jobs(np.arange(S), slot_rows, x_row), dev)
+    y_lo, y_hi = _slot_extrema(prefix_jobs, S, N, y)
     y32 = y.to(torch.float32)
     in_lo = in_hi = None
+    total = int(n.sum())
+    if input_scaler or target_scaler:  # slot s trains on its own copy of its machine's rows, at x_row[s]
+        x_row, copy_jobs = _slot_copies(n, row0, K, dev)
     if input_scaler:
         # every fold clone fits the Pipeline's MinMaxScaler on its own prefix: slot s trains on its own float64-scaled copy of its
-        # machine's rows -- the stacked machines repeated K + 1 times, slot s at x_row[s] (gb_affine_f64: sklearn's transform,
-        # rounded once)
-        in_lo, in_hi = (y_lo, y_hi) if y is x else extrema(x)
-        a, b = (torch.from_numpy(np.ascontiguousarray(v)).to(dev) for v in _minmax_attributes(in_lo, in_hi))
-        total = int(n.sum())
-        x_row = np.arange(K + 1, dtype=np.int64).repeat(M) * total + base
-        copy_jobs = engine.jobs_to_device(engine.make_jobs(np.arange(S), np.tile(n, K + 1), base, x_row), dev)
+        # machine's rows (gb_affine_f64: sklearn's transform, rounded once)
+        in_lo, in_hi = (y_lo, y_hi) if y is x else _slot_extrema(prefix_jobs, S, N, x)
+        a, b = (_f64(v, dev) for v in _minmax_attributes(in_lo, in_hi))
         xf = engine.affine_f64(copy_jobs, S, N, x, a, b, out_rows=(K + 1) * total)
         yf = y32[:total].repeat(K + 1, 1)
     else:
         xf = y32 if y is x else x.to(torch.float32)
-        yf, x_row = y32, base
+        yf = y32
     if target_scaler:
         # TransformedTargetRegressor(MinMaxScaler()): the transformer saw the extrema above, and slot s trains on its own float32 copy of
         # its scaled targets at x_row[s], laid out as the input scaler's copies are (one copy for both when they see the same array)
-        total = int(n.sum())
         if not input_scaler:
-            x_row = np.arange(K + 1, dtype=np.int64).repeat(M) * total + base
             xf = xf[:total].repeat(K + 1, 1)
-        copy_jobs = engine.jobs_to_device(engine.make_jobs(np.arange(S), np.tile(n, K + 1), base, x_row), dev)
         t_scale, t_offset = _minmax_attributes(y_lo, y_hi)
         yf = xf if (input_scaler and y is x) else engine.affine_f64(copy_jobs, S, N, y, _f64(t_scale, dev), _f64(t_offset, dev), out_rows=(K + 1) * total)
 
@@ -857,12 +871,8 @@ def build_lstm_fleet(eng: "engine.LSTMEngine", x, y, rows, lookahead: int = 0, e
     # (batches above 32 windows train on the tensor-core family, whose workspace grows with the batch)
     fit = eng.fit_for_batch(batch_size)
     per_machine_bytes = eng.fit_workspace_bytes_for_batch(K + 1, batch_size)
-    stop = epochs_run = best_epoch = None
-    if early_stopping is not None:
-        per_machine = list(early_stopping) if isinstance(early_stopping, (list, tuple)) else [early_stopping] * M
-        if len(per_machine) != M:
-            raise ValueError(f"early_stopping: {len(per_machine)} callbacks for {M} machines")
-        stop = engine.make_stop([per_machine[s % M] for s in range(S)])  # slot s belongs to machine s mod M
+    stop, epochs_run, best_epoch = _slot_stops(early_stopping, M, S), None, None
+    if stop is not None:
         per_machine_bytes += int(eng.lib.gb_lstm_fit_stop_state_bytes(K + 1))
         if stop["restore_best"].any():  # the snapshot area
             per_machine_bytes += (K + 1) * eng.param_stride * 4
@@ -909,36 +919,28 @@ def build_lstm_fleet(eng: "engine.LSTMEngine", x, y, rows, lookahead: int = 0, e
         res = engine.minmax_inverse_score_f64(score_jobs, KM, max_n, pred, y, _f64(y_scale[M:], dev), _f64(y_offset[M:], dev),
                                               scale=_f64(((y_scale + y_offset) - y_offset)[M:], dev), want=want, out={"model-output": pred})
     else:
-        fold_scale = torch.from_numpy(np.ascontiguousarray(y_scale[M:])).to(dev)
-        res = engine.anomaly_score(score_jobs, KM, max_n, pred.to(torch.float64), y, T, scale=fold_scale, want=want)
+        res = engine.anomaly_score(score_jobs, KM, max_n, pred.to(torch.float64), y, T, scale=_f64(y_scale[M:], dev), want=want)
     fold_sfeat = fold_sagg = None
     if window is None:
         feat, agg = engine.thresholds(score_jobs, KM, max_n, res["tag-anomaly-unscaled"], res["total-anomaly-scaled"], T, KM, 6, dev)
     else:
         feat, agg, sfeat, sagg = engine.thresholds_pair(score_jobs, KM, max_n, res["tag-anomaly-unscaled"], res["total-anomaly-scaled"], T, KM, 6,
                                                         int(window), dev)
-        fold_sfeat = np.ascontiguousarray(host(sfeat).reshape(K, M, T).transpose(1, 0, 2))
-        fold_sagg = np.ascontiguousarray(host(sagg).reshape(K, M).T)
+        fold_sfeat, fold_sagg = _folds(host(sfeat), M), _folds(host(sagg), M)
     # the evaluation metrics of ModelBuilder's cross validation reduce to five sums per (fold, tag)
-    moments = host(engine.cv_moments(score_jobs, KM, pred, y32, T)).reshape(K, M, 5, T).transpose(1, 0, 2, 3)
-    fold_feat = host(feat).reshape(K, M, T).transpose(1, 0, 2)
-    fold_agg = host(agg).reshape(K, M).T
+    moments = _folds(host(engine.cv_moments(score_jobs, KM, pred, y32, T)), M)
+    fold_feat, fold_agg = _folds(host(feat), M), _folds(host(agg), M)
     loss_h, acc_h = host(hist), host(acc)
-
-    def folds(a):  # slot-ordered [S, ...] -> the folds of every machine [M, K, ...]
-        return np.ascontiguousarray(np.swapaxes(a[M:].reshape((K, M) + a.shape[1:]), 0, 1))
-
+    finals = lambda a: None if a is None else a[:M]  # noqa: E731
+    folds = lambda a: None if a is None else _folds(a[M:], M)  # noqa: E731
     return LSTMFleetBuild(
-        eng, M, K, n, la, int(batch_size), starts, n_test, params[:M].contiguous(), params[M:].view(K, M, -1).permute(1, 0, 2).contiguous(),
+        eng, M, K, n, la, int(batch_size), starts, n_test, params[:M].contiguous(), _device_folds(params[M:], M).contiguous(),
         init_params, loss_h[:M], acc_h[:M], folds(loss_h), folds(acc_h), y_lo[:M], y_hi[:M], folds(y_lo), folds(y_hi),
-        np.ascontiguousarray(fold_feat[:, K - 1]), np.ascontiguousarray(fold_agg[:, K - 1]), np.ascontiguousarray(fold_feat),
-        np.ascontiguousarray(fold_agg), np.ascontiguousarray(moments), _FoldBlocks(pred, out0, job_n, M),
-        in_min=None if in_lo is None else in_lo[:M], in_max=None if in_hi is None else in_hi[:M],
-        fold_in_min=None if in_lo is None else folds(in_lo), fold_in_max=None if in_hi is None else folds(in_hi), epochs=int(epochs),
-        epochs_run=None if stop is None else epochs_run[:M], best_epoch=None if stop is None else best_epoch[:M],
-        fold_epochs_run=None if stop is None else epochs_run[M:].reshape(K, M).T.copy(),
-        fold_best_epoch=None if stop is None else best_epoch[M:].reshape(K, M).T.copy(), window=None if window is None else int(window),
-        fold_smooth_feat_thr=fold_sfeat, fold_smooth_agg_thr=fold_sagg, target_scaler=target_scaler)
+        np.ascontiguousarray(fold_feat[:, K - 1]), np.ascontiguousarray(fold_agg[:, K - 1]), fold_feat, fold_agg, moments,
+        _FoldBlocks(pred, out0, job_n, M), in_min=finals(in_lo), in_max=finals(in_hi), fold_in_min=folds(in_lo), fold_in_max=folds(in_hi),
+        epochs=int(epochs), epochs_run=finals(epochs_run), best_epoch=finals(best_epoch), fold_epochs_run=folds(epochs_run),
+        fold_best_epoch=folds(best_epoch), window=None if window is None else int(window), fold_smooth_feat_thr=fold_sfeat,
+        fold_smooth_agg_thr=fold_sagg, target_scaler=target_scaler)
 
 
 # ------------------------------------------------------------------------------------------------ fleet build of K-fold detectors
@@ -973,12 +975,8 @@ class KFoldFleetBuild:
         Machine ``m`` as its fitted ``DiffBasedKFCVAnomalyDetector``: ``template`` is an unfitted detector from the machine's own
         definition, filled in with the attributes the per-machine build leaves (picklable, servable).
         """
-        import pandas as pd
-
         det = self._fill(m, template, tags, input_tags)
-        det.feature_thresholds_ = pd.Series(self.feat_thr[m].copy(), index=list(tags) if tags is not None else list(range(self.eng.n_out)))
-        det.aggregate_threshold_ = float(self.agg_thr[m])
-        return det
+        return _fill_thresholds(det, list(tags) if tags is not None else list(range(self.eng.n_out)), self.feat_thr[m], self.agg_thr[m])
 
     def fold_detector(self, m: int, k: int, template, tags=None, input_tags=None):
         """Fold k's detector of machine m (a ``cross_validate`` estimator: fitted on fold k's training rows, no thresholds)."""
@@ -986,35 +984,19 @@ class KFoldFleetBuild:
 
     def _fill(self, s: int, template, tags, input_tags):
         """``template`` with the fitted state of slot ``s``: scalers, weights, History, the target transformer."""
-        from sklearn.pipeline import Pipeline
         from sklearn.preprocessing import MinMaxScaler
 
-        from .machine.model.models import History
-
-        eng, M = self.eng, self.n_machines
+        M = self.n_machines
         m = s % M
         n_rows = int(self.rows[m]) if s < M else int(self.rows[m] - self.n_test[m, (s - M) // M])  # the rows the slot's scalers saw
-        T = eng.n_out
-        tags = list(tags) if tags is not None else list(range(T))
+        tags = list(tags) if tags is not None else list(range(self.eng.n_out))
         det = template
-        ttr, reg = _target_regressor_of(det.base_estimator, self.target_scaler)
-        ae = reg.steps[-1][1] if isinstance(reg, Pipeline) else reg
-        if isinstance(reg, Pipeline) != (self.in_min is not None):
-            raise ValueError("the template's input scaler and the fleet's do not match")
-        if isinstance(reg, Pipeline):
+        ttr, reg, ae = _ff_template(self.eng, det, self.target_scaler, self.in_min is not None, self.params[s : s + 1])
+        if self.in_min is not None:
             _fill_minmax_from_extrema(reg.steps[0][1], self.in_min[s], self.in_max[s], n_rows, input_tags)
-        ae.kwargs.update({"n_features": eng.n_in, "n_features_out": T})
-        ae._prepare_model()
-        if list(ae.model.spec.dims) != list(eng.dims) or list(ae.model.spec.acts) != list(eng.acts):
-            raise ValueError("template architecture differs from the fleet's")
-        ae.model.weights = eng.unpack_params(self.params[s : s + 1])[0]
-        ran = int(self.epochs_run[s]) if self.epochs_run is not None else self.loss.shape[1]
-        hist = {"loss": [float(v) for v in self.loss[s, :ran]], "accuracy": [float(v) for v in self.acc[s, :ran]]}
-        if self.val_loss is not None:  # the keys and their order of the per-machine History
-            hist["val_loss"] = [float(v) for v in self.val_loss[s, :ran]]
-            hist["val_accuracy"] = [float(v) for v in self.val_acc[s, :ran]]
-        ae._history = History(hist, {"verbose": 0, "epochs": int(self.epochs), "steps": int(self.slot_steps[s])}, list(range(ran)))
-        ae.model.history = ae._history
+        slot = lambda a: None if a is None else a[s]  # noqa: E731
+        _fill_history(ae, ae.model.spec.metrics, self.epochs, int(self.slot_steps[s]), self.loss[s], self.acc[s], slot(self.val_loss),
+                      slot(self.val_acc), slot(self.epochs_run))
         if ttr is not None:
             _fill_target_regressor(ttr, reg, self.y_min[s], self.y_max[s], n_rows)
         # a fresh scaler: detectors made from definitions without a scaler share the constructor's default MinMaxScaler object
@@ -1136,9 +1118,6 @@ def build_kfold_fleet(eng: "engine.FFEngine", x, y, rows, cv, epochs: int = 1, b
     def jobs(slots, rows_, x_row, out_row=None):
         return engine.jobs_to_device(engine.make_jobs(slots, rows_, x_row, out_row), dev)
 
-    def f64(a):
-        return torch.from_numpy(np.ascontiguousarray(a, dtype=np.float64)).to(dev)
-
     to_fold, to_time = i32(to_fold), i32(to_time)
 
     # 1. fold order: one gather per array
@@ -1167,30 +1146,24 @@ def build_kfold_fleet(eng: "engine.FFEngine", x, y, rows, cv, epochs: int = 1, b
     # 3. the fits' inputs: with a scaler in front of the network or on the targets, slot s owns its own copy of its machine's rows
     # (the stacked machines repeated K + 1 times, slot s at slot_x[s])
     per_slot = input_scaler or target_scaler
-    machine_of = np.tile(row0, K + 1)
-    slot_x = np.arange(K + 1, dtype=np.int64).repeat(M) * total + machine_of if per_slot else machine_of  # first row of slot s in x / y
-    slot_rows = np.tile(n, K + 1)
-    copy_jobs = jobs(np.arange(S), slot_rows, machine_of, slot_x)
+    slot_x, copy_jobs = _slot_copies(n, row0, K, dev) if per_slot else (np.tile(row0, K + 1), None)  # first row of slot s in x / y
     per_slot_ofs = i64(np.tile(machine_ofs, K + 1))
     if input_scaler:
         a, b = _minmax_attributes(in_lo, in_hi)
-        xf = engine.affine_f64(copy_jobs, S, N, xq, f64(a), f64(b), out_rows=(K + 1) * total)
+        xf = engine.affine_f64(copy_jobs, S, N, xq, _f64(a, dev), _f64(b, dev), out_rows=(K + 1) * total)
     elif per_slot:
         xf = engine.gather_rows(copy_jobs, S, N, to_fold, x, (K + 1) * total, to_f32=True, map_ofs=per_slot_ofs)
     else:
         xf = engine.gather_rows(whole, M, N, to_fold, x, total, to_f32=True, map_ofs=per_machine)
     if target_scaler:
-        yf = xf if (input_scaler and y is x) else engine.affine_f64(copy_jobs, S, N, yq, f64(y_scale), f64(y_offset), out_rows=(K + 1) * total)
+        yf = xf if (input_scaler and y is x) else engine.affine_f64(copy_jobs, S, N, yq, _f64(y_scale, dev), _f64(y_offset, dev), out_rows=(K + 1) * total)
     elif per_slot:
         yf = engine.gather_rows(copy_jobs, S, N, to_fold, y, (K + 1) * total, to_f32=True, map_ofs=per_slot_ofs)
     else:
         yf = xf if y is x else engine.gather_rows(whole, M, N, to_fold, y, total, to_f32=True, map_ofs=per_machine)
 
     slot_n = np.concatenate([n] + [n - n_test[:, k] for k in range(K)])  # rows each slot's estimator receives
-    vsplit = float(validation_split or 0.0)
-    n_train = np.asarray([int(math.floor(v * (1.0 - vsplit))) if 0.0 < vsplit < 1.0 else int(v) for v in slot_n], dtype=np.int64)  # keras' split
-    if n_train.min() < 1:
-        raise ValueError(f"validation_split {vsplit} leaves the {int(slot_n.min())}-row slot without a training row")
+    n_train = _keras_train_rows(slot_n, validation_split)
     split = engine.make_split(slot_n - n_train, slot_map)
     row_map = i32(fit_maps)
     g = generator or torch.Generator(device=dev).manual_seed(seed)
@@ -1217,7 +1190,7 @@ def build_kfold_fleet(eng: "engine.FFEngine", x, y, rows, cv, epochs: int = 1, b
     else:  # predict, then in one pass sklearn's float32 inverse of the slot's transformer and float64 scoring against the float64 targets
         pred = eng.infer_score(params, sc_jobs, KM, max_test, xf, out_rows=total)["model-output"]
         mom_jobs = jobs(sc_slots, sc_n, out0, out0)
-        res = engine.minmax_inverse_score_f64(mom_jobs, KM, max_test, pred, yq, f64(y_scale), f64(y_offset), scale=f64(mult), want=want,
+        res = engine.minmax_inverse_score_f64(mom_jobs, KM, max_test, pred, yq, _f64(y_scale, dev), _f64(y_offset, dev), scale=_f64(mult, dev), want=want,
                                               out_rows=total)
         pred32, tag_err, tot_err = res["model-output"], res["tag-anomaly-unscaled"], res["total-anomaly-scaled"]
         y32 = engine.gather_rows(whole, M, N, to_fold, y, total, to_f32=True, map_ofs=per_machine)
@@ -1242,4 +1215,4 @@ def build_kfold_fleet(eng: "engine.FFEngine", x, y, rows, cv, epochs: int = 1, b
     return KFoldFleetBuild(
         eng, M, K, n, n_test, params, init_params, host(hist), host(acc), host(val_loss), host(val_acc), int(epochs), host(epochs_run),
         host(best_epoch), (n_train + int(batch_size) - 1) // int(batch_size), y_lo, y_hi, in_lo, in_hi, bool(target_scaler),
-        host(feat).astype(np.float64), host(agg).astype(np.float64), host(moments).reshape(K, M, 5, T).transpose(1, 0, 2, 3).copy())
+        host(feat).astype(np.float64), host(agg).astype(np.float64), _folds(host(moments), M))

@@ -182,6 +182,27 @@ def test_fleet_model_builder_end_to_end(engine, torch, tmp_path):
     assert set(m["metadata"]["build_metadata"]["model"]) == {"cross_validation"} and m["metadata"]["build_metadata"]["model"]["cross_validation"]["scores"]
 
 
+@pytest.mark.parametrize("definition", [DETECTOR, SCALED], ids=["bare", "pipeline"])
+def test_fleet_detectors_leave_the_history_on_the_network(engine, torch, definition):
+    """The estimator's fit leaves its Keras History on the network too (``model.history``); so does the batched build."""
+    from gordo_components_b200 import builder
+
+    data = _series(240, 4, 11)
+    machine = {"name": "history", "model": definition, "dataset": (data, data)}
+    assert builder._canonical(0, machine) is not None
+    batched = builder.FleetModelBuilder([dict(machine)]).build()[0][0]
+    single = builder.ModelBuilder(dict(machine)).build()[0]
+    got, want = (_network_of(m) for m in (batched, single))
+    assert got.model.history is got._history and want.model.history is want._history
+    assert list(got._history.history) == list(want._history.history) and got._history.params == want._history.params
+    assert got._history.epoch == want._history.epoch
+
+
+def _network_of(detector):
+    est = detector.base_estimator
+    return est.steps[-1][1] if hasattr(est, "steps") else est
+
+
 def frame(rows=160, tags=4, seed=5):
     """The data of the tests/golden/dropin.json build."""
     rng = np.random.default_rng(seed)

@@ -440,6 +440,30 @@ def test_fleet_builder_matches_the_per_machine_fit(engine, torch, km, tmp_path):
             list(single_meta["metadata"]["build_metadata"]["model"]["cross_validation"]["scores"])
 
 
+def test_kfold_fleet_builder_reports_the_loss_alone_without_metrics(engine, torch, monkeypatch):
+    """A raw regressor compiled without metrics: its K-fold detector's History has the loss (and val_loss) only, batched as per
+    machine."""
+    import pandas as pd
+
+    from gordo_components_b200 import builder
+
+    T, N = 4, 300
+    idx = pd.date_range("2020-01-01", periods=N, freq="10min", tz="UTC")
+    frame = pd.DataFrame(waves(np.random.default_rng(7), N, T), index=idx, columns=[f"tag-{c}" for c in range(T)])
+    est = {"gordo.machine.model.models.KerasRawModelRegressor": {"kind": raw_kind(T), "epochs": 2, "validation_split": 0.2}}
+    machine = {"name": "raw-kfold", "dataset": {"X": frame, "y": frame}, "evaluation": {"cv": {"sklearn.model_selection.KFold": {"n_splits": 3}}},
+               "model": {"gordo.machine.model.anomaly.diff.DiffBasedKFCVAnomalyDetector": {"base_estimator": est}}}
+    calls = []
+    orig = builder.FleetModelBuilder._build_bucket
+    monkeypatch.setattr(builder.FleetModelBuilder, "_build_bucket", staticmethod(lambda members: calls.append(len(members)) or orig(members)))
+    batched, batched_meta = builder.FleetModelBuilder([dict(machine)], kfcv=True).build()[0]
+    assert calls == [1]
+    single, single_meta = builder.ModelBuilder(dict(machine)).build()
+    for meta in (batched_meta, single_meta):
+        assert list(meta["metadata"]["build_metadata"]["model"]["model_meta"]["history"]) == ["loss", "val_loss", "params"]
+    assert batched.base_estimator._history.params == single.base_estimator._history.params
+
+
 def test_every_regularized_kernel_instantiation_runs(engine, torch):
     """The nine ffae_fit_reg_kernel<WG, DG, SPLIT, STOP> a record reaches, one per (memory plan group, entry point), read back from
     torch.profiler; the same launches without a record reach the MSE-Adam ffae_fit_kernel, never a regularized one."""
