@@ -285,7 +285,7 @@ __global__ void lstm_tc_tiles_kernel(const gb_job* __restrict__ jobs, int n_jobs
 
 // layer 0 input projection per x row of a job: xk[block][n'][r] = x[x_row + r] . K0[:, col(n')] + b0[col(n')] with the job's slot;
 // grid (ceil(rows/32), 4u/64, jobs from job0).  Job j writes its n_rows + lookback - 1 rows into the blocks from tile_base[j] + j * xk_pad
-// (never past the next job's first block).
+// (never past the next job's first block); a job without windows reads and writes nothing, wherever its x_row points.
 __global__ void __launch_bounds__(256) lstm_tc_xk_kernel(const gb_job* __restrict__ jobs, int job0, const int32_t* __restrict__ tile_base, int n_tiles,
                                                          const float* __restrict__ x, int F, int u, int up, int lookback, const float* __restrict__ params,
                                                          long pstride, int xk_pad, float* __restrict__ xk) {
@@ -293,7 +293,7 @@ __global__ void __launch_bounds__(256) lstm_tc_xk_kernel(const gb_job* __restric
   const gb_job job = jobs[job_id];
   const int tb0 = __ldg(tile_base + job_id), tb1 = __ldg(tile_base + job_id + 1);
   if (tb0 < 0 || tb1 < tb0 || tb1 > n_tiles) return;
-  const int n_x = (int)min((long)job.n_rows + lookback - 1, (long)(tb1 - tb0 + xk_pad) * TILE);  // x rows this job's windows touch
+  const int n_x = job.n_rows == 0 ? 0 : (int)min((long)job.n_rows + lookback - 1, (long)(tb1 - tb0 + xk_pad) * TILE);  // x rows this job's windows touch
   const int r0 = blockIdx.x * 32;
   if (r0 >= n_x) return;
   const float* P = params + (long)job.slot * pstride;  // layer 0: kernel [F][4u] first
