@@ -285,97 +285,58 @@ class ResidentBucket:
 
     def __init__(self, store: "ModelStore", names: Optional[List[str]] = None, input_scalers: bool = False, lstm: bool = False,
                  smoothing: bool = False, target_scaler: bool = False, **coalescer_kwargs):
-        from . import engine
+        from . import engine, serving
         from .machine.model.anomaly.diff import _compose_affine, _scaler_multiplier
-        from .serving import AnomalyCoalescer
 
-        if lstm:
-            self._init_lstm(store, names, smoothing, target_scaler, coalescer_kwargs)
-            return
-        groups = self.ff_groups({name: store.model(name) for name in (names if names is not None else store.names())}, input_scalers, smoothing,
-                                target_scaler)
+        candidates = {name: store.model(name) for name in (names if names is not None else store.names())}
+        groups = (self.lstm_groups(candidates, smoothing, target_scaler) if lstm
+                  else self.ff_groups(candidates, input_scalers, smoothing, target_scaler))
         if not groups:
-            raise ValueError("no model in the store can be served through a coalescer")
+            raise ValueError(f"no {'LSTM ' if lstm else ''}model in the store can be served through a coalescer")
+        self.lstm = lstm
         self.names = max(groups.values(), key=len)  # the largest architecture group
         self.slot = {name: i for i, name in enumerate(self.names)}
         models = [store.model(n) for n in self.names]
-        parts = [_served_parts(m) for m in models]
-        spec = parts[0][1].model.spec
-        eng = engine.ff_engine_for(spec)
+        parts = [_served_parts(m, lstm) for m in models]
+        eng = (engine.lstm_engine_for if lstm else engine.ff_engine_for)(parts[0][1].model.spec)
         torch = engine._torch()
-        params = eng.pack_params([ae.model.weights for _, ae in parts])
-        to_dev = lambda rows, dt=np.float32: torch.from_numpy(np.ascontiguousarray(np.stack(rows), dtype=dt)).to(eng.device)  # noqa: E731
+        params = eng.pack_params([net.model.weights for _, net in parts])
         self.target_scaler = _target_minmax(models[0]) is not None
-        dt = np.float64 if self.target_scaler else np.float32  # the scores of a target inverse are float64, as on the per-request route
-        scale = to_dev([_scaler_multiplier(m.scaler, eng.n_out) for m in models], dt)
+        # LSTM scores, and those of a target inverse, are float64, as on the per-request route
+        dt = np.float64 if lstm or self.target_scaler else np.float32
+        to_dev = lambda rows, dt=dt: torch.from_numpy(np.ascontiguousarray(np.stack(rows), dtype=dt)).to(eng.device)  # noqa: E731
+        scale = to_dev([_scaler_multiplier(m.scaler, eng.n_out) for m in models])
         feat, agg = zip(*(m._thresholds() for m in models))
-        feat_thr = to_dev([np.asarray(f, dtype=dt) for f in feat], dt) if feat[0] is not None else None
-        agg_thr = to_dev([dt(a) for a in agg], dt) if agg[0] is not None else None
+        feat_thr = to_dev([np.asarray(f, dtype=dt) for f in feat]) if feat[0] is not None else None
+        agg_thr = to_dev([dt(a) for a in agg]) if agg[0] is not None else None
         if self.target_scaler:
             y_scale, y_min = zip(*(_target_minmax(m) for m in models))
             coalescer_kwargs.update(y_inverse=(to_dev(y_scale, np.float64), to_dev(y_min, np.float64)))
-        self.input_scalers = bool(parts[0][0])
+        self.input_scalers = not lstm and bool(parts[0][0])  # an LSTM Pipeline's leading steps run on the host
         if self.input_scalers:
             a, b = zip(*(_compose_affine(pre, eng.n_in) for pre, _ in parts))
             coalescer_kwargs.update(x_scale=to_dev(a, np.float64), x_offset=to_dev(b, np.float64))
         self.smoothing = _smoothing_of(models[0])
-        self.coalescer = AnomalyCoalescer(eng, params, scale, feat_thr, agg_thr, smoothing=self.smoothing, **coalescer_kwargs)
-
-    def _init_lstm(self, store: "ModelStore", names: Optional[List[str]], smoothing: bool, target_scaler: bool, coalescer_kwargs):
-        from . import engine
-        from .machine.model.anomaly.diff import _scaler_multiplier
-        from .serving import LSTMAnomalyCoalescer
-
-        groups = self.lstm_groups({name: store.model(name) for name in (names if names is not None else store.names())}, smoothing,
-                                  target_scaler)
-        if not groups:
-            raise ValueError("no LSTM model in the store can be served through a coalescer")
-        self.lstm = True
-        self.names = max(groups.values(), key=len)  # the largest architecture group
-        self.slot = {name: i for i, name in enumerate(self.names)}
-        models = [store.model(n) for n in self.names]
-        nets = [_served_lstm_parts(m)[1] for m in models]
-        eng = engine.lstm_engine_for(nets[0].model.spec)
-        torch = engine._torch()
-        to_dev = lambda rows: torch.from_numpy(np.ascontiguousarray(np.stack(rows), dtype=np.float64)).to(eng.device)  # noqa: E731
-        params = eng.pack_params([net.model.weights for net in nets])
-        scale = to_dev([_scaler_multiplier(m.scaler, eng.n_out) for m in models])
-        feat, agg = zip(*(m._thresholds() for m in models))
-        feat_thr = to_dev([np.asarray(f, dtype=np.float64) for f in feat]) if feat[0] is not None else None
-        agg_thr = to_dev([np.float64(a) for a in agg]) if agg[0] is not None else None
-        self.smoothing = _smoothing_of(models[0])
-        self.target_scaler = _target_minmax(models[0]) is not None
-        if self.target_scaler:
-            y_scale, y_min = zip(*(_target_minmax(m) for m in models))
-            coalescer_kwargs.update(y_inverse=(to_dev(y_scale), to_dev(y_min)))
-        self.coalescer = LSTMAnomalyCoalescer(eng, params, scale, feat_thr, agg_thr, smoothing=self.smoothing, **coalescer_kwargs)
+        coalescer = serving.LSTMAnomalyCoalescer if lstm else serving.AnomalyCoalescer
+        self.coalescer = coalescer(eng, params, scale, feat_thr, agg_thr, smoothing=self.smoothing, **coalescer_kwargs)
 
     @classmethod
     def ff_groups(cls, models: Dict[str, Any], input_scalers: bool = False, smoothing: bool = False,
                   target_scaler: bool = False) -> Dict[Any, List[str]]:
-        """The eligible feed-forward detectors of ``models`` (name -> model) by (architecture, which thresholds are present, bare or
-        Pipeline, with or without a target transformer, smoothing)."""
-        groups: Dict[Any, List[str]] = {}
-        for name, model in models.items():
-            if cls.eligible(model, input_scalers, smoothing, target_scaler):
-                pre, ae = _served_parts(model)
-                spec = ae.model.spec
-                has_thr = tuple(t is not None for t in model._thresholds())
-                key = (tuple(spec.dims), tuple(spec.acts), tuple(spec.l1), has_thr, bool(pre), _target_minmax(model) is not None, _smoothing_of(model))
-                groups.setdefault(key, []).append(name)
-        return groups
+        """The eligible feed-forward detectors of ``models`` (name -> model) by (architecture, bare or Pipeline, which thresholds
+        are present, with or without a target transformer, smoothing)."""
+        def arch(model):
+            pre, ae = _served_parts(model)
+            spec = ae.model.spec
+            return tuple(spec.dims), tuple(spec.acts), tuple(spec.l1), bool(pre)
+
+        return _groups(models, lambda m: cls.eligible(m, input_scalers, smoothing, target_scaler), arch)
 
     @classmethod
     def lstm_groups(cls, models: Dict[str, Any], smoothing: bool = False, target_scaler: bool = False) -> Dict[Any, List[str]]:
         """The eligible LSTM detectors of ``models`` (name -> model) by (architecture, which thresholds are present, with or without
         a target transformer, smoothing)."""
-        groups: Dict[Any, List[str]] = {}
-        for name, model in models.items():
-            if cls.eligible_lstm(model, smoothing, target_scaler):
-                spec = _served_lstm_parts(model)[1].model.spec
-                key = (spec.key(), tuple(t is not None for t in model._thresholds()), _target_minmax(model) is not None, _smoothing_of(model))
-                groups.setdefault(key, []).append(name)
-        return groups
+        return _groups(models, lambda m: cls.eligible_lstm(m, smoothing, target_scaler), lambda m: (_served_parts(m, True)[1].model.spec.key(),))
 
     @staticmethod
     def eligible_lstm(model, smoothing: bool = False, target_scaler: bool = False) -> bool:
@@ -383,58 +344,35 @@ class ResidentBucket:
         needed)."""
         import ctypes as C
 
-        from sklearn.compose import TransformedTargetRegressor
-
         from . import _cabi
-        from .machine.model.anomaly.diff import _scaler_multiplier
 
-        if not (_frame_is_from_blocks(model) and _window_served(model, smoothing)
-                and not (model.require_thresholds and all(t is None for t in model._thresholds()))):
-            return False
-        parts = _served_lstm_parts(model)
-        if parts is None or parts[1].model is None:
+        parts = _admitted_parts(model, True, smoothing, target_scaler)
+        if parts is None:
             return False
         spec = parts[1].model.spec
-        if type(model.base_estimator) is TransformedTargetRegressor:
-            target = _target_minmax(model)
-            if not target_scaler or target is None or target[0].shape != (spec.n_features_out,):
-                return False
         net = _cabi.make_lstmnet(spec.n_features, spec.lstm_units, spec.acts, spec.n_features_out, spec.out_func, spec.lookback_window)
         if _cabi.load_library().gb_lstm_tc_supported(C.byref(net)) != 0:
             return False  # relu / linear cells: the fp32 kernel, on the per-request route
-        try:
-            _scaler_multiplier(model.scaler, spec.n_features_out)
-        except (ValueError, AttributeError):
-            return False
-        return True
+        return _error_scaler_is_affine(model, spec.n_features_out)
 
     @staticmethod
     def eligible(model, input_scalers: bool = False, smoothing: bool = False, target_scaler: bool = False) -> bool:
-        if not (_frame_is_from_blocks(model) and _window_served(model, smoothing)
-                and not (model.require_thresholds and all(t is None for t in model._thresholds()))):
-            return False
-        parts = _served_parts(model)
-        if parts is None or parts[1].model is None or (parts[0] and not input_scalers):
-            return False
-        pre, ae = parts
+        """True for a detector ``ResidentBucket(input_scalers=input_scalers, smoothing=smoothing, target_scaler=target_scaler)``
+        serves (no device needed)."""
         from sklearn.compose import TransformedTargetRegressor
         from sklearn.preprocessing import MinMaxScaler
 
-        from .machine.model.anomaly.diff import _compose_affine, _scaler_multiplier
+        from .machine.model.anomaly.diff import _compose_affine
 
+        parts = _admitted_parts(model, False, smoothing, target_scaler)
+        if parts is None or (parts[0] and not input_scalers):
+            return False
+        pre, ae = parts
         if pre and (_compose_affine(pre, ae.model.spec.dims[0]) is None or not _x64_launch_holds(ae.model.spec)):
             return False  # served per request: sklearn's own transform, or the separate gb_affine_f64 pass
-        if type(model.base_estimator) is TransformedTargetRegressor:
-            target = _target_minmax(model)
-            if not target_scaler or target is None or target[0].shape != (ae.model.spec.dims[-1],):
-                return False
-            if pre and not (len(pre) == 1 and type(pre[0]) is MinMaxScaler):
-                return False  # other scalers subtract and divide in sklearn's Pipeline.predict, which the composed affine does not round alike
-        try:  # a non-affine error scaler (clip=True, QuantileTransformer, ...) is served on the per-request path, not refused for the whole store
-            _scaler_multiplier(model.scaler, ae.model.spec.dims[-1])
-        except (ValueError, AttributeError):
-            return False
-        return True
+        if pre and type(model.base_estimator) is TransformedTargetRegressor and not (len(pre) == 1 and type(pre[0]) is MinMaxScaler):
+            return False  # other scalers subtract and divide in sklearn's Pipeline.predict, which the composed affine does not round alike
+        return _error_scaler_is_affine(model, ae.model.spec.dims[-1])
 
     def anomaly_blocks(self, store: "ModelStore", name: str, X: pd.DataFrame, y: pd.DataFrame, frequency=None, smooth: bool = True):
         """``model.anomaly_blocks(X, y, frequency, smooth)`` of the bucket's model ``name``, through the coalescer."""
@@ -476,10 +414,11 @@ class ResidentBucket:
         Around a TransformedTargetRegressor, the inverse's refusals follow the launch (``_scores``)."""
         from .machine.model.anomaly.diff import _has_inf, _values
 
-        pre, net = _served_lstm_parts(model)
+        pre, net = _served_parts(model, lstm=True)
         Xt = X
         for step in pre:
-            Xt = step.transform(Xt)
+            if step is not None and step != "passthrough":  # skipped, as Pipeline.predict skips them
+                Xt = step.transform(Xt)
         Xv = net._validate_and_fix_size_of_X(np.asarray(_values(Xt)))
         if _has_inf(Xv):
             return model.anomaly_blocks(X, y, frequency=frequency, smooth=smooth)
@@ -513,17 +452,18 @@ def _extract_X_y(store: ModelStore, name: str, json: Optional[dict], files: Opti
     return X, y
 
 
-def _served_parts(model):
-    """(input scaler steps, ``KerasAutoEncoder``) of a detector whose base estimator is a bare autoencoder ([] for the steps) or a
-    ``Pipeline`` ending in one, else None.  For a fitted ``TransformedTargetRegressor`` these are the parts of its ``regressor_``
-    (its target transformer: ``_target_minmax``).  A ``KerasRawModelRegressor`` is served as an autoencoder is: it is a Dense
-    stack too, and inference does not see its weight regularizers."""
+def _served_parts(model, lstm: bool = False):
+    """(leading Pipeline steps, network) of a detector whose base estimator is a bare network ([] for the steps) or a ``Pipeline``
+    ending in one, else None: a ``KerasAutoEncoder``, or with ``lstm`` a ``KerasLSTMAutoEncoder`` / ``KerasLSTMForecast``.  For a
+    fitted ``TransformedTargetRegressor`` these are the parts of its ``regressor_`` (its target transformer: ``_target_minmax``).
+    A ``KerasRawModelRegressor`` is served as an autoencoder is: it is a Dense stack too, and inference does not see its weight
+    regularizers."""
     from sklearn.compose import TransformedTargetRegressor
     from sklearn.pipeline import Pipeline
 
-    from .machine.model.models import KerasAutoEncoder, KerasRawModelRegressor
+    from .machine.model.models import KerasAutoEncoder, KerasLSTMAutoEncoder, KerasLSTMForecast, KerasRawModelRegressor
 
-    served = (KerasAutoEncoder, KerasRawModelRegressor)
+    served = (KerasLSTMAutoEncoder, KerasLSTMForecast) if lstm else (KerasAutoEncoder, KerasRawModelRegressor)
     est = model.base_estimator
     if type(est) is TransformedTargetRegressor:
         est = getattr(est, "regressor_", None)
@@ -532,6 +472,49 @@ def _served_parts(model):
     if type(est) is Pipeline and len(est.steps) > 1 and type(est.steps[-1][1]) in served:
         return [step for _, step in est.steps[:-1]], est.steps[-1][1]
     return None
+
+
+def _admitted_parts(model, lstm: bool, smoothing: bool, target_scaler: bool):
+    """``_served_parts(model, lstm)`` of a detector that passes the checks both kinds of bucket make, else None: this package's
+    ``anomaly``, a smoothing window the bucket takes (``_window_served``), the thresholds it requires, a fitted network, and around
+    a ``TransformedTargetRegressor`` (only with ``target_scaler``) a MinMax target transformer as wide as the network's output."""
+    from sklearn.compose import TransformedTargetRegressor
+
+    if not (_frame_is_from_blocks(model) and _window_served(model, smoothing)
+            and not (model.require_thresholds and all(t is None for t in model._thresholds()))):
+        return None
+    parts = _served_parts(model, lstm)
+    if parts is None or parts[1].model is None:
+        return None
+    if type(model.base_estimator) is TransformedTargetRegressor:
+        spec = parts[1].model.spec
+        target = _target_minmax(model)
+        if not target_scaler or target is None or target[0].shape != ((spec.n_features_out if lstm else spec.dims[-1]),):
+            return None
+    return parts
+
+
+def _error_scaler_is_affine(model, n_out: int) -> bool:
+    """True when the detector's error scaler is affine per feature.  A detector with any other (clip=True, QuantileTransformer, ...)
+    is served on the per-request route, not refused for the whole store."""
+    from .machine.model.anomaly.diff import _scaler_multiplier
+
+    try:
+        _scaler_multiplier(model.scaler, n_out)
+    except (ValueError, AttributeError):
+        return False
+    return True
+
+
+def _groups(models: Dict[str, Any], eligible, arch) -> Dict[Any, List[str]]:
+    """The names of the ``eligible`` detectors of ``models`` grouped by ``arch(model)`` + (which thresholds are present, with or
+    without a target transformer, smoothing), in the order of ``models``."""
+    groups: Dict[Any, List[str]] = {}
+    for name, model in models.items():
+        if eligible(model):
+            key = arch(model) + (tuple(t is not None for t in model._thresholds()), _target_minmax(model) is not None, _smoothing_of(model))
+            groups.setdefault(key, []).append(name)
+    return groups
 
 
 def _target_minmax(model):
@@ -551,26 +534,6 @@ def _target_minmax(model):
     if scale is None or mn is None or np.ndim(scale) != 1 or np.shape(scale) != np.shape(mn):
         return None
     return np.ascontiguousarray(scale, dtype=np.float64), np.ascontiguousarray(mn, dtype=np.float64)
-
-
-def _served_lstm_parts(model):
-    """(leading Pipeline steps, ``KerasLSTMAutoEncoder`` / ``KerasLSTMForecast``) of a detector whose base estimator is a bare LSTM
-    network ([] for the steps) or a ``Pipeline`` ending in one, else None.  Skipped steps (None, "passthrough") are left out, as
-    ``Pipeline.predict`` leaves them out.  For a fitted ``TransformedTargetRegressor`` these are the parts of its ``regressor_``
-    (its target transformer: ``_target_minmax``)."""
-    from sklearn.compose import TransformedTargetRegressor
-    from sklearn.pipeline import Pipeline
-
-    from .machine.model.models import KerasLSTMAutoEncoder, KerasLSTMForecast
-
-    est = model.base_estimator
-    if type(est) is TransformedTargetRegressor:
-        est = getattr(est, "regressor_", None)
-    if type(est) in (KerasLSTMAutoEncoder, KerasLSTMForecast):
-        return [], est
-    if type(est) is Pipeline and len(est.steps) > 1 and type(est.steps[-1][1]) in (KerasLSTMAutoEncoder, KerasLSTMForecast):
-        return [step for _, step in est.steps[:-1] if step is not None and step != "passthrough"], est.steps[-1][1]
-    return None
 
 
 def _smoothing_of(model):

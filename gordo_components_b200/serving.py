@@ -56,21 +56,16 @@ class AnomalyCoalescer:
     def __init__(self, eng: "engine.FFEngine", params, scale, feat_thr=None, agg_thr=None, max_batch_rows: int = 1 << 18,
                  max_wait_ms: float = 1.0, want: Optional[Sequence[str]] = None, x_scale=None, x_offset=None, smoothing=None, y_inverse=None):
         torch = engine._torch()
-        self.eng, self.params, self.scale, self.feat_thr, self.agg_thr = eng, params, scale, feat_thr, agg_thr
         if (x_scale is None) != (x_offset is None):
             raise ValueError("x_scale and x_offset go together")
+        self.max_rows = self.max_cost = int(max_batch_rows)
+        self._setup(eng, params, scale, feat_thr, agg_thr, max_wait_ms, want, smoothing, y_inverse)
         self.x_affine = (x_scale, x_offset) if x_scale is not None else None
         x_dtype = torch.float64 if self.x_affine is not None else torch.float32
         self._x_np = np.float64 if self.x_affine is not None else np.float32
-        self.y_inverse = tuple(y_inverse) if y_inverse is not None else None
         y_dtype, score_dtype = (torch.float64, torch.float64) if self.y_inverse is not None else (torch.float32, torch.float32)
         self._y_np = np.float64 if self.y_inverse is not None else np.float32
-        self.max_rows, self.max_wait = int(max_batch_rows), float(max_wait_ms) * 1e-3
-        self.want = tuple(want) if want is not None else tuple(
-            k for k in PER_TAG + PER_ROW if not ((feat_thr is None and k == "anomaly-confidence") or (agg_thr is None and k == "total-anomaly-confidence")))
-        self.smoothing = self._check_smoothing(smoothing)
         dev = eng.device
-        self._stream = torch.cuda.Stream(device=dev)
         self._xh = torch.empty((self.max_rows, eng.n_in), dtype=x_dtype).pin_memory()
         self._yh = torch.empty((self.max_rows, eng.n_out), dtype=y_dtype).pin_memory()
         self._xd = torch.empty((self.max_rows, eng.n_in), dtype=x_dtype, device=dev)
@@ -82,10 +77,20 @@ class AnomalyCoalescer:
         self._out_h = {k: torch.empty(v.shape, dtype=v.dtype).pin_memory() for k, v in self._out_d.items()}
         # the batch's jobs, then those of its requests that want the smoothed columns
         self._jobs_h = torch.empty((2 * self.max_jobs * engine._cabi.JOB_DTYPE.itemsize,), dtype=torch.uint8).pin_memory()
-        self.max_cost = self.max_rows
         self._start()
 
     max_jobs = 4096  # requests per batch: the pinned buffer the job records are staged through holds this many
+
+    def _setup(self, eng, params, scale, feat_thr, agg_thr, max_wait_ms, want, smoothing, y_inverse):
+        """What both coalescers keep: the bucket's device tensors, the score arrays a reply carries (by default all but the
+        confidences whose thresholds are absent), the smoothing option, the batching wait and the stream the batches run on."""
+        self.eng, self.params, self.scale, self.feat_thr, self.agg_thr = eng, params, scale, feat_thr, agg_thr
+        self.y_inverse = tuple(y_inverse) if y_inverse is not None else None
+        self.max_wait = float(max_wait_ms) * 1e-3
+        self.want = tuple(want) if want is not None else tuple(
+            k for k in PER_TAG + PER_ROW if not ((feat_thr is None and k == "anomaly-confidence") or (agg_thr is None and k == "total-anomaly-confidence")))
+        self.smoothing = self._check_smoothing(smoothing)
+        self._stream = engine._torch().cuda.Stream(device=eng.device)
 
     def _check_smoothing(self, smoothing):
         """``smoothing`` as (int window, method name), or None; ValueError for anything the smoothing launch does not take."""
@@ -202,12 +207,21 @@ class AnomalyCoalescer:
         return host
 
     @staticmethod
-    def _with_smoothed(result, item, smoothed, start, n):
-        """``result`` plus the request's rows of the smoothed arrays when it asked for them."""
-        if item[-2]:
-            lo = smoothed[1]
-            result.update({k: v[start - lo:start - lo + n].numpy().copy() for k, v in smoothed[0].items()})
-        return result
+    def _reply(batch, host, starts, counts, smoothed):
+        """Resolve each request of ``batch`` to copies of its rows ``[start, start + count)`` of the batch's host tensors ``host``
+        and, when it asked for them, of the smoothed arrays (``smoothed``: ``_smooth``'s result and its first row, or None).
+        ``host["raw-model-output"]`` (the network's prediction under a target inverse) goes only to a request whose
+        ``model-output`` holds ±inf."""
+        arrays = {k: v.numpy() for k, v in host.items()}
+        raw = arrays.pop("raw-model-output", None)
+        smooth, lo = ({k: v.numpy() for k, v in smoothed[0].items()}, smoothed[1]) if smoothed is not None else ({}, 0)
+        for item, start, n in zip(batch, starts, counts):
+            result = {k: v[start:start + n].copy() for k, v in arrays.items()}
+            if raw is not None and np.isinf(result.get("model-output", 0.0)).any():
+                result["raw-model-output"] = raw[start:start + n].copy()
+            if item[-2]:
+                result.update({k: v[start - lo:start - lo + n].copy() for k, v in smooth.items()})
+            item[-1].set_result(result)
 
     def _launch(self, torch, batch, rows):
         jobs = np.empty(len(batch), dtype=engine._cabi.JOB_DTYPE)
@@ -247,14 +261,7 @@ class AnomalyCoalescer:
         self._stream.synchronize()
         self.batches += 1
         self.requests += len(batch)
-        ofs = 0
-        for item in batch:
-            n = len(item[1])
-            result = {k: self._out_h[k][ofs:ofs + n].numpy().copy() for k in self.want}
-            if self.y_inverse is not None and np.isinf(result.get("model-output", 0.0)).any():
-                result["raw-model-output"] = self._out_h["raw-model-output"][ofs:ofs + n].numpy().copy()
-            item[-1].set_result(self._with_smoothed(result, item, smoothed, ofs, n))
-            ofs += n
+        self._reply(batch, self._out_h, jobs["out_row"].tolist(), jobs["n_rows"].tolist(), smoothed)
 
 
 class LSTMAnomalyCoalescer(AnomalyCoalescer):
@@ -277,13 +284,8 @@ class LSTMAnomalyCoalescer(AnomalyCoalescer):
     def __init__(self, eng: "engine.LSTMEngine", params, scale, feat_thr=None, agg_thr=None, max_batch_tiles: int = 1024,
                  max_wait_ms: float = 1.0, smoothing=None, y_inverse=None):
         torch = engine._torch()
-        self.eng, self.params, self.scale, self.feat_thr, self.agg_thr = eng, params, scale, feat_thr, agg_thr
-        self.y_inverse = tuple(y_inverse) if y_inverse is not None else None
-        self.max_cost, self.max_wait = int(max_batch_tiles), float(max_wait_ms) * 1e-3
-        self.want = tuple(k for k in PER_TAG + PER_ROW if not ((feat_thr is None and k == "anomaly-confidence")
-                                                                or (agg_thr is None and k == "total-anomaly-confidence")))
-        self.smoothing = self._check_smoothing(smoothing)
-        self._stream = torch.cuda.Stream(device=eng.device)
+        self.max_cost = int(max_batch_tiles)
+        self._setup(eng, params, scale, feat_thr, agg_thr, max_wait_ms, None, smoothing, y_inverse)
         # staged per batch in one copy: the infer jobs, the score jobs, the gather job, the smoothing jobs, tile_base and the
         # distinct slots
         jb = engine._cabi.JOB_DTYPE.itemsize
@@ -368,9 +370,4 @@ class LSTMAnomalyCoalescer(AnomalyCoalescer):
         self._stream.synchronize()
         self.batches += 1
         self.requests += k
-        raw = host.pop("raw-model-output", None)
-        for i, item in enumerate(batch):
-            result = {key: v[w_ofs[i]:w_ofs[i + 1]].numpy().copy() for key, v in host.items()}
-            if raw is not None and np.isinf(result["model-output"]).any():
-                result["raw-model-output"] = raw[w_ofs[i]:w_ofs[i + 1]].numpy().copy()
-            item[-1].set_result(self._with_smoothed(result, item, smoothed, int(w_ofs[i]), int(windows[i])))
+        self._reply(batch, host, w_ofs[:-1].tolist(), windows.tolist(), smoothed)
