@@ -12,6 +12,7 @@ number a `gordo build` user sees.
     python benchmarks/bench_fleet_builder.py --kfcv --machines 125 --rows 10000 --tags 64 --epochs 20 --single 1
     python benchmarks/bench_fleet_builder.py --ragged 5000:15000 --machines 125 --tags 64 --epochs 10 --single 1 [--kfcv | --lstm | --example-config]
     python benchmarks/bench_fleet_builder.py --ttr --scaled --machines 125 --rows 10000 --tags 64 --epochs 10 --single 1 [--lstm]
+    python benchmarks/bench_fleet_builder.py --tags 8:96 --machines 125 --rows 10000 --epochs 10 --runs 3 --single 0 [--kfcv]
 
 ``--lstm`` builds DiffBasedAnomalyDetector(KerasLSTMAutoEncoder(lstm_hourglass)) machines instead (batched by
 fleet.build_lstm_fleet).  ``--example-config`` builds the model of gordo's examples/model-configuration.yaml:
@@ -30,6 +31,10 @@ fleet.build_kfold_fleet makes after the fold scoring, on arrays of the bucket's 
 FleetModelBuilder(ragged=True) and with the default, alternating, ``--runs`` times each: wall time, the number of buckets and of
 fit launches, and the device time of the fit launches (CUDA events around each, summed per build).  Without the flag every
 length is its own bucket.
+``--tags LO:HI`` draws every machine's tag count uniformly from [LO, HI] (seeded) and builds the project with
+FleetModelBuilder(mixed_widths=True) and with the default, alternating, ``--runs`` times each, reporting as ``--ragged`` does
+(grouped fit launches counted and timed as one launch each).  Without the flag every tag count is its own bucket and its own fit
+launch; with it, the buckets whose nets share a memory plan train in one gb_ffae_fit_group launch.
 ``--window W`` gives the plain detectors a smoothing window W (smm) and builds them with FleetModelBuilder(smoothing=True), whose
 fold thresholds at 6 rows and at W come from one gb_thresholds_pair launch.
 ``--ttr`` wraps the plain detector's estimator (feed-forward, ``--scaled`` or ``--lstm``) in TransformedTargetRegressor(transformer=
@@ -56,7 +61,8 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--machines", type=int, default=125)
     ap.add_argument("--rows", type=int, default=10000)
-    ap.add_argument("--tags", type=int, default=64)
+    ap.add_argument("--tags", default="64", metavar="T|LO:HI", help="tags per machine, or LO:HI: per-machine tag counts drawn uniformly "
+                    "from [LO, HI]; FleetModelBuilder(mixed_widths=True) against the default")
     ap.add_argument("--epochs", type=int, default=10)
     ap.add_argument("--scaled", action="store_true", help="Pipeline([MinMaxScaler, AE]) as in gordo's example config")
     ap.add_argument("--single", type=int, default=3, help="machines to also build one at a time for comparison")
@@ -68,7 +74,7 @@ def main():
     ap.add_argument("--min-delta", type=float, default=0.0, help="--early-stopping: the callback's min_delta (the reference's definition has none)")
     ap.add_argument("--kfcv", action="store_true", help="the reference's production definition: a K-fold detector under KFold(5, shuffle, random_state=0)")
     ap.add_argument("--ragged", default=None, metavar="LO:HI", help="per-machine lengths drawn uniformly from [LO, HI]; ragged=True against the default")
-    ap.add_argument("--runs", type=int, default=2, help="--ragged: builds of each kind, alternating")
+    ap.add_argument("--runs", type=int, default=2, help="--ragged / --tags LO:HI: builds of each kind, alternating")
     ap.add_argument("--window", type=int, default=None, help="plain detectors with this smoothing window (smm), batched by FleetModelBuilder(smoothing=True)")
     ap.add_argument("--ttr", action="store_true", help="the plain detector's estimator inside TransformedTargetRegressor(MinMaxScaler), "
                                                         "batched by FleetModelBuilder(target_scaler=True)")
@@ -118,6 +124,8 @@ def main():
             "transformer": "sklearn.preprocessing.MinMaxScaler", "regressor": detector["base_estimator"]}}
         flags["target_scaler"] = True
     rng = np.random.default_rng(0)
+    lo, _, hi = a.tags.partition(":")
+    tag_counts = np.random.default_rng(2).integers(int(lo), int(hi) + 1, size=a.machines) if hi else np.full(a.machines, int(lo))
     if a.ragged:
         lo, hi = (int(v) for v in a.ragged.split(":"))
         lengths = np.random.default_rng(1).integers(lo, hi + 1, size=a.machines)
@@ -125,14 +133,19 @@ def main():
         lengths = np.full(a.machines, a.rows)
     machines = []
     for m in range(a.machines):
-        rows = int(lengths[m])
+        rows, tags = int(lengths[m]), int(tag_counts[m])
         idx = pd.date_range("2019-01-01", periods=rows, freq="10min", tz="UTC")
         t = np.linspace(0, 60 * rows / a.rows, rows)[:, None]
-        values = 0.5 + 0.4 * np.sin(t * rng.uniform(0.5, 2, a.tags) + rng.uniform(0, 6, a.tags)) + rng.normal(0, 0.02, (rows, a.tags))
-        frame = pd.DataFrame(values.astype(np.float32), index=idx, columns=[f"tag-{i}" for i in range(a.tags)])
+        values = 0.5 + 0.4 * np.sin(t * rng.uniform(0.5, 2, tags) + rng.uniform(0, 6, tags)) + rng.normal(0, 0.02, (rows, tags))
+        frame = pd.DataFrame(values.astype(np.float32), index=idx, columns=[f"tag-{i}" for i in range(tags)])
         machines.append({"name": f"machine-{m}", "model": model, "dataset": {"X": frame, "y": frame}, "evaluation": evaluation})
+    if hi:
+        if a.ragged:
+            flags["ragged"] = True
+        print(json.dumps(_alternating_builds(a, machines, flags, n_splits, lengths, "mixed_widths", tag_counts)))
+        return
     if a.ragged:
-        print(json.dumps(_ragged_builds(a, machines, flags, n_splits, lengths)))
+        print(json.dumps(_alternating_builds(a, machines, flags, n_splits, lengths, "ragged")))
         return
 
     builder.FleetModelBuilder(machines[:2], **flags).build()  # warm-up: library load, first launches
@@ -180,11 +193,12 @@ def main():
     print(json.dumps(out))
 
 
-def _ragged_builds(a, machines, flags, n_splits, lengths):
+def _alternating_builds(a, machines, flags, n_splits, lengths, option, tag_counts=None):
     """
-    The project built with FleetModelBuilder(ragged=True) and with the default, alternating: wall time of each build (host work and
-    the written files included), buckets, and the fit launches' device time (CUDA events around every fit launch of the build,
-    read after the build's final synchronise).  One warm-up of each kind first.
+    The project built with FleetModelBuilder(**{option: True}) (``ragged`` or ``mixed_widths``) and with the default, alternating:
+    wall time of each build (host work and the written files included), buckets, and the fit launches' device time (CUDA events
+    around every fit launch of the build, per-net and grouped, read after the build's final synchronise).  One warm-up of each kind
+    first.
     """
     import numpy as np
     import torch
@@ -203,31 +217,34 @@ def _ragged_builds(a, machines, flags, n_splits, lengths):
             return res
         return run
 
-    def counted(fn):
+    def counted(fn, joined=False):
         def run(members):
-            buckets.append(len(members))
+            buckets.extend(members if joined else [members])
             return fn(members)
         return run
 
     engine.FFEngine._fit_launch = timed(engine.FFEngine._fit_launch)
     engine.LSTMEngine._fit_launch = timed(engine.LSTMEngine._fit_launch)
+    engine.fit_group = timed(engine.fit_group)
     builder.FleetModelBuilder._build_bucket = staticmethod(counted(builder.FleetModelBuilder._build_bucket))
+    builder.FleetModelBuilder._build_buckets_joined = staticmethod(counted(builder.FleetModelBuilder._build_buckets_joined, joined=True))
 
-    def build(ragged, project):
+    def build(flagged, project):
         launches.clear()
         buckets.clear()
         with tempfile.TemporaryDirectory() as out:
             t0 = time.perf_counter()
-            builder.FleetModelBuilder(project, ragged=ragged, **flags).build(out)
+            builder.FleetModelBuilder(project, **{option: flagged}, **flags).build(out)
             torch.cuda.synchronize()
             wall = time.perf_counter() - t0
         return {"wall_s": wall, "buckets": len(buckets), "fit_launches": len(launches),
                 "fit_launch_ms": sum(e[0].elapsed_time(e[1]) for e in launches)}
 
+    name = "ragged" if option == "ragged" else "mixed"
     build(True, machines[:2]), build(False, machines[:2])  # warm-up
-    runs = {"ragged": [], "default": []}
+    runs = {name: [], "default": []}
     for _ in range(a.runs):
-        runs["ragged"].append(build(True, machines))
+        runs[name].append(build(True, machines))
         runs["default"].append(build(False, machines))
     single_s = None
     if a.single:
@@ -237,13 +254,15 @@ def _ragged_builds(a, machines, flags, n_splits, lengths):
         torch.cuda.synchronize()
         single_s = (time.perf_counter() - t0) / a.single
     kind = "K-fold detector (--kfcv)" if a.kfcv else ("LSTM hourglass" if a.lstm else ("example-config hourglass" if a.example_config else "hourglass"))
+    tags = f"{a.tags}-tag" if tag_counts is None else f"[{a.tags}]-tag (uniform, seed 2; {len(set(tag_counts.tolist()))} distinct)"
+    rows = f"lengths uniform in [{a.ragged}] (seed 1; total {int(lengths.sum())} rows)" if a.ragged else f"{a.rows} rows"
     out = {"gpu": torch.cuda.get_device_name(0), "power_limit_w": _power_limit(),
-           "workload": f"{a.machines} machines x {a.tags}-tag {kind}, lengths uniform in [{a.ragged}] (seed 1; total {int(lengths.sum())} rows), "
-                       f"{a.epochs} epochs, {n_splits}-fold CV, written to disk",
+           "workload": f"{a.machines} machines x {tags} {kind}, {rows}, {a.epochs} epochs, {n_splits}-fold CV, written to disk",
            "model_builder_s_per_machine": single_s}
     for kind, rs in runs.items():
         out[kind] = {key: [r[key] for r in rs] for key in rs[0]}
-    out["wall_speedup_median"] = float(np.median(out["default"]["wall_s"]) / np.median(out["ragged"]["wall_s"]))
+    out["wall_speedup_median"] = float(np.median(out["default"]["wall_s"]) / np.median(out[name]["wall_s"]))
+    out["fit_launch_speedup_median"] = float(np.median(out["default"]["fit_launch_ms"]) / np.median(out[name]["fit_launch_ms"]))
     return out
 
 
@@ -260,7 +279,7 @@ def _kfold_threshold_stage(a, runs: int = 5):
     from gordo_components_b200 import engine, fleet
 
     dev = engine.cuda_device()
-    M, N, T = a.machines, a.rows, a.tags
+    M, N, T = a.machines, a.rows, int(a.tags)
     tests, _, _, inverse = fleet.kfold_layout(KFold(5, shuffle=True, random_state=0), N)
     K = len(tests)
     n_test = np.asarray([len(t) for t in tests])
@@ -324,7 +343,7 @@ def _stop_launches(a, machines, stopping):
             self.ms = ev[0].elapsed_time(ev[1])
             return res
 
-    spec = feedforward_hourglass(n_features=a.tags, compression_factor=0.6, encoding_layers=1, func="tanh", out_func="linear")
+    spec = feedforward_hourglass(n_features=int(a.tags), compression_factor=0.6, encoding_layers=1, func="tanh", out_func="linear")
     eng = TimedEngine(engine.ff_engine_for(spec))
     x = engine.to_device_f32(np.concatenate([m["dataset"]["X"].values for m in machines]), eng.device)
     never = dict(stopping, patience=a.epochs)

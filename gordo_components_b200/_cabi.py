@@ -96,7 +96,7 @@ def make_dense_dropout(rate=None) -> GbDenseDropout:
 
 EXPORTS = (
     "gb_abi_version", "gb_last_error", "gb_device_check", "gb_ffnet_param_count", "gb_ffnet_param_stride",
-    "gb_ffae_infer_score", "gb_ffae_tc_supported", "gb_ffae_infer_plan", "gb_ffae_infer_score_x64", "gb_ffae_infer_plan_x64", "gb_anomaly_score", "gb_anomaly_score_f64", "gb_minmax_fit", "gb_minmax_f64", "gb_thresholds", "gb_thresholds_f64", "gb_thresholds_pair", "gb_thresholds_pair_f64", "gb_cv_moments", "gb_smooth", "gb_smooth_scores", "gb_quantile", "gb_affine_f64", "gb_gather_rows", "gb_gather_rows_ragged", "gb_minmax_inverse_f32", "gb_minmax_inverse_score_f64", "gb_ffae_fit_state_stride", "gb_ffae_fit", "gb_ffae_fit_split", "gb_ffae_fit_stop", "gb_ffae_fit_plan", "gb_ffae_fit_opt", "gb_ffae_fit_reg", "gb_ffae_fit_drop",
+    "gb_ffae_infer_score", "gb_ffae_tc_supported", "gb_ffae_infer_plan", "gb_ffae_infer_score_x64", "gb_ffae_infer_plan_x64", "gb_anomaly_score", "gb_anomaly_score_f64", "gb_minmax_fit", "gb_minmax_f64", "gb_thresholds", "gb_thresholds_f64", "gb_thresholds_pair", "gb_thresholds_pair_f64", "gb_cv_moments", "gb_smooth", "gb_smooth_scores", "gb_quantile", "gb_affine_f64", "gb_gather_rows", "gb_gather_rows_ragged", "gb_minmax_inverse_f32", "gb_minmax_inverse_score_f64", "gb_ffae_fit_state_stride", "gb_ffae_fit", "gb_ffae_fit_split", "gb_ffae_fit_stop", "gb_ffae_fit_plan", "gb_ffae_fit_opt", "gb_ffae_fit_reg", "gb_ffae_fit_drop", "gb_ffae_fit_group", "gb_ffae_fit_group_workspace_bytes",
     "gb_lstm_param_count", "gb_lstm_param_stride", "gb_lstm_workspace_bytes", "gb_lstm_infer", "gb_lstm_tc_supported", "gb_lstm_tc_workspace_bytes", "gb_lstm_infer_tc", "gb_lstm_tc_ragged_workspace_bytes", "gb_lstm_infer_tc_ragged", "gb_lstm_fit_workspace_bytes", "gb_lstm_fit", "gb_lstm_fit_loss", "gb_lstm_fit_tc_workspace_bytes", "gb_lstm_fit_tc", "gb_lstm_fit_opt", "gb_lstm_fit_tc_opt",
     "gb_lstm_fit_stop_state_bytes", "gb_lstm_fit_stop", "gb_lstm_fit_tc_stop",
     "gb_orthonormal_rows",
@@ -106,6 +106,11 @@ EXPORTS = (
 class GbFFNet(C.Structure):
     _fields_ = [("n_layers", C.c_int32), ("dims", C.c_int32 * (GB_MAX_LAYERS + 1)), ("act", C.c_int32 * GB_MAX_LAYERS),
                 ("l1", C.c_float * GB_MAX_LAYERS)]
+
+
+class GbFitGroup(C.Structure):
+    _fields_ = [("net", GbFFNet), ("params", C.c_void_p), ("adam_m", C.c_void_p), ("adam_v", C.c_void_p), ("best_params", C.c_void_p),
+                ("x", C.c_void_p), ("y", C.c_void_p)]
 
 
 class GbJob(C.Structure):
@@ -248,6 +253,12 @@ def _declare(lib):
     lib.gb_ffae_fit_reg.restype = C.c_int
     lib.gb_ffae_fit_drop.argtypes = lib.gb_ffae_fit_reg.argtypes[:-1] + [C.POINTER(GbDenseDropout), _P]
     lib.gb_ffae_fit_drop.restype = C.c_int
+    lib.gb_ffae_fit_group.argtypes = [C.POINTER(GbFitGroup), C.c_int32, C.POINTER(C.c_int32), _P, _P, C.c_int32, C.c_int32, _P, _P,
+                                      C.POINTER(GbFitHParams), C.c_int32] + [_P] * 7 + [C.POINTER(GbOptimizer), C.POINTER(GbDenseReg),
+                                                                                       C.POINTER(GbDenseDropout), _P, _P]
+    lib.gb_ffae_fit_group.restype = C.c_int
+    lib.gb_ffae_fit_group_workspace_bytes.argtypes = [C.c_int32, C.c_int32]
+    lib.gb_ffae_fit_group_workspace_bytes.restype = C.c_size_t
     for name in ("gb_lstm_fit_opt", "gb_lstm_fit_tc_opt"):
         getattr(lib, name).argtypes = lib.gb_lstm_fit_loss.argtypes[:-1] + [C.POINTER(GbOptimizer), _P]
         getattr(lib, name).restype = C.c_int

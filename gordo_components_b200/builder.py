@@ -766,11 +766,19 @@ class FleetModelBuilder:
     own scaled targets, and the fold models' predictions go through sklearn's float32 inverse and float64 scoring in one launch
     (``gb_minmax_inverse_score_f64``).  The target transformer is a bucket field.  Off by default for the same reason as ``kfcv``: without it such
     machines build through ``ModelBuilder`` as before.  K-fold detectors with a TransformedTargetRegressor are ``kfcv``'s.
+
+    ``mixed_widths``: build feed-forward buckets (plain and K-fold) whose keys differ only in the network's ``dims`` -- machines with
+    other tag counts -- together, when their nets share the fit's memory plan (``engine.fit_plan``): every bucket prepares its build,
+    their fits go out as one gb_ffae_fit_group launch (``fleet.build_joined``), and every bucket finishes on its own.  Buckets, their
+    initial weights and every machine's artefacts are those of the default build; only the fit launches are fewer.  If a joined
+    build raises, its buckets build one by one as without the flag.  LSTM buckets are untouched.  Off by default.
     """
 
     def __init__(self, machines: Sequence, early_stopping: bool = False, kfcv: bool = False, lstm_wide_batches: bool = False,
-                 lstm_early_stopping: bool = False, ragged: bool = False, smoothing: bool = False, target_scaler: bool = False):
+                 lstm_early_stopping: bool = False, ragged: bool = False, smoothing: bool = False, target_scaler: bool = False,
+                 mixed_widths: bool = False):
         self.ragged = bool(ragged)
+        self.mixed_widths = bool(mixed_widths)
         self.target_scaler = bool(target_scaler)
         self.smoothing = bool(smoothing)
         self.early_stopping = bool(early_stopping)
@@ -791,7 +799,7 @@ class FleetModelBuilder:
 
         return FleetModelBuilder([self.machines[i] for i in fleet.partition(len(self.machines), world)[rank]], early_stopping=self.early_stopping,
                                  kfcv=self.kfcv, lstm_wide_batches=self.lstm_wide_batches, lstm_early_stopping=self.lstm_early_stopping,
-                                 ragged=self.ragged, smoothing=self.smoothing, target_scaler=self.target_scaler)
+                                 ragged=self.ragged, smoothing=self.smoothing, target_scaler=self.target_scaler, mixed_widths=self.mixed_widths)
 
     def build(self, output_dir: Optional[str] = None) -> List[Tuple[Any, dict]]:
         results: List[Optional[Tuple[Any, dict]]] = [None] * len(self.machines)
@@ -808,14 +816,24 @@ class FleetModelBuilder:
                 results[i] = ModelBuilder(machine).build()
             else:
                 buckets.setdefault(c.bucket(self.ragged), []).append(c)
-        for members in buckets.values():
-            try:
-                built_bucket = self._build_bucket(members)
-            except Exception as exc:  # e.g. an architecture the batched fit kernel cannot hold: the machines still get built, one by one
-                logger.warning("batched build of %d machines failed (%s: %s); building them one at a time", len(members), type(exc).__name__, exc)
-                built_bucket = [ModelBuilder(c.machine).build() for c in members]
-            for c, built in zip(members, built_bucket):
-                results[c.index] = built
+        for joined in (launch_groups(buckets) if self.mixed_widths else [[members] for members in buckets.values()]):
+            built_buckets = None
+            if len(joined) > 1:
+                try:
+                    built_buckets = self._build_buckets_joined(joined)
+                except Exception as exc:  # the buckets still get built, each on its own
+                    logger.warning("joined build of %d buckets failed (%s: %s); building them one by one", len(joined), type(exc).__name__, exc)
+            for i, members in enumerate(joined):
+                if built_buckets is not None:
+                    built_bucket = built_buckets[i]
+                else:
+                    try:
+                        built_bucket = self._build_bucket(members)
+                    except Exception as exc:  # e.g. an architecture the batched fit kernel cannot hold: the machines still get built, one by one
+                        logger.warning("batched build of %d machines failed (%s: %s); building them one at a time", len(members), type(exc).__name__, exc)
+                        built_bucket = [ModelBuilder(c.machine).build() for c in members]
+                for c, built in zip(members, built_bucket):
+                    results[c.index] = built
         if output_dir is not None:
             for model, machine in results:
                 serializer.dump(model, os.path.join(output_dir, machine["name"]), metadata=machine)
@@ -825,21 +843,18 @@ class FleetModelBuilder:
     def _build_bucket(members: List[_Canonical]) -> List[Tuple[Any, dict]]:
         if isinstance(members[0], _CanonicalLSTM):
             return FleetModelBuilder._build_lstm_bucket(members)
-        if isinstance(members[0], _CanonicalKFold):
-            return FleetModelBuilder._build_kfold_bucket(members)
-        from . import engine, fleet
+        from . import fleet
 
-        first = members[0]
-        eng = engine.ff_engine_for(first.spec)
-        t0 = time.time()
-        xd, yd = _upload(members, eng.device, float64=first.target_scaler)  # TransformedTargetRegressor.fit hands its transformer float64 targets
-        fb = fleet.build_fleet(eng, xd, yd, [len(c.X) for c in members], epochs=first.fit["epochs"], batch_size=first.fit["batch_size"],
-                               n_splits=first.n_splits, seed=int(first.evaluation.get("seed", 0)), adam=first.spec.adam, shuffle=first.fit["shuffle"],
-                               input_scaler=first.input_scaler, detector_shuffle=first.split[0], validation_split=first.split[1],
-                               validation_batch_size=first.split[2], early_stopping=_stops(members), loss=first.spec.loss,
-                               optimizer=fit_optimizer(first.spec), reg=fit_reg(first.spec), window=first.window, dropout=fit_dropout(first.spec),
-                               target_scaler=first.target_scaler)
-        return _assemble(members, fb, fb.cv_moments.cpu().numpy(), fb.n_test, 0, TimeSeriesSplit(n_splits=first.n_splits), t0)  # a Dense stack answers every row
+        return fleet.build_joined([_ff_bucket_steps(members)])[0]
+
+    @staticmethod
+    def _build_buckets_joined(joined: List[List[_Canonical]]) -> List[List[Tuple[Any, dict]]]:
+        """Feed-forward buckets of one launch group (``launch_groups``), their fits in one launch (``fleet.build_joined``)."""
+        from . import fleet
+
+        out = fleet.build_joined([_ff_bucket_steps(members) for members in joined])
+        logger.info("built %d buckets of %d machines with their fits in one launch", len(joined), sum(len(m) for m in joined))
+        return out
 
     @staticmethod
     def _build_lstm_bucket(members: List[_CanonicalLSTM]) -> List[Tuple[Any, dict]]:
@@ -858,25 +873,53 @@ class FleetModelBuilder:
         logger.info("built %d LSTM machines in one batched bucket", len(members))
         return out
 
-    @staticmethod
-    def _build_kfold_bucket(members: List[_CanonicalKFold]) -> List[Tuple[Any, dict]]:
-        from . import engine, fleet
 
-        first = members[0]
-        eng = engine.ff_engine_for(first.spec)
-        t0 = time.time()
+def _ff_bucket_steps(members: List[_Canonical]):
+    """The batched build of a feed-forward bucket (plain or K-fold) as ``fleet.build_joined`` takes it: a generator that yields the
+    bucket's fit request, receives the fit's result and returns the machines as ``ModelBuilder`` returns them."""
+    from . import engine, fleet
+
+    first = members[0]
+    eng = engine.ff_engine_for(first.spec)
+    t0 = time.time()
+    if isinstance(first, _CanonicalKFold):
         xd, yd = _upload(members, eng.device, float64=True)
         det = first.model
-        fb = fleet.build_kfold_fleet(eng, xd, yd, [len(c.X) for c in members], first.cv, epochs=first.fit["epochs"], batch_size=first.fit["batch_size"],
-                                     seed=int(first.evaluation.get("seed", 0)), adam=first.spec.adam, shuffle=first.fit["shuffle"],
-                                     input_scaler=first.input_scaler, target_scaler=first.target_scaler, detector_shuffle=first.split[0],
-                                     validation_split=first.split[1], validation_batch_size=first.split[2], early_stopping=_stops(members),
-                                     window=det.window, smoothing_method=det.smoothing_method, threshold_percentile=det.threshold_percentile,
-                                     loss=first.spec.loss, optimizer=fit_optimizer(first.spec), reg=fit_reg(first.spec),
-                                     dropout=fit_dropout(first.spec))
+        fb = yield from fleet.build_kfold_fleet.steps(
+            eng, xd, yd, [len(c.X) for c in members], first.cv, epochs=first.fit["epochs"], batch_size=first.fit["batch_size"],
+            seed=int(first.evaluation.get("seed", 0)), adam=first.spec.adam, shuffle=first.fit["shuffle"], input_scaler=first.input_scaler,
+            target_scaler=first.target_scaler, detector_shuffle=first.split[0], validation_split=first.split[1],
+            validation_batch_size=first.split[2], early_stopping=_stops(members), window=det.window, smoothing_method=det.smoothing_method,
+            threshold_percentile=det.threshold_percentile, loss=first.spec.loss, optimizer=fit_optimizer(first.spec), reg=fit_reg(first.spec),
+            dropout=fit_dropout(first.spec))
         out = _assemble(members, fb, fb.cv_moments, fb.n_test, 0, first.cv, t0)  # a Dense stack answers every row
         logger.info("built %d K-fold machines in one batched bucket", len(members))
         return out
+    xd, yd = _upload(members, eng.device, float64=first.target_scaler)  # TransformedTargetRegressor.fit hands its transformer float64 targets
+    fb = yield from fleet.build_fleet.steps(
+        eng, xd, yd, [len(c.X) for c in members], epochs=first.fit["epochs"], batch_size=first.fit["batch_size"], n_splits=first.n_splits,
+        seed=int(first.evaluation.get("seed", 0)), adam=first.spec.adam, shuffle=first.fit["shuffle"], input_scaler=first.input_scaler,
+        detector_shuffle=first.split[0], validation_split=first.split[1], validation_batch_size=first.split[2], early_stopping=_stops(members),
+        loss=first.spec.loss, optimizer=fit_optimizer(first.spec), reg=fit_reg(first.spec), window=first.window,
+        dropout=fit_dropout(first.spec), target_scaler=first.target_scaler)
+    return _assemble(members, fb, fb.cv_moments.cpu().numpy(), fb.n_test, 0, TimeSeriesSplit(n_splits=first.n_splits), t0)  # a Dense stack answers every row
+
+
+def launch_groups(buckets: Dict[tuple, List[_Canonical]]) -> List[List[List[_Canonical]]]:
+    """
+    ``FleetModelBuilder(mixed_widths=True)``'s launch groups: the buckets (in key order of first appearance) whose keys differ only
+    in the network's ``dims`` and whose nets share the fit's memory plan, as lists of buckets; LSTM buckets, and buckets whose plan
+    the fit refuses, stay alone.
+    """
+    from . import engine
+
+    groups: Dict[tuple, List[List[_Canonical]]] = {}
+    for key, members in buckets.items():
+        c = members[0]
+        plan = None if isinstance(c, _CanonicalLSTM) else engine.fit_plan(c.spec.dims, c.spec.acts, c.spec.l1)
+        join = ("alone", key) if plan is None else (type(c).__name__, key[1:], plan)
+        groups.setdefault(join, []).append(members)
+    return list(groups.values())
 
 
 def _upload(members: List[_Canonical], device, float64: bool):

@@ -17,7 +17,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB = os.path.join(HERE, "libgordo_b200.so")
 OBJ = os.path.join(HERE, "build")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
-SOURCES = ["gb_api.cu", "ffae_infer_fma.cu", "ffae_infer_small.cu", "ffae_infer_tc.cu", "anomaly_reduce.cu", "threshold_pair.cu", "smooth.cu", "gather.cu", "ffae_fit.cu", "ffae_fit_drop.cu", "lstm_infer.cu", "lstm_infer_tc.cu", "lstm_fit.cu", "lstm_fit_tc.cu"]
+SOURCES = ["gb_api.cu", "ffae_infer_fma.cu", "ffae_infer_small.cu", "ffae_infer_tc.cu", "anomaly_reduce.cu", "threshold_pair.cu", "smooth.cu", "gather.cu", "ffae_fit.cu", "ffae_fit_drop.cu", "ffae_fit_group.cu", "lstm_infer.cu", "lstm_infer_tc.cu", "lstm_fit.cu", "lstm_fit_tc.cu"]
 HEADERS = ["gb_common.cuh", "ffae_fit_body.cuh", "ffae_fit_kernels.cuh", "gb_sm90.cuh", "lstm_fit_common.cuh", "postprocess.cuh", os.path.join("..", "..", "include", "gordo_b200.h")]
 NVCC_FLAGS = [
     *ARCH, "-O3", "-lineinfo", "-std=c++17",

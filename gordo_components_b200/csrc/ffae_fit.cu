@@ -85,72 +85,24 @@ int plan_fit(const gb_ffnet* net, FitArgs& a, bool& w_global, size_t& smem) {
   return GB_OK;
 }
 
+
 // gb_ffae_fit (FIT_PLAIN: the kernels without the held-out pass), gb_ffae_fit_split and gb_ffae_fit_stop
 int launch_fit(const gb_ffnet* net, float* params, float* adam_m, float* adam_v, const gb_job* jobs, const gb_fit_split* split,
                int32_t n_jobs, int32_t max_rows, const float* x, const float* y, const int32_t* row_map, const int32_t* perm,
                const gb_fit_hparams* hp, int32_t val_batch, float* out_loss, float* out_acc, float* out_val_loss, float* out_val_acc,
                const gb_fit_stop* stop, float* best_params, int32_t* out_epochs, int32_t* out_best_epoch, FitEntry entry,
                const gb_optimizer* opt, const gb_dense_reg* reg, const gb_dense_dropout* drop, void* stream) {
-  int rc = gb::validate_ffnet(net);
+  int rc = gb_fit::check_fit(net, params, adam_m, adam_v, jobs, x, y, perm, hp, out_loss, opt);
   if (rc != GB_OK) return rc;
-  rc = gb::validate_optimizer(opt);
-  if (rc != GB_OK) return rc;
-  GB_REQUIRE(params && adam_m && adam_v && jobs && x && y && hp && out_loss, GB_E_ARG,
-             "params/adam_m/adam_v/jobs/x/y/hp/out_loss must be non-NULL");
-  GB_REQUIRE(hp->epochs >= 1, GB_E_ARG, "epochs=%d must be >= 1", hp->epochs);
-  GB_REQUIRE(hp->batch_size >= 1, GB_E_ARG, "batch_size=%d must be >= 1", hp->batch_size);
-  GB_REQUIRE(hp->shuffle >= 0 && hp->shuffle <= 2, GB_E_ARG, "shuffle=%d unknown", hp->shuffle);
-  GB_REQUIRE(hp->shuffle != 2 || perm, GB_E_ARG, "shuffle=2 needs perm");
-  GB_REQUIRE(hp->loss >= GB_LOSS_MSE && hp->loss <= GB_LOSS_LOG_COSH, GB_E_ARG, "loss=%d unknown (gb_loss: 0..5)", hp->loss);
-  GB_REQUIRE(gb::aligned16(params) && gb::aligned16(adam_m) && gb::aligned16(adam_v) && gb::aligned16(x) &&
-                 gb::aligned16(y),
-             GB_E_ALIGN, "params/adam/x/y must be 16-byte aligned");
   if (n_jobs == 0 || max_rows == 0) return GB_OK;
 
   FitArgs a{};
   size_t smem = 0;
   bool w_global = false;
-  rc = plan_fit(net, a, w_global, smem);
+  rc = gb_fit::setup_fit(net, params, adam_m, adam_v, jobs, split, max_rows, x, y, row_map, perm, hp, val_batch, out_loss, out_acc,
+                         out_val_loss, out_val_acc, stop, best_params, out_epochs, out_best_epoch, opt, reg, drop, a, w_global, smem);
   if (rc != GB_OK) return rc;
-  a.hp = *hp;
-  const bool use_opt = !gb::plain_adam(opt);
-  if (opt != nullptr && !use_opt) {  // plain Adam runs the Adam kernels, from the optimizer's hyperparameters
-    a.hp.lr = opt->lr; a.hp.beta1 = opt->beta1; a.hp.beta2 = opt->beta2; a.hp.eps = opt->eps;
-  }
-  if (use_opt) a.opt = *opt;
-  if (reg != nullptr || drop != nullptr) {  // the REG and DROP kernels are OPT kernels: plain Adam, too, runs through gb::opt_update there
-    if (reg != nullptr) a.reg = *reg;  // else zeros: the DROP kernels add a penalty of 0
-    if (opt != nullptr) {
-      a.opt = *opt;
-    } else {
-      a.opt = gb_optimizer{};
-      a.opt.kind = GB_OPT_ADAM; a.opt.lr = hp->lr; a.opt.beta1 = hp->beta1; a.opt.beta2 = hp->beta2; a.opt.eps = hp->eps;
-    }
-  }
-  if (drop != nullptr) {
-    for (int l = 0; l < GB_MAX_LAYERS; ++l) {
-      if (drop->rate[l] == 0.f) continue;
-      const double r = (double)drop->rate[l];
-      a.drop_layers |= 1u << l;
-      a.drop_thr[l] = (uint32_t)floor(r * 4294967296.0);
-      a.drop_scale[l] = (float)(1.0 / (1.0 - r));
-    }
-  }
-  const int L = net->n_layers;
-  a.max_rows = max_rows;
-  a.pstride = (long)gb_ffnet_param_stride(net);
-  a.sstride = (long)gb_ffae_fit_state_stride(net);
-  a.gather_layer = 0;
-  for (int l = 1; l < L; ++l)
-    if (a.im.np[l] <= a.im.np[a.gather_layer]) a.gather_layer = l;  // the last of the narrowest layers
-  a.gather_layer2 = a.gather_layer;
-  for (int l = 0, best = 1 << 30; l < L; ++l)
-    if (l != a.gather_layer && a.im.np[l] < best) { best = a.im.np[l]; a.gather_layer2 = l; }  // the narrowest of the others
-  a.params = params; a.adam_m = adam_m; a.adam_v = adam_v; a.jobs = jobs; a.x = x; a.y = y; a.perm = perm;
-  a.out_loss = out_loss; a.out_acc = out_acc;
   a.trace = g_fit_trace;
-  a.split = split; a.row_map = row_map; a.val_batch = val_batch; a.out_val_loss = out_val_loss; a.out_val_acc = out_val_acc;
-  a.stop = stop; a.best_params = best_params; a.out_epochs = out_epochs; a.out_best_epoch = out_best_epoch;
   auto launch = [&](auto kernel) -> int {
     GB_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     kernel<<<n_jobs, THREADS, smem, (cudaStream_t)stream>>>(a);
@@ -176,10 +128,13 @@ int launch_fit(const gb_ffnet* net, float* params, float* adam_m, float* adam_v,
   // weight regularizers take the 9 ffae_fit_reg_kernel instantiations, dropout the 9 ffae_fit_drop_kernel ones (ffae_fit_drop.cu)
   const std::false_type no{};
   const std::true_type yes{};
-  if (drop != nullptr) rc = gb_fit::launch_drop(a, entry, w_global, smem, n_jobs, (cudaStream_t)stream);
-  else if (reg != nullptr) rc = dispatch(yes, yes, yes);
-  else if (use_opt) rc = dispatch(yes, yes, no);
-  else rc = hp->loss == GB_LOSS_MSE ? dispatch(no, no, no) : dispatch(yes, no, no);
+  switch (gb_fit::fit_family(hp, opt, reg, drop)) {
+    case gb_fit::FAMILY_DROP: rc = gb_fit::launch_drop(a, entry, w_global, smem, n_jobs, (cudaStream_t)stream); break;
+    case gb_fit::FAMILY_REG: rc = dispatch(yes, yes, yes); break;
+    case gb_fit::FAMILY_OPT: rc = dispatch(yes, yes, no); break;
+    case gb_fit::FAMILY_MSE: rc = dispatch(no, no, no); break;
+    default: rc = dispatch(yes, no, no);
+  }
   if (rc != GB_OK) return rc;
   GB_CUDA_CHECK(cudaGetLastError());
   return GB_OK;
@@ -255,33 +210,9 @@ int gb_ffae_fit_drop(const gb_ffnet* net, float* params, float* adam_m, float* a
   GB_REQUIRE(!stop || (best_params && out_epochs && out_best_epoch), GB_E_ARG,
              "stop needs best_params, out_epochs and out_best_epoch");
   GB_REQUIRE(!stop || gb::aligned16(best_params), GB_E_ARG, "best_params must be 16-byte aligned");
-  bool any = false;  // a record of zeros is no record: the kernels of gb_ffae_fit_opt
-  if (reg != nullptr) {
-    const int rc = gb::validate_ffnet(net);
-    if (rc != GB_OK) return rc;
-    auto ok = [](float v) { return v >= 0.f && v < 3.0e38f; };  // false for NaN and inf
-    const struct { const char* name; const float* c; } fields[] = {
-        {"kernel_l1", reg->kernel_l1}, {"kernel_l2", reg->kernel_l2}, {"bias_l1", reg->bias_l1}, {"bias_l2", reg->bias_l2}};
-    for (const auto& f : fields)
-      for (int l = 0; l < net->n_layers; ++l) {
-        GB_REQUIRE(ok(f.c[l]), GB_E_ARG, "reg %s[%d]=%g must be finite and >= 0", f.name, l, (double)f.c[l]);
-        any = any || f.c[l] != 0.f;
-      }
-  }
-  bool any_drop = false;  // likewise: all-zero rates run the kernels of gb_ffae_fit_reg
-  if (drop != nullptr) {
-    const int rc = gb::validate_ffnet(net);
-    if (rc != GB_OK) return rc;
-    for (int l = 0; l < GB_MAX_LAYERS; ++l) {
-      const float r = drop->rate[l];
-      GB_REQUIRE(r >= 0.f && r < 1.f, GB_E_ARG, "dropout rate[%d]=%g must be finite, >= 0 and < 1", l, (double)r);  // false for NaN
-      GB_REQUIRE(r == 0.f || l < net->n_layers, GB_E_ARG, "dropout rate[%d]=%g: the net has %d layers (rate[l] is on the input of layer l)",
-                 l, (double)r, net->n_layers);
-      GB_REQUIRE(r == 0.f || l == 0 || net->l1[l - 1] == 0.f, GB_E_ARG,
-                 "dropout rate[%d]=%g on the output of layer %d, which has an activity L1: not supported", l, (double)r, l - 1);
-      any_drop = any_drop || r != 0.f;
-    }
-  }
+  bool any = false, any_drop = false;
+  const int rc = gb_fit::check_reg_drop(net, reg, drop, any, any_drop);
+  if (rc != GB_OK) return rc;
   const FitEntry entry = stop ? FIT_STOP : split ? FIT_SPLIT : FIT_PLAIN;
   return launch_fit(net, params, adam_m, adam_v, jobs, split, n_jobs, max_rows, x, y, row_map, perm, hp, split ? val_batch : 1,
                     out_loss, out_acc, out_val_loss, out_val_acc, stop, best_params, out_epochs, out_best_epoch, entry, opt,
@@ -308,3 +239,131 @@ int gb_ffae_fit_opt(const gb_ffnet* net, float* params, float* adam_m, float* ad
 }
 
 }  // extern "C"
+
+// defined after the entry points: the tag nvcc gives this file's anonymous namespace follows its first external definition, and
+// the kernels' names carry that tag
+namespace gb_fit {
+
+int check_fit(const gb_ffnet* net, float* params, float* adam_m, float* adam_v, const gb_job* jobs, const float* x, const float* y,
+              const int32_t* perm, const gb_fit_hparams* hp, float* out_loss, const gb_optimizer* opt) {
+  int rc = gb::validate_ffnet(net);
+  if (rc != GB_OK) return rc;
+  rc = gb::validate_optimizer(opt);
+  if (rc != GB_OK) return rc;
+  GB_REQUIRE(params && adam_m && adam_v && jobs && x && y && hp && out_loss, GB_E_ARG,
+             "params/adam_m/adam_v/jobs/x/y/hp/out_loss must be non-NULL");
+  GB_REQUIRE(hp->epochs >= 1, GB_E_ARG, "epochs=%d must be >= 1", hp->epochs);
+  GB_REQUIRE(hp->batch_size >= 1, GB_E_ARG, "batch_size=%d must be >= 1", hp->batch_size);
+  GB_REQUIRE(hp->shuffle >= 0 && hp->shuffle <= 2, GB_E_ARG, "shuffle=%d unknown", hp->shuffle);
+  GB_REQUIRE(hp->shuffle != 2 || perm, GB_E_ARG, "shuffle=2 needs perm");
+  GB_REQUIRE(hp->loss >= GB_LOSS_MSE && hp->loss <= GB_LOSS_LOG_COSH, GB_E_ARG, "loss=%d unknown (gb_loss: 0..5)", hp->loss);
+  GB_REQUIRE(gb::aligned16(params) && gb::aligned16(adam_m) && gb::aligned16(adam_v) && gb::aligned16(x) &&
+                 gb::aligned16(y),
+             GB_E_ALIGN, "params/adam/x/y must be 16-byte aligned");
+  return GB_OK;
+}
+
+int check_split_stop(const gb_fit_split* split, int32_t val_batch, const float* out_val_loss, const gb_fit_stop* stop,
+                     const int32_t* out_epochs, const int32_t* out_best_epoch) {
+  GB_REQUIRE(!split || out_val_loss, GB_E_ARG, "split needs out_val_loss");
+  GB_REQUIRE(!split || val_batch >= 1, GB_E_ARG, "val_batch=%d must be >= 1", val_batch);
+  GB_REQUIRE(!stop || (out_epochs && out_best_epoch), GB_E_ARG, "stop needs best_params, out_epochs and out_best_epoch");
+  return GB_OK;
+}
+
+int check_best_params(const gb_fit_stop* stop, const float* best_params) {
+  GB_REQUIRE(!stop || best_params, GB_E_ARG, "stop needs best_params, out_epochs and out_best_epoch");
+  GB_REQUIRE(!stop || gb::aligned16(best_params), GB_E_ARG, "best_params must be 16-byte aligned");
+  return GB_OK;
+}
+
+int check_reg_drop(const gb_ffnet* net, const gb_dense_reg* reg, const gb_dense_dropout* drop, bool& any_reg, bool& any_drop) {
+  any_reg = false;  // a record of zeros is no record: the kernels of gb_ffae_fit_opt
+  if (reg != nullptr) {
+    const int rc = gb::validate_ffnet(net);
+    if (rc != GB_OK) return rc;
+    auto ok = [](float v) { return v >= 0.f && v < 3.0e38f; };  // false for NaN and inf
+    const struct { const char* name; const float* c; } fields[] = {
+        {"kernel_l1", reg->kernel_l1}, {"kernel_l2", reg->kernel_l2}, {"bias_l1", reg->bias_l1}, {"bias_l2", reg->bias_l2}};
+    for (const auto& f : fields)
+      for (int l = 0; l < net->n_layers; ++l) {
+        GB_REQUIRE(ok(f.c[l]), GB_E_ARG, "reg %s[%d]=%g must be finite and >= 0", f.name, l, (double)f.c[l]);
+        any_reg = any_reg || f.c[l] != 0.f;
+      }
+  }
+  any_drop = false;  // likewise: all-zero rates run the kernels of gb_ffae_fit_reg
+  if (drop != nullptr) {
+    const int rc = gb::validate_ffnet(net);
+    if (rc != GB_OK) return rc;
+    for (int l = 0; l < GB_MAX_LAYERS; ++l) {
+      const float r = drop->rate[l];
+      GB_REQUIRE(r >= 0.f && r < 1.f, GB_E_ARG, "dropout rate[%d]=%g must be finite, >= 0 and < 1", l, (double)r);  // false for NaN
+      GB_REQUIRE(r == 0.f || l < net->n_layers, GB_E_ARG, "dropout rate[%d]=%g: the net has %d layers (rate[l] is on the input of layer l)",
+                 l, (double)r, net->n_layers);
+      GB_REQUIRE(r == 0.f || l == 0 || net->l1[l - 1] == 0.f, GB_E_ARG,
+                 "dropout rate[%d]=%g on the output of layer %d, which has an activity L1: not supported", l, (double)r, l - 1);
+      any_drop = any_drop || r != 0.f;
+    }
+  }
+  return GB_OK;
+}
+
+FitFamily fit_family(const gb_fit_hparams* hp, const gb_optimizer* opt, const gb_dense_reg* reg, const gb_dense_dropout* drop) {
+  if (drop != nullptr) return FAMILY_DROP;
+  if (reg != nullptr) return FAMILY_REG;
+  if (!gb::plain_adam(opt)) return FAMILY_OPT;
+  return hp->loss == GB_LOSS_MSE ? FAMILY_MSE : FAMILY_LOSS;
+}
+
+int setup_fit(const gb_ffnet* net, float* params, float* adam_m, float* adam_v, const gb_job* jobs, const gb_fit_split* split,
+              int32_t max_rows, const float* x, const float* y, const int32_t* row_map, const int32_t* perm, const gb_fit_hparams* hp,
+              int32_t val_batch, float* out_loss, float* out_acc, float* out_val_loss, float* out_val_acc, const gb_fit_stop* stop,
+              float* best_params, int32_t* out_epochs, int32_t* out_best_epoch, const gb_optimizer* opt, const gb_dense_reg* reg,
+              const gb_dense_dropout* drop, FitArgs& a, bool& w_global, size_t& smem) {
+  a = FitArgs{};
+  smem = 0;
+  w_global = false;
+  int rc = plan_fit(net, a, w_global, smem);
+  if (rc != GB_OK) return rc;
+  a.hp = *hp;
+  const bool use_opt = !gb::plain_adam(opt);
+  if (opt != nullptr && !use_opt) {  // plain Adam runs the Adam kernels, from the optimizer's hyperparameters
+    a.hp.lr = opt->lr; a.hp.beta1 = opt->beta1; a.hp.beta2 = opt->beta2; a.hp.eps = opt->eps;
+  }
+  if (use_opt) a.opt = *opt;
+  if (reg != nullptr || drop != nullptr) {  // the REG and DROP kernels are OPT kernels: plain Adam, too, runs through gb::opt_update there
+    if (reg != nullptr) a.reg = *reg;  // else zeros: the DROP kernels add a penalty of 0
+    if (opt != nullptr) {
+      a.opt = *opt;
+    } else {
+      a.opt = gb_optimizer{};
+      a.opt.kind = GB_OPT_ADAM; a.opt.lr = hp->lr; a.opt.beta1 = hp->beta1; a.opt.beta2 = hp->beta2; a.opt.eps = hp->eps;
+    }
+  }
+  if (drop != nullptr) {
+    for (int l = 0; l < GB_MAX_LAYERS; ++l) {
+      if (drop->rate[l] == 0.f) continue;
+      const double r = (double)drop->rate[l];
+      a.drop_layers |= 1u << l;
+      a.drop_thr[l] = (uint32_t)floor(r * 4294967296.0);
+      a.drop_scale[l] = (float)(1.0 / (1.0 - r));
+    }
+  }
+  const int L = net->n_layers;
+  a.max_rows = max_rows;
+  a.pstride = (long)gb_ffnet_param_stride(net);
+  a.sstride = (long)gb_ffae_fit_state_stride(net);
+  a.gather_layer = 0;
+  for (int l = 1; l < L; ++l)
+    if (a.im.np[l] <= a.im.np[a.gather_layer]) a.gather_layer = l;  // the last of the narrowest layers
+  a.gather_layer2 = a.gather_layer;
+  for (int l = 0, best = 1 << 30; l < L; ++l)
+    if (l != a.gather_layer && a.im.np[l] < best) { best = a.im.np[l]; a.gather_layer2 = l; }  // the narrowest of the others
+  a.params = params; a.adam_m = adam_m; a.adam_v = adam_v; a.jobs = jobs; a.x = x; a.y = y; a.perm = perm;
+  a.out_loss = out_loss; a.out_acc = out_acc;
+  a.split = split; a.row_map = row_map; a.val_batch = val_batch; a.out_val_loss = out_val_loss; a.out_val_acc = out_val_acc;
+  a.stop = stop; a.best_params = best_params; a.out_epochs = out_epochs; a.out_best_epoch = out_best_epoch;
+  return GB_OK;
+}
+
+}  // namespace gb_fit

@@ -1,7 +1,8 @@
 // The Dense fit kernels' shared definitions: the launch record FitArgs, the device helpers and the three kernel templates
 // (ffae_fit_kernel, ffae_fit_reg_kernel, ffae_fit_drop_kernel) whose body is ffae_fit_body.cuh.  Included by ffae_fit.cu, which
 // instantiates and launches the first two, and by ffae_fit_drop.cu, which holds the nine instantiations of the third in an object of
-// their own (gb_fit::launch_drop), so that ffae_fit.o keeps exactly the kernels it had.
+// their own (gb_fit::launch_drop), so that ffae_fit.o keeps exactly the kernels it had; ffae_fit_group.cu holds the grouped kernels
+// of gb_ffae_fit_group, which take the same body and fill one record per group with ffae_fit.cu's setup_fit.
 #pragma once
 #include <cuda_pipeline.h>
 #include <math_constants.h>
@@ -57,8 +58,28 @@ struct FitArgs {
 
 enum FitEntry { FIT_PLAIN, FIT_SPLIT, FIT_STOP };
 
+// the kernel family a fit runs: plain MSE with Adam, another loss, another optimizer than plain Adam, weight regularizers, dropout
+enum FitFamily { FAMILY_MSE, FAMILY_LOSS, FAMILY_OPT, FAMILY_REG, FAMILY_DROP };
+
 // ffae_fit_drop.cu: one launch of the ffae_fit_drop_kernel instantiation of (entry, memory plan), the plan as plan_fit chose it
 int launch_drop(const FitArgs& a, FitEntry entry, bool w_global, size_t smem, int n_jobs, cudaStream_t stream);
+
+// ffae_fit.cu, the host side of one net's fit, shared with gb_ffae_fit_group (ffae_fit_group.cu).  check_fit: the net, optimizer,
+// pointer, hparams and alignment checks of launch_fit; check_split_stop / check_best_params: those of the split and stop entries;
+// check_reg_drop: gb_ffae_fit_drop's checks of reg and drop against the net, and whether either record is more than zeros;
+// fit_family: the family of the records that remain (NULL where they are zeros); setup_fit: the memory plan and the launch record.
+int check_fit(const gb_ffnet* net, float* params, float* adam_m, float* adam_v, const gb_job* jobs, const float* x, const float* y,
+              const int32_t* perm, const gb_fit_hparams* hp, float* out_loss, const gb_optimizer* opt);
+int check_split_stop(const gb_fit_split* split, int32_t val_batch, const float* out_val_loss, const gb_fit_stop* stop,
+                     const int32_t* out_epochs, const int32_t* out_best_epoch);
+int check_best_params(const gb_fit_stop* stop, const float* best_params);
+int check_reg_drop(const gb_ffnet* net, const gb_dense_reg* reg, const gb_dense_dropout* drop, bool& any_reg, bool& any_drop);
+FitFamily fit_family(const gb_fit_hparams* hp, const gb_optimizer* opt, const gb_dense_reg* reg, const gb_dense_dropout* drop);
+int setup_fit(const gb_ffnet* net, float* params, float* adam_m, float* adam_v, const gb_job* jobs, const gb_fit_split* split,
+              int32_t max_rows, const float* x, const float* y, const int32_t* row_map, const int32_t* perm, const gb_fit_hparams* hp,
+              int32_t val_batch, float* out_loss, float* out_acc, float* out_val_loss, float* out_val_acc, const gb_fit_stop* stop,
+              float* best_params, int32_t* out_epochs, int32_t* out_best_epoch, const gb_optimizer* opt, const gb_dense_reg* reg,
+              const gb_dense_dropout* drop, FitArgs& a, bool& w_global, size_t& smem);
 
 }  // namespace gb_fit
 

@@ -286,6 +286,116 @@ class FFEngine:
         return thresholds_pair(jobs_dev, n_jobs, max_rows, tag_unscaled, total_scaled, self.n_out, n_slots, w0, w1, self.device)
 
 
+def fit_plan(dims: Sequence[int], acts: Sequence[str], l1: Optional[Sequence[float]] = None) -> Optional[Tuple[int, int]]:
+    """The memory plan of the Dense fit for this architecture (gb_ffae_fit_plan; no device needed): (weights in L2, dz buffers in
+    L2), or None when the fit refuses the architecture.  Nets of one ``fit_group`` launch share it."""
+    lib = _cabi.load_library()
+    try:
+        net = _cabi.make_ffnet([int(d) for d in dims], list(acts), l1)
+    except ValueError:
+        return None
+    w, d = C.c_int32(0), C.c_int32(0)
+    return (w.value, d.value) if lib.gb_ffae_fit_plan(C.byref(net), C.byref(w), C.byref(d)) == 0 else None
+
+
+class FitGroup:
+    """One architecture's part of a ``fit_group`` launch, in the form ``FFEngine.fit_split`` takes it: the engine, the slots' params
+    (trained in place), the device jobs, their count and longest row range, x and y, and optionally the ``make_split`` records with
+    their row map, a pinned visiting order ``perm`` [n_jobs, epochs, max_rows], the optimizer state (m, v) and ``make_stop`` records."""
+
+    def __init__(self, eng: FFEngine, params, jobs_dev, n_jobs: int, max_rows: int, x, y, split=None, row_map=None, perm=None, state=None,
+                 stop=None):
+        self.eng, self.params, self.jobs_dev, self.n_jobs, self.max_rows = eng, params, jobs_dev, int(n_jobs), int(max_rows)
+        self.x, self.y, self.split, self.row_map, self.perm, self.state, self.stop = x, y, split, row_map, perm, state, stop
+
+
+def _host_records(rec, dtype, n: int) -> np.ndarray:
+    """``n`` split or stop records as a host array, from a host array or device bytes."""
+    if isinstance(rec, np.ndarray):
+        return np.ascontiguousarray(rec[:n])
+    return rec.cpu().numpy().view(dtype)[:n].copy()
+
+
+def fit_group(groups: Sequence[FitGroup], val_batch: Optional[int] = None, epochs: int = 1, batch_size: int = 32, shuffle=True,
+              adam: Optional[Dict[str, float]] = None, seed: int = 0, l1_div_batch: bool = False, step0: int = 0, loss: str = "mse",
+              optimizer=None, reg=None, dropout=None):
+    """
+    ``FFEngine.fit_split`` of several architectures in one launch (gb_ffae_fit_group): every group's jobs train its own slots on
+    its own rows, and each group gets back exactly what ``fit_split`` with the same arguments returns for it alone -- (loss,
+    accuracy, val_loss, val_accuracy, (m, v)), with ``epochs_run, best_epoch`` before (m, v) when the groups carry stop records --
+    bit for bit.  The keyword arguments are ``fit_split``'s and apply to every group.  The groups must share a memory plan
+    (``fit_plan``) and an entry point: split records for all or none, stop records for all or none, perm for all or none.
+    Row maps are laid end to end and each group's ``map_ofs`` moved with its map.
+    """
+    torch = _torch()
+    groups = list(groups)
+    if not groups:
+        return []
+    for what in ("split", "stop", "perm"):
+        if len({getattr(g, what) is None for g in groups}) > 1:
+            raise ValueError(f"fit_group: {what} for some groups but not all; the groups of one launch share an entry point")
+    dev = groups[0].eng.device
+    counts = [g.n_jobs for g in groups]
+    n, max_rows = sum(counts), max(g.max_rows for g in groups)
+    jobs_dev = torch.cat([g.jobs_dev[: c * _cabi.JOB_DTYPE.itemsize] for g, c in zip(groups, counts)])
+    job_group = np.repeat(np.arange(len(groups), dtype=np.int32), counts)
+    split = row_map = stop = perm = None
+    if groups[0].split is not None:
+        parts, maps, ofs = [], [], 0
+        for g, c in zip(groups, counts):
+            s = _host_records(g.split, _cabi.SPLIT_DTYPE, c)
+            if g.row_map is None:
+                s["map_ofs"] = -1  # without a map the kernel never reads it
+            else:
+                s["map_ofs"] = np.where(s["map_ofs"] >= 0, s["map_ofs"] + ofs, -1)
+                maps.append(g.row_map.reshape(-1))
+                ofs += int(g.row_map.numel())
+            parts.append(s)
+        split = jobs_to_device(np.concatenate(parts), dev)
+        row_map = torch.cat(maps) if maps else None
+    if groups[0].stop is not None:
+        stop = jobs_to_device(np.concatenate([_host_records(g.stop, _cabi.STOP_DTYPE, c) for g, c in zip(groups, counts)]), dev)
+    if groups[0].perm is not None:
+        perm = torch.zeros((n, int(epochs), max_rows), dtype=torch.int32, device=dev)
+        for g, j0, c in zip(groups, np.cumsum([0] + counts[:-1]), counts):
+            perm[j0:j0 + c, :, :g.max_rows] = g.perm[:c]
+    hp = _fit_hparams(epochs, batch_size, shuffle, perm, adam, seed, l1_div_batch, step0, loss)
+    states = [g.eng._fit_state(g.params, g.state) for g in groups]
+    shape = (n, hp.epochs)
+    make = torch.empty if stop is None else (lambda shape, **kw: torch.full(shape, float("nan"), **kw))  # noqa: E731
+    out = [make(shape, dtype=torch.float32, device=dev) for _ in range(2)]
+    out += [torch.full(shape, float("nan"), dtype=torch.float32, device=dev) for _ in range(2)]
+    bests = [None] * len(groups)
+    epochs_run = best_epoch = None
+    if stop is not None:
+        bests = [torch.empty_like(g.params) for g in groups]
+        epochs_run = torch.zeros((n,), dtype=torch.int32, device=dev)
+        best_epoch = torch.full((n,), -1, dtype=torch.int32, device=dev)
+    p = _cabi.ptr
+    recs = (_cabi.GbFitGroup * len(groups))()
+    for r, g, (m, v), best in zip(recs, groups, states, bests):
+        r.net = g.eng.net
+        r.params, r.adam_m, r.adam_v, r.best_params, r.x, r.y = (p(t) for t in (g.params, m, v, best, g.x, g.y))
+    opt = None if optimizer is None else _cabi.make_optimizer(*optimizer)
+    has_reg = reg is not None and any(v for vals in reg.values() for v in vals)
+    rec = _cabi.make_dense_reg(**reg) if has_reg else None
+    drop = _cabi.make_dense_dropout(dropout) if dropout is not None and any(dropout) else None
+    jg = np.ascontiguousarray(job_group)
+    lib = groups[0].eng.lib
+    ws = torch.empty((int(lib.gb_ffae_fit_group_workspace_bytes(len(groups), n)),), dtype=torch.uint8, device=dev)  # records + job_group
+    _cabi.check(lib.gb_ffae_fit_group(
+        recs, len(groups), jg.ctypes.data_as(C.POINTER(C.c_int32)), p(jobs_dev), p(split), n, max_rows, p(row_map), p(perm), C.byref(hp),
+        int(val_batch if val_batch is not None else batch_size), *(p(t) for t in out), p(stop), p(epochs_run), p(best_epoch),
+        None if opt is None else C.byref(opt), None if rec is None else C.byref(rec), None if drop is None else C.byref(drop), p(ws),
+        _stream_ptr()))
+    res, j0 = [], 0
+    for g, c, mv in zip(groups, counts, states):
+        part = tuple(t[j0:j0 + c] for t in out)
+        res.append((*part, mv) if stop is None else (*part, epochs_run[j0:j0 + c], best_epoch[j0:j0 + c], mv))
+        j0 += c
+    return res
+
+
 def _fit_hparams(epochs, batch_size, shuffle, perm, adam, seed, l1_div_batch, step0, loss="mse") -> "_cabi.GbFitHParams":
     adam = adam or {}
     hp = _cabi.GbFitHParams()

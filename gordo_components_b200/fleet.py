@@ -10,6 +10,7 @@ summaries -- there is no exchange step inside fit, predict or anomaly.
 """
 from __future__ import annotations
 
+import functools
 import math
 import time
 from typing import Dict, List, Optional, Sequence
@@ -378,6 +379,79 @@ def _fit_slots(eng, params, fit_jobs, n_jobs, max_rows, x, y, split, row_map, n_
     return hist, acc, val_loss, val_acc, epochs_run, best_epoch
 
 
+class _FitRequest:
+    """The arguments of a bucket's one fit launch (``_fit_slots``), as a build hands them to ``build_joined``."""
+
+    def __init__(self, eng, params, fit_jobs, n_jobs, max_rows, x, y, split, row_map, n_machines, epochs, batch_size, shuffle, adam, seed,
+                 validation_batch_size, early_stopping, loss="mse", optimizer=None, reg=None, dropout=None):
+        self.eng, self.params, self.fit_jobs, self.n_jobs, self.max_rows = eng, params, fit_jobs, n_jobs, max_rows
+        self.x, self.y, self.split, self.row_map, self.n_machines, self.early_stopping = x, y, split, row_map, n_machines, early_stopping
+        self.fit_kw = dict(val_batch=validation_batch_size or batch_size, epochs=epochs, batch_size=batch_size, shuffle=shuffle, adam=adam,
+                           seed=seed, loss=loss, optimizer=optimizer, reg=reg, dropout=dropout)
+        self.args = (eng, params, fit_jobs, n_jobs, max_rows, x, y, split, row_map, n_machines, epochs, batch_size, shuffle, adam, seed,
+                     validation_batch_size, early_stopping, loss, optimizer, reg, dropout)
+
+    def launch_key(self):
+        """What fits of one launch share: the memory plan, every fit argument but the network, and the entry point."""
+        return (engine.fit_plan(self.eng.dims, self.eng.acts, self.eng.l1), repr(sorted(self.fit_kw.items())), self.split is None,
+                self.early_stopping is None)
+
+
+def _fit_requests_together(reqs: Sequence[_FitRequest]):
+    """The fit launches of ``reqs`` that share a launch key, as one gb_ffae_fit_group launch: ``_fit_slots``'s result for each."""
+    groups = [engine.FitGroup(r.eng, r.params, r.fit_jobs, r.n_jobs, r.max_rows, r.x, r.y, split=r.split, row_map=r.row_map,
+                              stop=_slot_stops(r.early_stopping, r.n_machines, r.n_jobs)) for r in reqs]
+    out = []
+    for res in engine.fit_group(groups, **reqs[0].fit_kw):
+        hist, acc, val_loss, val_acc, *ran, _ = res
+        epochs_run, best_epoch = ran or (None, None)
+        out.append((hist, acc, val_loss, val_acc, epochs_run, best_epoch))
+    return out
+
+
+def build_joined(builds: Sequence) -> list:
+    """
+    Several batched builds (``build_fleet.steps(...)`` / ``build_kfold_fleet.steps(...)`` generators) with their fits joined: every
+    build runs up to its fit, the fits that share a memory plan and every fit argument but the network go out as one
+    gb_ffae_fit_group launch (a fit alone keeps its own launch), and every build finishes with its own fit's result.  Each build's
+    result is exactly what it gives on its own.  Returns the builds' results in order.
+    """
+    builds = list(builds)
+    reqs = [next(b) for b in builds]
+    results = [None] * len(reqs)
+    launches: Dict[tuple, List[int]] = {}
+    for i, r in enumerate(reqs):
+        launches.setdefault(r.launch_key(), []).append(i)
+    for key, idx in launches.items():
+        if len(idx) == 1 or key[0] is None:
+            for i in idx:
+                results[i] = _fit_slots(*reqs[i].args)
+        else:
+            for i, res in zip(idx, _fit_requests_together([reqs[i] for i in idx])):
+                results[i] = res
+    out = []
+    for b, res in zip(builds, results):
+        try:
+            b.send(res)
+        except StopIteration as done:
+            out.append(done.value)
+        else:
+            raise RuntimeError("a batched build asked for a second fit")
+    return out
+
+
+def _fit_joined(steps):
+    """A batched build from its generator of steps (which yields its one ``_FitRequest`` and receives ``_fit_slots``'s result):
+    the build on its own, its fit one launch; ``.steps`` keeps the generator for ``build_joined``."""
+
+    @functools.wraps(steps)
+    def build(*args, **kwargs):
+        return build_joined([steps(*args, **kwargs)])[0]
+
+    build.steps = steps
+    return build
+
+
 def _slot_stops(early_stopping, n_machines: int, n_slots: int):
     """The stop records of ``n_slots`` fits, slot s applying machine s mod M's EarlyStopping callback (``early_stopping``: one for
     every machine or one per machine), or None without a callback."""
@@ -451,6 +525,7 @@ def shuffle_maps(slot_rows):
     return maps, np.asarray([first[int(v)] for v in slot_rows], dtype=np.int64)
 
 
+@_fit_joined
 def build_fleet(eng: "engine.FFEngine", x, y, rows, epochs: int = 1, batch_size: int = 32, n_splits: int = 3, seed: int = 0,
                 adam: Optional[Dict[str, float]] = None, shuffle: bool = True, generator=None, input_scaler: bool = False,
                 detector_shuffle: bool = False, validation_split: float = 0.0, validation_batch_size: Optional[int] = None,
@@ -554,7 +629,7 @@ def build_fleet(eng: "engine.FFEngine", x, y, rows, epochs: int = 1, batch_size:
         y = y[:total].repeat(K + 1, 1)
         fit_x = copy0
     fit_jobs = engine.jobs_to_device(engine.make_jobs(np.arange(S), n_train, fit_x), dev)
-    hist, acc, val_loss, val_acc, epochs_run, best_epoch = _fit_slots(
+    hist, acc, val_loss, val_acc, epochs_run, best_epoch = yield _FitRequest(
         eng, params, fit_jobs, S, N, x, y, split, row_map, M, epochs, batch_size, shuffle, adam, seed, validation_batch_size, early_stopping,
         loss, optimizer, reg, dropout)
     if not held_out:
@@ -1068,6 +1143,7 @@ def combine_fold_extrema(lo, hi):
     return s_lo, s_hi
 
 
+@_fit_joined
 def build_kfold_fleet(eng: "engine.FFEngine", x, y, rows, cv, epochs: int = 1, batch_size: int = 32, seed: int = 0,
                       adam: Optional[Dict[str, float]] = None, shuffle: bool = True, generator=None, input_scaler: bool = False,
                       target_scaler: bool = False, detector_shuffle: bool = False, validation_split: float = 0.0,
@@ -1170,7 +1246,7 @@ def build_kfold_fleet(eng: "engine.FFEngine", x, y, rows, cv, epochs: int = 1, b
     params = _keras_initial_params(eng, S, g)
     init_params = params.clone() if keep_init_params else None
     fit_jobs = jobs(np.arange(S), n_train, slot_x)
-    hist, acc, val_loss, val_acc, epochs_run, best_epoch = _fit_slots(
+    hist, acc, val_loss, val_acc, epochs_run, best_epoch = yield _FitRequest(
         eng, params, fit_jobs, S, N, xf, yf, split, row_map, M, epochs, batch_size, shuffle, adam, seed, validation_batch_size, early_stopping,
         loss, optimizer, reg, dropout)
     if (n_train == slot_n).all():  # nothing held out

@@ -478,6 +478,37 @@ int gb_ffae_fit_drop(const gb_ffnet* net, float* params, float* adam_m, float* a
  * (gb_ffae_fit refuses the architecture with the same status); either output may be NULL. */
 int gb_ffae_fit_plan(const gb_ffnet* net, int32_t* weights_in_l2, int32_t* dz_in_l2);
 
+/* One architecture of a grouped Dense fit (gb_ffae_fit_group): its net, the state of its slots and its rows.  params, adam_m, adam_v:
+ * [this group's slots][param / state stride of net], 16-byte aligned; best_params likewise, needed (and read) only with a stop array.
+ * x, y: [rows][net.dims[0]], [rows][net.dims[L]], 16-byte aligned. */
+typedef struct gb_fit_group {
+  gb_ffnet net;
+  float *params, *adam_m, *adam_v, *best_params;
+  const float *x, *y;
+} gb_fit_group;
+
+/* gb_ffae_fit_drop over jobs of several architectures in one launch.  Job j belongs to group job_group[j] (a HOST array [n_jobs],
+ * copied to the device with the group records), and its gb_job.slot, x_row and row ranges are that group's.  Every other argument
+ * is gb_ffae_fit_drop's and applies to every job: the jobs, split and stop records, the perm and history rows and out_epochs /
+ * out_best_epoch are indexed by the launch's job index, row_map is shared through map_ofs, and hp, opt, reg and drop are every
+ * group's.  Each job's results are bit-identical to those of gb_ffae_fit_drop with groups[g].net and its group's pointers over
+ * that group's jobs alone: the shuffle permutation and the dropout masks are keyed by (hp->seed, slot), the group-local slot.
+ * Refused before any launch (GB_E_ARG unless noted; the message names the group): n_groups < 1; a NULL groups or job_group; a
+ * job_group entry outside [0, n_groups); any argument gb_ffae_fit_drop refuses for one group's net and pointers (reg and drop are
+ * checked against each group's net); groups whose memory plans (gb_ffae_fit_plan) differ, or whose nets take another kernel
+ * family from reg or drop (all-zero coefficients or rates on one net's layers but not another's); a group gb_ffae_fit_drop would
+ * refuse (GB_E_SMEM, GB_E_SHAPE, GB_E_ALIGN); a NULL or misaligned workspace.  The dynamic shared memory is the largest of the
+ * groups'.  workspace: gb_ffae_fit_group_workspace_bytes(n_groups, n_jobs) bytes of device memory, 16-byte aligned, that the call
+ * fills with the group records and job_group (a copy enqueued on `stream`) and the launch reads: it must stay allocated until the
+ * launch has run, as any device array of the call. */
+size_t gb_ffae_fit_group_workspace_bytes(int32_t n_groups, int32_t n_jobs);
+int gb_ffae_fit_group(const gb_fit_group* groups, int32_t n_groups, const int32_t* job_group, const gb_job* jobs,
+                      const gb_fit_split* split, int32_t n_jobs, int32_t max_rows, const int32_t* row_map, const int32_t* perm,
+                      const gb_fit_hparams* hp, int32_t val_batch, float* out_loss, float* out_acc, float* out_val_loss,
+                      float* out_val_acc, const gb_fit_stop* stop, int32_t* out_epochs, int32_t* out_best_epoch,
+                      const gb_optimizer* opt, const gb_dense_reg* reg, const gb_dense_dropout* drop, void* workspace,
+                      void* stream);
+
 /* ---- K3: LSTM autoencoder predict --------------------------------------------------------
  * lstm_model / lstm_symmetric / lstm_hourglass (factories/lstm_autoencoder.py:72-103):
  * LSTM layers (gate order i,f,c,o; sigmoid recurrent activation; zero initial state per
